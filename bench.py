@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — (region,token) pairs/s, forward+backward, of the ViLBERT two-stream hot path on B200.
+"""bench.py — (region,token) pairs/s, forward+backward, of the ViLBERT two-stream hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W [--config 2|3|4|5]   # this repo's CUDA engine
     python bench.py --impl reference --steps K --warmup W               # CPU arm (reference algorithm on the host cores)
@@ -20,6 +20,11 @@ and reported separately as `optimizer` / `train_step`.
 
 `value` is measured with inputs resident in HBM (CUDA-graph replay); `e2e` runs the same step from pinned HOST buffers
 through the engine API (H2D of the batch and D2H of the loss inside the timed region). Prints ONE JSON line.
+
+--dump-outputs DIR writes what the last timed step computed (losses, head / encoder outputs, that step's parameter
+gradients) as DIR/<name>.npy in float32, arrays larger than their share of a 60 MB budget as a fixed, seeded sample of their
+elements, so that two builds run with the same arguments can be compared output for output. For that, the gradient buffer is
+zeroed and the dropout step counter reset before the last timed step (one extra memset inside the timed region).
 """
 import argparse
 import json
@@ -71,16 +76,14 @@ def algorithmic_flops_fwd(c, Nv, Nt):
     return Lt * f_text + Lv * f_vis + Lc * f_conn + f_emb + f_pool + f_heads
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1425.6), d.get("bf16_tflops", 1650.9), d.get("hbm_gbs", 6575.1), "measured (MEASURED_PEAKS.json)"
-    return 1400.0, 1590.0, 6650.0, "fallback (B200_PROFILING.md)"
+def datasheet_peaks():
+    """Dense BF16 / FP16 tensor rate (TFLOP/s) and HBM3 bandwidth (GB/s) of the H100 SXM data sheet, for a card allowed 700 W.
+    Upper bounds, not reached rates: a card with a lower power limit (see `clocks.power_limit_w`) clocks lower."""
+    return 989.0, 3350.0, "H100 SXM data sheet (dense, 700 W)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe). The sampler
+    """nvidia-smi clocks / throttle reasons sampled during the timed region, with the card's name and power limit. The sampler
     is started before the warm-up (nvidia-smi needs a moment to come up); only samples whose timestamp falls inside the
     marked window are used (all samples if none does)."""
 
@@ -90,7 +93,7 @@ class ClockSampler:
 
     def start(self):
         q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-lms", "50", "-i", str(self.index)],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -111,7 +114,7 @@ class ClockSampler:
 
     def stop(self):
         if self.proc is None:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"gpu": None, "power_limit_w": None, "sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.12)
         self.proc.terminate()
         self.t.join(timeout=2)
@@ -125,7 +128,9 @@ class ClockSampler:
         reasons = [n for i, n in enumerate(names) if any(len(r) > 4 + i and r[4 + i].lower().startswith("active") for r in rows)]
         mx = [int(float(r[2])) for r in rows if len(r) > 2 and num(r[2])]
         pw = [float(r[3]) for r in rows if len(r) > 3 and num(r[3])]
-        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx[0] if mx else None, "reasons": reasons,
+        lim = [float(r[8]) for r in rows if len(r) > 8 and num(r[8])]
+        return {"gpu": rows[0][9] if rows and len(rows[0]) > 9 else None, "power_limit_w": lim[0] if lim else None,
+                "sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx[0] if mx else None, "reasons": reasons,
                 "samples": len(sm), "power_w_max": max(pw) if pw else None, "window": window}
 
 
@@ -133,10 +138,9 @@ class ClockSampler:
 def run_cpu_reference(cfgj, B, Nv, Nt, steps, warmup, budget_s=90.0, threads=None):
     """The reference algorithm's VILBertForVLTasks fwd + VQA loss + bwd, fp32, on the host cores, at a FIXED sample batch B:
     `warmup` untimed steps (>= 1, so that allocator / thread-pool start-up never lands in a timed step), then up to `steps` timed
-    steps (>= 3 unless the time budget runs out first). Uses the unmodified reference when $VILBERT_REFERENCE_ROOT (default
-    /root/reference) holds it (kind "reference"), else the oracle port, which is bit-identical to it on CPU (kind "port")."""
+    steps (>= 3 unless the time budget runs out first). Runs the oracle port (kind "port"), which tests/golden pins to the
+    reference's outputs and gradients on CPU."""
     import torch
-    from oracle import ref_loader
     from oracle import vilbert_oracle as O
     if threads is None:
         try:
@@ -150,34 +154,16 @@ def run_cpu_reference(cfgj, B, Nv, Nt, steps, warmup, budget_s=90.0, threads=Non
     inp = O.synth_inputs(cfg, B, Nv, Nt, seed=1234)
     tgt = O.synth_vqa_target(B, 3129)
     kind = "port"
-    model = None
-    if ref_loader.available() and os.environ.get("VB_CPU_ARM", "") != "port":
-        try:
-            ref = ref_loader.load()
-            model = ref.VILBertForVLTasks(ref.BertConfig.from_dict(cfgj), num_labels=1, default_gpu=False)
-            model.load_state_dict(P, strict=False)
-            model.train()
-            kind = "reference"
-        except Exception as e:   # noqa: BLE001
-            print(f"[bench] reference import failed ({e}); timing the oracle port", file=sys.stderr)
-            model = None
-    if model is None:
-        Pg = {k: v.clone().requires_grad_(True) for k, v in P.items() if k != "cls.predictions.decoder.weight"}
-        Pg["cls.predictions.decoder.weight"] = Pg["bert.embeddings.word_embeddings.weight"]
+    Pg = {k: v.clone().requires_grad_(True) for k, v in P.items() if k != "cls.predictions.decoder.weight"}
+    Pg["cls.predictions.decoder.weight"] = Pg["bert.embeddings.word_embeddings.weight"]
 
     def one_step():
         t0 = time.perf_counter()
-        if model is not None:
-            model.zero_grad()
-            out = model(inp["input_txt"], inp["input_imgs"], inp["image_loc"], inp["token_type_ids"], inp["attention_mask"], inp["image_attention_mask"],
-                        inp["co_attention_mask"], inp["task_ids"])
-            O.vqa_loss(out[0], tgt).backward()
-        else:
-            for v in Pg.values():
-                v.grad = None
-            _, heads = O.vilbert_for_vl_tasks(Pg, cfg, inp["input_txt"], inp["input_imgs"], inp["image_loc"], inp["token_type_ids"], inp["attention_mask"],
-                                              inp["image_attention_mask"], inp["co_attention_mask"], inp["task_ids"])
-            O.vqa_loss(heads[0], tgt).backward()
+        for v in Pg.values():
+            v.grad = None
+        _, heads = O.vilbert_for_vl_tasks(Pg, cfg, inp["input_txt"], inp["input_imgs"], inp["image_loc"], inp["token_type_ids"], inp["attention_mask"],
+                                          inp["image_attention_mask"], inp["co_attention_mask"], inp["task_ids"])
+        O.vqa_loss(heads[0], tgt).backward()
         return time.perf_counter() - t0
 
     t_start = time.perf_counter()
@@ -190,7 +176,7 @@ def run_cpu_reference(cfgj, B, Nv, Nt, steps, warmup, budget_s=90.0, threads=Non
             break
     sec = sum(times) / len(times)
     return dict(value=B * Nv * Nt / sec, unit="pairs/s", cores=threads, kind=kind, sec_per_step=sec, sample_batch=B, steps_timed=len(times),
-                sample=f"{'the unmodified reference' if kind == 'reference' else 'oracle port (bit-exact vs the reference on CPU)'}: VILBertForVLTasks fwd + VQA loss + "
+                sample="oracle port (pinned to the reference's outputs and gradients on CPU): VILBertForVLTasks fwd + VQA loss + "
                        f"bwd, fp32, fixed B={B} x {Nv} regions x {Nt} tokens, {max(warmup, 1)} warm-up + {len(times)} timed step(s), {threads} threads")
 
 
@@ -238,17 +224,17 @@ def main():
     ap.add_argument("--no-overlap", action="store_true", help="N > 1: all-reduce after the whole backward instead of overlapping it")
     ap.add_argument("--ddp-mode", default="pieces", choices=["graph", "pieces"],
                     help="N > 1 overlapped step: 'pieces' (default) = one graph per backward piece, collectives issued from the host between "
-                         "them; 'graph' = ONE CUDA graph per step with the NCCL all-reduces captured on a side stream (measured 0.6 %% faster at "
-                         "N = 2, but ProcessGroupNCCL's watchdog hangs at teardown while captured collectives are alive: opt-in)")
+                         "them; 'graph' = ONE CUDA graph per step with the NCCL all-reduces captured on a side stream (ProcessGroupNCCL's "
+                         "watchdog hangs at teardown while captured collectives are alive: opt-in)")
     ap.add_argument("--nccl-max-ctas", type=int, default=0, help="N > 1: cap NCCL's CTAs per collective (NCCL_MAX_CTAS) so that the all-reduce "
                                                                   "overlapping the backward takes fewer SMs from the persistent GEMMs; 0 = NCCL default")
     ap.add_argument("--bwd-gemm-ctas", type=int, default=-1,
                     help="N > 1: persistent CTAs of the backward-pass GEMMs (they run beside NCCL's all-reduce kernels; a GEMM CTA that finds "
-                         "its SM taken starts after the others and serialises its whole static tile share). -1 = 132 (measured at N = 2: 12.39 ms/step vs "
-                         "12.49 with one CTA per SM and 12.46 with 116), 0 = one per SM")
+                         "its SM taken starts after the others and serialises its whole static tile share). -1 = all SMs but 16, the SMs NCCL's all-reduce "
+                         "kernels hold (its channel count, which --nccl-max-ctas caps), not a share of the GPU; 0 = one per SM")
     ap.add_argument("--arena-gb", type=float, default=0.0,
                     help="share ONE activation arena of this size between the plans (Engine.enable_activation_arena): config 5 keeps 12 plans "
-                         "whose private activations add up to 42.7 GB; 0 = private buffers per plan")
+                         "with private activations each; 0 = private buffers per plan")
     ap.add_argument("--segments", type=int, default=8, help="N > 1: number of backward pieces whose gradient ranges are all-reduced while the rest runs")
     ap.add_argument("--eval-mode", action="store_true", help="disable the dropout layers (reference eval mode); default is train mode")
     ap.add_argument("--legacy-prologue", action="store_true", help="round-1 step body: weight cast + gradient memset inside the step, no fused optimizer")
@@ -256,6 +242,9 @@ def main():
     ap.add_argument("--no-module-api", action="store_true", help="skip the VILBertForVLTasks.forward -> loss.backward() leg")
     ap.add_argument("--cpu-batch", type=int, default=8)
     ap.add_argument("--profile-ops", action="store_true", help="print the per-kernel-class time table to stderr")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (float32, seeded samples of large arrays); "
+                         "the gradient buffer is zeroed and the dropout counter reset before that step")
     a = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -321,7 +310,7 @@ def main():
     cfg_o = O.make_config(cfgj)
     eng = Engine(BertConfig.from_dict(cfgj), dev, heads=C.get("heads", "vl"), precision=a.precision)
     if world > 1:
-        eng.bwd_gemm_max_ctas = a.bwd_gemm_ctas if a.bwd_gemm_ctas >= 0 else 132
+        eng.bwd_gemm_max_ctas = a.bwd_gemm_ctas if a.bwd_gemm_ctas >= 0 else torch.cuda.get_device_properties(dev).multi_processor_count - 16
     if a.arena_gb > 0:
         eng.enable_activation_arena(int(a.arena_gb * 2 ** 30))
     # random-init weights of the named architecture (reference init: N(0, 0.02), zero bias, LN 1/0); same seed on every rank
@@ -444,8 +433,18 @@ def main():
         step()
     torch.cuda.synchronize()
     clocks.mark_begin()
-    ms = timed(lambda i: step(), a.steps)
+    def timed_step(i):
+        if a.dump_outputs and i == a.steps - 1:
+            # the step body accumulates into the gradient buffer (the optimizer zeroes it): the dumped gradient is the last
+            # step's alone, and its dropout masks are those of step 1 whatever --warmup and --steps are
+            eng.zero_grad(force=True)
+            eng.set_dropout_step(0)
+        step()
+
+    ms = timed(timed_step, a.steps)
     clocks.mark_end()
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, T, eng, torch)
     clk = clocks.stop() if rank == 0 else None
     ms_step = ms / a.steps
     loss_val = float(sum(t["plan"].loss.item() for t in T))
@@ -582,7 +581,7 @@ def main():
             dist.destroy_process_group()
         return
 
-    peak_sus, peak_burst, hbm, peak_src = measured_peaks()
+    peak_tc, hbm, peak_src = datasheet_peaks()
     flops_step = sum(3.0 * algorithmic_flops_fwd(cfgj, t["plan"].Nv, t["plan"].Nt) * t["B"] for t in T)   # fwd+bwd = 3 x forward (SURVEY.md §8d), per GPU
     pairs = sum(t["B"] * t["plan"].Nv * t["plan"].Nt for t in T) * world
     samples = sum(t["B"] for t in T) * world
@@ -599,7 +598,7 @@ def main():
                                  else "NCCL AVG of the flat fp32 gradient buffer after each backward (8 buckets)")),
                    "bwd_gemm_ctas": (eng.bwd_gemm_max_ctas or "one per SM"),
                    "activation_arena_gb": (round(max(t["plan"].arena_bytes for t in T) / 2 ** 30, 2) if eng.arena is not None else None),
-                   "l2": "working set (activations + weights + grads, GBs per step) exceeds the 126 MB L2; no explicit flush",
+                   "l2": "working set (activations + weights + grads, GBs per step) exceeds the 50 MB L2; no explicit flush",
                    "streams": "text and vision segments on two CUDA streams (parallel graph branches)" if eng.two_streams else "single stream",
                    "numerics": {"fp16": "fp16 forward tensor-core operands, bf16 gradient operands, fp32 accumulate/residual/LayerNorm/softmax",
                                 "bf16": "bf16 tensor-core operands, fp32 accumulate/residual/LayerNorm/softmax",
@@ -610,7 +609,7 @@ def main():
                    "loss": loss_val, "peak_memory_gb": round(mem_gb, 2), "plans": len(T)},
         "samples_per_s": samples / (ms_step / 1e3),
         "model_tflops_per_gpu": flops_step / (ms_step / 1e3) / 1e12,
-        "mfu_vs_measured_sustained_bf16": flops_step / (ms_step / 1e3) / 1e12 / peak_sus,
+        "mfu_vs_datasheet_bf16": flops_step / (ms_step / 1e3) / 1e12 / peak_tc,
         "gpu_launches": n_launch * a.steps,
         "clocks": clk,
         "e2e": {"value": pairs / (ms_e2e_step / 1e3), "unit": "pairs/s", "ms_per_step": ms_e2e_step, "h2d_bytes_per_step": h2d_bytes,
@@ -636,20 +635,18 @@ def main():
         dom, (dn, dms) = max(sigs.items(), key=lambda kv: kv[1][1])
         dflops = 2.0 * dom[0] * dom[1] * dom[2]
         dach = dflops / (dms / dn / 1e3) / 1e12
-        traffic, traffic_src = ncu_traffic(dom)
         out["roofline"] = {"bound": "tensor",
-                           "kernel": f"gemm_tcgen05_kernel M={dom[0]} N={dom[1]} K={dom[2]} (a_mn={dom[3]} b_mn={dom[4]} act={dom[5]} residual={dom[6]} "
+                           "kernel": f"gemm_wgmma_kernel M={dom[0]} N={dom[1]} K={dom[2]} (a_mn={dom[3]} b_mn={dom[4]} act={dom[5]} residual={dom[6]} "
                                      f"atomic={dom[7]}): the GEMM signature with the largest share of the step ({dn} launches, {dms:.3f} ms)",
-                           "achieved": dach, "peak": peak_sus, "unit": "TFLOP/s", "frac": dach / peak_sus,
-                           "traffic": traffic, "traffic_unit": "bytes/launch (ncu dram__bytes_read.sum + dram__bytes_write.sum, cold cache)", "traffic_source": traffic_src,
+                           "achieved": dach, "peak": peak_tc, "unit": "TFLOP/s", "frac": dach / peak_tc,
                            "algorithmic_flops_per_launch": dflops, "avg_launch_us": dms / dn * 1e3,
-                           "peak_source": peak_src + ", sustained cuBLAS bf16",
+                           "peak_source": peak_src,
                            "how": "algorithmic 2MNK / mean CUDA-event duration of that launch in an eager single-stream replay of the step"}
-        out["roofline_all_gemm"] = {"bound": "tensor", "kernel": "gemm_tcgen05_kernel (all launches of one step)",
+        out["roofline_all_gemm"] = {"bound": "tensor", "kernel": "gemm_wgmma_kernel (all launches of one step)",
                            "how": "sum of algorithmic 2MNK over the step's GEMM launches / sum of their CUDA-event durations in an eager single-stream replay "
                                   "(each launch bracketed by events, so launch gaps and event latency count against the kernel)",
-                           "achieved": ach, "peak": peak_sus,
-                           "unit": "TFLOP/s", "frac": ach / peak_sus, "traffic": None, "peak_source": peak_src + ", sustained cuBLAS bf16",
+                           "achieved": ach, "peak": peak_tc,
+                           "unit": "TFLOP/s", "frac": ach / peak_tc, "peak_source": peak_src,
                            "launches_per_step": gm["n"], "kernel_ms_per_step": gm["ms"], "algorithmic_flops_per_step": gm["flops"],
                            "share_of_step": gm["ms"] / sum(d["ms"] for d in prof.values())}
         out["kernel_classes_ms"] = {k: round(d["ms"], 4) for k, d in sorted(prof.items(), key=lambda kv: -kv[1]["ms"])}
@@ -667,21 +664,32 @@ def main():
         dist.destroy_process_group()
 
 
-def ncu_traffic(sig):
-    """DRAM bytes per launch of a GEMM signature from the newest committed `ncu --set full` summary that lists it
-    (profiles/*_ncu_gemm_traffic.json, written by tools/ncu_summary.py from the capture of the SAME kernels); None (and the
-    reason) when no capture of the shipped kernels covers it — never a number from an older kernel."""
-    import glob
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_ncu_gemm_traffic.json")))
-    for f in reversed(files):
-        try:
-            d = json.load(open(f))
-        except Exception:   # noqa: BLE001
-            continue
-        key = ",".join(str(int(x)) for x in sig)
-        if key in d.get("signatures", {}):
-            return d["signatures"][key], os.path.basename(f)
-    return None, "no ncu capture of the shipped kernels lists this signature"
+def dump_outputs(dirname, T, eng, torch, budget_bytes=60 << 20):
+    """Writes what the last timed step left in the plans' output buffers: per task the loss and every output the plan returns
+    (with a shared activation arena only the last task's outputs are still intact), and the flat gradient buffer, which holds the
+    last step's gradients alone (zeroed before it). An array
+    larger than its share of the budget is replaced by a fixed sample of its elements (seeded by the array's name and size)."""
+    import zlib
+    import numpy as np
+    torch.cuda.synchronize()
+    arrays = []
+    multi = len(T) > 1
+    for i, t in enumerate(T):
+        plan, pre = t["plan"], (t["name"] + "." if multi else "")
+        if plan.loss is not None:
+            arrays.append((pre + "loss", plan.loss))
+        if eng.arena is None or i == len(T) - 1:
+            arrays += [(pre + k, v) for k, v in sorted(plan.outputs.items())]
+    arrays.append(("grad", eng.ps.grad))
+    cap = budget_bytes // 4 // len(arrays)
+    os.makedirs(dirname, exist_ok=True)
+    for name, x in arrays:
+        x = x.detach().reshape(-1)
+        if x.numel() > cap:
+            g = torch.Generator().manual_seed(zlib.crc32(f"{name}:{x.numel()}".encode()))
+            idx = torch.randint(0, x.numel(), (cap,), generator=g).to(x.device)
+            x, name = x[idx], name + ".sample"
+        np.save(os.path.join(dirname, name + ".npy"), x.float().cpu().numpy())
 
 
 def run_module_api(cfgj, t, a, torch, O, timed):

@@ -1,5 +1,5 @@
 /*
- * vilbert_b200.h — C ABI of libvilbert_b200.so: the sm_100a kernels behind the ViLBERT two-stream
+ * vilbert_b200.h — C ABI of libvilbert_b200.so: the sm_90a kernels behind the ViLBERT two-stream
  * co-attentional encoder hot path (reference: vilbert/vilbert.py:396-1107 BertLayer / BertImageLayer /
  * BertConnectionLayer / BertEncoder, :320-367 + :1409-1432 embeddings, :1110-1137 poolers,
  * :1140-1258 + :1638-1722 heads).
@@ -31,7 +31,7 @@ typedef int vb_status;
 enum {
   VB_OK = 0,
   VB_ERR_INVALID = 1,     /* bad shape / alignment / argument                     */
-  VB_ERR_UNSUPPORTED = 2, /* device is not sm_100 or an unsupported configuration */
+  VB_ERR_UNSUPPORTED = 2, /* device is not sm_90 or an unsupported configuration  */
   VB_ERR_CUDA = 3         /* a CUDA runtime / driver call failed                  */
 };
 
@@ -57,7 +57,7 @@ const char* vb_last_error(void);
 vb_status vb_device_info(int* sm_count, int* cc);
 
 /* ------------------------------------------------------------------------------------------------
- * Dense contraction on the tcgen05 tensor cores (TMA -> 128B-swizzled smem -> tcgen05.mma -> TMEM).
+ * Dense contraction on the Hopper tensor cores (TMA -> 128B-swizzled smem -> wgmma -> fp32 registers).
  *   D[M,N] = alpha * sum_k A(m,k) * B(n,k)   followed by the fused epilogue
  *   v = D (+ bias[n]); act; (+ residual[m,n]); -> out_f32 / out_bf16
  * Replaces every nn.Linear on the path (vilbert.py:410-412,466,492,509 text; :553-555,625,653,670
@@ -105,16 +105,15 @@ typedef struct vb_gemm_args {
   /* debug/test overrides for the smem matrix descriptors (0 = library default) */
   uint32_t dbg_lbo_a, dbg_sbo_a, dbg_lbo_b, dbg_sbo_b;
   void* dbg_timeline;    /* NULL, or u64 [grid][10]: per-CTA clock64 / globaltimer stamps (development only) */
-  int32_t cluster_m;     /* 0 = auto, 1 = no clusters, 2 = CTA pairs (tcgen05 cta_group::2) on adjacent row blocks */
+  int32_t cluster_m;     /* 0 = auto, 1 = no clusters, 2 = CTA pairs (2-CTA clusters sharing B by TMA multicast) on adjacent row blocks */
   /* ---- ABI v2: 16-bit operand formats and split precision -------------------------------------------------
    * Forward operands (activations, weights) are IEEE fp16 (11 significant bits; the reference's own reduced
    * precision mode is fp16, train_concap.py:504-505), gradient operands are bf16 (range). a_fp16 / b_fp16 / out_fp16:
-   * 0 = bf16, 1 = fp16 (out_fp16 is the format of out_bf16 and out_lo). A and B must have the SAME format: tcgen05
-   * kind::f16 encodes them separately but B200 raises an illegal-instruction fault on fp16 x bf16 (measured, round 2),
-   * so the backward contractions (dy bf16) read bf16 copies of the forward operands: out_b16 (same ld as out_bf16) is an
+   * 0 = bf16, 1 = fp16 (out_fp16 is the format of out_bf16 and out_lo). A and B must have the SAME format (wgmma takes
+   * one operand type for both), so the backward contractions (dy bf16) read bf16 copies of the forward operands: out_b16 (same ld as out_bf16) is an
    * additional, always-bf16 copy of the 16-bit output, written by the forward GEMM for the weight-gradient GEMM.
    * Split precision ("fp32 parity mode", 1e-3): an operand x is stored as hi = fp16(x), lo = fp16(x - hi); with
-   * A_lo and/or B_lo given the contraction is A.B + A_lo.B + A.B_lo (three passes over K into the same TMEM
+   * A_lo and/or B_lo given the contraction is A.B + A_lo.B + A.B_lo (three passes over K into the same register
    * accumulator; the lo.lo term, 2^-22 relative, is dropped). A_lo / B_lo use lda / ldb and the major of A / B.
    * out_lo (same ld as out_bf16) receives the low part of the value written to out_bf16. */
   int32_t a_fp16, b_fp16, out_fp16;

@@ -1,6 +1,7 @@
 """Shared GPU check helpers (used by the -m gpu tests and by the tools/ probe drivers).
 Every check runs the CUDA path through the C ABI (ctypes) and compares with torch fp32 / the oracle."""
 import ctypes as C
+import gc
 import math
 
 import torch
@@ -239,6 +240,10 @@ def model_case(cfgj, B, Nv, Nt, seed=0, qk_scale=1.0, names=None, grads=True, de
     where each is {tensor name: error}; gradient errors are (max-rel with floor, rel-L2).
     train_step=k runs the engine in TRAIN mode (every nn.Dropout of the reference active, dropout step counter = k) against
     the oracle with the same stateless masks (oracle.DropMasks(k))."""
+    # engines and plans of earlier cases hold each other in reference cycles: collect them before building a new one, an 80 GB
+    # card does not hold several full-size engines at once
+    gc.collect()
+    torch.cuda.empty_cache()
     dev = torch.device(device)
     cfg = O.make_config(cfgj)
     names = O.HEAD_NAMES if names is None else names

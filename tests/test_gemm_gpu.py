@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (vb_gemm_bf16) through the C ABI vs torch fp32 matmul of the same bf16 operands.
+"""wgmma GEMM (vb_gemm_bf16) through the C ABI vs torch fp32 matmul of the same bf16 operands.
 Tolerance: 2e-3 of max|ref| (fp32 accumulation-order noise; bf16 output rounding is discounted in the helper)."""
 import pytest
 
@@ -51,7 +51,7 @@ def test_mn_major_operands(a_mn, b_mn, M, N, K, bn):
     (dict(a_mn=True, b_mn=True, atomic=True, split_k=3), (768, 520, 2304)),
 ])
 def test_cta_pairs(kw, shape, bn):
-    """cluster_m=2: CTA pairs (tcgen05 cta_group::2) on adjacent row blocks; the leader issues 256 x BN MMAs for both (vb_gemm.cu)."""
+    """cluster_m=2: CTA pairs (2-CTA clusters) on adjacent row blocks; each CTA loads half of the B tile and multicasts it to both (vb_gemm.cu)."""
     from _gpu_util import gemm_case
     err, _ = gemm_case(*shape, block_n=bn, cluster_m=2, **kw)
     assert err < 2e-3, err
@@ -74,8 +74,7 @@ def test_fp16_operands(kw, shape):
 
 
 def test_mixed_operand_formats_are_rejected():
-    """tcgen05 kind::f16 encodes the A and B formats separately, but fp16 x bf16 raises an illegal-instruction fault on B200
-    (measured in round 2): the library refuses the combination instead of launching it."""
+    """wgmma takes one 16-bit operand type for both A and B: the library refuses fp16 x bf16 instead of launching it."""
     import ctypes as C
     import torch
     lib = L.lib()
@@ -97,7 +96,7 @@ def test_mixed_operand_formats_are_rejected():
     (dict(bias=True, res=True, cluster_m=2), (6400, 1024, 4096)),
 ])
 def test_split_precision(kw, shape):
-    """fp32 parity mode: operands as fp16 hi + lo, three passes (hi.hi + lo.hi + hi.lo) into one TMEM accumulator; the
+    """fp32 parity mode: operands as fp16 hi + lo, three passes (hi.hi + lo.hi + hi.lo) into one register accumulator; the
     16-bit output is written as hi + lo too. Compared with the float64 product of the fp32 operands: 5e-5 of max|ref|
     (single-pass fp16 operands give ~5e-4, bf16 ~4e-3)."""
     from _gpu_util import gemm_case

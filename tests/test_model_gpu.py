@@ -3,12 +3,10 @@
 Numerical contract (BASELINE.json north_star: outputs "within 1e-3 rel fp32 / 1e-2 bf16" of the reference), checked as
 `max|a-b| / max|ref|` per tensor against the fp32 oracle (== the reference, bit-exact on CPU), on EVERY one of the 13 outputs
 (sequence_output_t/v, pooled_output_t/v and the nine task-head outputs) with no per-head allowance:
-  * default precision "fp16" (fp16 forward operands, bf16 gradient operands, fp32 accumulate): 1e-2 — measured 0.8-3.6e-3 at
-    config 2 (B=64), 5.2e-3 worst on bert_large (profiles/r02_model_probe_precisions_v1.log);
-  * precision "fp32" (split precision, fp16 hi+lo operands, 3 tensor-core passes): 1e-3 — measured <= 7.5e-5 (base), 1.7e-4 (large).
+  * default precision "fp16" (fp16 forward operands, bf16 gradient operands, fp32 accumulate): 1e-2;
+  * precision "fp32" (split precision, fp16 hi+lo operands, 3 tensor-core passes): 1e-3.
 Gradients are not part of the north_star contract; they are bounded against the fp32 oracle by rel-L2 per tensor (worst and
-median over all parameter tensors) with the measured values (median 5e-3, worst 8e-3 on base-6-6; 9e-3 / 2.3e-2 on
-bert_large) plus margin, and against the oracle run under the engine's operand rounding ("op" mode).
+median over all parameter tensors), and against the oracle run under the engine's operand rounding ("op" mode).
 """
 import json
 import math
@@ -199,7 +197,7 @@ def test_dynamic_attention_base_shape(golden_dir):
     """dynamic_attention at the base 6-layer widths (Hv 1024 gated by Ht 768) and the VQA sequence lengths, small batch."""
     from _gpu_util import model_case
     cfgj = dict(_cfg(golden_dir, "base_6layer_6conect_b4"), dynamic_attention=True)
-    # measured worst gradient rel-L2 3.1e-2 (query / key biases of the first text layers, whose exact gradient is close to zero at B=4)
+    # looser worst-case gradient bound: the query / key biases of the first text layers have an exact gradient close to zero at B=4
     _check(model_case(cfgj, 4, 100, 36, seed=0), grad_worst=5e-2, grad_median=1.5e-2)
     import vilbert_b200
     with pytest.raises(NotImplementedError):
@@ -375,7 +373,7 @@ def test_config3_pretraining_objective_fused_losses(golden_dir):
     # tensors whose exact gradient is ~0 (key biases: softmax shift invariance) are excluded by a floor of 1e-3 of the largest gradient
     gmax = max(v.grad.abs().max().item() for v in Pg.values() if v.grad is not None)
     l2 = sorted((rel_l2(eng.ps.g(k), Pg[k].grad), k) for k in eng.ps.entries if Pg[k].grad is not None and Pg[k].grad.abs().max().item() > 1e-3 * gmax)
-    assert len(l2) > 100 and l2[-1][0] < 5e-2 and l2[len(l2) // 2][0] < 1.5e-2, l2[-3:]   # measured 1.5e-2 worst, 1.06e-2 median at B=64
+    assert len(l2) > 100 and l2[-1][0] < 5e-2 and l2[len(l2) // 2][0] < 1.5e-2, l2[-3:]
 
 
 @pytest.mark.parametrize("precision", ["fp16", "fp32"])
@@ -608,7 +606,7 @@ def test_config5_split_precision_forward(golden_dir, B, Nv, Nt):
 def test_config4_bert_large_vcr_shape_full_size(precision):
     """BASELINE.json configs[3] per-GPU share: bert_large_6layer_6conect (24 text layers, 1024/4096, 16 heads), B=32 (global 256
     / 8), 100 regions, 60 tokens; all 13 outputs inside the contract, gradients of the VL-logit + VQA heads' paths bounded
-    (36 sub-layers deep: measured median 9e-3, worst 2.3e-2 rel-L2 in the default precision)."""
+    (36 sub-layers deep, hence the looser gradient bounds)."""
     from _gpu_util import model_case
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     cfgj = json.load(open(os.path.join(root, "vilbert-multi-task_b200", "configs", "bert_large_6layer_6conect.json")))

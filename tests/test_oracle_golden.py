@@ -45,8 +45,12 @@ def test_oracle_matches_reference_tensors(name, golden_dir):
         assert rel(bert_o[k], v) < 1e-5, k
     for k, v in gold["heads"].items():
         assert rel(heads_o[k], v) < 1e-5, k
+    # Key biases get an analytically zero gradient (softmax is invariant to a per-row shift): what is left of it is fp32
+    # rounding noise whose digits depend on the host's BLAS, so gradients are held to 1e-5 of their own magnitude but not
+    # below 1e-6 of the largest gradient.
+    gmax = max(v.abs().max().item() for v in gold["grads"].values())
     for k, v in gold["grads"].items():
-        assert rel(Pg[k].grad, v) < 1e-5, k
+        assert (Pg[k].grad - v).abs().max().item() <= 1e-5 * max(v.abs().max().item(), 1e-6 * gmax), k
     # q_dense1/2 never receive a gradient (vilbert.py:834,841)
     assert all(Pg[k].grad is None for k in Pg if "q_dense" in k)
 

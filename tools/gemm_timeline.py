@@ -9,7 +9,8 @@ def run(M, N, K, bn, res=False, a_mn=False, b_mn=False, atomic=False, split_k=1,
     B = (torch.randn(K, N, device=dev) if b_mn else torch.randn(N, K, device=dev)).to(BF)
     o16 = torch.empty(M, N, device=dev, dtype=BF)
     out = torch.empty(M, N, device=dev); r = torch.randn(M, N, device=dev)
-    dbg = torch.zeros(148 * 10, dtype=torch.int64, device=dev)
+    nsm = torch.cuda.get_device_properties(0).multi_processor_count
+    dbg = torch.zeros(nsm * 10, dtype=torch.int64, device=dev)
     g = L.GemmArgs(); g.M, g.N, g.K = M, N, K
     g.A, g.lda, g.a_mn_major, g.B, g.ldb, g.b_mn_major = A.data_ptr(), (M if a_mn else K), int(a_mn), B.data_ptr(), (N if b_mn else K), int(b_mn)
     g.alpha, g.split_k, g.block_n, g.atomic_out = 1.0, split_k, bn, int(atomic)
@@ -22,7 +23,7 @@ def run(M, N, K, bn, res=False, a_mn=False, b_mn=False, atomic=False, split_k=1,
     g.dbg_timeline = dbg.data_ptr()
     e0, e1 = torch.cuda.Event(True), torch.cuda.Event(True)
     e0.record(); L.check(lib.vb_gemm_bf16(C.byref(g), st)); e1.record(); torch.cuda.synchronize()
-    full = dbg.view(148, 10).cpu()
+    full = dbg.view(nsm, 10).cpu()
     live = full[:, 0] != 0
     full = full[live]
     t = full[:, :8]

@@ -1,14 +1,14 @@
 #!/usr/bin/env bash
-# Counts, per shipped object (sm_100a), the SASS mnemonics that prove tcgen05 / TMEM / TMA use (B200_PROFILING.md):
-#   UTCHMMA = tcgen05.mma, UTCBAR = tcgen05.commit, UTMALDG / UTMASTG = TMA tensor load / store, LDTM / STTM = tcgen05.ld / st,
-#   HMMA = legacy mma.sync, LDGSTS = cp.async, LDSM = ldmatrix. CPU-only (cuobjdump).   usage: tools/sass_counts.sh > profiles/rNN_sass_mnemonic_counts.txt
+# Counts, per shipped object (sm_90a), the SASS mnemonics that show wgmma / TMA use:
+#   HGMMA = wgmma.mma_async, UTMALDG / UTMASTG = TMA tensor load / store, SYNCS = mbarrier operations,
+#   HMMA = mma.sync, LDGSTS = cp.async, LDSM = ldmatrix. CPU-only (cuobjdump).   usage: tools/sass_counts.sh
 set -euo pipefail
 cd "$(dirname "$0")/../vilbert-multi-task_b200/csrc"
-echo "# cuobjdump -sass of the shipped objects (sm_100a): counts of the mnemonics that prove tcgen05 / TMEM / TMA use"
+echo "# cuobjdump -sass of the shipped objects (sm_90a): counts of the mnemonics that show wgmma / TMA use"
 for o in vb_*.o; do
   echo "## $o"
   s=$(/usr/local/cuda/bin/cuobjdump -sass "$o")
-  for m in UTCHMMA UTCBAR UTMALDG UTMASTG LDTM STTM HMMA LDGSTS LDSM 'ATOMS\|RED'; do
+  for m in HGMMA UTMALDG UTMASTG SYNCS HMMA LDGSTS LDSM 'ATOMS\|RED'; do
     printf "  %-14s %6d\n" "$m" "$(printf '%s\n' "$s" | grep -c "$m" || true)"
   done
 done

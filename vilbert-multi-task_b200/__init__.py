@@ -1,7 +1,7 @@
-"""vilbert-multi-task_b200 — Blackwell-native ViLBERT two-stream co-attentional encoder.
+"""vilbert-multi-task_b200 — Hopper-native ViLBERT two-stream co-attentional encoder.
 
 Python surface mirrors the reference (vilbert/vilbert.py: BertConfig, BertModel, VILBertForVLTasks,
-BertForMultiModalPreTraining); the arithmetic runs in libvilbert_b200.so (hand-written sm_100a CUDA,
+BertForMultiModalPreTraining); the arithmetic runs in libvilbert_b200.so (hand-written sm_90a CUDA,
 C ABI in include/vilbert_b200.h). Import as ``vilbert_b200``.
 """
 __version__ = "0.1.0"

@@ -123,7 +123,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise VBError(
                 f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(there is no CPU or PyTorch fallback for the ViLBERT B200 kernels)")
+                "(there is no CPU or PyTorch fallback for the ViLBERT kernels)")
         _lib = C.CDLL(LIB_PATH)
         _lib.vb_last_error.restype = C.c_char_p
         _lib.vb_version.restype = C.c_int

@@ -88,7 +88,7 @@ class BertConfig(object):
     def to_json_string(self):
         return json.dumps(self.to_dict(), indent=2, sort_keys=True) + "\n"
 
-    # ---- support checks for the B200 engine (features the reference has but the hot path here does not)
+    # ---- support checks for the H100 engine (features the reference has but the hot path here does not)
     def check_supported(self):
         unsupported = []
         if self.hidden_act != "gelu" or self.v_hidden_act != "gelu":

@@ -6,7 +6,7 @@
 // lives in shared memory and S / P never touch HBM. One CTA = (64-row query tile, head, batch) with
 // 4 warps x 16 rows; tensor-core work uses warp-level mma.sync m16n8k16 (bf16 -> fp32) with ldmatrix
 // operand fetch, row statistics via warp-shuffle online softmax over 64-key blocks. 1.8 % of the
-// model FLOPs live here (SURVEY.md §8d); the tcgen05 path is reserved for the dense contractions.
+// model FLOPs live here (SURVEY.md §8d); the wgmma path is reserved for the dense contractions.
 // Q/K/V are read in place from the packed QKV GEMM output (row stride = ld, head offset h*D), so the
 // reference's permute().contiguous() copies (vilbert.py:416-422, 447) never materialise.
 //
@@ -751,16 +751,9 @@ static int launch_att(Kern kern, dim3 grid, size_t smem, const AttnParams& p, cu
 
 }  // namespace vb
 
-namespace vb {
-// tcgen05 / TMEM / TMA forward for Nq, Nk <= 128 and head dim 64 / 128 (vb_attn_tc.cu)
-bool attn_fwd_tc_eligible(const vb_attn_args* a);
-int attn_fwd_tc_launch(const vb_attn_args* a, cudaStream_t st);
-}  // namespace vb
-
 extern "C" vb_status vb_attention_fwd(const vb_attn_args* a, void* stream) {
   using namespace vb;
   if (int s = validate(a, false)) return s;
-  if (attn_fwd_tc_eligible(a)) return attn_fwd_tc_launch(a, (cudaStream_t)stream);
   const AttnParams p = to_params(a);
   const int nkp = (a->Nk + KB - 1) / KB * KB;
   const bool split = a->Q_lo || a->K_lo || a->V_lo;
@@ -839,7 +832,7 @@ extern "C" vb_status vb_attention_probs(const vb_attn_args* a, float* probs, voi
   AttnParams p = to_params(a);
   const long long rows = (long long)a->B * a->H * a->Nq;
   long long blocks = (rows + 7) / 8;
-  int cap = sm_count() * 8; if (cap <= 0) cap = 148 * 8;
+  int cap = sm_count() * 8; if (cap <= 0) cap = 132 * 8;
   const int grid = (int)(blocks < cap ? blocks : cap);
   cudaError_t e = launch_pdl(attn_probs_kernel, dim3(grid), dim3(256), (size_t)(8 * a->D * sizeof(float)), (cudaStream_t)stream, p, probs, (int)a->D);
   if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_attention_probs: %s", cudaGetErrorString(e));

@@ -1,20 +1,22 @@
-// vb_gemm.cu — persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// vb_gemm.cu — persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   D[M,N] = alpha * A[M,K] . B[N,K]^T  (bf16 operands, fp32 accumulation in TMEM) + fused epilogue.
+//   D[M,N] = alpha * A[M,K] . B[N,K]^T  (16-bit operands, fp32 accumulation in registers) + fused epilogue.
 //
 // Replaces the aten addmm behind every nn.Linear on the ViLBERT hot path and its autograd
 // (reference: vilbert/vilbert.py:410-412,466,492,509,553-555,625,653,670,716-725,830,837,865-869 and
 // SURVEY.md appendix A). Design:
-//   warp 0      TMA producer: cp.async.bulk.tensor 2D boxes (64 x rows, 128B swizzle) into a
-//               NUM_STAGES-deep smem ring, completion on mbarriers (complete_tx);
-//   warp 1      single-thread tcgen05.mma issuer (UMMA 128 x BN x 16, cta_group::1), accumulators
-//               double-buffered in TMEM (2 x BN fp32 columns) so the epilogue of tile i overlaps the
-//               main loop of tile i+1; tcgen05.commit releases smem stages / publishes accumulators;
-//   warps 2..9  epilogue (two per TMEM lane quadrant, alternate 32-column chunks): tcgen05.ld (32 lanes x 32 columns)
-//               -> XOR-swizzled smem transpose -> row-wise,
-//               128-bit coalesced pass doing bias / erf-GELU / GELU' / residual / bf16 conversion.
-// Operands may be K-major (nn.Linear forward) or MN-major (dgrad / wgrad operands read in place, no
-// transposed copies); both use the canonical SWIZZLE_128B UMMA layouts written directly by TMA.
+//   warpgroup 0      TMA producer: one elected lane of warp 0 issues cp.async.bulk.tensor 2D boxes (64 x rows, 128B swizzle)
+//                    into a NUM_STAGES-deep smem ring, completion on mbarriers (complete_tx); warps 1..3 only hold the
+//                    warpgroup slot so that the consumers start at a warpgroup boundary;
+//   warpgroups 1, 2  consumers, 64 rows of the 128 x BN tile each: wgmma.mma_async (m64 n128 k16, two per k step when BN = 256)
+//                    from the swizzled stages into fp32 register accumulators; a stage is released once the wgmma group
+//                    reading it has retired (one group stays in flight). Then the epilogue of the warp's 16 rows: registers ->
+//                    XOR-swizzled smem tile -> row-wise, 128-bit coalesced pass doing bias / erf-GELU / GELU' / residual /
+//                    16-bit conversion, while the producer already loads the next tile's stages.
+// Operands may be K-major (nn.Linear forward) or MN-major (dgrad / wgrad operands read in place, no transposed copies); both
+// are the canonical SWIZZLE_128B layouts TMA writes, wgmma reads the MN-major ones with its transpose flag.
+// CTA pairs (cluster_m = 2): a 2-CTA cluster on adjacent row blocks of one column block; each CTA loads half of the common B
+// tile and multicasts it into both, so B crosses from L2 once per pair.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -25,31 +27,28 @@
 
 namespace vb {
 
-constexpr int BM = 128;          // UMMA M (cta_group::1)
-constexpr int BK = 64;           // one 128-byte swizzle span of bf16
-constexpr int UK = 16;           // UMMA K for 16-bit inputs
-constexpr int EPI_WARPS = 8;      // two epilogue warps per TMEM lane quadrant: twice the global-memory requests in flight
-constexpr int GEMM_THREADS = 64 + EPI_WARPS * 32;
-// (Round 2 experiment, rejected: staging the fp32 residual of the F32 epilogue through a TMA ring fed by an 11th warp. The
-// epilogue is not latency-bound but bandwidth-bound — all 148 CTAs run their epilogues in lockstep, 64 KB read + 64 KB written
-// per tile = 7.5 TB/s chip-wide during that phase — and giving up two operand stages for the ring slowed the main loop:
-// 34.3 us vs 29.8 us on 6400x1024x1024, profiles/r02_gemm_timeline_residual_tma_ring_rejected.log.)
-// Epilogue staging tile per warp: 32 rows x 32 fp32, dense 128-byte rows whose 16-byte chunks are XOR-swizzled with the
-// row index (chunk ^ (row & 7)): thread-per-row 128-bit stores and row-wise 128-bit loads are both bank-conflict free
-// without padding (4 KB per warp).
-constexpr int STAGING_BYTES_PER_WARP = 32 * 32 * 4;
+constexpr int BM = 128;          // rows of a CTA tile: two consumer warpgroups x wgmma M = 64
+constexpr int BK = 64;           // one 128-byte swizzle span of a 16-bit operand
+constexpr int UK = 16;           // wgmma K for 16-bit inputs
+constexpr int CONSUMER_WARPS = 8;
+constexpr int GEMM_THREADS = 128 + CONSUMER_WARPS * 32;
+constexpr int EPI_ROWS = 16;              // rows of the tile whose accumulators one consumer warp holds
+constexpr int EPI_PS = EPI_ROWS / 4;      // passes of the coalesced epilogue (4 rows per pass)
+// Epilogue staging tile per warp: 16 rows x 32 fp32, dense 128-byte rows whose 16-byte chunks are XOR-swizzled with the
+// row index (chunk ^ (row & 7)): the fragment stores and the row-wise 128-bit loads spread over all banks without padding
+// (2 KB per warp).
+constexpr int STAGING_BYTES_PER_WARP = EPI_ROWS * 32 * 4;
 __device__ __forceinline__ int stg_off(int row, int col) { return row * 32 + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3)); }
 
-// CG = 1: one CTA per 128 x BN tile. CG = 2: CTA pairs (tcgen05 cta_group::2) on a 256 x BN tile; each CTA stages its 128
-// rows of A and its BN/2 rows of B, so a stage is smaller and the ring deeper (192 KB of operand stages either way).
-template <int BN, int CG>
+// One stage = the 128 x 64 A box and the BN x 64 B box (in a CTA pair each CTA still holds the whole B box: half loaded by
+// itself, half multicast by the peer). 192 KB of stages leave room for the staging tiles within the 227 KB of an H100 block.
+template <int BN>
 struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = (BN / CG) * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int NUM_STAGES = (192 * 1024) / STAGE_BYTES;   // 6 / 4 (CG 1), 8 / 6 (CG 2)
-  static constexpr int TMEM_COLS = 2 * BN;
-  static constexpr int SMEM_BYTES = NUM_STAGES * STAGE_BYTES + EPI_WARPS * STAGING_BYTES_PER_WARP + 256 /*barriers*/;
+  static constexpr int NUM_STAGES = (192 * 1024) / STAGE_BYTES;   // 6 (BN 128) / 4 (BN 256)
+  static constexpr int SMEM_BYTES = NUM_STAGES * STAGE_BYTES + CONSUMER_WARPS * STAGING_BYTES_PER_WARP + 256 /*barriers*/;
 };
 
 struct GemmKernelParams {
@@ -79,22 +78,19 @@ struct GemmKernelParams {
   float* out_colsum;
   int vec_f32, vec_bf16, vec_pre, vec_res, vec_aux;  // 128/64-bit access legal for that buffer
   uint64_t desc_base_a, desc_base_b;                 // smem descriptor without the address field
-  uint32_t kadv_a, kadv_b;                           // descriptor address advance per UMMA_K (bytes)
-  uint32_t idesc;
+  int mma_kind;              // bit 0: B MN-major, bit 1: A MN-major, bit 2: fp16 operands (else bf16)
   DropCfg drop;              // dropout on the epilogue value before the residual add (EPI_F32 / generic)
-  int a_mn, b_mn;            // operand majors (runtime: only the TMA producer cares)
-  int cluster;               // 1, or 2 = CTA pairs (tcgen05 cta_group::2): the two CTAs take adjacent row blocks of one column
-                             // block; the leader issues 256 x BN MMAs for both, each CTA stages its 128 rows of A and its
-                             // half of the B tile -> per-SM operand traffic (L2 -> smem and smem -> tensor core) drops by 25-33 %
+  int a_mn, b_mn;            // operand majors
+  int cluster;               // 1, or 2 = CTA pairs: the two CTAs of a cluster take adjacent row blocks of one column block and
+                             // share its B tile through TMA multicast
   int num_m_groups;          // ceil(num_m_blocks / cluster)
   int fast_ok;               // every buffer the specialised epilogue touches allows 128/64-bit accesses
   unsigned long long* dbg;   // optional per-CTA timeline [grid][10] (8 x clock64 + 2 x globaltimer ns), NULL in production
 };
 
-// Epilogue specialisations. Each instantiation keeps ONE compact, fully unrolled fast path (whole 32x32 chunk inside
-// the matrix, 128/64-bit aligned buffers) plus a shared non-inlined generic path for ragged edges / odd layouts.
-// (A single kernel with every variant inlined is ~180 KB of SASS and thrashes the instruction cache: the epilogue
-// of one 128x128 tile then costs ~29k cycles instead of ~2k — measured with the clock64 timeline, profiles/.)
+// Epilogue specialisations. Each instantiation keeps ONE compact, fully unrolled fast path (whole 16x32 chunk inside
+// the matrix, 128/64-bit aligned buffers) plus a shared non-inlined generic path for ragged edges / odd layouts, so that
+// the epilogue code of a kernel stays small enough for the instruction cache.
 enum { EPI_F32 = 0,     // v = alpha*acc (+bias) (ReLU) (+fp32 residual) -> out_f32 (+ 16-bit copy)   (out-proj / FFN2 / dgrad-into-residual / logits / poolers)
        EPI_BF16 = 1,    // v = alpha*acc (+bias) -> out_bf16                                 (QKV, plain dgrads)
        EPI_GELU = 2,    // pre = acc + bias; gelu(pre) -> out_bf16 / out_f32; gelu'(pre) -> out_pre (bf16, saved for backward)
@@ -103,18 +99,13 @@ enum { EPI_F32 = 0,     // v = alpha*acc (+bias) (ReLU) (+fp32 residual) -> out_
        EPI_GENERIC = 5, // runtime flags only (ReLU poolers, unusual output combinations)
        EPI_COUNT = 6 };
 
-struct EpiCtx {
-  int m_base, n, nv, rr, cc;
-  bool full4;
-};
-
 // Generic, compact (non-unrolled) path: any flags, any alignment, ragged rows / columns.
 __device__ __noinline__ void epi_generic_chunk(const GemmKernelParams& p, const float* stg, int m_base, int n, int rr, int cc) {
   const int nv = min(4, p.N - n);
   if (nv <= 0) return;
   float cs[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll 1
-  for (int ps = 0; ps < 8; ++ps) {
+  for (int ps = 0; ps < EPI_PS; ++ps) {
     const int row = ps * 4 + rr;
     const long long m = m_base + row;
     if (m >= p.M) break;
@@ -188,7 +179,7 @@ __device__ __forceinline__ void store16x4(const GemmKernelParams& p, long long o
 // compact out-of-line routine selected per chunk inside the F32 kernel, so that kernel's unrolled fast path stays as small as it was.
 __device__ __noinline__ void epi_pool_chunk(const GemmKernelParams& p, const float* stg, int m_base, int n, int rr, int cc, const float4 b4) {
 #pragma unroll 1
-  for (int ps = 0; ps < 8; ++ps) {
+  for (int ps = 0; ps < EPI_PS; ++ps) {
     const int row = ps * 4 + rr;
     const long long m = m_base + row;
     const float4 a4 = *reinterpret_cast<const float4*>(stg + stg_off(row, cc));
@@ -201,11 +192,11 @@ __device__ __noinline__ void epi_pool_chunk(const GemmKernelParams& p, const flo
 
 template <int EPI, int OUT16>
 __device__ __forceinline__ void epi_fast_chunk(const GemmKernelParams& p, const float* stg, int m_base, int n, int rr, int cc,
-                                               const float4 (&resv)[8], const uint2 (&auxv)[8], const float4 b4) {
+                                               const float4 (&resv)[EPI_PS], const uint2 (&auxv)[EPI_PS], const float4 b4) {
   float cs0 = 0.f, cs1 = 0.f, cs2 = 0.f, cs3 = 0.f;
   const uint32_t dseed = (EPI == EPI_F32 && p.drop.ctr) ? drop_seed(p.drop) : 0u;
 #pragma unroll
-  for (int ps = 0; ps < 8; ++ps) {
+  for (int ps = 0; ps < EPI_PS; ++ps) {
     const int row = ps * 4 + rr;
     const long long m = m_base + row;
     const float4 a4 = *reinterpret_cast<const float4*>(stg + stg_off(row, cc));
@@ -254,14 +245,42 @@ __device__ __forceinline__ void epi_fast_chunk(const GemmKernelParams& p, const 
   }
 }
 
+// One 64-deep k-block of a consumer warpgroup: 4 k steps of wgmma (NACC n128 halves each), committed as one group.
+// MN-major operands advance 16 k rows = two 8-row groups (2 KB) per step, K-major ones 32 bytes inside the swizzle span.
+template <int NACC, int F16, int TA, int TB>
+__device__ __forceinline__ void mma_kblock(float (&acc)[NACC][64], uint32_t sa, uint32_t sb, const GemmKernelParams& p, bool accumulate) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < BK / UK; ++k) {
+    const uint64_t da = gmma_desc_at(p.desc_base_a, sa + k * (TA ? 2048 : UK * 2));
+#pragma unroll
+    for (int j = 0; j < NACC; ++j)
+      wgmma_m64n128k16<F16, TA, TB>(acc[j], da, gmma_desc_at(p.desc_base_b, sb + j * (128 * BK * 2) + k * (TB ? 2048 : UK * 2)),
+                                    (accumulate || k > 0) ? 1u : 0u);
+  }
+  wgmma_commit();
+}
+
+// Columns [32 c4, +32) of one n128 accumulator half -> the warp's staging tile (row = fragment row within the warp's 16).
+__device__ __forceinline__ void stage_chunk(const float (&d)[64], int c4, float* stg, int lane) {
+  const int r0 = lane >> 2, c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int ii = 0; ii < 4; ++ii) {
+    const int i = c4 * 4 + ii;
+    *reinterpret_cast<float2*>(stg + stg_off(r0, ii * 8 + c0)) = make_float2(d[4 * i], d[4 * i + 1]);
+    *reinterpret_cast<float2*>(stg + stg_off(r0 + 8, ii * 8 + c0)) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+  }
+}
+
 template <int BN, int EPI, int CG, int OUT16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                    const __grid_constant__ CUtensorMap tmap_a_lo, const __grid_constant__ CUtensorMap tmap_b_lo,
-                    const GemmKernelParams p) {
-  using Cfg = GemmCfg<BN, CG>;
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                  const __grid_constant__ CUtensorMap tmap_a_lo, const __grid_constant__ CUtensorMap tmap_b_lo,
+                  const GemmKernelParams p) {
+  using Cfg = GemmCfg<BN>;
   constexpr bool pair = (CG == 2);
   constexpr int NUM_STAGES = Cfg::NUM_STAGES;
+  constexpr int NACC = BN / 128;
 
   // SWIZZLE_128B tiles need 1024-byte alignment: the kernel has no static shared memory, so the dynamic window starts at
   // the CTA's (1024-aligned) shared base; checked once below.
@@ -269,12 +288,9 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* smem_tiles = smem;
   float* staging = reinterpret_cast<float*>(smem + NUM_STAGES * Cfg::STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NUM_STAGES * Cfg::STAGE_BYTES + EPI_WARPS * STAGING_BYTES_PER_WARP);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NUM_STAGES * Cfg::STAGE_BYTES + CONSUMER_WARPS * STAGING_BYTES_PER_WARP);
   uint64_t* full_bar = bars;                       // [NUM_STAGES]
   uint64_t* empty_bar = bars + NUM_STAGES;         // [NUM_STAGES]
-  uint64_t* tmem_full_bar = bars + 2 * NUM_STAGES; // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;    // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -282,47 +298,32 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
 #define VB_DBG_NS(slot) do { if (p.dbg) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); p.dbg[blockIdx.x * 10 + (slot)] = t_; } } while (0)
   if (threadIdx.x == 0) { VB_DBG(0); VB_DBG_NS(8); }
 
-  if (warp_idx == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     if (p.npass > 1) { tma_prefetch_desc(&tmap_a_lo); tma_prefetch_desc(&tmap_b_lo); }
     for (int s = 0; s < NUM_STAGES; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&tmem_full_bar[s]), 1);
-      mbar_init(smem_u32(&tmem_empty_bar[s]), EPI_WARPS * CG);   // one arrive per epilogue warp (of both CTAs of a pair)
+      mbar_init(smem_u32(&empty_bar[s]), CONSUMER_WARPS * CG);   // one arrive per consumer warp (of both CTAs of a pair)
     }
     fence_mbar_init();
   }
-  __syncwarp();
-  if (warp_idx == 1) {
-    if constexpr (pair) { tmem_alloc_pair(smem_u32(tmem_ptr_smem), Cfg::TMEM_COLS); tmem_relinquish_pair(); }
-    else                { tmem_alloc(smem_u32(tmem_ptr_smem), Cfg::TMEM_COLS); tmem_relinquish(); }
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  // the barriers of both CTAs of a pair must exist before the peer's TMA / commits / arrives reach them
+  // the barriers of both CTAs of a pair must exist before the peer's multicast loads / arrives reach them
   if constexpr (pair) cluster_sync_all();
-  pdl_entry();   // everything above (barrier init, TMEM alloc, descriptor prefetch) overlapped the previous kernel's tail
+  pdl_entry();   // everything above (barrier init, descriptor prefetch) overlapped the previous kernel's tail
   if (threadIdx.x == 0) VB_DBG(1);
 
   // work items = (row-block group, column block, k split); the CTAs of a pair walk the same items in lockstep, CTA
   // `crank` takes row block group * cluster + crank (possibly past the matrix: it then loads zero rows and stores
-  // nothing, but still stages its half of B)
+  // nothing, but still loads and multicasts its half of B)
   const int crank = pair ? (int)cluster_ctarank() : 0;
   const int group = blockIdx.x / CG;
   const int num_groups = gridDim.x / CG;
   const int total_work = p.num_m_groups * p.num_n_blocks * p.split_k;
-  const bool leader = (crank == 0);
 
   if (warp_idx == 0) {
-    // ================================================================ TMA producer (one elected lane issues; the warp stays converged).
-    // The guard must be elect.sync, not `lane == 0`: only then does ptxas know a single thread is active and emit the
-    // UTMALDG / UTCHMMA / UTCBAR once instead of inside a per-thread BRA.U.ANY serialisation loop (~80 cycles per MMA)
+    // ================================================================ TMA producer (one elected lane issues; the warp stays converged)
     int stage = 0;
     uint32_t phase = 0;
     for (int w = group; w < total_work; w += num_groups) {
@@ -332,21 +333,21 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
       const int n_blk = t2 / p.num_m_groups;
       const int kb0 = split * p.k_blocks_per_split;
       const int kb1 = min(kb0 + p.k_blocks_per_split, p.num_k_blocks);
-      // loads of one (real) k-block from the given tensor maps. Single-pass launches call it with the kernel's own
-      // __grid_constant__ maps (compile-time parameter addresses, as in round 1); split precision selects hi / lo maps per pass.
+      // loads of one (real) k-block from the given tensor maps; split precision selects hi / lo maps per pass
       auto issue_loads = [&](const CUtensorMap* tma_a, const CUtensorMap* tma_b, int kb) {
+        // in a pair this stage of BOTH CTAs is free: each consumer warp arrives on its own and on the peer's empty barrier
         mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
         const uint32_t sa = smem_u32(smem_tiles + stage * Cfg::STAGE_BYTES);
         const uint32_t sb = sa + Cfg::A_BYTES;
-        if constexpr (!pair) {
-          const uint32_t fb = smem_u32(&full_bar[stage]);
-          mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
-          if (p.a_mn) {
+        const uint32_t fb = smem_u32(&full_bar[stage]);
+        mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);   // a pair's B bytes arrive half from this CTA, half from the peer
+        if (p.a_mn) {
 #pragma unroll
-            for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * (BK * 128), tma_a, m_blk * BM + j * 64, kb * BK, fb);
-          } else {
-            tma_load_2d(sa, tma_a, kb * BK, m_blk * BM, fb);
-          }
+          for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * (BK * 128), tma_a, m_blk * BM + j * 64, kb * BK, fb);
+        } else {
+          tma_load_2d(sa, tma_a, kb * BK, m_blk * BM, fb);
+        }
+        if constexpr (!pair) {
           if (p.b_mn) {
 #pragma unroll
             for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * (BK * 128), tma_b, n_blk * BN + j * 64, kb * BK, fb);
@@ -354,22 +355,14 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
             tma_load_2d(sb, tma_b, kb * BK, n_blk * BN, fb);
           }
         } else {
-          // both CTAs complete their bytes on the LEADER's full barrier (the leader issues the MMAs for the pair);
-          // this CTA stages its 128 rows of A and columns [crank * BN/2, +BN/2) of the B tile
-          const uint32_t fb = mapa_shared(smem_u32(&full_bar[stage]), 0);
-          if (leader) mbar_arrive_expect_tx(smem_u32(&full_bar[stage]), 2 * Cfg::STAGE_BYTES);
-          if (p.a_mn) {
+          if (p.b_mn) {   // 64-column boxes [crank * BN/128, +BN/128) of the tile
 #pragma unroll
-            for (int j = 0; j < BM / 64; ++j) tma_load_2d_pair(sa + j * (BK * 128), tma_a, m_blk * BM + j * 64, kb * BK, fb);
-          } else {
-            tma_load_2d_pair(sa, tma_a, kb * BK, m_blk * BM, fb);
-          }
-          const int n0 = n_blk * BN + crank * (BN / 2);
-          if (p.b_mn) {
-#pragma unroll
-            for (int j = 0; j < BN / 128; ++j) tma_load_2d_pair(sb + j * (BK * 128), tma_b, n0 + j * 64, kb * BK, fb);
-          } else {
-            tma_load_2d_pair(sb, tma_b, kb * BK, n0, fb);   // tensor-map box = BN/2 rows
+            for (int j = 0; j < BN / 128; ++j) {
+              const int jj = crank * (BN / 128) + j;
+              tma_load_2d_multicast(sb + jj * (BK * 128), tma_b, n_blk * BN + jj * 64, kb * BK, fb, 0x3);
+            }
+          } else {        // rows [crank * BN/2, +BN/2) of the tile (tensor-map box = BN/2 rows)
+            tma_load_2d_multicast(sb + crank * (BN / 2) * 128, tma_b, kb * BK, n_blk * BN + crank * (BN / 2), fb, 0x3);
           }
         }
       };
@@ -389,159 +382,114 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp_idx == 1) {
-    // ================================================================ MMA issuer (one elected lane issues; the warp stays converged)
+  } else if (warp_idx >= 4) {
+    // ================================================================ consumers (warps 4..11 = warpgroups 1, 2)
+    const int cw = warp_idx - 4;
+    const int wg = cw >> 2;                 // rows [64 wg, +64) of the tile
+    float* stg = staging + cw * (EPI_ROWS * 32);
+    const int rr = lane >> 3;               // row within a 4-row group of the coalesced pass
+    const int cc = (lane & 7) * 4;          // first of 4 columns handled by this lane
+    // 64 rows of A start 8 KB into the stage in both majors (K-major: 64 rows x 128 B; MN-major: the second 64-wide box)
+    const uint32_t a_off = wg * (64 * 128);
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(smem_u32(&empty_bar[s]));
+        if constexpr (pair) mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[s]), (uint32_t)(crank ^ 1)));
+      }
+    };
+    float acc[NACC][64];
     int stage = 0;
     uint32_t phase = 0;
-    int it = 0;
-    for (int w = group; w < total_work && leader; w += num_groups, ++it) {   // in a pair only the leader issues
+    for (int w = group; w < total_work; w += num_groups) {
       const int split = w % p.split_k;
-      const int kb0 = split * p.k_blocks_per_split;
-      const int kb1 = min(kb0 + p.k_blocks_per_split, p.num_k_blocks);
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      const uint32_t tmem_d = tmem_base + as * BN;
-      if (elect_one()) {
-        mbar_wait(smem_u32(&tmem_empty_bar[as]), aphase ^ 1);
-        tc_fence_after();
-      }
-      __syncwarp();
-      for (int kb = kb0; kb < kb1; ++kb) {
-        if (elect_one()) {
-          mbar_wait(smem_u32(&full_bar[stage]), phase);
-          tc_fence_after();
-          if (kb == kb0 && w == group) VB_DBG(3);
-          const uint32_t sa = smem_u32(smem_tiles + stage * Cfg::STAGE_BYTES);
-          const uint32_t sb = sa + Cfg::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / UK; ++k) {
-            const uint64_t da = umma_desc_at(p.desc_base_a, sa + k * p.kadv_a);
-            const uint64_t db = umma_desc_at(p.desc_base_b, sb + k * p.kadv_b);
-            if constexpr (pair) umma_bf16_pair(tmem_d, da, db, p.idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            else                umma_bf16(tmem_d, da, db, p.idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          // smem slot free once these MMAs retire (in both CTAs of a pair)
-          if constexpr (pair) umma_commit_pair(smem_u32(&empty_bar[stage]), 0x3);
-          else                umma_commit(smem_u32(&empty_bar[stage]));
-        }
-        __syncwarp();
-        if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (elect_one()) {
-        if constexpr (pair) umma_commit_pair(smem_u32(&tmem_full_bar[as]), 0x3);   // accumulator complete (both halves)
-        else                umma_commit(smem_u32(&tmem_full_bar[as]));
-        if (w == group) VB_DBG(4);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ================================================================ epilogue (warps 2..9)
-    // Per 32-column chunk: (1) issue the global reads of this chunk (fp32 residual / bf16 GELU pre-activation) so their
-    // latency overlaps the TMEM read, (2) tcgen05.ld 32 lanes x 32 columns -> registers (thread = row), (3) 128-bit
-    // stores into a padded smem tile, (4) row-wise pass where a lane owns 4 consecutive columns of rows {rr, rr+4, ..}:
-    // 128-bit smem reads, fused math, 128-bit coalesced global stores.
-    const int lane_grp = warp_idx & 3;  // TMEM lanes [32*lane_grp, +32) are visible to this warp
-    float* stg = staging + (warp_idx - 2) * (32 * 32);
-    const int half = (warp_idx - 2) >> 2;   // the two warps of a lane quadrant take alternate 32-column chunks
-    const int rr = lane >> 3;           // row within a 4-row group of the coalesced pass
-    const int cc = (lane & 7) * 4;      // first of 4 columns handled by this lane
-    int it = 0;
-    for (int w = group; w < total_work; w += num_groups, ++it) {
       const int t2 = w / p.split_k;
       const int m_blk = (t2 % p.num_m_groups) * CG + crank;
       const int n_blk = t2 / p.num_m_groups;
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      const int m_base = m_blk * BM + lane_grp * 32;
-      const uint32_t taddr = tmem_base + (uint32_t(lane_grp * 32) << 16) + as * BN;
-      const bool rows_full = (m_base + 32 <= p.M);
-      const bool rows_live = (m_base < p.M);
-      bool waited = false;
-      constexpr int NC = BN / 32;
-      // software pipeline over chunk pairs: the global operands of chunk c+1 are in flight while chunk c is processed
-      float4 res0[8], res1[8];
-      uint2 aux0[8], aux1[8];
-      float4 bia0, bia1;
-      auto chunk_fast = [&](int c) -> bool {
-        return (EPI != EPI_GENERIC) && p.fast_ok && rows_full && (n_blk * BN + c * 32 + 32 <= p.N);
-      };
-      auto prefetch = [&](int c, float4 (&resv)[8], uint2 (&auxv)[8], float4& b4) {
-        b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (c >= NC || !rows_live || !chunk_fast(c)) return;
-        const int n = n_blk * BN + c * 32 + cc;
-        if (EPI == EPI_F32 && p.residual) {
-#pragma unroll
-          for (int ps = 0; ps < 8; ++ps) {
-            const float* src = p.residual + (long long)(m_base + ps * 4 + rr) * p.ld_res + n;
-            if (p.vec_res) resv[ps] = *reinterpret_cast<const float4*>(src);
-            else resv[ps] = make_float4(src[0], src[1], src[2], src[3]);
-          }
+      const int kb0 = split * p.k_blocks_per_split;
+      const int kb1 = min(kb0 + p.k_blocks_per_split, p.num_k_blocks);
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(smem_u32(&full_bar[stage]), phase);
+        if (kb == kb0 && w == group && threadIdx.x == 128) VB_DBG(3);
+        const uint32_t sa = smem_u32(smem_tiles + stage * Cfg::STAGE_BYTES) + a_off;
+        const uint32_t sb = smem_u32(smem_tiles + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+        const bool accum = kb > kb0;
+        switch (p.mma_kind) {
+          case 0: mma_kblock<NACC, 0, 0, 0>(acc, sa, sb, p, accum); break;
+          case 1: mma_kblock<NACC, 0, 0, 1>(acc, sa, sb, p, accum); break;
+          case 2: mma_kblock<NACC, 0, 1, 0>(acc, sa, sb, p, accum); break;
+          case 3: mma_kblock<NACC, 0, 1, 1>(acc, sa, sb, p, accum); break;
+          case 4: mma_kblock<NACC, 1, 0, 0>(acc, sa, sb, p, accum); break;
+          case 5: mma_kblock<NACC, 1, 0, 1>(acc, sa, sb, p, accum); break;
+          case 6: mma_kblock<NACC, 1, 1, 0>(acc, sa, sb, p, accum); break;
+          default: mma_kblock<NACC, 1, 1, 1>(acc, sa, sb, p, accum); break;
         }
-        if (EPI == EPI_DGELU) {
-#pragma unroll
-          for (int ps = 0; ps < 8; ++ps)
-            auxv[ps] = *reinterpret_cast<const uint2*>(p.aux + (long long)(m_base + ps * 4 + rr) * p.ld_aux + n);
-        }
-        if (p.bias) b4 = *reinterpret_cast<const float4*>(p.bias + n);
-      };
-      auto process = [&](int c, const float4 (&resv)[8], const uint2 (&auxv)[8], const float4 b4) {
-        const int n_chunk = n_blk * BN + c * 32;
-        const bool chunk_live = (n_chunk < p.N) && rows_live;  // warp-uniform
-        if (!waited) {
-          mbar_wait(smem_u32(&tmem_full_bar[as]), aphase);
-          tc_fence_after();
-          waited = true;
-          if (w == group && warp_idx == 2 && lane == 0) VB_DBG(5);
-        }
-        // TMEM -> registers -> padded smem tile (row = lane)
-        if (chunk_live) {
-          uint32_t r[32];
-          tmem_ld_32x32(taddr + c * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<uint4*>(stg + stg_off(lane, j * 4)) = make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-        }
-        if (c == NC - 2 + half) {
-          // every TMEM read this warp makes of the accumulator stage has landed in registers
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if constexpr (pair) mbar_arrive_cluster(mapa_shared(smem_u32(&tmem_empty_bar[as]), 0));   // the leader's MMA warp waits for both CTAs
-            else                mbar_arrive(smem_u32(&tmem_empty_bar[as]));
-          }
-        }
-        if (!chunk_live) return;
-        __syncwarp();
-        // coalesced row pass
-        if (EPI == EPI_F32 && p.act == VB_ACT_RELU && chunk_fast(c)) epi_pool_chunk(p, stg, m_base, n_chunk + cc, rr, cc, b4);
-        else if (chunk_fast(c)) epi_fast_chunk<EPI, OUT16>(p, stg, m_base, n_chunk + cc, rr, cc, resv, auxv, b4);
-        else               epi_generic_chunk(p, stg, m_base, n_chunk + cc, rr, cc);
-        __syncwarp();
-      };
-      prefetch(half, res0, aux0, bia0);
-#pragma unroll 1
-      for (int c = half; c < NC; c += 4) {
-        prefetch(c + 2, res1, aux1, bia1);
-        process(c, res0, aux0, bia0);
-        prefetch(c + 4, res0, aux0, bia0);
-        process(c + 2, res1, aux1, bia1);
+        // the group of the previous k-block has retired: its stage may be refilled
+        wgmma_wait<1>();
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
       }
-      if (w == group && warp_idx == 2 && lane == 0) VB_DBG(6);
+      wgmma_wait<0>();
+#pragma unroll
+      for (int j = 0; j < NACC; ++j)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) reg_fence(acc[j][i]);
+      if (prev >= 0) release(prev);
+      if (w == group && threadIdx.x == 128) VB_DBG(5);
+
+      // ---- epilogue of the warp's 16 rows, 32 columns at a time
+      const int m_base = m_blk * BM + wg * 64 + (cw & 3) * EPI_ROWS;
+      const bool rows_full = (m_base + EPI_ROWS <= p.M);
+      if (m_base < p.M) {
+        constexpr int NC = BN / 32;
+#pragma unroll 1
+        for (int c = 0; c < NC; ++c) {
+          const int n_chunk = n_blk * BN + c * 32;
+          if (n_chunk >= p.N) break;   // warp-uniform
+          const bool fast = (EPI != EPI_GENERIC) && p.fast_ok && rows_full && (n_chunk + 32 <= p.N);
+          const int n = n_chunk + cc;
+          // global operands of the chunk first, so that their latency overlaps the staging
+          float4 resv[EPI_PS];
+          uint2 auxv[EPI_PS];
+          float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (fast) {
+            if (EPI == EPI_F32 && p.residual) {
+#pragma unroll
+              for (int ps = 0; ps < EPI_PS; ++ps) {
+                const float* src = p.residual + (long long)(m_base + ps * 4 + rr) * p.ld_res + n;
+                if (p.vec_res) resv[ps] = *reinterpret_cast<const float4*>(src);
+                else resv[ps] = make_float4(src[0], src[1], src[2], src[3]);
+              }
+            }
+            if (EPI == EPI_DGELU) {
+#pragma unroll
+              for (int ps = 0; ps < EPI_PS; ++ps)
+                auxv[ps] = *reinterpret_cast<const uint2*>(p.aux + (long long)(m_base + ps * 4 + rr) * p.ld_aux + n);
+            }
+            if (p.bias) b4 = *reinterpret_cast<const float4*>(p.bias + n);
+          }
+          // registers -> staging tile: the accumulator half and its 32-column quarter must be compile-time indices
+#pragma unroll
+          for (int c2 = 0; c2 < NC; ++c2)
+            if (c2 == c) stage_chunk(acc[c2 >> 2], c2 & 3, stg, lane);
+          __syncwarp();
+          if (EPI == EPI_F32 && p.act == VB_ACT_RELU && fast) epi_pool_chunk(p, stg, m_base, n, rr, cc, b4);
+          else if (fast) epi_fast_chunk<EPI, OUT16>(p, stg, m_base, n, rr, cc, resv, auxv, b4);
+          else           epi_generic_chunk(p, stg, m_base, n, rr, cc);
+          __syncwarp();
+        }
+      }
+      if (w == group && threadIdx.x == 128) VB_DBG(6);
     }
   }
 
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  // the peer may still arrive on this CTA's barriers / the leader's MMAs may still write the peer's TMEM until both are done
+  // a pair's peer may still multicast into this CTA's stages / arrive on its barriers until both are done
   if constexpr (pair) cluster_sync_all();
   if (threadIdx.x == 0) { VB_DBG(7); VB_DBG_NS(9); }
-  if (warp_idx == 1) {
-    tc_fence_after();
-    if constexpr (pair) tmem_dealloc_pair(tmem_base, Cfg::TMEM_COLS);
-    else                tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
+#undef VB_DBG
+#undef VB_DBG_NS
 }
 
 // ------------------------------------------------------------------------------------------ host
@@ -581,8 +529,8 @@ static int make_tmap(CUtensorMap* tm, const void* ptr, uint64_t inner, uint64_t 
 template <int BN, int EPI, int CG, int OUT16 = 0>
 static int launch_gemm(const CUtensorMap* tm, GemmKernelParams& p, long long total_work, int max_ctas,
                        cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, CG>;
-  auto kern = gemm_tcgen05_kernel<BN, EPI, CG, OUT16>;
+  using Cfg = GemmCfg<BN>;
+  auto kern = gemm_wgmma_kernel<BN, EPI, CG, OUT16>;
   static bool attr_set = false;  // per template instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
@@ -590,13 +538,13 @@ static int launch_gemm(const CUtensorMap* tm, GemmKernelParams& p, long long tot
     attr_set = true;
   }
   // persistent grid: one CTA per SM; with clusters, as many clusters as the device can keep resident at once (a GPC
-  // with an odd number of free SMs cannot host a pair there) so that no cluster waits for a second wave
+  // with an odd number of SMs cannot host a pair on all of them) so that no cluster waits for a second wave
   int groups_cap = max_ctas;
   if (CG > 1) {
     static int max_clusters = -1;   // per template instantiation; cluster size is 2 whenever it is not 1
     if (max_clusters < 0) {
       cudaLaunchConfig_t cfg{};
-      cfg.gridDim = dim3(2 * 148); cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+      cfg.gridDim = dim3(2 * sm_count()); cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
       cudaLaunchAttribute at[1];
       at[0].id = cudaLaunchAttributeClusterDimension;
       at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
@@ -648,30 +596,16 @@ static int default_cluster() {
   return v;
 }
 
-// Modelled fixed cost of running a problem as CTA pairs. In isolation a pair launch costs only ~600 cycles more (cluster
-// sync, leader-only issue), but inside the two-stream step a pair needs both SMs of a TPC free at once while kernels of the
-// other stream hold SMs: sweeping this constant on the full training step (profiles/r01_bench_v15_pair_penalty_sweep.txt:
-// 600 -> 11.24 ms, 2500 -> 11.15, 6000 -> 11.07, 10000 -> 11.11, 16000 -> 11.17, 30000 -> 11.18) puts the optimum at ~6000,
-// i.e. pairs only where they save at least ~3 us.
-static long long pair_penalty() {
-  static long long v = -1;
-  if (v < 0) {
-    const char* e = getenv("VB_GEMM_PAIR_PENALTY");   // cycles; development override
-    v = e ? atoll(e) : 6000;
-  }
-  return v;
-}
-
 // Chooses (tile width, CTAs per tile group, k splits) for a problem; honours the values the caller fixed. Pure host code.
 static int choose_config(const vb_gemm_args* a, int max_ctas, int* bn_out, int* cluster_out, int* split_out) {
   const int num_m = (a->M + BM - 1) / BM;
   const int num_k = (a->K + BK - 1) / BK * (1 + (a->A_lo ? 1 : 0) + (a->B_lo ? 1 : 0));   // virtual k-blocks (split precision passes)
   // Tile configuration = (tile width bn, CTAs per tile group cg, k splits): minimise the modelled time of the busiest CTA,
-  // in SM cycles, with constants measured on B200 (clock64 timelines / feed probes in profiles/):
-  //   main loop per 64-deep k-block: 128x128 ~430 (bound by the SM's operand ingest, ~98 B/clk of TMA writes competing with
-  //   the tensor core's smem reads), 128x256 ~650 (L2 -> SM bandwidth with all SMs pulling), CTA pair 256x128 ~400,
-  //   CTA pair 256x256 ~505 (= the tcgen05 floor); the epilogue of a tile overlaps the next tile's main loop, the last one
-  //   is exposed; ~3k cycles of prologue + first-load latency per launch.
+  // in SM cycles. The constants are estimates, not measurements: a 64-deep k-block of a 128 x 128 tile is 2.1 MFLOP, ~512
+  // cycles at the dense BF16 / FP16 rate of an H100 SM (4096 FLOP per cycle), plus ~10 % for barrier waits and wgmma issue
+  // (128 x 256: twice that); the epilogue of a tile follows its main loop (the accumulators live in the consumers' registers)
+  // while the producer already loads the next tile; ~3k cycles of prologue + first-load latency per launch. CTA pairs only
+  // save L2 -> SM traffic of B, which this model does not charge, so they are used when the caller asks for them.
   if (a->block_n != 0 && a->block_n != 128 && a->block_n != 256) return set_error(VB_ERR_INVALID, "vb_gemm_bf16: block_n must be 0, 128 or 256");
   int cluster_req = a->cluster_m ? a->cluster_m : default_cluster();
   if (cluster_req != 0 && cluster_req != 1 && cluster_req != 2) return set_error(VB_ERR_INVALID, "vb_gemm_bf16: cluster_m must be 0, 1 or 2");
@@ -691,9 +625,10 @@ static int choose_config(const vb_gemm_args* a, int max_ctas, int* bn_out, int* 
       if (a->block_n && a->block_n != w) continue;
       if (!a->block_n && w == 256 && a->N <= 128) continue;
       for (int cg = 1; cg <= 2; ++cg) {
-        if (cluster_req && cluster_req != cg && !(cluster_req == 2 && cg == 1 && (num_m < 2 || max_ctas < 2))) continue;
+        if (cluster_req != 2 && cg == 2) continue;
+        if (cluster_req == 2 && cg == 1 && num_m >= 2 && max_ctas >= 2) continue;
         if (cg == 2 && (num_m < 2 || max_ctas < 2)) continue;
-        const long long t_kb = (w == 128) ? (cg == 1 ? 430 : 400) : (cg == 1 ? 650 : 505);
+        const long long t_kb = (w == 128) ? 560 : 1100;
         const long long epi = epi_base * (w / 128);
         const long long groups = (cg == 1) ? max_ctas : max_ctas / 2;
         const long long tiles = (long long)((num_m + cg - 1) / cg) * ((a->N + w - 1) / w);
@@ -706,7 +641,7 @@ static int choose_config(const vb_gemm_args* a, int max_ctas, int* bn_out, int* 
           sp = (int)((num_k + kps_ - 1) / kps_);   // no empty splits
           const long long rounds = (tiles * sp + groups - 1) / groups;
           const long long ml = kps_ * t_kb;
-          const long long c = 3000 + (cg == 2 ? pair_penalty() : 0) + rounds * (ml > epi ? ml : epi) + epi;
+          const long long c = 3000 + rounds * (ml + epi);
           if (best < 0 || c < best) { best = c; bn = w; cluster = cg; split_k = sp; }
         }
       }
@@ -737,10 +672,10 @@ extern "C" vb_status vb_gemm_bf16(const vb_gemm_args* a, void* stream_) {
     return set_error(VB_ERR_INVALID, "vb_gemm_bf16: A_lo / B_lo must be 16-byte aligned");
   if ((a->out_lo || a->out_b16) && !a->out_bf16) return set_error(VB_ERR_INVALID, "vb_gemm_bf16: out_lo / out_b16 need out_bf16");
   if ((a->a_fp16 != 0) != (a->b_fp16 != 0))
-    return set_error(VB_ERR_UNSUPPORTED, "vb_gemm_bf16: A and B must have the same 16-bit format (fp16 x bf16 faults on sm_100)");
+    return set_error(VB_ERR_UNSUPPORTED, "vb_gemm_bf16: A and B must have the same 16-bit format (wgmma takes one operand type for both)");
   int dev_sms = 0, cc = 0;
   if (int s = vb_device_info(&dev_sms, &cc)) return s;
-  if (cc / 10 != 10) return set_error(VB_ERR_UNSUPPORTED, "vb_gemm_bf16: needs an sm_100 device (found sm_%d)", cc);
+  if (cc != 90) return set_error(VB_ERR_UNSUPPORTED, "vb_gemm_bf16: needs an sm_90 device (found sm_%d)", cc);
 
   const int num_m = (a->M + BM - 1) / BM;
   const int real_k = (a->K + BK - 1) / BK;
@@ -786,11 +721,9 @@ extern "C" vb_status vb_gemm_bf16(const vb_gemm_args* a, void* stream_) {
   const uint32_t sbo_a = a->dbg_sbo_a ? a->dbg_sbo_a : 1024;
   const uint32_t lbo_b = a->dbg_lbo_b ? a->dbg_lbo_b : (a->b_mn_major ? BK * 128 : 16);
   const uint32_t sbo_b = a->dbg_sbo_b ? a->dbg_sbo_b : 1024;
-  p.desc_base_a = umma_desc_base(lbo_a, sbo_a);
-  p.desc_base_b = umma_desc_base(lbo_b, sbo_b);
-  p.kadv_a = a->a_mn_major ? 2 * 1024 : UK * 2;
-  p.kadv_b = a->b_mn_major ? 2 * 1024 : UK * 2;
-  p.idesc = umma_idesc_bf16(BM * cluster, bn, a->a_mn_major ? 1 : 0, a->b_mn_major ? 1 : 0, a->a_fp16, a->b_fp16);   // pairs: 256 x bn MMAs
+  p.desc_base_a = gmma_desc_base(lbo_a, sbo_a);
+  p.desc_base_b = gmma_desc_base(lbo_b, sbo_b);
+  p.mma_kind = (a->b_mn_major ? 1 : 0) | (a->a_mn_major ? 2 : 0) | (a->a_fp16 ? 4 : 0);
   p.dbg = reinterpret_cast<unsigned long long*>(a->dbg_timeline);
   p.a_mn = a->a_mn_major ? 1 : 0;
   p.b_mn = a->b_mn_major ? 1 : 0;
@@ -813,7 +746,7 @@ extern "C" vb_status vb_gemm_bf16(const vb_gemm_args* a, void* stream_) {
       else               st = make_tmap(&tm[i], ptr, (uint64_t)a->K, (uint64_t)a->M, (uint64_t)a->lda, BK, BM);
     } else {
       if (a->b_mn_major) st = make_tmap(&tm[i], ptr, (uint64_t)a->N, (uint64_t)a->K, (uint64_t)a->ldb, 64, BK);
-      else               st = make_tmap(&tm[i], ptr, (uint64_t)a->K, (uint64_t)a->N, (uint64_t)a->ldb, BK, (uint32_t)(bn / cluster));   // a pair CTA stages half the tile
+      else               st = make_tmap(&tm[i], ptr, (uint64_t)a->K, (uint64_t)a->N, (uint64_t)a->ldb, BK, (uint32_t)(bn / cluster));   // a pair CTA loads half the tile
     }
     if (st) return st;
   }

@@ -17,7 +17,7 @@ int sm_count();
 // Programmatic dependent launch (PDL): every kernel of the library starts with `griddepcontrol.wait` (all global
 // traffic happens after it) followed by `griddepcontrol.launch_dependents`, and is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization so that launch processing, CTA scheduling and per-CTA setup
-// (barrier init, TMEM allocation, tensor-map prefetch) of kernel N+1 overlap the tail of kernel N — also inside
+// (barrier init, tensor-map prefetch) of kernel N+1 overlap the tail of kernel N — also inside
 // captured CUDA graphs. VB_PDL=0 in the environment restores plain stream serialization.
 bool pdl_enabled();
 

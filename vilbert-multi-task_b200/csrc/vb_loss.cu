@@ -206,7 +206,7 @@ __global__ void scatter_rows_f32_kernel(const float4* __restrict__ src, float4* 
 
 static inline int loss_grid(int rows) {
   int cap = sm_count() * 8;
-  if (cap <= 0) cap = 148 * 8;
+  if (cap <= 0) cap = 132 * 8;
   return rows < cap ? (rows > 0 ? rows : 1) : cap;
 }
 
@@ -255,7 +255,7 @@ extern "C" vb_status vb_compact_rows(const int64_t* labels, int64_t ignore_index
 extern "C" vb_status vb_gather_rows16(const void* src, void* dst, const void* src2, void* dst2, const int32_t* idx, int32_t cap, int32_t cols,
                                       void* stream) {
   if (cap <= 0 || cols <= 0 || (cols & 7) || !src || !dst || !idx) return set_error(VB_ERR_INVALID, "vb_gather_rows16: bad arguments (cols % 8 == 0)");
-  int grid = sm_count() * 8; if (grid <= 0) grid = 148 * 8;
+  int grid = sm_count() * 8; if (grid <= 0) grid = 132 * 8;
   launch_pdl(gather_rows16_kernel, dim3(grid), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream), static_cast<const uint4*>(src),
              static_cast<uint4*>(dst), static_cast<const uint4*>(src2), static_cast<uint4*>(dst2), idx, (int)cap, (int)(cols / 8));
   return check_launch("vb_gather_rows16");
@@ -264,7 +264,7 @@ extern "C" vb_status vb_gather_rows16(const void* src, void* dst, const void* sr
 extern "C" vb_status vb_scatter_rows_f32(const float* src, float* dst, const int32_t* idx, int32_t cap, int32_t cols, const int32_t* count,
                                          float* poison, void* stream) {
   if (cap <= 0 || cols <= 0 || (cols & 3) || !src || !dst || !idx) return set_error(VB_ERR_INVALID, "vb_scatter_rows_f32: bad arguments (cols % 4 == 0)");
-  int grid = sm_count() * 8; if (grid <= 0) grid = 148 * 8;
+  int grid = sm_count() * 8; if (grid <= 0) grid = 132 * 8;
   launch_pdl(scatter_rows_f32_kernel, dim3(grid), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream), reinterpret_cast<const float4*>(src),
              reinterpret_cast<float4*>(dst), idx, (int)cap, (int)(cols / 4), count, poison);
   return check_launch("vb_scatter_rows_f32");

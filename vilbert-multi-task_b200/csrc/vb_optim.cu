@@ -100,7 +100,7 @@ extern "C" vb_status vb_adamw_step(float* p, float* g, float* m, float* v, void*
   if (!al(p, 16) || !al(g, 16) || !al(m, 16) || !al(v, 16) || (p16 && !al(p16, 8)) || (p16_lo && (!al(p16_lo, 8) || !p16)) || !al(p16_b, 8))
     return set_error(VB_ERR_INVALID, "vb_adamw_step: buffers must be 16-byte aligned (16-bit copies 8-byte)");
   int grid = sm_count() * 8;
-  if (grid <= 0) grid = 148 * 8;
+  if (grid <= 0) grid = 132 * 8;
   if (grid > n_chunks) grid = n_chunks;
   cudaError_t e = launch_pdl(adamw_kernel, dim3(grid), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
                              static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),

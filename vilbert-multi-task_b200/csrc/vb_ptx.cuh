@@ -1,5 +1,5 @@
-// sm_100a PTX wrappers used by the ViLBERT B200 kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / fences), ldmatrix + mma.sync for the attention tiles.
+// sm_90a PTX wrappers used by the ViLBERT kernels: mbarrier, TMA (cp.async.bulk.tensor, cluster multicast),
+// wgmma (warpgroup MMA from shared-memory descriptors), ldmatrix + mma.sync for the attention tiles.
 // Everything here is inline PTX; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda_runtime.h>
@@ -104,14 +104,14 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* tmap,
       : "memory");
 }
 
-// CTA-pair variant (tcgen05 cta_group::2): the box lands in this CTA's shared memory, the bytes complete on an mbarrier
-// given as a shared::cluster address (the pair leader's barrier, see mapa_shared).
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t smem_dst, const void* tmap, int c0, int c1,
-                                                 uint32_t cluster_bar) {
+// Multicast variant: the box lands at the same shared-memory offset in every CTA of `cta_mask`, and its bytes complete on the
+// mbarrier at the same offset in each of them.
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t smem_dst, const void* tmap, int c0, int c1, uint32_t bar,
+                                                      uint16_t cta_mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%2, %3}], [%4];"
-      ::"r"(smem_dst), "l"(tmap), "r"(c0), "r"(c1), "r"(cluster_bar)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%2, %3}], [%4], %5;"
+      ::"r"(smem_dst), "l"(tmap), "r"(c0), "r"(c1), "r"(bar), "h"(cta_mask)
       : "memory");
 }
 
@@ -136,117 +136,51 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// cta_group::2 allocation: the same warp index of both CTAs of the pair executes these with the same arguments.
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 inputs, fp32 accumulate (kind::f16).
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-// CTA pair (cta_group::2): issued by the leader CTA only; D is 256 x N, rows [0,128) in the leader's TMEM and rows
-// [128,256) in the peer's at the same TMEM address; each CTA holds its 128 rows of A and its N/2 rows of B at the same
-// shared-memory offsets.
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                               uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on the mbarrier at this shared-memory offset in every CTA of `cta_mask` once the pair's MMAs have completed.
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask)
-               : "memory");
-}
-// TMEM -> registers: 32 lanes x 32 consecutive fp32 columns (thread t gets lane base+t).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor (sm_100 "version 1"), SWIZZLE_128B layouts.
+// ---------------------------------------------------------------- wgmma (Hopper warpgroup MMA)
+// Shared-memory matrix descriptor of wgmma, SWIZZLE_128B layouts:
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-__host__ __device__ __forceinline__ uint64_t umma_desc_base(uint32_t lbo_bytes, uint32_t sbo_bytes) {
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout type (1 = SWIZZLE_128B)
+__host__ __device__ __forceinline__ uint64_t gmma_desc_base(uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-__device__ __forceinline__ uint64_t umma_desc_at(uint64_t base, uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t gmma_desc_at(uint64_t base, uint32_t smem_addr) {
   return base | (uint64_t)((smem_addr & 0x3FFFF) >> 4);
 }
-// Instruction descriptor for kind::f16: A and B independently fp16 (format 0) or bf16 (format 1), fp32 accumulate.
-__host__ __device__ __forceinline__ uint32_t umma_idesc_bf16(int M, int N, int a_mn_major,
-                                                             int b_mn_major, int a_fp16 = 0, int b_fp16 = 0) {
-  uint32_t d = 0;
-  d |= 1u << 4;                         // C format: F32
-  d |= (a_fp16 ? 0u : 1u) << 7;         // A format: F16 = 0, BF16 = 1
-  d |= (b_fp16 ? 0u : 1u) << 10;        // B format
-  d |= (uint32_t)(a_mn_major & 1) << 15;
-  d |= (uint32_t)(b_mn_major & 1) << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
-  return d;
+// Orders the register accesses of the warpgroup before the next wgmma.mma_async that reads / writes the same accumulators.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// Waits until at most N committed wgmma groups of this thread are still pending.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accesses of an accumulator register across wgmma_wait / wgmma_fence.
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128], both operands from shared memory (descriptors), fp32 accumulators in the registers
+// of the issuing warpgroup. F16: fp16 operands (else bf16; wgmma takes one format for both). TA / TB: operand stored MN-major.
+// Fragment of thread t (warp w = t / 32 of the warpgroup, lane l): d[4i + {0,1}] = D[16w + l/4][8i + 2(l%4) + {0,1}],
+// d[4i + {2,3}] = the same columns of row 16w + l/4 + 8.
+template <int F16, int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  if constexpr (F16) {
+      asm volatile(
+          "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+          "%64, %65, p, 1, 1, %67, %68;\n\t}\n"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+          : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB));
+  } else {
+      asm volatile(
+          "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+          "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+          "%64, %65, p, 1, 1, %67, %68;\n\t}\n"
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+          : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB));
+  }
 }
 
 // ---------------------------------------------------------------- warp-level MMA (attention tiles)

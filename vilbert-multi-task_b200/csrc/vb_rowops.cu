@@ -24,7 +24,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 static inline int row_grid(long long rows) {
   long long blocks = (rows + ROW_WARPS - 1) / ROW_WARPS;
   long long cap = (long long)sm_count() * 8;
-  if (cap <= 0) cap = 148 * 8;
+  if (cap <= 0) cap = 132 * 8;
   return (int)(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
 }
 
@@ -670,7 +670,7 @@ static inline DropCfg make_drop(const vb_dropout* d) {
 static inline int ew_grid(long long n, int threads = 256) {
   long long blocks = (n + threads - 1) / threads;
   long long cap = (long long)sm_count() * 8;
-  if (cap <= 0) cap = 148 * 8;
+  if (cap <= 0) cap = 132 * 8;
   return (int)(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
 }
 static inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }

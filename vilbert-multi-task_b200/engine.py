@@ -1,19 +1,19 @@
-"""Execution engine of the B200 ViLBERT hot path.
+"""Execution engine of the H100 ViLBERT hot path.
 
 Mirrors, operation for operation, what the reference's eager modules do in
 VILBertForVLTasks.forward -> BertModel.forward -> BertEncoder.forward (vilbert/vilbert.py:1638-1708,
 :1309-1406, :934-1107) and what autograd derives from them, but as a static *plan*: for a given
 (B, Nt, Nv) shape every activation buffer is allocated once and the forward and backward passes
-become flat lists of C-ABI calls into libvilbert_b200.so (tcgen05 GEMMs, fused attention, row-wise
+become flat lists of C-ABI calls into libvilbert_b200.so (wgmma GEMMs, fused attention, row-wise
 kernels). A plan can be replayed eagerly (a tight loop of ctypes calls) or captured into one CUDA
 graph per pass. PyTorch is used for device memory, streams and (optionally) graph capture only.
 
-Numerics (DESIGN.md §6). Accumulation is always fp32 (TMEM / registers); the residual stream, LayerNorm
+Numerics (DESIGN.md §6). Accumulation is always fp32 (registers); the residual stream, LayerNorm
 statistics and outputs, softmax statistics, biases and every gradient accumulation are fp32; 16-bit copies of
 activations and weights exist only as tensor-core operands. Three operand precisions (Engine(precision=...)):
   "fp16" (default)  forward operands (activations, weights) fp16 — 11 significant bits, the reference's own reduced
                     precision (model.half(), train_concap.py:504-505) — gradient operands (dy, dS, ...) bf16 for range.
-                    tcgen05 faults on fp16 x bf16 (measured), so every forward operand the backward contracts with a
+                    wgmma takes one operand type for both inputs, so every forward operand the backward contracts with a
                     gradient (weights for dgrad, saved activations for wgrad) also has a bf16 copy, written by the kernel
                     that produces it (Act.bw, ParamStore.shadow_b);
   "fp32"            split precision: every forward operand is stored as fp16 hi + lo and every forward contraction
@@ -1651,7 +1651,7 @@ class Engine:
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda" and not _build_only:
-            raise L.VBError("vilbert_b200 runs on sm_100a GPUs only; there is no CPU path (device=%s)" % device)
+            raise L.VBError("vilbert_b200 runs on sm_90a GPUs only; there is no CPU path (device=%s)" % device)
         L.lib()  # fail loudly now if the extension is missing
         self.ps = ParamStore(cfg, self.device, heads, self.op_dtype, self.split)
         self.two_streams = two_streams   # text / vision segments on two CUDA streams (parallel graph branches)

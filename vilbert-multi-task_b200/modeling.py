@@ -1,6 +1,6 @@
 """Drop-in module surface: BertModel, VILBertForVLTasks, BertForMultiModalPreTraining with the
 reference's constructor / forward signatures, output tuples and state_dict key names
-(vilbert/vilbert.py:1288-1406, :1435-1597, :1600-1708; SURVEY.md §8b), executing on the B200 engine
+(vilbert/vilbert.py:1288-1406, :1435-1597, :1600-1708; SURVEY.md §8b), executing on the H100 engine
 (engine.py -> libvilbert_b200.so). There is no PyTorch / CPU fallback: constructing a model on a
 non-CUDA device or without the built extension raises.
 """
@@ -153,7 +153,7 @@ class BertPreTrainedModel(nn.Module):
         precision = precision or os.environ.get("VILBERT_B200_PRECISION", "fp16")
         dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
         if dev.type != "cuda" or not torch.cuda.is_available():
-            raise L.VBError("vilbert_b200 models run on sm_100a GPUs only; there is no CPU path")
+            raise L.VBError("vilbert_b200 models run on sm_90a GPUs only; there is no CPU path")
         self.engine = Engine(config, dev, heads=self._heads, precision=precision)
         self._params = _register_tree(self, self.engine.ps)
         self._grad_hint = {}
