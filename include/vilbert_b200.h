@@ -349,6 +349,21 @@ vb_status vb_adamw_step(float* p, float* g, float* m, float* v, void* p16, void*
                         const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
                         const vb_adamw_group* groups, const int32_t* step, float grad_scale, int32_t zero_grad, void* stream);
 
+/* Fused multi-tensor RAdam on the same flat buffers, chunk table and group table (correct_bias is ignored): the reference's
+ * `--optim RAdam` (vilbert/optimization.py:16-100, built at train_tasks.py:427-428) + model.zero_grad() + the weight-copy cast:
+ *   v = b2 v + (1-b2) g^2;  m = b1 m + (1-b1) g;  p -= lr wd p   (own group's betas / lr / wd; decay FIRST, on the old p)
+ *   p -= step_size m / (sqrt(v) + eps)  if N_sma >= 5,  else  p -= step_size m
+ *   N_sma_max = 2/(1-b2) - 1,  N_sma = N_sma_max - 2t b2^t/(1-b2^t),  t = *step
+ *   step_size = lr sqrt((1-b2^t)(N_sma-4)/(N_sma_max-4)(N_sma-2)/N_sma N_sma_max/(N_sma_max-2)) / (1-b1^t)  (N_sma >= 5)
+ *             = lr / (1-b1^t)  otherwise
+ * N_sma and step_size are computed in float64 from the lr / b1 / b2 of groups[leader_group] and used for every tensor: the
+ * reference caches them per step in one buffer shared by all groups, so the first tensor's group supplies them.
+ * advance_step != 0: *step += 1 on `stream` first (one call = one capturable step). Other arguments as vb_adamw_step. */
+vb_status vb_radam_step(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                        const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
+                        const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step, float grad_scale,
+                        int32_t zero_grad, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

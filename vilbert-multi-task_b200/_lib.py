@@ -111,6 +111,7 @@ _SIGNATURES = {
     "vb_gather_rows16": [_P, _P, _P, _P, _P, _I32, _I32, _P],
     "vb_scatter_rows_f32": [_P, _P, _P, _I32, _I32, _P, _P, _P],
     "vb_adamw_step": [_P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _P, _F, _I32, _P],
+    "vb_radam_step": [_P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _I32, _P, _I32, _F, _I32, _P],
 }
 
 _lib = None

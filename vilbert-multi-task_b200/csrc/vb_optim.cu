@@ -1,4 +1,4 @@
-// vb_optim.cu — fused multi-tensor AdamW on the engine's flat buffers (SURVEY.md §8 f2).
+// vb_optim.cu — fused multi-tensor AdamW and RAdam on the engine's flat buffers (SURVEY.md §8 f2).
 //
 // Reference semantics: pytorch_transformers==1.0.0 AdamW as constructed at train_tasks.py:425-426
 // (AdamW(optimizer_grouped_parameters, lr=base_lr, correct_bias=False), one param group PER TENSOR with its own
@@ -22,6 +22,34 @@
 namespace vb {
 
 constexpr int OPT_THREADS = 256;
+
+// The 16-bit tensor-core operand copies of four updated weights at float4 index i of the chunk starting at s0: hi (and its
+// split-precision low part when p16_lo) in fp16 or bf16, and the always-bf16 backward copy when p16_b.
+__device__ __forceinline__ void store_copies4(uint16_t* __restrict__ p16, uint16_t* __restrict__ p16_lo, __nv_bfloat16* __restrict__ p16_b,
+                                              int fp16, long long s0, int i, float4 pv) {
+  if (p16) {
+    if (p16_lo) {
+      uint32_t l01, l23;
+      const uint32_t h01 = pack16_split(pv.x, pv.y, fp16, l01), h23 = pack16_split(pv.z, pv.w, fp16, l23);
+      reinterpret_cast<uint2*>(p16 + s0)[i] = make_uint2(h01, h23);
+      reinterpret_cast<uint2*>(p16_lo + s0)[i] = make_uint2(l01, l23);
+    } else {
+      reinterpret_cast<uint2*>(p16 + s0)[i] = make_uint2(pack16(pv.x, pv.y, fp16), pack16(pv.z, pv.w, fp16));
+    }
+  }
+  if (p16_b) reinterpret_cast<uint2*>(p16_b + s0)[i] = make_uint2(pack_bf16(pv.x, pv.y), pack_bf16(pv.z, pv.w));
+}
+
+// The same for one weight at flat element e (the ragged tail of a tensor).
+__device__ __forceinline__ void store_copies1(uint16_t* __restrict__ p16, uint16_t* __restrict__ p16_lo, __nv_bfloat16* __restrict__ p16_b,
+                                              int fp16, long long e, float pv) {
+  if (p16) {
+    const uint16_t hi = cvt16(pv, fp16);
+    p16[e] = hi;
+    if (p16_lo) p16_lo[e] = cvt16(pv - cvt16_to_f32(hi, fp16), fp16);
+  }
+  if (p16_b) p16_b[e] = __float2bfloat16(pv);
+}
 
 __global__ void __launch_bounds__(OPT_THREADS)
 adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
@@ -59,17 +87,7 @@ adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
       pv.z = upd(pv.z, gv.z, mv.z, vv.z); pv.w = upd(pv.w, gv.w, mv.w, vv.w);
       p4[i] = pv; m4[i] = mv; v4[i] = vv;
       if (zero_grad) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (p16) {
-        if (p16_lo) {
-          uint32_t l01, l23;
-          const uint32_t h01 = pack16_split(pv.x, pv.y, fp16, l01), h23 = pack16_split(pv.z, pv.w, fp16, l23);
-          reinterpret_cast<uint2*>(p16 + s0)[i] = make_uint2(h01, h23);
-          reinterpret_cast<uint2*>(p16_lo + s0)[i] = make_uint2(l01, l23);
-        } else {
-          reinterpret_cast<uint2*>(p16 + s0)[i] = make_uint2(pack16(pv.x, pv.y, fp16), pack16(pv.z, pv.w, fp16));
-        }
-      }
-      if (p16_b) reinterpret_cast<uint2*>(p16_b + s0)[i] = make_uint2(pack_bf16(pv.x, pv.y), pack_bf16(pv.z, pv.w));
+      store_copies4(p16, p16_lo, p16_b, fp16, s0, i, pv);
     }
     for (int i = (n4 << 2) + threadIdx.x; i < n; i += OPT_THREADS) {   // ragged tail of a tensor (e.g. a 3129-entry bias)
       const long long e = s0 + i;
@@ -77,14 +95,95 @@ adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
       const float pv = upd(p[e], g[e], mv, vv);
       p[e] = pv; m[e] = mv; v[e] = vv;
       if (zero_grad) g[e] = 0.f;
-      if (p16) {
-        const uint16_t hi = cvt16(pv, fp16);
-        p16[e] = hi;
-        if (p16_lo) p16_lo[e] = cvt16(pv - cvt16_to_f32(hi, fp16), fp16);
-      }
-      if (p16_b) p16_b[e] = __float2bfloat16(pv);
+      store_copies1(p16, p16_lo, p16_b, fp16, e, pv);
     }
   }
+}
+
+// RAdam as vilbert/optimization.py:16-100 defines it (the reference's `--optim RAdam`, train_tasks.py:427-428), per element:
+//     v = b2 v + (1 - b2) g g;  m = b1 m + (1 - b1) g;  p -= wd lr p   (own group's betas, lr, wd; decay FIRST, on the old p)
+//     p -= step_size m / (sqrt(v) + eps)   if N_sma >= 5,   else   p -= step_size m
+// with, at step t,  N_sma_max = 2 / (1 - b2) - 1,  N_sma = N_sma_max - 2 t b2^t / (1 - b2^t)  and
+//     step_size = lr sqrt((1 - b2^t) (N_sma - 4) / (N_sma_max - 4) (N_sma - 2) / N_sma N_sma_max / (N_sma_max - 2)) / (1 - b1^t)
+//     (N_sma >= 5),  lr / (1 - b1^t) otherwise.
+// The reference caches (N_sma, step_size) per step in one buffer shared by all param groups (optimization.py:59-86), so
+// within a step every tensor uses the values computed from the FIRST tensor's group: the lr, b1 and b2 of the leader group
+// `leader` drive the rectified step of all tensors. Both scalars are computed in float64 like the reference's Python floats:
+// in fp32, 1 - b2^t cancels (at b2 = 0.999 N_sma(6) comes out 6.0005 instead of 5.994).
+__global__ void __launch_bounds__(OPT_THREADS)
+radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+             uint16_t* __restrict__ p16, uint16_t* __restrict__ p16_lo, __nv_bfloat16* __restrict__ p16_b, int fp16,
+             const long long* __restrict__ chunk_start, const int* __restrict__ chunk_count, const int* __restrict__ chunk_group,
+             int n_chunks, const vb_adamw_group* __restrict__ groups, int leader, const int* __restrict__ step, float grad_scale,
+             int zero_grad) {
+  __shared__ float s_step_size;
+  __shared__ int s_rect;
+  pdl_entry();
+  if (threadIdx.x == 0) {
+    const vb_adamw_group L = groups[leader];
+    const double t = (double)max(*step, 1);   // the counter is advanced before the first step; 0 would divide by zero
+    const double b1 = L.beta1, b2 = L.beta2, lr = L.lr;
+    const double b2t = pow(b2, t);
+    const double n_max = 2.0 / (1.0 - b2) - 1.0;
+    const double n_sma = n_max - 2.0 * t * b2t / (1.0 - b2t);
+    const int rect = n_sma >= 5.0;
+    const double ss = rect ? lr * sqrt((1.0 - b2t) * (n_sma - 4.0) / (n_max - 4.0) * (n_sma - 2.0) / n_sma * n_max / (n_max - 2.0)) / (1.0 - pow(b1, t))
+                           : lr / (1.0 - pow(b1, t));
+    s_step_size = (float)ss;
+    s_rect = rect;
+  }
+  __syncthreads();
+  const float step_size = s_step_size;
+  const bool rect = s_rect != 0;
+  for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
+    const long long s0 = chunk_start[c];
+    const int n = chunk_count[c];
+    const vb_adamw_group G = groups[chunk_group[c]];
+    const float decay = G.weight_decay * G.lr;
+    const float ob1 = 1.f - G.beta1, ob2 = 1.f - G.beta2;
+    auto upd = [&](float pv, float gv, float& mv, float& vv) -> float {
+      gv *= grad_scale;
+      vv = G.beta2 * vv + ob2 * gv * gv;
+      mv = G.beta1 * mv + ob1 * gv;
+      if (G.weight_decay != 0.f) pv = pv - decay * pv;
+      return rect ? pv - step_size * (mv / (sqrtf(vv) + G.eps)) : pv - step_size * mv;
+    };
+    const int n4 = n >> 2;
+    float4* p4 = reinterpret_cast<float4*>(p + s0);
+    float4* g4 = reinterpret_cast<float4*>(g + s0);
+    float4* m4 = reinterpret_cast<float4*>(m + s0);
+    float4* v4 = reinterpret_cast<float4*>(v + s0);
+    for (int i = threadIdx.x; i < n4; i += OPT_THREADS) {
+      float4 pv = p4[i], mv = m4[i], vv = v4[i];
+      const float4 gv = g4[i];
+      pv.x = upd(pv.x, gv.x, mv.x, vv.x); pv.y = upd(pv.y, gv.y, mv.y, vv.y);
+      pv.z = upd(pv.z, gv.z, mv.z, vv.z); pv.w = upd(pv.w, gv.w, mv.w, vv.w);
+      p4[i] = pv; m4[i] = mv; v4[i] = vv;
+      if (zero_grad) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      store_copies4(p16, p16_lo, p16_b, fp16, s0, i, pv);
+    }
+    for (int i = (n4 << 2) + threadIdx.x; i < n; i += OPT_THREADS) {
+      const long long e = s0 + i;
+      float mv = m[e], vv = v[e];
+      const float pv = upd(p[e], g[e], mv, vv);
+      p[e] = pv; m[e] = mv; v[e] = vv;
+      if (zero_grad) g[e] = 0.f;
+      store_copies1(p16, p16_lo, p16_b, fp16, e, pv);
+    }
+  }
+}
+
+// Grid of the optimizer kernels: up to 8 CTAs per SM, never more CTAs than chunks.
+static int opt_grid(int n_chunks) {
+  int grid = sm_count() * 8;
+  if (grid <= 0) grid = 132 * 8;
+  return grid > n_chunks ? n_chunks : grid;
+}
+
+static bool opt_buffers_aligned(const void* p, const void* g, const void* m, const void* v, const void* p16, const void* p16_lo,
+                                const void* p16_b) {
+  auto al = [](const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q) % a) == 0; };
+  return al(p, 16) && al(g, 16) && al(m, 16) && al(v, 16) && (!p16 || al(p16, 8)) && (!p16_lo || (al(p16_lo, 8) && p16)) && al(p16_b, 8);
 }
 
 }  // namespace vb
@@ -96,16 +195,35 @@ extern "C" vb_status vb_adamw_step(float* p, float* g, float* m, float* v, void*
   if (n_chunks <= 0) return VB_OK;
   if (!p || !g || !m || !v || !chunk_start || !chunk_count || !chunk_group || !groups)
     return set_error(VB_ERR_INVALID, "vb_adamw_step: null argument");
-  auto al = [](const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q) % a) == 0; };
-  if (!al(p, 16) || !al(g, 16) || !al(m, 16) || !al(v, 16) || (p16 && !al(p16, 8)) || (p16_lo && (!al(p16_lo, 8) || !p16)) || !al(p16_b, 8))
+  if (!opt_buffers_aligned(p, g, m, v, p16, p16_lo, p16_b))
     return set_error(VB_ERR_INVALID, "vb_adamw_step: buffers must be 16-byte aligned (16-bit copies 8-byte)");
-  int grid = sm_count() * 8;
-  if (grid <= 0) grid = 132 * 8;
-  if (grid > n_chunks) grid = n_chunks;
-  cudaError_t e = launch_pdl(adamw_kernel, dim3(grid), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
+  cudaError_t e = launch_pdl(adamw_kernel, dim3(opt_grid(n_chunks)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
                              static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),
                              reinterpret_cast<const long long*>(chunk_start), chunk_count, chunk_group, (int)n_chunks, groups, step,
                              grad_scale, (int)(zero_grad ? 1 : 0));
   if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_adamw_step: %s", cudaGetErrorString(e));
+  return VB_OK;
+}
+
+extern "C" vb_status vb_radam_step(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                   const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
+                                   const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step, float grad_scale,
+                                   int32_t zero_grad, void* stream) {
+  using namespace vb;
+  if (!step || leader_group < 0) return set_error(VB_ERR_INVALID, "vb_radam_step: null step counter or negative leader group");
+  if (advance_step) {
+    const vb_status st = vb_step_counter_bump(reinterpret_cast<uint32_t*>(step), stream);
+    if (st != VB_OK) return st;
+  }
+  if (n_chunks <= 0) return VB_OK;
+  if (!p || !g || !m || !v || !chunk_start || !chunk_count || !chunk_group || !groups)
+    return set_error(VB_ERR_INVALID, "vb_radam_step: null argument");
+  if (!opt_buffers_aligned(p, g, m, v, p16, p16_lo, p16_b))
+    return set_error(VB_ERR_INVALID, "vb_radam_step: buffers must be 16-byte aligned (16-bit copies 8-byte)");
+  cudaError_t e = launch_pdl(radam_kernel, dim3(opt_grid(n_chunks)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
+                             static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),
+                             reinterpret_cast<const long long*>(chunk_start), chunk_count, chunk_group, (int)n_chunks, groups, (int)leader_group,
+                             static_cast<const int*>(step), grad_scale, (int)(zero_grad ? 1 : 0));
+  if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_radam_step: %s", cudaGetErrorString(e));
   return VB_OK;
 }

@@ -1,16 +1,18 @@
-"""Fused multi-tensor AdamW on the engine's flat parameter / gradient buffers (SURVEY.md §8 f2).
+"""Fused multi-tensor AdamW and RAdam on the engine's flat parameter / gradient buffers (SURVEY.md §8 f2).
 
-Drop-in for the optimizer the reference builds at train_tasks.py:401-426:
+Drop-ins for the two optimizers the reference's training driver offers (train_tasks.py:401-428, `--optim`):
 
     optimizer = AdamW(optimizer_grouped_parameters, lr=base_lr, correct_bias=False)        # pytorch_transformers 1.0.0
  -> optimizer = FusedAdamW(optimizer_grouped_parameters, lr=base_lr, correct_bias=False, model=model)
 
-Same constructor arguments and defaults (lr 1e-3, betas (0.9, 0.999), eps 1e-6, weight_decay 0, correct_bias True), same
-`param_groups` list of dicts (one group per tensor with its own lr / weight_decay in the reference; the warm-up schedulers
-of train_tasks.py:431-437 mutate group["lr"] exactly as before). step() is ONE kernel launch over the flat buffers
-(csrc/vb_optim.cu) that also writes the 16-bit tensor-core operand copy of the updated weights and zeroes the gradients,
-so the training step needs no separate weight cast and the `model.zero_grad()` that follows optimizer.step() in the
-reference (train_tasks.py:551) finds the buffer already clean.
+    optimizer = RAdam(optimizer_grouped_parameters, lr=base_lr)                             # vilbert/optimization.py
+ -> optimizer = FusedRAdam(optimizer_grouped_parameters, lr=base_lr, model=model)
+
+Same constructor arguments and defaults, same `param_groups` list of dicts (one group per tensor with its own lr /
+weight_decay in the reference; the warm-up schedulers of train_tasks.py:431-437 mutate group["lr"] exactly as before).
+step() is ONE kernel launch over the flat buffers (csrc/vb_optim.cu) that also writes the 16-bit tensor-core operand copy
+of the updated weights and zeroes the gradients, so the training step needs no separate weight cast and the
+`model.zero_grad()` that follows optimizer.step() in the reference (train_tasks.py:551) finds the buffer already clean.
 """
 import ctypes as C
 
@@ -35,20 +37,26 @@ def build_chunks(ranges, chunk=32768):
     return np.asarray(st, np.int64), np.asarray(cn, np.int32), np.asarray(gr, np.int32)
 
 
-class FusedAdamW(torch.optim.Optimizer):
-    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0, correct_bias=True, model=None, engine=None,
-                 zero_grad=True, chunk=32768):
+class _FlatBufferOptimizer(torch.optim.Optimizer):
+    """What the fused optimizers share: the parameters must be views of the engine's flat fp32 buffer; the moments are two
+    flat buffers of the same layout (per-parameter state entries are views of them); the work list is a chunk table over
+    the trainable tensors; the hyper-parameters live in a device table (one vb_adamw_group row per param group) that is
+    re-uploaded from pinned memory when a scheduler changed it; the step counter is a device int32."""
+
+    def __init__(self, params, defaults, model, engine, zero_grad, chunk):
+        name = type(self).__name__
         if engine is None:
             if model is None:
-                raise ValueError("FusedAdamW needs model= (a vilbert_b200 model) or engine=")
+                raise ValueError(f"{name} needs model= (a vilbert_b200 model) or engine=")
             engine = model.engine
-        if lr < 0.0:
-            raise ValueError("Invalid learning rate: {} - should be >= 0.0".format(lr))
+        if defaults["lr"] < 0.0:
+            raise ValueError("Invalid learning rate: {} - should be >= 0.0".format(defaults["lr"]))
+        betas = defaults["betas"]
         if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
             raise ValueError("Invalid beta parameters: {} - should be in [0.0, 1.0[".format(betas))
-        if not 0.0 <= eps:
-            raise ValueError("Invalid epsilon value: {} - should be >= 0.0".format(eps))
-        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, correct_bias=correct_bias))
+        if not 0.0 <= defaults["eps"]:
+            raise ValueError("Invalid epsilon value: {} - should be >= 0.0".format(defaults["eps"]))
+        super().__init__(params, defaults)
         self.engine = engine
         self.fused_zero_grad = bool(zero_grad)
         ps = engine.ps
@@ -66,7 +74,7 @@ class FusedAdamW(torch.optim.Optimizer):
                     continue
                 off = (p.data_ptr() - base) // 4
                 if (p.data_ptr() - base) % 4 or off < 0 or off + p.numel() > numel or not p.is_contiguous() or p.dtype != torch.float32:
-                    raise ValueError("FusedAdamW: every parameter must be a contiguous fp32 view of the engine's flat buffer")
+                    raise ValueError(f"{name}: every parameter must be a contiguous fp32 view of the engine's flat buffer")
                 ranges.append((off, p.numel(), gi))
                 self.state[p] = dict(step=0, exp_avg=self.exp_avg[off:off + p.numel()].view(p.shape),
                                      exp_avg_sq=self.exp_avg_sq[off:off + p.numel()].view(p.shape))
@@ -89,53 +97,33 @@ class FusedAdamW(torch.optim.Optimizer):
             engine.shadow_trusted = True
 
     # ------------------------------------------------------------------ hyper-parameter table
+    def _group_row(self, grp):
+        """The vb_adamw_group row of one param group."""
+        return (grp["lr"], grp["betas"][0], grp["betas"][1], grp["eps"], grp["weight_decay"], 0)
+
     def _upload_groups(self):
         g = self._groups_np
         for i, grp in enumerate(self.param_groups):
-            g[i] = (grp["lr"], grp["betas"][0], grp["betas"][1], grp["eps"], grp["weight_decay"], 1 if grp["correct_bias"] else 0)
+            g[i] = self._group_row(grp)
         key = g.tobytes()
         if key != self._groups_last:
             self._groups_dev.copy_(self._groups_host, non_blocking=True)
             self._groups_last = key
 
-    # ------------------------------------------------------------------ stepping
-    def launch(self, stream=None):
-        """The kernel launch alone (capturable in a CUDA graph): uses the hyper-parameter table and step counter currently on the
-        device. `step()` = advance the counter + refresh the table + launch."""
+    def _buffer_args(self):
+        """The leading arguments of vb_adamw_step / vb_radam_step: buffers, 16-bit copies, chunk table and group table."""
         ps = self.engine.ps
-        if stream is None:
-            stream = torch.cuda.current_stream().cuda_stream
-        L.check(L.lib().vb_adamw_step(ps.flat.data_ptr(), ps.grad.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
-                                      ps.shadow.data_ptr(), ps.shadow_lo.data_ptr() if ps.split else None,
-                                      ps.shadow_b.data_ptr() if ps.shadow_b is not ps.shadow else None, 1 if ps.op_dtype == torch.float16 else 0,
-                                      self._chunk_start.data_ptr(), self._chunk_count.data_ptr(), self._chunk_group.data_ptr(), self.n_chunks,
-                                      self._groups_dev.data_ptr(), self._step_dev.data_ptr(), C.c_float(self.grad_scale),
-                                      1 if self.fused_zero_grad else 0, stream), "vb_adamw_step")
+        return (ps.flat.data_ptr(), ps.grad.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
+                ps.shadow.data_ptr(), ps.shadow_lo.data_ptr() if ps.split else None,
+                ps.shadow_b.data_ptr() if ps.shadow_b is not ps.shadow else None, 1 if ps.op_dtype == torch.float16 else 0,
+                self._chunk_start.data_ptr(), self._chunk_count.data_ptr(), self._chunk_group.data_ptr(), self.n_chunks,
+                self._groups_dev.data_ptr())
 
-    def op(self):
-        """(fn, args) for an engine op list (Plan.epilogue): the launch as a plan operation."""
-        ps = self.engine.ps
-        return (L.lib().vb_adamw_step, (ps.flat.data_ptr(), ps.grad.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
-                                        ps.shadow.data_ptr(), ps.shadow_lo.data_ptr() if ps.split else None,
-                                      ps.shadow_b.data_ptr() if ps.shadow_b is not ps.shadow else None, 1 if ps.op_dtype == torch.float16 else 0,
-                                        self._chunk_start.data_ptr(), self._chunk_count.data_ptr(), self._chunk_group.data_ptr(), self.n_chunks,
-                                        self._groups_dev.data_ptr(), self._step_dev.data_ptr(), C.c_float(self.grad_scale),
-                                        1 if self.fused_zero_grad else 0))
-
-    @torch.no_grad()
-    def step(self, closure=None):
-        loss = closure() if closure is not None else None
-        self.step_count += 1
-        self._step_dev.add_(1)
-        for st in self.state.values():
-            st["step"] = self.step_count
-        self._upload_groups()
-        self.launch()
+    def _after_step(self):
         eng = self.engine
         eng.shadow_clean = True
         if self.fused_zero_grad:
             eng.grad_clean = True
-        return loss
 
     def zero_grad(self, set_to_none=False):
         """The gradients live in the engine's flat buffer and were zeroed by step(); the views stay attached."""
@@ -160,3 +148,92 @@ class FusedAdamW(torch.optim.Optimizer):
                 if k != "params":
                     g_old[k] = v
         self._upload_groups()
+
+
+class FusedAdamW(_FlatBufferOptimizer):
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0, correct_bias=True, model=None, engine=None,
+                 zero_grad=True, chunk=32768):
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, correct_bias=correct_bias),
+                         model, engine, zero_grad, chunk)
+
+    def _group_row(self, grp):
+        return super()._group_row(grp)[:5] + (1 if grp["correct_bias"] else 0,)
+
+    # ------------------------------------------------------------------ stepping
+    def launch(self, stream=None):
+        """The kernel launch alone (capturable in a CUDA graph): uses the hyper-parameter table and step counter currently on the
+        device. `step()` = advance the counter + refresh the table + launch."""
+        if stream is None:
+            stream = torch.cuda.current_stream().cuda_stream
+        L.check(L.lib().vb_adamw_step(*self._buffer_args(), self._step_dev.data_ptr(), C.c_float(self.grad_scale),
+                                      1 if self.fused_zero_grad else 0, stream), "vb_adamw_step")
+
+    def op(self):
+        """(fn, args) for an engine op list (Plan.epilogue): the launch as a plan operation."""
+        return (L.lib().vb_adamw_step, self._buffer_args() + (self._step_dev.data_ptr(), C.c_float(self.grad_scale),
+                                                              1 if self.fused_zero_grad else 0))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = closure() if closure is not None else None
+        self.step_count += 1
+        self._step_dev.add_(1)
+        for st in self.state.values():
+            st["step"] = self.step_count
+        self._upload_groups()
+        self.launch()
+        self._after_step()
+        return loss
+
+
+class FusedRAdam(_FlatBufferOptimizer):
+    """The reference's RAdam (vilbert/optimization.py:16-100; `--optim RAdam`, train_tasks.py:427-428) as one launch of
+    `radam_kernel` per step. Same defaults (lr 1e-3, betas (0.9, 0.999), eps 1e-8, weight_decay 0) and checkpoint layout
+    (per parameter index: {step, exp_avg, exp_avg_sq}), so state dicts move between the two.
+
+    Reference behaviour kept on purpose: the rectification term and step size of a step are computed once, from the lr and
+    betas of the first param group holding a trainable tensor (the "leader group"), and used for every tensor; each group's
+    own lr only enters its weight decay (and its betas its moments). With the reference's grouping that group is the word
+    embeddings' at base_lr, so the vil_* heads' lr of 1e-4 does not reach their RAdam update."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, model=None, engine=None, zero_grad=True,
+                 chunk=32768):
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), model, engine, zero_grad, chunk)
+        self.leader_group = next((gi for gi, g in enumerate(self.param_groups) if any(p in self.state for p in g["params"])), 0)
+
+    def _args(self, advance_step):
+        return self._buffer_args() + (self.leader_group, self._step_dev.data_ptr(), advance_step, C.c_float(self.grad_scale),
+                                      1 if self.fused_zero_grad else 0)
+
+    # ------------------------------------------------------------------ stepping
+    def launch(self, stream=None, advance_step=False):
+        """The kernel launch alone (capturable in a CUDA graph): uses the hyper-parameter table currently on the device, and the
+        device step counter, first advanced by one on the same stream when `advance_step`. `step()` = refresh the table +
+        launch(advance_step=True)."""
+        if stream is None:
+            stream = torch.cuda.current_stream().cuda_stream
+        L.check(L.lib().vb_radam_step(*self._args(1 if advance_step else 0), stream), "vb_radam_step")
+
+    def op(self):
+        """(fn, args) for an engine op list (Plan.epilogue): advance the step counter + the launch, as one plan operation, so
+        every replay of a captured step moves one step along the rectification schedule."""
+        return (L.lib().vb_radam_step, self._args(1))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        loss = closure() if closure is not None else None
+        self.step_count += 1
+        for st in self.state.values():
+            st["step"] = self.step_count
+        self._upload_groups()
+        self.launch(advance_step=True)
+        self._after_step()
+        return loss
+
+    def state_dict(self):
+        """The per-parameter "step" is the device counter's value: replays of a captured step advance it without the host
+        knowing."""
+        self.step_count = int(self._step_dev.item())
+        for st in self.state.values():
+            st["step"] = self.step_count
+        return super().state_dict()
