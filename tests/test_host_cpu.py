@@ -145,6 +145,68 @@ def test_special_mode_plans_build_on_cpu(golden_dir):
     assert small.lm_c["cap"] == 40                                              # never more rows than there are (8-padded)
 
 
+@pytest.mark.parametrize("precision", ["fp16", "fp32", "bf16"])
+@pytest.mark.parametrize("mode", ["base", "dynamic_attention", "in_batch_pairs"])
+def test_tensor_core_operands_are_in_the_format_of_their_pass(golden_dir, precision, mode):
+    """Every operand pointer a plan hands the GEMM and attention kernels lies in a tensor of the format the kernel reads it
+    as: the forward format (fp16, or bf16) for the forward GEMMs and for Q / K / V / O, bf16 for the backward GEMMs, the
+    attention gradients and every bf16 copy. An fp16 buffer passed where its bf16 copy belongs would otherwise be read as
+    bf16 bits without any error."""
+    bf16 = torch.bfloat16
+    cfgj = json.load(open(os.path.join(golden_dir, "tiny_b4.json")))["config"]
+    if mode != "base":
+        cfgj = dict(cfgj, **{mode: True})
+    eng = Engine(BertConfig.from_dict(cfgj), "cpu", _build_only=True, precision=precision)
+    plan = eng.plan(4, 9, 11, grad_outputs=O.HEAD_NAMES, train=True)
+    ps, fwd_dt = eng.ps, eng.op_dtype
+    tensors = [t for t in [ps.shadow, ps.shadow_b, ps.shadow_lo] + plan._keep if torch.is_tensor(t)]
+    spans = [(t.data_ptr(), t.data_ptr() + t.numel() * t.element_size(), t.dtype) for t in tensors]
+
+    def dtype_at(p):
+        return next(dt for lo, hi, dt in spans if lo <= p < hi)
+
+    n_gemm = n_attn = 0
+    wrong = []
+    for section, ops in (("fwd", plan.fwd), ("bwd", plan.bwd)):
+        pass_dt = fwd_dt if section == "fwd" else bf16
+        for fn, args, _ in ops:
+            name = getattr(fn, "__name__", None)
+            if name == "vb_gemm_bf16":
+                n_gemm += 1
+                s = args[0]._obj
+                want = [(f, pass_dt) for f in ("A", "B", "A_lo", "B_lo", "out_bf16", "out_lo")] + [("out_b16", bf16)]
+                if precision == "fp32" and section == "fwd":
+                    assert s.A_lo and s.B_lo, "split-precision forward GEMM without low parts"
+            elif name in ("vb_attention_fwd", "vb_attention_bwd"):
+                n_attn += 1
+                s = args[0]._obj
+                want = [(f, fwd_dt) for f in ("Q", "K", "V", "O", "Q_lo", "K_lo", "V_lo", "O_lo")] + \
+                       [(f, bf16) for f in ("dO", "dQ", "dK", "dV", "O_b16")]
+            else:
+                continue
+            wrong += [(section, name, f, dtype_at(getattr(s, f))) for f, dt in want if getattr(s, f) and dtype_at(getattr(s, f)) != dt]
+    assert n_gemm > 100 and n_attn > 10
+    assert not wrong, wrong
+
+
+def test_plan_rejects_operands_in_the_wrong_format(golden_dir):
+    """Plan.gemm refuses, while the plan is built, a forward operand that is not an Operand of the engine's format and a
+    backward operand that is not bf16."""
+    from vilbert_b200.engine import Operand
+    cfgj = json.load(open(os.path.join(golden_dir, "tiny_b4.json")))["config"]
+    plan = Engine(BertConfig.from_dict(cfgj), "cpu", _build_only=True).plan(4, 9, 11)
+    a16, ab = torch.zeros(8, 8, dtype=torch.float16), torch.zeros(8, 8, dtype=torch.bfloat16)
+    with pytest.raises(TypeError):
+        plan.gemm(8, 8, 8, a16, 8, Operand(a16), 8)                     # forward: plain tensor
+    with pytest.raises(TypeError):
+        plan.gemm(8, 8, 8, Operand(ab, bw=ab), 8, Operand(a16), 8)       # forward: bf16 in an fp16 engine
+    plan.cur = plan.bwd
+    with pytest.raises(TypeError):
+        plan.gemm(8, 8, 8, ab, 8, a16, 8, out_f32=torch.zeros(8, 8))    # backward: fp16 weight copy in place of its bf16 copy
+    plan.gemm(8, 8, 8, ab, 8, ab, 8, out_f32=torch.zeros(8, 8))
+    assert plan.bwd[-1][0].__name__ == "vb_gemm_bf16"
+
+
 def test_shared_activation_arena_layout(golden_dir):
     """Engine.enable_activation_arena: activation / scratch buffers of every plan are sub-allocated from one arena (plans overlay
     each other), while everything loaded or initialised outside a run (inputs, targets, output gradients) stays private."""

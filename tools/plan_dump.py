@@ -1,0 +1,149 @@
+"""Canonical text listing of the launches the engine's plans make, for checking that a host-side refactor of engine.py /
+optim.py launches exactly what it launched before. Needs the built libvilbert_b200.so, no GPU (plans are built with
+_build_only=True on the CPU).
+
+    python tools/plan_dump.py ROOT [--out FILE]
+
+imports the package from the repository tree ROOT. For every plan of the case matrix below it lists each op of the prologue,
+forward, backward and epilogue: section, stream id, function name (MARK for a stream barrier / event marker) and every
+argument. Structs passed by reference are expanded field by field, and every pointer (a c_void_p argument or struct field) is
+written as `allocation+byte offset` against the plan's allocations, so two runs, or two trees that launch the same work,
+produce byte-identical listings."""
+import argparse
+import ctypes as C
+import json
+import os
+import sys
+
+ARENA_BYTES = 64 << 20
+NT, NV = 9, 11
+
+
+def cases(O, LOSS_HEADS):
+    """(name, config overrides, engine heads, B, plan kwargs) of the case matrix."""
+    train = dict(grad_outputs=O.HEAD_NAMES, train=True)
+    return [
+        ("heads_train", {}, "vl", 4, train),
+        ("vqa_loss", {}, "vl", 4, dict(grad_outputs=("vil_prediction",), vqa_loss=True, train=True)),
+        ("task_tokens", dict(task_specific_tokens=True), "vl", 4, train),
+        ("dynamic_attention", dict(dynamic_attention=True), "vl", 4, train),
+        ("fast_mode", dict(fast_mode=True), "vl", 4, {}),
+        ("in_batch_pairs", dict(in_batch_pairs=True), "vl", 4, train),
+        ("visualization", dict(visualization=True), "vl", 4, dict(grad_outputs=O.HEAD_NAMES)),
+        ("fixed_t_layer", dict(fixed_t_layer=1), "vl", 4, train),
+        ("pretraining", {}, "pretraining", 4, dict(grad_outputs=LOSS_HEADS["pretraining"], loss="pretraining", train=True)),
+        ("odd_b3", {}, "vl", 3, train),
+    ]
+
+
+class Allocations:
+    """Names pointers after the first allocation (in the order given) whose storage contains them."""
+
+    def __init__(self, named):
+        self.ranges = []
+        for name, t in named:
+            if t is None or not hasattr(t, "untyped_storage"):
+                continue
+            s = t.untyped_storage()
+            if s.nbytes():
+                self.ranges.append((name, s.data_ptr(), s.nbytes()))
+
+    def name(self, p):
+        if not p:
+            return "0"
+        for name, base, n in self.ranges:
+            if base <= p < base + n:
+                return f"{name}+{p - base}"
+        raise ValueError(f"pointer {p:#x} lies in none of the plan's allocations")
+
+
+def allocations(plan, opt=None):
+    import torch
+    e, ps = plan.e, plan.e.ps
+    named = [("flat", ps.flat), ("grad", ps.grad), ("shadow", ps.shadow), ("shadow_b", ps.shadow_b), ("shadow_lo", ps.shadow_lo),
+             ("drop_step", e.drop_step), ("arena", e.arena)]
+    named += [(f"keep{i}", t) for i, t in enumerate(t for t in plan._keep if torch.is_tensor(t))]
+    named += [(f"plan.{k}", v) for k, v in sorted(vars(plan).items()) if torch.is_tensor(v)]
+    if opt is not None:
+        named += [(f"opt.{k}", v) for k, v in sorted(vars(opt).items()) if torch.is_tensor(v)]
+    return Allocations(named)
+
+
+def value(v, ctype, alloc):
+    if v is None:
+        return "0"
+    if hasattr(v, "_obj"):          # byref(struct), also where the argtype is a plain void*
+        return struct(v._obj, alloc)
+    if ctype is C.c_void_p:
+        return alloc.name(v)
+    if isinstance(ctype, type) and issubclass(ctype, C.Structure):
+        return struct(v, alloc)
+    if isinstance(v, C._SimpleCData):
+        v = v.value
+    return repr(float(v)) if isinstance(v, float) or ctype is C.c_float else str(int(v))
+
+
+def struct(s, alloc):
+    return "{" + ",".join(f"{f}={value(getattr(s, f), t, alloc)}" for f, t in s._fields_) + "}"
+
+
+def dump_plan(out, title, plan, opt=None):
+    alloc = allocations(plan, opt)
+    n = 0
+    out.append(f"== {title}")
+    for section in ("prologue", "fwd", "bwd", "epilogue"):
+        for i, (fn, args, sid) in enumerate(getattr(plan, section)):
+            if fn is None:
+                rec = "MARK " + " ".join(str(a) for a in args)
+            else:
+                types = fn.argtypes[:len(args)]
+                assert len(types) == len(args) == len(fn.argtypes) - 1, fn.__name__     # the trailing argument is the stream
+                rec = fn.__name__ + " " + " ".join(value(a, t, alloc) for a, t in zip(args, types))
+            out.append(f"{section} {i} s{sid} {rec.rstrip()}")
+            n += 1
+    return n
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("root", help="repository tree to import the package from")
+    ap.add_argument("--out", help="output file (default: stdout)")
+    a = ap.parse_args()
+    root = os.path.abspath(a.root)
+    sys.path.insert(0, root)
+    import torch
+    from oracle import vilbert_oracle as O
+    from vilbert_b200.config import BertConfig
+    from vilbert_b200.engine import LOSS_HEADS, PRECISIONS, Engine
+    from vilbert_b200.optim import FusedAdamW, FusedRAdam
+    tiny = json.load(open(os.path.join(root, "tests", "golden", "tiny_b4.json")))["config"]
+    out, n_plans, n_ops = [], 0, 0
+    for prec in PRECISIONS:
+        for name, over, heads, B, kw in cases(O, LOSS_HEADS):
+            for arena in (False, True):
+                eng = Engine(BertConfig.from_dict(dict(tiny, **over)), "cpu", heads=heads, _build_only=True, precision=prec)
+                if arena:
+                    eng.enable_activation_arena(ARENA_BYTES)
+                plan = eng.plan(B, NT, NV, **kw)
+                plan.enable_training_prologue()
+                n_ops += dump_plan(out, f"{prec} {name} arena={int(arena)}", plan)
+                n_plans += 1
+        for opt_cls in (FusedAdamW, FusedRAdam):
+            eng = Engine(BertConfig.from_dict(tiny), "cpu", _build_only=True, precision=prec)
+            plan = eng.plan(4, NT, NV, grad_outputs=O.HEAD_NAMES, train=True)
+            params = [torch.nn.Parameter(eng.ps.p(nm)) for nm in eng.ps.entries]
+            opt = opt_cls(params, lr=1e-4, engine=eng)
+            plan.enable_optimizer(opt)
+            n_ops += dump_plan(out, f"{prec} {opt_cls.__name__}", plan, opt)
+            n_plans += 1
+    text = "\n".join(out) + "\n"
+    if a.out:
+        with open(a.out, "w") as f:
+            f.write(text)
+    else:
+        sys.stdout.write(text)
+    print(f"plan_dump: {n_plans} plans, {n_ops} op records", file=sys.stderr)
+
+
+if __name__ == "__main__":
+    main()

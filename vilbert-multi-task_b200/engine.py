@@ -15,7 +15,7 @@ activations and weights exist only as tensor-core operands. Three operand precis
                     precision (model.half(), train_concap.py:504-505) — gradient operands (dy, dS, ...) bf16 for range.
                     wgmma takes one operand type for both inputs, so every forward operand the backward contracts with a
                     gradient (weights for dgrad, saved activations for wgrad) also has a bf16 copy, written by the kernel
-                    that produces it (Act.bw, ParamStore.shadow_b);
+                    that produces it (Operand.bw);
   "fp32"            split precision: every forward operand is stored as fp16 hi + lo and every forward contraction
                     runs as three tensor-core passes (hi.hi + lo.hi + hi.lo), ~fp32 accuracy (north_star 1e-3);
   "bf16"            every operand bf16 (round-1 arithmetic; kept for A/B measurements).
@@ -40,6 +40,42 @@ def _pad8(n):
 def dropout_site_id(name):
     """Stable 32-bit id of a dropout layer, shared with the oracle's mask generator (crc32 of its canonical name)."""
     return zlib.crc32(name.encode()) & 0xFFFFFFFF
+
+
+class Operand:
+    """A 16-bit tensor-core operand: `hi` in the engine's forward format (fp16, or bf16 with precision="bf16"), `lo` its
+    split-precision low part (None unless precision="fp32"), `bw` the bf16 copy the backward GEMMs contract with (hi itself
+    when hi is bf16, None when nothing in the backward reads it)."""
+    __slots__ = ("hi", "lo", "bw")
+
+    def __init__(self, hi, lo=None, bw=None):
+        self.hi, self.lo, self.bw = hi, lo, bw
+
+    @property
+    def fp16(self):
+        """Format flag of the C ABI (1 = fp16, 0 = bf16)."""
+        return 1 if self.hi.dtype == F16 else 0
+
+    @property
+    def extra_bw(self):
+        """The bf16 copy as a separate output of the kernel that writes hi: None when there is none or it is hi itself."""
+        return None if self.bw is None or self.bw is self.hi else self.bw
+
+    def _map(self, f):
+        hi = f(self.hi)
+        return Operand(hi, None if self.lo is None else f(self.lo), hi if self.bw is self.hi else (None if self.bw is None else f(self.bw)))
+
+    def cols(self, a, b):
+        """Columns [a, b) (the Q / K / V panels of a packed projection)."""
+        return self._map(lambda t: t[:, a:b])
+
+    def view(self, *shape):
+        return self._map(lambda t: t.view(*shape))
+
+    def ptrs(self, off=0):
+        """(hi, lo, extra_bw) data pointers `off` elements in (None for a missing part): the 16-bit outputs of the cast and
+        optimizer kernels."""
+        return tuple(None if t is None else t.data_ptr() + t.element_size() * off for t in (self.hi, self.lo, self.extra_bw))
 
 
 # ------------------------------------------------------------------------------------------ parameters
@@ -130,6 +166,7 @@ class ParamStore:
         self.shadow_lo = torch.zeros(self.numel, dtype=op_dtype, device=device) if split else None
         # bf16 copy for the backward (dgrad: dy bf16 x W): the shadow itself when the operand format is already bf16
         self.shadow_b = self.shadow if op_dtype == BF16 else torch.zeros(self.numel, dtype=BF16, device=device)
+        self.shadows = Operand(self.shadow, self.shadow_lo, self.shadow_b)
         self.shadow_version = None
 
     def _add(self, name, shape):
@@ -169,21 +206,20 @@ class ParamStore:
     def g(self, name):
         return self._view(self.grad, name)
 
-    def w16(self, name):
-        return self._view(self.shadow, name)
+    def w(self, name):
+        """The 16-bit operand copies of one weight."""
+        return self.shadows._map(lambda t: self._view(t, name))
 
-    def w16lo(self, name):
-        return self._view(self.shadow_lo, name) if self.split else None
-
-    def w16b(self, name):
-        return self._view(self.shadow_b, name)
+    def cast_args(self, off, n):
+        """Arguments (without the stream) of the vb_cast_f32_to_bf16 launch that refreshes elements [off, off + n) of the 16-bit
+        copies from the fp32 parameters."""
+        hi, lo, bw = self.shadows.ptrs(off)
+        return (self.flat.data_ptr() + 4 * off, hi, n, self.shadows.fp16, lo, bw)
 
     def refresh_shadow(self, stream):
         """16-bit operand copy (hi, and lo in split precision) of every parameter in one launch (belongs with the
         optimizer step in training)."""
-        L.check(L.lib().vb_cast_f32_to_bf16(self.flat.data_ptr(), self.shadow.data_ptr(), self.numel, 1 if self.op_dtype == F16 else 0,
-                                            self.shadow_lo.data_ptr() if self.split else None,
-                                            self.shadow_b.data_ptr() if self.shadow_b is not self.shadow else None, stream), "vb_cast_f32_to_bf16")
+        L.check(L.lib().vb_cast_f32_to_bf16(*self.cast_args(0, self.numel), stream), "vb_cast_f32_to_bf16")
 
 
 # ------------------------------------------------------------------------------------------ plan
@@ -209,14 +245,11 @@ class _TrackedParams:
 
 
 class Act:
-    """A residual-stream activation: fp32 values, 16-bit operand copy (b16; lo = its split-precision low part or None),
-    fp32 gradient (lazily allocated)."""
-    __slots__ = ("f32", "b16", "lo", "bw", "g32", "gw", "M", "H", "frozen")
+    """A residual-stream activation: fp32 values, its tensor-core Operand, fp32 gradient (lazily allocated)."""
+    __slots__ = ("f32", "op", "g32", "gw", "M", "H", "frozen")
 
-    def __init__(self, f32, b16, M, H, lo=None, bw=None):
-        """bw: bf16 copy of the operand for the backward's weight-gradient GEMM (== b16 when the operand format is bf16)."""
-        self.f32, self.b16, self.lo, self.M, self.H = f32, b16, lo, M, H
-        self.bw = b16 if bw is None else bw
+    def __init__(self, f32, op, M, H):
+        self.f32, self.op, self.M, self.H = f32, op, M, H
         self.g32, self.gw = None, False
         self.frozen = False     # produced under the reference's torch.no_grad() (fixed_t_layer / fixed_v_layer): no gradient flows into it
 
@@ -274,8 +307,7 @@ class Plan:
             raise ValueError(f"loss must be one of {sorted(LOSS_HEADS)}")
         self.vqa_loss = self.loss_kind == "vqa"
         self.train = bool(train)          # nn.Dropout layers active (model.train()); False = the reference's eval mode
-        self.op_fp16 = 1 if engine.op_dtype == F16 else 0   # format of the forward operands (activations, weights)
-        self.op_dtype, self.split = engine.op_dtype, engine.split
+        self.op_dtype, self.split = engine.op_dtype, engine.split   # format of the forward operands (activations, weights)
         self.head_dropout_prob = engine.head_dropout_prob
         self.heads = engine.ps.heads if heads is None else heads   # "vl" | "pretraining" | "none"
         self.fwd_id = 0
@@ -323,17 +355,10 @@ class Plan:
         return arena[off:off + nbytes].view(dtype).view(shape)
 
     def buf16(self, shape, bw=True):
-        """Forward-operand buffer in the engine's operand format: (hi, lo, bw) with lo = None unless split precision and
-        bw = the bf16 copy the backward's weight-gradient GEMM reads (hi itself when the format is bf16, None if not wanted)."""
+        """Forward-operand buffer in the engine's operand format; bw=False: no bf16 copy (nothing in the backward reads it)."""
         hi = self.buf(shape, self.op_dtype)
         lo = self.buf(shape, self.op_dtype) if self.split else None
-        b = None if not bw else (hi if self.op_dtype == BF16 else self.buf(shape, BF16))
-        return hi, lo, b
-
-    @staticmethod
-    def _extra(bw, hi):
-        """Pointer for a kernel's optional bf16-copy output: None when the copy IS the primary output."""
-        return None if (bw is None or bw is hi) else bw
+        return Operand(hi, lo, None if not bw else (hi if self.op_dtype == BF16 else self.buf(shape, BF16)))
 
     def scratch(self, tag, shape, dtype):
         # with asynchronous weight-gradient streams a temporary may still be read after its layer's backward has moved on:
@@ -397,20 +422,32 @@ class Plan:
     def _ref(d):
         return C.byref(d) if d is not None else None
 
+    def _check_operands(self, fwd_ops, bwd_ops):
+        """The kernels are told a format flag, not typed pointers: a buffer of the other format would be read as its bits.
+        So forward operands must be Operands in the engine's format and backward operands bf16 tensors (None = absent)."""
+        if any(o is not None and (not isinstance(o, Operand) or o.hi.dtype != self.op_dtype) for o in fwd_ops):
+            raise TypeError(f"forward tensor-core operands must be Operands in {self.op_dtype}, got {[type(o).__name__ for o in fwd_ops]}")
+        if any(t is not None and (not torch.is_tensor(t) or t.dtype != BF16) for t in bwd_ops):
+            raise TypeError(f"backward tensor-core operands must be bf16 tensors, got {[getattr(t, 'dtype', t) for t in bwd_ops]}")
+
     def gemm(self, M, N, K, A, lda, B, ldb, a_mn=0, b_mn=0, bias=None, residual=None, ld_res=0, aux=None, ld_aux=0, act=0,
              out_f32=None, ld_of=0, out_bf16=None, ld_ob=0, out_pre=None, ld_op=0, atomic=0, split_k=1, alpha=1.0, out_colsum=None,
-             dropout=None, a_lo=None, b_lo=None, out_lo=None, out_b16=None):
-        """Operand formats follow the pass being emitted: in the forward pass A, B and the 16-bit output are forward
-        operands (engine format, + low parts in split precision; out_b16 = optional bf16 copy of the output for the
-        backward); in the backward pass everything is bf16: A is a gradient operand, B the bf16 copy of a weight (dgrad) or
-        of a saved activation (wgrad), 16-bit outputs are gradients."""
+             dropout=None):
+        """Operand formats follow the pass being emitted: in the forward pass A, B and the 16-bit output (out_bf16) are
+        Operands (engine format, + low parts in split precision, + the output's bf16 copy for the backward); in the backward
+        pass they are bf16 tensors: A a gradient, B the bf16 copy of a weight (dgrad) or of a saved activation (wgrad),
+        the 16-bit output a gradient."""
         g = L.GemmArgs()
         fwd = self.cur is self.fwd
-        g.a_fp16 = g.b_fp16 = g.out_fp16 = self.op_fp16 if fwd else 0
         if fwd:
-            g.out_b16 = self._ptr(out_b16)
-        if fwd and self.split:
-            g.A_lo, g.B_lo, g.out_lo = self._ptr(a_lo), self._ptr(b_lo), self._ptr(out_lo)
+            self._check_operands((A, B, out_bf16), ())
+            g.a_fp16 = g.b_fp16 = g.out_fp16 = A.fp16
+            g.A_lo, g.B_lo = self._ptr(A.lo), self._ptr(B.lo)
+            if out_bf16 is not None:
+                g.out_lo, g.out_b16, out_bf16 = self._ptr(out_bf16.lo), self._ptr(out_bf16.extra_bw), out_bf16.hi
+            A, B = A.hi, B.hi
+        else:
+            self._check_operands((), (A, B, out_bf16))      # the format flags stay 0 (bf16)
         g.M, g.N, g.K = M, N, K
         g.A, g.lda, g.a_mn_major = self._ptr(A), lda, a_mn
         g.B, g.ldb, g.b_mn_major = self._ptr(B), ldb, b_mn
@@ -430,17 +467,18 @@ class Plan:
         self.emit(self.lib.vb_gemm_bf16, C.byref(g))
 
     def attention(self, bwd, B, H, Nq, Nk, D, Q, ldq, K, ldk, V, ldv, mask, O, ldo, lse, dO=None, lddo=0, dQ=None, lddq=0,
-                  dK=None, lddk=0, dV=None, lddv=0, delta=None, dbq=None, dbk=None, dbv=None, dropout=None, q_lo=None, k_lo=None,
-                  v_lo=None, o_lo=None, o_b16=None):
+                  dK=None, lddk=0, dV=None, lddv=0, delta=None, dbq=None, dbk=None, dbv=None, dropout=None):
+        """Q, K, V and O are Operands (the forward's; the backward re-reads them), dO / dQ / dK / dV bf16 tensors."""
+        self._check_operands((Q, K, V, O), (dO, dQ, dK, dV))
         a = L.AttnArgs()
-        a.qkv_fp16 = self.op_fp16
-        a.O_b16 = self._ptr(o_b16)     # forward: written; backward: read for delta (consistent with the bf16 backward products)
-        if not bwd and self.split:
-            a.Q_lo, a.K_lo, a.V_lo, a.O_lo = self._ptr(q_lo), self._ptr(k_lo), self._ptr(v_lo), self._ptr(o_lo)
+        a.qkv_fp16 = Q.fp16
+        a.O_b16 = self._ptr(O.extra_bw)     # forward: written; backward: read for delta (consistent with the bf16 backward products)
+        if not bwd:
+            a.Q_lo, a.K_lo, a.V_lo, a.O_lo = self._ptr(Q.lo), self._ptr(K.lo), self._ptr(V.lo), self._ptr(O.lo)
         a.B, a.H, a.Nq, a.Nk, a.D = B, H, Nq, Nk, D
-        a.Q, a.ldq, a.K, a.ldk, a.V, a.ldv = self._ptr(Q), ldq, self._ptr(K), ldk, self._ptr(V), ldv
+        a.Q, a.ldq, a.K, a.ldk, a.V, a.ldv = self._ptr(Q.hi), ldq, self._ptr(K.hi), ldk, self._ptr(V.hi), ldv
         a.mask, a.scale = self._ptr(mask), 1.0 / math.sqrt(D)
-        a.O, a.ldo, a.lse = self._ptr(O), ldo, self._ptr(lse)
+        a.O, a.ldo, a.lse = self._ptr(O.hi), ldo, self._ptr(lse)
         a.dO, a.lddo, a.dQ, a.lddq = self._ptr(dO), lddo, self._ptr(dQ), lddq
         a.dK, a.lddk, a.dV, a.lddv, a.delta = self._ptr(dK), lddk, self._ptr(dV), lddv, self._ptr(delta)
         a.dbias_q, a.dbias_k, a.dbias_v = self._ptr(dbq), self._ptr(dbk), self._ptr(dbv)
@@ -452,15 +490,17 @@ class Plan:
             # config.visualization: the probabilities (fp32 [B, heads, Nq, Nk]) and views of the queries / keys the reference returns
             probs = self.buf((B, H, Nq, Nk), F32)
             self.emit(self.lib.vb_attention_probs, C.byref(a), probs.data_ptr())
-            self._last_attn = dict(attn=probs, q=Q, k=K, B=B, H=H, Nq=Nq, Nk=Nk, D=D)
+            self._last_attn = dict(attn=probs, q=Q.hi, k=K.hi, B=B, H=H, Nq=Nq, Nk=Nk, D=D)
 
     def ln_fwd(self, x, gamma, beta, M, H, want_f32=True, out_drop=None):
+        """-> (fp32 output or None, Operand output, mean, rstd)"""
         y32 = self.buf((M, H), F32) if want_f32 else None
-        y16, ylo, ybw = self.buf16((M, H))
+        y = self.buf16((M, H))
         mean, rstd = self.buf((M,), F32), self.buf((M,), F32)
-        self.emit(self.lib.vb_layernorm_fwd, x.data_ptr(), H, gamma.data_ptr(), beta.data_ptr(), 1e-12, self._ptr(y32), y16.data_ptr(), H,
-                  mean.data_ptr(), rstd.data_ptr(), M, H, self._ref(out_drop), self.op_fp16, self._ptr(ylo), self._ptr(self._extra(ybw, y16)))
-        return y32, y16, mean, rstd, ylo, ybw
+        hi, lo, bw = y.ptrs()
+        self.emit(self.lib.vb_layernorm_fwd, x.data_ptr(), H, gamma.data_ptr(), beta.data_ptr(), 1e-12, self._ptr(y32), hi, H,
+                  mean.data_ptr(), rstd.data_ptr(), M, H, self._ref(out_drop), y.fp16, lo, bw)
+        return y32, y, mean, rstd
 
     def ln_bwd(self, dy, x, gamma, mean, rstd, dx32, dx16, M, H, ggamma, gbeta, pre=None, gbias=None, out_drop=None, in_drop=None):
         """gbias: bias gradient of the Linear feeding this LayerNorm (column sums of dx), fused into the same pass."""
@@ -519,15 +559,14 @@ class Plan:
         self.emit(self.lib.vb_axpy_f32, src32.data_ptr(), g.data_ptr(), g.numel(), 1.0)
 
     # ------------------------------------------------------------------ blocks
-    def dense_res_ln(self, a16, K_in, res, wname, lnname, tag, drop=None, a_lo=None, a_bw=None):
+    def dense_res_ln(self, a, K_in, res, wname, lnname, tag, drop=None):
         """LN(dense(a) + residual)  — BertSelfOutput / BertOutput / BertBiOutput halves (vilbert.py:470-474, 513-517, 844-855)."""
         ps, M, H = self.ps, res.M, res.H
         y = self.buf((M, H), F32)
-        self.gemm(M, H, K_in, a16, K_in, ps.w16(wname + ".weight"), K_in, bias=ps.p(wname + ".bias"), residual=res.f32, ld_res=H,
-                  out_f32=y, ld_of=H, dropout=drop, a_lo=a_lo, b_lo=ps.w16lo(wname + ".weight"))
-        o32, o16, mean, rstd, olo, obw = self.ln_fwd(y, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, H)
-        out = Act(o32, o16, M, H, lo=olo, bw=obw)
-        a_bw = a16 if a_bw is None else a_bw
+        self.gemm(M, H, K_in, a, K_in, ps.w(wname + ".weight"), K_in, bias=ps.p(wname + ".bias"), residual=res.f32, ld_res=H,
+                  out_f32=y, ld_of=H, dropout=drop)
+        o32, o, mean, rstd = self.ln_fwd(y, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, H)
+        out = Act(o32, o, M, H)
 
         def bwd():
             """returns (dy16, dy32) of the dense output (== grad of the LN input); adds dy32 to res."""
@@ -537,7 +576,7 @@ class Plan:
             dy16 = self.scratch(tag + ".dy16", (M, H), BF16)
             self.ln_bwd(out.g32, y, ps.p(lnname + ".weight"), mean, rstd, dy32, dy16, M, H, ps.g(lnname + ".weight"), ps.g(lnname + ".bias"),
                         gbias=ps.g(wname + ".bias"), in_drop=drop)
-            self.linear_wgrad(dy16, H, None, 0, a_bw, K_in, M, H, K_in, wname)
+            self.linear_wgrad(dy16, H, None, 0, a.bw, K_in, M, H, K_in, wname)
             return dy16, dy32
         return out, bwd
 
@@ -545,10 +584,10 @@ class Plan:
         """LN(dense2(gelu(dense1(x))) + x) — BertIntermediate + BertOutput (vilbert.py:500-503, 513-517)."""
         ps, M, H = self.ps, x.M, x.H
         pre16 = self.buf((M, I), BF16)          # gelu'(pre), bf16 in every mode (only the backward reads it)
-        f16, flo, fbw = self.buf16((M, I))
-        self.gemm(M, I, H, x.b16, H, ps.w16(w1 + ".weight"), H, bias=ps.p(w1 + ".bias"), act=L.VB_ACT_GELU, out_bf16=f16, ld_ob=I,
-                  out_pre=pre16, ld_op=I, a_lo=x.lo, b_lo=ps.w16lo(w1 + ".weight"), out_lo=flo, out_b16=self._extra(fbw, f16))
-        out, out_bwd = self.dense_res_ln(f16, I, x, w2, lnname, tag + ".o", drop=drop, a_lo=flo, a_bw=fbw)
+        f = self.buf16((M, I))
+        self.gemm(M, I, H, x.op, H, ps.w(w1 + ".weight"), H, bias=ps.p(w1 + ".bias"), act=L.VB_ACT_GELU, out_bf16=f, ld_ob=I,
+                  out_pre=pre16, ld_op=I)
+        out, out_bwd = self.dense_res_ln(f, I, x, w2, lnname, tag + ".o", drop=drop)
 
         def bwd():
             r = out_bwd()
@@ -557,10 +596,10 @@ class Plan:
             dy16, dy32 = r
             dpre16 = self.scratch(tag + ".dpre16", (M, I), BF16)
             # d pre = (dy W2) * gelu'(pre)
-            self.gemm(M, I, H, dy16, H, ps.w16b(w2 + ".weight"), I, b_mn=1, aux=pre16, ld_aux=I, act=L.VB_ACT_DGELU, out_bf16=dpre16, ld_ob=I,
+            self.gemm(M, I, H, dy16, H, ps.w(w2 + ".weight").bw, I, b_mn=1, aux=pre16, ld_aux=I, act=L.VB_ACT_DGELU, out_bf16=dpre16, ld_ob=I,
                       out_colsum=ps.g(w1 + ".bias"))
-            self.linear_wgrad(dpre16, I, None, 0, x.bw, H, M, I, H, w1)
-            self.dgrad_into(x, dpre16, I, ps.w16b(w1 + ".weight"), M, I, H, extra32=dy32)
+            self.linear_wgrad(dpre16, I, None, 0, x.op.bw, H, M, I, H, w1)
+            self.dgrad_into(x, dpre16, I, ps.w(w1 + ".weight").bw, M, I, H, extra32=dy32)
         self.push_bwd(bwd)
         return out
 
@@ -569,27 +608,23 @@ class Plan:
         (text_pool) when config.dynamic_attention gates this image layer's queries and keys (:577-586)."""
         ps, M, H = self.ps, x.M, x.H
         D = H // nh
-        qkv, qkvl, _ = self.buf16((M, 3 * H), bw=False)     # the attention backward converts its Q/K/V panels in shared memory
-        self.gemm(M, 3 * H, H, x.b16, H, ps.w16(prefix + ".self.qkv.weight"), H, bias=ps.p(prefix + ".self.qkv.bias"), out_bf16=qkv, ld_ob=3 * H,
-                  a_lo=x.lo, b_lo=ps.w16lo(prefix + ".self.qkv.weight"), out_lo=qkvl)
+        qkv = self.buf16((M, 3 * H), bw=False)     # the attention backward converts its Q/K/V panels in shared memory
+        self.gemm(M, 3 * H, H, x.op, H, ps.w(prefix + ".self.qkv.weight"), H, bias=ps.p(prefix + ".self.qkv.bias"), out_bf16=qkv, ld_ob=3 * H)
         if pool is not None:
             # z = dyLinear_q | dyLinear_k (pool) as one [B, 2H] GEMM; Q and K are scaled in place by 1 + sigmoid(z)
             Kp = pool.H
             z = self.buf((B, 2 * H), F32)
-            self.gemm(B, 2 * H, Kp, pool.b16, Kp, ps.w16(prefix + ".self.dy.weight"), Kp, bias=ps.p(prefix + ".self.dy.bias"), out_f32=z, ld_of=2 * H,
-                      a_lo=pool.lo, b_lo=ps.w16lo(prefix + ".self.dy.weight"))
-            self.emit(self.lib.vb_gate_scale_fwd, qkv.data_ptr(), self._ptr(qkvl), 3 * H, z.data_ptr(), B, N, 2 * H, self.op_fp16)
-        ctx, ctxl, ctxb = self.buf16((M, H))
+            self.gemm(B, 2 * H, Kp, pool.op, Kp, ps.w(prefix + ".self.dy.weight"), Kp, bias=ps.p(prefix + ".self.dy.bias"), out_f32=z, ld_of=2 * H)
+            self.emit(self.lib.vb_gate_scale_fwd, qkv.hi.data_ptr(), self._ptr(qkv.lo), 3 * H, z.data_ptr(), B, N, 2 * H, qkv.fp16)
+        ctx = self.buf16((M, H))
         lse = self.buf((B, nh, N), F32)
-        q, k, v = qkv[:, 0:H], qkv[:, H:2 * H], qkv[:, 2 * H:]
-        ql, kl, vl = (qkvl[:, 0:H], qkvl[:, H:2 * H], qkvl[:, 2 * H:]) if self.split else (None, None, None)
+        q, k, v = qkv.cols(0, H), qkv.cols(H, 2 * H), qkv.cols(2 * H, 3 * H)
         adrop = self.drop(prefix + ".self.dropout", p_attn)
-        self.attention(False, B, nh, N, N, D, q, 3 * H, k, 3 * H, v, 3 * H, mask, ctx, H, lse, dropout=adrop, q_lo=ql, k_lo=kl, v_lo=vl, o_lo=ctxl,
-                       o_b16=self._extra(ctxb, ctx))
+        self.attention(False, B, nh, N, N, D, q, 3 * H, k, 3 * H, v, 3 * H, mask, ctx, H, lse, dropout=adrop)
         if self.viz:
             (self.attn_t if tag == "t" else self.attn_v).append(self._last_attn)
         out, out_bwd = self.dense_res_ln(ctx, H, x, prefix + ".output.dense", prefix + ".output.LayerNorm", tag + ".ao",
-                                         drop=self.drop(prefix + ".output.dropout", p_hidden), a_lo=ctxl, a_bw=ctxb)
+                                         drop=self.drop(prefix + ".output.dropout", p_hidden))
 
         def bwd():
             r = out_bwd()
@@ -597,25 +632,24 @@ class Plan:
                 return
             dy16, dy32 = r
             dctx = self.scratch(tag + ".dctx", (M, H), BF16)
-            self.gemm(M, H, H, dy16, H, ps.w16b(prefix + ".output.dense.weight"), H, b_mn=1, out_bf16=dctx, ld_ob=H)
+            self.gemm(M, H, H, dy16, H, ps.w(prefix + ".output.dense.weight").bw, H, b_mn=1, out_bf16=dctx, ld_ob=H)
             dqkv = self.scratch(tag + ".dqkv", (M, 3 * H), BF16)
             delta = self.scratch(tag + ".delta", (B, nh, N), F32)
             gb = ps.g(prefix + ".self.qkv.bias")     # bias gradients = column sums of dQ|dK|dV, fused into the attention backward
             gated = pool is not None                 # ... except under the gate, where the biases sit before the scaling
             self.attention(True, B, nh, N, N, D, q, 3 * H, k, 3 * H, v, 3 * H, mask, ctx, H, lse, dO=dctx, lddo=H,
                            dQ=dqkv[:, 0:H], lddq=3 * H, dK=dqkv[:, H:2 * H], lddk=3 * H, dV=dqkv[:, 2 * H:], lddv=3 * H, delta=delta,
-                           dbq=None if gated else gb[0:H], dbk=None if gated else gb[H:2 * H], dbv=gb[2 * H:], dropout=adrop,
-                           o_b16=self._extra(ctxb, ctx))
+                           dbq=None if gated else gb[0:H], dbk=None if gated else gb[H:2 * H], dbv=gb[2 * H:], dropout=adrop)
             if gated:
                 dz32 = self.scratch(tag + ".dz32", (B, 2 * H), F32)
                 dz16 = self.scratch(tag + ".dz16", (B, 2 * H), BF16)
-                self.emit(self.lib.vb_gate_scale_bwd, dqkv.data_ptr(), 3 * H, qkv.data_ptr(), self._ptr(qkvl), 3 * H, z.data_ptr(), dz32.data_ptr(),
-                          dz16.data_ptr(), B, N, 2 * H, self.op_fp16)
+                self.emit(self.lib.vb_gate_scale_bwd, dqkv.data_ptr(), 3 * H, qkv.hi.data_ptr(), self._ptr(qkv.lo), 3 * H, z.data_ptr(), dz32.data_ptr(),
+                          dz16.data_ptr(), B, N, 2 * H, qkv.fp16)
                 self.colsum(dqkv, 3 * H, gb[0:2 * H], M, 2 * H)
-                self.linear_wgrad(dz16, 2 * H, dz32, 2 * H, pool.bw, pool.H, B, 2 * H, pool.H, prefix + ".self.dy")
-                self.dgrad_into(pool, dz16, 2 * H, ps.w16b(prefix + ".self.dy.weight"), B, 2 * H, pool.H)
-            self.linear_wgrad(dqkv, 3 * H, None, 0, x.bw, H, M, 3 * H, H, prefix + ".self.qkv")
-            self.dgrad_into(x, dqkv, 3 * H, ps.w16b(prefix + ".self.qkv.weight"), M, 3 * H, H, extra32=dy32)
+                self.linear_wgrad(dz16, 2 * H, dz32, 2 * H, pool.op.bw, pool.H, B, 2 * H, pool.H, prefix + ".self.dy")
+                self.dgrad_into(pool, dz16, 2 * H, ps.w(prefix + ".self.dy.weight").bw, B, 2 * H, pool.H)
+            self.linear_wgrad(dqkv, 3 * H, None, 0, x.op.bw, H, M, 3 * H, H, prefix + ".self.qkv")
+            self.dgrad_into(x, dqkv, 3 * H, ps.w(prefix + ".self.qkv.weight").bw, M, 3 * H, H, extra32=dy32)
         self.push_bwd(bwd)
         return out
 
@@ -626,42 +660,33 @@ class Plan:
         Hb, nh = c.bi_hidden_size, c.bi_num_attention_heads
         D = Hb // nh
         Mv, Mt, Hv, Ht, Nv, Nt = v.M, t.M, v.H, t.H, self.Nv, self.Nt
-        qkv1, qkv1l, _ = self.buf16((Mv, 3 * Hb), bw=False)
-        qkv2, qkv2l, _ = self.buf16((Mt, 3 * Hb), bw=False)
+        qkv1 = self.buf16((Mv, 3 * Hb), bw=False)
+        qkv2 = self.buf16((Mt, 3 * Hb), bw=False)
         with self.on(1):
-            self.gemm(Mv, 3 * Hb, Hv, v.b16, Hv, ps.w16(p + ".biattention.qkv1.weight"), Hv, bias=ps.p(p + ".biattention.qkv1.bias"), out_bf16=qkv1, ld_ob=3 * Hb,
-                      a_lo=v.lo, b_lo=ps.w16lo(p + ".biattention.qkv1.weight"), out_lo=qkv1l)
-        self.gemm(Mt, 3 * Hb, Ht, t.b16, Ht, ps.w16(p + ".biattention.qkv2.weight"), Ht, bias=ps.p(p + ".biattention.qkv2.bias"), out_bf16=qkv2, ld_ob=3 * Hb,
-                  a_lo=t.lo, b_lo=ps.w16lo(p + ".biattention.qkv2.weight"), out_lo=qkv2l)
+            self.gemm(Mv, 3 * Hb, Hv, v.op, Hv, ps.w(p + ".biattention.qkv1.weight"), Hv, bias=ps.p(p + ".biattention.qkv1.bias"), out_bf16=qkv1, ld_ob=3 * Hb)
+        self.gemm(Mt, 3 * Hb, Ht, t.op, Ht, ps.w(p + ".biattention.qkv2.weight"), Ht, bias=ps.p(p + ".biattention.qkv2.bias"), out_bf16=qkv2, ld_ob=3 * Hb)
         self.sync_streams()      # each direction needs the other stream's keys / values
-        q1, k1, v1 = qkv1[:, 0:Hb], qkv1[:, Hb:2 * Hb], qkv1[:, 2 * Hb:]
-        q2, k2, v2 = qkv2[:, 0:Hb], qkv2[:, Hb:2 * Hb], qkv2[:, 2 * Hb:]
-        ctx1, ctx1l, ctx1b = self.buf16((Mt, Hb)); lse1 = self.buf((B, nh, Nt), F32)   # text queries over vision keys/values
-        ctx2, ctx2l, ctx2b = self.buf16((Mv, Hb)); lse2 = self.buf((B, nh, Nv), F32)   # vision queries over text keys/values
+        q1, k1, v1 = qkv1.cols(0, Hb), qkv1.cols(Hb, 2 * Hb), qkv1.cols(2 * Hb, 3 * Hb)
+        q2, k2, v2 = qkv2.cols(0, Hb), qkv2.cols(Hb, 2 * Hb), qkv2.cols(2 * Hb, 3 * Hb)
+        ctx1 = self.buf16((Mt, Hb)); lse1 = self.buf((B, nh, Nt), F32)   # text queries over vision keys/values
+        ctx2 = self.buf16((Mv, Hb)); lse2 = self.buf((B, nh, Nv), F32)   # vision queries over text keys/values
         L3 = 3 * Hb
-        if self.split:
-            q1l, k1l, v1l = qkv1l[:, 0:Hb], qkv1l[:, Hb:2 * Hb], qkv1l[:, 2 * Hb:]
-            q2l, k2l, v2l = qkv2l[:, 0:Hb], qkv2l[:, Hb:2 * Hb], qkv2l[:, 2 * Hb:]
-        else:
-            q1l = k1l = v1l = q2l = k2l = v2l = None
         # dropout1 acts on attention_probs1 (text queries over regions), dropout2 on attention_probs2 (vilbert.py:730, 738, 778, 800)
         adrop1 = self.drop(p + ".biattention.dropout1", c.v_attention_probs_dropout_prob)
         adrop2 = self.drop(p + ".biattention.dropout2", c.attention_probs_dropout_prob)
-        self.attention(False, B, nh, Nt, Nv, D, q2, L3, k1, L3, v1, L3, self.mask_v, ctx1, Hb, lse1, dropout=adrop1,
-                       q_lo=q2l, k_lo=k1l, v_lo=v1l, o_lo=ctx1l, o_b16=self._extra(ctx1b, ctx1))
+        self.attention(False, B, nh, Nt, Nv, D, q2, L3, k1, L3, v1, L3, self.mask_v, ctx1, Hb, lse1, dropout=adrop1)
         a1 = self._last_attn if self.viz else None
         with self.on(1):
-            self.attention(False, B, nh, Nv, Nt, D, q1, L3, k2, L3, v2, L3, self.mask_t, ctx2, Hb, lse2, dropout=adrop2,
-                           q_lo=q1l, k_lo=k2l, v_lo=v2l, o_lo=ctx2l, o_b16=self._extra(ctx2b, ctx2))
+            self.attention(False, B, nh, Nv, Nt, D, q1, L3, k2, L3, v2, L3, self.mask_t, ctx2, Hb, lse2, dropout=adrop2)
             a2 = self._last_attn if self.viz else None
         if self.viz:
             self.attn_c.append((a1, a2))
         # biOutput: ctx2 -> vision stream (dense1 / LayerNorm1), ctx1 -> text stream (dense2 / LayerNorm2) (:890-892)
         with self.on(1):
             v1o, v1_bwd = self.dense_res_ln(ctx2, Hb, v, p + ".biOutput.dense1", p + ".biOutput.LayerNorm1", "c.v.bo",
-                                            drop=self.drop(p + ".biOutput.dropout1", c.v_hidden_dropout_prob), a_lo=ctx2l, a_bw=ctx2b)
+                                            drop=self.drop(p + ".biOutput.dropout1", c.v_hidden_dropout_prob))
         t1o, t1_bwd = self.dense_res_ln(ctx1, Hb, t, p + ".biOutput.dense2", p + ".biOutput.LayerNorm2", "c.t.bo",
-                                        drop=self.drop(p + ".biOutput.dropout2", c.hidden_dropout_prob), a_lo=ctx1l, a_bw=ctx1b)
+                                        drop=self.drop(p + ".biOutput.dropout2", c.hidden_dropout_prob))
 
         def bwd():
             if not (v1o.gw or t1o.gw):
@@ -678,21 +703,21 @@ class Plan:
             dctx1 = self.scratch("c.dctx1", (Mt, Hb), BF16)
             dyv16, dyv32 = rv
             dyt16, dyt32 = rt
-            self.gemm(Mv, Hb, Hv, dyv16, Hv, ps.w16b(p + ".biOutput.dense1.weight"), Hb, b_mn=1, out_bf16=dctx2, ld_ob=Hb)
-            self.gemm(Mt, Hb, Ht, dyt16, Ht, ps.w16b(p + ".biOutput.dense2.weight"), Hb, b_mn=1, out_bf16=dctx1, ld_ob=Hb)
+            self.gemm(Mv, Hb, Hv, dyv16, Hv, ps.w(p + ".biOutput.dense1.weight").bw, Hb, b_mn=1, out_bf16=dctx2, ld_ob=Hb)
+            self.gemm(Mt, Hb, Ht, dyt16, Ht, ps.w(p + ".biOutput.dense2.weight").bw, Hb, b_mn=1, out_bf16=dctx1, ld_ob=Hb)
             gb1, gb2 = ps.g(p + ".biattention.qkv1.bias"), ps.g(p + ".biattention.qkv2.bias")
             d1 = self.scratch("c.delta1", (B, nh, Nt), F32)
             d2 = self.scratch("c.delta2", (B, nh, Nv), F32)
             self.attention(True, B, nh, Nt, Nv, D, q2, L3, k1, L3, v1, L3, self.mask_v, ctx1, Hb, lse1, dO=dctx1, lddo=Hb,
                            dQ=dqkv2[:, 0:Hb], lddq=L3, dK=dqkv1[:, Hb:2 * Hb], lddk=L3, dV=dqkv1[:, 2 * Hb:], lddv=L3, delta=d1,
-                           dbq=gb2[0:Hb], dbk=gb1[Hb:2 * Hb], dbv=gb1[2 * Hb:], dropout=adrop1, o_b16=self._extra(ctx1b, ctx1))
+                           dbq=gb2[0:Hb], dbk=gb1[Hb:2 * Hb], dbv=gb1[2 * Hb:], dropout=adrop1)
             self.attention(True, B, nh, Nv, Nt, D, q1, L3, k2, L3, v2, L3, self.mask_t, ctx2, Hb, lse2, dO=dctx2, lddo=Hb,
                            dQ=dqkv1[:, 0:Hb], lddq=L3, dK=dqkv2[:, Hb:2 * Hb], lddk=L3, dV=dqkv2[:, 2 * Hb:], lddv=L3, delta=d2,
-                           dbq=gb1[0:Hb], dbk=gb2[Hb:2 * Hb], dbv=gb2[2 * Hb:], dropout=adrop2, o_b16=self._extra(ctx2b, ctx2))
-            self.linear_wgrad(dqkv1, L3, None, 0, v.bw, Hv, Mv, L3, Hv, p + ".biattention.qkv1")
-            self.linear_wgrad(dqkv2, L3, None, 0, t.bw, Ht, Mt, L3, Ht, p + ".biattention.qkv2")
-            self.dgrad_into(v, dqkv1, L3, ps.w16b(p + ".biattention.qkv1.weight"), Mv, L3, Hv, extra32=dyv32)
-            self.dgrad_into(t, dqkv2, L3, ps.w16b(p + ".biattention.qkv2.weight"), Mt, L3, Ht, extra32=dyt32)
+                           dbq=gb1[0:Hb], dbk=gb2[Hb:2 * Hb], dbv=gb2[2 * Hb:], dropout=adrop2)
+            self.linear_wgrad(dqkv1, L3, None, 0, v.op.bw, Hv, Mv, L3, Hv, p + ".biattention.qkv1")
+            self.linear_wgrad(dqkv2, L3, None, 0, t.op.bw, Ht, Mt, L3, Ht, p + ".biattention.qkv2")
+            self.dgrad_into(v, dqkv1, L3, ps.w(p + ".biattention.qkv1.weight").bw, Mv, L3, Hv, extra32=dyv32)
+            self.dgrad_into(t, dqkv2, L3, ps.w(p + ".biattention.qkv2.weight").bw, Mt, L3, Ht, extra32=dyt32)
         # the cross-modal backward touches both streams' tensors: it runs on the main stream between two barriers
         self._bwd_emitters.append(None)
         self.push_bwd(bwd)
@@ -708,11 +733,10 @@ class Plan:
         """FAST_MODE: t [1*Nt, H] -> [B*Nt, H] (fp32 values and operand copies), and the text mask [1, Nt] -> [B, Nt]."""
         B, M1, H = self.B, t.M, t.H
         f32 = self.buf((B * M1, H), F32)
-        b16, lo, _ = self.buf16((B * M1, H), bw=False)
-        self.emit(self.lib.vb_broadcast_rows, t.f32.data_ptr(), f32.data_ptr(), M1 * H * 4, B)
-        self.emit(self.lib.vb_broadcast_rows, t.b16.data_ptr(), b16.data_ptr(), M1 * H * 2, B)
-        if lo is not None:
-            self.emit(self.lib.vb_broadcast_rows, t.lo.data_ptr(), lo.data_ptr(), M1 * H * 2, B)
+        op = self.buf16((B * M1, H), bw=False)      # FAST_MODE is inference only: no backward copy
+        for src, dst in ((t.f32, f32), (t.op.hi, op.hi), (t.op.lo, op.lo)):
+            if dst is not None:
+                self.emit(self.lib.vb_broadcast_rows, src.data_ptr(), dst.data_ptr(), M1 * H * dst.element_size(), B)
         nt4 = (self.Nt * 4 + 15) // 16 * 16           # the mask row is padded to 16 bytes for the broadcast kernel
         if nt4 == self.Nt * 4:
             m = self.buf((B, self.Nt), F32)
@@ -721,7 +745,7 @@ class Plan:
             m = self.mask_t.new_empty((B, self.Nt)); self._keep.append(m)
             self.emit(self.lib.vb_mask_to_additive, self.in_amask_b.data_ptr(), m.data_ptr(), B, self.Nt_in, 1 if self.has_task else 0)
         self.mask_t = m
-        return Act(f32, b16, B * M1, H, lo=lo)
+        return Act(f32, op, B * M1, H)
 
     def expand_pairs(self, t, v):
         """in_batch_pairs (vilbert.py:1008-1040): sample p = i * b + j of the expanded batch pairs text i with image j —
@@ -733,14 +757,15 @@ class Plan:
         for act, N, is_text in ((t, self.Nt, True), (v, self.Nv, False)):
             n = N * act.H
             f32 = self.buf((b * b * N, act.H), F32)
-            b16, lo, bw = self.buf16((b * b * N, act.H))
-            bufs = [(act.f32, f32, 4), (act.b16, b16, 2)] + ([(act.lo, lo, 2)] if lo is not None else []) + ([(act.bw, bw, 2)] if bw is not b16 else [])
-            for src, dst, sz in bufs:
+            op = self.buf16((b * b * N, act.H))
+            for src, dst in zip((act.f32, act.op.hi, act.op.lo, act.op.extra_bw), (f32, op.hi, op.lo, op.extra_bw)):
+                if dst is None:
+                    continue
                 if is_text:
-                    self.emit(lib.vb_repeat_rows, src.data_ptr(), dst.data_ptr(), n * sz, b, b)
+                    self.emit(lib.vb_repeat_rows, src.data_ptr(), dst.data_ptr(), n * dst.element_size(), b, b)
                 else:
-                    self.emit(lib.vb_broadcast_rows, src.data_ptr(), dst.data_ptr(), b * n * sz, b)
-            out = Act(f32, b16, b * b * N, act.H, lo=lo, bw=bw)
+                    self.emit(lib.vb_broadcast_rows, src.data_ptr(), dst.data_ptr(), b * n * dst.element_size(), b)
+            out = Act(f32, op, b * b * N, act.H)
             outs.append(out)
 
             def bwd(act=act, out=out, n=n, is_text=is_text):
@@ -779,10 +804,9 @@ class Plan:
         barrier before the image layers that read it (their backward accumulates d pool, mirrored barrier, then this backward)."""
         B, Ht, lib = self.B, t.H, self.lib
         p32 = self.buf((B, Ht), F32)
-        p16, plo, pbw = self.buf16((B, Ht))
-        self.emit(lib.vb_masked_mean_fwd, t.f32.data_ptr(), self.mask_t.data_ptr(), p32.data_ptr(), p16.data_ptr(), self._ptr(plo),
-                  self._ptr(self._extra(pbw, p16)), self.op_fp16, B, self.Nt, Ht)
-        pool = Act(p32, p16, B, Ht, lo=plo, bw=pbw)
+        p = self.buf16((B, Ht))
+        self.emit(lib.vb_masked_mean_fwd, t.f32.data_ptr(), self.mask_t.data_ptr(), p32.data_ptr(), *p.ptrs(), p.fp16, B, self.Nt, Ht)
+        pool = Act(p32, p, B, Ht)
         mask = self.mask_t
 
         def bwd():
@@ -832,8 +856,8 @@ class Plan:
                   ps.p(e + ".position_embeddings.weight").data_ptr(), ps.p(e + ".token_type_embeddings.weight").data_ptr(),
                   ps.p(e + ".task_embeddings.weight").data_ptr() if self.has_task else None, xe.data_ptr(), Bt, self.Nt_in, Ht)
         tdrop = self.drop(e + ".dropout", c.hidden_dropout_prob)
-        t32, t16, tmean, trstd, tlo, tbw = self.ln_fwd(xe, ps.p(e + ".LayerNorm.weight"), ps.p(e + ".LayerNorm.bias"), Mt, Ht, out_drop=tdrop)
-        t = Act(t32, t16, Mt, Ht, lo=tlo, bw=tbw)
+        t32, top, tmean, trstd = self.ln_fwd(xe, ps.p(e + ".LayerNorm.weight"), ps.p(e + ".LayerNorm.bias"), Mt, Ht, out_drop=tdrop)
+        t = Act(t32, top, Mt, Ht)
 
         def bwd_text():
             if t.gw:
@@ -848,18 +872,18 @@ class Plan:
         # image: region features fp32 -> bf16 ingest, 2048 -> Hv GEMM with the 5 -> Hv box projection as residual, LayerNorm (:1421-1432)
         ve = "bert.v_embeddings"
         with self.on(1):
-            feat16, featl, featb = self.buf16((Mv, Fv))
-            self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), feat16.data_ptr(), Mv * Fv, self.op_fp16, self._ptr(featl),
-                      self._ptr(self._extra(featb, feat16)))
+            feat = self.buf16((Mv, Fv))
+            hi, lo, bw = feat.ptrs()
+            self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), hi, Mv * Fv, feat.fp16, lo, bw)
             locp = self.buf((Mv, Hv), F32)
             self.emit(lib.vb_loc_proj_fwd, self.in_loc.data_ptr(), ps.p(ve + ".image_location_embeddings.weight").data_ptr(),
                       ps.p(ve + ".image_location_embeddings.bias").data_ptr(), locp.data_ptr(), Mv, Hv)
             yv = self.buf((Mv, Hv), F32)
-            self.gemm(Mv, Hv, Fv, feat16, Fv, ps.w16(ve + ".image_embeddings.weight"), Fv, bias=ps.p(ve + ".image_embeddings.bias"),
-                      residual=locp, ld_res=Hv, out_f32=yv, ld_of=Hv, a_lo=featl, b_lo=ps.w16lo(ve + ".image_embeddings.weight"))
+            self.gemm(Mv, Hv, Fv, feat, Fv, ps.w(ve + ".image_embeddings.weight"), Fv, bias=ps.p(ve + ".image_embeddings.bias"),
+                      residual=locp, ld_res=Hv, out_f32=yv, ld_of=Hv)
             vdrop = self.drop(ve + ".dropout", c.hidden_dropout_prob)     # BertImageEmbeddings uses hidden_dropout_prob (vilbert.py:1419)
-            v32, v16, vmean, vrstd, vlo, vbw = self.ln_fwd(yv, ps.p(ve + ".LayerNorm.weight"), ps.p(ve + ".LayerNorm.bias"), Mv, Hv, out_drop=vdrop)
-            v = Act(v32, v16, Mv, Hv, lo=vlo, bw=vbw)
+            v32, vop, vmean, vrstd = self.ln_fwd(yv, ps.p(ve + ".LayerNorm.weight"), ps.p(ve + ".LayerNorm.bias"), Mv, Hv, out_drop=vdrop)
+            v = Act(v32, vop, Mv, Hv)
 
             def bwd_image():
                 if v.gw:
@@ -867,7 +891,7 @@ class Plan:
                     dyv16 = self.scratch("emb.dyv16", (Mv, Hv), BF16)
                     self.ln_bwd(v.g32, yv, ps.p(ve + ".LayerNorm.weight"), vmean, vrstd, dyv32, dyv16, Mv, Hv, ps.g(ve + ".LayerNorm.weight"), ps.g(ve + ".LayerNorm.bias"),
                                 gbias=ps.g(ve + ".image_embeddings.bias"), out_drop=vdrop)
-                    self.linear_wgrad(dyv16, Hv, None, 0, featb, Fv, Mv, Hv, Fv, ve + ".image_embeddings")
+                    self.linear_wgrad(dyv16, Hv, None, 0, feat.bw, Fv, Mv, Hv, Fv, ve + ".image_embeddings")
                     self.emit(lib.vb_loc_proj_bwd, dyv32.data_ptr(), self.in_loc.data_ptr(), ps.g(ve + ".image_location_embeddings.weight").data_ptr(),
                               ps.g(ve + ".image_location_embeddings.bias").data_ptr(), Mv, Hv)
             self.push_bwd(bwd_image)
@@ -878,10 +902,10 @@ class Plan:
         """Linear + ReLU on token 0 (vilbert.py:1116-1122, 1131-1137); A is read with row pitch N*H."""
         ps, B, H, Hb = self.ps, self.B, seq.H, self.cfg.bi_hidden_size
         p32 = self.buf((B, Hb), F32)
-        p16, plo, _ = self.buf16((B, Hb), bw=False)
-        self.gemm(B, Hb, H, seq.b16, N * H, ps.w16(wname + ".weight"), H, bias=ps.p(wname + ".bias"), act=L.VB_ACT_RELU, out_f32=p32, ld_of=Hb,
-                  out_bf16=p16, ld_ob=Hb, a_lo=seq.lo, b_lo=ps.w16lo(wname + ".weight"), out_lo=plo)
-        pooled = Act(p32, p16, B, Hb, lo=plo)
+        p = self.buf16((B, Hb), bw=False)
+        self.gemm(B, Hb, H, seq.op, N * H, ps.w(wname + ".weight"), H, bias=ps.p(wname + ".bias"), act=L.VB_ACT_RELU, out_f32=p32, ld_of=Hb,
+                  out_bf16=p, ld_ob=Hb)
+        pooled = Act(p32, p, B, Hb)
 
         def bwd():
             if not pooled.gw:
@@ -889,13 +913,13 @@ class Plan:
             dpre = self.scratch("pool.dpre", (B, Hb), BF16)
             dpre32 = self.scratch("pool.dpre32", (B, Hb), F32)
             self.emit(self.lib.vb_relu_bwd, pooled.g32.data_ptr(), p32.data_ptr(), dpre.data_ptr(), dpre32.data_ptr(), B * Hb)
-            self.linear_wgrad(dpre, Hb, dpre32, Hb, seq.bw, N * H, B, Hb, H, wname)
+            self.linear_wgrad(dpre, Hb, dpre32, Hb, seq.op.bw, N * H, B, Hb, H, wname)
             g = self.grad_of(seq)
             if not seq.gw:
                 self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
                 seq.gw = True
             # rows b*N of the sequence gradient += dpre @ W
-            self.gemm(B, H, Hb, dpre, Hb, ps.w16b(wname + ".weight"), H, b_mn=1, residual=g, ld_res=N * H, out_f32=g, ld_of=N * H)
+            self.gemm(B, H, Hb, dpre, Hb, ps.w(wname + ".weight").bw, H, b_mn=1, residual=g, ld_res=N * H, out_f32=g, ld_of=N * H)
         self.push_bwd(bwd)
         return pooled
 
@@ -905,15 +929,14 @@ class Plan:
             self.gout[name] = self.buf(shape, F32, zero=True)
         return self.gout[name]
 
-    def big_head(self, name, x16, ld_x, x_act, M, K_in, N_out, wname, bias_name, w16=None, gw=None, w16lo=None, w16b=None):
+    def big_head(self, name, x, ld_x, M, K_in, N_out, wname, bias_name, w=None, gw=None):
         """Wide linear head (N_out in the thousands): logits = x W^T + b as fp32 [M, N_out]; backward from a
-        caller-supplied fp32 d(logits) (cast to a bf16 operand with an 8-padded row pitch)."""
+        caller-supplied fp32 d(logits) (cast to a bf16 operand with an 8-padded row pitch). w / gw: a weight and gradient
+        not named by `wname` (the decoder tied to the word embeddings)."""
         ps = self.ps
-        W16 = w16 if w16 is not None else ps.w16(wname + ".weight")
-        W16lo = w16lo if w16 is not None else ps.w16lo(wname + ".weight")
-        W16b = w16b if w16 is not None else ps.w16b(wname + ".weight")
+        W = w if w is not None else ps.w(wname + ".weight")
         logits = self.buf((M, N_out), F32)
-        self.gemm(M, N_out, K_in, x16, ld_x, W16, K_in, bias=ps.p(bias_name), out_f32=logits, ld_of=N_out, a_lo=x_act.lo, b_lo=W16lo)
+        self.gemm(M, N_out, K_in, x.op, ld_x, W, K_in, bias=ps.p(bias_name), out_f32=logits, ld_of=N_out)
         self.outputs[name] = logits
 
         def bwd():
@@ -927,8 +950,8 @@ class Plan:
                 dl16 = self.scratch("head.dl16." + name, (M, ldp), BF16)
                 self.emit(self.lib.vb_cast2d_f32_to_bf16, dl32.data_ptr(), N_out, dl16.data_ptr(), ldp, M, N_out, 1.0)
             self.colsum(dl32, N_out, ps.g(bias_name), M, N_out)
-            self.linear_wgrad(dl16, ldp, None, 0, x_act.bw, ld_x, M, N_out, K_in, wname, gw=gw)
-            return dl16, ldp, W16b
+            self.linear_wgrad(dl16, ldp, None, 0, x.op.bw, ld_x, M, N_out, K_in, wname, gw=gw)
+            return dl16, ldp, W.bw
         return bwd
 
     def lm_head_compact(self, ht, ht_bwd):
@@ -944,14 +967,14 @@ class Plan:
         self.loss_inputs["masked_lm_labels"] = labels
         idx, cnt, lab_c = self.buf((cap,), torch.int32), self.buf((1,), torch.int32, zero=True), self.buf((cap,), I64)
         self.emit(lib.vb_compact_rows, labels.data_ptr(), -1, M, cap, idx.data_ptr(), cnt.data_ptr(), lab_c.data_ptr())
-        hc, hclo, hcbw = self.buf16((cap, Ht))
-        self.emit(lib.vb_gather_rows16, ht.b16.data_ptr(), hc.data_ptr(), self._ptr(self._extra(ht.bw, ht.b16)), self._ptr(self._extra(hcbw, hc)),
+        hc = self.buf16((cap, Ht))
+        self.emit(lib.vb_gather_rows16, ht.op.hi.data_ptr(), hc.hi.data_ptr(), self._ptr(ht.op.extra_bw), self._ptr(hc.extra_bw),
                   idx.data_ptr(), cap, Ht)
-        if hclo is not None:
-            self.emit(lib.vb_gather_rows16, ht.lo.data_ptr(), hclo.data_ptr(), None, None, idx.data_ptr(), cap, Ht)
+        if hc.lo is not None:
+            self.emit(lib.vb_gather_rows16, ht.op.lo.data_ptr(), hc.lo.data_ptr(), None, None, idx.data_ptr(), cap, Ht)
         wn = "bert.embeddings.word_embeddings.weight"
         logits = self.buf((cap, V), F32)
-        self.gemm(cap, V, Ht, hc, Ht, ps.w16(wn), Ht, bias=ps.p("cls.predictions.bias"), out_f32=logits, ld_of=V, a_lo=hclo, b_lo=ps.w16lo(wn))
+        self.gemm(cap, V, Ht, hc, Ht, ps.w(wn), Ht, bias=ps.p("cls.predictions.bias"), out_f32=logits, ld_of=V)
         ldp = _pad8(V)
         self.lm_c = dict(cap=cap, idx=idx, count=cnt, labels=lab_c, logits=logits, dl32=self.buf((cap, V), F32),
                          dl16=self.buf((cap, ldp), BF16, zero=True), ldp=ldp)
@@ -959,11 +982,11 @@ class Plan:
         def bwd():
             lc = self.lm_c
             self.colsum(lc["dl32"], V, ps.g("cls.predictions.bias"), cap, V)
-            self.linear_wgrad(lc["dl16"], ldp, None, 0, hcbw, Ht, cap, V, Ht, None, gw=ps.g(wn))
+            self.linear_wgrad(lc["dl16"], ldp, None, 0, hc.bw, Ht, cap, V, Ht, None, gw=ps.g(wn))
             if ht.frozen:
                 return
             gc = self.scratch("lm.gc", (cap, Ht), F32)
-            self.gemm(cap, Ht, V, lc["dl16"], ldp, ps.w16b(wn), Ht, b_mn=1, out_f32=gc, ld_of=Ht)
+            self.gemm(cap, Ht, V, lc["dl16"], ldp, ps.w(wn).bw, Ht, b_mn=1, out_f32=gc, ld_of=Ht)
             g = self.grad_of(ht)
             self.emit(lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
             self.emit(lib.vb_scatter_rows_f32, gc.data_ptr(), g.data_ptr(), idx.data_ptr(), cap, Ht, cnt.data_ptr(), self.loss.data_ptr())
@@ -977,15 +1000,15 @@ class Plan:
 
     def transform(self, x, wdense, lnname, tag):
         """Linear -> GELU -> LayerNorm (BertPredictionHeadTransform / BertImgPredictionHeadTransform / the first three
-        stages of SimpleClassifier; vilbert.py:1152-1156, 1172-1176, 1714-1718). x: Act or (b16, M, K) for a plain operand."""
+        stages of SimpleClassifier; vilbert.py:1152-1156, 1172-1176, 1714-1718)."""
         ps = self.ps
         M, K = x.M, x.H
         Hh = ps.p(wdense + ".weight").shape[0]
         g32, pre16 = self.buf((M, Hh), F32), self.buf((M, Hh), BF16)
-        self.gemm(M, Hh, K, x.b16, K, ps.w16(wdense + ".weight"), K, bias=ps.p(wdense + ".bias"), act=L.VB_ACT_GELU, out_f32=g32, ld_of=Hh,
-                  out_pre=pre16, ld_op=Hh, a_lo=x.lo, b_lo=ps.w16lo(wdense + ".weight"))
-        _, h16, mean, rstd, hlo, hbw = self.ln_fwd(g32, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, Hh, want_f32=False)
-        hn = Act(None, h16, M, Hh, lo=hlo, bw=hbw)
+        self.gemm(M, Hh, K, x.op, K, ps.w(wdense + ".weight"), K, bias=ps.p(wdense + ".bias"), act=L.VB_ACT_GELU, out_f32=g32, ld_of=Hh,
+                  out_pre=pre16, ld_op=Hh)
+        _, h, mean, rstd = self.ln_fwd(g32, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, Hh, want_f32=False)
+        hn = Act(None, h, M, Hh)
 
         def bwd():
             if not hn.gw:
@@ -993,8 +1016,8 @@ class Plan:
             dpre16 = self.scratch(tag + ".dpre16", (M, Hh), BF16)
             self.ln_bwd(hn.g32, g32, ps.p(lnname + ".weight"), mean, rstd, None, dpre16, M, Hh, ps.g(lnname + ".weight"), ps.g(lnname + ".bias"), pre=pre16,
                         gbias=ps.g(wdense + ".bias"))
-            self.linear_wgrad(dpre16, Hh, None, 0, x.bw, K, M, Hh, K, wdense)
-            self.dgrad_into(x, dpre16, Hh, ps.w16b(wdense + ".weight"), M, Hh, K)
+            self.linear_wgrad(dpre16, Hh, None, 0, x.op.bw, K, M, Hh, K, wdense)
+            self.dgrad_into(x, dpre16, Hh, ps.w(wdense + ".weight").bw, M, Hh, K)
         return hn, bwd
 
     def small_head(self, name, x, wname, N_out, addend=None, x32=None, M=None, K=None, in_drop=None):
@@ -1026,10 +1049,11 @@ class Plan:
         mul = 1 if c.fusion_method == "mul" else 0
         def fuse(drop):
             f32 = self.buf((B, Hb), F32)
-            f16, flo, fbw = self.buf16((B, Hb))
-            self.emit(lib.vb_fuse_pooled_fwd, pooled_t.f32.data_ptr(), pooled_v.f32.data_ptr(), f32.data_ptr(), f16.data_ptr(), B * Hb, mul, self._ref(drop),
-                      self.op_fp16, self._ptr(flo), self._ptr(self._extra(fbw, f16)))
-            act = Act(f32, f16, B, Hb, lo=flo, bw=fbw)
+            f = self.buf16((B, Hb))
+            hi, lo, bw = f.ptrs()
+            self.emit(lib.vb_fuse_pooled_fwd, pooled_t.f32.data_ptr(), pooled_v.f32.data_ptr(), f32.data_ptr(), hi, B * Hb, mul, self._ref(drop),
+                      f.fp16, lo, bw)
+            act = Act(f32, f, B, Hb)
 
             def fuse_bwd():
                 if not act.gw:
@@ -1052,7 +1076,6 @@ class Plan:
             fused_cls = fuse(cls_drop) if (cls_drop is not None or fused is None) else fused
         else:
             fused_cls = None
-        f32, f16, f16lo, f16bw = (fused.f32, fused.b16, fused.lo, fused.bw) if fused is not None else (None, None, None, None)
 
         # --- cls: masked-LM head (decoder tied to the word embeddings), image-region head, alignment head
         ht, ht_bwd = self.transform(seq_t, "cls.predictions.transform.dense", "cls.predictions.transform.LayerNorm", "lm.tr")
@@ -1062,11 +1085,10 @@ class Plan:
             lm_bwd = None
             lm_compact_bwd = self.lm_head_compact(ht, ht_bwd)
         else:
-            lm_bwd = self.big_head("linguisic_prediction", ht.b16, Ht, ht, B * Nt, Ht, c.vocab_size, None, "cls.predictions.bias",
-                                   w16=ps.w16("bert.embeddings.word_embeddings.weight"), gw=ps.g("bert.embeddings.word_embeddings.weight"),
-                                   w16lo=ps.w16lo("bert.embeddings.word_embeddings.weight"), w16b=ps.w16b("bert.embeddings.word_embeddings.weight"))
+            lm_bwd = self.big_head("linguisic_prediction", ht, Ht, B * Nt, Ht, c.vocab_size, None, "cls.predictions.bias",
+                                   w=ps.w("bert.embeddings.word_embeddings.weight"), gw=ps.g("bert.embeddings.word_embeddings.weight"))
         hv, hv_bwd = self.transform(seq_v, "cls.imagePredictions.transform.dense", "cls.imagePredictions.transform.LayerNorm", "im.tr")
-        im_bwd = self.big_head("vision_prediction", hv.b16, Hv, hv, B * Nv, Hv, c.v_target_size, "cls.imagePredictions.decoder",
+        im_bwd = self.big_head("vision_prediction", hv, Hv, B * Nv, Hv, c.v_target_size, "cls.imagePredictions.decoder",
                                "cls.imagePredictions.decoder.bias")
 
         def wide_bwd(head_bwd, hn, tr_bwd, K, N_out):
@@ -1089,7 +1111,7 @@ class Plan:
             return
         if B % 2 == 0:
             # vil_binary_prediction pairs consecutive samples: pooled.view(-1, 2*Hb) (:1686-1689)
-            pair = Act(f32.view(B // 2, 2 * Hb), f16.view(B // 2, 2 * Hb), B // 2, 2 * Hb, lo=f16lo.view(B // 2, 2 * Hb) if f16lo is not None else None, bw=f16bw.view(B // 2, 2 * Hb))
+            pair = Act(fused.f32.view(B // 2, 2 * Hb), fused.op.view(B // 2, 2 * Hb), B // 2, 2 * Hb)
             hb, hb_bwd = self.transform(pair, "vil_binary_prediction.logit_fc.0", "vil_binary_prediction.logit_fc.2", "bin.tr")
             # LayerNorm output is needed in fp32 for the 2-way linear: recompute it from the bf16 copy is lossy, so run the small
             # linear on an fp32 LayerNorm output
@@ -1113,7 +1135,7 @@ class Plan:
 
         for nm, n_out in (("vil_prediction", 3129), ("vil_prediction_gqa", 1533)):
             hh, hh_bwd = self.transform(fused, nm + ".logit_fc.0", nm + ".logit_fc.2", nm + ".tr")
-            head_bwd = self.big_head(nm, hh.b16, 2 * Hb, hh, B, 2 * Hb, n_out, nm + ".logit_fc.3", nm + ".logit_fc.3.bias")
+            head_bwd = self.big_head(nm, hh, 2 * Hb, B, 2 * Hb, n_out, nm + ".logit_fc.3", nm + ".logit_fc.3.bias")
             self.push_bwd(wide_bwd(head_bwd, hh, hh_bwd, 2 * Hb, n_out))
         self.small_head("vil_logit", fused, "vil_logit", 1)
         self.small_head("vil_tri_prediction", fused, "vil_tri_prediction", 3)
@@ -1402,16 +1424,12 @@ class Plan:
         first_c = [off for name, (off, _) in ps.entries.items() if ".c_layer." in name]
         split = min(first_c) if (self.two_streams and first_c) else n
         if refresh_weights and split > 0:
-            sb = ps.shadow_b if ps.shadow_b is not ps.shadow else None
-            self.prologue.append((lib.vb_cast_f32_to_bf16, (ps.flat.data_ptr(), ps.shadow.data_ptr(), split, self.op_fp16,
-                                                            ps.shadow_lo.data_ptr() if self.split else None, sb.data_ptr() if sb is not None else None), 0))
+            self.prologue.append((lib.vb_cast_f32_to_bf16, ps.cast_args(0, split), 0))
         tail = []
         if zero_grad:
             tail.append((lib.vb_memset_zero, (ps.grad.data_ptr(), ps.grad.numel() * 4), 1 if self.two_streams else 0))
         if refresh_weights and split < n:
-            tail.append((lib.vb_cast_f32_to_bf16, (ps.flat.data_ptr() + 4 * split, ps.shadow.data_ptr() + 2 * split, n - split, self.op_fp16,
-                                                   ps.shadow_lo.data_ptr() + 2 * split if self.split else None,
-                                                   ps.shadow_b.data_ptr() + 2 * split if ps.shadow_b is not ps.shadow else None), 1))
+            tail.append((lib.vb_cast_f32_to_bf16, ps.cast_args(split, n - split), 1))
         if self.two_streams:
             self.prologue += [(None, (), 0)] + tail       # barrier: the vision stream starts after the main-stream part
         else:

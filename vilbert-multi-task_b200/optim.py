@@ -113,10 +113,8 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
     def _buffer_args(self):
         """The leading arguments of vb_adamw_step / vb_radam_step: buffers, 16-bit copies, chunk table and group table."""
         ps = self.engine.ps
-        return (ps.flat.data_ptr(), ps.grad.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
-                ps.shadow.data_ptr(), ps.shadow_lo.data_ptr() if ps.split else None,
-                ps.shadow_b.data_ptr() if ps.shadow_b is not ps.shadow else None, 1 if ps.op_dtype == torch.float16 else 0,
-                self._chunk_start.data_ptr(), self._chunk_count.data_ptr(), self._chunk_group.data_ptr(), self.n_chunks,
+        return (ps.flat.data_ptr(), ps.grad.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), *ps.shadows.ptrs(),
+                ps.shadows.fp16, self._chunk_start.data_ptr(), self._chunk_count.data_ptr(), self._chunk_group.data_ptr(), self.n_chunks,
                 self._groups_dev.data_ptr())
 
     def _after_step(self):
