@@ -267,6 +267,39 @@ vb_status vb_ce_loss(const float* logits, int64_t ld_logits, const int64_t* labe
                      float* dlogits_f32, int64_t ld_d32, void* dlogits_bf16, int64_t ld_d16, int32_t rows, int32_t cols,
                      float grad_scale, int32_t accumulate_loss, void* stream);
 
+/* Task objectives and scores of the 12-in-1 task table (task_utils.py:31-376, 618-623), used by the forward-placed objectives of
+ * the engine's plans (vilbert_b200.tasks).
+ *
+ * vb_bce_gather_loss: BCE-with-logits over an optional column gather, V-logit-mc (vision_logit[:, 101:].gather(1, ids), then
+ * BCE mean * C, task_utils.py:352-360) and the soft-target binary / tri heads (BCE mean, :362-374):
+ *   x[r,c] = logits[r * ld_logits + col_off + (ids ? ids[r*C + c] : c)],  t = target[r*C + c]  (f32 [rows, C])
+ *   *loss (+= when accumulate_loss) = loss_mul * mean_{r,c} (max(x,0) - x t + log1p(exp(-|x|)))
+ *   dlogits (f32 and/or bf16, `width` columns per row, ld_d32 / ld_d16) = d loss / d logits over the WHOLE row: 0 where nothing
+ *   was gathered; a column gathered by several choices gets the sum of their gradients, added in choice order (deterministic).
+ * One CTA per row with the row (width floats) and C gradients in shared memory (width*4 + C*8 <= 48 KiB). An id outside
+ * [0, width - col_off) reads nothing and makes the loss NaN. row_loss: f32 workspace [rows] (the per-row sums, then added in a
+ * fixed order by a second one-CTA launch: no atomics, the loss is bitwise reproducible).
+ *
+ * vb_task_score: batch score of one task type on the device, *score (+= when accumulate) = sum over rows of
+ *   VB_SCORE_SOFT       target[r, a]                    compute_score_with_logits(logits, target).sum()   (:618-623)
+ *   VB_SCORE_LABEL      a == labels[r]                  VL-logit: (argmax(vil_logit.view(B, options)) == target).sum()
+ *   VB_SCORE_THRESHOLD  target[r, a] > 0.5              V-logit: (target.gather(1, argmax over regions) > 0.5).sum()
+ *   VB_SCORE_CHOICE     a == argmax_c target[r, c]      V-logit-mc, a over the gathered logits (ids as above; an id out of
+ *                                                       range reads as NaN)
+ * where a = argmax_c logits[r * ld_logits + col_off + c] (or of the gathered logits) with torch.max's rules: a NaN is the maximum,
+ * the first index wins among equals. target rows have pitch ld_target. preds (int64 [rows], may be NULL) receives a. One CTA. */
+enum { VB_SCORE_SOFT = 0, VB_SCORE_LABEL = 1, VB_SCORE_THRESHOLD = 2, VB_SCORE_CHOICE = 3 };
+vb_status vb_bce_gather_loss(const float* logits, int64_t ld_logits, int32_t col_off, int32_t width, const int64_t* ids,
+                             const float* target, int32_t rows, int32_t C, float loss_mul, float* row_loss, float* loss,
+                             int32_t accumulate_loss, float* dlogits_f32, int64_t ld_d32, void* dlogits_bf16, int64_t ld_d16, void* stream);
+vb_status vb_task_score(int32_t mode, const float* logits, int64_t ld_logits, int32_t col_off, int32_t cols, const int64_t* ids,
+                        int32_t width, const float* target, int64_t ld_target, const int64_t* labels, int32_t rows, float* score,
+                        int32_t accumulate, int64_t* preds, void* stream);
+/* dst = src * (*scale), f32, scale read on the device: the backward of a forward-placed objective starts from the stored
+ * d loss / d head times d(total) / d loss (loss_scale[task] / gradient_accumulation_steps, train_tasks.py:247-251, 545-548)
+ * without a host synchronisation. */
+vb_status vb_scale_by_device(const float* src, float* dst, int64_t n, const float* scale, void* stream);
+
 /* Masked-region KL objective of BertForMultiModalPreTraining (visual_target == 0, vilbert.py:1506-1525):
  *   loss = sum_{b,r: label[b,r]==1} sum_c t_c (log t_c - log_softmax(scores[b, r+1, :])_c) / max(#(label == 1), 0)
  * scores f32 [B, Nv, C] (region 0 = the global feature is skipped, :1506), target f32 [B, Nv-1, C], label int64 [B, Nv-1].

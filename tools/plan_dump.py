@@ -20,8 +20,13 @@ NT, NV = 9, 11
 
 
 def cases(O, LOSS_HEADS):
-    """(name, config overrides, engine heads, B, plan kwargs) of the case matrix."""
+    """(name, config overrides, engine heads, B, plan kwargs[, Nv]) of the case matrix. A case the tree cannot build (an objective
+    kind or a plan option it does not have) is skipped with a note on stderr, so listings of two trees compare case by case."""
     train = dict(grad_outputs=O.HEAD_NAMES, train=True)
+
+    def obj(kind, **kw):
+        return dict(grad_outputs=LOSS_HEADS.get(kind, ()), loss=kind, train=True, **kw)
+    task = dict(score=True, loss_in_forward=True)
     return [
         ("heads_train", {}, "vl", 4, train),
         ("vqa_loss", {}, "vl", 4, dict(grad_outputs=("vil_prediction",), vqa_loss=True, train=True)),
@@ -33,6 +38,24 @@ def cases(O, LOSS_HEADS):
         ("fixed_t_layer", dict(fixed_t_layer=1), "vl", 4, train),
         ("pretraining", {}, "pretraining", 4, dict(grad_outputs=LOSS_HEADS["pretraining"], loss="pretraining", train=True)),
         ("odd_b3", {}, "vl", 3, train),
+        # the fine-tuning objectives, as emitted at the start of the backward
+        ("loss_gqa", {}, "vl", 4, obj("gqa")),
+        ("loss_vlogit_bce", {}, "vl", 4, obj("vlogit_bce")),
+        ("loss_logit_ce", {}, "vl", 4, obj("logit_ce")),
+        ("loss_binary_ce", {}, "vl", 4, obj("binary_ce")),
+        ("loss_tri_ce", {}, "vl", 4, obj("tri_ce")),
+        ("loss_vlogit_mc", {}, "vl", 4, obj("vlogit_mc", choices=4), 110),
+        ("loss_binary_bce", {}, "vl", 4, obj("binary_bce")),
+        ("loss_tri_bce", {}, "vl", 4, obj("tri_bce")),
+        # ... and placed at the end of the forward with the batch score (vilbert_b200.tasks)
+        ("task_vqa", {}, "vl", 4, obj("vqa", **task)),
+        ("task_gqa_eval", {}, "vl", 4, dict(loss="gqa", **task)),
+        ("task_logit_ce", {}, "vl", 4, obj("logit_ce", choices=2, **task)),
+        ("task_vlogit_bce", {}, "vl", 4, obj("vlogit_bce", **task)),
+        ("task_vlogit_mc", dict(task_specific_tokens=True), "vl", 4, obj("vlogit_mc", choices=6, **task), 110),
+        ("task_binary_bce", {}, "vl", 4, obj("binary_bce", **task)),
+        ("task_tri_bce", {}, "vl", 4, obj("tri_bce", **task)),
+        ("task_binary_ce_nscore", {}, "vl", 4, obj("binary_ce", loss_in_forward=True)),
     ]
 
 
@@ -119,12 +142,16 @@ def main():
     tiny = json.load(open(os.path.join(root, "tests", "golden", "tiny_b4.json")))["config"]
     out, n_plans, n_ops = [], 0, 0
     for prec in PRECISIONS:
-        for name, over, heads, B, kw in cases(O, LOSS_HEADS):
+        for name, over, heads, B, kw, *nv in cases(O, LOSS_HEADS):
             for arena in (False, True):
                 eng = Engine(BertConfig.from_dict(dict(tiny, **over)), "cpu", heads=heads, _build_only=True, precision=prec)
                 if arena:
                     eng.enable_activation_arena(ARENA_BYTES)
-                plan = eng.plan(B, NT, NV, **kw)
+                try:
+                    plan = eng.plan(B, NT, nv[0] if nv else NV, **kw)
+                except (TypeError, ValueError) as ex:
+                    print(f"plan_dump: {prec} {name} arena={int(arena)} skipped: {ex}", file=sys.stderr)
+                    continue
                 plan.enable_training_prologue()
                 n_ops += dump_plan(out, f"{prec} {name} arena={int(arena)}", plan)
                 n_plans += 1

@@ -14,6 +14,9 @@ def __getattr__(name):
     if name in ("BertModel", "VILBertForVLTasks", "BertForMultiModalPreTraining", "BertPreTrainedModel"):
         from . import modeling
         return getattr(modeling, name)
+    if name in ("ForwardModelsTrain", "ForwardModelsVal", "LoadLosses"):
+        from . import tasks
+        return getattr(tasks, name)
     if name in ("Engine", "Plan", "ParamStore"):
         from . import engine
         return getattr(engine, name)

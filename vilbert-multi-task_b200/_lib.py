@@ -10,6 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvilbert_b200.so")
 
 VB_ACT_NONE, VB_ACT_GELU, VB_ACT_RELU, VB_ACT_DGELU = 0, 1, 2, 3
+VB_SCORE_SOFT, VB_SCORE_LABEL, VB_SCORE_THRESHOLD, VB_SCORE_CHOICE = 0, 1, 2, 3
 
 
 class VBError(RuntimeError):
@@ -102,6 +103,9 @@ _SIGNATURES = {
     "vb_mask_to_additive": [_P, _P, _I32, _I32, _I32, _P],
     "vb_memset_zero": [_P, _I64, _P],
     "vb_ce_loss": [_P, _I64, _P, _I64, _P, _P, _I64, _P, _I64, _I32, _I32, _F, _I32, _P],
+    "vb_bce_gather_loss": [_P, _I64, _I32, _I32, _P, _P, _I32, _I32, _F, _P, _P, _I32, _P, _I64, _P, _I64, _P],
+    "vb_task_score": [_I32, _P, _I64, _I32, _I32, _P, _I32, _P, _I64, _P, _I32, _P, _I32, _P, _P],
+    "vb_scale_by_device": [_P, _P, _I64, _P, _P],
     "vb_kl_masked_loss": [_P, _P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _F, _I32, _P],
     "vb_masked_mean_fwd": [_P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
     "vb_masked_mean_bwd": [_P, _P, _P, _I32, _I32, _I32, _I32, _P],

@@ -204,6 +204,146 @@ __global__ void scatter_rows_f32_kernel(const float4* __restrict__ src, float4* 
   }
 }
 
+// ------------------------------------------------------------------------------------------ task objectives and scores (12-in-1)
+// BCE-with-logits over gathered columns (task_utils.py:352-374): for row r and choice c, x = logits[r, off + ids[r, c]] (ids NULL:
+// c), loss_rc = max(x,0) - x t + log1p(exp(-|x|)). One CTA per row; the logits row and the per-choice gradients live in shared
+// memory. d logits[r, j] = sum over the choices c that gathered column j of (sigmoid(x) - t) * gs, summed in choice order by the
+// thread owning column j (no atomics: the result does not depend on scheduling); columns nobody gathered get 0. An id outside
+// [0, width - off) reads nothing and makes the row's loss NaN. row_loss[r] = sum_c loss_rc * loss_scale.
+__global__ void __launch_bounds__(LOSS_THREADS)
+bce_gather_rows_kernel(const float* __restrict__ logits, long long ld, int off, int width, const long long* __restrict__ ids,
+                       const float* __restrict__ target, int C, float loss_scale, float* __restrict__ row_loss,
+                       float* __restrict__ d32, long long ldd32, __nv_bfloat16* __restrict__ d16, long long ldd16) {
+  pdl_entry();
+  extern __shared__ float smem[];
+  float* xs = smem;                                          // [width] the logits row
+  float* gs = xs + width;                                    // [C] gradient of each choice
+  int* col = reinterpret_cast<int*>(gs + C);                 // [C] column it gathered (-1: out of range)
+  __shared__ float red[LOSS_THREADS / 32];
+  const int r = blockIdx.x;
+  const float* zr = logits + (long long)r * ld;
+  for (int j = threadIdx.x; j < width; j += LOSS_THREADS) xs[j] = zr[j];
+  __syncthreads();
+  float acc = 0.f;
+  for (int c = threadIdx.x; c < C; c += LOSS_THREADS) {
+    const long long id = ids ? ids[(long long)r * C + c] : (long long)c;
+    const bool ok = id >= 0 && id < (long long)(width - off);
+    const float t = target[(long long)r * C + c];
+    if (ok) {
+      const int j = off + (int)id;
+      const float x = xs[j];
+      const float e = __expf(-fabsf(x));
+      acc += fmaxf(x, 0.f) - x * t + log1pf(e);
+      const float s = x >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
+      gs[c] = (s - t) * loss_scale;
+      col[c] = j;
+    } else {
+      acc += CUDART_NAN_F;
+      gs[c] = 0.f;
+      col[c] = -1;
+    }
+  }
+  acc = block_reduce(acc, red, false);       // ends with a barrier: gs / col are visible
+  if (threadIdx.x == 0) row_loss[r] = acc * loss_scale;
+  for (int j = threadIdx.x; j < width; j += LOSS_THREADS) {
+    float g = 0.f;
+    if (ids) {
+      for (int c = 0; c < C; ++c) g += col[c] == j ? gs[c] : 0.f;
+    } else if (j >= off && j - off < C) {
+      g = gs[j - off];
+    }
+    if (d32) d32[(long long)r * ldd32 + j] = g;
+    if (d16) d16[(long long)r * ldd16 + j] = __float2bfloat16(g);
+  }
+}
+
+// *loss (+)= sum of row_loss[0..rows) in a fixed order (one CTA)
+__global__ void __launch_bounds__(LOSS_THREADS) sum_rows_kernel(const float* __restrict__ row_loss, int rows, float* __restrict__ loss, int accumulate) {
+  pdl_entry();
+  __shared__ float red[LOSS_THREADS / 32];
+  float s = 0.f;
+  for (int i = threadIdx.x; i < rows; i += LOSS_THREADS) s += row_loss[i];
+  s = block_reduce(s, red, false);
+  if (threadIdx.x == 0) *loss = accumulate ? *loss + s : s;
+}
+
+// torch.max(dim) rules: a NaN is the maximum, the first index wins among equals (and among NaNs)
+__device__ __forceinline__ bool arg_better(float a, int ia, float b, int ib) {
+  const bool na = a != a, nb = b != b;
+  if (na || nb) return na && (!nb || ia < ib);
+  return a > b || (a == b && ia < ib);
+}
+
+__device__ __forceinline__ void warp_argmax(float& v, int& i) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float w = __shfl_xor_sync(0xffffffffu, v, o);
+    const int k = __shfl_xor_sync(0xffffffffu, i, o);
+    if (arg_better(w, k, v, i)) { v = w; i = k; }
+  }
+}
+
+// one warp per row (grid-stride over the rows of one CTA): argmax, then the per-row score of `mode`; the CTA sums in fixed order
+__global__ void __launch_bounds__(LOSS_THREADS)
+task_score_kernel(int mode, const float* __restrict__ logits, long long ld, int off, int cols, const long long* __restrict__ ids,
+                  int width, const float* __restrict__ target, long long ldt, const long long* __restrict__ labels, int rows,
+                  float* __restrict__ score, int accumulate, long long* __restrict__ preds) {
+  pdl_entry();
+  __shared__ double part[LOSS_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double s = 0.0;
+  for (int r = warp; r < rows; r += LOSS_THREADS / 32) {
+    const float* zr = logits + (long long)r * ld;
+    float v = -CUDART_INF_F;
+    int a = 0x7fffffff;
+    for (int c = lane; c < cols; c += 32) {
+      float x;
+      if (ids) {
+        const long long id = ids[(long long)r * cols + c];
+        x = (id >= 0 && id < (long long)(width - off)) ? zr[off + id] : CUDART_NAN_F;
+      } else {
+        x = zr[off + c];
+      }
+      if (arg_better(x, c, v, a)) { v = x; a = c; }
+    }
+    warp_argmax(v, a);
+    const float* tr = target ? target + (long long)r * ldt : nullptr;
+    float hit = 0.f;
+    if (mode == VB_SCORE_SOFT) {
+      hit = tr[a];
+    } else if (mode == VB_SCORE_LABEL) {
+      hit = (long long)a == labels[r] ? 1.f : 0.f;
+    } else if (mode == VB_SCORE_THRESHOLD) {
+      hit = tr[a] > 0.5f ? 1.f : 0.f;
+    } else {   // VB_SCORE_CHOICE: argmax of the target row
+      float tv = -CUDART_INF_F;
+      int ta = 0x7fffffff;
+      for (int c = lane; c < cols; c += 32)
+        if (arg_better(tr[c], c, tv, ta)) { tv = tr[c]; ta = c; }
+      warp_argmax(tv, ta);
+      hit = a == ta ? 1.f : 0.f;
+    }
+    if (lane == 0) {
+      s += (double)hit;
+      if (preds) preds[r] = a;
+    }
+  }
+  if (lane == 0) part[warp] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int w = 0; w < LOSS_THREADS / 32; ++w) t += part[w];
+    *score = (float)((accumulate ? (double)*score : 0.0) + t);
+  }
+}
+
+// dst = src * (*scale): the head gradient of a forward-placed objective times the d(total)/d(loss) the caller holds on the device
+__global__ void scale_by_device_kernel(const float* __restrict__ src, float* __restrict__ dst, long long n, const float* __restrict__ scale) {
+  pdl_entry();
+  const float s = *scale;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i] * s;
+}
+
 static inline int loss_grid(int rows) {
   int cap = sm_count() * 8;
   if (cap <= 0) cap = 132 * 8;
@@ -227,6 +367,46 @@ extern "C" vb_status vb_ce_loss(const float* logits, int64_t ld_logits, const in
              reinterpret_cast<const long long*>(labels), (long long)ignore_index, loss, dlogits_f32, (long long)ld_d32,
              static_cast<__nv_bfloat16*>(dlogits_bf16), (long long)ld_d16, (int)rows, (int)cols, grad_scale);
   return check_launch("vb_ce_loss");
+}
+
+extern "C" vb_status vb_bce_gather_loss(const float* logits, int64_t ld_logits, int32_t col_off, int32_t width, const int64_t* ids,
+                                        const float* target, int32_t rows, int32_t C, float loss_mul, float* row_loss, float* loss,
+                                        int32_t accumulate_loss, float* dlogits_f32, int64_t ld_d32, void* dlogits_bf16, int64_t ld_d16,
+                                        void* stream) {
+  if (rows <= 0 || C <= 0 || col_off < 0 || width <= col_off || (!ids && C > width - col_off) || !logits || !target || !row_loss || !loss)
+    return set_error(VB_ERR_INVALID, "vb_bce_gather_loss: bad arguments");
+  const size_t smem = (size_t)width * sizeof(float) + (size_t)C * (sizeof(float) + sizeof(int));
+  if (smem > 48 * 1024) return set_error(VB_ERR_INVALID, "vb_bce_gather_loss: row of %d logits and %d choices exceeds 48 KiB of shared memory", width, C);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const float scale = loss_mul / ((float)rows * (float)C);
+  launch_pdl(bce_gather_rows_kernel, dim3(rows), dim3(LOSS_THREADS), smem, st, logits, (long long)ld_logits, (int)col_off, (int)width,
+             reinterpret_cast<const long long*>(ids), target, (int)C, scale, row_loss, dlogits_f32, (long long)ld_d32,
+             static_cast<__nv_bfloat16*>(dlogits_bf16), (long long)ld_d16);
+  vb_status s = check_launch("vb_bce_gather_loss");
+  if (s != VB_OK) return s;
+  launch_pdl(sum_rows_kernel, dim3(1), dim3(LOSS_THREADS), (size_t)0, st, (const float*)row_loss, (int)rows, loss, (int)(accumulate_loss ? 1 : 0));
+  return check_launch("vb_bce_gather_loss");
+}
+
+extern "C" vb_status vb_task_score(int32_t mode, const float* logits, int64_t ld_logits, int32_t col_off, int32_t cols, const int64_t* ids,
+                                   int32_t width, const float* target, int64_t ld_target, const int64_t* labels, int32_t rows, float* score,
+                                   int32_t accumulate, int64_t* preds, void* stream) {
+  const bool need_target = mode == VB_SCORE_SOFT || mode == VB_SCORE_THRESHOLD || mode == VB_SCORE_CHOICE;
+  if (mode < VB_SCORE_SOFT || mode > VB_SCORE_CHOICE || rows <= 0 || cols <= 0 || col_off < 0 || !logits || !score ||
+      (need_target && !target) || (mode == VB_SCORE_LABEL && !labels) || (mode == VB_SCORE_CHOICE) != (ids != nullptr) ||
+      (ids && width <= col_off))
+    return set_error(VB_ERR_INVALID, "vb_task_score: bad arguments");
+  launch_pdl(task_score_kernel, dim3(1), dim3(LOSS_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), (int)mode, logits,
+             (long long)ld_logits, (int)col_off, (int)cols, reinterpret_cast<const long long*>(ids), (int)width, target, (long long)ld_target,
+             reinterpret_cast<const long long*>(labels), (int)rows, score, (int)(accumulate ? 1 : 0), reinterpret_cast<long long*>(preds));
+  return check_launch("vb_task_score");
+}
+
+extern "C" vb_status vb_scale_by_device(const float* src, float* dst, int64_t n, const float* scale, void* stream) {
+  if (n <= 0 || !src || !dst || !scale) return set_error(VB_ERR_INVALID, "vb_scale_by_device: bad arguments");
+  const int grid = (int)((n + 255) / 256 < 1024 ? (n + 255) / 256 : 1024);
+  launch_pdl(scale_by_device_kernel, dim3(grid), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream), src, dst, (long long)n, scale);
+  return check_launch("vb_scale_by_device");
 }
 
 extern "C" vb_status vb_kl_masked_loss(const float* scores, const float* target, const int64_t* label, float* loss, float* dscores_f32,

@@ -260,10 +260,23 @@ LOSS_HEADS = {
     "gqa": ("vil_prediction_gqa",),             # VL-classifier-GQA: BCEWithLogits.mean() * 1533
     "vlogit_bce": ("vision_logit",),            # V-logit (refcoco*): BCEWithLogits(vision_logit [B,Nv,1], target).mean() * Nv
     "logit_ce": ("vil_logit",),                 # VL-logit (retrieval, VCR): CE over vil_logit.view(B / options, options)
-    "binary_ce": ("vil_binary_prediction",),    # VL-binary-classifier (NLVR2): CE over the 2-way paired head
-    "tri_ce": ("vil_tri_prediction",),          # VL-tri-classifier (SNLI-VE): CE over 3 classes
+    "binary_ce": ("vil_binary_prediction",),    # VL-binary-classifier with CrossEntropyLoss (Foil): CE over the 2-way head, int labels
+    "tri_ce": ("vil_tri_prediction",),          # VL-tri-classifier with CrossEntropyLoss: CE over 3 classes, int labels
+    "vlogit_mc": ("vision_logit",),             # V-logit-mc (Visual7w, GuessWhatPointing): BCE(vision_logit[:, 101:].gather(1, ids), target).mean() * C
+    "binary_bce": ("vil_binary_prediction",),   # VL-binary-classifier with BCEWithLogitLoss (NLVR2): BCE over soft [B, 2] targets, mean()
+    "tri_bce": ("vil_tri_prediction",),         # VL-tri-classifier with BCEWithLogitLoss (SNLI-VE): BCE over soft [B, 3] targets, mean()
     "pretraining": ("linguisic_prediction", "vision_prediction", "seq_relationship_score"),   # masked-LM CE + masked-region KL + alignment CE
 }
+
+# the fine-tuning objectives of the task table (everything but the pre-training objective): these can be placed at the end of the
+# forward pass and given an on-device batch score (Plan(loss_in_forward=..., score=...))
+TASK_KINDS = tuple(k for k in LOSS_HEADS if k != "pretraining")
+# V-logit-mc scores the regions after the first 101 (task_utils.py:353: vision_logit[:, 101:])
+MC_REGION_OFFSET = 101
+# score of each task objective (task_utils.py:121-162, 618-623); binary_ce / tri_ce have none: with int labels the reference's
+# compute_score_with_logits scatters into a 1-D tensor and raises (INTEGRATION.md)
+SCORE_MODES = {"vqa": L.VB_SCORE_SOFT, "gqa": L.VB_SCORE_SOFT, "logit_ce": L.VB_SCORE_LABEL, "vlogit_bce": L.VB_SCORE_THRESHOLD,
+               "vlogit_mc": L.VB_SCORE_CHOICE, "binary_bce": L.VB_SCORE_SOFT, "tri_bce": L.VB_SCORE_SOFT}
 
 HEAD_NAMES = ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_prediction", "vil_tri_prediction",
               "vision_prediction", "vision_logit", "linguisic_prediction", "linguisic_logit")
@@ -273,9 +286,16 @@ BERT_OUT_NAMES = ("sequence_output_t", "sequence_output_v", "pooled_output_t", "
 class Plan:
     """Static execution plan for one input shape. `grad_outputs` names the outputs that will receive a
     gradient in backward (dead branches are not emitted); `vqa_loss` fuses the VQA BCE objective
-    (task_utils.py:325-327) and its gradient after the forward."""
+    (task_utils.py:325-327) and its gradient after the forward.
 
-    def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None):
+    Task objectives (TASK_KINDS) take three more options. loss_in_forward=True emits the objective at the END of the forward list
+    (a forward-only plan yields the loss) and stores d loss / d head; the backward then starts with head gradient = stored gradient
+    x self.loss_grad (a device scalar, 1 by default: what the caller's d(total)/d(loss) is copied into). score=True also emits the
+    on-device batch score of the kind (self.score, device f32 [1]; self.preds, the per-row argmax). `choices`: answer options of
+    logit_ce (default engine.loss_options) and multiple-choice ids per sample of vlogit_mc."""
+
+    def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
+                 loss_in_forward=False):
         self.e, self.cfg = engine, engine.cfg
         self.grad_touch = {}           # (flat offset, numel) -> index of the last backward op writing that gradient range
         self.ps = _TrackedParams(engine.ps, self)
@@ -305,7 +325,18 @@ class Plan:
         self.loss_kind = "vqa" if vqa_loss else loss
         if self.loss_kind is not None and self.loss_kind not in LOSS_HEADS:
             raise ValueError(f"loss must be one of {sorted(LOSS_HEADS)}")
-        self.vqa_loss = self.loss_kind == "vqa"
+        self.loss_in_forward, self.want_score, self.choices = bool(loss_in_forward), bool(score), choices
+        self.task_objective = self.loss_in_forward or self.want_score     # the objective's scalars live in self.objective_out
+        if self.task_objective and self.loss_kind not in TASK_KINDS:
+            raise ValueError(f"loss_in_forward / score need a task objective, one of {TASK_KINDS}")
+        if self.want_score and self.loss_kind not in SCORE_MODES:
+            raise ValueError(f"loss={self.loss_kind!r} has no batch score: with int labels the reference's compute_score_with_logits "
+                             "raises (task_utils.py:618-623)")
+        if self.loss_kind == "vlogit_mc" and not (choices and choices > 0):
+            raise ValueError("loss='vlogit_mc' needs choices= (multiple-choice ids per sample)")
+        if self.loss_kind == "vlogit_mc" and Nv <= MC_REGION_OFFSET:
+            raise ValueError(f"loss='vlogit_mc' scores the regions after the first {MC_REGION_OFFSET}: Nv must exceed it")
+        self.vqa_loss = self.loss_kind == "vqa" and not self.task_objective
         self.train = bool(train)          # nn.Dropout layers active (model.train()); False = the reference's eval mode
         self.op_dtype, self.split = engine.op_dtype, engine.split   # format of the forward operands (activations, weights)
         self.head_dropout_prob = engine.head_dropout_prob
@@ -1147,7 +1178,15 @@ class Plan:
         c, B = self.cfg, self.B
         self.outputs, self.gout = OrderedDict(), {}
         self.loss_inputs = {}
-        self.loss = self.buf((1,), F32, zero=True) if (self.loss_kind is not None and not self.vqa_loss) else None
+        self.head_grad = {}           # loss_in_forward: d loss / d head, written by the forward-placed objective
+        self.score = self.preds = None
+        if self.task_objective:
+            # loss and score side by side: one device-to-host copy reads both
+            self.objective_out = self.buf((2,), F32, zero=True)
+            self.loss = self.objective_out[0:1]
+            self.score = self.objective_out[1:2] if self.want_score else None
+        else:
+            self.loss = self.buf((1,), F32, zero=True) if (self.loss_kind is not None and not self.vqa_loss) else None
         self.enc_t, self.enc_v = [], []
         t, v = self.embeddings()
         # BertEncoder.forward interleaving schedule (vilbert.py:960-1096)
@@ -1208,11 +1247,15 @@ class Plan:
                 if nm in self.outputs:
                     self.outputs[nm] = self.outputs[nm].view(B, self.Nt, -1)
         self.sync_streams(mirror=False)
+        if self.loss_in_forward:
+            self._emit_loss()
         self.n_kernels_fwd = sum(1 for op in self.fwd if op[0] is not None)
 
         # ---------------- backward
         self.cur = self.bwd
-        if self.vqa_loss:
+        if self.loss_in_forward:
+            self._emit_grad_scale()
+        elif self.vqa_loss:
             lg = self.outputs["vil_prediction"]
             self.vqa_target = self.buf(tuple(lg.shape), F32, zero=True)
             self.loss = self.buf((1,), F32, zero=True)
@@ -1260,29 +1303,39 @@ class Plan:
         caller-supplied gradient. Labels / targets are static plan inputs (self.loss_inputs)."""
         lib, B, k = self.lib, self.B, self.loss_kind
         missing = [n for n in LOSS_HEADS[k] if n not in self.grad_outputs]
-        if missing:
+        if missing and not self.loss_in_forward:      # a forward-placed objective also serves forward-only (eval) plans
             raise ValueError(f"loss={k!r} differentiates {LOSS_HEADS[k]}: add them to grad_outputs")
         li = self.loss_inputs
 
         def ce(name, rows, cols, label_key, acc):
             lg = self.outputs[name]
             li[label_key] = self.buf((rows,), I64, zero=True)
-            d = self.out_grad_buffer(name, tuple(lg.shape))
+            d = self._head_grad(name, tuple(lg.shape))
             self.emit(lib.vb_ce_loss, lg.data_ptr(), cols, li[label_key].data_ptr(), -1, self.loss.data_ptr(), d.data_ptr(), cols, None, 0,
                       rows, cols, 1.0, 1 if acc else 0)
 
         def bce(name, rows, cols):
             lg = self.outputs[name]
             li["target"] = self.buf((rows, cols), F32, zero=True)
-            d = self.out_grad_buffer(name, tuple(lg.shape))
+            d = self._head_grad(name, tuple(lg.shape))
             self.emit(lib.vb_bce_logits_loss, lg.data_ptr(), li["target"].data_ptr(), self.loss.data_ptr(), d.data_ptr(), None, 0, rows, cols, 1.0)
 
-        if k == "gqa":
+        def bce_gather(name, rows, width, C, off, ids, loss_mul):
+            lg = self.outputs[name]
+            li["target"] = self.buf((rows, C), F32, zero=True)
+            d = self._head_grad(name, tuple(lg.shape))
+            row_loss = self.buf((rows,), F32)
+            self.emit(lib.vb_bce_gather_loss, lg.data_ptr(), width, off, width, self._ptr(ids), li["target"].data_ptr(), rows, C, float(loss_mul),
+                      row_loss.data_ptr(), self.loss.data_ptr(), 0, d.data_ptr(), width, None, 0)
+
+        if k == "vqa":      # task objective path only (the round-1 path is vqa_loss)
+            bce("vil_prediction", B, 3129)
+        elif k == "gqa":
             bce("vil_prediction_gqa", B, 1533)
         elif k == "vlogit_bce":
             bce("vision_logit", B, self.Nv)
         elif k == "logit_ce":
-            opts = self.e.loss_options
+            opts = self.choices or self.e.loss_options
             if B % opts:
                 raise ValueError(f"loss='logit_ce': batch {B} is not a multiple of {opts} options")
             ce("vil_logit", B // opts, opts, "labels", False)
@@ -1290,6 +1343,14 @@ class Plan:
             ce("vil_binary_prediction", self.outputs["vil_binary_prediction"].shape[0], 2, "labels", False)
         elif k == "tri_ce":
             ce("vil_tri_prediction", B, 3, "labels", False)
+        elif k == "vlogit_mc":
+            C = int(self.choices)
+            li["multiple_choice_ids"] = self.buf((B, C), I64, zero=True)
+            bce_gather("vision_logit", B, self.Nv, C, MC_REGION_OFFSET, li["multiple_choice_ids"], C)
+        elif k in ("binary_bce", "tri_bce"):
+            name = "vil_binary_prediction" if k == "binary_bce" else "vil_tri_prediction"
+            cols = 2 if k == "binary_bce" else 3
+            bce_gather(name, self.outputs[name].shape[0], cols, cols, 0, None, 1.0)
         elif k == "pretraining":
             # vilbert.py:1578-1590 (+ train_concap.py: loss = masked_loss_t + masked_loss_v + next_sentence_loss)
             V, C = self.cfg.vocab_size, self.cfg.v_target_size
@@ -1306,6 +1367,48 @@ class Plan:
             self.emit(lib.vb_kl_masked_loss, sv.data_ptr(), li["image_target"].data_ptr(), li["image_label"].data_ptr(), self.loss.data_ptr(),
                       dv.data_ptr(), None, 0, B, self.Nv, C, 1.0, 1)
             ce("seq_relationship_score", B, 2, "next_sentence_label", True)
+        if self.want_score:
+            self._emit_score()
+
+    def _head_grad(self, name, shape):
+        """Where the objective writes d loss / d head: the head's output-gradient buffer, or with loss_in_forward a buffer of its own
+        that the backward scales into it (_emit_grad_scale)."""
+        if not self.loss_in_forward:
+            return self.out_grad_buffer(name, shape)
+        self.head_grad[name] = self.buf(shape, F32, zero=True)
+        return self.head_grad[name]
+
+    def _emit_score(self):
+        """The batch score of the task objective (task_utils.py:121-162, 325-374, 618-623) into self.score, argmax per row into
+        self.preds, from the head logits and the objective's own inputs."""
+        k, li, B, Nv = self.loss_kind, self.loss_inputs, self.B, self.Nv
+        mode = SCORE_MODES[k]
+        ids, width, off, labels, target = None, 0, 0, None, li.get("target")
+        if k in ("vqa", "gqa", "binary_bce", "tri_bce"):
+            lg = self.outputs[LOSS_HEADS[k][0]]
+            rows, cols = lg.shape[0], lg.shape[1]
+        elif k == "logit_ce":
+            lg, labels = self.outputs["vil_logit"], li["labels"]
+            cols = self.choices or self.e.loss_options
+            rows = B // cols
+        elif k == "vlogit_bce":
+            lg, rows, cols = self.outputs["vision_logit"], B, Nv
+        else:   # vlogit_mc
+            lg, rows, cols = self.outputs["vision_logit"], B, int(self.choices)
+            ids, width, off = li["multiple_choice_ids"], Nv, MC_REGION_OFFSET
+        ld = Nv if k in ("vlogit_bce", "vlogit_mc") else cols
+        self.preds = self.buf((rows,), I64, zero=True)
+        self.emit(self.lib.vb_task_score, mode, lg.data_ptr(), ld, off, cols, self._ptr(ids), width, self._ptr(target),
+                  cols if target is not None else 0, self._ptr(labels), rows, self.score.data_ptr(), 0, self.preds.data_ptr())
+
+    def _emit_grad_scale(self):
+        """Backward of a forward-placed objective: head gradient = stored d loss / d head x self.loss_grad (device scalar)."""
+        self.loss_grad = self.buf((1,), F32, zero=True)
+        self.loss_grad.fill_(1.0)
+        for name, d in self.head_grad.items():
+            if name in self.grad_outputs:
+                g = self.out_grad_buffer(name, tuple(d.shape))
+                self.emit(self.lib.vb_scale_by_device, d.data_ptr(), g.data_ptr(), d.numel(), self.loss_grad.data_ptr())
 
     # ------------------------------------------------------------------ execution
     def load_inputs(self, input_txt, input_imgs, image_loc, token_type_ids=None, attention_mask=None, image_attention_mask=None,
@@ -1690,15 +1793,19 @@ class Engine:
         self.lm_compact = True           # fused pre-training objective: masked-LM decoder + CE on the labelled rows only (Plan.lm_head_compact)
         self.lm_capacity = 0.25          # ... with room for this fraction of the token rows (15 % are masked; more poisons the loss with NaN)
 
-    def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None):
+    def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
+             loss_in_forward=False):
+        """The cached plan of this shape and these options (Plan)."""
         loss = "vqa" if vqa_loss else loss
-        key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), (self.lm_compact, self.lm_capacity) if loss == "pretraining" else None)
+        key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), (self.lm_compact, self.lm_capacity) if loss == "pretraining" else None,
+               choices, bool(score), bool(loss_in_forward))
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]
         while len(self.plans) >= self.max_plans:   # evict the least recently used plan: its buffers go back to the allocator
             self.plans.popitem(last=False)
-        self.plans[key] = Plan(self, B, Nt, Nv, grad_outputs, False, heads, train, loss=loss)
+        self.plans[key] = Plan(self, B, Nt, Nv, grad_outputs, False, heads, train, loss=loss, choices=choices, score=score,
+                               loss_in_forward=loss_in_forward)
         return self.plans[key]
 
     def enable_activation_arena(self, nbytes):

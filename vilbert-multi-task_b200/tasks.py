@@ -1,0 +1,230 @@
+"""Drop-in replacements for the reference's per-task training and validation steps, ForwardModelsTrain and ForwardModelsVal
+(vilbert/task_utils.py:31-376), with the same signatures and return values:
+
+    from vilbert_b200.tasks import ForwardModelsTrain, ForwardModelsVal, LoadLosses
+
+Each call runs ONE plan of the engine in which the task's objective and its batch score are fused kernels at the end of the forward
+(Plan(loss_in_forward=True, score=True)): no head outputs are cloned, no torch loss is formed, and no score is read back to the host.
+The task table's (type, loss) pairs map to the engine's objective kinds as in TASK_KINDS below.
+
+Reference behaviour that is reproduced, not fixed (INTEGRATION.md):
+  * batch_size is taken before the batch is reshaped: questions for `expand`, image pairs for `nlvr`, question rounds for `dialog`;
+  * ForwardModelsVal returns the summed batch score, ForwardModelsTrain the score divided by batch_size;
+  * the VL-binary-classifier with CrossEntropyLoss (Foil, TASK16) fails as in the reference: with an even batch the CE refuses the
+    per-sample int labels of the paired head (ValueError), otherwise compute_score_with_logits raises on the 1-D labels (IndexError,
+    task_utils.py:618-623 scatters into a 1-D tensor).
+What differs: ForwardModelsTrain returns `score` as a 0-d CUDA tensor (float(score) gives the reference's number) and takes the
+next batch with next() (the reference calls the Python 2 `.next()`).
+"""
+import torch
+import torch.nn as nn
+
+from .data import expand_batch
+from .engine import LOSS_HEADS
+
+LossMap = {
+    "BCEWithLogitLoss": nn.BCEWithLogitsLoss,
+    "CrossEntropyLoss": nn.CrossEntropyLoss,
+}
+
+# (task type, loss) of vilbert_tasks.yml -> the engine's objective kind
+TASK_KINDS = {
+    ("VL-classifier", "BCEWithLogitLoss"): "vqa",
+    ("VL-classifier-GQA", "BCEWithLogitLoss"): "gqa",
+    ("VL-logit", "CrossEntropyLoss"): "logit_ce",
+    ("V-logit", "BCEWithLogitLoss"): "vlogit_bce",
+    ("V-logit-mc", "BCEWithLogitLoss"): "vlogit_mc",
+    ("VL-binary-classifier", "BCEWithLogitLoss"): "binary_bce",
+    ("VL-binary-classifier", "CrossEntropyLoss"): "binary_ce",
+    ("VL-tri-classifier", "BCEWithLogitLoss"): "tri_bce",
+    ("VL-tri-classifier", "CrossEntropyLoss"): "tri_ce",
+}
+
+_NO_SCORE = ("binary_ce", "tri_ce")
+
+
+def LoadLosses(args, task_cfg, task_ids):
+    """The reference's LoadLosses (task_utils.py:379-391): task id -> the loss module its `loss` entry names."""
+    return {"TASK" + t: LossMap[task_cfg["TASK" + t]["loss"]](**({"reduction": "mean"} if task_cfg["TASK" + t]["loss"] == "BCEWithLogitLoss" else {}))
+            for t in task_ids}
+
+
+def task_kind(task_cfg, task_id):
+    """The engine objective kind of one task of the task table."""
+    key = (task_cfg[task_id]["type"], task_cfg[task_id]["loss"])
+    if key not in TASK_KINDS:
+        raise NotImplementedError(f"{task_id}: task type {key[0]!r} with loss {key[1]!r} has no fused objective")
+    return TASK_KINDS[key]
+
+
+def _check_loss(task_cfg, task_id, task_losses):
+    """The fused objectives restate the modules LoadLosses builds (BCEWithLogitsLoss(reduction="mean"), CrossEntropyLoss()); any
+    other module would be silently ignored, so it is refused."""
+    name = task_cfg[task_id]["loss"]
+    fn = task_losses[task_id] if task_losses is not None and task_id in task_losses else None
+    want = LossMap.get(name)
+    ok = want is not None and type(fn) is want and fn.reduction == "mean" and getattr(fn, "weight", None) is None
+    if ok and want is nn.BCEWithLogitsLoss:
+        ok = fn.pos_weight is None
+    if ok and want is nn.CrossEntropyLoss:
+        ok = fn.ignore_index == -100 and fn.label_smoothing == 0.0
+    if not ok:
+        raise NotImplementedError(f"task_losses[{task_id!r}] must be the {name} module LoadLosses builds, got {fn!r}")
+
+
+def _unpack(task_id, batch):
+    """task_utils.py:189-196: Visual7w (TASK4) and GuessWhatPointing (TASK17) carry multiple_choice_ids."""
+    if task_id in ("TASK4", "TASK17"):
+        features, spatials, image_mask, question, target, input_mask, segment_ids, mc_ids, co_attention_mask, question_id = batch
+    else:
+        features, spatials, image_mask, question, target, input_mask, segment_ids, co_attention_mask, question_id = batch
+        mc_ids = None
+    return features, spatials, image_mask, question, target, input_mask, segment_ids, mc_ids, co_attention_mask
+
+
+class _Step:
+    """One task batch on the device, reshaped for the model, with its plan built and inputs loaded."""
+
+    def __init__(self, task_cfg, task_id, batch, model, train, grad, processes):
+        eng = model.engine
+        self.kind = kind = task_kind(task_cfg, task_id)
+        features, spatials, image_mask, question, target, input_mask, segment_ids, mc_ids, _ = _unpack(task_id, batch)
+        process = task_cfg[task_id]["process"]
+        batch_size = features.size(0)
+        if process in processes:
+            features, spatials, image_mask, question, input_mask, segment_ids, _, B, num_options = expand_batch(
+                process, features, spatials, image_mask, question, input_mask, segment_ids)
+            if process == "dialog":
+                target = target.reshape(-1)
+                batch_size = B
+        else:
+            num_options = None     # VL-logit tasks are always expanded (otherwise the engine's default, engine.loss_options)
+        self.batch_size = batch_size
+        task_tokens = question.new_full((question.size(0), 1), int(task_id[4:]))
+        B, Nt = question.shape
+        Nv = features.size(1)
+        choices = None
+        if kind == "logit_ce":
+            choices = num_options
+        elif kind == "vlogit_mc":
+            choices = mc_ids.size(1)
+        self.plan = plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS[kind] if grad else (), train=train, loss=kind, choices=choices,
+                                    score=kind not in _NO_SCORE, loss_in_forward=True)
+        self.inputs = dict(input_txt=question, input_imgs=features, image_loc=spatials, token_type_ids=segment_ids, attention_mask=input_mask,
+                           image_attention_mask=image_mask, task_ids=task_tokens)
+        self.targets = {}
+        li = plan.loss_inputs
+        if "labels" in li:
+            if target.numel() != li["labels"].numel():
+                # Foil with an even batch: the binary head pairs consecutive samples (vilbert.py:1686-1689) and CrossEntropyLoss
+                # refuses the int labels of every sample, as F.cross_entropy does in the reference
+                raise ValueError(f"Expected input batch_size ({li['labels'].numel()}) to match target batch_size ({target.numel()}).")
+            self.targets["labels"] = target.reshape(li["labels"].shape)
+        else:
+            self.targets["target"] = target.reshape(li["target"].shape)
+        if mc_ids is not None and "multiple_choice_ids" in li:
+            self.targets["multiple_choice_ids"] = mc_ids
+        self.model, self.train = model, train
+
+    def load(self):
+        self.plan.load_inputs(**self.inputs)
+        for k, v in self.targets.items():
+            self.plan.loss_inputs[k].copy_(v, non_blocking=True)
+
+    def forward(self):
+        model, plan = self.model, self.plan
+        model._sync_weights()
+        if self.train:
+            model.engine.bump_dropout_step()
+        self.drop_step = int(model.engine.drop_step_host)
+        self.load()
+        if model.engine.auto_graph:
+            plan.maybe_capture_passes()
+        plan.run_forward()
+        self.fwd_id = plan.fwd_id
+        model._last_plan = plan
+
+    def score_error(self):
+        if self.kind in _NO_SCORE:
+            raise IndexError(f"{self.kind}: the reference's compute_score_with_logits scatters the argmax into a 1-D one-hot of the int "
+                             "labels and raises 'Dimension out of range' (task_utils.py:618-623); there is no score to reproduce")
+
+
+class _TaskLossFn(torch.autograd.Function):
+    """loss.backward() of ForwardModelsTrain: d(total)/d(loss) is copied, on the device, into the plan's loss_grad and the plan's
+    backward runs into the model's flat gradient buffer (then the data-parallel all-reduce when one is attached, like the module
+    surface). If another plan ran in between, the forward is recomputed first with the same inputs and dropout masks."""
+
+    @staticmethod
+    def forward(ctx, anchor, step):
+        ctx.step = step
+        return step.plan.loss.detach().reshape(()).clone()
+
+    @staticmethod
+    def backward(ctx, g):
+        step = ctx.step
+        if g is None:
+            return None, None
+        model, plan = step.model, step.plan
+        eng = model.engine
+        clobbered = eng.arena is not None and eng.arena_owner != (plan, step.fwd_id)
+        if plan.fwd_id != step.fwd_id or clobbered:
+            step.load()
+            now = int(eng.drop_step_host)
+            if step.train and now != step.drop_step:
+                eng.set_dropout_step(step.drop_step)
+                plan.run_forward()
+                eng.set_dropout_step(now)
+            else:
+                plan.run_forward()
+            step.fwd_id = plan.fwd_id
+        model._attach_grads()
+        if eng.auto_graph:
+            plan.maybe_capture_passes()
+        plan.loss_grad.copy_(g.detach().reshape(1))
+        plan.run_backward()
+        if model._ddp_reducer is not None:
+            model._ddp_reducer.allreduce()
+        return None, None
+
+
+def _model(model):
+    m = getattr(model, "module", model)    # a data-parallel wrapper around the model
+    if not hasattr(m, "engine") or m._heads != "vl":
+        raise TypeError("ForwardModelsTrain / ForwardModelsVal need a vilbert_b200 VILBertForVLTasks")
+    return m
+
+
+def ForwardModelsTrain(args, task_cfg, device, task_id, task_count, task_iter_train, task_dataloader_train, model, task_losses):
+    """task_utils.py:167-376. Returns (loss, score): loss a 0-d CUDA tensor whose backward() runs the fused backward into the model's
+    gradients; score a 0-d CUDA tensor, batch_score / batch_size."""
+    if task_count[task_id] % len(task_dataloader_train[task_id]) == 0:
+        task_iter_train[task_id] = iter(task_dataloader_train[task_id])
+    task_count[task_id] += 1
+    batch = next(task_iter_train[task_id])
+    batch = tuple(t.cuda(device=device, non_blocking=True) for t in batch)
+    m = _model(model)
+    _check_loss(task_cfg, task_id, task_losses)
+    step = _Step(task_cfg, task_id, batch, m, bool(m.training), True, ("dialog", "expand", "retrieval", "nlvr"))
+    step.forward()
+    loss = _TaskLossFn.apply(m._anchor, step)
+    step.score_error()
+    score = step.plan.score.reshape(()) / float(step.batch_size)
+    return loss, score
+
+
+def ForwardModelsVal(args, task_cfg, device, task_id, batch, model, task_losses):
+    """task_utils.py:31-164: (float(loss), float(batch_score), batch_size) from a forward-only plan in the model's current mode,
+    with one device-to-host copy of (loss, score). The reference's validation step has no `dialog` reshape; neither has this one."""
+    batch = tuple(t.cuda(device=device, non_blocking=True) for t in batch)
+    m = _model(model)
+    _check_loss(task_cfg, task_id, task_losses)
+    with torch.no_grad():
+        step = _Step(task_cfg, task_id, batch, m, bool(m.training), False, ("expand", "retrieval", "nlvr"))
+        step.forward()
+        step.score_error()
+        loss, score = step.plan.objective_out.tolist()
+    return loss, score, step.batch_size
+
+
+__all__ = ["ForwardModelsTrain", "ForwardModelsVal", "LoadLosses", "TASK_KINDS", "task_kind"]
