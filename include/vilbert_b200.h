@@ -308,6 +308,27 @@ vb_status vb_kl_masked_loss(const float* scores, const float* target, const int6
                             void* dscores_bf16, int64_t ld_d16, int32_t B, int32_t Nv, int32_t C, float grad_scale,
                             int32_t accumulate_loss, void* stream);
 
+/* The other two masked-region objectives of BertForMultiModalPreTraining, on scores f32 [B, Nv, D] (region 0 skipped), target f32
+ * [B, R, D] and label int64 [B, R], R = Nv - 1; a row is masked where label == 1. One CTA per row of scores writes its loss into
+ * row_loss (f32 workspace [B * Nv]), then a one-CTA launch adds them in a fixed order into *loss (+= when accumulate_loss): no
+ * atomics, loss and gradient are bitwise reproducible. dscores_f32 (f32 [B, Nv, D], NULL: no gradient) = grad_scale * d loss /
+ * d scores, zero on region 0 and on unmasked rows.
+ *
+ * vb_mse_masked_loss: visual_target == 1 (vilbert.py:1507-1513, MSELoss(reduction="none") over the masked elements)
+ *   loss = sum_{masked} sum_d (s - t)^2 / max(n_masked * D, 1)        (no masked row: 0)
+ *
+ * vb_nce_region_loss: visual_target == 2 (vilbert.py:1523-1575). For a masked (b, r): candidate 0 is target[b, r], candidate
+ * k = 1..n_neg is row neg_index[b, r, k-1] (int64 [B, R, n_neg]) of target viewed as [B * R, D]; score_k = <candidate_k,
+ * scores[b, r+1]>; loss = mean over the masked rows of CrossEntropy(score, 0) (no masked row: NaN, like torch). The prediction
+ * row and the n_neg + 1 scores sit in shared memory ((D + n_neg + 1) * 4 <= 48 KiB); candidates are read with 128-bit loads
+ * (D % 4 == 0, 16-byte aligned rows), no [n_masked, n_neg + 1, D] tensor exists. An index outside [0, B * R) is not read and
+ * makes the loss NaN. Duplicate indices count once per occurrence. */
+vb_status vb_mse_masked_loss(const float* scores, const float* target, const int64_t* label, int32_t B, int32_t Nv, int32_t D,
+                             float grad_scale, float* row_loss, float* loss, int32_t accumulate_loss, float* dscores_f32, void* stream);
+vb_status vb_nce_region_loss(const float* scores, const float* target, const int64_t* label, const int64_t* neg_index, int32_t B,
+                             int32_t Nv, int32_t D, int32_t n_neg, float grad_scale, float* row_loss, float* loss,
+                             int32_t accumulate_loss, float* dscores_f32, void* stream);
+
 /* config.dynamic_attention (BertImageSelfAttention, vilbert.py:557-586): the image self-attention's queries and keys are scaled per
  * (sample, channel) by gate = 1 + sigmoid(dyLinear(pool)), pool = mean of the current text states over the unmasked tokens.
  *   vb_masked_mean_fwd  pool[b,:] = sum_n m[b,n] x[b,n,:] / sum_n m[b,n]; x f32 [B,N,H]; add_mask f32 [B,N] is the additive text mask

@@ -56,6 +56,12 @@ def cases(O, LOSS_HEADS):
         ("task_binary_bce", {}, "vl", 4, obj("binary_bce", **task)),
         ("task_tri_bce", {}, "vl", 4, obj("tri_bce", **task)),
         ("task_binary_ce_nscore", {}, "vl", 4, obj("binary_ce", loss_in_forward=True)),
+        # the pre-training objective for every config.visual_target: summed, and with three losses placed at the end of the forward
+        # (train, and eval without gradients)
+        *[case for vt, over in ((0, {}), (1, dict(visual_target=1, v_target_size=48)), (2, dict(visual_target=2, v_target_size=48)))
+          for case in ([] if vt == 0 else [(f"pretraining_vt{vt}", over, "pretraining", 4, obj("pretraining"))]) +
+          [(f"pretraining_fwd_vt{vt}", over, "pretraining", 4, obj("pretraining", loss_in_forward=True)),
+           (f"pretraining_fwd_vt{vt}_eval", over, "pretraining", 4, dict(loss="pretraining", loss_in_forward=True))]],
     ]
 
 

@@ -107,6 +107,8 @@ _SIGNATURES = {
     "vb_task_score": [_I32, _P, _I64, _I32, _I32, _P, _I32, _P, _I64, _P, _I32, _P, _I32, _P, _P],
     "vb_scale_by_device": [_P, _P, _I64, _P, _P],
     "vb_kl_masked_loss": [_P, _P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _F, _I32, _P],
+    "vb_mse_masked_loss": [_P, _P, _P, _I32, _I32, _I32, _F, _P, _P, _I32, _P, _P],
+    "vb_nce_region_loss": [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _F, _P, _P, _I32, _P, _P],
     "vb_masked_mean_fwd": [_P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
     "vb_masked_mean_bwd": [_P, _P, _P, _I32, _I32, _I32, _I32, _P],
     "vb_gate_scale_fwd": [_P, _P, _I64, _P, _I32, _I32, _I32, _I32, _P],

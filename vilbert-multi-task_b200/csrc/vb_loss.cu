@@ -337,6 +337,112 @@ task_score_kernel(int mode, const float* __restrict__ logits, long long ld, int 
   }
 }
 
+// ------------------------------------------------------------------------------------------ masked-region regression and NCE
+// Both objectives score rows [b, r+1] of prediction_scores_v (region 0, the global feature, is dropped) against target[b, r] and
+// label[b, r] == 1, R = Nv - 1. One CTA per row of scores (region 0 and unmasked rows write a zero gradient and a zero row loss);
+// row_loss[B * Nv] is summed afterwards in a fixed order by sum_rows_kernel, so loss and gradient are bitwise reproducible.
+
+// visual_target == 1 (vilbert.py:1507-1513): loss = sum over masked rows of sum_d (s - t)^2 / max(n_masked * D, 1)
+__global__ void __launch_bounds__(LOSS_THREADS)
+mse_masked_rows_kernel(const float* __restrict__ scores, const float* __restrict__ target, const long long* __restrict__ label, int B,
+                       int Nv, int D, float grad_scale, float* __restrict__ row_loss, float* __restrict__ d32) {
+  pdl_entry();
+  __shared__ float red[LOSS_THREADS / 32];
+  const int R = Nv - 1, rr = blockIdx.x, b = rr / Nv, reg = rr % Nv;
+  const float n_pos = block_count(label, B * R, red, [](long long l) { return l == 1; });
+  const float inv = 1.f / fmaxf(n_pos * (float)D, 1.f);
+  const bool live = reg > 0 && label[(long long)b * R + reg - 1] == 1;
+  const float* sr = scores + (long long)rr * D;
+  const float* tr = target + ((long long)b * R + (reg > 0 ? reg - 1 : 0)) * D;
+  float acc = 0.f;
+  for (int j = threadIdx.x; j < D; j += LOSS_THREADS) {
+    float g = 0.f;
+    if (live) {
+      const float e = sr[j] - tr[j];
+      acc += e * e;
+      g = 2.f * e * grad_scale * inv;
+    }
+    if (d32) d32[(long long)rr * D + j] = g;
+  }
+  acc = block_reduce(acc, red, false);
+  if (threadIdx.x == 0) row_loss[rr] = acc * inv;
+}
+
+// visual_target == 2 (vilbert.py:1523-1575): for a masked row, candidate 0 is target[b, r] and candidate k >= 1 is row
+// neg[b, r, k-1] of target viewed as [B * R, D]; score_k = <candidate_k, s>; loss = CE(score, 0) averaged over the masked rows.
+// d s = sum_k (softmax_k - [k == 0]) candidate_k * gs / n_masked, summed in candidate order by the thread owning the columns.
+// The prediction row lives in shared memory; candidates are read with 128-bit loads, once for the scores and once for the
+// gradient. An index outside [0, B * R) is not read: it makes the row's loss NaN and adds nothing to the gradient.
+__global__ void __launch_bounds__(LOSS_THREADS)
+nce_region_rows_kernel(const float* __restrict__ scores, const float* __restrict__ target, const long long* __restrict__ label,
+                       const long long* __restrict__ neg, int B, int Nv, int D, int n, float grad_scale, float* __restrict__ row_loss,
+                       float* __restrict__ d32) {
+  pdl_entry();
+  extern __shared__ __align__(16) float smem[];
+  float* s = smem;                          // [D] the prediction row
+  float* sc = smem + D;                     // [n + 1] candidate scores (NaN: index out of range)
+  __shared__ float red[LOSS_THREADS / 32];
+  const int R = Nv - 1, rr = blockIdx.x, b = rr / Nv, reg = rr % Nv, D4 = D / 4;
+  const long long rows_t = (long long)B * R;
+  const float n_pos = block_count(label, (int)rows_t, red, [](long long l) { return l == 1; });
+  const bool live = reg > 0 && label[(long long)b * R + reg - 1] == 1;
+  float4* g4 = d32 ? reinterpret_cast<float4*>(d32 + (long long)rr * D) : nullptr;
+  if (!live) {
+    for (int j = threadIdx.x; j < D4; j += LOSS_THREADS)
+      if (g4) g4[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (threadIdx.x == 0) row_loss[rr] = (rr == 0 && n_pos == 0.f) ? CUDART_NAN_F : 0.f;   // CE over no rows is NaN
+    return;
+  }
+  const float4* s_src = reinterpret_cast<const float4*>(scores + (long long)rr * D);
+  float4* s4 = reinterpret_cast<float4*>(s);
+  for (int j = threadIdx.x; j < D4; j += LOSS_THREADS) s4[j] = s_src[j];
+  __syncthreads();
+  const long long own = (long long)b * R + reg - 1;
+  const long long* nr = neg + own * n;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int k = warp; k <= n; k += LOSS_THREADS / 32) {     // one warp per candidate
+    const long long row = k == 0 ? own : nr[k - 1];
+    float dot = CUDART_NAN_F;
+    if (row >= 0 && row < rows_t) {
+      const float4* c4 = reinterpret_cast<const float4*>(target + row * D);
+      float a = 0.f;
+      for (int j = lane; j < D4; j += 32) {
+        const float4 c = c4[j], p = s4[j];
+        a += c.x * p.x + c.y * p.y + c.z * p.z + c.w * p.w;
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+      dot = a;
+    }
+    if (lane == 0) sc[k] = dot;
+  }
+  __syncthreads();
+  float mx = -CUDART_INF_F;
+  for (int k = threadIdx.x; k <= n; k += LOSS_THREADS) mx = fmaxf(mx, sc[k]);      // fmaxf drops NaN
+  mx = block_reduce(mx, red, true);
+  float se = 0.f, bad = 0.f;
+  for (int k = threadIdx.x; k <= n; k += LOSS_THREADS) {
+    if (sc[k] != sc[k]) bad = 1.f; else se += __expf(sc[k] - mx);
+  }
+  se = block_reduce(se, red, false);
+  bad = block_reduce(bad, red, true);
+  const float lse = mx + __logf(se);
+  if (threadIdx.x == 0) row_loss[rr] = bad > 0.f ? CUDART_NAN_F : (lse - sc[0]) / n_pos;
+  if (!g4) return;
+  const float gs = grad_scale / n_pos;
+  for (int j = threadIdx.x; j < D4; j += LOSS_THREADS) {
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int k = 0; k <= n; ++k) {
+      const float z = sc[k];
+      if (z != z) continue;
+      const float w = (__expf(z - lse) - (k == 0 ? 1.f : 0.f)) * gs;
+      const float4 c = reinterpret_cast<const float4*>(target + (k == 0 ? own : nr[k - 1]) * D)[j];
+      acc.x += w * c.x; acc.y += w * c.y; acc.z += w * c.z; acc.w += w * c.w;
+    }
+    g4[j] = acc;
+  }
+}
+
 // dst = src * (*scale): the head gradient of a forward-placed objective times the d(total)/d(loss) the caller holds on the device
 __global__ void scale_by_device_kernel(const float* __restrict__ src, float* __restrict__ dst, long long n, const float* __restrict__ scale) {
   pdl_entry();
@@ -422,6 +528,39 @@ extern "C" vb_status vb_kl_masked_loss(const float* scores, const float* target,
              reinterpret_cast<const long long*>(label), loss, dscores_f32, static_cast<__nv_bfloat16*>(dscores_bf16), (long long)ld_d16,
              (int)B, (int)Nv, (int)C, grad_scale);
   return check_launch("vb_kl_masked_loss");
+}
+
+extern "C" vb_status vb_mse_masked_loss(const float* scores, const float* target, const int64_t* label, int32_t B, int32_t Nv, int32_t D,
+                                        float grad_scale, float* row_loss, float* loss, int32_t accumulate_loss, float* dscores_f32,
+                                        void* stream) {
+  if (B <= 0 || Nv <= 1 || D <= 0 || !scores || !target || !label || !row_loss || !loss)
+    return set_error(VB_ERR_INVALID, "vb_mse_masked_loss: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int rows = B * Nv;
+  launch_pdl(mse_masked_rows_kernel, dim3(rows), dim3(LOSS_THREADS), (size_t)0, st, scores, target, reinterpret_cast<const long long*>(label),
+             (int)B, (int)Nv, (int)D, grad_scale, row_loss, dscores_f32);
+  vb_status s = check_launch("vb_mse_masked_loss");
+  if (s != VB_OK) return s;
+  launch_pdl(sum_rows_kernel, dim3(1), dim3(LOSS_THREADS), (size_t)0, st, (const float*)row_loss, rows, loss, (int)(accumulate_loss ? 1 : 0));
+  return check_launch("vb_mse_masked_loss");
+}
+
+extern "C" vb_status vb_nce_region_loss(const float* scores, const float* target, const int64_t* label, const int64_t* neg_index, int32_t B,
+                                        int32_t Nv, int32_t D, int32_t n_neg, float grad_scale, float* row_loss, float* loss,
+                                        int32_t accumulate_loss, float* dscores_f32, void* stream) {
+  if (B <= 0 || Nv <= 1 || D <= 0 || (D & 3) || n_neg < 0 || !scores || !target || !label || (n_neg > 0 && !neg_index) || !row_loss || !loss ||
+      (reinterpret_cast<uintptr_t>(scores) & 15) || (reinterpret_cast<uintptr_t>(target) & 15) || (reinterpret_cast<uintptr_t>(dscores_f32) & 15))
+    return set_error(VB_ERR_INVALID, "vb_nce_region_loss: bad arguments (D % 4 == 0, 16-byte aligned rows)");
+  const size_t smem = ((size_t)D + (size_t)n_neg + 1) * sizeof(float);
+  if (smem > 48 * 1024) return set_error(VB_ERR_INVALID, "vb_nce_region_loss: row of %d features and %d negatives exceeds 48 KiB of shared memory", D, n_neg);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int rows = B * Nv;
+  launch_pdl(nce_region_rows_kernel, dim3(rows), dim3(LOSS_THREADS), smem, st, scores, target, reinterpret_cast<const long long*>(label),
+             reinterpret_cast<const long long*>(neg_index), (int)B, (int)Nv, (int)D, (int)n_neg, grad_scale, row_loss, dscores_f32);
+  vb_status s = check_launch("vb_nce_region_loss");
+  if (s != VB_OK) return s;
+  launch_pdl(sum_rows_kernel, dim3(1), dim3(LOSS_THREADS), (size_t)0, st, (const float*)row_loss, rows, loss, (int)(accumulate_loss ? 1 : 0));
+  return check_launch("vb_nce_region_loss");
 }
 
 extern "C" vb_status vb_compact_rows(const int64_t* labels, int64_t ignore_index, int32_t rows, int32_t cap, int32_t* idx, int32_t* count,

@@ -278,6 +278,16 @@ MC_REGION_OFFSET = 101
 SCORE_MODES = {"vqa": L.VB_SCORE_SOFT, "gqa": L.VB_SCORE_SOFT, "logit_ce": L.VB_SCORE_LABEL, "vlogit_bce": L.VB_SCORE_THRESHOLD,
                "vlogit_mc": L.VB_SCORE_CHOICE, "binary_bce": L.VB_SCORE_SOFT, "tri_bce": L.VB_SCORE_SOFT}
 
+# slots of the three pre-training losses in Plan.objective_out / Plan.loss_grad (loss="pretraining", loss_in_forward=True)
+PRETRAINING_SLOTS = {"linguisic_prediction": 0, "vision_prediction": 1, "seq_relationship_score": 2}
+
+
+def nce_negative_count(cfg):
+    """Negatives per masked region of visual_target == 2: int(0.7 N) from other samples + int(0.3 N) from the same sample
+    (vilbert.py:1524-1557), N = config.num_negative."""
+    return int(cfg.num_negative * 0.7) + int(cfg.num_negative * 0.3)
+
+
 HEAD_NAMES = ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_prediction", "vil_tri_prediction",
               "vision_prediction", "vision_logit", "linguisic_prediction", "linguisic_logit")
 BERT_OUT_NAMES = ("sequence_output_t", "sequence_output_v", "pooled_output_t", "pooled_output_v")
@@ -292,7 +302,11 @@ class Plan:
     (a forward-only plan yields the loss) and stores d loss / d head; the backward then starts with head gradient = stored gradient
     x self.loss_grad (a device scalar, 1 by default: what the caller's d(total)/d(loss) is copied into). score=True also emits the
     on-device batch score of the kind (self.score, device f32 [1]; self.preds, the per-row argmax). `choices`: answer options of
-    logit_ce (default engine.loss_options) and multiple-choice ids per sample of vlogit_mc."""
+    logit_ce (default engine.loss_options) and multiple-choice ids per sample of vlogit_mc.
+
+    loss="pretraining" with loss_in_forward=True keeps the three pre-training losses apart: self.objective_out (device f32 [3]) holds
+    masked_lm, masked_img and next_sentence, self.loss is None, and self.loss_grad (f32 [3]) scales each head gradient by its own
+    slot. A plan without grad_outputs computes the losses only and writes no gradient."""
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
                  loss_in_forward=False):
@@ -327,8 +341,8 @@ class Plan:
             raise ValueError(f"loss must be one of {sorted(LOSS_HEADS)}")
         self.loss_in_forward, self.want_score, self.choices = bool(loss_in_forward), bool(score), choices
         self.task_objective = self.loss_in_forward or self.want_score     # the objective's scalars live in self.objective_out
-        if self.task_objective and self.loss_kind not in TASK_KINDS:
-            raise ValueError(f"loss_in_forward / score need a task objective, one of {TASK_KINDS}")
+        if self.task_objective and self.loss_kind not in TASK_KINDS and not (self.loss_kind == "pretraining" and not self.want_score):
+            raise ValueError(f"loss_in_forward needs a task objective, one of {TASK_KINDS}, or 'pretraining'; score needs a task objective")
         if self.want_score and self.loss_kind not in SCORE_MODES:
             raise ValueError(f"loss={self.loss_kind!r} has no batch score: with int labels the reference's compute_score_with_logits "
                              "raises (task_utils.py:618-623)")
@@ -1011,6 +1025,8 @@ class Plan:
                          dl16=self.buf((cap, ldp), BF16, zero=True), ldp=ldp)
 
         def bwd():
+            if "linguisic_prediction" not in self.grad_outputs:     # a forward-only plan of the forward-placed objective
+                return
             lc = self.lm_c
             self.colsum(lc["dl32"], V, ps.g("cls.predictions.bias"), cap, V)
             self.linear_wgrad(lc["dl16"], ldp, None, 0, hc.bw, Ht, cap, V, Ht, None, gw=ps.g(wn))
@@ -1020,10 +1036,14 @@ class Plan:
             self.gemm(cap, Ht, V, lc["dl16"], ldp, ps.w(wn).bw, Ht, b_mn=1, out_f32=gc, ld_of=Ht)
             g = self.grad_of(ht)
             self.emit(lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
-            self.emit(lib.vb_scatter_rows_f32, gc.data_ptr(), g.data_ptr(), idx.data_ptr(), cap, Ht, cnt.data_ptr(), self.loss.data_ptr())
+            self.emit(lib.vb_scatter_rows_f32, gc.data_ptr(), g.data_ptr(), idx.data_ptr(), cap, Ht, cnt.data_ptr(), self._lm_loss().data_ptr())
             ht.gw = True
             ht_bwd()
         return bwd
+
+    def _lm_loss(self):
+        """Where the masked-LM loss lands: the summed scalar, or the first slot of the three-slot pre-training objective."""
+        return self.loss if self.loss is not None else self.objective_out[0:1]
 
     def lm_rows(self):
         """(labelled rows of the last step, capacity) of the compacted masked-LM head (device sync)."""
@@ -1180,7 +1200,11 @@ class Plan:
         self.loss_inputs = {}
         self.head_grad = {}           # loss_in_forward: d loss / d head, written by the forward-placed objective
         self.score = self.preds = None
-        if self.task_objective:
+        if self.task_objective and self.loss_kind == "pretraining":
+            # masked_lm, masked_img, next_sentence side by side: one device-to-host copy reads all three
+            self.objective_out = self.buf((3,), F32, zero=True)
+            self.loss = None
+        elif self.task_objective:
             # loss and score side by side: one device-to-host copy reads both
             self.objective_out = self.buf((2,), F32, zero=True)
             self.loss = self.objective_out[0:1]
@@ -1352,23 +1376,71 @@ class Plan:
             cols = 2 if k == "binary_bce" else 3
             bce_gather(name, self.outputs[name].shape[0], cols, cols, 0, None, 1.0)
         elif k == "pretraining":
-            # vilbert.py:1578-1590 (+ train_concap.py: loss = masked_loss_t + masked_loss_v + next_sentence_loss)
-            V, C = self.cfg.vocab_size, self.cfg.v_target_size
-            if self.lm_c is not None:
-                lc = self.lm_c
-                self.emit(lib.vb_ce_loss, lc["logits"].data_ptr(), V, lc["labels"].data_ptr(), -1, self.loss.data_ptr(), lc["dl32"].data_ptr(), V,
-                          lc["dl16"].data_ptr(), lc["ldp"], lc["cap"], V, 1.0, 0)
-            else:
-                ce("linguisic_prediction", B * self.Nt, V, "masked_lm_labels", False)
-            sv = self.outputs["vision_prediction"]
-            li["image_target"] = self.buf((B, self.Nv - 1, C), F32, zero=True)
-            li["image_label"] = self.buf((B, self.Nv - 1), I64, zero=True)
-            dv = self.out_grad_buffer("vision_prediction", tuple(sv.shape))
-            self.emit(lib.vb_kl_masked_loss, sv.data_ptr(), li["image_target"].data_ptr(), li["image_label"].data_ptr(), self.loss.data_ptr(),
-                      dv.data_ptr(), None, 0, B, self.Nv, C, 1.0, 1)
-            ce("seq_relationship_score", B, 2, "next_sentence_label", True)
+            self._emit_pretraining_loss()
         if self.want_score:
             self._emit_score()
+
+    def _emit_pretraining_loss(self):
+        """vilbert.py:1578-1590: masked-LM CE (ignore_index -1), the masked-region objective of config.visual_target (0: KL to the
+        class distribution, 1: masked MSE, 2: NCE against the negatives in loss_inputs["neg_index"]) and the alignment CE
+        (ignore_index -1, :1450). The summed plan adds all three into self.loss (train_concap.py's masked_loss_t + masked_loss_v +
+        next_sentence_loss) and writes the gradients into the heads' output-gradient buffers; with loss_in_forward each loss gets
+        its slot of self.objective_out and each gradient a buffer of its own (none in a forward-only plan)."""
+        lib, B, Nv, li, c = self.lib, self.B, self.Nv, self.loss_inputs, self.cfg
+        V, C, R = c.vocab_size, c.v_target_size, Nv - 1
+        sep = self.loss_in_forward
+        slot = [self.objective_out[i:i + 1] for i in range(3)] if sep else [self.loss] * 3
+        acc = 0 if sep else 1           # the summed plan adds the region and alignment losses to the masked-LM loss
+
+        def grad(name, shape):
+            if not sep:
+                return self.out_grad_buffer(name, shape)
+            return self._head_grad(name, shape) if name in self.grad_outputs else None
+
+        if self.lm_c is not None:
+            lc = self.lm_c
+            d32 = grad("linguisic_prediction", (lc["cap"], V)) if sep else lc["dl32"]
+            d16 = None if sep else lc["dl16"]      # loss_in_forward: the backward scales d32, then casts it into dl16
+            self.emit(lib.vb_ce_loss, lc["logits"].data_ptr(), V, lc["labels"].data_ptr(), -1, slot[0].data_ptr(), self._ptr(d32), V,
+                      self._ptr(d16), lc["ldp"], lc["cap"], V, 1.0, 0)
+            if sep:
+                # more labelled rows than the capacity must already show in the forward (eval plans have no backward): the scatter
+                # kernel's count check poisons the masked-LM slot; the rows it moves are a 4-column dummy
+                src = self.scratch("lm.cap.src", (lc["cap"], 4), F32)
+                dst = self.scratch("lm.cap.dst", (B * self.Nt, 4), F32)
+                self.emit(lib.vb_scatter_rows_f32, src.data_ptr(), dst.data_ptr(), lc["idx"].data_ptr(), lc["cap"], 4, lc["count"].data_ptr(),
+                          slot[0].data_ptr())
+        else:
+            lg, rows = self.outputs["linguisic_prediction"], B * self.Nt
+            li["masked_lm_labels"] = self.buf((rows,), I64, zero=True)
+            d = grad("linguisic_prediction", tuple(lg.shape))
+            self.emit(lib.vb_ce_loss, lg.data_ptr(), V, li["masked_lm_labels"].data_ptr(), -1, slot[0].data_ptr(), self._ptr(d), V, None, 0,
+                      rows, V, 1.0, 0)
+        sv = self.outputs["vision_prediction"]
+        li["image_target"] = self.buf((B, R, C), F32, zero=True)
+        li["image_label"] = self.buf((B, R), I64, zero=True)
+        dv = grad("vision_prediction", tuple(sv.shape))
+        vt = c.visual_target
+        if vt == 0:
+            self.emit(lib.vb_kl_masked_loss, sv.data_ptr(), li["image_target"].data_ptr(), li["image_label"].data_ptr(), slot[1].data_ptr(),
+                      self._ptr(dv), None, 0, B, Nv, C, 1.0, acc)
+        elif vt == 1:
+            row_loss = self.buf((B * Nv,), F32)
+            self.emit(lib.vb_mse_masked_loss, sv.data_ptr(), li["image_target"].data_ptr(), li["image_label"].data_ptr(), B, Nv, C, 1.0,
+                      row_loss.data_ptr(), slot[1].data_ptr(), acc, self._ptr(dv))
+        elif vt == 2:
+            n = nce_negative_count(c)
+            li["neg_index"] = self.buf((B, R, n), I64, zero=True)
+            row_loss = self.buf((B * Nv,), F32)
+            self.emit(lib.vb_nce_region_loss, sv.data_ptr(), li["image_target"].data_ptr(), li["image_label"].data_ptr(), li["neg_index"].data_ptr(),
+                      B, Nv, C, n, 1.0, row_loss.data_ptr(), slot[1].data_ptr(), acc, self._ptr(dv))
+        else:
+            raise ValueError(f"visual_target must be 0, 1 or 2, got {vt!r}")
+        ns = self.outputs["seq_relationship_score"]
+        li["next_sentence_label"] = self.buf((B,), I64, zero=True)
+        d = grad("seq_relationship_score", tuple(ns.shape))
+        self.emit(lib.vb_ce_loss, ns.data_ptr(), 2, li["next_sentence_label"].data_ptr(), -1, slot[2].data_ptr(), self._ptr(d), 2, None, 0, B, 2,
+                  1.0, acc)
 
     def _head_grad(self, name, shape):
         """Where the objective writes d loss / d head: the head's output-gradient buffer, or with loss_in_forward a buffer of its own
@@ -1402,13 +1474,23 @@ class Plan:
                   cols if target is not None else 0, self._ptr(labels), rows, self.score.data_ptr(), 0, self.preds.data_ptr())
 
     def _emit_grad_scale(self):
-        """Backward of a forward-placed objective: head gradient = stored d loss / d head x self.loss_grad (device scalar)."""
-        self.loss_grad = self.buf((1,), F32, zero=True)
+        """Backward of a forward-placed objective: head gradient = stored d loss / d head x self.loss_grad (device scalar). The
+        pre-training objective has one scalar per loss (PRETRAINING_SLOTS); its compacted masked-LM gradient is scaled into
+        lm_c["dl32"] and cast from there into its bf16 operand lm_c["dl16"]."""
+        pre = self.loss_kind == "pretraining"
+        self.loss_grad = self.buf((3 if pre else 1,), F32, zero=True)
         self.loss_grad.fill_(1.0)
         for name, d in self.head_grad.items():
             if name in self.grad_outputs:
+                s = self.loss_grad[PRETRAINING_SLOTS[name]] if pre else self.loss_grad
+                if name == "linguisic_prediction" and self.lm_c is not None:
+                    lc = self.lm_c
+                    V = self.cfg.vocab_size
+                    self.emit(self.lib.vb_scale_by_device, d.data_ptr(), lc["dl32"].data_ptr(), d.numel(), s.data_ptr())
+                    self.emit(self.lib.vb_cast2d_f32_to_bf16, lc["dl32"].data_ptr(), V, lc["dl16"].data_ptr(), lc["ldp"], lc["cap"], V, 1.0)
+                    continue
                 g = self.out_grad_buffer(name, tuple(d.shape))
-                self.emit(self.lib.vb_scale_by_device, d.data_ptr(), g.data_ptr(), d.numel(), self.loss_grad.data_ptr())
+                self.emit(self.lib.vb_scale_by_device, d.data_ptr(), g.data_ptr(), d.numel(), s.data_ptr())
 
     # ------------------------------------------------------------------ execution
     def load_inputs(self, input_txt, input_imgs, image_loc, token_type_ids=None, attention_mask=None, image_attention_mask=None,
@@ -1797,8 +1879,8 @@ class Engine:
              loss_in_forward=False):
         """The cached plan of this shape and these options (Plan)."""
         loss = "vqa" if vqa_loss else loss
-        key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), (self.lm_compact, self.lm_capacity) if loss == "pretraining" else None,
-               choices, bool(score), bool(loss_in_forward))
+        pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
+        key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward))
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]

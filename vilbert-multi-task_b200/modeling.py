@@ -12,7 +12,7 @@ import torch.nn.functional as F
 
 from . import _lib as L
 from .config import BertConfig
-from .engine import BERT_OUT_NAMES, HEAD_NAMES, Engine
+from .engine import BERT_OUT_NAMES, HEAD_NAMES, LOSS_HEADS, Engine
 
 
 # Any torch.optim.Optimizer.step() (pytorch_transformers.AdamW and the reference's RAdam subclass it) may have rewritten
@@ -371,17 +371,105 @@ class VILBertForVLTasks(BertPreTrainedModel):
         return tuple(o[n] for n in HEAD_NAMES) + (self._attention_masks(output_all_attention_masks),)
 
 
+class _PretrainStep:
+    """One labelled pre-training batch with its plan (Plan(loss="pretraining", loss_in_forward=True)), inputs and NCE negatives."""
+
+    def __init__(self, model, inputs, targets, grad):
+        eng = model.engine
+        Nt = inputs["input_txt"].shape[1]
+        B, Nv = inputs["input_imgs"].shape[:2]
+        self.train = bool(model.training)
+        self.plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS["pretraining"] if grad else (), train=self.train, loss="pretraining",
+                             loss_in_forward=True)
+        self.model, self.inputs, self.targets = model, inputs, targets
+
+    def load(self):
+        self.plan.load_inputs(**self.inputs)
+        li = self.plan.loss_inputs
+        for k, v in self.targets.items():
+            li[k].copy_(v.reshape(li[k].shape), non_blocking=True)
+
+    def forward(self):
+        model, plan = self.model, self.plan
+        model._sync_weights()
+        if self.train:
+            model.engine.bump_dropout_step()
+        self.drop_step = int(model.engine.drop_step_host)
+        self.load()
+        if model.engine.auto_graph:
+            plan.maybe_capture_passes()
+        plan.run_forward()
+        self.fwd_id = plan.fwd_id
+        model._last_plan = plan
+
+
+class _PretrainLossFn(torch.autograd.Function):
+    """The three losses of the fused pre-training objective. backward copies (d total / d masked_lm, d masked_img, d next_sentence)
+    into the plan's loss_grad on the device (an unused loss contributes 0) and runs the plan's backward into the flat gradient
+    buffer, then the data-parallel all-reduce when one is attached. The backward runs at the dropout step of its forward; if
+    this plan ran again since, or the shared arena was overwritten, the forward is recomputed first with the same inputs,
+    negatives and dropout masks."""
+
+    @staticmethod
+    def forward(ctx, anchor, step):
+        ctx.step = step
+        ctx.set_materialize_grads(False)
+        out = step.plan.objective_out.detach()
+        return out[0:1].clone(), out[1:2].clone(), out[2:3].clone()
+
+    @staticmethod
+    def backward(ctx, *grads):
+        step = ctx.step
+        if all(g is None for g in grads):
+            return None, None
+        model, plan = step.model, step.plan
+        eng = model.engine
+        # the backward regenerates the forward's dropout masks from the device step counter, which a forward in between has moved
+        now = int(eng.drop_step_host)
+        moved = step.train and now != step.drop_step
+        if moved:
+            eng.set_dropout_step(step.drop_step)
+        try:
+            clobbered = eng.arena is not None and eng.arena_owner != (plan, step.fwd_id)
+            if plan.fwd_id != step.fwd_id or clobbered:
+                step.load()
+                plan.run_forward()
+                step.fwd_id = plan.fwd_id
+            model._attach_grads()
+            if eng.auto_graph:
+                plan.maybe_capture_passes()
+            for i, g in enumerate(grads):
+                if g is None:
+                    plan.loss_grad[i:i + 1].zero_()
+                else:
+                    plan.loss_grad[i:i + 1].copy_(g.detach().reshape(1))
+            plan.run_backward()
+        finally:
+            if moved:
+                eng.set_dropout_step(now)
+        if model._ddp_reducer is not None:
+            model._ddp_reducer.allreduce()
+        return None, None
+
+
 class BertForMultiModalPreTraining(BertPreTrainedModel):
     """Reference: vilbert/vilbert.py:1435-1597; the masked-region objective follows config.visual_target (0: KL divergence to the
     detector's class distribution, 1: feature regression, 2: noise-contrastive against sampled regions). The encoder
-    and the three heads run on the engine; the three scalar losses are formed with torch on the head outputs
-    exactly as the reference does (:1506-1590) and their gradients re-enter the engine through autograd."""
+    and the three heads run on the engine; by default the three scalar losses are formed with torch on the head outputs
+    exactly as the reference does (:1506-1590) and their gradients re-enter the engine through autograd.
+
+    fused_objective=True: a call with masked_lm_labels, next_sentence_label and image_target runs the three objectives as fused
+    kernels at the end of the forward (Plan(loss="pretraining", loss_in_forward=True)); no head output is cloned and the tied
+    decoder runs on the labelled token rows only. The losses come back as [1]-shaped CUDA tensors whose backward scales each head
+    gradient by its own d(total)/d(loss) on the device. Unlike the torch path, more labelled tokens than engine.lm_capacity of the
+    rows make the masked-LM loss NaN."""
     _heads = "pretraining"
 
-    def __init__(self, config, device=None, precision=None):
+    def __init__(self, config, device=None, precision=None, fused_objective=False):
         super().__init__(config, device, precision)
         self.visual_target = config.visual_target
         self.num_negative = config.num_negative
+        self.fused_objective = bool(fused_objective)
         if self.visual_target not in (0, 1, 2):
             raise ValueError("visual_target must be 0, 1 or 2")
 
@@ -412,6 +500,9 @@ class BertForMultiModalPreTraining(BertPreTrainedModel):
 
     def forward(self, input_ids, image_feat, image_loc, token_type_ids=None, attention_mask=None, image_attention_mask=None,
                 masked_lm_labels=None, image_label=None, image_target=None, next_sentence_label=None, output_all_attention_masks=False):
+        if self.fused_objective and masked_lm_labels is not None and next_sentence_label is not None and image_target is not None:
+            return self._fused_losses(input_ids, image_feat, image_loc, token_type_ids, attention_mask, image_attention_mask, masked_lm_labels,
+                                      image_label, image_target, next_sentence_label)
         names = ("linguisic_prediction", "vision_prediction", "seq_relationship_score")
         o = self._run(names, input_ids, image_feat, image_loc, token_type_ids, attention_mask, image_attention_mask, None)
         prediction_scores_t, prediction_scores_v, seq_relationship_score = (o[n] for n in names)
@@ -430,3 +521,17 @@ class BertForMultiModalPreTraining(BertPreTrainedModel):
             next_sentence_loss = F.cross_entropy(seq_relationship_score.view(-1, 2), next_sentence_label.view(-1), ignore_index=-1)
             return masked_lm_loss.unsqueeze(0), masked_img_loss.unsqueeze(0), next_sentence_loss.unsqueeze(0)
         return prediction_scores_t, prediction_scores_v, seq_relationship_score, self._attention_masks(output_all_attention_masks)
+
+    def _fused_losses(self, input_ids, image_feat, image_loc, token_type_ids, attention_mask, image_attention_mask, masked_lm_labels,
+                      image_label, image_target, next_sentence_label):
+        inputs = dict(input_txt=input_ids, input_imgs=image_feat, image_loc=image_loc, token_type_ids=token_type_ids,
+                      attention_mask=attention_mask, image_attention_mask=image_attention_mask)
+        targets = dict(masked_lm_labels=masked_lm_labels, image_label=image_label, image_target=image_target,
+                       next_sentence_label=next_sentence_label)
+        if self.visual_target == 2:
+            B, R = image_feat.shape[0], image_feat.shape[1] - 1
+            sampler = getattr(self, "nce_sampler", None)
+            targets["neg_index"] = sampler(B, R, image_feat.device) if sampler is not None else self._nce_negatives(B, R, image_feat.device)
+        step = _PretrainStep(self, inputs, targets, torch.is_grad_enabled())
+        step.forward()
+        return _PretrainLossFn.apply(self._anchor, step)
