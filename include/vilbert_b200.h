@@ -295,6 +295,20 @@ vb_status vb_bce_gather_loss(const float* logits, int64_t ld_logits, int32_t col
 vb_status vb_task_score(int32_t mode, const float* logits, int64_t ld_logits, int32_t col_off, int32_t cols, const int64_t* ids,
                         int32_t width, const float* target, int64_t ld_target, const int64_t* labels, int32_t rows, float* score,
                         int32_t accumulate, int64_t* preds, void* stream);
+/* vb_task_results: the per-row results of one evaluation batch (EvaluatingModel, task_utils.py:777-847), formed on the device so
+ * that one device-to-host copy reads them. Rows are addressed as in vb_task_score: x[r, c] = logits[r * ld_logits + col_off + c],
+ * or with ids (int64 [rows, cols]) logits[r * ld_logits + col_off + ids[r * cols + c]], an id outside [0, width - col_off)
+ * reading as NaN. Always argmax[r] (int64) = a, the argmax of row r with torch.max's rules (a NaN is the maximum, the first
+ * index wins among equals); then by mode
+ *   VB_RESULT_ARGMAX   nothing else (VL-classifier / GQA answers, V-logit-mc predictions; values may be NULL)
+ *   VB_RESULT_SOFTMAX  values[r * ld_values + c] = softmax(x[r, :])_c in fp32 (VL-logit option probabilities); a NaN or +inf in
+ *                      the row makes the whole row NaN, as torch.softmax does
+ *   VB_RESULT_GATHER   values[r] = target[r * ld_target + a] (V-logit: the IoU of the chosen region)
+ * A warp per row, eight rows per CTA, no atomics: every output is written once, results are deterministic. */
+enum { VB_RESULT_ARGMAX = 0, VB_RESULT_SOFTMAX = 1, VB_RESULT_GATHER = 2 };
+vb_status vb_task_results(int32_t mode, const float* logits, int64_t ld_logits, int32_t col_off, int32_t cols, const int64_t* ids,
+                          int32_t width, const float* target, int64_t ld_target, int32_t rows, int64_t* argmax, float* values,
+                          int64_t ld_values, void* stream);
 /* dst = src * (*scale), f32, scale read on the device: the backward of a forward-placed objective starts from the stored
  * d loss / d head times d(total) / d loss (loss_scale[task] / gradient_accumulation_steps, train_tasks.py:247-251, 545-548)
  * without a host synchronisation. */

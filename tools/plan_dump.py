@@ -56,6 +56,17 @@ def cases(O, LOSS_HEADS):
         ("task_binary_bce", {}, "vl", 4, obj("binary_bce", **task)),
         ("task_tri_bce", {}, "vl", 4, obj("tri_bce", **task)),
         ("task_binary_ce_nscore", {}, "vl", 4, obj("binary_ce", loss_in_forward=True)),
+        # forward-only evaluation plans that build only the head their task type reads, with the per-row results
+        # (vilbert_b200.tasks.EvaluatingModel)
+        ("eval_vqa", {}, "vl", 4, dict(outputs=("vil_prediction",), results="vqa")),
+        ("eval_gqa_odd", {}, "vl", 3, dict(outputs=("vil_prediction_gqa",), results="gqa")),
+        ("eval_logit_ce", {}, "vl", 4, dict(loss="logit_ce", choices=2, outputs=("vil_logit",), results="logit_ce", **task)),
+        ("eval_vlogit_bce", {}, "vl", 4, dict(loss="vlogit_bce", outputs=("vision_logit",), results="vlogit_bce", **task)),
+        ("eval_vlogit_mc", dict(task_specific_tokens=True), "vl", 4,
+         dict(loss="vlogit_mc", choices=6, outputs=("vision_logit",), results="vlogit_mc", **task), 110),
+        ("eval_binary_bce", {}, "vl", 4, dict(loss="binary_bce", outputs=("vil_binary_prediction",), **task)),
+        ("eval_binary_bce_odd", {}, "vl", 3, dict(loss="binary_bce", outputs=("vil_binary_prediction",), **task)),
+        ("eval_tri_bce", {}, "vl", 4, dict(loss="tri_bce", outputs=("vil_tri_prediction",), **task)),
         # the pre-training objective for every config.visual_target: summed, and with three losses placed at the end of the forward
         # (train, and eval without gradients)
         *[case for vt, over in ((0, {}), (1, dict(visual_target=1, v_target_size=48)), (2, dict(visual_target=2, v_target_size=48)))

@@ -11,6 +11,7 @@ LIB_PATH = os.path.join(_HERE, "libvilbert_b200.so")
 
 VB_ACT_NONE, VB_ACT_GELU, VB_ACT_RELU, VB_ACT_DGELU = 0, 1, 2, 3
 VB_SCORE_SOFT, VB_SCORE_LABEL, VB_SCORE_THRESHOLD, VB_SCORE_CHOICE = 0, 1, 2, 3
+VB_RESULT_ARGMAX, VB_RESULT_SOFTMAX, VB_RESULT_GATHER = 0, 1, 2
 
 
 class VBError(RuntimeError):
@@ -105,6 +106,7 @@ _SIGNATURES = {
     "vb_ce_loss": [_P, _I64, _P, _I64, _P, _P, _I64, _P, _I64, _I32, _I32, _F, _I32, _P],
     "vb_bce_gather_loss": [_P, _I64, _I32, _I32, _P, _P, _I32, _I32, _F, _P, _P, _I32, _P, _I64, _P, _I64, _P],
     "vb_task_score": [_I32, _P, _I64, _I32, _I32, _P, _I32, _P, _I64, _P, _I32, _P, _I32, _P, _P],
+    "vb_task_results": [_I32, _P, _I64, _I32, _I32, _P, _I32, _P, _I64, _I32, _P, _P, _I64, _P],
     "vb_scale_by_device": [_P, _P, _I64, _P, _P],
     "vb_kl_masked_loss": [_P, _P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _F, _I32, _P],
     "vb_mse_masked_loss": [_P, _P, _P, _I32, _I32, _I32, _F, _P, _P, _I32, _P, _P],

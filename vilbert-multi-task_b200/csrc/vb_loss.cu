@@ -337,6 +337,48 @@ task_score_kernel(int mode, const float* __restrict__ logits, long long ld, int 
   }
 }
 
+// per-row evaluation results (vb_task_results): one warp per row, RESULTS_ROWS rows per CTA, every row written by its own warp
+constexpr int RESULTS_ROWS = LOSS_THREADS / 32;
+
+__device__ __forceinline__ float result_logit(const float* zr, int off, const long long* idr, int width, int c) {
+  if (!idr) return zr[off + c];
+  const long long id = idr[c];
+  return (id >= 0 && id < (long long)(width - off)) ? zr[off + id] : CUDART_NAN_F;
+}
+
+__global__ void __launch_bounds__(LOSS_THREADS)
+task_results_kernel(int mode, const float* __restrict__ logits, long long ld, int off, int cols, const long long* __restrict__ ids,
+                    int width, const float* __restrict__ target, long long ldt, int rows, long long* __restrict__ argmax,
+                    float* __restrict__ values, long long ldv) {
+  pdl_entry();
+  const int lane = threadIdx.x & 31;
+  const int r = blockIdx.x * RESULTS_ROWS + (threadIdx.x >> 5);
+  if (r >= rows) return;
+  const float* zr = logits + (long long)r * ld;
+  const long long* idr = ids ? ids + (long long)r * cols : nullptr;
+  float v = -CUDART_INF_F;
+  int a = 0x7fffffff;
+  for (int c = lane; c < cols; c += 32) {
+    const float x = result_logit(zr, off, idr, width, c);
+    if (arg_better(x, c, v, a)) { v = x; a = c; }
+  }
+  warp_argmax(v, a);
+  if (lane == 0) {
+    argmax[r] = a;
+    if (mode == VB_RESULT_GATHER) values[r] = target[(long long)r * ldt + a];
+  }
+  if (mode != VB_RESULT_SOFTMAX) return;
+  // softmax(row) = exp(x - max) / sum: the exponentials in double (exact to the float result, whatever --use_fast_math does to
+  // expf) and summed in double; a NaN maximum (a NaN in the row) or an infinite one makes every probability NaN, as in torch
+  double s = 0.0;
+  for (int c = lane; c < cols; c += 32) s += exp((double)(result_logit(zr, off, idr, width, c) - v));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const double inv = 1.0 / s;
+  float* out = values + (long long)r * ldv;
+  for (int c = lane; c < cols; c += 32) out[c] = (float)(exp((double)(result_logit(zr, off, idr, width, c) - v)) * inv);
+}
+
 // ------------------------------------------------------------------------------------------ masked-region regression and NCE
 // Both objectives score rows [b, r+1] of prediction_scores_v (region 0, the global feature, is dropped) against target[b, r] and
 // label[b, r] == 1, R = Nv - 1. One CTA per row of scores (region 0 and unmasked rows write a zero gradient and a zero row loss);
@@ -506,6 +548,21 @@ extern "C" vb_status vb_task_score(int32_t mode, const float* logits, int64_t ld
              (long long)ld_logits, (int)col_off, (int)cols, reinterpret_cast<const long long*>(ids), (int)width, target, (long long)ld_target,
              reinterpret_cast<const long long*>(labels), (int)rows, score, (int)(accumulate ? 1 : 0), reinterpret_cast<long long*>(preds));
   return check_launch("vb_task_score");
+}
+
+extern "C" vb_status vb_task_results(int32_t mode, const float* logits, int64_t ld_logits, int32_t col_off, int32_t cols, const int64_t* ids,
+                                     int32_t width, const float* target, int64_t ld_target, int32_t rows, int64_t* argmax, float* values,
+                                     int64_t ld_values, void* stream) {
+  if (mode < VB_RESULT_ARGMAX || mode > VB_RESULT_GATHER || rows <= 0 || cols <= 0 || col_off < 0 || !logits || !argmax ||
+      (ids && width <= col_off) || (mode == VB_RESULT_GATHER && (!target || !values)) ||
+      (mode == VB_RESULT_SOFTMAX && (!values || ld_values < cols)))
+    return set_error(VB_ERR_INVALID, "vb_task_results: bad arguments (mode %d, rows %d, cols %d, col_off %d)", (int)mode, (int)rows,
+                     (int)cols, (int)col_off);
+  const int grid = (int)(((long long)rows + RESULTS_ROWS - 1) / RESULTS_ROWS);
+  launch_pdl(task_results_kernel, dim3(grid), dim3(LOSS_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), (int)mode, logits,
+             (long long)ld_logits, (int)col_off, (int)cols, reinterpret_cast<const long long*>(ids), (int)width, target, (long long)ld_target,
+             (int)rows, reinterpret_cast<long long*>(argmax), values, (long long)ld_values);
+  return check_launch("vb_task_results");
 }
 
 extern "C" vb_status vb_scale_by_device(const float* src, float* dst, int64_t n, const float* scale, void* stream) {

@@ -292,6 +292,13 @@ HEAD_NAMES = ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_p
               "vision_prediction", "vision_logit", "linguisic_prediction", "linguisic_logit")
 BERT_OUT_NAMES = ("sequence_output_t", "sequence_output_v", "pooled_output_t", "pooled_output_v")
 
+# per-row evaluation results of a task kind (EvaluatingModel, task_utils.py:777-847; Plan(results=...)): the head they read and the
+# mode of vb_task_results. VL-classifier / GQA: the answer index; VL-logit: the option probabilities; V-logit: the region and its
+# IoU; V-logit-mc: the chosen choice. The binary / tri types have no per-row results.
+RESULT_MODES = {"vqa": ("vil_prediction", L.VB_RESULT_ARGMAX), "gqa": ("vil_prediction_gqa", L.VB_RESULT_ARGMAX),
+                "logit_ce": ("vil_logit", L.VB_RESULT_SOFTMAX), "vlogit_bce": ("vision_logit", L.VB_RESULT_GATHER),
+                "vlogit_mc": ("vision_logit", L.VB_RESULT_ARGMAX)}
+
 
 class Plan:
     """Static execution plan for one input shape. `grad_outputs` names the outputs that will receive a
@@ -306,10 +313,16 @@ class Plan:
 
     loss="pretraining" with loss_in_forward=True keeps the three pre-training losses apart: self.objective_out (device f32 [3]) holds
     masked_lm, masked_img and next_sentence, self.loss is None, and self.loss_grad (f32 [3]) scales each head gradient by its own
-    slot. A plan without grad_outputs computes the losses only and writes no gradient."""
+    slot. A plan without grad_outputs computes the losses only and writes no gradient.
+
+    outputs: the heads (names of HEAD_NAMES) the plan builds; None builds all of them. A head not named gets no kernel, no buffer
+    and no entry in self.outputs (the four BertModel outputs are always there); what a kept head reads (the fused pooled vector,
+    the alignment head of an odd batch, dropout sites) is built as in the all-heads plan, so a kept head is bitwise the same.
+    results: a kind of RESULT_MODES; the forward ends with vb_task_results on that kind's head, and self.results_out packs
+    objective_out (loss, score), the per-row argmax and the per-row values into one device buffer (fetch_results)."""
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-                 loss_in_forward=False):
+                 loss_in_forward=False, outputs=None, results=None):
         self.e, self.cfg = engine, engine.cfg
         self.grad_touch = {}           # (flat offset, numel) -> index of the last backward op writing that gradient range
         self.ps = _TrackedParams(engine.ps, self)
@@ -355,6 +368,9 @@ class Plan:
         self.op_dtype, self.split = engine.op_dtype, engine.split   # format of the forward operands (activations, weights)
         self.head_dropout_prob = engine.head_dropout_prob
         self.heads = engine.ps.heads if heads is None else heads   # "vl" | "pretraining" | "none"
+        self.keep = None if outputs is None else frozenset(outputs)
+        self.results = results
+        self._check_outputs()
         self.fwd_id = 0
         self.fwd, self.bwd = [], []
         self.prologue = []       # optional per-step ops run before the forward (see enable_training_prologue)
@@ -374,6 +390,37 @@ class Plan:
         self._eager_runs = [0, 0]      # eager forward / backward executions (maybe_capture_passes)
         self._arena_off = self.arena_bytes = 0
         self._build()
+
+    def _check_outputs(self):
+        """Build-time checks of outputs= and results=: known head names, and every head the objective, a gradient or the results
+        read is kept."""
+        k, r = self.loss_kind, self.results
+        if r is not None:
+            if r not in RESULT_MODES:
+                raise ValueError(f"results must be one of {sorted(RESULT_MODES)}, got {r!r}")
+            if k is not None and (k != r or not self.loss_in_forward):
+                raise ValueError(f"results={r!r} goes with loss=None or loss={r!r}, loss_in_forward=True (got loss={k!r})")
+            if r not in ("vqa", "gqa") and k != r:
+                raise ValueError(f"results={r!r} reads the inputs of its objective: build it with loss={r!r}, loss_in_forward=True")
+        if self.keep is None:
+            return
+        unknown = sorted(n for n in self.keep if n not in HEAD_NAMES)
+        if unknown:
+            raise ValueError(f"outputs: unknown head name(s) {unknown}; the heads are {HEAD_NAMES}")
+        if self.heads != "vl":
+            raise ValueError(f"outputs= selects among the heads of VILBertForVLTasks (heads='vl'), not heads={self.heads!r}")
+        need = {n for n in self.grad_outputs if n in HEAD_NAMES}
+        if k is not None:
+            need |= set(LOSS_HEADS[k])
+        if r is not None:
+            need.add(RESULT_MODES[r][0])
+        missing = sorted(need - self.keep)
+        if missing:
+            raise ValueError(f"outputs={sorted(self.keep)} misses {missing}, which the plan's objective, gradients or results read")
+
+    def want(self, name):
+        """Whether the head `name` is built (outputs=)."""
+        return self.keep is None or name in self.keep
 
     # ------------------------------------------------------------------ infrastructure
     def buf(self, shape, dtype=F32, zero=False):
@@ -1120,27 +1167,17 @@ class Plan:
             return act
         # VILBertForVLTasks.dropout on the fused vector (vilbert.py:1677-1682); BertPreTrainingHeads has its own nn.Dropout(0.1)
         # on its own fused vector (:1233-1241) — a different mask, needed only where the alignment score is an output
-        fused = fuse(self.drop("dropout.pooled", self.head_dropout_prob)) if self.heads == "vl" else None
-        need_cls_fused = self.heads == "pretraining" or (B % 2 == 1)
+        # outputs=: the fused vector feeds the vil_* heads (the binary one only at even B), the alignment head the binary one at odd B
+        want = self.want
+        need_fused = any(want(n) for n in ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_tri_prediction")) or (
+            want("vil_binary_prediction") and B % 2 == 0)
+        fused = fuse(self.drop("dropout.pooled", self.head_dropout_prob)) if self.heads == "vl" and need_fused else None
+        need_cls_fused = self.heads == "pretraining" or (B % 2 == 1 and want("vil_binary_prediction"))
         cls_drop = self.drop("cls.dropout", 0.1)
         if need_cls_fused:
             fused_cls = fuse(cls_drop) if (cls_drop is not None or fused is None) else fused
         else:
             fused_cls = None
-
-        # --- cls: masked-LM head (decoder tied to the word embeddings), image-region head, alignment head
-        ht, ht_bwd = self.transform(seq_t, "cls.predictions.transform.dense", "cls.predictions.transform.LayerNorm", "lm.tr")
-        # fused pre-training objective: only the masked rows enter the LM cross-entropy, so the tied decoder runs on those alone
-        self.lm_c = None
-        if self.loss_kind == "pretraining" and self.e.lm_compact:
-            lm_bwd = None
-            lm_compact_bwd = self.lm_head_compact(ht, ht_bwd)
-        else:
-            lm_bwd = self.big_head("linguisic_prediction", ht, Ht, B * Nt, Ht, c.vocab_size, None, "cls.predictions.bias",
-                                   w=ps.w("bert.embeddings.word_embeddings.weight"), gw=ps.g("bert.embeddings.word_embeddings.weight"))
-        hv, hv_bwd = self.transform(seq_v, "cls.imagePredictions.transform.dense", "cls.imagePredictions.transform.LayerNorm", "im.tr")
-        im_bwd = self.big_head("vision_prediction", hv, Hv, B * Nv, Hv, c.v_target_size, "cls.imagePredictions.decoder",
-                               "cls.imagePredictions.decoder.bias")
 
         def wide_bwd(head_bwd, hn, tr_bwd, K, N_out):
             def f():
@@ -1153,14 +1190,32 @@ class Plan:
                 hn.gw = True
                 tr_bwd()
             return f
-        self.push_bwd(wide_bwd(lm_bwd, ht, ht_bwd, Ht, c.vocab_size) if lm_bwd is not None else lm_compact_bwd)
-        self.push_bwd(wide_bwd(im_bwd, hv, hv_bwd, Hv, c.v_target_size))
+
+        # --- cls: masked-LM head (decoder tied to the word embeddings), image-region head, alignment head
+        self.lm_c = None
+        if want("linguisic_prediction"):
+            ht, ht_bwd = self.transform(seq_t, "cls.predictions.transform.dense", "cls.predictions.transform.LayerNorm", "lm.tr")
+            # fused pre-training objective: only the masked rows enter the LM cross-entropy, so the tied decoder runs on those alone
+            if self.loss_kind == "pretraining" and self.e.lm_compact:
+                lm_bwd = None
+                lm_compact_bwd = self.lm_head_compact(ht, ht_bwd)
+            else:
+                lm_bwd = self.big_head("linguisic_prediction", ht, Ht, B * Nt, Ht, c.vocab_size, None, "cls.predictions.bias",
+                                       w=ps.w("bert.embeddings.word_embeddings.weight"), gw=ps.g("bert.embeddings.word_embeddings.weight"))
+        if want("vision_prediction"):
+            hv, hv_bwd = self.transform(seq_v, "cls.imagePredictions.transform.dense", "cls.imagePredictions.transform.LayerNorm", "im.tr")
+            im_bwd = self.big_head("vision_prediction", hv, Hv, B * Nv, Hv, c.v_target_size, "cls.imagePredictions.decoder",
+                                   "cls.imagePredictions.decoder.bias")
+        if want("linguisic_prediction"):
+            self.push_bwd(wide_bwd(lm_bwd, ht, ht_bwd, Ht, c.vocab_size) if lm_bwd is not None else lm_compact_bwd)
+        if want("vision_prediction"):
+            self.push_bwd(wide_bwd(im_bwd, hv, hv_bwd, Hv, c.v_target_size))
 
         if self.heads == "pretraining":
             # BertForMultiModalPreTraining returns the alignment score of self.cls (vilbert.py:1497)
             self.small_head("seq_relationship_score", fused_cls, "cls.bi_seq_relationship", 2)
             return
-        if B % 2 == 0:
+        if want("vil_binary_prediction") and B % 2 == 0:
             # vil_binary_prediction pairs consecutive samples: pooled.view(-1, 2*Hb) (:1686-1689)
             pair = Act(fused.f32.view(B // 2, 2 * Hb), fused.op.view(B // 2, 2 * Hb), B // 2, 2 * Hb)
             hb, hb_bwd = self.transform(pair, "vil_binary_prediction.logit_fc.0", "vil_binary_prediction.logit_fc.2", "bin.tr")
@@ -1180,18 +1235,25 @@ class Plan:
                     self.add_grad(fused, pair.g32.view(B, Hb))
             self.push_bwd(bin_bwd)   # registered first => runs after the 2-way linear's backward
             self.small_head("vil_binary_prediction", hb, "vil_binary_prediction.logit_fc.3", 2)
-        else:
+        elif want("vil_binary_prediction"):
             # odd batch: the reference returns the [B, 2] alignment output of self.cls here (:1673, 1686)
             self.small_head("vil_binary_prediction", fused_cls, "cls.bi_seq_relationship", 2)
 
         for nm, n_out in (("vil_prediction", 3129), ("vil_prediction_gqa", 1533)):
+            if not want(nm):
+                continue
             hh, hh_bwd = self.transform(fused, nm + ".logit_fc.0", nm + ".logit_fc.2", nm + ".tr")
             head_bwd = self.big_head(nm, hh, 2 * Hb, B, 2 * Hb, n_out, nm + ".logit_fc.3", nm + ".logit_fc.3.bias")
             self.push_bwd(wide_bwd(head_bwd, hh, hh_bwd, 2 * Hb, n_out))
-        self.small_head("vil_logit", fused, "vil_logit", 1)
-        self.small_head("vil_tri_prediction", fused, "vil_tri_prediction", 3)
-        self.small_head("vision_logit", seq_v, "vision_logit", 1, addend=self.mask_v, in_drop=self.drop("dropout.seq_v", self.head_dropout_prob))
-        self.small_head("linguisic_logit", seq_t, "linguisic_logit", 1, in_drop=self.drop("dropout.seq_t", self.head_dropout_prob))
+        if want("vil_logit"):
+            self.small_head("vil_logit", fused, "vil_logit", 1)
+        if want("vil_tri_prediction"):
+            self.small_head("vil_tri_prediction", fused, "vil_tri_prediction", 3)
+        if want("vision_logit"):
+            self.small_head("vision_logit", seq_v, "vision_logit", 1, addend=self.mask_v,
+                            in_drop=self.drop("dropout.seq_v", self.head_dropout_prob))
+        if want("linguisic_logit"):
+            self.small_head("linguisic_logit", seq_t, "linguisic_logit", 1, in_drop=self.drop("dropout.seq_t", self.head_dropout_prob))
 
     # ------------------------------------------------------------------ whole model
     def _build(self):
@@ -1204,6 +1266,10 @@ class Plan:
             # masked_lm, masked_img, next_sentence side by side: one device-to-host copy reads all three
             self.objective_out = self.buf((3,), F32, zero=True)
             self.loss = None
+        elif self.results is not None:
+            self._alloc_results()
+            self.loss = self.objective_out[0:1] if self.task_objective else None
+            self.score = self.objective_out[1:2] if self.want_score else None
         elif self.task_objective:
             # loss and score side by side: one device-to-host copy reads both
             self.objective_out = self.buf((2,), F32, zero=True)
@@ -1273,6 +1339,8 @@ class Plan:
         self.sync_streams(mirror=False)
         if self.loss_in_forward:
             self._emit_loss()
+        if self.results is not None:
+            self._emit_results()
         self.n_kernels_fwd = sum(1 for op in self.fwd if op[0] is not None)
 
         # ---------------- backward
@@ -1472,6 +1540,48 @@ class Plan:
         self.preds = self.buf((rows,), I64, zero=True)
         self.emit(self.lib.vb_task_score, mode, lg.data_ptr(), ld, off, cols, self._ptr(ids), width, self._ptr(target),
                   cols if target is not None else 0, self._ptr(labels), rows, self.score.data_ptr(), 0, self.preds.data_ptr())
+
+    def _results_shape(self):
+        """(rows, columns, values per row) of the results of self.results: VL-logit has a row per question over its options."""
+        k = self.results
+        if k in ("vqa", "gqa"):
+            return self.B, (3129 if k == "vqa" else 1533), 0
+        if k == "logit_ce":
+            opts = self.choices or self.e.loss_options
+            return self.B // opts, opts, opts
+        if k == "vlogit_bce":
+            return self.B, self.Nv, 1
+        return self.B, int(self.choices), 0          # vlogit_mc
+
+    def _alloc_results(self):
+        """One private device buffer: objective_out (f32 loss, score), the per-row argmax (int64) and the per-row values (f32)."""
+        rows, _, nval = self._results_shape()
+        self.results_out = self.buf((8 + 8 * rows + 4 * rows * nval,), torch.uint8, zero=True)
+        self.objective_out = self.results_out[:8].view(F32)
+        self.results_argmax = self.results_out[8:8 + 8 * rows].view(I64)
+        self.results_values = self.results_out[8 + 8 * rows:].view(F32).view(rows, nval) if nval else None
+
+    def _emit_results(self):
+        """vb_task_results on the head of self.results (RESULT_MODES), addressed as the score kernel addresses it."""
+        k, li, Nv = self.results, self.loss_inputs, self.Nv
+        name, mode = RESULT_MODES[k]
+        rows, cols, nval = self._results_shape()
+        ids, width, off, target, ld = None, 0, 0, None, cols
+        if k == "vlogit_bce":
+            target = li["target"]
+        elif k == "vlogit_mc":
+            ids, width, off, ld = li["multiple_choice_ids"], Nv, MC_REGION_OFFSET, Nv
+        self.emit(self.lib.vb_task_results, mode, self.outputs[name].data_ptr(), ld, off, cols, self._ptr(ids), width, self._ptr(target),
+                  Nv if target is not None else 0, rows, self.results_argmax.data_ptr(), self._ptr(self.results_values), max(nval, 1))
+
+    def fetch_results(self):
+        """Reads results_out with one device-to-host copy: (loss, score, argmax int64 [rows], values f32 [rows, n] or None) on the
+        host. loss and score are 0 where the plan has no objective / score."""
+        raw = self.results_out.cpu()
+        rows, _, nval = self._results_shape()
+        loss, score = raw[:8].view(F32).tolist()
+        vals = raw[8 + 8 * rows:].view(F32).view(rows, nval) if nval else None
+        return loss, score, raw[8:8 + 8 * rows].view(I64), vals
 
     def _emit_grad_scale(self):
         """Backward of a forward-placed objective: head gradient = stored d loss / d head x self.loss_grad (device scalar). The
@@ -1876,18 +1986,19 @@ class Engine:
         self.lm_capacity = 0.25          # ... with room for this fraction of the token rows (15 % are masked; more poisons the loss with NaN)
 
     def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-             loss_in_forward=False):
+             loss_in_forward=False, outputs=None, results=None):
         """The cached plan of this shape and these options (Plan)."""
         loss = "vqa" if vqa_loss else loss
         pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
-        key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward))
+        key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward),
+               None if outputs is None else frozenset(outputs), results)
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]
         while len(self.plans) >= self.max_plans:   # evict the least recently used plan: its buffers go back to the allocator
             self.plans.popitem(last=False)
         self.plans[key] = Plan(self, B, Nt, Nv, grad_outputs, False, heads, train, loss=loss, choices=choices, score=score,
-                               loss_in_forward=loss_in_forward)
+                               loss_in_forward=loss_in_forward, outputs=outputs, results=results)
         return self.plans[key]
 
     def enable_activation_arena(self, nbytes):

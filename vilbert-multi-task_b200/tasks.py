@@ -1,7 +1,7 @@
-"""Drop-in replacements for the reference's per-task training and validation steps, ForwardModelsTrain and ForwardModelsVal
-(vilbert/task_utils.py:31-376), with the same signatures and return values:
+"""Drop-in replacements for the reference's per-task training, validation and evaluation steps, ForwardModelsTrain,
+ForwardModelsVal (vilbert/task_utils.py:31-376) and EvaluatingModel (:626-859), with the same signatures and return values:
 
-    from vilbert_b200.tasks import ForwardModelsTrain, ForwardModelsVal, LoadLosses
+    from vilbert_b200.tasks import EvaluatingModel, ForwardModelsTrain, ForwardModelsVal, LoadLosses
 
 Each call runs ONE plan of the engine in which the task's objective and its batch score are fused kernels at the end of the forward
 (Plan(loss_in_forward=True, score=True)): no head outputs are cloned, no torch loss is formed, and no score is read back to the host.
@@ -20,7 +20,7 @@ import torch
 import torch.nn as nn
 
 from .data import expand_batch
-from .engine import LOSS_HEADS
+from .engine import LOSS_HEADS, RESULT_MODES
 
 LossMap = {
     "BCEWithLogitLoss": nn.BCEWithLogitsLoss,
@@ -85,7 +85,7 @@ def _unpack(task_id, batch):
 class _Step:
     """One task batch on the device, reshaped for the model, with its plan built and inputs loaded."""
 
-    def __init__(self, task_cfg, task_id, batch, model, train, grad, processes):
+    def __init__(self, task_cfg, task_id, batch, model, train, grad, processes, evaluate=False):
         eng = model.engine
         self.kind = kind = task_kind(task_cfg, task_id)
         features, spatials, image_mask, question, target, input_mask, segment_ids, mc_ids, _ = _unpack(task_id, batch)
@@ -108,8 +108,15 @@ class _Step:
             choices = num_options
         elif kind == "vlogit_mc":
             choices = mc_ids.size(1)
-        self.plan = plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS[kind] if grad else (), train=train, loss=kind, choices=choices,
-                                    score=kind not in _NO_SCORE, loss_in_forward=True)
+        if evaluate:
+            # EvaluatingModel: a forward-only plan of the one head the type reads; VL-classifier / GQA have no loss and no score
+            has_loss = kind not in ("vqa", "gqa")
+            self.plan = plan = eng.plan(B, Nt, Nv, train=train, loss=kind if has_loss else None, choices=choices,
+                                        score=has_loss and kind not in _NO_SCORE, loss_in_forward=has_loss, outputs=LOSS_HEADS[kind],
+                                        results=kind if kind in RESULT_MODES else None)
+        else:
+            self.plan = plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS[kind] if grad else (), train=train, loss=kind, choices=choices,
+                                        score=kind not in _NO_SCORE, loss_in_forward=True)
         self.inputs = dict(input_txt=question, input_imgs=features, image_loc=spatials, token_type_ids=segment_ids, attention_mask=input_mask,
                            image_attention_mask=image_mask, task_ids=task_tokens)
         self.targets = {}
@@ -120,7 +127,7 @@ class _Step:
                 # refuses the int labels of every sample, as F.cross_entropy does in the reference
                 raise ValueError(f"Expected input batch_size ({li['labels'].numel()}) to match target batch_size ({target.numel()}).")
             self.targets["labels"] = target.reshape(li["labels"].shape)
-        else:
+        elif "target" in li:
             self.targets["target"] = target.reshape(li["target"].shape)
         if mc_ids is not None and "multiple_choice_ids" in li:
             self.targets["multiple_choice_ids"] = mc_ids
@@ -227,4 +234,52 @@ def ForwardModelsVal(args, task_cfg, device, task_id, batch, model, task_losses)
     return loss, score, step.batch_size
 
 
-__all__ = ["ForwardModelsTrain", "ForwardModelsVal", "LoadLosses", "TASK_KINDS", "task_kind"]
+# the objective kinds EvaluatingModel forms results for (task_utils.py:777-857); binary_ce (Foil) fails like ForwardModelsVal
+_EVAL_KINDS = ("vqa", "gqa", "logit_ce", "vlogit_bce", "vlogit_mc", "binary_bce", "tri_bce", "binary_ce")
+
+
+def EvaluatingModel(args, task_cfg, device, task_id, batch, model, task_dataloader, task_losses, results, others):
+    """task_utils.py:626-859: (float(loss), float(batch_score), batch_size, results, others), the result dicts of the task type
+    appended to `results`. One forward-only plan in the model's current mode builds only the head the type reads and ends with the
+    type's objective, its score and vb_task_results (argmax, option probabilities or the IoU at the argmax); one device-to-host
+    copy reads loss, score and every per-row result, and the dicts are built on the host. question_id is read from the batch as
+    passed in; a row without an id (VisDial's `dialog` batches carry one id per image for batch_size * rounds rows) raises
+    IndexError after the rows before it are appended, as in the reference."""
+    kind = task_kind(task_cfg, task_id)
+    if kind not in _EVAL_KINDS:
+        raise NotImplementedError(f"{task_id}: EvaluatingModel has no result for task type {task_cfg[task_id]['type']!r} with loss "
+                                  f"{task_cfg[task_id]['loss']!r}")
+    question_id = batch[-1].tolist()
+    batch = tuple(t.cuda(device=device, non_blocking=True) for t in batch)
+    m = _model(model)
+    if kind not in ("vqa", "gqa"):            # VL-classifier / GQA do not read task_losses
+        _check_loss(task_cfg, task_id, task_losses)
+    with torch.no_grad():
+        step = _Step(task_cfg, task_id, batch, m, bool(m.training), False, ("dialog", "expand", "retrieval", "nlvr"), evaluate=True)
+        step.score_error()
+        step.forward()
+        plan = step.plan
+        if plan.results is None:              # VL-binary / VL-tri: loss and score only
+            loss, score = plan.objective_out.tolist()
+            return loss, score, step.batch_size, results, others
+        loss, score, argmax, values = plan.fetch_results()
+    pick = argmax.tolist()
+    if kind in ("vqa", "gqa"):
+        label2ans = task_dataloader[task_id].dataset.label2ans
+        for i, a in enumerate(pick):
+            results.append({"question_id": question_id[i], "answer": label2ans[a]} if kind == "vqa" else
+                           {"questionId": str(question_id[i]), "prediction": label2ans[a]})
+    elif kind == "logit_ce":
+        for i, probs in enumerate(values.tolist()):
+            results.append({"question_id": question_id[i], "answer": probs})
+    elif kind == "vlogit_bce":
+        iou = values.view(-1).tolist()
+        for i, a in enumerate(pick):
+            results.append({"id": question_id[i], "target": a, "IOU": iou[i]})
+    else:                                     # vlogit_mc
+        for i, a in enumerate(pick):
+            results.append({"id": question_id[i], "target": a})
+    return loss, score, step.batch_size, results, others
+
+
+__all__ = ["EvaluatingModel", "ForwardModelsTrain", "ForwardModelsVal", "LoadLosses", "TASK_KINDS", "task_kind"]
