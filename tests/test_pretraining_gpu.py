@@ -1,6 +1,6 @@
 """The fused pre-training objective on the GPU: the masked-MSE and NCE region kernels through the C ABI against the float64 closed
 forms, and BertForMultiModalPreTraining(fused_objective=True) against the reference's recorded losses, the oracle and the module's
-own torch objective, with per-loss gradient scaling, graph replay, recomputation and the capacity limit."""
+own torch objective, with per-loss gradient scaling, graph replay and the capacity limit (recomputation: test_replay_gpu.py)."""
 import ctypes as C
 import json
 import math
@@ -322,31 +322,6 @@ def test_graph_replay_matches_eager(golden_dir):
     (l0, g0), (l3, g3) = res[0], res[3]
     assert torch.equal(l0, l3) or torch.allclose(l0, l3, rtol=1e-6, atol=0)
     assert ((g3 - g0).abs().max() / g0.abs().max()).item() < 1e-5
-
-
-@pytest.mark.parametrize("arena", [False, True])
-def test_forward_of_another_shape_in_between(golden_dir, arena):
-    """Another plan's forward between forward and backward (and, with the shared arena, over the saved activations): the backward
-    recomputes the forward with the same inputs, negatives and dropout masks."""
-    cfgj = _cfgj(golden_dir, "tiny_visual_target_2")[1]
-    model, cfg, _ = _model(cfgj)
-    if arena:
-        model.engine.enable_activation_arena(256 << 20)
-    model.train()
-    a, b = _args(cfg, 4, 9, 8, 2), _args(cfg, 6, 11, 10, 2, seed=3)
-    # every call draws new negatives from torch's CPU generator: a recomputation that drew again would change the gradient
-    model.nce_sampler = lambda bb, r, dev: O.nce_negative_indices(bb, r, cfg["num_negative"]).to(dev)
-    torch.manual_seed(1)
-    model.engine.set_dropout_step(5); model.zero_grad()
-    sum(model(*a)).sum().backward()
-    want = model.engine.ps.grad.clone()
-    torch.manual_seed(1)
-    model.engine.set_dropout_step(5); model.zero_grad()
-    la = model(*a)
-    model(*b)
-    model.zero_grad()
-    sum(la).sum().backward()
-    assert ((model.engine.ps.grad - want).abs().max() / want.abs().max()).item() < 1e-5
 
 
 def test_labels_beyond_the_capacity_give_a_nan_masked_lm_loss(golden_dir):

@@ -1676,8 +1676,13 @@ class Plan:
             self._run(self.fwd)
             self._eager_runs[0] += 1
 
+    def holds_forward(self, fwd_id):
+        """The activations are still those of this plan's forward `fwd_id`: no later forward of this plan ran and, with the shared
+        arena, no other plan's forward overwrote them."""
+        return self.fwd_id == fwd_id and (self.e.arena is None or self.e.arena_owner == (self, fwd_id))
+
     def run_backward(self):
-        if self.e.arena is not None and self.e.arena_owner != (self, self.fwd_id):
+        if not self.holds_forward(self.fwd_id):
             raise L.VBError("shared activation arena: another plan's forward ran between this plan's forward and backward "
                             "(its saved activations are gone); run forward + backward per batch, or disable the arena")
         self.e.grad_clean = False

@@ -74,64 +74,106 @@ def _attach(root, dotted, prm):
     mod.register_parameter(parts[-1], prm)
 
 
-class _EngineFn(torch.autograd.Function):
-    """Bridges the engine's static plans into torch.autograd: forward runs the plan's forward pass and returns
-    its outputs; backward copies d(loss)/d(outputs) into the plan's static buffers and runs the hand-written
-    backward pass, which accumulates parameter gradients directly into the flat gradient buffer (the
-    Parameters' .grad are views of it). A plan is specialised on the set of outputs that receive a gradient;
-    the set seen in the previous backward of a shape is used as the hint for the next forward, so in a
-    steady training loop forward and backward share one plan and nothing is recomputed."""
+class _PlanCall:
+    """One call of the module surface on an engine plan: the model, the plan, its inputs and loss-input targets, and the dropout
+    step and forward id its forward() ran at. With `names` the call returns those plan outputs and takes their gradients into
+    plan.gout; without, it returns the plan's objective (the task loss as a 0-d tensor, or the three [1] pre-training losses) and
+    takes d(total)/d(loss) into plan.loss_grad, 0 for a loss that receives none.
 
-    @staticmethod
-    def forward(ctx, model, names, anchor, inputs):
-        Nt = inputs["input_txt"].shape[1]
-        B, Nv = inputs["input_imgs"].shape[:2]     # FAST_MODE: the text batch is 1, the image batch sets the plan
-        train = bool(model.training)
-        hint = model._grad_hint.get((B, Nt, Nv, names, train), ())
-        plan = model.engine.plan(B, Nt, Nv, grad_outputs=hint, heads=model._heads_for(names), train=train)
+    backward() always runs at its own forward. If the plan no longer holds that forward (the plan ran again, another plan
+    overwrote the shared arena, or the backward switched to the plan of another gradient set), the forward is recomputed from the
+    same inputs and targets. In train mode, if another forward moved the dropout step since, the step of this forward is set
+    around the recomputed forward and the backward, which regenerate their dropout masks from it, and restored afterwards. The
+    backward accumulates into the flat gradient buffer (the Parameters' .grad are views of it) and ends with the data-parallel
+    all-reduce when one is attached."""
+
+    def __init__(self, model, plan, inputs, targets=None, names=None):
+        self.model, self.plan, self.inputs, self.targets, self.names = model, plan, inputs, targets or {}, names
+        self.drop_step = self.fwd_id = None
+
+    def _load(self):
+        plan = self.plan
+        plan.load_inputs(**self.inputs)
+        li = plan.loss_inputs
+        for k, v in self.targets.items():
+            li[k].copy_(v.reshape(li[k].shape), non_blocking=True)
+
+    def forward(self):
+        model, plan, eng = self.model, self.plan, self.model.engine
         model._sync_weights()
-        if train:
-            model.engine.bump_dropout_step()      # fresh nn.Dropout masks for this forward
-        plan.load_inputs(**inputs)
-        if model.engine.auto_graph:
+        if plan.train:
+            eng.bump_dropout_step()      # fresh nn.Dropout masks for this forward
+        self.drop_step = eng.drop_step_host
+        self._load()
+        if eng.auto_graph:
             plan.maybe_capture_passes()
         plan.run_forward()
-        ctx.model, ctx.names, ctx.inputs, ctx.plan, ctx.fwd_id, ctx.train = model, names, inputs, plan, plan.fwd_id, train
-        ctx.drop_step = int(model.engine.drop_step_host)     # the masks this forward used (needed if it has to be recomputed)
+        self.fwd_id = plan.fwd_id
         model._last_plan = plan
+
+    def outputs(self):
+        plan = self.plan
+        if self.names is not None:
+            return tuple(plan.outputs[n].clone() for n in self.names)
+        if plan.loss_kind == "pretraining":
+            out = plan.objective_out.detach()
+            return out[0:1].clone(), out[1:2].clone(), out[2:3].clone()
+        return (plan.loss.detach().reshape(()).clone(),)
+
+    def backward(self, grads):
+        model, eng = self.model, self.model.engine
+        if self.names is not None:
+            live = tuple(n for n, g in zip(self.names, grads) if g is not None)
+            if frozenset(live) != self.plan.grad_outputs:     # the plan's backward reaches other outputs: take the plan of this set
+                self.plan = model._outputs_plan(self.names, self.inputs, self.plan.train, live)
+                self.fwd_id = None
+        plan = self.plan
+        now = eng.drop_step_host
+        moved = plan.train and now != self.drop_step
+        if moved:
+            eng.set_dropout_step(self.drop_step)
+        try:
+            if not plan.holds_forward(self.fwd_id):
+                self._load()
+                plan.run_forward()
+                self.fwd_id = plan.fwd_id
+            model._attach_grads()
+            if eng.auto_graph:
+                plan.maybe_capture_passes()
+            if self.names is not None:
+                for n, g in zip(self.names, grads):
+                    if g is not None:
+                        plan.gout[n].copy_(g.reshape(plan.gout[n].shape))
+            else:
+                for i, g in enumerate(grads):
+                    if g is None:
+                        plan.loss_grad[i:i + 1].zero_()
+                    else:
+                        plan.loss_grad[i:i + 1].copy_(g.detach().reshape(1))
+            plan.run_backward()
+        finally:
+            if moved:
+                eng.set_dropout_step(now)
+        if model._ddp_reducer is not None:     # data parallel: average the flat gradient buffer over the ranks (apex DDP, delay_allreduce=True)
+            model._ddp_reducer.allreduce()
+
+
+class _PlanFn(torch.autograd.Function):
+    """Bridges a _PlanCall into torch.autograd: forward runs the call's forward and returns its outputs, backward hands the
+    incoming gradients to the call's backward (nothing runs when none of them is live)."""
+
+    @staticmethod
+    def forward(ctx, anchor, call):
+        ctx.call = call
         ctx.set_materialize_grads(False)
-        return tuple(plan.outputs[n].clone() for n in names)
+        call.forward()
+        return call.outputs()
 
     @staticmethod
     def backward(ctx, *grads):
-        model, names, inputs, plan = ctx.model, ctx.names, ctx.inputs, ctx.plan
-        live = tuple(n for n, g in zip(names, grads) if g is not None)
-        if live:
-            Nt = inputs["input_txt"].shape[1]
-            B, Nv = inputs["input_imgs"].shape[:2]
-            clobbered = model.engine.arena is not None and model.engine.arena_owner != (plan, ctx.fwd_id)   # another plan used the shared arena
-            if frozenset(live) != plan.grad_outputs or plan.fwd_id != ctx.fwd_id or clobbered:
-                model._grad_hint[(B, Nt, Nv, names, ctx.train)] = live
-                plan = model.engine.plan(B, Nt, Nv, grad_outputs=live, heads=model._heads_for(names), train=ctx.train)
-                plan.load_inputs(**inputs)     # different plan (or overwritten activations): recompute the forward ...
-                eng = model.engine
-                now = int(eng.drop_step_host)
-                if ctx.train and now != ctx.drop_step:
-                    eng.set_dropout_step(ctx.drop_step)   # ... with the dropout masks of the forward the loss was computed on
-                    plan.run_forward()
-                    eng.set_dropout_step(now)
-                else:
-                    plan.run_forward()
-            model._attach_grads()
-            if model.engine.auto_graph:
-                plan.maybe_capture_passes()
-            for n, g in zip(names, grads):
-                if g is not None:
-                    plan.gout[n].copy_(g.reshape(plan.gout[n].shape))
-            plan.run_backward()
-            if model._ddp_reducer is not None:     # data parallel: average the flat gradient buffer over the ranks (apex DDP, delay_allreduce=True)
-                model._ddp_reducer.allreduce()
-        return None, None, None, None
+        if any(g is not None for g in grads):
+            ctx.call.backward(grads)
+        return None, None
 
 
 class BertPreTrainedModel(nn.Module):
@@ -325,10 +367,25 @@ class BertPreTrainedModel(nn.Module):
         return (seq_t, seq_v, o["pooled_output_t"], o["pooled_output_v"], self._attention_masks(output_all_attention_masks))
 
     # ---- shared forward machinery
+    def _outputs_plan(self, names, inputs, train, live=None):
+        """The plan of the outputs `names`. A plan is specialised on the set of outputs that receive a gradient; the set `live` a
+        backward found is kept as the hint for the next forward of this shape, so in a steady training loop forward and backward
+        share one plan and nothing is recomputed."""
+        Nt = inputs["input_txt"].shape[1]
+        B, Nv = inputs["input_imgs"].shape[:2]     # FAST_MODE: the text batch is 1, the image batch sets the plan
+        key = (B, Nt, Nv, names, train)
+        if live is None:
+            live = self._grad_hint.get(key, ())
+        else:
+            self._grad_hint[key] = live
+        return self.engine.plan(B, Nt, Nv, grad_outputs=live, heads=self._heads_for(names), train=train)
+
     def _run(self, names, input_txt, input_imgs, image_loc, token_type_ids, attention_mask, image_attention_mask, task_ids):
         inputs = dict(input_txt=input_txt, input_imgs=input_imgs, image_loc=image_loc, token_type_ids=token_type_ids,
                       attention_mask=attention_mask, image_attention_mask=image_attention_mask, task_ids=task_ids)
-        outs = _EngineFn.apply(self, tuple(names), self._anchor, inputs)
+        names = tuple(names)
+        plan = self._outputs_plan(names, inputs, bool(self.training))
+        outs = _PlanFn.apply(self._anchor, _PlanCall(self, plan, inputs, names=names))
         return dict(zip(names, outs))
 
 
@@ -369,87 +426,6 @@ class VILBertForVLTasks(BertPreTrainedModel):
             raise TypeError("image_attention_mask is required by VILBertForVLTasks.forward (vilbert.py:1693)")
         o = self._run(HEAD_NAMES, input_txt, input_imgs, image_loc, token_type_ids, attention_mask, image_attention_mask, task_ids)
         return tuple(o[n] for n in HEAD_NAMES) + (self._attention_masks(output_all_attention_masks),)
-
-
-class _PretrainStep:
-    """One labelled pre-training batch with its plan (Plan(loss="pretraining", loss_in_forward=True)), inputs and NCE negatives."""
-
-    def __init__(self, model, inputs, targets, grad):
-        eng = model.engine
-        Nt = inputs["input_txt"].shape[1]
-        B, Nv = inputs["input_imgs"].shape[:2]
-        self.train = bool(model.training)
-        self.plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS["pretraining"] if grad else (), train=self.train, loss="pretraining",
-                             loss_in_forward=True)
-        self.model, self.inputs, self.targets = model, inputs, targets
-
-    def load(self):
-        self.plan.load_inputs(**self.inputs)
-        li = self.plan.loss_inputs
-        for k, v in self.targets.items():
-            li[k].copy_(v.reshape(li[k].shape), non_blocking=True)
-
-    def forward(self):
-        model, plan = self.model, self.plan
-        model._sync_weights()
-        if self.train:
-            model.engine.bump_dropout_step()
-        self.drop_step = int(model.engine.drop_step_host)
-        self.load()
-        if model.engine.auto_graph:
-            plan.maybe_capture_passes()
-        plan.run_forward()
-        self.fwd_id = plan.fwd_id
-        model._last_plan = plan
-
-
-class _PretrainLossFn(torch.autograd.Function):
-    """The three losses of the fused pre-training objective. backward copies (d total / d masked_lm, d masked_img, d next_sentence)
-    into the plan's loss_grad on the device (an unused loss contributes 0) and runs the plan's backward into the flat gradient
-    buffer, then the data-parallel all-reduce when one is attached. The backward runs at the dropout step of its forward; if
-    this plan ran again since, or the shared arena was overwritten, the forward is recomputed first with the same inputs,
-    negatives and dropout masks."""
-
-    @staticmethod
-    def forward(ctx, anchor, step):
-        ctx.step = step
-        ctx.set_materialize_grads(False)
-        out = step.plan.objective_out.detach()
-        return out[0:1].clone(), out[1:2].clone(), out[2:3].clone()
-
-    @staticmethod
-    def backward(ctx, *grads):
-        step = ctx.step
-        if all(g is None for g in grads):
-            return None, None
-        model, plan = step.model, step.plan
-        eng = model.engine
-        # the backward regenerates the forward's dropout masks from the device step counter, which a forward in between has moved
-        now = int(eng.drop_step_host)
-        moved = step.train and now != step.drop_step
-        if moved:
-            eng.set_dropout_step(step.drop_step)
-        try:
-            clobbered = eng.arena is not None and eng.arena_owner != (plan, step.fwd_id)
-            if plan.fwd_id != step.fwd_id or clobbered:
-                step.load()
-                plan.run_forward()
-                step.fwd_id = plan.fwd_id
-            model._attach_grads()
-            if eng.auto_graph:
-                plan.maybe_capture_passes()
-            for i, g in enumerate(grads):
-                if g is None:
-                    plan.loss_grad[i:i + 1].zero_()
-                else:
-                    plan.loss_grad[i:i + 1].copy_(g.detach().reshape(1))
-            plan.run_backward()
-        finally:
-            if moved:
-                eng.set_dropout_step(now)
-        if model._ddp_reducer is not None:
-            model._ddp_reducer.allreduce()
-        return None, None
 
 
 class BertForMultiModalPreTraining(BertPreTrainedModel):
@@ -532,6 +508,7 @@ class BertForMultiModalPreTraining(BertPreTrainedModel):
             B, R = image_feat.shape[0], image_feat.shape[1] - 1
             sampler = getattr(self, "nce_sampler", None)
             targets["neg_index"] = sampler(B, R, image_feat.device) if sampler is not None else self._nce_negatives(B, R, image_feat.device)
-        step = _PretrainStep(self, inputs, targets, torch.is_grad_enabled())
-        step.forward()
-        return _PretrainLossFn.apply(self._anchor, step)
+        B, Nv, Nt = image_feat.shape[0], image_feat.shape[1], input_ids.shape[1]
+        plan = self.engine.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS["pretraining"] if torch.is_grad_enabled() else (), train=bool(self.training),
+                                loss="pretraining", loss_in_forward=True)
+        return _PlanFn.apply(self._anchor, _PlanCall(self, plan, inputs, targets))

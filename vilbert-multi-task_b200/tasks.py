@@ -21,6 +21,7 @@ import torch.nn as nn
 
 from .data import expand_batch
 from .engine import LOSS_HEADS, RESULT_MODES
+from .modeling import _PlanCall, _PlanFn
 
 LossMap = {
     "BCEWithLogitLoss": nn.BCEWithLogitsLoss,
@@ -83,7 +84,7 @@ def _unpack(task_id, batch):
 
 
 class _Step:
-    """One task batch on the device, reshaped for the model, with its plan built and inputs loaded."""
+    """One task batch on the device, reshaped for the model, with the plan of its objective and the call that runs it."""
 
     def __init__(self, task_cfg, task_id, batch, model, train, grad, processes, evaluate=False):
         eng = model.engine
@@ -111,88 +112,32 @@ class _Step:
         if evaluate:
             # EvaluatingModel: a forward-only plan of the one head the type reads; VL-classifier / GQA have no loss and no score
             has_loss = kind not in ("vqa", "gqa")
-            self.plan = plan = eng.plan(B, Nt, Nv, train=train, loss=kind if has_loss else None, choices=choices,
-                                        score=has_loss and kind not in _NO_SCORE, loss_in_forward=has_loss, outputs=LOSS_HEADS[kind],
-                                        results=kind if kind in RESULT_MODES else None)
+            plan = eng.plan(B, Nt, Nv, train=train, loss=kind if has_loss else None, choices=choices,
+                            score=has_loss and kind not in _NO_SCORE, loss_in_forward=has_loss, outputs=LOSS_HEADS[kind],
+                            results=kind if kind in RESULT_MODES else None)
         else:
-            self.plan = plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS[kind] if grad else (), train=train, loss=kind, choices=choices,
-                                        score=kind not in _NO_SCORE, loss_in_forward=True)
-        self.inputs = dict(input_txt=question, input_imgs=features, image_loc=spatials, token_type_ids=segment_ids, attention_mask=input_mask,
-                           image_attention_mask=image_mask, task_ids=task_tokens)
-        self.targets = {}
+            plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS[kind] if grad else (), train=train, loss=kind, choices=choices,
+                            score=kind not in _NO_SCORE, loss_in_forward=True)
+        inputs = dict(input_txt=question, input_imgs=features, image_loc=spatials, token_type_ids=segment_ids, attention_mask=input_mask,
+                      image_attention_mask=image_mask, task_ids=task_tokens)
+        targets = {}
         li = plan.loss_inputs
         if "labels" in li:
             if target.numel() != li["labels"].numel():
                 # Foil with an even batch: the binary head pairs consecutive samples (vilbert.py:1686-1689) and CrossEntropyLoss
                 # refuses the int labels of every sample, as F.cross_entropy does in the reference
                 raise ValueError(f"Expected input batch_size ({li['labels'].numel()}) to match target batch_size ({target.numel()}).")
-            self.targets["labels"] = target.reshape(li["labels"].shape)
+            targets["labels"] = target.reshape(li["labels"].shape)
         elif "target" in li:
-            self.targets["target"] = target.reshape(li["target"].shape)
+            targets["target"] = target.reshape(li["target"].shape)
         if mc_ids is not None and "multiple_choice_ids" in li:
-            self.targets["multiple_choice_ids"] = mc_ids
-        self.model, self.train = model, train
-
-    def load(self):
-        self.plan.load_inputs(**self.inputs)
-        for k, v in self.targets.items():
-            self.plan.loss_inputs[k].copy_(v, non_blocking=True)
-
-    def forward(self):
-        model, plan = self.model, self.plan
-        model._sync_weights()
-        if self.train:
-            model.engine.bump_dropout_step()
-        self.drop_step = int(model.engine.drop_step_host)
-        self.load()
-        if model.engine.auto_graph:
-            plan.maybe_capture_passes()
-        plan.run_forward()
-        self.fwd_id = plan.fwd_id
-        model._last_plan = plan
+            targets["multiple_choice_ids"] = mc_ids
+        self.plan, self.call = plan, _PlanCall(model, plan, inputs, targets)
 
     def score_error(self):
         if self.kind in _NO_SCORE:
             raise IndexError(f"{self.kind}: the reference's compute_score_with_logits scatters the argmax into a 1-D one-hot of the int "
                              "labels and raises 'Dimension out of range' (task_utils.py:618-623); there is no score to reproduce")
-
-
-class _TaskLossFn(torch.autograd.Function):
-    """loss.backward() of ForwardModelsTrain: d(total)/d(loss) is copied, on the device, into the plan's loss_grad and the plan's
-    backward runs into the model's flat gradient buffer (then the data-parallel all-reduce when one is attached, like the module
-    surface). If another plan ran in between, the forward is recomputed first with the same inputs and dropout masks."""
-
-    @staticmethod
-    def forward(ctx, anchor, step):
-        ctx.step = step
-        return step.plan.loss.detach().reshape(()).clone()
-
-    @staticmethod
-    def backward(ctx, g):
-        step = ctx.step
-        if g is None:
-            return None, None
-        model, plan = step.model, step.plan
-        eng = model.engine
-        clobbered = eng.arena is not None and eng.arena_owner != (plan, step.fwd_id)
-        if plan.fwd_id != step.fwd_id or clobbered:
-            step.load()
-            now = int(eng.drop_step_host)
-            if step.train and now != step.drop_step:
-                eng.set_dropout_step(step.drop_step)
-                plan.run_forward()
-                eng.set_dropout_step(now)
-            else:
-                plan.run_forward()
-            step.fwd_id = plan.fwd_id
-        model._attach_grads()
-        if eng.auto_graph:
-            plan.maybe_capture_passes()
-        plan.loss_grad.copy_(g.detach().reshape(1))
-        plan.run_backward()
-        if model._ddp_reducer is not None:
-            model._ddp_reducer.allreduce()
-        return None, None
 
 
 def _model(model):
@@ -213,8 +158,7 @@ def ForwardModelsTrain(args, task_cfg, device, task_id, task_count, task_iter_tr
     m = _model(model)
     _check_loss(task_cfg, task_id, task_losses)
     step = _Step(task_cfg, task_id, batch, m, bool(m.training), True, ("dialog", "expand", "retrieval", "nlvr"))
-    step.forward()
-    loss = _TaskLossFn.apply(m._anchor, step)
+    loss, = _PlanFn.apply(m._anchor, step.call)
     step.score_error()
     score = step.plan.score.reshape(()) / float(step.batch_size)
     return loss, score
@@ -228,7 +172,7 @@ def ForwardModelsVal(args, task_cfg, device, task_id, batch, model, task_losses)
     _check_loss(task_cfg, task_id, task_losses)
     with torch.no_grad():
         step = _Step(task_cfg, task_id, batch, m, bool(m.training), False, ("expand", "retrieval", "nlvr"))
-        step.forward()
+        step.call.forward()
         step.score_error()
         loss, score = step.plan.objective_out.tolist()
     return loss, score, step.batch_size
@@ -257,7 +201,7 @@ def EvaluatingModel(args, task_cfg, device, task_id, batch, model, task_dataload
     with torch.no_grad():
         step = _Step(task_cfg, task_id, batch, m, bool(m.training), False, ("dialog", "expand", "retrieval", "nlvr"), evaluate=True)
         step.score_error()
-        step.forward()
+        step.call.forward()
         plan = step.plan
         if plan.results is None:              # VL-binary / VL-tri: loss and score only
             loss, score = plan.objective_out.tolist()
