@@ -309,6 +309,15 @@ enum { VB_RESULT_ARGMAX = 0, VB_RESULT_SOFTMAX = 1, VB_RESULT_GATHER = 2 };
 vb_status vb_task_results(int32_t mode, const float* logits, int64_t ld_logits, int32_t col_off, int32_t cols, const int64_t* ids,
                           int32_t width, const float* target, int64_t ld_target, int32_t rows, int64_t* argmax, float* values,
                           int64_t ld_values, void* stream);
+/* vb_retrieval_rank: caption-to-image retrieval ranks (eval_retrieval.py:315-337) on the device. Row r of scores (f32 [rows, cols],
+ * row pitch ld_scores) is put in the stable descending order: column j comes before column i when s_j > s_i, or s_j == s_i and
+ * j < i; -0.0 ties with +0.0 and every NaN comes after every number, NaNs in column order (np.argsort(-s, kind="stable")).
+ *   rank_out[r] (int32)     position of column target[r] (int64) in that order, -1 when target[r] is outside [0, cols)
+ *   topk_out[r, 0..k) (int32, NULL: none)  the first min(k, cols) columns of that order, -1 after them
+ * One CTA per row with the row's keys in dynamic shared memory: one block-wide count for the rank, k block-wide arg-max rounds
+ * for the top-k; no atomics, results are deterministic. cols <= 50000, 1 <= k <= 64; otherwise VB_ERR_INVALID. */
+vb_status vb_retrieval_rank(const float* scores, int64_t ld_scores, int32_t rows, int32_t cols, const int64_t* target, int32_t k,
+                            int32_t* rank_out, int32_t* topk_out, void* stream);
 /* dst = src * (*scale), f32, scale read on the device: the backward of a forward-placed objective starts from the stored
  * d loss / d head times d(total) / d loss (loss_scale[task] / gradient_accumulation_steps, train_tasks.py:247-251, 545-548)
  * without a host synchronisation. */

@@ -5,7 +5,7 @@ _build_only=True on the CPU).
     python tools/plan_dump.py ROOT [--out FILE]
 
 imports the package from the repository tree ROOT. For every plan of the case matrix below it lists each op of the prologue,
-forward, backward and epilogue: section, stream id, function name (MARK for a stream barrier / event marker) and every
+image prefix, forward, backward and epilogue: section, stream id, function name (MARK for a stream barrier / event marker) and every
 argument. Structs passed by reference are expanded field by field, and every pointer (a c_void_p argument or struct field) is
 written as `allocation+byte offset` against the plan's allocations, so two runs, or two trees that launch the same work,
 produce byte-identical listings."""
@@ -73,6 +73,10 @@ def cases(O, LOSS_HEADS):
           for case in ([] if vt == 0 else [(f"pretraining_vt{vt}", over, "pretraining", 4, obj("pretraining"))]) +
           [(f"pretraining_fwd_vt{vt}", over, "pretraining", 4, obj("pretraining", loss_in_forward=True)),
            (f"pretraining_fwd_vt{vt}_eval", over, "pretraining", 4, dict(loss="pretraining", loss_in_forward=True))]],
+        # caption-to-image retrieval (vilbert_b200.retrieval): fast-mode plans whose image embedding runs once per image chunk
+        ("retrieval_prefix", {}, "vl", 4, dict(outputs=("vil_logit",), fast_mode=True, image_prefix=True)),
+        ("retrieval_prefix_task_tokens", dict(task_specific_tokens=True), "vl", 4, dict(outputs=("vil_logit",), fast_mode=True, image_prefix=True)),
+        ("retrieval_zero_shot", {}, "pretraining", 4, dict(outputs=("seq_relationship_score",), fast_mode=True, image_prefix=True)),
     ]
 
 
@@ -131,8 +135,8 @@ def dump_plan(out, title, plan, opt=None):
     alloc = allocations(plan, opt)
     n = 0
     out.append(f"== {title}")
-    for section in ("prologue", "fwd", "bwd", "epilogue"):
-        for i, (fn, args, sid) in enumerate(getattr(plan, section)):
+    for section in ("prologue", "prefix", "fwd", "bwd", "epilogue"):
+        for i, (fn, args, sid) in enumerate(getattr(plan, section, ())):     # prefix: image_prefix plans only
             if fn is None:
                 rec = "MARK " + " ".join(str(a) for a in args)
             else:

@@ -1,0 +1,140 @@
+"""Times caption-to-image retrieval at the reference's real shapes: bert_base_6layer_6conect with task tokens, 101 regions, 30 + 1
+tokens, a gallery of 1,000 random-feature images, random weights. Two arms alternate in one process after a warm-up:
+
+  (a) RetrievalEvaluator(chunk=500): each 500-image chunk loaded and embedded once, one graph replay per caption and chunk;
+  (b) the reference loop (eval_retrieval.py:264-313) restated on the module surface: model(...) per caption and gallery half with
+      config.fast_mode set, the half's features copied from pinned host memory on every call, the scores read back with .cpu().
+
+    python tools/retrieval_probe.py [--captions 200] [--rounds 3] [--out retrieval_probe.json]
+
+Reports ms per caption (median and min-max over the rounds), model TFLOP/s from the FLOPs of the plans' GEMMs and attentions, the
+evaluator's plan bytes, the card's name, power limit and SM clock, and how far the two arms' outputs agree."""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def plan_flops(plan):
+    """Forward FLOPs of one run of a plan: 2 M N K per GEMM, 4 B H Nq Nk D per attention."""
+    total = 0
+    for fn, args, _ in plan.fwd:
+        if fn is None:
+            continue
+        if fn.__name__ == "vb_gemm_bf16":
+            g = args[0]._obj
+            total += 2 * g.M * g.N * g.K
+        elif fn.__name__ == "vb_attention_fwd":
+            a = args[0]._obj
+            total += 4 * a.B * a.H * a.Nq * a.Nk * a.D
+    return total
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, power, sm, sm_max = [x.strip() for x in q.split(",")]
+        return dict(name=name, power_limit=power, sm_clock=sm, sm_clock_max=sm_max)
+    except Exception as ex:         # the probe still reports what torch knows
+        return dict(name=torch.cuda.get_device_name(), error=str(ex))
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--captions", type=int, default=200)
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--images", type=int, default=1000)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    import vilbert_b200
+    from vilbert_b200.retrieval import RetrievalEvaluator
+    cfgj = dict(json.load(open(os.path.join(ROOT, "vilbert-multi-task_b200", "configs", "bert_base_6layer_6conect.json"))),
+                task_specific_tokens=True)
+    torch.manual_seed(0)
+    model = vilbert_b200.VILBertForVLTasks(vilbert_b200.BertConfig.from_dict(cfgj))
+    model.eval()
+    G, Nv, Nt, C, half = a.images, 101, 30, a.captions, 500
+    feats = torch.relu(torch.randn(G, Nv, 2048)).pin_memory()
+    locs = torch.rand(G, Nv, 5).pin_memory()
+    imask = torch.ones(G, Nv, dtype=torch.long).pin_memory()
+    caps = torch.randint(1000, 30000, (C, Nt))
+    amask = torch.ones(C, Nt, dtype=torch.long)
+    amask[:, 20:] = torch.randint(0, 2, (C, Nt - 20)).sort(dim=1, descending=True)[0]
+    seg = torch.zeros(C, Nt, dtype=torch.long)
+    target = torch.arange(C) % G
+
+    ev = RetrievalEvaluator(model, feats, locs, imask, chunk=half)
+
+    def arm_a(n):
+        return ev.score(caps[:n], amask[:n], seg[:n], task_id=8)
+
+    def arm_b(n):
+        model.config.fast_mode = True
+        out = np.zeros((n, G), dtype=np.float32)
+        task = torch.full((1, 1), 8, dtype=torch.long, device="cuda")
+        with torch.no_grad():
+            for c in range(n):
+                cap, m, s = caps[c:c + 1].cuda(), amask[c:c + 1].cuda(), seg[c:c + 1].cuda()
+                for h in range(0, G, half):
+                    sl = slice(h, h + half)
+                    logit = model(cap, feats[sl].cuda(non_blocking=True), locs[sl].cuda(non_blocking=True), s, m,
+                                  imask[sl].cuda(non_blocking=True), task_ids=task)[2]
+                    out[c, sl] = logit.view(-1).cpu().numpy()
+        model.config.fast_mode = False
+        return out
+
+    def timed(f, n):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        r = f(n)
+        torch.cuda.synchronize()
+        return (time.perf_counter() - t0) * 1e3 / n, r
+
+    timed(arm_a, 4)        # warm-up: plans, graph capture, kernels loaded
+    timed(arm_b, 4)
+    ta, tb = [], []
+    sa = sb = None
+    for _ in range(a.rounds):
+        t, sa = timed(arm_a, C)
+        ta.append(t)
+        t, sb = timed(arm_b, C)
+        tb.append(t)
+    eng = model.engine
+    pa = [p for p in eng.plans.values() if p.image_prefix]
+    pb = [p for p in eng.plans.values() if not p.image_prefix and p.B == half]
+    flops_caption = sum(plan_flops(p) * (G // p.B) for p in pa if p.B == half) + sum(plan_flops(p) for p in pa if p.B != half and G % half)
+    flops_module = plan_flops(pb[0]) * (G // half) if pb else 0
+    ranks_a, _ = ev.rank(sa, target, k=20)
+    ranks_b, _ = ev.rank(torch.from_numpy(sb).cuda(), target, k=20)
+    res = dict(
+        card=card(), config="bert_base_6layer_6conect + task tokens", images=G, regions=Nv, tokens=Nt + 1, captions=C, rounds=a.rounds,
+        precision=eng.precision,
+        evaluator_ms_per_caption=dict(median=statistics.median(ta), min=min(ta), max=max(ta)),
+        module_loop_ms_per_caption=dict(median=statistics.median(tb), min=min(tb), max=max(tb)),
+        evaluator_tflops=flops_caption / (statistics.median(ta) * 1e-3) / 1e12,
+        module_loop_tflops=flops_module / (statistics.median(tb) * 1e-3) / 1e12,
+        flops_per_caption=flops_caption, module_flops_per_caption=flops_module,
+        evaluator_plan_bytes=sum(sum(t.numel() * t.element_size() for t in p._keep if torch.is_tensor(t)) for p in pa),
+        max_abs_score_diff=float((sa.cpu() - torch.from_numpy(sb)).abs().max()),
+        ranks_differing=int((ranks_a != ranks_b).sum()),
+    )
+    text = json.dumps(res, indent=1)
+    print(text)
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            f.write(text + "\n")
+
+
+if __name__ == "__main__":
+    main()

@@ -17,6 +17,9 @@ def __getattr__(name):
     if name in ("ForwardModelsTrain", "ForwardModelsVal", "LoadLosses"):
         from . import tasks
         return getattr(tasks, name)
+    if name in ("RetrievalEvaluator", "evaluate_retrieval", "retrieval_metrics"):
+        from . import retrieval
+        return getattr(retrieval, name)
     if name in ("Engine", "Plan", "ParamStore"):
         from . import engine
         return getattr(engine, name)

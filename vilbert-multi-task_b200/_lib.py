@@ -107,6 +107,7 @@ _SIGNATURES = {
     "vb_bce_gather_loss": [_P, _I64, _I32, _I32, _P, _P, _I32, _I32, _F, _P, _P, _I32, _P, _I64, _P, _I64, _P],
     "vb_task_score": [_I32, _P, _I64, _I32, _I32, _P, _I32, _P, _I64, _P, _I32, _P, _I32, _P, _P],
     "vb_task_results": [_I32, _P, _I64, _I32, _I32, _P, _I32, _P, _I64, _I32, _P, _P, _I64, _P],
+    "vb_retrieval_rank": [_P, _I64, _I32, _I32, _P, _I32, _P, _P, _P],
     "vb_scale_by_device": [_P, _P, _I64, _P, _P],
     "vb_kl_masked_loss": [_P, _P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _F, _I32, _P],
     "vb_mse_masked_loss": [_P, _P, _P, _I32, _I32, _I32, _F, _P, _P, _I32, _P, _P],

@@ -379,6 +379,86 @@ task_results_kernel(int mode, const float* __restrict__ logits, long long ld, in
   for (int c = lane; c < cols; c += 32) out[c] = (float)(exp((double)(result_logit(zr, off, idr, width, c) - v)) * inv);
 }
 
+// ------------------------------------------------------------------------------------------ retrieval ranks (vb_retrieval_rank)
+// Stable descending order of a score row as one 64-bit key per column, higher = earlier: the high word maps the float to an
+// unsigned integer that orders like the number (-0.0 folded onto +0.0, every NaN to 0, below -inf), the low word is ~column, so
+// equal scores keep the column order. Integer keys only: no float comparison, so --use_fast_math's flush-to-zero does not tie
+// subnormal scores with 0.
+constexpr int RANK_THREADS = 512;
+constexpr int RANK_MAX_COLS = 50000;
+constexpr int RANK_MAX_K = 64;
+
+__device__ __forceinline__ uint32_t rank_key_hi(float x) {
+  uint32_t u = __float_as_uint(x);
+  if ((u & 0x7fffffffu) > 0x7f800000u) return 0u;          // NaN: after every number
+  if (u == 0x80000000u) u = 0u;                              // -0.0 ties with +0.0
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+__device__ __forceinline__ unsigned long long rank_key(const uint32_t* hi, int j) {
+  return ((unsigned long long)hi[j] << 32) | (uint32_t)~(uint32_t)j;
+}
+
+// block-wide max of a 64-bit key (red: RANK_THREADS / 32 entries); every thread gets the result
+__device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v, unsigned long long* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long w = __shfl_xor_sync(0xffffffffu, v, o);
+    v = w > v ? w : v;
+  }
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  unsigned long long r = red[0];
+  for (int w = 1; w < RANK_THREADS / 32; ++w) r = red[w] > r ? red[w] : r;
+  return r;
+}
+
+// one CTA per row: the row's keys are staged in dynamic shared memory (4 bytes per column); the rank is one block-wide count of
+// the keys above the target's, the top-k k block-wide arg-max rounds, each bounded by the previous pick. No atomics.
+__global__ void __launch_bounds__(RANK_THREADS)
+retrieval_rank_kernel(const float* __restrict__ scores, long long ld, int N, const long long* __restrict__ target, int k,
+                      int* __restrict__ rank_out, int* __restrict__ topk_out) {
+  pdl_entry();
+  extern __shared__ uint32_t keys[];
+  __shared__ unsigned long long red64[RANK_THREADS / 32];
+  __shared__ int red32[RANK_THREADS / 32];
+  const int r = blockIdx.x;
+  const float* row = scores + (long long)r * ld;
+  for (int j = threadIdx.x; j < N; j += RANK_THREADS) keys[j] = rank_key_hi(row[j]);
+  __syncthreads();
+  const long long t = target[r];
+  int above = 0;
+  if (t >= 0 && t < N) {
+    const unsigned long long kt = rank_key(keys, (int)t);
+    for (int j = threadIdx.x; j < N; j += RANK_THREADS) above += rank_key(keys, j) > kt ? 1 : 0;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) above += __shfl_xor_sync(0xffffffffu, above, o);
+  if ((threadIdx.x & 31) == 0) red32[threadIdx.x >> 5] = above;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int s = 0;
+    for (int w = 0; w < RANK_THREADS / 32; ++w) s += red32[w];
+    rank_out[r] = (t >= 0 && t < N) ? s : -1;
+  }
+  if (!topk_out) return;
+  int* out = topk_out + (long long)r * k;
+  unsigned long long bound = ~0ull;                          // no key reaches it: the low word of a key is ~column, column < 2^31
+  const int kk = k < N ? k : N;
+  for (int i = 0; i < kk; ++i) {
+    unsigned long long best = 0ull;
+    for (int j = threadIdx.x; j < N; j += RANK_THREADS) {
+      const unsigned long long x = rank_key(keys, j);
+      if (x < bound && x > best) best = x;
+    }
+    best = block_max_u64(best, red64);
+    if (threadIdx.x == 0) out[i] = (int)~(uint32_t)best;
+    bound = best;
+  }
+  for (int i = kk + threadIdx.x; i < k; i += RANK_THREADS) out[i] = -1;
+}
+
 // ------------------------------------------------------------------------------------------ masked-region regression and NCE
 // Both objectives score rows [b, r+1] of prediction_scores_v (region 0, the global feature, is dropped) against target[b, r] and
 // label[b, r] == 1, R = Nv - 1. One CTA per row of scores (region 0 and unmasked rows write a zero gradient and a zero row loss);
@@ -563,6 +643,24 @@ extern "C" vb_status vb_task_results(int32_t mode, const float* logits, int64_t 
              (long long)ld_logits, (int)col_off, (int)cols, reinterpret_cast<const long long*>(ids), (int)width, target, (long long)ld_target,
              (int)rows, reinterpret_cast<long long*>(argmax), values, (long long)ld_values);
   return check_launch("vb_task_results");
+}
+
+extern "C" vb_status vb_retrieval_rank(const float* scores, int64_t ld_scores, int32_t rows, int32_t cols, const int64_t* target, int32_t k,
+                                       int32_t* rank_out, int32_t* topk_out, void* stream) {
+  if (rows <= 0 || cols <= 0 || ld_scores < cols || !scores || !target || !rank_out || (topk_out && (k <= 0 || k > RANK_MAX_K)))
+    return set_error(VB_ERR_INVALID, "vb_retrieval_rank: bad arguments (rows %d, cols %d, ld %lld, k %d; 1 <= k <= %d)", (int)rows,
+                     (int)cols, (long long)ld_scores, (int)k, RANK_MAX_K);
+  if (cols > RANK_MAX_COLS)
+    return set_error(VB_ERR_INVALID, "vb_retrieval_rank: %d columns exceed the %d a row of shared memory holds", (int)cols, RANK_MAX_COLS);
+  const size_t smem = (size_t)cols * sizeof(uint32_t);
+  if (smem > 48 * 1024) {      // set per call, as the attention kernels do: it holds for the current device only
+    cudaError_t e = cudaFuncSetAttribute(retrieval_rank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_retrieval_rank: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+  }
+  launch_pdl(retrieval_rank_kernel, dim3(rows), dim3(RANK_THREADS), smem, static_cast<cudaStream_t>(stream), scores, (long long)ld_scores,
+             (int)cols, reinterpret_cast<const long long*>(target), (int)(topk_out ? k : 0), reinterpret_cast<int*>(rank_out),
+             reinterpret_cast<int*>(topk_out));
+  return check_launch("vb_retrieval_rank");
 }
 
 extern "C" vb_status vb_scale_by_device(const float* src, float* dst, int64_t n, const float* scale, void* stream) {

@@ -291,6 +291,8 @@ def nce_negative_count(cfg):
 HEAD_NAMES = ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_prediction", "vil_tri_prediction",
               "vision_prediction", "vision_logit", "linguisic_prediction", "linguisic_logit")
 BERT_OUT_NAMES = ("sequence_output_t", "sequence_output_v", "pooled_output_t", "pooled_output_v")
+# the heads of BertForMultiModalPreTraining (vilbert.py:1497), in the order its forward returns them
+PRETRAINING_HEAD_NAMES = ("linguisic_prediction", "vision_prediction", "seq_relationship_score")
 
 # per-row evaluation results of a task kind (EvaluatingModel, task_utils.py:777-847; Plan(results=...)): the head they read and the
 # mode of vb_task_results. VL-classifier / GQA: the answer index; VL-logit: the option probabilities; V-logit: the region and its
@@ -319,10 +321,17 @@ class Plan:
     and no entry in self.outputs (the four BertModel outputs are always there); what a kept head reads (the fused pooled vector,
     the alignment head of an odd batch, dropout sites) is built as in the all-heads plan, so a kept head is bitwise the same.
     results: a kind of RESULT_MODES; the forward ends with vb_task_results on that kind's head, and self.results_out packs
-    objective_out (loss, score), the per-row argmax and the per-row values into one device buffer (fetch_results)."""
+    objective_out (loss, score), the per-row argmax and the per-row values into one device buffer (fetch_results).
+    With heads="pretraining", outputs= names heads of PRETRAINING_HEAD_NAMES: ("seq_relationship_score",) builds no masked-LM or
+    region decoder.
+
+    fast_mode: text batch 1 broadcast to the image batch (None: config.fast_mode). image_prefix=True (forward-only plans): the image
+    embedding (feature cast, box projection, embedding GEMM, LayerNorm) and the additive image mask are emitted into self.prefix,
+    run by run_image_prefix() on what load_images() loaded, and write private buffers that no op of the forward writes; the forward
+    starts at the text embeddings and reads those image states as they are, so one image batch serves many text forwards."""
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-                 loss_in_forward=False, outputs=None, results=None):
+                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False):
         self.e, self.cfg = engine, engine.cfg
         self.grad_touch = {}           # (flat offset, numel) -> index of the last backward op writing that gradient range
         self.ps = _TrackedParams(engine.ps, self)
@@ -342,10 +351,17 @@ class Plan:
         if self.viz and train:
             raise ValueError("visualization exports the undropped attention probabilities: eval mode only")
         self.dyn = bool(getattr(self.cfg, "dynamic_attention", False))
-        self.fast = bool(getattr(self.cfg, "fast_mode", False))
+        self.fast = bool(getattr(self.cfg, "fast_mode", False)) if fast_mode is None else bool(fast_mode)
         self.Bt = 1 if self.fast else B
         if self.fast and (train or grad_outputs or vqa_loss or loss):
             raise ValueError("fast_mode is an inference path (text batch 1 broadcast to the image batch): no train mode / gradients")
+        self.image_prefix = bool(image_prefix)
+        if self.image_prefix and (train or grad_outputs or vqa_loss):
+            raise ValueError("image_prefix keeps the image states across forwards: forward-only plans (no train mode, no grad_outputs)")
+        if self.image_prefix and self.pairs:
+            raise ValueError("image_prefix: in_batch_pairs re-expands the image batch inside the forward")
+        self.prefix = []         # image_prefix: the image embedding and mask, run by run_image_prefix()
+        self._private = False    # while set, buf() allocates private buffers (the image states of image_prefix)
         self.grad_outputs = frozenset(grad_outputs)
         # objective fused into the step (LOSS_HEADS): its scalar lands in self.loss (device) and its gradient goes straight into the
         # backward of the head(s) it reads; vqa_loss=True is the round-1 spelling of loss="vqa"
@@ -404,12 +420,19 @@ class Plan:
                 raise ValueError(f"results={r!r} reads the inputs of its objective: build it with loss={r!r}, loss_in_forward=True")
         if self.keep is None:
             return
-        unknown = sorted(n for n in self.keep if n not in HEAD_NAMES)
-        if unknown:
-            raise ValueError(f"outputs: unknown head name(s) {unknown}; the heads are {HEAD_NAMES}")
-        if self.heads != "vl":
-            raise ValueError(f"outputs= selects among the heads of VILBertForVLTasks (heads='vl'), not heads={self.heads!r}")
-        need = {n for n in self.grad_outputs if n in HEAD_NAMES}
+        if self.heads == "pretraining" and all(n in HEAD_NAMES + PRETRAINING_HEAD_NAMES for n in self.keep):
+            other = sorted(n for n in self.keep if n not in PRETRAINING_HEAD_NAMES)
+            if other:
+                raise ValueError(f"outputs: {other} are heads of VILBertForVLTasks (heads='vl'); the heads of heads='pretraining' are "
+                                 f"{PRETRAINING_HEAD_NAMES}")
+        else:
+            unknown = sorted(n for n in self.keep if n not in HEAD_NAMES)
+            if unknown:
+                raise ValueError(f"outputs: unknown head name(s) {unknown}; the heads are {HEAD_NAMES}")
+            if self.heads != "vl":
+                raise ValueError(f"outputs= selects among the heads of VILBertForVLTasks (heads='vl') or of BertForMultiModalPreTraining "
+                                 f"(heads='pretraining'), not heads={self.heads!r}")
+        need = {n for n in self.grad_outputs if n in HEAD_NAMES + PRETRAINING_HEAD_NAMES}
         if k is not None:
             need |= set(LOSS_HEADS[k])
         if r is not None:
@@ -430,6 +453,7 @@ class Plan:
         initialised at build time or loaded from outside a run (zero=True: inputs, labels, output gradients, zero-padded
         operands) stay private."""
         arena = self.e.arena
+        zero = zero or self._private
         if arena is None or zero:
             t = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=self.dev)
             self._keep.append(t)
@@ -530,7 +554,7 @@ class Plan:
         pass they are bf16 tensors: A a gradient, B the bf16 copy of a weight (dgrad) or of a saved activation (wgrad),
         the 16-bit output a gradient."""
         g = L.GemmArgs()
-        fwd = self.cur is self.fwd
+        fwd = self.cur is not self.bwd          # the forward or the image prefix
         if fwd:
             self._check_operands((A, B, out_bf16), ())
             g.a_fp16 = g.b_fp16 = g.out_fp16 = A.fp16
@@ -937,9 +961,12 @@ class Plan:
         self.in_feat = self.buf((B, Nv, Fv), F32, zero=True)
         self.in_loc = self.buf((B, Nv, 5), F32, zero=True)
         self.mask_t = self.buf((Bt, Nt), F32)
-        self.mask_v = self.buf((B, Nv), F32)
+        self.mask_v = self.buf((B, Nv), F32, zero=self.image_prefix)
         self.emit(lib.vb_mask_to_additive, self.in_amask.data_ptr(), self.mask_t.data_ptr(), Bt, self.Nt_in, 1 if self.has_task else 0)
+        if self.image_prefix:
+            self.cur = self.prefix
         self.emit(lib.vb_mask_to_additive, self.in_imask.data_ptr(), self.mask_v.data_ptr(), B, Nv, 0)
+        self.cur = self.fwd
         self.sync_streams()
         # text: gather-sum (+ task row) then LayerNorm (vilbert.py:346-367)
         xe = self.buf((Mt, Ht), F32)
@@ -961,9 +988,13 @@ class Plan:
                           ps.g(e + ".token_type_embeddings.weight").data_ptr(),
                           ps.g(e + ".task_embeddings.weight").data_ptr() if self.has_task else None, B, self.Nt_in, Ht)
         self.push_bwd(bwd_text)
-        # image: region features fp32 -> bf16 ingest, 2048 -> Hv GEMM with the 5 -> Hv box projection as residual, LayerNorm (:1421-1432)
+        # image: region features fp32 -> bf16 ingest, 2048 -> Hv GEMM with the 5 -> Hv box projection as residual, LayerNorm (:1421-1432).
+        # image_prefix: the same launches go to self.prefix on the main stream, and the LayerNorm's outputs (the image states the
+        # forward reads) are private buffers
         ve = "bert.v_embeddings"
-        with self.on(1):
+        if self.image_prefix:
+            self.cur = self.prefix
+        with self.on(0 if self.image_prefix else 1):
             feat = self.buf16((Mv, Fv))
             hi, lo, bw = feat.ptrs()
             self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), hi, Mv * Fv, feat.fp16, lo, bw)
@@ -974,8 +1005,13 @@ class Plan:
             self.gemm(Mv, Hv, Fv, feat, Fv, ps.w(ve + ".image_embeddings.weight"), Fv, bias=ps.p(ve + ".image_embeddings.bias"),
                       residual=locp, ld_res=Hv, out_f32=yv, ld_of=Hv)
             vdrop = self.drop(ve + ".dropout", c.hidden_dropout_prob)     # BertImageEmbeddings uses hidden_dropout_prob (vilbert.py:1419)
+            self._private = self.image_prefix
             v32, vop, vmean, vrstd = self.ln_fwd(yv, ps.p(ve + ".LayerNorm.weight"), ps.p(ve + ".LayerNorm.bias"), Mv, Hv, out_drop=vdrop)
+            self._private = False
+            self.cur = self.fwd
             v = Act(v32, vop, Mv, Hv)
+            if self.image_prefix:
+                self.image_states = (v32, vop.hi, vop.lo, self.mask_v)
 
             def bwd_image():
                 if v.gw:
@@ -1172,7 +1208,7 @@ class Plan:
         need_fused = any(want(n) for n in ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_tri_prediction")) or (
             want("vil_binary_prediction") and B % 2 == 0)
         fused = fuse(self.drop("dropout.pooled", self.head_dropout_prob)) if self.heads == "vl" and need_fused else None
-        need_cls_fused = self.heads == "pretraining" or (B % 2 == 1 and want("vil_binary_prediction"))
+        need_cls_fused = (self.heads == "pretraining" and want("seq_relationship_score")) or (B % 2 == 1 and want("vil_binary_prediction"))
         cls_drop = self.drop("cls.dropout", 0.1)
         if need_cls_fused:
             fused_cls = fuse(cls_drop) if (cls_drop is not None or fused is None) else fused
@@ -1213,7 +1249,8 @@ class Plan:
 
         if self.heads == "pretraining":
             # BertForMultiModalPreTraining returns the alignment score of self.cls (vilbert.py:1497)
-            self.small_head("seq_relationship_score", fused_cls, "cls.bi_seq_relationship", 2)
+            if want("seq_relationship_score"):
+                self.small_head("seq_relationship_score", fused_cls, "cls.bi_seq_relationship", 2)
             return
         if want("vil_binary_prediction") and B % 2 == 0:
             # vil_binary_prediction pairs consecutive samples: pooled.view(-1, 2*Hb) (:1686-1689)
@@ -1605,7 +1642,10 @@ class Plan:
     # ------------------------------------------------------------------ execution
     def load_inputs(self, input_txt, input_imgs, image_loc, token_type_ids=None, attention_mask=None, image_attention_mask=None,
                     task_ids=None, non_blocking=True):
-        """Host (ideally pinned) or device tensors -> the plan's static input buffers."""
+        """Host (ideally pinned) or device tensors -> the plan's static input buffers. An image_prefix plan loads the text side only:
+        its images come from load_images(), and input_imgs / image_loc / image_attention_mask must be None."""
+        if self.image_prefix and not (input_imgs is None and image_loc is None and image_attention_mask is None):
+            raise ValueError("image_prefix plan: load the images with load_images() (load_inputs loads the text side only)")
         self.in_ids.copy_(input_txt, non_blocking=non_blocking)
         if token_type_ids is None:
             self.in_tt.zero_()
@@ -1617,20 +1657,36 @@ class Plan:
             self.in_amask.copy_(attention_mask, non_blocking=non_blocking)
         if self.fast:
             self.in_amask_b.copy_(self.in_amask.expand_as(self.in_amask_b))
-        if image_attention_mask is None:
-            self.in_imask.fill_(1)
-        else:
-            self.in_imask.copy_(image_attention_mask, non_blocking=non_blocking)
+        if not self.image_prefix:
+            self.load_images(input_imgs, image_loc, image_attention_mask, non_blocking)
         if self.pairs:
             b = self.Bin
             self.in_amask_pairs.view(b, b, -1).copy_(self.in_amask.unsqueeze(1).expand(b, b, -1))
             self.in_imask_pairs.view(b, b, -1).copy_(self.in_imask.unsqueeze(0).expand(b, b, -1))
-        self.in_feat.copy_(input_imgs, non_blocking=non_blocking)
-        self.in_loc.copy_(image_loc, non_blocking=non_blocking)
         if self.has_task:
             if task_ids is None:
                 raise ValueError("task_specific_tokens is set: task_ids is required")
             self.in_task.copy_(task_ids.reshape(-1), non_blocking=non_blocking)
+
+    def load_images(self, input_imgs, image_loc, image_attention_mask=None, non_blocking=True):
+        """Region features [B, Nv, 2048], boxes [B, Nv, 5] and the 0/1 image mask [B, Nv] (None: all ones) -> the plan's image inputs.
+        An image_prefix plan then runs run_image_prefix(); any other plan reads them in its forward (load_inputs calls this)."""
+        if image_attention_mask is None:
+            self.in_imask.fill_(1)
+        else:
+            self.in_imask.copy_(image_attention_mask, non_blocking=non_blocking)
+        self.in_feat.copy_(input_imgs, non_blocking=non_blocking)
+        self.in_loc.copy_(image_loc, non_blocking=non_blocking)
+
+    def run_image_prefix(self):
+        """image_prefix: the image embedding and the additive image mask from the loaded images into the plan's private image
+        states, which every later run_forward() reads until the next call. Its intermediates may live in the shared arena, so it
+        counts as a forward of this plan there."""
+        if not self.image_prefix:
+            raise ValueError("run_image_prefix: the plan was built without image_prefix=True")
+        self.fwd_id += 1
+        self.e.arena_owner = (self, self.fwd_id)
+        self._run(self.prefix)
 
     def _run(self, ops):
         """Issues the ops on their streams. Markers: (None, ()) = barrier between the text and vision streams;
@@ -1991,19 +2047,20 @@ class Engine:
         self.lm_capacity = 0.25          # ... with room for this fraction of the token rows (15 % are masked; more poisons the loss with NaN)
 
     def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-             loss_in_forward=False, outputs=None, results=None):
+             loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False):
         """The cached plan of this shape and these options (Plan)."""
         loss = "vqa" if vqa_loss else loss
         pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
         key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward),
-               None if outputs is None else frozenset(outputs), results)
+               None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix))
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]
         while len(self.plans) >= self.max_plans:   # evict the least recently used plan: its buffers go back to the allocator
             self.plans.popitem(last=False)
         self.plans[key] = Plan(self, B, Nt, Nv, grad_outputs, False, heads, train, loss=loss, choices=choices, score=score,
-                               loss_in_forward=loss_in_forward, outputs=outputs, results=results)
+                               loss_in_forward=loss_in_forward, outputs=outputs, results=results, fast_mode=fast_mode,
+                               image_prefix=image_prefix)
         return self.plans[key]
 
     def enable_activation_arena(self, nbytes):

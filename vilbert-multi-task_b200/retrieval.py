@@ -1,0 +1,199 @@
+"""Caption-to-image retrieval evaluation on the device: the drop-in for the loop of eval_retrieval.py:253-358 (fine-tuned TASK7 /
+TASK8 model) and of evaluation/eval_coco_retrieval.py:336-412 (zero-shot pre-trained model).
+
+    from vilbert_b200.retrieval import RetrievalEvaluator, evaluate_retrieval, retrieval_metrics
+
+    ev = RetrievalEvaluator(model, features, spatials, image_mask, chunk=500)   # gallery [G, Nv, 2048] / [G, Nv, 5] / [G, Nv]
+    scores = ev.score(captions, input_mask, segment_ids, task_id=8)            # device f32 [C, G]
+    ranks, topk = ev.rank(scores, target_image, k=20)                           # device int32 [C], [C, k]
+    r1, r5, r10, medr, meanr = retrieval_metrics(ranks)
+
+    r1, r5, r10, medr, meanr, results = evaluate_retrieval(model, dataset, task_id="TASK8")
+
+The reference scores every caption against the same gallery with one model call per caption and gallery half, so each call moves
+the half's region features to the device and embeds them again. Here the work runs chunk outer, caption inner: a chunk of images
+is loaded and embedded once (Plan(image_prefix=True).run_image_prefix()), then every caption costs a few device-to-device copies
+from a caption bank uploaded once and one replay of a fast-mode forward (text batch 1 broadcast to the chunk) that builds only the
+score head. Scores stay on the device; vb_retrieval_rank ranks them there, and one read-back returns ranks and top-k lists.
+
+Differences from the reference: equal scores are ordered by image index (the reference's default argsort leaves their order
+unspecified), and progress is logged once per chunk rather than after every caption (no caption has a full score row before the
+last chunk).
+"""
+import logging
+
+import numpy as np
+import torch
+
+from . import _lib as L
+
+logger = logging.getLogger(__name__)
+
+# the score head of each model kind (Engine heads): VILBertForVLTasks' vil_logit (eval_retrieval.py:299-310), the pre-training
+# model's alignment logits, scored as softmax(logits, 1)[:, 0] (eval_coco_retrieval.py:357-363)
+SCORE_HEAD = {"vl": "vil_logit", "pretraining": "seq_relationship_score"}
+MAX_TOPK = 64            # vb_retrieval_rank: k <= 64
+MAX_GALLERY = 50000      # ... and at most 50,000 images per row
+
+
+def retrieval_metrics(ranks):
+    """(r1, r5, r10, medr, meanr) of 0-based target ranks with the reference's formulas (eval_retrieval.py:340-345). A rank of -1
+    (the target is outside the gallery) raises IndexError, as the reference's np.where(...)[0][0] does."""
+    r = ranks.detach().cpu().numpy() if torch.is_tensor(ranks) else np.asarray(ranks)
+    r = r.astype(np.float64)
+    if (r < 0).any():
+        raise IndexError("retrieval_metrics: a caption's target image is not in the gallery")
+    r1 = 100.0 * np.sum(r < 1) / len(r)
+    r5 = 100.0 * np.sum(r < 5) / len(r)
+    r10 = 100.0 * np.sum(r < 10) / len(r)
+    medr = np.floor(np.median(r) + 1)
+    meanr = np.mean(r) + 1
+    return r1, r5, r10, medr, meanr
+
+
+def _task_number(task_id):
+    """eval_retrieval.py:269-271 fills the task tokens with int(task_id[4:]): "TASK8" -> 8; an int passes through."""
+    if isinstance(task_id, str):
+        return int(task_id[4:])
+    return int(task_id)
+
+
+def read_retrieval_dataset(dataset):
+    """The reference's retrieval item protocol (RetreivalDatasetVal.__getitem__, retreival_dataset.py:430-468): item 2c + h is
+    (features, spatials, image_mask, caption, input_mask, segment_ids, target, caption_idx, image_idx) of caption c against gallery
+    half h. Returns the gallery (the two halves of items 0 and 1, concatenated), the captions in item order (int64 [C, Nt] each) and
+    every caption's target: the first image whose target is 1 (np.where(...)[0][0]); a caption without one raises IndexError."""
+    n = len(dataset)
+    if n < 2 or n % 2:
+        raise ValueError(f"retrieval dataset: {n} items; expected two gallery halves per caption")
+    halves = [dataset[0], dataset[1]]
+    feats = torch.cat([torch.as_tensor(h[0]) for h in halves])
+    spats = torch.cat([torch.as_tensor(h[1]) for h in halves])
+    imask = torch.cat([torch.as_tensor(h[2]) for h in halves])
+    caps, masks, segs, targets = [], [], [], []
+    for c in range(n // 2):
+        a, b = (halves[0], halves[1]) if c == 0 else (dataset[2 * c], dataset[2 * c + 1])
+        caps.append(torch.as_tensor(a[3]).reshape(-1))
+        masks.append(torch.as_tensor(a[4]).reshape(-1))
+        segs.append(torch.as_tensor(a[5]).reshape(-1))
+        t = np.concatenate([np.asarray(torch.as_tensor(a[6]).reshape(-1).float()), np.asarray(torch.as_tensor(b[6]).reshape(-1).float())])
+        hit = np.where(t == 1)[0]
+        if len(hit) == 0:
+            raise IndexError(f"retrieval dataset: caption {c} has no target image")
+        targets.append(int(hit[0]))
+    return (feats, spats, imask, torch.stack(caps).long(), torch.stack(masks).long(), torch.stack(segs).long(),
+            torch.tensor(targets, dtype=torch.int64))
+
+
+class RetrievalEvaluator:
+    """Scores captions against a fixed image gallery on fast-mode forward-only plans with a precomputed image prefix.
+
+    model: VILBertForVLTasks (scores = vil_logit) or BertForMultiModalPreTraining (zero shot: softmax(seq_relationship_score, 1)[:, 0]),
+    in eval mode. features f32 [G, Nv, 2048], spatials f32 [G, Nv, 5], image_mask [G, Nv], on the host (staged through pinned memory
+    one chunk at a time) or on the model's device. Chunks of `chunk` images share one plan; a smaller last chunk gets its own."""
+
+    def __init__(self, model, features, spatials, image_mask, chunk=500):
+        self.model = model
+        heads = getattr(model, "_heads", None)
+        if heads not in SCORE_HEAD:
+            raise TypeError("RetrievalEvaluator scores with VILBertForVLTasks or BertForMultiModalPreTraining")
+        if model.training:
+            raise ValueError("RetrievalEvaluator runs forward-only plans: call model.eval() first")
+        if features.dim() != 3 or spatials.shape[:2] != features.shape[:2] or tuple(image_mask.shape) != tuple(features.shape[:2]):
+            raise ValueError("gallery: features [G, Nv, F], spatials [G, Nv, 5] and image_mask [G, Nv]")
+        self.G, self.Nv = int(features.shape[0]), int(features.shape[1])
+        if self.G > MAX_GALLERY:
+            raise ValueError(f"gallery of {self.G} images: the device ranking supports at most {MAX_GALLERY}")
+        if chunk < 1:
+            raise ValueError("chunk must be positive")
+        self.features, self.spatials, self.image_mask = features, spatials, image_mask
+        self.chunk = min(int(chunk), self.G)
+        self.heads = heads
+        self.head = SCORE_HEAD[heads]
+
+    def _plan(self, n, Nt):
+        return self.model.engine.plan(n, Nt, self.Nv, heads=self.heads, outputs=(self.head,), fast_mode=True, image_prefix=True)
+
+    def _load_chunk(self, plan, lo, n):
+        dev = self.model.engine.device
+        parts = []
+        for t in (self.features, self.spatials, self.image_mask):
+            x = t[lo:lo + n]
+            if x.device.type == "cpu" and not x.is_pinned():
+                x = x.pin_memory()          # asynchronous upload; the caching host allocator keeps it alive until the copy ran
+            parts.append(x if x.device == dev or x.device.type == "cpu" else x.to(dev))
+        plan.load_images(*parts)
+        plan.run_image_prefix()
+
+    def score(self, captions, input_mask, segment_ids, task_id=None):
+        """Device f32 [C, G]: the score of every caption (int64 [C, Nt], with its mask and segment ids) against every image.
+        task_id (int or "TASKn") sets the task tokens of a model with config.task_specific_tokens; the pre-training model takes
+        none (TypeError, as its forward has no task_ids parameter)."""
+        model, eng = self.model, self.model.engine
+        if self.heads == "pretraining" and task_id is not None:
+            raise TypeError("BertForMultiModalPreTraining.forward() takes no task_ids (vilbert.py:1471-1484): score without task_id")
+        if model.training:
+            raise ValueError("RetrievalEvaluator runs forward-only plans: call model.eval() first")
+        has_task = bool(model.config.task_specific_tokens) and self.heads == "vl"
+        if has_task and task_id is None:
+            raise ValueError("config.task_specific_tokens is set: task_id is required")
+        dev = eng.device
+        C, Nt = int(captions.shape[0]), int(captions.shape[1])
+        # the caption bank: uploaded once, read row by row with device-to-device copies
+        ids = captions.to(dev, torch.int64, non_blocking=True)
+        mask = input_mask.to(dev, torch.int64, non_blocking=True)
+        seg = segment_ids.to(dev, torch.int64, non_blocking=True)
+        task = torch.full((1, 1), _task_number(task_id), dtype=torch.int64, device=dev) if has_task else None
+        scores = torch.empty((C, self.G), dtype=torch.float32, device=dev)
+        model._sync_weights()
+        n_chunks = (self.G + self.chunk - 1) // self.chunk
+        for ci, lo in enumerate(range(0, self.G, self.chunk)):
+            n = min(self.chunk, self.G - lo)
+            plan = self._plan(n, Nt)
+            self._load_chunk(plan, lo, n)
+            out = plan.outputs[self.head]
+            for c in range(C):
+                plan.load_inputs(ids[c:c + 1], None, None, seg[c:c + 1], mask[c:c + 1], None, task)
+                if eng.auto_graph:
+                    plan.maybe_capture_passes(after=1)
+                plan.run_forward()
+                if self.heads == "vl":
+                    scores[c, lo:lo + n].copy_(out.view(-1))
+                else:
+                    scores[c, lo:lo + n].copy_(torch.softmax(out, dim=1)[:, 0])
+            logger.info("retrieval: chunk %d/%d (images %d-%d) scored against %d captions", ci + 1, n_chunks, lo, lo + n - 1, C)
+        return scores
+
+    @staticmethod
+    def rank(scores, target_image, k=20):
+        """(ranks int32 [C], topk int32 [C, k]) on the device: the 0-based position of each caption's target image in its row's stable
+        descending order (ties by image index, NaN last), -1 for a target outside the gallery, and the first k images of that order
+        (-1 past the gallery's end). k <= 64."""
+        if scores.dim() != 2 or scores.dtype != torch.float32 or not scores.is_cuda or scores.stride(1) != 1:
+            raise ValueError("scores: device f32 [C, G] with contiguous rows")
+        C, G = scores.shape
+        target = torch.as_tensor(target_image).to(scores.device, torch.int64).reshape(-1).contiguous()
+        if target.numel() != C:
+            raise ValueError(f"target_image: one per caption ({C}), got {target.numel()}")
+        ranks = torch.empty(C, dtype=torch.int32, device=scores.device)
+        topk = torch.empty((C, int(k)), dtype=torch.int32, device=scores.device)
+        L.check(L.lib().vb_retrieval_rank(scores.data_ptr(), scores.stride(0), C, G, target.data_ptr(), int(k), ranks.data_ptr(),
+                                          topk.data_ptr(), torch.cuda.current_stream(scores.device).cuda_stream), "vb_retrieval_rank")
+        return ranks, topk
+
+
+def evaluate_retrieval(model, dataset, task_id=None, chunk=500, k=20):
+    """The loop of eval_retrieval.py:253-358 (and, with the pre-training model and task_id=None, of eval_coco_retrieval.py:336-412):
+    (r1, r5, r10, medr, meanr, results), results being each caption's top-k image list (the reference dumps the top 20 into
+    *_result.json). The dataset is read through the reference's item protocol (read_retrieval_dataset); metrics are taken over the
+    captions evaluated, which with the reference's 5,000 x 1,000 sizes is exactly its number. Puts the model in eval mode, as the
+    reference loop does."""
+    model.eval()
+    feats, spats, imask, caps, masks, segs, targets = read_retrieval_dataset(dataset)
+    ev = RetrievalEvaluator(model, feats, spats, imask, chunk=chunk)
+    scores = ev.score(caps, masks, segs, task_id=task_id)
+    ranks, topk = ev.rank(scores, targets, k=k)
+    both = torch.cat((ranks.view(-1, 1), topk), dim=1).cpu()       # the one read-back
+    r1, r5, r10, medr, meanr = retrieval_metrics(both[:, 0])
+    logger.info("Final r1:%.3f, r5:%.3f, r10:%.3f, mder:%.3f, meanr:%.3f", r1, r5, r10, medr, meanr)
+    return r1, r5, r10, medr, meanr, both[:, 1:1 + min(k, ev.G)].tolist()
