@@ -141,6 +141,9 @@ vb_status vb_gemm_plan(const vb_gemm_args* args, int32_t sm_count, int32_t* bloc
  *   lse:  f32 [B, H, Nq] row log-sum-exp in the log2 domain (saved for backward; may be NULL in fwd)
  * Backward recomputes P from lse: needs dO (bf16), writes dQ/dK/dV (bf16, same indexing as Q/K/V with
  * their own ld) and uses delta [B, H, Nq] f32 as scratch. D in {16, 32, 64, 128}; Nq, Nk <= ~320.
+ * Partial backward: dQ may be NULL (dK / dV only), or dK and dV may both be NULL (dQ only); what is written is bitwise what the
+ * full backward writes there. dK without dV (or the reverse) and all three NULL return VB_ERR_INVALID. A bias sum follows its
+ * gradient: dbias_q is ignored when dQ is NULL, dbias_k / dbias_v when dK / dV are.
  */
 typedef struct vb_attn_args {
   int32_t B, H, Nq, Nk, D;
@@ -213,7 +216,8 @@ vb_status vb_cast2d_f32_to_bf16(const float* src, int64_t lds, void* dst, int64_
 /* BertEmbeddings.forward before its LayerNorm (vilbert.py:346-362): out[b,p,:] = word[ids] + pos[arange] +
  * type[token_type_ids]; if task_ids != NULL the task embedding row is inserted at position 1 (no pos/type
  * term) and the output has Nt+1 rows per sample. ids / token_type_ids [B,Nt] int64, task_ids [B] int64.
- * Backward scatter-adds into the tables (word row 0 = padding_idx gets no gradient, :328-330). */
+ * Backward scatter-adds into the tables (word row 0 = padding_idx gets no gradient, :328-330); any of dword / dpos / dtype /
+ * dtask may be NULL (a frozen table: nothing is written to it). */
 vb_status vb_embed_text_fwd(const int64_t* ids, const int64_t* token_type_ids, const int64_t* task_ids,
                             const float* word, const float* pos, const float* type, const float* task,
                             float* out, int32_t B, int32_t Nt, int32_t H, void* stream);
@@ -222,7 +226,7 @@ vb_status vb_embed_text_bwd(const float* dout, const int64_t* ids, const int64_t
                             int32_t B, int32_t Nt, int32_t H, void* stream);
 
 /* BertImageEmbeddings.image_location_embeddings (vilbert.py:1416,1424): out[m,:] = loc[m,:5] W^T + b,
- * W [H,5]; consumed as the residual of the 2048 -> Hv region-feature GEMM. Backward accumulates dW, db. */
+ * W [H,5]; consumed as the residual of the 2048 -> Hv region-feature GEMM. Backward accumulates dW, db (either may be NULL). */
 vb_status vb_loc_proj_fwd(const float* loc, const float* W, const float* b, float* out, int32_t M, int32_t H, void* stream);
 vb_status vb_loc_proj_bwd(const float* dy, const float* loc, float* dW, float* db, int32_t M, int32_t H, void* stream);
 
@@ -232,7 +236,7 @@ vb_status vb_colsum(const void* X, int32_t is_bf16, int64_t ld, float* out, int3
 /* Linears with 1..8 outputs (vil_logit, vil_tri_prediction, vision_logit, linguisic_logit,
  * bi_seq_relationship, the 2-way output of vil_binary_prediction; vilbert.py:1231,1620-1628,1684-1695):
  * y[m,j] = x[m,:] . W[j,:] + b[j] (+ row_addend[m]). Backward: dx (=, or += when accumulate_dx),
- * dW and db ACCUMULATED. */
+ * dW and db ACCUMULATED; each of dx / dW / db may be NULL (not computed). */
 vb_status vb_small_linear_fwd(const float* x, int64_t ldx, const float* W, const float* b, const float* row_addend,
                               float* y, int32_t M, int32_t K, int32_t N,
                               const vb_dropout* in_dropout /* NULL or dropout applied to x first (index m*K + k; needs ldx == K) */, void* stream);
@@ -241,7 +245,7 @@ vb_status vb_small_linear_bwd(const float* dy, const float* x, int64_t ldx, cons
                               const vb_dropout* in_dropout, void* stream);
 
 /* pooled_output = pooled_t (*|+) pooled_v (fusion_method, vilbert.py:1677-1682, 1236-1241); backward
- * ACCUMULATES into da / db. */
+ * ACCUMULATES into da / db (either may be NULL). */
 vb_status vb_fuse_pooled_fwd(const float* a, const float* b, float* out_f32, void* out_bf16, int64_t n, int32_t mul,
                              const vb_dropout* dropout /* NULL or dropout on the fused vector (index i) */,
                              int32_t out_fp16, void* out_lo /* format / split-precision low part of out_bf16 */,
@@ -361,7 +365,8 @@ vb_status vb_nce_region_loss(const float* scores, const float* target, const int
  *   vb_gate_scale_fwd   qk[b*N+n, c] *= 1 + sigmoid(z[b,c]) for c < cols, in place on the Q|K sections of the 16-bit projection
  *                       buffer (row pitch ld elements, hi (+ lo) parts, fp16 or bf16); z f32 [B, cols] = dyLinear_q | dyLinear_k outputs
  *   vb_gate_scale_bwd   dqk (bf16, in place) <- gate * dqk;  dz[b,c] = s(1-s) * sum_n dqk[b,n,c] qk[b,n,c] / gate, s = sigmoid(z);
- *                       qk is the GATED forward buffer; dz f32 [B, cols] and its bf16 operand copy dz16 */
+ *                       qk is the GATED forward buffer; dz f32 [B, cols] and its bf16 operand copy dz16, each may be NULL (both
+ *                       NULL: only dqk is scaled, for a frozen gate Linear whose input needs no gradient) */
 vb_status vb_masked_mean_fwd(const float* x, const float* add_mask, float* pool, void* pool16, void* pool16_lo, void* pool16_b, int32_t out_fp16,
                              int32_t B, int32_t N, int32_t H, void* stream);
 vb_status vb_masked_mean_bwd(const float* dpool, const float* add_mask, float* dx, int32_t accumulate, int32_t B, int32_t N, int32_t H, void* stream);

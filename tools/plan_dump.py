@@ -77,6 +77,15 @@ def cases(O, LOSS_HEADS):
         ("retrieval_prefix", {}, "vl", 4, dict(outputs=("vil_logit",), fast_mode=True, image_prefix=True)),
         ("retrieval_prefix_task_tokens", dict(task_specific_tokens=True), "vl", 4, dict(outputs=("vil_logit",), fast_mode=True, image_prefix=True)),
         ("retrieval_zero_shot", {}, "pretraining", 4, dict(outputs=("seq_relationship_score",), fast_mode=True, image_prefix=True)),
+        # frozen parameters (requires_grad=False): the text embeddings; the image embedding and the image-side projections of the
+        # first connection layer (partial co-attention backward)
+        ("frozen_text_embeddings", {}, "vl", 4, dict(train, frozen=frozenset(
+            f"bert.embeddings.{n}" for n in ("word_embeddings.weight", "position_embeddings.weight", "token_type_embeddings.weight",
+                                             "LayerNorm.weight", "LayerNorm.bias")))),
+        ("frozen_vision_input", {}, "vl", 4, dict(train, frozen=frozenset(
+            [f"bert.v_embeddings.{n}" for n in ("image_embeddings.weight", "image_embeddings.bias", "image_location_embeddings.weight",
+                                               "image_location_embeddings.bias", "LayerNorm.weight", "LayerNorm.bias")] +
+            [f"bert.encoder.c_layer.0.biattention.{n}{i}.{w}" for n in ("query", "key", "value") for i in (1,) for w in ("weight", "bias")]))),
     ]
 
 

@@ -300,7 +300,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
 }
 
 // ------------------------------------------------------------------------------------------ backward: dQ
-template <int D>
+// DQ = false (dK / dV-only backward): the kernel writes delta, which the dK / dV kernel reads, and nothing else; it stages only dO.
+template <int D, bool DQ = true>
 __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnParams p) {
   constexpr int LD = D + 8;
   extern __shared__ __align__(16) uint8_t smem_att[];
@@ -317,15 +318,17 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
   const int g = lane >> 2, t = lane & 3;
   const int rows_valid = min(TQ, p.Nq - q0);
 
-  load_panel<D>(sQ, p.Q + ((long long)b * p.Nq + q0) * p.ldq + h * D, p.ldq, rows_valid, TQ);
+  if constexpr (DQ) load_panel<D>(sQ, p.Q + ((long long)b * p.Nq + q0) * p.ldq + h * D, p.ldq, rows_valid, TQ);
   load_panel<D>(sdO, p.dO + ((long long)b * p.Nq + q0) * p.lddo + h * D, p.lddo, rows_valid, TQ);
-  load_panel<D>(sK, p.K + (long long)b * p.Nk * p.ldk + h * D, p.ldk, p.Nk, nkp);
-  load_panel<D>(sV, p.V + (long long)b * p.Nk * p.ldv + h * D, p.ldv, p.Nk, nkp);
-  for (int j = threadIdx.x; j < nkp; j += ATT_THREADS)
-    sMask[j] = (j < p.Nk) ? (p.mask ? p.mask[(long long)b * p.Nk + j] * LOG2E : 0.f) : -CUDART_INF_F;
+  if constexpr (DQ) {
+    load_panel<D>(sK, p.K + (long long)b * p.Nk * p.ldk + h * D, p.ldk, p.Nk, nkp);
+    load_panel<D>(sV, p.V + (long long)b * p.Nk * p.ldv + h * D, p.ldv, p.Nk, nkp);
+    for (int j = threadIdx.x; j < nkp; j += ATT_THREADS)
+      sMask[j] = (j < p.Nk) ? (p.mask ? p.mask[(long long)b * p.Nk + j] * LOG2E : 0.f) : -CUDART_INF_F;
+  }
   cp_async_wait_all();
   __syncthreads();
-  if (p.qkv_fp16) {
+  if (DQ && p.qkv_fp16) {
     panel_f16_to_bf16<D, ATT_THREADS>(sQ, TQ); panel_f16_to_bf16<D, ATT_THREADS>(sK, nkp); panel_f16_to_bf16<D, ATT_THREADS>(sV, nkp);
     __syncthreads();
   }
@@ -372,6 +375,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
       if (r0 + g + 8 < rows_valid) dg[r0 + g + 8] = dl[1];
     }
   }
+  if constexpr (!DQ) return;
 
   const float c = p.scale * LOG2E;
   const uint32_t dseed = p.drop.ctr ? drop_seed(p.drop) : 0u;
@@ -523,8 +527,10 @@ __device__ __forceinline__ void mma_at_b(float (&acc)[D / 8][4], const __nv_bflo
 // block from registers, dQ += dS K, and P (with the dropout factor) / dS are parked as bf16 [query][key] tiles in shared
 // memory. Phase 2: warp w owns key rows [16w, 16w+16): dV = P^T dO and dK = dS^T Q over all queries (A fragments by
 // ldmatrix.trans). No recompute, no atomics, deterministic; the two-kernel path below remains for longer sequences.
+// Partial backward (a frozen side of a co-attention): DQ = false skips the dQ accumulation and its store; DKV = false skips phase 2
+// and the P / dS tiles parked for it (and their shared memory). Every output written is bitwise the full backward's.
 constexpr int ATT1_THREADS = 256;
-template <int D>
+template <int D, bool DQ = true, bool DKV = true>
 __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const AttnParams p) {
   constexpr int LD = D + 8;
   extern __shared__ __align__(16) uint8_t smem_att[];
@@ -538,7 +544,7 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
   __nv_bfloat16* sV = sK + nkp * LD;
   __nv_bfloat16* sP = sV + nkp * LD;
   __nv_bfloat16* sdS = sP + nqp * LDP;
-  float* sMask = reinterpret_cast<float*>(sdS + nqp * LDP);
+  float* sMask = reinterpret_cast<float*>(DKV ? sdS + nqp * LDP : sP);
 
   const int b = blockIdx.y, h = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -621,16 +627,20 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
         // dS = P o (mask/(1-p) o dP - delta); the tile kept for dV is mask/(1-p) o P
         s[nt][0] = p0 * (dp[nt][0] * f0 - dl[0]); s[nt][1] = p1 * (dp[nt][1] * f1 - dl[0]);
         s[nt][2] = p2 * (dp[nt][2] * f2 - dl[1]); s[nt][3] = p3 * (dp[nt][3] * f3 - dl[1]);
-        *reinterpret_cast<uint32_t*>(sP + (r0 + g) * LDP + col) = pack_bf16(p0 * f0, p1 * f1);
-        *reinterpret_cast<uint32_t*>(sP + (r0 + g + 8) * LDP + col) = pack_bf16(p2 * f2, p3 * f3);
-        *reinterpret_cast<uint32_t*>(sdS + (r0 + g) * LDP + col) = pack_bf16(s[nt][0], s[nt][1]);
-        *reinterpret_cast<uint32_t*>(sdS + (r0 + g + 8) * LDP + col) = pack_bf16(s[nt][2], s[nt][3]);
+        if constexpr (DKV) {
+          *reinterpret_cast<uint32_t*>(sP + (r0 + g) * LDP + col) = pack_bf16(p0 * f0, p1 * f1);
+          *reinterpret_cast<uint32_t*>(sP + (r0 + g + 8) * LDP + col) = pack_bf16(p2 * f2, p3 * f3);
+          *reinterpret_cast<uint32_t*>(sdS + (r0 + g) * LDP + col) = pack_bf16(s[nt][0], s[nt][1]);
+          *reinterpret_cast<uint32_t*>(sdS + (r0 + g + 8) * LDP + col) = pack_bf16(s[nt][2], s[nt][3]);
+        }
       }
-      mma_p_b<D>(dq, s, sK, kb, lane, p.Nk);
+      if constexpr (DQ) mma_p_b<D>(dq, s, sK, kb, lane, p.Nk);
     }
-    store_tile<D>(p.dQ + (long long)b * p.Nq * p.lddq + h * D, p.lddq, dq, p.scale, p.scale, r0, p.Nq, lane,
-                  p.dbq ? p.dbq + h * D : nullptr);
+    if constexpr (DQ)
+      store_tile<D>(p.dQ + (long long)b * p.Nq * p.lddq + h * D, p.lddq, dq, p.scale, p.scale, r0, p.Nq, lane,
+                    p.dbq ? p.dbq + h * D : nullptr);
   }
+  if constexpr (!DKV) return;
   __syncthreads();
   // ---- phase 2: this warp's 16 key rows
   if (r0 < p.Nk) {
@@ -705,8 +715,12 @@ static int validate(const vb_attn_args* a, bool bwd) {
   if ((a->ldq % 8) || (a->ldk % 8) || (a->ldv % 8) || (a->ldo % 8) || !al16(a->Q) || !al16(a->K) || !al16(a->V) || !al16(a->O))
     return set_error(VB_ERR_INVALID, "vb_attention: tensors need ld %% 8 == 0 and 16-byte aligned bases");
   if (bwd) {
-    if (!a->dO || !a->dQ || !a->dK || !a->dV || !a->lse || !a->delta) return set_error(VB_ERR_INVALID, "vb_attention_bwd: null tensor");
-    if ((a->lddo % 8) || (a->lddq % 8) || (a->lddk % 8) || (a->lddv % 8) || !al16(a->dO) || !al16(a->dQ) || !al16(a->dK) || !al16(a->dV))
+    // partial output sets: dQ alone, or dK and dV together (either side of a co-attention may be frozen)
+    if (!a->dQ && !a->dK && !a->dV) return set_error(VB_ERR_INVALID, "vb_attention_bwd: dQ, dK and dV are all NULL");
+    if (!a->dK != !a->dV) return set_error(VB_ERR_INVALID, "vb_attention_bwd: dK and dV are computed together (both or neither)");
+    if (!a->dO || !a->lse || !a->delta) return set_error(VB_ERR_INVALID, "vb_attention_bwd: null tensor");
+    if ((a->lddo % 8) || !al16(a->dO) || (a->dQ && ((a->lddq % 8) || !al16(a->dQ))) ||
+        (a->dK && ((a->lddk % 8) || (a->lddv % 8) || !al16(a->dK) || !al16(a->dV))))
       return set_error(VB_ERR_INVALID, "vb_attention_bwd: gradient tensors need ld %% 8 == 0 and 16-byte aligned bases");
   }
   return VB_OK;
@@ -789,6 +803,7 @@ extern "C" vb_status vb_attention_bwd(const vb_attn_args* a, void* stream) {
   if (int s = validate(a, true)) return s;
   const AttnParams p = to_params(a);
   cudaStream_t st = (cudaStream_t)stream;
+  const bool want_dq = a->dQ != nullptr, want_dkv = a->dK != nullptr;
   const int nkp = (a->Nk + KB - 1) / KB * KB, nqp = (a->Nq + KB - 1) / KB * KB;
   // short sequences (all of ViLBERT's): one CTA per (batch, head) computes dQ, dK and dV in a single pass
   static const bool two_kernels_forced = getenv("VB_ATTN_BWD_TWO_KERNELS") != nullptr;   // development switch (tools/attn_probe.py)
@@ -797,31 +812,40 @@ extern "C" vb_status vb_attention_bwd(const vb_attn_args* a, void* stream) {
     const size_t smem_f = (size_t)(2 * nq16 + 2 * nkp) * (a->D + 8) * 2 + (size_t)2 * nq16 * (nkp + 8) * 2 + (size_t)nkp * 4;
     if (smem_f <= 227 * 1024) {
       dim3 gf(a->H, a->B);
+      const char* what = "vb_attention_bwd(fused)";
+      // the dQ-only variant keeps no P / dS tiles
+      const size_t smem_q = smem_f - (size_t)2 * nq16 * (nkp + 8) * 2;
+#define VB_BWD_FUSED(DD)                                                                                            \
+  if (!want_dkv) return launch_att(attn_bwd_fused_kernel<DD, true, false>, gf, smem_q, p, st, what, ATT1_THREADS); \
+  if (!want_dq) return launch_att(attn_bwd_fused_kernel<DD, false, true>, gf, smem_f, p, st, what, ATT1_THREADS);  \
+  return launch_att(attn_bwd_fused_kernel<DD>, gf, smem_f, p, st, what, ATT1_THREADS);
       switch (a->D) {
-        case 32: return launch_att(attn_bwd_fused_kernel<32>, gf, smem_f, p, st, "vb_attention_bwd(fused)", ATT1_THREADS);
-        case 64: return launch_att(attn_bwd_fused_kernel<64>, gf, smem_f, p, st, "vb_attention_bwd(fused)", ATT1_THREADS);
-        default: return launch_att(attn_bwd_fused_kernel<128>, gf, smem_f, p, st, "vb_attention_bwd(fused)", ATT1_THREADS);
+        case 32: VB_BWD_FUSED(32)
+        case 64: VB_BWD_FUSED(64)
+        default: VB_BWD_FUSED(128)
       }
+#undef VB_BWD_FUSED
     }
   }
+  // two kernels: dQ (which also writes delta), then dK / dV. Without dQ the first kernel only writes delta; without dK / dV the
+  // second is not launched.
   const size_t smem_q = (size_t)(2 * TQ + 2 * nkp) * (a->D + 8) * 2 + (size_t)nkp * 4;
+  const size_t smem_delta = (size_t)(2 * TQ) * (a->D + 8) * 2;
   const size_t smem_k = (size_t)(2 * TQ + 2 * nqp) * (a->D + 8) * 2 + (size_t)nqp * 8;
   dim3 gq((a->Nq + TQ - 1) / TQ, a->H, a->B), gk((a->Nk + TQ - 1) / TQ, a->H, a->B);
   int s;
+#define VB_BWD_TWO(DD)                                                                                                         \
+  s = want_dq ? launch_att(attn_bwd_dq_kernel<DD>, gq, smem_q, p, st, "vb_attention_bwd(dq)")                                  \
+              : launch_att(attn_bwd_dq_kernel<DD, false>, gq, smem_delta, p, st, "vb_attention_bwd(delta)");                  \
+  if (s || !want_dkv) return s;                                                                                                \
+  return launch_att(attn_bwd_dkv_kernel<DD>, gk, smem_k, p, st, "vb_attention_bwd(dkv)");
   switch (a->D) {
-    case 16:
-      if ((s = launch_att(attn_bwd_dq_kernel<16>, gq, smem_q, p, st, "vb_attention_bwd(dq)"))) return s;
-      return launch_att(attn_bwd_dkv_kernel<16>, gk, smem_k, p, st, "vb_attention_bwd(dkv)");
-    case 32:
-      if ((s = launch_att(attn_bwd_dq_kernel<32>, gq, smem_q, p, st, "vb_attention_bwd(dq)"))) return s;
-      return launch_att(attn_bwd_dkv_kernel<32>, gk, smem_k, p, st, "vb_attention_bwd(dkv)");
-    case 64:
-      if ((s = launch_att(attn_bwd_dq_kernel<64>, gq, smem_q, p, st, "vb_attention_bwd(dq)"))) return s;
-      return launch_att(attn_bwd_dkv_kernel<64>, gk, smem_k, p, st, "vb_attention_bwd(dkv)");
-    default:
-      if ((s = launch_att(attn_bwd_dq_kernel<128>, gq, smem_q, p, st, "vb_attention_bwd(dq)"))) return s;
-      return launch_att(attn_bwd_dkv_kernel<128>, gk, smem_k, p, st, "vb_attention_bwd(dkv)");
+    case 16: VB_BWD_TWO(16)
+    case 32: VB_BWD_TWO(32)
+    case 64: VB_BWD_TWO(64)
+    default: VB_BWD_TWO(128)
   }
+#undef VB_BWD_TWO
 }
 
 extern "C" vb_status vb_attention_probs(const vb_attn_args* a, float* probs, void* stream) {

@@ -277,7 +277,8 @@ embed_text_fwd_kernel(const long long* __restrict__ ids, const long long* __rest
   }
 }
 
-// scatter-add of d(out) into the embedding tables; word row 0 is padding_idx (no gradient, vilbert.py:328-330)
+// scatter-add of d(out) into the embedding tables; word row 0 is padding_idx (no gradient, vilbert.py:328-330). A NULL table
+// (a frozen embedding) receives nothing.
 __global__ void __launch_bounds__(ROW_THREADS)
 embed_text_bwd_kernel(const float* __restrict__ dout, const long long* __restrict__ ids, const long long* __restrict__ tts,
                       const long long* __restrict__ task_ids, float* __restrict__ dword, float* __restrict__ dpos,
@@ -290,20 +291,22 @@ embed_text_bwd_kernel(const float* __restrict__ dout, const long long* __restric
     const int b = (int)(row / No), p = (int)(row % No);
     const float* d = dout + row * H;
     if (has_task && p == 1) {
-      float* dt = dtask + task_ids[b] * H;
-      for (int c = lane; c < H; c += 32) atomicAdd(dt + c, d[c]);
+      if (dtask) {
+        float* dt = dtask + task_ids[b] * H;
+        for (int c = lane; c < H; c += 32) atomicAdd(dt + c, d[c]);
+      }
       continue;
     }
     const int t = (has_task && p > 1) ? p - 1 : p;
     const long long id = ids[(long long)b * Nt + t];
-    float* dw = dword + id * H;
-    float* dp = dpos + (long long)t * H;
-    float* dty = dtype + tts[(long long)b * Nt + t] * H;
+    float* dw = (dword && id != 0) ? dword + id * H : nullptr;
+    float* dp = dpos ? dpos + (long long)t * H : nullptr;
+    float* dty = dtype ? dtype + tts[(long long)b * Nt + t] * H : nullptr;
     for (int c = lane; c < H; c += 32) {
       const float v = d[c];
-      if (id != 0) atomicAdd(dw + c, v);
-      atomicAdd(dp + c, v);
-      atomicAdd(dty + c, v);
+      if (dw) atomicAdd(dw + c, v);
+      if (dp) atomicAdd(dp + c, v);
+      if (dty) atomicAdd(dty + c, v);
     }
   }
 }
@@ -330,7 +333,7 @@ __global__ void loc_proj_fwd_kernel(const float* __restrict__ loc, const float* 
   }
 }
 
-// dW[h, j] += sum_m dy[m, h] * loc[m, j];  db[h] += sum_m dy[m, h]
+// dW[h, j] += sum_m dy[m, h] * loc[m, j];  db[h] += sum_m dy[m, h]  (either may be NULL: not accumulated)
 __global__ void loc_proj_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ loc, float* __restrict__ dW,
                                     float* __restrict__ db, int M, int H, int rows_per_block) {
   pdl_entry();
@@ -345,9 +348,11 @@ __global__ void loc_proj_bwd_kernel(const float* __restrict__ dy, const float* _
     for (int j = 0; j < 5; ++j) acc[j] += d * __ldg(loc + m * 5 + j);
     acc[5] += d;
   }
+  if (dW) {
 #pragma unroll
-  for (int j = 0; j < 5; ++j) atomicAdd(dW + (long long)h * 5 + j, acc[j]);
-  atomicAdd(db + h, acc[5]);
+    for (int j = 0; j < 5; ++j) atomicAdd(dW + (long long)h * 5 + j, acc[j]);
+  }
+  if (db) atomicAdd(db + h, acc[5]);
 }
 
 // ------------------------------------------------------------------------------------------ column sums (bias grads)
@@ -403,7 +408,7 @@ small_linear_fwd_kernel(const float* __restrict__ x, long long ldx, const float*
   }
 }
 
-// dx[m, :] (+)= sum_j dy[m, j] W[j, :];  dW[j, :] += sum_m dy[m, j] x[m, :];  db[j] += sum_m dy[m, j]
+// dx[m, :] (+)= sum_j dy[m, j] W[j, :];  dW[j, :] += sum_m dy[m, j] x[m, :];  db[j] += sum_m dy[m, j]  (NULL dx / dW / db: skipped)
 __global__ void __launch_bounds__(ROW_THREADS)
 small_linear_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, long long ldx, const float* __restrict__ W,
                         float* __restrict__ dx, long long lddx, int accumulate_dx, float* __restrict__ dW, float* __restrict__ db,
@@ -413,16 +418,18 @@ small_linear_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ 
   // one CTA handles a strided set of rows; per-thread partial dW over columns k = threadIdx.x + i*ROW_THREADS
   for (int j = 0; j < N; ++j) {
     float dbp = 0.f;
-    for (int k = threadIdx.x; k < K; k += ROW_THREADS) {
-      float acc = 0.f;
-      for (long long m = blockIdx.x; m < M; m += gridDim.x) {
-        float xv = x[m * ldx + k];
-        if (drop.ctr) xv = drop_apply(xv, dseed, (uint32_t)(m * K + k), drop);
-        acc += dy[m * N + j] * xv;
+    if (dW) {
+      for (int k = threadIdx.x; k < K; k += ROW_THREADS) {
+        float acc = 0.f;
+        for (long long m = blockIdx.x; m < M; m += gridDim.x) {
+          float xv = x[m * ldx + k];
+          if (drop.ctr) xv = drop_apply(xv, dseed, (uint32_t)(m * K + k), drop);
+          acc += dy[m * N + j] * xv;
+        }
+        atomicAdd(dW + (long long)j * K + k, acc);
       }
-      atomicAdd(dW + (long long)j * K + k, acc);
     }
-    if (threadIdx.x == 0) {
+    if (db && threadIdx.x == 0) {
       for (long long m = blockIdx.x; m < M; m += gridDim.x) dbp += dy[m * N + j];
       atomicAdd(db + j, dbp);
     }
@@ -467,8 +474,8 @@ __global__ void fuse_pooled_bwd_kernel(const float* __restrict__ d, const float*
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     float g = d[i];
     if (drop.ctr) g = drop_apply(g, dseed, (uint32_t)i, drop);
-    da[i] += mul ? g * b[i] : g;
-    db[i] += mul ? g * a[i] : g;
+    if (da) da[i] += mul ? g * b[i] : g;     // a NULL side needs no gradient
+    if (db) db[i] += mul ? g * a[i] : g;
   }
 }
 // dx = dy * (y > 0) -> bf16 (pooler ReLU, vilbert.py:1121,1136)
@@ -596,6 +603,7 @@ __global__ void gate_scale_fwd_kernel(uint32_t* __restrict__ qk, uint32_t* __res
 
 // Backward of the gate: with q = gate * q_pre,   d q_pre = gate * dq (in place, bf16)   and
 // d z[b, c] = s (1 - s) * sum_n dq[b, n, c] q_pre[b, n, c],   s = sigmoid(z) = gate - 1,   q_pre = q / gate  (gate in (1, 2)).
+// dz and dz16 may each be NULL (a frozen gate Linear over text states that need no gradient): with both NULL only dq is scaled.
 __global__ void __launch_bounds__(256)
 gate_scale_bwd_kernel(__nv_bfloat16* __restrict__ dqk, long long ldd, const uint16_t* __restrict__ qk, const uint16_t* __restrict__ qk_lo, long long ld,
                       const float* __restrict__ z, float* __restrict__ dz, __nv_bfloat16* __restrict__ dz16, int N, int cols, int fp16) {
@@ -603,18 +611,22 @@ gate_scale_bwd_kernel(__nv_bfloat16* __restrict__ dqk, long long ldd, const uint
   const int b = blockIdx.y, c = blockIdx.x * 256 + threadIdx.x;
   if (c >= cols) return;
   const float s = sigmoidf_(z[(long long)b * cols + c]), g = 1.f + s;
+  const bool want_dz = dz || dz16;
   float acc = 0.f;
   for (int n = 0; n < N; ++n) {
     const long long r = (long long)b * N + n;
     const float d = __bfloat162float(dqk[r * ldd + c]);
-    float q = cvt16_to_f32(qk[r * ld + c], fp16);
-    if (qk_lo) q += cvt16_to_f32(qk_lo[r * ld + c], fp16);
-    acc += d * q;
+    if (want_dz) {
+      float q = cvt16_to_f32(qk[r * ld + c], fp16);
+      if (qk_lo) q += cvt16_to_f32(qk_lo[r * ld + c], fp16);
+      acc += d * q;
+    }
     dqk[r * ldd + c] = __float2bfloat16(d * g);
   }
+  if (!want_dz) return;
   const float v = acc / g * s * (1.f - s);
-  dz[(long long)b * cols + c] = v;
-  dz16[(long long)b * cols + c] = __float2bfloat16(v);
+  if (dz) dz[(long long)b * cols + c] = v;
+  if (dz16) dz16[(long long)b * cols + c] = __float2bfloat16(v);
 }
 
 // dst[r][i] = src[i] for r < repeats (16-byte words): FAST_MODE broadcast of the batch-1 text stream to the image batch
@@ -756,6 +768,7 @@ extern "C" vb_status vb_embed_text_bwd(const float* dout, const int64_t* ids, co
                                        void* stream) {
   if (B <= 0 || Nt <= 0) return set_error(VB_ERR_INVALID, "vb_embed_text_bwd: bad shape");
   const int has_task = task_ids != nullptr;
+  if (!dword && !dpos && !dtype && !(has_task && dtask)) return VB_OK;     // every table frozen
   const long long rows = (long long)B * (Nt + has_task);
   launch_pdl(embed_text_bwd_kernel, dim3(row_grid(rows)), dim3(ROW_THREADS), (size_t)(0), ST(stream), 
       dout, reinterpret_cast<const long long*>(ids), reinterpret_cast<const long long*>(token_type_ids),
@@ -774,6 +787,7 @@ extern "C" vb_status vb_loc_proj_fwd(const float* loc, const float* W, const flo
 
 extern "C" vb_status vb_loc_proj_bwd(const float* dy, const float* loc, float* dW, float* db, int32_t M, int32_t H, void* stream) {
   if (M <= 0 || H <= 0) return set_error(VB_ERR_INVALID, "vb_loc_proj_bwd: bad shape");
+  if (!dW && !db) return VB_OK;
   const int rpb = 64;
   dim3 grid((H + 127) / 128, (M + rpb - 1) / rpb);
   launch_pdl(loc_proj_bwd_kernel, dim3(grid), dim3(128), (size_t)(0), ST(stream), dy, loc, dW, db, M, H, rpb);
@@ -800,6 +814,7 @@ extern "C" vb_status vb_small_linear_bwd(const float* dy, const float* x, int64_
                                          int32_t accumulate_dx, float* dW, float* db, int32_t M, int32_t K, int32_t N,
                                          const vb_dropout* in_dropout, void* stream) {
   if (M <= 0 || K <= 0 || N <= 0 || N > 8) return set_error(VB_ERR_INVALID, "vb_small_linear_bwd: bad shape (N <= 8)");
+  if (!dx && !dW && !db) return VB_OK;
   int grid = sm_count(); if (grid > M) grid = M; if (grid <= 0) grid = 1;
   launch_pdl(small_linear_bwd_kernel, dim3(grid), dim3(ROW_THREADS), (size_t)(0), ST(stream), dy, x, ldx, W, dx, lddx, accumulate_dx, dW, db, M, K, N, make_drop(in_dropout));
   return check_launch("vb_small_linear_bwd");
@@ -896,7 +911,7 @@ extern "C" vb_status vb_gate_scale_fwd(void* qk, void* qk_lo, int64_t ld, const 
 
 extern "C" vb_status vb_gate_scale_bwd(void* dqk, int64_t ldd, const void* qk, const void* qk_lo, int64_t ld, const float* z, float* dz, void* dz16,
                                        int32_t B, int32_t N, int32_t cols, int32_t fp16, void* stream) {
-  if (B <= 0 || N <= 0 || cols <= 0 || !dqk || !qk || !z || !dz || !dz16) return set_error(VB_ERR_INVALID, "vb_gate_scale_bwd: bad arguments");
+  if (B <= 0 || N <= 0 || cols <= 0 || !dqk || !qk || !z) return set_error(VB_ERR_INVALID, "vb_gate_scale_bwd: bad arguments");
   launch_pdl(gate_scale_bwd_kernel, dim3((cols + 255) / 256, B), dim3(256), (size_t)0, ST(stream), static_cast<__nv_bfloat16*>(dqk), (long long)ldd,
              static_cast<const uint16_t*>(qk), static_cast<const uint16_t*>(qk_lo), (long long)ld, z, dz, static_cast<__nv_bfloat16*>(dz16), (int)N,
              (int)cols, (int)(fp16 ? 1 : 0));

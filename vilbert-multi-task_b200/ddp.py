@@ -7,6 +7,26 @@ on contiguous, fixed-address buckets (NCCL over NVLink/NVSwitch on GPUs; gloo in
 import torch
 import torch.distributed as dist
 
+from .engine import _pad8
+
+
+def trainable_ranges(ps, frozen):
+    """Coalesced [lo, hi) ranges of the flat gradient buffer of ParamStore `ps` owned by parameters not in `frozen` (entry names),
+    each entry with its padding: with nothing frozen, the whole buffer."""
+    out = []
+    for name, (off, shape) in ps.entries.items():
+        if name in frozen:
+            continue
+        n = 1
+        for d in shape:
+            n *= d
+        hi = off + _pad8(n)
+        if out and out[-1][1] == off:
+            out[-1][1] = hi
+        else:
+            out.append([off, hi])
+    return [tuple(r) for r in out]
+
 
 class FlatGradAllReducer:
     def __init__(self, flat_grad, n_buckets=8, group=None, align=1024):
@@ -16,9 +36,15 @@ class FlatGradAllReducer:
         n = flat_grad.numel()
         step = max(align, (n + n_buckets - 1) // n_buckets)
         step = (step + align - 1) // align * align
-        self.buckets = [flat_grad[i:min(i + step, n)] for i in range(0, n, step)]
+        self._bounds = [(i, min(i + step, n)) for i in range(0, n, step)]
+        self.set_ranges([(0, n)])
         # NCCL has a fused average; gloo only sums
         self.use_avg = dist.is_initialized() and dist.get_backend(group) == "nccl"
+
+    def set_ranges(self, ranges):
+        """Restricts allreduce() to the flat ranges [lo, hi) of `ranges` (the trainable parameters; frozen ones have no gradient
+        to exchange): every bucket is cut to its parts inside them. The whole buffer gives the full buckets."""
+        self.buckets = [self.flat[max(lo, a):min(hi, b)] for (lo, hi) in self._bounds for (a, b) in ranges if min(hi, b) > max(lo, a)]
 
     def allreduce(self, stream=None):
         """Averages the flat gradient buffer over all ranks, bucket by bucket (in place)."""
@@ -63,7 +89,7 @@ class FlatGradAllReducer:
 class DistributedDataParallel:
     """Drop-in for `apex.parallel.DistributedDataParallel(model, delay_allreduce=True)` as the reference uses it
     (train_tasks.py:490-497): rank 0's parameters are broadcast at wrap time and every `loss.backward()` ends with ONE all-reduce
-    (average over the world) of the flat fp32 gradient buffer. Not an nn.Module wrapper with hooks: the engine's backward calls
+    (average over the world) of the flat fp32 gradient buffer, restricted to the ranges of the trainable parameters. Not an nn.Module wrapper with hooks: the engine's backward calls
     the reducer itself. `.module` is the wrapped model, calls are forwarded."""
 
     def __init__(self, model, delay_allreduce=True, n_buckets=8, group=None):
@@ -73,6 +99,9 @@ class DistributedDataParallel:
         self.reducer.broadcast_params(eng.ps.flat)
         eng.shadow_clean = False
         model._ddp_reducer = self.reducer
+        # only the ranges of trainable parameters are exchanged; the model updates them when a requires_grad flag changes
+        model._ddp_set_ranges = self.reducer.set_ranges
+        self.reducer.set_ranges(model._trainable_ranges())
 
     def __call__(self, *args, **kwargs):
         return self.module(*args, **kwargs)

@@ -97,6 +97,7 @@ class ParamStore:
         self.device = device
         self.entries = OrderedDict()   # reference name -> (offset, shape)
         self.fused = {}                # fused qkv name -> (offset, shape)
+        self.parts = {}                # fused qkv name -> the entry names it spans, in order
         self._off = 0
         c = cfg
         Ht, It, Hv, Iv, Hb = c.hidden_size, c.intermediate_size, c.v_hidden_size, c.v_intermediate_size, c.bi_hidden_size
@@ -192,6 +193,8 @@ class ParamStore:
             self._add(f"{prefix}.{nm}.bias", (o,))
         self.fused[f"{prefix}.{fused}.weight"] = (w0, (len(names) * o, i))
         self.fused[f"{prefix}.{fused}.bias"] = (b0, (len(names) * o,))
+        self.parts[f"{prefix}.{fused}.weight"] = tuple(f"{prefix}.{nm}.weight" for nm in names)
+        self.parts[f"{prefix}.{fused}.bias"] = tuple(f"{prefix}.{nm}.bias" for nm in names)
 
     def _view(self, flat, name):
         off, shape = self.entries[name] if name in self.entries else self.fused[name]
@@ -251,7 +254,9 @@ class Act:
     def __init__(self, f32, op, M, H):
         self.f32, self.op, self.M, self.H = f32, op, M, H
         self.g32, self.gw = None, False
-        self.frozen = False     # produced under the reference's torch.no_grad() (fixed_t_layer / fixed_v_layer): no gradient flows into it
+        # no gradient flows into it: produced under the reference's torch.no_grad() (fixed_t_layer / fixed_v_layer), or by ops
+        # with no trainable parameter from inputs that need no gradient (Plan(frozen=...))
+        self.frozen = False
 
 
 # Objectives that can be fused into a plan, and the outputs each differentiates (task_utils.py:325-374, vilbert.py:1506-1590):
@@ -328,11 +333,23 @@ class Plan:
     fast_mode: text batch 1 broadcast to the image batch (None: config.fast_mode). image_prefix=True (forward-only plans): the image
     embedding (feature cast, box projection, embedding GEMM, LayerNorm) and the additive image mask are emitted into self.prefix,
     run by run_image_prefix() on what load_images() loaded, and write private buffers that no op of the forward writes; the forward
-    starts at the text embeddings and reads those image states as they are, so one image batch serves many text forwards."""
+    starts at the text embeddings and reads those image states as they are, so one image batch serves many text forwards.
+
+    frozen: ParamStore entry names whose parameters take no gradient (requires_grad=False; the tied decoder is the word-embedding
+    entry). While the forward is emitted every activation records whether it needs a gradient, as autograd does: it does when the
+    op that produced it has a trainable parameter or an input that needs one (Act.frozen is the negation). The forward is the
+    same; the backward computes no gradient of a frozen parameter (no weight-gradient GEMM, bias column sum, LayerNorm gamma /
+    beta sum or embedding scatter), no gradient of an activation that needs none, and registers nothing for a block with nothing
+    to do. No range a frozen parameter owns appears in grad_touch. self.out_rg tells which outputs carry a gradient."""
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False):
+                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset()):
         self.e, self.cfg = engine, engine.cfg
+        self.frozen = frozenset(frozen)
+        unknown = sorted(n for n in self.frozen if n not in engine.ps.entries)
+        if unknown:
+            raise ValueError(f"frozen: {unknown[:4]} are not parameter entries of this model")
+        self.out_rg = {}              # output name -> it carries a gradient (some trainable parameter lies upstream of it)
         self.grad_touch = {}           # (flat offset, numel) -> index of the last backward op writing that gradient range
         self.ps = _TrackedParams(engine.ps, self)
         self.lib = L.lib()
@@ -444,6 +461,41 @@ class Plan:
     def want(self, name):
         """Whether the head `name` is built (outputs=)."""
         return self.keep is None or name in self.keep
+
+    # ------------------------------------------------------------------ frozen parameters
+    def trainable(self, *names):
+        """Whether any of the parameters `names` (entries or fused projections) takes a gradient."""
+        parts = self.e.ps.parts
+        return any(p not in self.frozen for n in names for p in parts.get(n, (n,)))
+
+    def pg(self, name):
+        """Gradient view of the entry `name` for a backward op to write, or None when it is frozen."""
+        return None if name in self.frozen else self.ps.g(name)
+
+    def gparts(self, name):
+        """Gradient views of the parts of `name` (the entries of a fused projection, or the entry itself), None for a frozen part.
+        With every part trainable they are slices of one view of the whole range."""
+        ps = self.ps
+        parts = ps.parts.get(name)
+        if parts is None:
+            return [self.pg(name)]
+        if not any(p in self.frozen for p in parts):
+            g = ps.g(name)
+            n = g.shape[0] // len(parts)
+            return [g[i * n:(i + 1) * n] for i in range(len(parts))]
+        return [self.pg(p) for p in parts]
+
+    @staticmethod
+    def _runs(parts):
+        """Maximal runs [a, b) of consecutive non-None entries of `parts`."""
+        runs, a = [], None
+        for i, g in enumerate(list(parts) + [None]):
+            if g is not None and a is None:
+                a = i
+            elif g is None and a is not None:
+                runs.append((a, i))
+                a = None
+        return runs
 
     # ------------------------------------------------------------------ infrastructure
     def buf(self, shape, dtype=F32, zero=False):
@@ -621,7 +673,7 @@ class Plan:
     def ln_bwd(self, dy, x, gamma, mean, rstd, dx32, dx16, M, H, ggamma, gbeta, pre=None, gbias=None, out_drop=None, in_drop=None):
         """gbias: bias gradient of the Linear feeding this LayerNorm (column sums of dx), fused into the same pass."""
         self.emit(self.lib.vb_layernorm_bwd, dy.data_ptr(), H, x.data_ptr(), H, gamma.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
-                  self._ptr(dx32), self._ptr(dx16), H, self._ptr(pre), H, ggamma.data_ptr(), gbeta.data_ptr(), self._ptr(gbias), M, H,
+                  self._ptr(dx32), self._ptr(dx16), H, self._ptr(pre), H, self._ptr(ggamma), self._ptr(gbeta), self._ptr(gbias), M, H,
                   self._ref(out_drop), self._ref(in_drop))
 
     def colsum(self, X, ld, out, M, N):
@@ -636,10 +688,22 @@ class Plan:
     def linear_wgrad(self, dy16, ld_dy, dy_bias, ld_dyb, x16, ld_x, M, N_out, K_in, wname, gw=None):
         """dW += dy^T x (split-K, atomics). Nothing on the critical chain depends on it, so with wgrad_streams it is issued on
         a side stream (2 = text chain, 3 = vision chain) right after an event marking that dy is ready; the side streams are
-        joined at the data-parallel segment cuts and at the end of the backward pass."""
+        joined at the data-parallel segment cuts and at the end of the backward pass. Frozen parameters (parts of a fused
+        projection) get no column sum and no GEMM: each run of trainable parts gets its own on its columns of dy."""
         if dy_bias is not None:
-            self.colsum(dy_bias, ld_dyb, self.ps.g(wname + ".bias"), M, N_out)
-        out = gw if gw is not None else self.ps.g(wname + ".weight")
+            gb = self.gparts(wname + ".bias")
+            nb = N_out // len(gb)
+            for a, b in self._runs(gb):
+                self.colsum(dy_bias[:, a * nb:b * nb], ld_dyb, gb[a], M, (b - a) * nb)
+        if gw is not None:
+            self._wgrad(dy16, ld_dy, x16, ld_x, M, N_out, K_in, gw)
+            return
+        gws = self.gparts(wname + ".weight")
+        nw = N_out // len(gws)
+        for a, b in self._runs(gws):
+            self._wgrad(dy16[:, a * nw:b * nw], ld_dy, x16, ld_x, M, (b - a) * nw, K_in, gws[a])
+
+    def _wgrad(self, dy16, ld_dy, x16, ld_x, M, N_out, K_in, out):
         if not self.wgrad_streams:
             self.gemm(N_out, K_in, M, dy16, ld_dy, x16, ld_x, a_mn=1, b_mn=1, out_f32=out, ld_of=K_in, atomic=1, split_k=0)
             return
@@ -654,7 +718,7 @@ class Plan:
 
     # act.g32 (+)= dy16 @ W (+ extra32)
     def dgrad_into(self, act, dy16, ld_dy, W16, M, N_out, K_in, extra32=None):
-        if act.frozen:      # the producer ran under no_grad: the gradient stops here
+        if act.frozen:      # the activation needs no gradient (frozen producer, or fixed_*_layer's no_grad): it stops here
             return
         g = self.grad_of(act)
         if not act.gw:
@@ -675,14 +739,16 @@ class Plan:
         self.emit(self.lib.vb_axpy_f32, src32.data_ptr(), g.data_ptr(), g.numel(), 1.0)
 
     # ------------------------------------------------------------------ blocks
-    def dense_res_ln(self, a, K_in, res, wname, lnname, tag, drop=None):
-        """LN(dense(a) + residual)  — BertSelfOutput / BertOutput / BertBiOutput halves (vilbert.py:470-474, 513-517, 844-855)."""
+    def dense_res_ln(self, a, K_in, res, wname, lnname, tag, drop=None, a_rg=True):
+        """LN(dense(a) + residual)  — BertSelfOutput / BertOutput / BertBiOutput halves (vilbert.py:470-474, 513-517, 844-855).
+        a_rg: whether `a` needs a gradient (the caller's backward takes the returned dy16 into it)."""
         ps, M, H = self.ps, res.M, res.H
         y = self.buf((M, H), F32)
         self.gemm(M, H, K_in, a, K_in, ps.w(wname + ".weight"), K_in, bias=ps.p(wname + ".bias"), residual=res.f32, ld_res=H,
                   out_f32=y, ld_of=H, dropout=drop)
         o32, o, mean, rstd = self.ln_fwd(y, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, H)
         out = Act(o32, o, M, H)
+        out.frozen = not (a_rg or not res.frozen or self.trainable(wname + ".weight", wname + ".bias", lnname + ".weight", lnname + ".bias"))
 
         def bwd():
             """returns (dy16, dy32) of the dense output (== grad of the LN input); adds dy32 to res."""
@@ -690,8 +756,8 @@ class Plan:
                 return None
             dy32 = self.scratch(tag + ".dy32", (M, H), F32)
             dy16 = self.scratch(tag + ".dy16", (M, H), BF16)
-            self.ln_bwd(out.g32, y, ps.p(lnname + ".weight"), mean, rstd, dy32, dy16, M, H, ps.g(lnname + ".weight"), ps.g(lnname + ".bias"),
-                        gbias=ps.g(wname + ".bias"), in_drop=drop)
+            self.ln_bwd(out.g32, y, ps.p(lnname + ".weight"), mean, rstd, dy32, dy16, M, H, self.pg(lnname + ".weight"), self.pg(lnname + ".bias"),
+                        gbias=self.pg(wname + ".bias"), in_drop=drop)
             self.linear_wgrad(dy16, H, None, 0, a.bw, K_in, M, H, K_in, wname)
             return dy16, dy32
         return out, bwd
@@ -703,20 +769,22 @@ class Plan:
         f = self.buf16((M, I))
         self.gemm(M, I, H, x.op, H, ps.w(w1 + ".weight"), H, bias=ps.p(w1 + ".bias"), act=L.VB_ACT_GELU, out_bf16=f, ld_ob=I,
                   out_pre=pre16, ld_op=I)
-        out, out_bwd = self.dense_res_ln(f, I, x, w2, lnname, tag + ".o", drop=drop)
+        f_rg = not x.frozen or self.trainable(w1 + ".weight", w1 + ".bias")
+        out, out_bwd = self.dense_res_ln(f, I, x, w2, lnname, tag + ".o", drop=drop, a_rg=f_rg)
 
         def bwd():
             r = out_bwd()
-            if r is None:
+            if r is None or not f_rg:
                 return
             dy16, dy32 = r
             dpre16 = self.scratch(tag + ".dpre16", (M, I), BF16)
             # d pre = (dy W2) * gelu'(pre)
             self.gemm(M, I, H, dy16, H, ps.w(w2 + ".weight").bw, I, b_mn=1, aux=pre16, ld_aux=I, act=L.VB_ACT_DGELU, out_bf16=dpre16, ld_ob=I,
-                      out_colsum=ps.g(w1 + ".bias"))
+                      out_colsum=self.pg(w1 + ".bias"))
             self.linear_wgrad(dpre16, I, None, 0, x.op.bw, H, M, I, H, w1)
             self.dgrad_into(x, dpre16, I, ps.w(w1 + ".weight").bw, M, I, H, extra32=dy32)
-        self.push_bwd(bwd)
+        if not out.frozen:
+            self.push_bwd(bwd)
         return out
 
     def self_attention_block(self, x, B, N, nh, mask, prefix, tag, p_attn=0.0, p_hidden=0.0, pool=None):
@@ -739,34 +807,43 @@ class Plan:
         self.attention(False, B, nh, N, N, D, q, 3 * H, k, 3 * H, v, 3 * H, mask, ctx, H, lse, dropout=adrop)
         if self.viz:
             (self.attn_t if tag == "t" else self.attn_v).append(self._last_attn)
+        qkv_rg = not x.frozen or self.trainable(prefix + ".self.qkv.weight", prefix + ".self.qkv.bias")
+        gate_rg = pool is not None and (not pool.frozen or self.trainable(prefix + ".self.dy.weight", prefix + ".self.dy.bias"))
+        ctx_rg = qkv_rg or gate_rg
         out, out_bwd = self.dense_res_ln(ctx, H, x, prefix + ".output.dense", prefix + ".output.LayerNorm", tag + ".ao",
-                                         drop=self.drop(prefix + ".output.dropout", p_hidden))
+                                         drop=self.drop(prefix + ".output.dropout", p_hidden), a_rg=ctx_rg)
 
         def bwd():
             r = out_bwd()
-            if r is None:
+            if r is None or not ctx_rg:
                 return
             dy16, dy32 = r
             dctx = self.scratch(tag + ".dctx", (M, H), BF16)
             self.gemm(M, H, H, dy16, H, ps.w(prefix + ".output.dense.weight").bw, H, b_mn=1, out_bf16=dctx, ld_ob=H)
             dqkv = self.scratch(tag + ".dqkv", (M, 3 * H), BF16)
             delta = self.scratch(tag + ".delta", (B, nh, N), F32)
-            gb = ps.g(prefix + ".self.qkv.bias")     # bias gradients = column sums of dQ|dK|dV, fused into the attention backward
+            # bias gradients = column sums of dQ|dK|dV, fused into the attention backward
+            gq, gk, gv = self.gparts(prefix + ".self.qkv.bias")
             gated = pool is not None                 # ... except under the gate, where the biases sit before the scaling
             self.attention(True, B, nh, N, N, D, q, 3 * H, k, 3 * H, v, 3 * H, mask, ctx, H, lse, dO=dctx, lddo=H,
                            dQ=dqkv[:, 0:H], lddq=3 * H, dK=dqkv[:, H:2 * H], lddk=3 * H, dV=dqkv[:, 2 * H:], lddv=3 * H, delta=delta,
-                           dbq=None if gated else gb[0:H], dbk=None if gated else gb[H:2 * H], dbv=gb[2 * H:], dropout=adrop)
+                           dbq=None if gated else gq, dbk=None if gated else gk, dbv=gv, dropout=adrop)
             if gated:
-                dz32 = self.scratch(tag + ".dz32", (B, 2 * H), F32)
-                dz16 = self.scratch(tag + ".dz16", (B, 2 * H), BF16)
-                self.emit(self.lib.vb_gate_scale_bwd, dqkv.data_ptr(), 3 * H, qkv.hi.data_ptr(), self._ptr(qkv.lo), 3 * H, z.data_ptr(), dz32.data_ptr(),
-                          dz16.data_ptr(), B, N, 2 * H, qkv.fp16)
-                self.colsum(dqkv, 3 * H, gb[0:2 * H], M, 2 * H)
-                self.linear_wgrad(dz16, 2 * H, dz32, 2 * H, pool.op.bw, pool.H, B, 2 * H, pool.H, prefix + ".self.dy")
-                self.dgrad_into(pool, dz16, 2 * H, ps.w(prefix + ".self.dy.weight").bw, B, 2 * H, pool.H)
+                # the gate Linear needs dz32 for its bias sum, dz16 for its weight gradient and for d pool
+                dyw_rg = self.trainable(prefix + ".self.dy.weight") or not pool.frozen
+                dz32 = self.scratch(tag + ".dz32", (B, 2 * H), F32) if self.trainable(prefix + ".self.dy.bias") else None
+                dz16 = self.scratch(tag + ".dz16", (B, 2 * H), BF16) if dyw_rg else None
+                self.emit(self.lib.vb_gate_scale_bwd, dqkv.data_ptr(), 3 * H, qkv.hi.data_ptr(), self._ptr(qkv.lo), 3 * H, z.data_ptr(), self._ptr(dz32),
+                          self._ptr(dz16), B, N, 2 * H, qkv.fp16)
+                for (a, b) in self._runs((gq, gk)):      # the parts of one range are adjacent in the flat buffer
+                    self.colsum(dqkv[:, a * H:b * H], 3 * H, (gq, gk)[a], M, (b - a) * H)
+                if dz32 is not None or dz16 is not None:
+                    self.linear_wgrad(dz16, 2 * H, dz32, 2 * H, pool.op.bw, pool.H, B, 2 * H, pool.H, prefix + ".self.dy")
+                    self.dgrad_into(pool, dz16, 2 * H, ps.w(prefix + ".self.dy.weight").bw, B, 2 * H, pool.H)
             self.linear_wgrad(dqkv, 3 * H, None, 0, x.op.bw, H, M, 3 * H, H, prefix + ".self.qkv")
             self.dgrad_into(x, dqkv, 3 * H, ps.w(prefix + ".self.qkv.weight").bw, M, 3 * H, H, extra32=dy32)
-        self.push_bwd(bwd)
+        if not out.frozen:
+            self.push_bwd(bwd)
         return out
 
     def connection_layer(self, v, t, idx):
@@ -798,21 +875,28 @@ class Plan:
         if self.viz:
             self.attn_c.append((a1, a2))
         # biOutput: ctx2 -> vision stream (dense1 / LayerNorm1), ctx1 -> text stream (dense2 / LayerNorm2) (:890-892)
+        # a side whose projections are frozen and whose input needs no gradient takes no gradient: dQ of its queries' direction
+        # and dK / dV of the other are not computed
+        need1 = not v.frozen or self.trainable(p + ".biattention.qkv1.weight", p + ".biattention.qkv1.bias")
+        need2 = not t.frozen or self.trainable(p + ".biattention.qkv2.weight", p + ".biattention.qkv2.bias")
+        ctx_rg = need1 or need2
         with self.on(1):
             v1o, v1_bwd = self.dense_res_ln(ctx2, Hb, v, p + ".biOutput.dense1", p + ".biOutput.LayerNorm1", "c.v.bo",
-                                            drop=self.drop(p + ".biOutput.dropout1", c.v_hidden_dropout_prob))
+                                            drop=self.drop(p + ".biOutput.dropout1", c.v_hidden_dropout_prob), a_rg=ctx_rg)
         t1o, t1_bwd = self.dense_res_ln(ctx1, Hb, t, p + ".biOutput.dense2", p + ".biOutput.LayerNorm2", "c.t.bo",
-                                        drop=self.drop(p + ".biOutput.dropout2", c.hidden_dropout_prob))
+                                        drop=self.drop(p + ".biOutput.dropout2", c.hidden_dropout_prob), a_rg=ctx_rg)
 
         def bwd():
             if not (v1o.gw or t1o.gw):
                 return
             for a in (v1o, t1o):   # a stream without downstream gradient contributes zeros
-                if not a.gw:
+                if not a.gw and not a.frozen:
                     g = self.grad_of(a)
                     self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
                     a.gw = True
             rv, rt = v1_bwd(), t1_bwd()
+            if not ctx_rg:
+                return
             dqkv1 = self.scratch("c.dqkv1", (Mv, L3), BF16)
             dqkv2 = self.scratch("c.dqkv2", (Mt, L3), BF16)
             dctx2 = self.scratch("c.dctx2", (Mv, Hb), BF16)
@@ -821,22 +905,28 @@ class Plan:
             dyt16, dyt32 = rt
             self.gemm(Mv, Hb, Hv, dyv16, Hv, ps.w(p + ".biOutput.dense1.weight").bw, Hb, b_mn=1, out_bf16=dctx2, ld_ob=Hb)
             self.gemm(Mt, Hb, Ht, dyt16, Ht, ps.w(p + ".biOutput.dense2.weight").bw, Hb, b_mn=1, out_bf16=dctx1, ld_ob=Hb)
-            gb1, gb2 = ps.g(p + ".biattention.qkv1.bias"), ps.g(p + ".biattention.qkv2.bias")
+            gq1, gk1, gv1 = self.gparts(p + ".biattention.qkv1.bias") if need1 else (None,) * 3
+            gq2, gk2, gv2 = self.gparts(p + ".biattention.qkv2.bias") if need2 else (None,) * 3
             d1 = self.scratch("c.delta1", (B, nh, Nt), F32)
             d2 = self.scratch("c.delta2", (B, nh, Nv), F32)
+            part1 = (lambda a, b: dqkv1[:, a:b]) if need1 else (lambda a, b: None)
+            part2 = (lambda a, b: dqkv2[:, a:b]) if need2 else (lambda a, b: None)
             self.attention(True, B, nh, Nt, Nv, D, q2, L3, k1, L3, v1, L3, self.mask_v, ctx1, Hb, lse1, dO=dctx1, lddo=Hb,
-                           dQ=dqkv2[:, 0:Hb], lddq=L3, dK=dqkv1[:, Hb:2 * Hb], lddk=L3, dV=dqkv1[:, 2 * Hb:], lddv=L3, delta=d1,
-                           dbq=gb2[0:Hb], dbk=gb1[Hb:2 * Hb], dbv=gb1[2 * Hb:], dropout=adrop1)
+                           dQ=part2(0, Hb), lddq=L3, dK=part1(Hb, 2 * Hb), lddk=L3, dV=part1(2 * Hb, L3), lddv=L3, delta=d1,
+                           dbq=gq2, dbk=gk1, dbv=gv1, dropout=adrop1)
             self.attention(True, B, nh, Nv, Nt, D, q1, L3, k2, L3, v2, L3, self.mask_t, ctx2, Hb, lse2, dO=dctx2, lddo=Hb,
-                           dQ=dqkv1[:, 0:Hb], lddq=L3, dK=dqkv2[:, Hb:2 * Hb], lddk=L3, dV=dqkv2[:, 2 * Hb:], lddv=L3, delta=d2,
-                           dbq=gb1[0:Hb], dbk=gb2[Hb:2 * Hb], dbv=gb2[2 * Hb:], dropout=adrop2)
-            self.linear_wgrad(dqkv1, L3, None, 0, v.op.bw, Hv, Mv, L3, Hv, p + ".biattention.qkv1")
-            self.linear_wgrad(dqkv2, L3, None, 0, t.op.bw, Ht, Mt, L3, Ht, p + ".biattention.qkv2")
+                           dQ=part1(0, Hb), lddq=L3, dK=part2(Hb, 2 * Hb), lddk=L3, dV=part2(2 * Hb, L3), lddv=L3, delta=d2,
+                           dbq=gq1, dbk=gk2, dbv=gv2, dropout=adrop2)
+            if need1:
+                self.linear_wgrad(dqkv1, L3, None, 0, v.op.bw, Hv, Mv, L3, Hv, p + ".biattention.qkv1")
+            if need2:
+                self.linear_wgrad(dqkv2, L3, None, 0, t.op.bw, Ht, Mt, L3, Ht, p + ".biattention.qkv2")
             self.dgrad_into(v, dqkv1, L3, ps.w(p + ".biattention.qkv1.weight").bw, Mv, L3, Hv, extra32=dyv32)
             self.dgrad_into(t, dqkv2, L3, ps.w(p + ".biattention.qkv2.weight").bw, Mt, L3, Ht, extra32=dyt32)
         # the cross-modal backward touches both streams' tensors: it runs on the main stream between two barriers
         self._bwd_emitters.append(None)
-        self.push_bwd(bwd)
+        if not (v1o.frozen and t1o.frozen):
+            self.push_bwd(bwd)
         self._bwd_emitters.append(None)
         with self.on(1):
             v2o = self.ffn(v1o, c.v_intermediate_size, p + ".v_intermediate.dense", p + ".v_output.dense", p + ".v_output.LayerNorm", "c.v.ffn",
@@ -861,7 +951,9 @@ class Plan:
             m = self.mask_t.new_empty((B, self.Nt)); self._keep.append(m)
             self.emit(self.lib.vb_mask_to_additive, self.in_amask_b.data_ptr(), m.data_ptr(), B, self.Nt_in, 1 if self.has_task else 0)
         self.mask_t = m
-        return Act(f32, op, B * M1, H)
+        out = Act(f32, op, B * M1, H)
+        out.frozen = t.frozen
+        return out
 
     def expand_pairs(self, t, v):
         """in_batch_pairs (vilbert.py:1008-1040): sample p = i * b + j of the expanded batch pairs text i with image j —
@@ -882,6 +974,7 @@ class Plan:
                 else:
                     self.emit(lib.vb_broadcast_rows, src.data_ptr(), dst.data_ptr(), b * n * dst.element_size(), b)
             out = Act(f32, op, b * b * N, act.H)
+            out.frozen = act.frozen
             outs.append(out)
 
             def bwd(act=act, out=out, n=n, is_text=is_text):
@@ -895,7 +988,8 @@ class Plan:
                     self.emit(lib.vb_sum_strided, out.g32.data_ptr(), g.data_ptr(), n, b, n, b, b * n, acc)
                 act.gw = True
             self._bwd_emitters.append(None)
-            self.push_bwd(bwd)
+            if not act.frozen:
+                self.push_bwd(bwd)
             self._bwd_emitters.append(None)
         # masks: text mask rows repeated, image mask tiled (4-byte rows: plain torch-free kernels need 16-byte items -> host-side views)
         mt = self.buf((b * b, self.Nt), F32); mv = self.buf((b * b, self.Nv), F32)
@@ -923,6 +1017,7 @@ class Plan:
         p = self.buf16((B, Ht))
         self.emit(lib.vb_masked_mean_fwd, t.f32.data_ptr(), self.mask_t.data_ptr(), p32.data_ptr(), *p.ptrs(), p.fp16, B, self.Nt, Ht)
         pool = Act(p32, p, B, Ht)
+        pool.frozen = t.frozen
         mask = self.mask_t
 
         def bwd():
@@ -931,7 +1026,8 @@ class Plan:
             g = self.grad_of(t)
             self.emit(lib.vb_masked_mean_bwd, pool.g32.data_ptr(), mask.data_ptr(), g.data_ptr(), 1 if t.gw else 0, B, self.Nt, Ht)
             t.gw = True
-        self.push_bwd(bwd)
+        if not t.frozen:
+            self.push_bwd(bwd)
         return pool
 
     def image_layer(self, x, i, pool=None):
@@ -977,17 +1073,21 @@ class Plan:
         tdrop = self.drop(e + ".dropout", c.hidden_dropout_prob)
         t32, top, tmean, trstd = self.ln_fwd(xe, ps.p(e + ".LayerNorm.weight"), ps.p(e + ".LayerNorm.bias"), Mt, Ht, out_drop=tdrop)
         t = Act(t32, top, Mt, Ht)
+        tables = [e + n for n in (".word_embeddings.weight", ".position_embeddings.weight", ".token_type_embeddings.weight")]
+        tables.append(e + ".task_embeddings.weight" if self.has_task else None)
+        t.frozen = not self.trainable(e + ".LayerNorm.weight", e + ".LayerNorm.bias", *[n for n in tables if n is not None])
 
         def bwd_text():
             if t.gw:
                 dxe = self.scratch("emb.dxe", (Mt, Ht), F32)
-                self.ln_bwd(t.g32, xe, ps.p(e + ".LayerNorm.weight"), tmean, trstd, dxe, None, Mt, Ht, ps.g(e + ".LayerNorm.weight"), ps.g(e + ".LayerNorm.bias"),
-                            out_drop=tdrop)
-                self.emit(lib.vb_embed_text_bwd, dxe.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), self._ptr(self.in_task),
-                          ps.g(e + ".word_embeddings.weight").data_ptr(), ps.g(e + ".position_embeddings.weight").data_ptr(),
-                          ps.g(e + ".token_type_embeddings.weight").data_ptr(),
-                          ps.g(e + ".task_embeddings.weight").data_ptr() if self.has_task else None, B, self.Nt_in, Ht)
-        self.push_bwd(bwd_text)
+                self.ln_bwd(t.g32, xe, ps.p(e + ".LayerNorm.weight"), tmean, trstd, dxe, None, Mt, Ht, self.pg(e + ".LayerNorm.weight"),
+                            self.pg(e + ".LayerNorm.bias"), out_drop=tdrop)
+                gt = [None if n is None else self.pg(n) for n in tables]
+                if any(g is not None for g in gt):
+                    self.emit(lib.vb_embed_text_bwd, dxe.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), self._ptr(self.in_task),
+                              *[self._ptr(g) for g in gt], B, self.Nt_in, Ht)
+        if not t.frozen:
+            self.push_bwd(bwd_text)
         # image: region features fp32 -> bf16 ingest, 2048 -> Hv GEMM with the 5 -> Hv box projection as residual, LayerNorm (:1421-1432).
         # image_prefix: the same launches go to self.prefix on the main stream, and the LayerNorm's outputs (the image states the
         # forward reads) are private buffers
@@ -1010,6 +1110,8 @@ class Plan:
             self._private = False
             self.cur = self.fwd
             v = Act(v32, vop, Mv, Hv)
+            v.frozen = not self.trainable(ve + ".image_embeddings.weight", ve + ".image_embeddings.bias", ve + ".image_location_embeddings.weight",
+                                          ve + ".image_location_embeddings.bias", ve + ".LayerNorm.weight", ve + ".LayerNorm.bias")
             if self.image_prefix:
                 self.image_states = (v32, vop.hi, vop.lo, self.mask_v)
 
@@ -1017,12 +1119,14 @@ class Plan:
                 if v.gw:
                     dyv32 = self.scratch("emb.dyv32", (Mv, Hv), F32)
                     dyv16 = self.scratch("emb.dyv16", (Mv, Hv), BF16)
-                    self.ln_bwd(v.g32, yv, ps.p(ve + ".LayerNorm.weight"), vmean, vrstd, dyv32, dyv16, Mv, Hv, ps.g(ve + ".LayerNorm.weight"), ps.g(ve + ".LayerNorm.bias"),
-                                gbias=ps.g(ve + ".image_embeddings.bias"), out_drop=vdrop)
+                    self.ln_bwd(v.g32, yv, ps.p(ve + ".LayerNorm.weight"), vmean, vrstd, dyv32, dyv16, Mv, Hv, self.pg(ve + ".LayerNorm.weight"),
+                                self.pg(ve + ".LayerNorm.bias"), gbias=self.pg(ve + ".image_embeddings.bias"), out_drop=vdrop)
                     self.linear_wgrad(dyv16, Hv, None, 0, feat.bw, Fv, Mv, Hv, Fv, ve + ".image_embeddings")
-                    self.emit(lib.vb_loc_proj_bwd, dyv32.data_ptr(), self.in_loc.data_ptr(), ps.g(ve + ".image_location_embeddings.weight").data_ptr(),
-                              ps.g(ve + ".image_location_embeddings.bias").data_ptr(), Mv, Hv)
-            self.push_bwd(bwd_image)
+                    gl = (self.pg(ve + ".image_location_embeddings.weight"), self.pg(ve + ".image_location_embeddings.bias"))
+                    if gl[0] is not None or gl[1] is not None:
+                        self.emit(lib.vb_loc_proj_bwd, dyv32.data_ptr(), self.in_loc.data_ptr(), self._ptr(gl[0]), self._ptr(gl[1]), Mv, Hv)
+            if not v.frozen:
+                self.push_bwd(bwd_image)
         return t, v
 
     # ------------------------------------------------------------------ poolers and heads
@@ -1034,6 +1138,7 @@ class Plan:
         self.gemm(B, Hb, H, seq.op, N * H, ps.w(wname + ".weight"), H, bias=ps.p(wname + ".bias"), act=L.VB_ACT_RELU, out_f32=p32, ld_of=Hb,
                   out_bf16=p, ld_ob=Hb)
         pooled = Act(p32, p, B, Hb)
+        pooled.frozen = seq.frozen and not self.trainable(wname + ".weight", wname + ".bias")
 
         def bwd():
             if not pooled.gw:
@@ -1042,13 +1147,16 @@ class Plan:
             dpre32 = self.scratch("pool.dpre32", (B, Hb), F32)
             self.emit(self.lib.vb_relu_bwd, pooled.g32.data_ptr(), p32.data_ptr(), dpre.data_ptr(), dpre32.data_ptr(), B * Hb)
             self.linear_wgrad(dpre, Hb, dpre32, Hb, seq.op.bw, N * H, B, Hb, H, wname)
+            if seq.frozen:
+                return
             g = self.grad_of(seq)
             if not seq.gw:
                 self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
                 seq.gw = True
             # rows b*N of the sequence gradient += dpre @ W
             self.gemm(B, H, Hb, dpre, Hb, ps.w(wname + ".weight").bw, H, b_mn=1, residual=g, ld_res=N * H, out_f32=g, ld_of=N * H)
-        self.push_bwd(bwd)
+        if not pooled.frozen:
+            self.push_bwd(bwd)
         return pooled
 
     def out_grad_buffer(self, name, shape):
@@ -1057,18 +1165,21 @@ class Plan:
             self.gout[name] = self.buf(shape, F32, zero=True)
         return self.gout[name]
 
-    def big_head(self, name, x, ld_x, M, K_in, N_out, wname, bias_name, w=None, gw=None):
+    def big_head(self, name, x, ld_x, M, K_in, N_out, wname, bias_name, w=None, gw_name=None):
         """Wide linear head (N_out in the thousands): logits = x W^T + b as fp32 [M, N_out]; backward from a
-        caller-supplied fp32 d(logits) (cast to a bf16 operand with an 8-padded row pitch). w / gw: a weight and gradient
-        not named by `wname` (the decoder tied to the word embeddings)."""
+        caller-supplied fp32 d(logits) (cast to a bf16 operand with an 8-padded row pitch). w / gw_name: a weight and the entry of
+        its gradient not named by `wname` (the decoder tied to the word embeddings). The backward returns None when nothing
+        below the logits takes a gradient."""
         ps = self.ps
         W = w if w is not None else ps.w(wname + ".weight")
+        wkey = gw_name if gw_name is not None else wname + ".weight"
         logits = self.buf((M, N_out), F32)
         self.gemm(M, N_out, K_in, x.op, ld_x, W, K_in, bias=ps.p(bias_name), out_f32=logits, ld_of=N_out)
         self.outputs[name] = logits
+        self.out_rg[name] = not x.frozen or self.trainable(wkey, bias_name)
 
         def bwd():
-            if name not in self.grad_outputs:
+            if name not in self.grad_outputs or not self.out_rg[name]:
                 return None
             ldp = _pad8(N_out)
             if self.vqa_loss and name == "vil_prediction":
@@ -1077,9 +1188,14 @@ class Plan:
                 dl32 = self.out_grad_buffer(name, (M, N_out))
                 dl16 = self.scratch("head.dl16." + name, (M, ldp), BF16)
                 self.emit(self.lib.vb_cast2d_f32_to_bf16, dl32.data_ptr(), N_out, dl16.data_ptr(), ldp, M, N_out, 1.0)
-            self.colsum(dl32, N_out, ps.g(bias_name), M, N_out)
-            self.linear_wgrad(dl16, ldp, None, 0, x.op.bw, ld_x, M, N_out, K_in, wname, gw=gw)
-            return dl16, ldp, W.bw
+            gb = self.pg(bias_name)
+            if gb is not None:
+                self.colsum(dl32, N_out, gb, M, N_out)
+            if gw_name is None:
+                self.linear_wgrad(dl16, ldp, None, 0, x.op.bw, ld_x, M, N_out, K_in, wname)
+            elif self.trainable(gw_name):
+                self.linear_wgrad(dl16, ldp, None, 0, x.op.bw, ld_x, M, N_out, K_in, None, gw=ps.g(gw_name))
+            return None if x.frozen else (dl16, ldp, W.bw)
         return bwd
 
     def lm_head_compact(self, ht, ht_bwd):
@@ -1106,13 +1222,17 @@ class Plan:
         ldp = _pad8(V)
         self.lm_c = dict(cap=cap, idx=idx, count=cnt, labels=lab_c, logits=logits, dl32=self.buf((cap, V), F32),
                          dl16=self.buf((cap, ldp), BF16, zero=True), ldp=ldp)
+        self.out_rg["linguisic_prediction"] = not ht.frozen or self.trainable(wn, "cls.predictions.bias")
 
         def bwd():
             if "linguisic_prediction" not in self.grad_outputs:     # a forward-only plan of the forward-placed objective
                 return
             lc = self.lm_c
-            self.colsum(lc["dl32"], V, ps.g("cls.predictions.bias"), cap, V)
-            self.linear_wgrad(lc["dl16"], ldp, None, 0, hc.bw, Ht, cap, V, Ht, None, gw=ps.g(wn))
+            gb = self.pg("cls.predictions.bias")
+            if gb is not None:
+                self.colsum(lc["dl32"], V, gb, cap, V)
+            if self.trainable(wn):
+                self.linear_wgrad(lc["dl16"], ldp, None, 0, hc.bw, Ht, cap, V, Ht, None, gw=ps.g(wn))
             if ht.frozen:
                 return
             gc = self.scratch("lm.gc", (cap, Ht), F32)
@@ -1143,13 +1263,14 @@ class Plan:
                   out_pre=pre16, ld_op=Hh)
         _, h, mean, rstd = self.ln_fwd(g32, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, Hh, want_f32=False)
         hn = Act(None, h, M, Hh)
+        hn.frozen = x.frozen and not self.trainable(wdense + ".weight", wdense + ".bias", lnname + ".weight", lnname + ".bias")
 
         def bwd():
             if not hn.gw:
                 return
             dpre16 = self.scratch(tag + ".dpre16", (M, Hh), BF16)
-            self.ln_bwd(hn.g32, g32, ps.p(lnname + ".weight"), mean, rstd, None, dpre16, M, Hh, ps.g(lnname + ".weight"), ps.g(lnname + ".bias"), pre=pre16,
-                        gbias=ps.g(wdense + ".bias"))
+            self.ln_bwd(hn.g32, g32, ps.p(lnname + ".weight"), mean, rstd, None, dpre16, M, Hh, self.pg(lnname + ".weight"), self.pg(lnname + ".bias"),
+                        pre=pre16, gbias=self.pg(wdense + ".bias"))
             self.linear_wgrad(dpre16, Hh, None, 0, x.op.bw, K, M, Hh, K, wdense)
             self.dgrad_into(x, dpre16, Hh, ps.w(wdense + ".weight").bw, M, Hh, K)
         return hn, bwd
@@ -1163,17 +1284,21 @@ class Plan:
         self.emit(self.lib.vb_small_linear_fwd, xin.data_ptr(), K, ps.p(wname + ".weight").data_ptr(), ps.p(wname + ".bias").data_ptr(),
                   self._ptr(addend), y.data_ptr(), M, K, N_out, self._ref(in_drop))
         self.outputs[name] = y
+        self.out_rg[name] = not x.frozen or self.trainable(wname + ".weight", wname + ".bias")
 
         def bwd():
             if name not in self.grad_outputs:
                 return
             dy = self.out_grad_buffer(name, (M, N_out))
-            g = self.grad_of(x)
-            acc = 1 if x.gw else 0
-            x.gw = True
-            self.emit(self.lib.vb_small_linear_bwd, dy.data_ptr(), xin.data_ptr(), K, ps.p(wname + ".weight").data_ptr(), g.data_ptr(), K, acc,
-                      ps.g(wname + ".weight").data_ptr(), ps.g(wname + ".bias").data_ptr(), M, K, N_out, self._ref(in_drop))
-        self.push_bwd(bwd)
+            g, acc = None, 0
+            if not x.frozen:
+                g = self.grad_of(x)
+                acc = 1 if x.gw else 0
+                x.gw = True
+            self.emit(self.lib.vb_small_linear_bwd, dy.data_ptr(), xin.data_ptr(), K, ps.p(wname + ".weight").data_ptr(), self._ptr(g), K, acc,
+                      self._ptr(self.pg(wname + ".weight")), self._ptr(self.pg(wname + ".bias")), M, K, N_out, self._ref(in_drop))
+        if self.out_rg[name]:
+            self.push_bwd(bwd)
 
     def build_heads(self, seq_t, seq_v, pooled_t, pooled_v):
         """VILBertForVLTasks.forward after self.bert (vilbert.py:1673-1708) + BertPreTrainingHeads (:1228-1243).
@@ -1188,18 +1313,22 @@ class Plan:
             self.emit(lib.vb_fuse_pooled_fwd, pooled_t.f32.data_ptr(), pooled_v.f32.data_ptr(), f32.data_ptr(), hi, B * Hb, mul, self._ref(drop),
                       f.fp16, lo, bw)
             act = Act(f32, f, B, Hb)
+            act.frozen = pooled_t.frozen and pooled_v.frozen
 
             def fuse_bwd():
                 if not act.gw:
                     return
                 for a in (pooled_t, pooled_v):
+                    if a.frozen:
+                        continue
                     g = self.grad_of(a)
                     if not a.gw:
                         self.emit(lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
                         a.gw = True
-                self.emit(lib.vb_fuse_pooled_bwd, act.g32.data_ptr(), pooled_t.f32.data_ptr(), pooled_v.f32.data_ptr(), pooled_t.g32.data_ptr(),
-                          pooled_v.g32.data_ptr(), B * Hb, mul, self._ref(drop))
-            self.push_bwd(fuse_bwd)
+                self.emit(lib.vb_fuse_pooled_bwd, act.g32.data_ptr(), pooled_t.f32.data_ptr(), pooled_v.f32.data_ptr(), self._ptr(pooled_t.g32),
+                          self._ptr(pooled_v.g32), B * Hb, mul, self._ref(drop))
+            if not act.frozen:
+                self.push_bwd(fuse_bwd)
             return act
         # VILBertForVLTasks.dropout on the fused vector (vilbert.py:1677-1682); BertPreTrainingHeads has its own nn.Dropout(0.1)
         # on its own fused vector (:1233-1241) — a different mask, needed only where the alignment score is an output
@@ -1220,7 +1349,7 @@ class Plan:
                 r = head_bwd()
                 if r is None:
                     return
-                dl16, ldp, W16 = r
+                dl16, ldp, W16 = r        # (r is None when hn takes no gradient)
                 g = self.grad_of(hn)
                 self.gemm(hn.M, K, N_out, dl16, ldp, W16, K, b_mn=1, out_f32=g, ld_of=K)
                 hn.gw = True
@@ -1237,7 +1366,7 @@ class Plan:
                 lm_compact_bwd = self.lm_head_compact(ht, ht_bwd)
             else:
                 lm_bwd = self.big_head("linguisic_prediction", ht, Ht, B * Nt, Ht, c.vocab_size, None, "cls.predictions.bias",
-                                       w=ps.w("bert.embeddings.word_embeddings.weight"), gw=ps.g("bert.embeddings.word_embeddings.weight"))
+                                       w=ps.w("bert.embeddings.word_embeddings.weight"), gw_name="bert.embeddings.word_embeddings.weight")
         if want("vision_prediction"):
             hv, hv_bwd = self.transform(seq_v, "cls.imagePredictions.transform.dense", "cls.imagePredictions.transform.LayerNorm", "im.tr")
             im_bwd = self.big_head("vision_prediction", hv, Hv, B * Nv, Hv, c.v_target_size, "cls.imagePredictions.decoder",
@@ -1255,6 +1384,7 @@ class Plan:
         if want("vil_binary_prediction") and B % 2 == 0:
             # vil_binary_prediction pairs consecutive samples: pooled.view(-1, 2*Hb) (:1686-1689)
             pair = Act(fused.f32.view(B // 2, 2 * Hb), fused.op.view(B // 2, 2 * Hb), B // 2, 2 * Hb)
+            pair.frozen = fused.frozen
             hb, hb_bwd = self.transform(pair, "vil_binary_prediction.logit_fc.0", "vil_binary_prediction.logit_fc.2", "bin.tr")
             # LayerNorm output is needed in fp32 for the 2-way linear: recompute it from the bf16 copy is lossy, so run the small
             # linear on an fp32 LayerNorm output
@@ -1270,7 +1400,8 @@ class Plan:
                 hb_bwd()
                 if pair.gw:   # gradient landed in pair.g32 [B/2, 2Hb] == [B, Hb]
                     self.add_grad(fused, pair.g32.view(B, Hb))
-            self.push_bwd(bin_bwd)   # registered first => runs after the 2-way linear's backward
+            if not hb.frozen:
+                self.push_bwd(bin_bwd)   # registered first => runs after the 2-way linear's backward
             self.small_head("vil_binary_prediction", hb, "vil_binary_prediction.logit_fc.3", 2)
         elif want("vil_binary_prediction"):
             # odd batch: the reference returns the [B, 2] alignment output of self.cls here (:1673, 1686)
@@ -1326,7 +1457,7 @@ class Plan:
                 self._no_grad = frozen
                 t = self.text_layer(t, i)
                 self._no_grad = False
-                t.frozen = frozen
+                t.frozen = t.frozen or frozen
             pool = None
             if self.dyn and v_end > v_start:
                 # dynamic_attention: this segment's image layers read the pooled text states of the segment's END (the text layers
@@ -1339,7 +1470,7 @@ class Plan:
                     self._no_grad = frozen
                     v = self.image_layer(v, i, pool)
                     self._no_grad = False
-                    v.frozen = frozen
+                    v.frozen = v.frozen or frozen
             if count == 0 and self.fast:
                 t = self.broadcast_text(t)
             if count == 0 and self.pairs:
@@ -1365,6 +1496,8 @@ class Plan:
         self.outputs["sequence_output_v"] = v.f32.view(B, self.Nv, -1)
         self.outputs["pooled_output_t"] = self.pooled_t.f32
         self.outputs["pooled_output_v"] = self.pooled_v.f32
+        for nm, act in (("sequence_output_t", t), ("sequence_output_v", v), ("pooled_output_t", self.pooled_t), ("pooled_output_v", self.pooled_v)):
+            self.out_rg[nm] = not act.frozen
         if self.heads != "none":
             self.build_heads(t, v, self.pooled_t, self.pooled_v)
             for nm in ("vision_prediction", "vision_logit"):
@@ -2047,12 +2180,13 @@ class Engine:
         self.lm_capacity = 0.25          # ... with room for this fraction of the token rows (15 % are masked; more poisons the loss with NaN)
 
     def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-             loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False):
-        """The cached plan of this shape and these options (Plan)."""
+             loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset()):
+        """The cached plan of this shape and these options (Plan). frozen: ParamStore entry names that take no gradient."""
+        frozen = frozenset(frozen)
         loss = "vqa" if vqa_loss else loss
         pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
         key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward),
-               None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix))
+               None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix), frozen)
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]
@@ -2060,7 +2194,7 @@ class Engine:
             self.plans.popitem(last=False)
         self.plans[key] = Plan(self, B, Nt, Nv, grad_outputs, False, heads, train, loss=loss, choices=choices, score=score,
                                loss_in_forward=loss_in_forward, outputs=outputs, results=results, fast_mode=fast_mode,
-                               image_prefix=image_prefix)
+                               image_prefix=image_prefix, frozen=frozen)
         return self.plans[key]
 
     def enable_activation_arena(self, nbytes):

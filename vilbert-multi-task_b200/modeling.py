@@ -4,6 +4,7 @@ reference's constructor / forward signatures, output tuples and state_dict key n
 (engine.py -> libvilbert_b200.so). There is no PyTorch / CPU fallback: constructing a model on a
 non-CUDA device or without the built extension raises.
 """
+import operator
 import os
 
 import torch
@@ -12,12 +13,13 @@ import torch.nn.functional as F
 
 from . import _lib as L
 from .config import BertConfig
-from .engine import BERT_OUT_NAMES, HEAD_NAMES, LOSS_HEADS, Engine
+from .engine import BERT_OUT_NAMES, HEAD_NAMES, LOSS_HEADS, PRETRAINING_HEAD_NAMES, Engine
 
 
 # Any torch.optim.Optimizer.step() (pytorch_transformers.AdamW and the reference's RAdam subclass it) may have rewritten
 # parameters through p.data: bump a global epoch that every model compares with the epoch its 16-bit weight copy was made at.
 _OPT_EPOCH = [0]
+_REQUIRES_GRAD = operator.attrgetter("requires_grad")
 
 
 def _on_optimizer_step(optimizer, args, kwargs):
@@ -111,6 +113,15 @@ class _PlanCall:
         self.fwd_id = plan.fwd_id
         model._last_plan = plan
 
+    def differentiable(self):
+        """Per output of outputs(): whether a trainable parameter lies upstream of it (Plan.out_rg)."""
+        rg = self.plan.out_rg
+        if self.names is not None:
+            return tuple(rg.get(n, True) for n in self.names)
+        if self.plan.loss_kind == "pretraining":
+            return tuple(rg.get(n, True) for n in PRETRAINING_HEAD_NAMES)
+        return (rg.get(LOSS_HEADS[self.plan.loss_kind][0], True),)
+
     def outputs(self):
         plan = self.plan
         if self.names is not None:
@@ -125,7 +136,7 @@ class _PlanCall:
         if self.names is not None:
             live = tuple(n for n, g in zip(self.names, grads) if g is not None)
             if frozenset(live) != self.plan.grad_outputs:     # the plan's backward reaches other outputs: take the plan of this set
-                self.plan = model._outputs_plan(self.names, self.inputs, self.plan.train, live)
+                self.plan = model._outputs_plan(self.names, self.inputs, self.plan.train, live, self.plan.frozen)
                 self.fwd_id = None
         plan = self.plan
         now = eng.drop_step_host
@@ -160,14 +171,19 @@ class _PlanCall:
 
 class _PlanFn(torch.autograd.Function):
     """Bridges a _PlanCall into torch.autograd: forward runs the call's forward and returns its outputs, backward hands the
-    incoming gradients to the call's backward (nothing runs when none of them is live)."""
+    incoming gradients to the call's backward (nothing runs when none of them is live). An output with no trainable parameter
+    upstream (every parameter it depends on has requires_grad=False) does not require grad, as in torch."""
 
     @staticmethod
     def forward(ctx, anchor, call):
         ctx.call = call
         ctx.set_materialize_grads(False)
         call.forward()
-        return call.outputs()
+        outs = call.outputs()
+        dead = [o for o, live in zip(outs, call.differentiable()) if not live]
+        if dead:
+            ctx.mark_non_differentiable(*dead)
+        return outs
 
     @staticmethod
     def backward(ctx, *grads):
@@ -198,11 +214,14 @@ class BertPreTrainedModel(nn.Module):
             raise L.VBError("vilbert_b200 models run on sm_90a GPUs only; there is no CPU path")
         self.engine = Engine(config, dev, heads=self._heads, precision=precision)
         self._params = _register_tree(self, self.engine.ps)
+        self._pnames, self._plist = tuple(self._params), tuple(self._params.values())
+        self._frozen_flags, self._frozen_set = None, frozenset()
         self._grad_hint = {}
         self._anchor = torch.zeros((), device=dev, requires_grad=True)
         self._shadow_version = None
         self._opt_epoch = -1
         self._ddp_reducer = None
+        self._ddp_set_ranges = None     # data parallel: restricts the reducer to the trainable ranges (ddp.DistributedDataParallel)
         self.init_weights()
 
     # ---- reference init (vilbert.py:1274-1285): N(0, initializer_range) for Linear/Embedding weights, zero bias, LN 1/0
@@ -254,17 +273,38 @@ class BertPreTrainedModel(nn.Module):
         return r
 
     def zero_grad(self, set_to_none=False):
-        """Zeroes the flat gradient buffer. The Parameters' .grad stay views of it (set_to_none is accepted and ignored: the
-        engine accumulates into the flat buffer, dropping the views would only hide the gradients from the optimizer)."""
+        """Zeroes the flat gradient buffer. The trainable Parameters' .grad stay views of it (set_to_none is accepted and ignored:
+        the engine accumulates into the flat buffer, dropping the views would only hide the gradients from the optimizer); a
+        frozen Parameter's (requires_grad=False) .grad is None."""
         self.engine.zero_grad()
         self._attach_grads(zero_if_detached=False)
 
+    def _frozen(self):
+        """ParamStore entry names of the Parameters with requires_grad=False: the set every plan-backed call is specialised on.
+        Rebuilt only when a flag changed (one pass over the flags per call). A data-parallel reducer is told the new trainable
+        ranges."""
+        flags = tuple(map(_REQUIRES_GRAD, self._plist))
+        if flags != self._frozen_flags:
+            self._frozen_flags = flags
+            self._frozen_set = frozenset(n for n, f in zip(self._pnames, flags) if not f)
+            if self._ddp_set_ranges is not None:
+                self._ddp_set_ranges(self._trainable_ranges())
+        return self._frozen_set
+
+    def _trainable_ranges(self):
+        from .ddp import trainable_ranges
+        return trainable_ranges(self.engine.ps, self._frozen())
+
     def _attach_grads(self, zero_if_detached=True):
         """torch.optim.Optimizer.zero_grad() defaults to set_to_none=True and detaches every .grad from the flat buffer.
-        Before a backward the views are re-attached; if they had been dropped since the last backward the flat buffer (which
-        the engine kept accumulating into) is zeroed first, which is what the caller asked for."""
+        Before a backward the views of the trainable Parameters are re-attached; if they had been dropped since the last backward
+        the flat buffer (which the engine kept accumulating into) is zeroed first, which is what the caller asked for. Frozen
+        Parameters get .grad None (their range of the flat buffer is never written)."""
         ps = self.engine.ps
-        detached = [name for name, prm in self._params.items() if prm.grad is None]
+        frozen = self._frozen()
+        for name in frozen:
+            self._params[name].grad = None
+        detached = [name for name, prm in self._params.items() if prm.grad is None and name not in frozen]
         if not detached:
             return
         if zero_if_detached:
@@ -367,10 +407,13 @@ class BertPreTrainedModel(nn.Module):
         return (seq_t, seq_v, o["pooled_output_t"], o["pooled_output_v"], self._attention_masks(output_all_attention_masks))
 
     # ---- shared forward machinery
-    def _outputs_plan(self, names, inputs, train, live=None):
+    def _outputs_plan(self, names, inputs, train, live=None, frozen=None):
         """The plan of the outputs `names`. A plan is specialised on the set of outputs that receive a gradient; the set `live` a
         backward found is kept as the hint for the next forward of this shape, so in a steady training loop forward and backward
-        share one plan and nothing is recomputed."""
+        share one plan and nothing is recomputed. It is also specialised on the frozen parameters (default: the current
+        requires_grad flags)."""
+        if frozen is None:
+            frozen = self._frozen()
         Nt = inputs["input_txt"].shape[1]
         B, Nv = inputs["input_imgs"].shape[:2]     # FAST_MODE: the text batch is 1, the image batch sets the plan
         key = (B, Nt, Nv, names, train)
@@ -378,7 +421,7 @@ class BertPreTrainedModel(nn.Module):
             live = self._grad_hint.get(key, ())
         else:
             self._grad_hint[key] = live
-        return self.engine.plan(B, Nt, Nv, grad_outputs=live, heads=self._heads_for(names), train=train)
+        return self.engine.plan(B, Nt, Nv, grad_outputs=live, heads=self._heads_for(names), train=train, frozen=frozen)
 
     def _run(self, names, input_txt, input_imgs, image_loc, token_type_ids, attention_mask, image_attention_mask, task_ids):
         inputs = dict(input_txt=input_txt, input_imgs=input_imgs, image_loc=image_loc, token_type_ids=token_type_ids,
@@ -510,5 +553,5 @@ class BertForMultiModalPreTraining(BertPreTrainedModel):
             targets["neg_index"] = sampler(B, R, image_feat.device) if sampler is not None else self._nce_negatives(B, R, image_feat.device)
         B, Nv, Nt = image_feat.shape[0], image_feat.shape[1], input_ids.shape[1]
         plan = self.engine.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS["pretraining"] if torch.is_grad_enabled() else (), train=bool(self.training),
-                                loss="pretraining", loss_in_forward=True)
+                                loss="pretraining", loss_in_forward=True, frozen=self._frozen())
         return _PlanFn.apply(self._anchor, _PlanCall(self, plan, inputs, targets))

@@ -41,7 +41,11 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
     """What the fused optimizers share: the parameters must be views of the engine's flat fp32 buffer; the moments are two
     flat buffers of the same layout (per-parameter state entries are views of them); the work list is a chunk table over
     the trainable tensors; the hyper-parameters live in a device table (one vb_adamw_group row per param group) that is
-    re-uploaded from pinned memory when a scheduler changed it; the step counter is a device int32."""
+    re-uploaded from pinned memory when a scheduler changed it; the step counter is a device int32.
+
+    Parameters frozen (requires_grad=False) when the optimizer is built stay out of it. One frozen later is skipped from the next
+    step() on, as torch skips a parameter whose .grad is None: step() rebuilds the chunk table in place when the trainable set
+    changed. (A step already placed in a plan with Plan.enable_optimizer keeps its chunk count: enable it again after freezing.)"""
 
     def __init__(self, params, defaults, model, engine, zero_grad, chunk):
         name = type(self).__name__
@@ -64,6 +68,8 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
         self.exp_avg = torch.zeros_like(ps.flat)
         self.exp_avg_sq = torch.zeros_like(ps.flat)
         base, numel = ps.flat.data_ptr(), ps.numel
+        self._chunk = chunk
+        self._tracked = []       # (param, flat offset, numel, group index) of every parameter trainable at construction
         ranges, seen = [], set()
         for gi, group in enumerate(self.param_groups):
             for p in group["params"]:
@@ -76,6 +82,7 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
                 if (p.data_ptr() - base) % 4 or off < 0 or off + p.numel() > numel or not p.is_contiguous() or p.dtype != torch.float32:
                     raise ValueError(f"{name}: every parameter must be a contiguous fp32 view of the engine's flat buffer")
                 ranges.append((off, p.numel(), gi))
+                self._tracked.append((p, off, p.numel(), gi))
                 self.state[p] = dict(step=0, exp_avg=self.exp_avg[off:off + p.numel()].view(p.shape),
                                      exp_avg_sq=self.exp_avg_sq[off:off + p.numel()].view(p.shape))
         st, cn, gr = build_chunks(ranges, chunk)
@@ -83,6 +90,7 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
         self._chunk_start = torch.from_numpy(st).to(dev)
         self._chunk_count = torch.from_numpy(cn).to(dev)
         self._chunk_group = torch.from_numpy(gr).to(dev)
+        self._trainable_key = (True,) * len(self._tracked)
         self._groups_host = torch.zeros(len(self.param_groups) * _GROUP_DT.itemsize, dtype=torch.uint8).pin_memory() if dev.type == "cuda" else \
             torch.zeros(len(self.param_groups) * _GROUP_DT.itemsize, dtype=torch.uint8)
         self._groups_np = self._groups_host.numpy().view(_GROUP_DT)
@@ -95,6 +103,21 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
         if dev.type == "cuda":
             engine.refresh_weights()         # frozen tensors (not in any group) keep this copy; updated ones are rewritten every step
             engine.shadow_trusted = True
+
+    def _refresh_trainable(self):
+        """Drops parameters frozen since construction from the chunk table (rewritten in place, so the device pointers stay valid);
+        returns whether the table changed."""
+        key = tuple(p.requires_grad for p, _, _, _ in self._tracked)
+        if key == self._trainable_key:
+            return False
+        self._trainable_key = key
+        st, cn, gr = build_chunks([(off, n, gi) for (p, off, n, gi), rg in zip(self._tracked, key) if rg], self._chunk)
+        self.n_chunks = len(st)
+        if self.n_chunks:
+            self._chunk_start[:self.n_chunks].copy_(torch.from_numpy(st))
+            self._chunk_count[:self.n_chunks].copy_(torch.from_numpy(cn))
+            self._chunk_group[:self.n_chunks].copy_(torch.from_numpy(gr))
+        return True
 
     # ------------------------------------------------------------------ hyper-parameter table
     def _group_row(self, grp):
@@ -174,12 +197,14 @@ class FusedAdamW(_FlatBufferOptimizer):
     @torch.no_grad()
     def step(self, closure=None):
         loss = closure() if closure is not None else None
+        self._refresh_trainable()
         self.step_count += 1
         self._step_dev.add_(1)
         for st in self.state.values():
             st["step"] = self.step_count
         self._upload_groups()
-        self.launch()
+        if self.n_chunks:
+            self.launch()
         self._after_step()
         return loss
 
@@ -197,7 +222,12 @@ class FusedRAdam(_FlatBufferOptimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, model=None, engine=None, zero_grad=True,
                  chunk=32768):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), model, engine, zero_grad, chunk)
-        self.leader_group = next((gi for gi, g in enumerate(self.param_groups) if any(p in self.state for p in g["params"])), 0)
+        self._set_leader()
+
+    def _set_leader(self):
+        """The leader is the first param group holding a trainable tensor."""
+        trainable = {id(p) for (p, _, _, _), rg in zip(self._tracked, self._trainable_key) if rg}
+        self.leader_group = next((gi for gi, g in enumerate(self.param_groups) if any(id(p) in trainable for p in g["params"])), 0)
 
     def _args(self, advance_step):
         return self._buffer_args() + (self.leader_group, self._step_dev.data_ptr(), advance_step, C.c_float(self.grad_scale),
@@ -220,11 +250,16 @@ class FusedRAdam(_FlatBufferOptimizer):
     @torch.no_grad()
     def step(self, closure=None):
         loss = closure() if closure is not None else None
+        if self._refresh_trainable():
+            self._set_leader()
         self.step_count += 1
         for st in self.state.values():
             st["step"] = self.step_count
         self._upload_groups()
-        self.launch(advance_step=True)
+        if self.n_chunks:
+            self.launch(advance_step=True)
+        else:
+            self._step_dev.add_(1)
         self._after_step()
         return loss
 

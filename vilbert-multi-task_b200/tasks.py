@@ -117,7 +117,7 @@ class _Step:
                             results=kind if kind in RESULT_MODES else None)
         else:
             plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS[kind] if grad else (), train=train, loss=kind, choices=choices,
-                            score=kind not in _NO_SCORE, loss_in_forward=True)
+                            score=kind not in _NO_SCORE, loss_in_forward=True, frozen=model._frozen())
         inputs = dict(input_txt=question, input_imgs=features, image_loc=spatials, token_type_ids=segment_ids, attention_mask=input_mask,
                       image_attention_mask=image_mask, task_ids=task_tokens)
         targets = {}
