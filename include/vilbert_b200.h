@@ -446,6 +446,41 @@ vb_status vb_radam_step(float* p, float* g, float* m, float* v, void* p16, void*
                         const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step, float grad_scale,
                         int32_t zero_grad, void* stream);
 
+/* Gradient-norm clipping and non-finite step skipping for the two optimizers above: apex FusedAdam's max_grad_norm (the
+ * reference's --fp16 optimizer, train_concap.py:452-457), torch.nn.utils.clip_grad_norm_, and the step skip of
+ * torch.amp.GradScaler, decided on the device.
+ *
+ * vb_grad_norm: sum of g^2 over the chunk table in float64 (one partial per chunk into partials, double [n_chunks], then a
+ * one-CTA launch adds them in a fixed order; the result does not depend on the grid, so ranks holding bitwise-equal gradients
+ * compute bitwise-equal records), then writes *record:
+ *   norm = |grad_scale| sqrt(sum g^2)   in fp32: the norm of the gradient the update uses, before clipping
+ *   skip = 1 when the sum is not finite, i.e. some g is NaN or +-inf (a finite fp32 g cannot overflow the float64 sum)
+ *   coef = 0 when skip, else min(1, max_norm / (norm + 1e-6)) with torch.nn.utils.clip_grad_norm_'s fp32 arithmetic
+ *   skipped += skip;  *step += 1 unless skip (step may be NULL: no counter is advanced)
+ * max_norm > 0 (+inf: skip without clipping). n_chunks == 0 writes norm 0 (partials may then be NULL).
+ *
+ * vb_adamw_step_clipped / vb_radam_step_clipped: vb_adamw_step / vb_radam_step reading *record (written by vb_grad_norm
+ * earlier on the stream) after their dependency wait: the update uses g grad_scale coef; when record->skip is set p, m, v and
+ * the 16-bit copies are left untouched and g is still zeroed when zero_grad. The plain calls are the record == NULL case of the
+ * same kernels. Since vb_grad_norm advances the counter, callers pass advance_step = 0 to vb_radam_step_clipped. */
+typedef struct vb_clip_record {
+  float norm;
+  float coef;
+  int32_t skip;
+  int32_t skipped;
+} vb_clip_record;
+
+vb_status vb_grad_norm(const float* g, const int64_t* chunk_start, const int32_t* chunk_count, int32_t n_chunks, float grad_scale,
+                       float max_norm, double* partials, vb_clip_record* record, int32_t* step, void* stream);
+vb_status vb_adamw_step_clipped(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
+                                const vb_adamw_group* groups, const int32_t* step, float grad_scale, int32_t zero_grad,
+                                const vb_clip_record* record, void* stream);
+vb_status vb_radam_step_clipped(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
+                                const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step,
+                                float grad_scale, int32_t zero_grad, const vb_clip_record* record, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

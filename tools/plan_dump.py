@@ -157,6 +157,16 @@ def dump_plan(out, title, plan, opt=None):
     return n
 
 
+def dump_optimizer_plan(out, torch, O, Engine, BertConfig, tiny, prec, opt_cls, title, **opt_kw):
+    """The training plan of the tiny config with the fused optimizer `opt_cls(**opt_kw)` in its epilogue."""
+    eng = Engine(BertConfig.from_dict(tiny), "cpu", _build_only=True, precision=prec)
+    plan = eng.plan(4, NT, NV, grad_outputs=O.HEAD_NAMES, train=True)
+    params = [torch.nn.Parameter(eng.ps.p(nm)) for nm in eng.ps.entries]
+    opt = opt_cls(params, lr=1e-4, engine=eng, **opt_kw)
+    plan.enable_optimizer(opt)
+    return dump_plan(out, title, plan, opt)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("root", help="repository tree to import the package from")
@@ -186,12 +196,13 @@ def main():
                 n_ops += dump_plan(out, f"{prec} {name} arena={int(arena)}", plan)
                 n_plans += 1
         for opt_cls in (FusedAdamW, FusedRAdam):
-            eng = Engine(BertConfig.from_dict(tiny), "cpu", _build_only=True, precision=prec)
-            plan = eng.plan(4, NT, NV, grad_outputs=O.HEAD_NAMES, train=True)
-            params = [torch.nn.Parameter(eng.ps.p(nm)) for nm in eng.ps.entries]
-            opt = opt_cls(params, lr=1e-4, engine=eng)
-            plan.enable_optimizer(opt)
-            n_ops += dump_plan(out, f"{prec} {opt_cls.__name__}", plan, opt)
+            n_ops += dump_optimizer_plan(out, torch, O, Engine, BertConfig, tiny, prec, opt_cls, f"{prec} {opt_cls.__name__}")
+            n_plans += 1
+    # gradient-norm clipping: listed after the matrix above, so that the listing of a tree without it is a prefix of this one
+    for prec in PRECISIONS:
+        for opt_cls in (FusedAdamW, FusedRAdam):
+            n_ops += dump_optimizer_plan(out, torch, O, Engine, BertConfig, tiny, prec, opt_cls, f"{prec} {opt_cls.__name__} max_grad_norm=1.0",
+                                         max_grad_norm=1.0)
             n_plans += 1
     text = "\n".join(out) + "\n"
     if a.out:

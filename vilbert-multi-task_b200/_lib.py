@@ -121,6 +121,9 @@ _SIGNATURES = {
     "vb_scatter_rows_f32": [_P, _P, _P, _I32, _I32, _P, _P, _P],
     "vb_adamw_step": [_P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _P, _F, _I32, _P],
     "vb_radam_step": [_P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _I32, _P, _I32, _F, _I32, _P],
+    "vb_grad_norm": [_P, _P, _P, _I32, _F, _F, _P, _P, _P, _P],
+    "vb_adamw_step_clipped": [_P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _P, _F, _I32, _P, _P],
+    "vb_radam_step_clipped": [_P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _I32, _P, _I32, _F, _I32, _P, _P],
 }
 
 _lib = None

@@ -51,13 +51,119 @@ __device__ __forceinline__ void store_copies1(uint16_t* __restrict__ p16, uint16
   if (p16_b) p16_b[e] = __float2bfloat16(pv);
 }
 
+// Sum over the CTA in a fixed order (warp trees, then the warp sums in warp order); valid in thread 0. Ends with a barrier so
+// that `red` may be reused by the next call.
+__device__ __forceinline__ double block_sum_f64(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    v = threadIdx.x < OPT_THREADS / 32 ? red[threadIdx.x] : 0.0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  }
+  __syncthreads();
+  return v;
+}
+
+__device__ __forceinline__ double add_squares4(double acc, float4 x) {
+  acc = fma((double)x.x, (double)x.x, acc); acc = fma((double)x.y, (double)x.y, acc);
+  acc = fma((double)x.z, (double)x.z, acc); return fma((double)x.w, (double)x.w, acc);
+}
+
+// Gradient norm for clipping and non-finite step skipping, pass 1: partials[c] = sum of g^2 over chunk c in float64. One CTA
+// reduces a whole chunk in a fixed thread order, so each partial, and the norm the finalize forms from them, is bitwise the same
+// whatever the grid size. The square of an fp32 value is exact in float64 and 2^28 of them cannot overflow it: the sum is
+// finite unless some gradient element is NaN or +-inf. 4 B of HBM traffic per element, four 128-bit loads in flight per thread.
+__global__ void __launch_bounds__(OPT_THREADS)
+grad_sq_partials_kernel(const float* __restrict__ g, const long long* __restrict__ chunk_start, const int* __restrict__ chunk_count,
+                        int n_chunks, double* __restrict__ partials) {
+  __shared__ double red[OPT_THREADS / 32];
+  pdl_entry();
+  for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
+    const long long s0 = chunk_start[c];
+    const int n = chunk_count[c];
+    const int n4 = n >> 2;
+    const float4* g4 = reinterpret_cast<const float4*>(g + s0);
+    double acc = 0.0;
+    for (int i0 = threadIdx.x; i0 < n4; i0 += 4 * OPT_THREADS) {
+      float4 x[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int i = i0 + u * OPT_THREADS;
+        x[u] = i < n4 ? g4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) acc = add_squares4(acc, x[u]);
+    }
+    for (int i = (n4 << 2) + threadIdx.x; i < n; i += OPT_THREADS) {
+      const double x = g[s0 + i];
+      acc = fma(x, x, acc);
+    }
+    acc = block_sum_f64(acc, red);
+    if (threadIdx.x == 0) partials[c] = acc;
+  }
+}
+
+// Pass 2 (one CTA): adds the partials in a fixed order and writes the record the clipped optimizer launches read. The clip
+// coefficient is torch.nn.utils.clip_grad_norm_'s fp32 arithmetic, clamp(max_norm * reciprocal(norm + 1e-6), max=1) (torch
+// evaluates `max_norm / tensor` as reciprocal times max_norm), with IEEE rounding whatever the fast-math flags.
+__global__ void __launch_bounds__(OPT_THREADS)
+grad_norm_finalize_kernel(const double* __restrict__ partials, int n_chunks, float grad_scale, float max_norm,
+                          vb_clip_record* __restrict__ rec, int* __restrict__ step) {
+  __shared__ double red[OPT_THREADS / 32];
+  pdl_entry();
+  double s = 0.0;
+  for (int c = threadIdx.x; c < n_chunks; c += OPT_THREADS) s += partials[c];
+  s = block_sum_f64(s, red);
+  if (threadIdx.x == 0) {
+    const int skip = isfinite(s) ? 0 : 1;
+    const float norm = (float)(fabs((double)grad_scale) * sqrt(s));
+    rec->norm = norm;
+    rec->coef = skip ? 0.f : fminf(__fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), max_norm), 1.f);
+    rec->skip = skip;
+    rec->skipped += skip;
+    if (step && !skip) *step += 1;
+  }
+}
+
+// What a skipped step still does: zero the gradient over the chunk table (keeps the caller's "gradient is clean" bookkeeping).
+__device__ void zero_chunks(float* __restrict__ g, const long long* __restrict__ chunk_start, const int* __restrict__ chunk_count,
+                            int n_chunks) {
+  for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
+    const long long s0 = chunk_start[c];
+    const int n = chunk_count[c];
+    const int n4 = n >> 2;
+    float4* g4 = reinterpret_cast<float4*>(g + s0);
+    for (int i = threadIdx.x; i < n4; i += OPT_THREADS) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = (n4 << 2) + threadIdx.x; i < n; i += OPT_THREADS) g[s0 + i] = 0.f;
+  }
+}
+
+// The effective gradient multiplier of an optimizer launch: grad_scale, times the clip coefficient when a record is given.
+// Returns false when the record says to skip the step (the caller then only zeroes the gradient).
+__device__ __forceinline__ bool step_scale(const vb_clip_record* __restrict__ rec, float grad_scale, float& gs) {
+  gs = grad_scale;
+  if (!rec) return true;
+  if (rec->skip) return false;
+  gs = grad_scale * rec->coef;
+  return true;
+}
+
 __global__ void __launch_bounds__(OPT_THREADS)
 adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
              uint16_t* __restrict__ p16, uint16_t* __restrict__ p16_lo, __nv_bfloat16* __restrict__ p16_b, int fp16,
              const long long* __restrict__ chunk_start,
              const int* __restrict__ chunk_count, const int* __restrict__ chunk_group, int n_chunks,
-             const vb_adamw_group* __restrict__ groups, const int* __restrict__ step, float grad_scale, int zero_grad) {
+             const vb_adamw_group* __restrict__ groups, const int* __restrict__ step, float grad_scale, int zero_grad,
+             const vb_clip_record* __restrict__ rec) {
   pdl_entry();
+  float gs;
+  if (!step_scale(rec, grad_scale, gs)) {
+    if (zero_grad) zero_chunks(g, chunk_start, chunk_count, n_chunks);
+    return;
+  }
   const int t = step ? *step : 1;
   for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
     const long long s0 = chunk_start[c];
@@ -68,7 +174,7 @@ adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
     const float decay = 1.f - G.lr * G.weight_decay;   // p <- p - lr wd p  (weight_decay > 0 only)
     const float ob1 = 1.f - G.beta1, ob2 = 1.f - G.beta2;
     auto upd = [&](float pv, float gv, float& mv, float& vv) -> float {
-      gv *= grad_scale;
+      gv *= gs;
       mv = G.beta1 * mv + ob1 * gv;
       vv = G.beta2 * vv + ob2 * gv * gv;
       pv = pv - step_size * (mv / (sqrtf(vv) + G.eps));
@@ -115,10 +221,15 @@ radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
              uint16_t* __restrict__ p16, uint16_t* __restrict__ p16_lo, __nv_bfloat16* __restrict__ p16_b, int fp16,
              const long long* __restrict__ chunk_start, const int* __restrict__ chunk_count, const int* __restrict__ chunk_group,
              int n_chunks, const vb_adamw_group* __restrict__ groups, int leader, const int* __restrict__ step, float grad_scale,
-             int zero_grad) {
+             int zero_grad, const vb_clip_record* __restrict__ rec) {
   __shared__ float s_step_size;
   __shared__ int s_rect;
   pdl_entry();
+  float gs;
+  if (!step_scale(rec, grad_scale, gs)) {   // uniform over the CTA: no thread reaches the barrier below
+    if (zero_grad) zero_chunks(g, chunk_start, chunk_count, n_chunks);
+    return;
+  }
   if (threadIdx.x == 0) {
     const vb_adamw_group L = groups[leader];
     const double t = (double)max(*step, 1);   // the counter is advanced before the first step; 0 would divide by zero
@@ -142,7 +253,7 @@ radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
     const float decay = G.weight_decay * G.lr;
     const float ob1 = 1.f - G.beta1, ob2 = 1.f - G.beta2;
     auto upd = [&](float pv, float gv, float& mv, float& vv) -> float {
-      gv *= grad_scale;
+      gv *= gs;
       vv = G.beta2 * vv + ob2 * gv * gv;
       mv = G.beta1 * mv + ob1 * gv;
       if (G.weight_decay != 0.f) pv = pv - decay * pv;
@@ -186,44 +297,97 @@ static bool opt_buffers_aligned(const void* p, const void* g, const void* m, con
   return al(p, 16) && al(g, 16) && al(m, 16) && al(v, 16) && (!p16 || al(p16, 8)) && (!p16_lo || (al(p16_lo, 8) && p16)) && al(p16_b, 8);
 }
 
-}  // namespace vb
-
-extern "C" vb_status vb_adamw_step(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
-                                   const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
-                                   const vb_adamw_group* groups, const int32_t* step, float grad_scale, int32_t zero_grad, void* stream) {
-  using namespace vb;
+// The two step calls share their launch code with their clipped variants; rec == NULL is the plain step.
+static vb_status adamw_launch(const char* name, float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b,
+                              int32_t p16_fp16, const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
+                              int32_t n_chunks, const vb_adamw_group* groups, const int32_t* step, float grad_scale, int32_t zero_grad,
+                              const vb_clip_record* rec, void* stream) {
   if (n_chunks <= 0) return VB_OK;
   if (!p || !g || !m || !v || !chunk_start || !chunk_count || !chunk_group || !groups)
-    return set_error(VB_ERR_INVALID, "vb_adamw_step: null argument");
+    return set_error(VB_ERR_INVALID, "%s: null argument", name);
   if (!opt_buffers_aligned(p, g, m, v, p16, p16_lo, p16_b))
-    return set_error(VB_ERR_INVALID, "vb_adamw_step: buffers must be 16-byte aligned (16-bit copies 8-byte)");
+    return set_error(VB_ERR_INVALID, "%s: buffers must be 16-byte aligned (16-bit copies 8-byte)", name);
   cudaError_t e = launch_pdl(adamw_kernel, dim3(opt_grid(n_chunks)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
                              static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),
                              reinterpret_cast<const long long*>(chunk_start), chunk_count, chunk_group, (int)n_chunks, groups, step,
-                             grad_scale, (int)(zero_grad ? 1 : 0));
-  if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_adamw_step: %s", cudaGetErrorString(e));
+                             grad_scale, (int)(zero_grad ? 1 : 0), rec);
+  if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "%s: %s", name, cudaGetErrorString(e));
   return VB_OK;
 }
 
-extern "C" vb_status vb_radam_step(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
-                                   const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
-                                   const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step, float grad_scale,
-                                   int32_t zero_grad, void* stream) {
-  using namespace vb;
-  if (!step || leader_group < 0) return set_error(VB_ERR_INVALID, "vb_radam_step: null step counter or negative leader group");
+static vb_status radam_launch(const char* name, float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b,
+                              int32_t p16_fp16, const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
+                              int32_t n_chunks, const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step,
+                              float grad_scale, int32_t zero_grad, const vb_clip_record* rec, void* stream) {
+  if (!step || leader_group < 0) return set_error(VB_ERR_INVALID, "%s: null step counter or negative leader group", name);
   if (advance_step) {
     const vb_status st = vb_step_counter_bump(reinterpret_cast<uint32_t*>(step), stream);
     if (st != VB_OK) return st;
   }
   if (n_chunks <= 0) return VB_OK;
   if (!p || !g || !m || !v || !chunk_start || !chunk_count || !chunk_group || !groups)
-    return set_error(VB_ERR_INVALID, "vb_radam_step: null argument");
+    return set_error(VB_ERR_INVALID, "%s: null argument", name);
   if (!opt_buffers_aligned(p, g, m, v, p16, p16_lo, p16_b))
-    return set_error(VB_ERR_INVALID, "vb_radam_step: buffers must be 16-byte aligned (16-bit copies 8-byte)");
+    return set_error(VB_ERR_INVALID, "%s: buffers must be 16-byte aligned (16-bit copies 8-byte)", name);
   cudaError_t e = launch_pdl(radam_kernel, dim3(opt_grid(n_chunks)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
                              static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),
                              reinterpret_cast<const long long*>(chunk_start), chunk_count, chunk_group, (int)n_chunks, groups, (int)leader_group,
-                             static_cast<const int*>(step), grad_scale, (int)(zero_grad ? 1 : 0));
-  if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_radam_step: %s", cudaGetErrorString(e));
+                             static_cast<const int*>(step), grad_scale, (int)(zero_grad ? 1 : 0), rec);
+  if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "%s: %s", name, cudaGetErrorString(e));
   return VB_OK;
+}
+
+}  // namespace vb
+
+extern "C" vb_status vb_adamw_step(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                   const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
+                                   const vb_adamw_group* groups, const int32_t* step, float grad_scale, int32_t zero_grad, void* stream) {
+  return vb::adamw_launch("vb_adamw_step", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group, n_chunks,
+                          groups, step, grad_scale, zero_grad, nullptr, stream);
+}
+
+extern "C" vb_status vb_radam_step(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                   const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
+                                   const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step, float grad_scale,
+                                   int32_t zero_grad, void* stream) {
+  return vb::radam_launch("vb_radam_step", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group, n_chunks,
+                          groups, leader_group, step, advance_step, grad_scale, zero_grad, nullptr, stream);
+}
+
+extern "C" vb_status vb_grad_norm(const float* g, const int64_t* chunk_start, const int32_t* chunk_count, int32_t n_chunks, float grad_scale,
+                                  float max_norm, double* partials, vb_clip_record* record, int32_t* step, void* stream) {
+  using namespace vb;
+  if (!record) return set_error(VB_ERR_INVALID, "vb_grad_norm: null record");
+  if (!(max_norm > 0.f)) return set_error(VB_ERR_INVALID, "vb_grad_norm: max_norm must be > 0 (inf: skip without clipping)");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (n_chunks > 0) {
+    if (!g || !chunk_start || !chunk_count || !partials) return set_error(VB_ERR_INVALID, "vb_grad_norm: null argument");
+    if (reinterpret_cast<uintptr_t>(g) % 16) return set_error(VB_ERR_INVALID, "vb_grad_norm: g must be 16-byte aligned");
+    cudaError_t e = launch_pdl(grad_sq_partials_kernel, dim3(opt_grid(n_chunks)), dim3(OPT_THREADS), (size_t)0, st, g,
+                               reinterpret_cast<const long long*>(chunk_start), chunk_count, (int)n_chunks, partials);
+    if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_grad_norm: %s", cudaGetErrorString(e));
+  }
+  cudaError_t e = launch_pdl(grad_norm_finalize_kernel, dim3(1), dim3(OPT_THREADS), (size_t)0, st, (const double*)partials,
+                             (int)(n_chunks > 0 ? n_chunks : 0), grad_scale, max_norm, record, static_cast<int*>(step));
+  if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_grad_norm: %s", cudaGetErrorString(e));
+  return VB_OK;
+}
+
+extern "C" vb_status vb_adamw_step_clipped(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                           const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
+                                           int32_t n_chunks, const vb_adamw_group* groups, const int32_t* step, float grad_scale,
+                                           int32_t zero_grad, const vb_clip_record* record, void* stream) {
+  if (!record) return vb::set_error(VB_ERR_INVALID, "vb_adamw_step_clipped: null record");
+  return vb::adamw_launch("vb_adamw_step_clipped", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group,
+                          n_chunks, groups, step, grad_scale, zero_grad, record, stream);
+}
+
+extern "C" vb_status vb_radam_step_clipped(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                           const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
+                                           int32_t n_chunks, const vb_adamw_group* groups, int32_t leader_group, int32_t* step,
+                                           int32_t advance_step, float grad_scale, int32_t zero_grad, const vb_clip_record* record,
+                                           void* stream) {
+  if (!record) return vb::set_error(VB_ERR_INVALID, "vb_radam_step_clipped: null record");
+  return vb::radam_launch("vb_radam_step_clipped", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group,
+                          n_chunks, groups, leader_group, step, advance_step, grad_scale, zero_grad, record, stream);
 }

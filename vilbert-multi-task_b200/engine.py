@@ -1929,12 +1929,12 @@ class Plan:
         """Training step with the fused optimizer (optim.FusedAdamW): the step body becomes [dropout step bump] + forward + loss +
         backward + ONE AdamW launch that also rewrites the 16-bit weight copy and zeroes the gradients — no weight cast and no
         gradient memset in the step. (The host-side lr table of `opt` is refreshed by opt.step(); here the launch alone is
-        replayed, e.g. inside the step graph, with the table currently on the device.)"""
+        replayed, e.g. inside the step graph, with the table currently on the device.) With `max_grad_norm` the gradient-norm
+        launch precedes it, so every replay clips and skips a non-finite step on the device."""
         self.prologue = []
         if self.train and dropout_bump:
             self.prologue.append((self.lib.vb_step_counter_bump, (self.e.drop_step.data_ptr(),), 0))
-        fn, args = opt.op()
-        self.epilogue = [(fn, args, 0)]
+        self.epilogue = [(fn, args, 0) for fn, args in opt.ops()]
         self.graph_step = None
 
     @property
@@ -2059,7 +2059,8 @@ class Plan:
         each finished gradient range captured on a communication stream inside the same graph (NCCL collectives are capturable),
         forked after its piece and joined at the end. Compared with capture_segments / run_step_overlapped there is a single
         graph launch per step and no host-side event bookkeeping between pieces. `allreduce_range(lo, hi)` must enqueue the
-        collective on the current stream (async_op=False semantics)."""
+        collective on the current stream (async_op=False semantics). The epilogue (enable_optimizer) runs after the
+        communication stream has joined, so a clipping optimizer takes the norm of the averaged gradient."""
         self.segments = self.ddp_segments(n_segments, tail_cut=tail_cut)
         torch.cuda.synchronize()
         barrier = [(None, ("all",), 0)]
@@ -2093,7 +2094,9 @@ class Plan:
         """Replays the segment graphs; after each one the finished tail range of the flat gradient buffer is handed to
         `allreduce_range(lo, hi)` (issued under `comm_stream`, which first waits for that segment) so the collective
         overlaps the rest of the backward. Ranges no backward op of this plan writes (live_ranges) are not exchanged.
-        Returns the list of whatever allreduce_range returned (async work handles)."""
+        Returns the list of whatever allreduce_range returned (async work handles). No epilogue runs here: a caller that
+        launches the optimizer afterwards must first wait for these collectives, and with max_grad_norm so must the gradient
+        norm, which is to be taken of the averaged gradient."""
         self.fwd_id += 1
         self.e.grad_clean = False
         main = torch.cuda.current_stream()

@@ -13,6 +13,11 @@ weight_decay in the reference; the warm-up schedulers of train_tasks.py:431-437 
 step() is ONE kernel launch over the flat buffers (csrc/vb_optim.cu) that also writes the 16-bit tensor-core operand copy
 of the updated weights and zeroes the gradients, so the training step needs no separate weight cast and the
 `model.zero_grad()` that follows optimizer.step() in the reference (train_tasks.py:551) finds the buffer already clean.
+
+`max_grad_norm=c` (apex FusedAdam's keyword, passed by the reference's --fp16 optimizer, train_concap.py:452-457) clips the
+global L2 norm of the trainable gradients to c as torch.nn.utils.clip_grad_norm_ does, and skips a step whose gradient holds a
+NaN or an inf, both decided on the device: one norm launch over the gradient buffer writes a small record that the optimizer
+launch reads, so nothing is read back to the host.
 """
 import ctypes as C
 
@@ -47,7 +52,7 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
     step() on, as torch skips a parameter whose .grad is None: step() rebuilds the chunk table in place when the trainable set
     changed. (A step already placed in a plan with Plan.enable_optimizer keeps its chunk count: enable it again after freezing.)"""
 
-    def __init__(self, params, defaults, model, engine, zero_grad, chunk):
+    def __init__(self, params, defaults, model, engine, zero_grad, chunk, max_grad_norm):
         name = type(self).__name__
         if engine is None:
             if model is None:
@@ -60,6 +65,11 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
             raise ValueError("Invalid beta parameters: {} - should be in [0.0, 1.0[".format(betas))
         if not 0.0 <= defaults["eps"]:
             raise ValueError("Invalid epsilon value: {} - should be >= 0.0".format(defaults["eps"]))
+        if max_grad_norm is not None:
+            max_grad_norm = float(max_grad_norm)
+            if not max_grad_norm > 0.0:      # also false for NaN
+                raise ValueError(f"Invalid max_grad_norm: {max_grad_norm} - should be > 0.0 (float('inf'): skip non-finite steps "
+                                 "without clipping)")
         super().__init__(params, defaults)
         self.engine = engine
         self.fused_zero_grad = bool(zero_grad)
@@ -99,6 +109,15 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
         self._step_dev = torch.zeros(1, dtype=torch.int32, device=dev)
         self.step_count = 0
         self.grad_scale = 1.0
+        self.max_grad_norm = max_grad_norm
+        self.grad_norm = self.skipped_steps = None
+        if max_grad_norm is not None:
+            # vb_clip_record {norm f32, coef f32, skip i32, skipped i32}; the partials table keeps its size when frozen parameters
+            # shrink the chunk table
+            self._clip_record = torch.zeros(4, dtype=torch.int32, device=dev)
+            self._norm_partials = torch.zeros(max(self.n_chunks, 1), dtype=torch.float64, device=dev)
+            self.grad_norm = self._clip_record.view(torch.float32)[0]
+            self.skipped_steps = self._clip_record[3]
         self._upload_groups()
         if dev.type == "cuda":
             engine.refresh_weights()         # frozen tensors (not in any group) keep this copy; updated ones are rewritten every step
@@ -140,6 +159,26 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
                 ps.shadows.fp16, self._chunk_start.data_ptr(), self._chunk_count.data_ptr(), self._chunk_group.data_ptr(), self.n_chunks,
                 self._groups_dev.data_ptr())
 
+    def _norm_op(self, step_ptr):
+        """(fn, args) of vb_grad_norm over the chunk table; it advances the counter at step_ptr (None: none) unless it skips."""
+        return (L.lib().vb_grad_norm, (self.engine.ps.grad.data_ptr(), self._chunk_start.data_ptr(), self._chunk_count.data_ptr(),
+                                       self.n_chunks, C.c_float(self.grad_scale), C.c_float(self.max_grad_norm),
+                                       self._norm_partials.data_ptr(), self._clip_record.data_ptr(), step_ptr))
+
+    def op(self):
+        """(fn, args) of the step launch for an engine op list when max_grad_norm is None (the step is then one operation)."""
+        ops = self.ops()
+        if len(ops) != 1:
+            raise ValueError(f"{type(self).__name__} with max_grad_norm is two operations (gradient norm, step): use ops()")
+        return ops[0]
+
+    @staticmethod
+    def _run(ops, stream):
+        if stream is None:
+            stream = torch.cuda.current_stream().cuda_stream
+        for fn, args in ops:
+            L.check(fn(*args, stream), fn.__name__)
+
     def _after_step(self):
         eng = self.engine
         eng.shadow_clean = True
@@ -170,40 +209,50 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
                     g_old[k] = v
         self._upload_groups()
 
+    def state_dict(self):
+        """The per-parameter "step" is the device counter's value: replays of a captured step advance it without the host
+        knowing, and with max_grad_norm only the device knows which steps were skipped."""
+        self.step_count = int(self._step_dev.item())
+        for st in self.state.values():
+            st["step"] = self.step_count
+        return super().state_dict()
+
 
 class FusedAdamW(_FlatBufferOptimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0, correct_bias=True, model=None, engine=None,
-                 zero_grad=True, chunk=32768):
+                 zero_grad=True, chunk=32768, max_grad_norm=None):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, correct_bias=correct_bias),
-                         model, engine, zero_grad, chunk)
+                         model, engine, zero_grad, chunk, max_grad_norm)
 
     def _group_row(self, grp):
         return super()._group_row(grp)[:5] + (1 if grp["correct_bias"] else 0,)
 
     # ------------------------------------------------------------------ stepping
     def launch(self, stream=None):
-        """The kernel launch alone (capturable in a CUDA graph): uses the hyper-parameter table and step counter currently on the
-        device. `step()` = advance the counter + refresh the table + launch."""
-        if stream is None:
-            stream = torch.cuda.current_stream().cuda_stream
-        L.check(L.lib().vb_adamw_step(*self._buffer_args(), self._step_dev.data_ptr(), C.c_float(self.grad_scale),
-                                      1 if self.fused_zero_grad else 0, stream), "vb_adamw_step")
+        """The kernel launches alone (capturable in a CUDA graph): use the hyper-parameter table and step counter currently on the
+        device. `step()` = advance the counter + refresh the table + launch. With max_grad_norm the gradient norm comes first and
+        advances the device counter itself, unless the step is skipped."""
+        self._run(self.ops(), stream)
 
-    def op(self):
-        """(fn, args) for an engine op list (Plan.epilogue): the launch as a plan operation."""
-        return (L.lib().vb_adamw_step, self._buffer_args() + (self._step_dev.data_ptr(), C.c_float(self.grad_scale),
-                                                              1 if self.fused_zero_grad else 0))
+    def ops(self):
+        """[(fn, args)] of one step for an engine op list (Plan.epilogue): the step launch, preceded by the gradient norm when
+        max_grad_norm is set."""
+        args = self._buffer_args() + (self._step_dev.data_ptr(), C.c_float(self.grad_scale), 1 if self.fused_zero_grad else 0)
+        if self.max_grad_norm is None:
+            return [(L.lib().vb_adamw_step, args)]
+        return [self._norm_op(self._step_dev.data_ptr()), (L.lib().vb_adamw_step_clipped, args + (self._clip_record.data_ptr(),))]
 
     @torch.no_grad()
     def step(self, closure=None):
         loss = closure() if closure is not None else None
         self._refresh_trainable()
-        self.step_count += 1
-        self._step_dev.add_(1)
-        for st in self.state.values():
-            st["step"] = self.step_count
+        if self.max_grad_norm is None:
+            self.step_count += 1
+            self._step_dev.add_(1)
+            for st in self.state.values():
+                st["step"] = self.step_count
         self._upload_groups()
-        if self.n_chunks:
+        if self.n_chunks or self.max_grad_norm is not None:
             self.launch()
         self._after_step()
         return loss
@@ -220,8 +269,9 @@ class FusedRAdam(_FlatBufferOptimizer):
     embeddings' at base_lr, so the vil_* heads' lr of 1e-4 does not reach their RAdam update."""
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, model=None, engine=None, zero_grad=True,
-                 chunk=32768):
-        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), model, engine, zero_grad, chunk)
+                 chunk=32768, max_grad_norm=None):
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), model, engine, zero_grad, chunk,
+                         max_grad_norm)
         self._set_leader()
 
     def _set_leader(self):
@@ -235,38 +285,33 @@ class FusedRAdam(_FlatBufferOptimizer):
 
     # ------------------------------------------------------------------ stepping
     def launch(self, stream=None, advance_step=False):
-        """The kernel launch alone (capturable in a CUDA graph): uses the hyper-parameter table currently on the device, and the
-        device step counter, first advanced by one on the same stream when `advance_step`. `step()` = refresh the table +
-        launch(advance_step=True)."""
-        if stream is None:
-            stream = torch.cuda.current_stream().cuda_stream
-        L.check(L.lib().vb_radam_step(*self._args(1 if advance_step else 0), stream), "vb_radam_step")
+        """The kernel launches alone (capturable in a CUDA graph): use the hyper-parameter table currently on the device, and the
+        device step counter, first advanced by one on the same stream when `advance_step` (with max_grad_norm: by the gradient
+        norm, unless the step is skipped). `step()` = refresh the table + launch(advance_step=True)."""
+        self._run(self.ops(advance_step), stream)
 
-    def op(self):
-        """(fn, args) for an engine op list (Plan.epilogue): advance the step counter + the launch, as one plan operation, so
-        every replay of a captured step moves one step along the rectification schedule."""
-        return (L.lib().vb_radam_step, self._args(1))
+    def ops(self, advance_step=True):
+        """[(fn, args)] of one step for an engine op list (Plan.epilogue): the step launch, preceded by the gradient norm when
+        max_grad_norm is set. Advancing the step counter is part of the step, so every replay of a captured step moves one step
+        along the rectification schedule."""
+        if self.max_grad_norm is None:
+            return [(L.lib().vb_radam_step, self._args(1 if advance_step else 0))]
+        return [self._norm_op(self._step_dev.data_ptr() if advance_step else None),
+                (L.lib().vb_radam_step_clipped, self._args(0) + (self._clip_record.data_ptr(),))]
 
     @torch.no_grad()
     def step(self, closure=None):
         loss = closure() if closure is not None else None
         if self._refresh_trainable():
             self._set_leader()
-        self.step_count += 1
-        for st in self.state.values():
-            st["step"] = self.step_count
+        if self.max_grad_norm is None:
+            self.step_count += 1
+            for st in self.state.values():
+                st["step"] = self.step_count
         self._upload_groups()
-        if self.n_chunks:
+        if self.n_chunks or self.max_grad_norm is not None:
             self.launch(advance_step=True)
         else:
             self._step_dev.add_(1)
         self._after_step()
         return loss
-
-    def state_dict(self):
-        """The per-parameter "step" is the device counter's value: replays of a captured step advance it without the host
-        knowing."""
-        self.step_count = int(self._step_dev.item())
-        for st in self.state.values():
-            st["step"] = self.step_count
-        return super().state_dict()
