@@ -481,6 +481,43 @@ vb_status vb_radam_step_clipped(float* p, float* g, float* m, float* v, void* p1
                                 const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step,
                                 float grad_scale, int32_t zero_grad, const vb_clip_record* record, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Single-stream baseline (BaseBertForVLTasks, vilbert/basebert.py:893-978).
+ *
+ * vb_concat_embed_ln_fwd: the text rows xt [B*Nt, H] (word + position + type, vb_embed_text_fwd) and the image rows xv [B*Nv, H]
+ * (region GEMM + box projection) plus v_type_row (row 1 of the image token-type table) go through their own LayerNorm
+ * (gamma_t / beta_t, gamma_v / beta_v) and dropout (index = row within the modality * H + col), written interleaved as the stream
+ * [B, Nt+Nv, H]: y_f32 and the operand copies (y16 in the y_fp16 format, y_lo its split-precision low part, y_b16 bf16; each may be
+ * NULL), with the row statistics mean / rstd [B*(Nt+Nv)].
+ * vb_concat_embed_ln_bwd: dy [B*(Nt+Nv), H] -> dxt [B*Nt, H] (f32), dxv [B*Nv, H] (f32) and dxv_bf16; ACCUMULATES dgamma / dbeta of
+ * both LayerNorms and the image column sum of dx into dcol_v and dcol_v2 (the region GEMM's bias and image token-type row 1). Every
+ * output may be NULL. H <= 2048. */
+vb_status vb_concat_embed_ln_fwd(const float* xt, const float* xv, const float* v_type_row, const float* gamma_t, const float* beta_t,
+                                 const float* gamma_v, const float* beta_v, float* y_f32, void* y16, void* y_lo, void* y_b16, int32_t y_fp16,
+                                 float* mean, float* rstd, int32_t B, int32_t Nt, int32_t Nv, int32_t H, const vb_dropout* drop_t,
+                                 const vb_dropout* drop_v, void* stream);
+vb_status vb_concat_embed_ln_bwd(const float* dy, const float* xt, const float* xv, const float* v_type_row, const float* gamma_t,
+                                 const float* gamma_v, const float* mean, const float* rstd, float* dxt, float* dxv, void* dxv_bf16,
+                                 float* dgamma_t, float* dbeta_t, float* dgamma_v, float* dbeta_v, float* dcol_v, float* dcol_v2,
+                                 int32_t B, int32_t Nt, int32_t Nv, int32_t H, const vb_dropout* drop_t, const vb_dropout* drop_v, void* stream);
+/* Scatter-add of d(text embeddings) [B*Nt, H] into word / position / token-type tables that all have padding_idx = 0: row 0 of
+ * each receives nothing (basebert.py:290-298). Any table may be NULL. */
+vb_status vb_embed_text_bwd_padded(const float* dout, const int64_t* ids, const int64_t* token_type_ids, float* dword, float* dpos,
+                                   float* dtype, int32_t B, int32_t Nt, int32_t H, void* stream);
+/* weight_norm(dim=None) (SimpleClassifier, basebert.py:965-978): w = v * (g / ||v||_F), g a scalar, written as w_f32 and the
+ * operand copies (each may be NULL). Backward: dg += <dw, v> / ||v||, dv += (g / ||v||)(dw - (dg / ||v||) v) (either may be NULL).
+ * Both reductions are fixed-order (bitwise reproducible). scratch: VB_WEIGHT_NORM_SCRATCH bytes of device memory per launch. */
+#define VB_WEIGHT_NORM_SCRATCH 1024
+vb_status vb_weight_norm_fwd(const float* v, const float* g, int64_t n, float* w_f32, void* w16, void* w_lo, void* w_b16, int32_t w_fp16,
+                             double* scratch, void* stream);
+vb_status vb_weight_norm_bwd(const float* dw, const float* v, const float* g, int64_t n, float* dg, float* dv, double* scratch, void* stream);
+/* BertPooler's tanh (basebert.py:507-519): y = tanh(x) as y_f32 (may alias x) and operand copies. Backward: dx = dy (1 - y^2) as a
+ * bf16 [M, N] operand, dbias[c] += sum over rows of dx (fixed order). */
+vb_status vb_tanh_fwd(const float* x, float* y_f32, void* y16, void* y_lo, void* y_b16, int32_t y_fp16, int64_t n, void* stream);
+vb_status vb_tanh_bwd(const float* dy, const float* y, void* dx_bf16, float* dbias, int32_t M, int32_t N, void* stream);
+/* out [B, Nt+Nv] = cat((1 - mask_t) * -10000, (1 - mask_v) * -10000) (basebert.py:723-750); masks int64 0/1. */
+vb_status vb_mask_concat_additive(const int64_t* mask_t, const int64_t* mask_v, float* out, int32_t B, int32_t Nt, int32_t Nv, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

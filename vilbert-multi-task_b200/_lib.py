@@ -124,7 +124,17 @@ _SIGNATURES = {
     "vb_grad_norm": [_P, _P, _P, _I32, _F, _F, _P, _P, _P, _P],
     "vb_adamw_step_clipped": [_P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _P, _F, _I32, _P, _P],
     "vb_radam_step_clipped": [_P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _I32, _P, _I32, _F, _I32, _P, _P],
+    "vb_concat_embed_ln_fwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P],
+    "vb_concat_embed_ln_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P],
+    "vb_embed_text_bwd_padded": [_P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _P],
+    "vb_weight_norm_fwd": [_P, _P, _I64, _P, _P, _P, _P, _I32, _P, _P],
+    "vb_weight_norm_bwd": [_P, _P, _P, _I64, _P, _P, _P, _P],
+    "vb_tanh_fwd": [_P, _P, _P, _P, _P, _I32, _I64, _P],
+    "vb_tanh_bwd": [_P, _P, _P, _P, _I32, _I32, _P],
+    "vb_mask_concat_additive": [_P, _P, _P, _I32, _I32, _I32, _P],
 }
+# device scratch of one vb_weight_norm_fwd / _bwd launch (include/vilbert_b200.h)
+VB_WEIGHT_NORM_SCRATCH = 1024
 
 _lib = None
 

@@ -31,6 +31,13 @@ from . import _lib as L
 
 F32, BF16, F16, I64 = torch.float32, torch.bfloat16, torch.float16, torch.int64
 PRECISIONS = ("fp16", "fp32", "bf16")
+# the single-stream baseline hard-codes its region-feature width and region-class count (basebert.py:329, 613); v_feature_size and
+# v_target_size do not apply to it
+BASE_FEATURE_SIZE, BASE_REGION_CLASSES = 2048, 1601
+# outputs of the baseline, in the order BaseBertForVLTasks.forward returns them (basebert.py:954-962), and of its BertModel
+BASE_HEAD_NAMES = ("vil_prediction", "vil_logit", "vil_binary_prediction", "vision_prediction", "vision_logit", "linguisic_prediction",
+                   "linguisic_logit")
+BASE_BERT_OUT_NAMES = ("sequence_output", "pooled_output")
 
 
 def _pad8(n):
@@ -85,13 +92,15 @@ class ParamStore:
     bf16 shadow used as GEMM operands. query/key/value weights of one attention are allocated contiguously
     so that the fused [3H, H] QKV GEMM reads them in place."""
 
-    def __init__(self, cfg, device, heads="vl", op_dtype=F16, split=False):
+    def __init__(self, cfg, device, heads="vl", op_dtype=F16, split=False, num_labels=None):
         """heads: "vl" = pre-training heads + the 7 task heads (VILBertForVLTasks), "pretraining" = cls.* only
-        (BertForMultiModalPreTraining), "none" = bare BertModel. op_dtype: format of the 16-bit weight shadow;
-        split: also keep the low parts (shadow_lo) for the split-precision mode."""
-        assert heads in ("vl", "pretraining", "none")
+        (BertForMultiModalPreTraining), "none" = bare BertModel; "base" = the single-stream baseline BaseBertForVLTasks with
+        `num_labels` answers (vilbert/basebert.py), "base_none" = its bare BertModel. op_dtype: format of the 16-bit weight
+        shadow; split: also keep the low parts (shadow_lo) for the split-precision mode."""
+        assert heads in ("vl", "pretraining", "none", "base", "base_none")
         self.op_dtype, self.split = op_dtype, split
         self.heads = heads
+        self.base = heads in ("base", "base_none")
         with_task_heads = heads == "vl"
         self.cfg = cfg
         self.device = device
@@ -100,6 +109,10 @@ class ParamStore:
         self.parts = {}                # fused qkv name -> the entry names it spans, in order
         self._off = 0
         c = cfg
+        if self.base:
+            self._base_layout(num_labels)
+            self._alloc()
+            return
         Ht, It, Hv, Iv, Hb = c.hidden_size, c.intermediate_size, c.v_hidden_size, c.v_intermediate_size, c.bi_hidden_size
         for h in (Ht, It, Hv, Iv, Hb, c.v_feature_size):
             if h % 8:
@@ -160,6 +173,50 @@ class ParamStore:
             for nm, i, o in (("vil_prediction", Hb, 3129), ("vil_prediction_gqa", Hb, 1533), ("vil_binary_prediction", 2 * Hb, 2)):
                 lin(f"{nm}.logit_fc.0", 2 * Hb, i); ln(f"{nm}.logit_fc.2", 2 * Hb); lin(f"{nm}.logit_fc.3", o, 2 * Hb)
             lin("vil_logit", 1, Hb); lin("vil_tri_prediction", 3, Hb); lin("vision_logit", 1, Hv); lin("linguisic_logit", 1, Ht)
+        self._alloc()
+
+    def _base_layout(self, num_labels):
+        """BaseBertForVLTasks' parameters (basebert.py:284-359, 507-519, 893-978) under the reference's state_dict names, in execution
+        order: embeddings, layers, pooler, heads. SimpleClassifier's weight-normed linears keep weight_g (0-d) and weight_v."""
+        c, add, lin, ln = self.cfg, self._add, self._lin, self._ln
+        H, I = c.hidden_size, c.intermediate_size
+        for h in (H, I):
+            if h % 8:
+                raise ValueError("vilbert_b200: hidden sizes must be multiples of 8 (TMA row pitch)")
+        self.with_task_heads = False
+        add("bert.embeddings.word_embeddings.weight", (c.vocab_size, H))
+        add("bert.embeddings.position_embeddings.weight", (c.max_position_embeddings, H))
+        add("bert.embeddings.token_type_embeddings.weight", (c.type_vocab_size, H))
+        ln("bert.embeddings.LayerNorm", H)
+        lin("bert.image_embeddings.image_embeddings", H, BASE_FEATURE_SIZE)
+        add("bert.image_embeddings.token_type_embeddings.weight", (c.type_vocab_size, H))
+        lin("bert.image_embeddings.image_location_embeddings", H, 5)
+        ln("bert.image_embeddings.LayerNorm", H)
+        for i in range(c.num_hidden_layers):
+            p = f"bert.encoder.layer.{i}"
+            self._qkv(f"{p}.attention.self", ("query", "key", "value"), H, H)
+            lin(f"{p}.attention.output.dense", H, H); ln(f"{p}.attention.output.LayerNorm", H)
+            lin(f"{p}.intermediate.dense", I, H)
+            lin(f"{p}.output.dense", H, I); ln(f"{p}.output.LayerNorm", H)
+        lin("bert.pooler.dense", H, H)
+        if self.heads == "base_none":
+            return
+        if not num_labels or num_labels < 1:
+            raise ValueError("BaseBertForVLTasks needs num_labels >= 1")
+        self.num_labels = int(num_labels)
+        add("cls.predictions.bias", (c.vocab_size,))
+        lin("cls.predictions.transform.dense", H, H); ln("cls.predictions.transform.LayerNorm", H)
+        lin("cls.seq_relationship", 2, H)
+        lin("cls.imagePredictions.transform.dense", H, H); ln("cls.imagePredictions.transform.LayerNorm", H)
+        lin("cls.imagePredictions.decoder", BASE_REGION_CLASSES, H)
+        for i, (o, k) in ((0, (2 * H, H)), (3, (self.num_labels, 2 * H))):
+            add(f"vil_prediction.main.{i}.weight_g", ())
+            add(f"vil_prediction.main.{i}.weight_v", (o, k))
+            add(f"vil_prediction.main.{i}.bias", (o,))
+        lin("vil_logit", 1, H); lin("vision_logit", 1, H); lin("linguisic_logit", 1, H)
+
+    def _alloc(self):
+        device, op_dtype, split = self.device, self.op_dtype, self.split
         self.numel = self._off
         self.flat = torch.zeros(self.numel, dtype=F32, device=device)
         self.grad = torch.zeros(self.numel, dtype=F32, device=device)
@@ -356,19 +413,25 @@ class Plan:
         self.dev = engine.device
         # in_batch_pairs (vilbert.py:1008-1040): at the first connection layer every (text i, image j) combination of the input
         # batch becomes one sample: the streams run at the input batch before it and at B^2 from there on
-        self.pairs = bool(getattr(engine.cfg, "in_batch_pairs", False))
+        # the single-stream baseline (BaseBertForVLTasks) has none of the two-stream options: no batch pairs, task token, fast mode,
+        # gate or attention export, and its plans take no fused objective, outputs= selection or image prefix
+        self.base = engine.ps.base
+        if self.base and (vqa_loss or loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
+                          or loss_in_forward):
+            raise ValueError("single-stream baseline plans support grad_outputs, train and frozen only")
+        self.pairs = bool(getattr(engine.cfg, "in_batch_pairs", False)) and not self.base
         self.Bin = B
         self.B, self.Nt_in, self.Nv = (B * B if self.pairs else B), Nt, Nv
-        self.has_task = bool(self.cfg.task_specific_tokens)
+        self.has_task = bool(self.cfg.task_specific_tokens) and not self.base
         self.Nt = Nt + (1 if self.has_task else 0)
         # FAST_MODE (vilbert.py:1042-1053, eval_retrieval.py): one caption (text batch 1) against B images; inference only
         # config.visualization (vilbert.py:451-458, 610-617, 813-821): export attention probabilities, queries and keys per layer
-        self.viz = bool(getattr(self.cfg, "visualization", False))
+        self.viz = bool(getattr(self.cfg, "visualization", False)) and not self.base
         self.attn_t, self.attn_v, self.attn_c = [], [], []
         if self.viz and train:
             raise ValueError("visualization exports the undropped attention probabilities: eval mode only")
-        self.dyn = bool(getattr(self.cfg, "dynamic_attention", False))
-        self.fast = bool(getattr(self.cfg, "fast_mode", False)) if fast_mode is None else bool(fast_mode)
+        self.dyn = bool(getattr(self.cfg, "dynamic_attention", False)) and not self.base
+        self.fast = (bool(getattr(self.cfg, "fast_mode", False)) if fast_mode is None else bool(fast_mode)) and not self.base
         self.Bt = 1 if self.fast else B
         if self.fast and (train or grad_outputs or vqa_loss or loss):
             raise ValueError("fast_mode is an inference path (text batch 1 broadcast to the image batch): no train mode / gradients")
@@ -1425,6 +1488,9 @@ class Plan:
 
     # ------------------------------------------------------------------ whole model
     def _build(self):
+        if self.base:
+            self._build_base()
+            return
         c, B = self.cfg, self.B
         self.outputs, self.gout = OrderedDict(), {}
         self.loss_inputs = {}
@@ -1544,6 +1610,301 @@ class Plan:
         self.cur.append((None, ("all",), 0))     # join every stream (incl. the weight-gradient side streams)
         self.n_kernels_bwd = sum(1 for op in self.bwd if op[0] is not None)
         self.cur = self.fwd
+
+    # ------------------------------------------------------------------ single-stream baseline (BaseBertForVLTasks)
+    def _build_base(self):
+        """basebert.BertModel.forward + BaseBertForVLTasks.forward (basebert.py:706-774, 923-962): both embeddings LayerNormed into one
+        [B, Nt+Nv, H] stream under the concatenated mask, num_hidden_layers BERT layers over it, the tanh pooler on row 0 and the seven
+        heads. The wide heads (masked-LM, region classes) read their rows gathered into compact operands and scatter their gradient
+        back; the 1-output heads run over the whole stream with a zero output gradient on the rows they do not return."""
+        c, B = self.cfg, self.B
+        self.outputs, self.gout = OrderedDict(), {}
+        self.loss_inputs, self.head_grad = {}, {}
+        self.loss = self.score = self.preds = None
+        self.N = self.Nt + self.Nv
+        self._scatter_ok = False
+        x = self.base_embeddings()
+        self.enc = []
+        for i in range(c.num_hidden_layers):
+            x = self.base_layer(x, i)
+            self.enc.append(x)
+        self.seq = x
+        self.pooled = self.base_pooler(x)
+        self.outputs["sequence_output"] = x.f32.view(B, self.N, -1)
+        self.outputs["pooled_output"] = self.pooled.f32
+        self.out_rg["sequence_output"] = not x.frozen
+        self.out_rg["pooled_output"] = not self.pooled.frozen
+        views = self.build_base_heads(x, self.pooled) if self.heads == "base" else {}
+        self.n_kernels_fwd = sum(1 for op in self.fwd if op[0] is not None)
+
+        self.cur = self.bwd
+        for nm, act in (("sequence_output", self.seq), ("pooled_output", self.pooled)):
+            if nm in self.grad_outputs:
+                self.add_grad(act, self.out_grad_buffer(nm, (act.M, act.H)))
+        self.sync_streams()
+        for entry in reversed(self._bwd_emitters):
+            if entry is None:
+                self.sync_streams()
+            else:
+                self.sid, emitter = entry
+                self._scratch_epoch += 1
+                emitter()
+        self.sid = 0
+        self.cur.append((None, ("all",), 0))
+        self.n_kernels_bwd = sum(1 for op in self.bwd if op[0] is not None)
+        self.cur = self.fwd
+        self.gout.update(views)      # the 1-output heads take their caller's gradient into their rows of the whole-stream buffer
+
+    def base_embeddings(self):
+        """BertEmbeddings + BertImageEmbeddings + torch.cat (basebert.py:284-359, 718-747). The region side (feature cast, box
+        projection, 2048 -> H GEMM) runs on the second stream under the text gather; vb_concat_embed_ln_fwd adds the image token-type
+        row, applies both LayerNorms and dropouts and writes the stream with its operand copies."""
+        ps, c, B, lib = self.ps, self.cfg, self.B, self.lib
+        H, Nt, Nv, Fv = c.hidden_size, self.Nt, self.Nv, BASE_FEATURE_SIZE
+        Mt, Mv, M = B * Nt, B * Nv, B * self.N
+        self.in_ids = self.buf((B, Nt), I64, zero=True)
+        self.in_tt = self.buf((B, Nt), I64, zero=True)
+        self.in_task = None
+        self.in_amask = self.buf((B, Nt), I64, zero=True)
+        self.in_imask = self.buf((B, Nv), I64, zero=True)
+        self.in_feat = self.buf((B, Nv, Fv), F32, zero=True)
+        self.in_loc = self.buf((B, Nv, 5), F32, zero=True)
+        self.mask = self.buf((B, self.N), F32)
+        self.emit(lib.vb_mask_concat_additive, self.in_amask.data_ptr(), self.in_imask.data_ptr(), self.mask.data_ptr(), B, Nt, Nv)
+        self.sync_streams()      # the second stream reads the inputs that load_inputs copied on the main stream
+        e, ie = "bert.embeddings", "bert.image_embeddings"
+        t_tables = [e + n for n in (".word_embeddings.weight", ".position_embeddings.weight", ".token_type_embeddings.weight")]
+        xt = self.buf((Mt, H), F32)
+        self.emit(lib.vb_embed_text_fwd, self.in_ids.data_ptr(), self.in_tt.data_ptr(), None, *[ps.p(n).data_ptr() for n in t_tables], None,
+                  xt.data_ptr(), B, Nt, H)
+        with self.on(1):
+            feat = self.buf16((Mv, Fv))
+            hi, lo, bw = feat.ptrs()
+            self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), hi, Mv * Fv, feat.fp16, lo, bw)
+            locp = self.buf((Mv, H), F32)
+            self.emit(lib.vb_loc_proj_fwd, self.in_loc.data_ptr(), ps.p(ie + ".image_location_embeddings.weight").data_ptr(),
+                      ps.p(ie + ".image_location_embeddings.bias").data_ptr(), locp.data_ptr(), Mv, H)
+            xv = self.buf((Mv, H), F32)
+            self.gemm(Mv, H, Fv, feat, Fv, ps.w(ie + ".image_embeddings.weight"), Fv, bias=ps.p(ie + ".image_embeddings.bias"),
+                      residual=locp, ld_res=H, out_f32=xv, ld_of=H)
+        self.sync_streams()
+        trow = ps.p(ie + ".token_type_embeddings.weight")[1]
+        tdrop = self.drop(e + ".dropout", c.hidden_dropout_prob)
+        vdrop = self.drop(ie + ".dropout", c.hidden_dropout_prob)
+        y32, y = self.buf((M, H), F32), self.buf16((M, H))
+        mean, rstd = self.buf((M,), F32), self.buf((M,), F32)
+        lnt, lnv = e + ".LayerNorm", ie + ".LayerNorm"
+        self.emit(lib.vb_concat_embed_ln_fwd, xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
+                  ps.p(lnt + ".bias").data_ptr(), ps.p(lnv + ".weight").data_ptr(), ps.p(lnv + ".bias").data_ptr(), y32.data_ptr(), *y.ptrs(),
+                  y.fp16, mean.data_ptr(), rstd.data_ptr(), B, Nt, Nv, H, self._ref(tdrop), self._ref(vdrop))
+        x = Act(y32, y, M, H)
+        img = [ie + n for n in (".image_embeddings.weight", ".image_embeddings.bias", ".token_type_embeddings.weight",
+                                ".image_location_embeddings.weight", ".image_location_embeddings.bias")]
+        lns = [lnt + ".weight", lnt + ".bias", lnv + ".weight", lnv + ".bias"]
+        x.frozen = not self.trainable(*t_tables, *img, *lns)
+
+        def bwd():
+            if not x.gw:
+                return
+            gt = [self.pg(n) for n in t_tables]
+            dxt = self.scratch("emb.dxt", (Mt, H), F32) if any(g is not None for g in gt) else None
+            img_w = self.trainable(ie + ".image_embeddings.weight")
+            loc = (self.pg(img[3]), self.pg(img[4]))
+            dxv32 = self.scratch("emb.dxv32", (Mv, H), F32) if (loc[0] is not None or loc[1] is not None) else None
+            dxv16 = self.scratch("emb.dxv16", (Mv, H), BF16) if img_w else None
+            gtype = self.pg(img[2])
+            self.emit(lib.vb_concat_embed_ln_bwd, x.g32.data_ptr(), xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
+                      ps.p(lnv + ".weight").data_ptr(), mean.data_ptr(), rstd.data_ptr(), self._ptr(dxt), self._ptr(dxv32), self._ptr(dxv16),
+                      *[self._ptr(self.pg(n)) for n in lns], self._ptr(self.pg(img[1])), None if gtype is None else gtype[1].data_ptr(),
+                      B, Nt, Nv, H, self._ref(tdrop), self._ref(vdrop))
+            if dxt is not None:
+                self.emit(lib.vb_embed_text_bwd_padded, dxt.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), *[self._ptr(g) for g in gt],
+                          B, Nt, H)
+            if dxv16 is not None:
+                self.linear_wgrad(dxv16, H, None, 0, feat.bw, Fv, Mv, H, Fv, ie + ".image_embeddings")
+            if dxv32 is not None:
+                self.emit(lib.vb_loc_proj_bwd, dxv32.data_ptr(), self.in_loc.data_ptr(), self._ptr(loc[0]), self._ptr(loc[1]), Mv, H)
+        if not x.frozen:
+            self.push_bwd(bwd)
+        return x
+
+    def base_layer(self, x, i):
+        """basebert.BertLayer over the whole stream at N = Nt + Nv with the concatenated mask (basebert.py:480-485)."""
+        p, c = f"bert.encoder.layer.{i}", self.cfg
+        h1 = self.self_attention_block(x, self.B, self.N, c.num_attention_heads, self.mask, p + ".attention", "t",
+                                       p_attn=c.attention_probs_dropout_prob, p_hidden=c.hidden_dropout_prob)
+        return self.ffn(h1, c.intermediate_size, p + ".intermediate.dense", p + ".output.dense", p + ".output.LayerNorm", "t.ffn",
+                        drop=self.drop(p + ".output.dropout", c.hidden_dropout_prob))
+
+    def base_pooler(self, seq):
+        """BertPooler (basebert.py:507-519): Linear on row 0 of every sample (A read with row pitch N*H), then tanh."""
+        ps, B, H, N, w = self.ps, self.B, seq.H, self.N, "bert.pooler.dense"
+        pre = self.buf((B, H), F32)
+        self.gemm(B, H, H, seq.op, N * H, ps.w(w + ".weight"), H, bias=ps.p(w + ".bias"), out_f32=pre, ld_of=H)
+        y32, y = self.buf((B, H), F32), self.buf16((B, H))
+        self.emit(self.lib.vb_tanh_fwd, pre.data_ptr(), y32.data_ptr(), *y.ptrs(), y.fp16, B * H)
+        pooled = Act(y32, y, B, H)
+        pooled.frozen = seq.frozen and not self.trainable(w + ".weight", w + ".bias")
+
+        def bwd():
+            if not pooled.gw:
+                return
+            dpre = self.scratch("pool.dpre", (B, H), BF16)
+            self.emit(self.lib.vb_tanh_bwd, pooled.g32.data_ptr(), y32.data_ptr(), dpre.data_ptr(), self._ptr(self.pg(w + ".bias")), B, H)
+            self.linear_wgrad(dpre, H, None, 0, seq.op.bw, N * H, B, H, H, w)
+            if seq.frozen:
+                return
+            g = self.grad_of(seq)
+            if not seq.gw:
+                self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
+                seq.gw = True
+            self.gemm(B, H, H, dpre, H, ps.w(w + ".weight").bw, H, b_mn=1, residual=g, ld_res=N * H, out_f32=g, ld_of=N * H)
+        if not pooled.frozen:
+            self.push_bwd(bwd)
+        return pooled
+
+    def base_rows(self, seq, a, b, tag):
+        """Rows [a, b) of every sample of the stream as a compact Act (operand copies: the head transform reads nothing else). Its
+        backward scatters the compact gradient into those rows of the stream gradient."""
+        lib, B, N, H = self.lib, self.B, self.N, seq.H
+        n = b - a
+        idx = self.buf((B * n,), torch.int32, zero=True)
+        idx.copy_((torch.arange(B).view(B, 1) * N + torch.arange(a, b).view(1, n)).reshape(-1).to(torch.int32))
+        op = self.buf16((B * n, H))
+        self.emit(lib.vb_gather_rows16, seq.op.hi.data_ptr(), op.hi.data_ptr(), self._ptr(seq.op.extra_bw), self._ptr(op.extra_bw), idx.data_ptr(),
+                  B * n, H)
+        if op.lo is not None:
+            self.emit(lib.vb_gather_rows16, seq.op.lo.data_ptr(), op.lo.data_ptr(), None, None, idx.data_ptr(), B * n, H)
+        rows = Act(None, op, B * n, H)
+        rows.frozen = seq.frozen
+
+        def bwd():
+            if not rows.gw:
+                return
+            g = self.grad_of(seq)
+            if not seq.gw:      # the gathered heads' backward runs first: zero the stream gradient once, then scatter disjoint rows
+                self.emit(lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
+                seq.gw = self._scatter_ok = True
+            if self._scatter_ok:
+                self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), g.data_ptr(), idx.data_ptr(), B * n, H, None, None)
+                return
+            full = self.scratch(tag + ".full", (B * N, H), F32)      # the stream gradient already holds other contributions
+            self.emit(lib.vb_memset_zero, full.data_ptr(), full.numel() * 4)
+            self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), full.data_ptr(), idx.data_ptr(), B * n, H, None, None)
+            self.emit(lib.vb_axpy_f32, full.data_ptr(), g.data_ptr(), full.numel(), 1.0)
+        if not seq.frozen:
+            self.push_bwd(bwd)
+        return rows
+
+    def _wide_bwd(self, head_bwd, hn, tr_bwd, K, N_out):
+        """Backward of a transform + wide decoder head: d(transform output) = d(logits) W, then the transform's backward."""
+        def f():
+            r = head_bwd()
+            if r is None:
+                return
+            dl16, ldp, W16 = r
+            g = self.grad_of(hn)
+            self.gemm(hn.M, K, N_out, dl16, ldp, W16, K, b_mn=1, out_f32=g, ld_of=K)
+            hn.gw = True
+            tr_bwd()
+        return f
+
+    def base_simple_classifier(self, x):
+        """vil_prediction = SimpleClassifier (basebert.py:965-978): weight_norm(Linear(H, 2H), dim=None) -> ReLU -> Dropout(0.5) ->
+        weight_norm(Linear(2H, num_labels), dim=None) on the pooled output. Like the reference's weight_norm pre-forward hook, every
+        forward first derives both weights from (g, v) (vb_weight_norm_fwd: fp32 and the operand copies), so a parameter update by
+        any optimizer is picked up without a separate refresh. The dropout sits in the first GEMM's epilogue after the ReLU; its
+        backward folds the 1 / (1 - p) scale into the dgrad GEMM and gates by the dropped output."""
+        ps, lib, B, H, Lb = self.ps, self.lib, self.B, x.H, self.ps.num_labels
+        H2 = 2 * H
+        W, self.wn_weights = {}, {}
+        for i in (0, 3):
+            nm = f"vil_prediction.main.{i}"
+            v, g = ps.p(nm + ".weight_v"), ps.p(nm + ".weight_g")
+            w32, op = self.buf(tuple(v.shape), F32), self.buf16(tuple(v.shape))
+            scr = self.buf((L.VB_WEIGHT_NORM_SCRATCH // 8,), torch.float64)
+            self.emit(lib.vb_weight_norm_fwd, v.data_ptr(), g.data_ptr(), v.numel(), w32.data_ptr(), *op.ptrs(), op.fp16, scr.data_ptr())
+            W[i] = (nm, v, g, op, scr)
+            self.wn_weights[nm] = w32
+        p_drop = 0.5
+        drop = self.drop("vil_prediction.main.2", p_drop)
+        h32, h = self.buf((B, H2), F32), self.buf16((B, H2))
+        self.gemm(B, H2, H, x.op, H, W[0][3], H, bias=ps.p("vil_prediction.main.0.bias"), act=L.VB_ACT_RELU, out_f32=h32, ld_of=H2,
+                  out_bf16=h, ld_ob=H2, dropout=drop)
+        logits = self.buf((B, Lb), F32)
+        self.gemm(B, Lb, H2, h, H2, W[3][3], H2, bias=ps.p("vil_prediction.main.3.bias"), out_f32=logits, ld_of=Lb)
+        self.outputs["vil_prediction"] = logits
+        part = lambda i: [f"vil_prediction.main.{i}.{s}" for s in ("weight_g", "weight_v", "bias")]
+        h_rg = not x.frozen or self.trainable(*part(0))
+        self.out_rg["vil_prediction"] = h_rg or self.trainable(*part(3))
+        scale = 1.0 / (1.0 - p_drop) if drop is not None else 1.0
+
+        def wn_wgrad(i, dy16, ld_dy, x16, ld_x, M, N_out, K_in):
+            nm, v, g, _, scr = W[i]
+            gg, gv = self.pg(nm + ".weight_g"), self.pg(nm + ".weight_v")
+            if gg is None and gv is None:
+                return
+            dw = self.scratch(f"vilp.dw{i}", (N_out, K_in), F32)
+            self.emit(lib.vb_memset_zero, dw.data_ptr(), dw.numel() * 4)
+            self.gemm(N_out, K_in, M, dy16, ld_dy, x16, ld_x, a_mn=1, b_mn=1, out_f32=dw, ld_of=K_in, atomic=1, split_k=0)
+            self.emit(lib.vb_weight_norm_bwd, dw.data_ptr(), v.data_ptr(), g.data_ptr(), v.numel(), self._ptr(gg), self._ptr(gv), scr.data_ptr())
+
+        def bwd():
+            if "vil_prediction" not in self.grad_outputs:
+                return
+            ldp = _pad8(Lb)
+            dl32 = self.out_grad_buffer("vil_prediction", (B, Lb))
+            dl16 = self.scratch("vilp.dl16", (B, ldp), BF16)
+            self.emit(lib.vb_cast2d_f32_to_bf16, dl32.data_ptr(), Lb, dl16.data_ptr(), ldp, B, Lb, 1.0)
+            gb = self.pg("vil_prediction.main.3.bias")
+            if gb is not None:
+                self.colsum(dl32, Lb, gb, B, Lb)
+            wn_wgrad(3, dl16, ldp, h.bw, H2, B, Lb, H2)
+            if not h_rg:
+                return
+            dh = self.scratch("vilp.dh32", (B, H2), F32)
+            self.gemm(B, H2, Lb, dl16, ldp, W[3][3].bw, H2, b_mn=1, out_f32=dh, ld_of=H2, alpha=scale)
+            dpre16, dpre32 = self.scratch("vilp.dpre16", (B, H2), BF16), self.scratch("vilp.dpre32", (B, H2), F32)
+            self.emit(lib.vb_relu_bwd, dh.data_ptr(), h32.data_ptr(), dpre16.data_ptr(), dpre32.data_ptr(), B * H2)
+            gb = self.pg("vil_prediction.main.0.bias")
+            if gb is not None:
+                self.colsum(dpre32, H2, gb, B, H2)
+            wn_wgrad(0, dpre16, H2, x.op.bw, H, B, H2, H)
+            self.dgrad_into(x, dpre16, H2, W[0][3].bw, B, H2, H)
+        if self.out_rg["vil_prediction"]:
+            self.push_bwd(bwd)
+
+    def build_base_heads(self, seq, pooled):
+        """The seven outputs of BaseBertForVLTasks.forward (basebert.py:929-962). Returns the views of the whole-stream output-gradient
+        buffers that the caller's gradients of the 1-output heads go into. Emission order is chosen for the backward, which runs it
+        in reverse: the gathered heads first (their scatters are the first writes to the stream gradient), then the 1-output heads
+        over the stream and the pooled heads (which accumulate), then the pooler."""
+        ps, c, B = self.ps, self.cfg, self.B
+        H, Nt, Nv, N = seq.H, self.Nt, self.Nv, self.N
+        self.base_simple_classifier(pooled)
+        self.small_head("vil_logit", pooled, "vil_logit", 1)
+        self.small_head("vil_binary_prediction", pooled, "cls.seq_relationship", 2)
+        views = {}
+        # self.dropout is one nn.Dropout called twice (basebert.py:949-952): two sites, each a mask over the whole stream
+        for name, site, a, b in (("vision_logit", "dropout.seq_v", Nt, N), ("linguisic_logit", "dropout.seq_t", 0, Nt)):
+            full = self.out_grad_buffer(name, (B * N, 1))
+            self.small_head(name, seq, name, 1, addend=self.mask if name == "vision_logit" else None,
+                            in_drop=self.drop(site, self.head_dropout_prob))
+            self.outputs[name] = self.outputs[name].view(B, N, 1)[:, a:b]
+            views[name] = full.view(B, N, 1)[:, a:b]
+        rows_t = self.base_rows(seq, 0, Nt, "rows.t")
+        rows_v = self.base_rows(seq, Nt, N, "rows.v")
+        wn = "bert.embeddings.word_embeddings.weight"
+        ht, ht_bwd = self.transform(rows_t, "cls.predictions.transform.dense", "cls.predictions.transform.LayerNorm", "lm.tr")
+        lm_bwd = self.big_head("linguisic_prediction", ht, H, B * Nt, H, c.vocab_size, None, "cls.predictions.bias", w=ps.w(wn), gw_name=wn)
+        hv, hv_bwd = self.transform(rows_v, "cls.imagePredictions.transform.dense", "cls.imagePredictions.transform.LayerNorm", "im.tr")
+        im_bwd = self.big_head("vision_prediction", hv, H, B * Nv, H, BASE_REGION_CLASSES, "cls.imagePredictions.decoder",
+                               "cls.imagePredictions.decoder.bias")
+        self.push_bwd(self._wide_bwd(lm_bwd, ht, ht_bwd, H, c.vocab_size))
+        self.push_bwd(self._wide_bwd(im_bwd, hv, hv_bwd, H, BASE_REGION_CLASSES))
+        self.outputs["linguisic_prediction"] = self.outputs["linguisic_prediction"].view(B, Nt, -1)
+        self.outputs["vision_prediction"] = self.outputs["vision_prediction"].view(B, Nv, -1)
+        return views
 
     def attention_export(self):
         """The reference's all_attention_mask triple (BertEncoder.forward, vilbert.py:1098-1107) for config.visualization: lists of
@@ -2149,9 +2510,10 @@ class Plan:
 class Engine:
     """Owns the parameters and the per-shape plans."""
 
-    def __init__(self, cfg, device="cuda", heads="vl", _build_only=False, two_streams=True, wgrad_streams=True, precision="fp16"):
+    def __init__(self, cfg, device="cuda", heads="vl", _build_only=False, two_streams=True, wgrad_streams=True, precision="fp16",
+                 num_labels=None):
         """_build_only=True (tests) allows a CPU device: plans can be constructed and inspected but never run.
-        precision: "fp16" | "fp32" | "bf16" (module docstring)."""
+        precision: "fp16" | "fp32" | "bf16" (module docstring). num_labels: answers of the baseline's vil_prediction (heads="base")."""
         cfg.check_supported()
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be one of {PRECISIONS}")
@@ -2163,7 +2525,7 @@ class Engine:
         if self.device.type != "cuda" and not _build_only:
             raise L.VBError("vilbert_b200 runs on sm_90a GPUs only; there is no CPU path (device=%s)" % device)
         L.lib()  # fail loudly now if the extension is missing
-        self.ps = ParamStore(cfg, self.device, heads, self.op_dtype, self.split)
+        self.ps = ParamStore(cfg, self.device, heads, self.op_dtype, self.split, num_labels=num_labels)
         self.two_streams = two_streams   # text / vision segments on two CUDA streams (parallel graph branches)
         self.wgrad_streams = wgrad_streams   # weight-gradient GEMMs on two more side streams (off the backward critical chain)
         self.plans = OrderedDict()       # LRU cache of per-shape plans (each owns its activation buffers)

@@ -199,7 +199,7 @@ class BertPreTrainedModel(nn.Module):
     config_class = BertConfig
     _heads = "vl"          # which heads own parameters: "vl" | "pretraining" | "none"
 
-    def __init__(self, config, device=None, precision=None):
+    def __init__(self, config, device=None, precision=None, num_labels=None):
         """precision: "fp16" (default: fp16 forward operands, bf16 gradient operands, fp32 accumulation / residual stream),
         "fp32" (split precision, matches the reference's fp32 outputs to 1e-3) or "bf16"; default from
         $VILBERT_B200_PRECISION. The reference's constructors have no such argument: it selects what `model.half()` /
@@ -212,7 +212,7 @@ class BertPreTrainedModel(nn.Module):
         dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
         if dev.type != "cuda" or not torch.cuda.is_available():
             raise L.VBError("vilbert_b200 models run on sm_90a GPUs only; there is no CPU path")
-        self.engine = Engine(config, dev, heads=self._heads, precision=precision)
+        self.engine = Engine(config, dev, heads=self._heads, precision=precision, num_labels=num_labels)
         self._params = _register_tree(self, self.engine.ps)
         self._pnames, self._plist = tuple(self._params), tuple(self._params.values())
         self._frozen_flags, self._frozen_set = None, frozenset()
