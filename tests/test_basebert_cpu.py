@@ -122,6 +122,18 @@ def test_frozen_baseline_plan_skips_frozen_work(golden_dir):
     assert all(off >= lo for (off, _n) in plan.grad_touch)
 
 
+def test_baseline_box_projection_gradient_is_recorded_at_its_kernel(golden_dir):
+    """grad_touch names the backward op that writes each gradient range last; for the box projection that is vb_loc_proj_bwd, so
+    no data-parallel segment hands the range to the all-reduce before that kernel has run."""
+    meta, _ = _golden(golden_dir)
+    from vilbert_b200.engine import BASE_HEAD_NAMES
+    eng = _engine(meta)
+    plan = eng.plan(3, 9, 11, grad_outputs=BASE_HEAD_NAMES, train=True)
+    for n in ("weight", "bias"):
+        i = plan.grad_touch[eng.ps.span(f"bert.image_embeddings.image_location_embeddings.{n}")]
+        assert plan.bwd[i][0].__name__ == "vb_loc_proj_bwd"
+
+
 def test_baseline_plan_options_are_checked(golden_dir):
     meta, _ = _golden(golden_dir)
     eng = _engine(meta)

@@ -19,10 +19,14 @@ ARENA_BYTES = 64 << 20
 NT, NV = 9, 11
 
 
-def cases(O, LOSS_HEADS):
-    """(name, config overrides, engine heads, B, plan kwargs[, Nv]) of the case matrix. A case the tree cannot build (an objective
-    kind or a plan option it does not have) is skipped with a note on stderr, so listings of two trees compare case by case."""
+def cases(O, E, base_labels):
+    """(name, config overrides, engine heads, B, plan kwargs[, Nv[, Engine kwargs]]) of the case matrix. The overrides apply to
+    tests/golden/tiny_b4.json, or for the single-stream baseline (heads "base*") to tests/golden/tiny_basebert.json, whose answer
+    count is `base_labels`. A case the tree cannot build (an objective kind or a plan option it does not have) is skipped with a
+    note on stderr, so listings of two trees compare case by case."""
+    LOSS_HEADS = E.LOSS_HEADS
     train = dict(grad_outputs=O.HEAD_NAMES, train=True)
+    base = dict(num_labels=base_labels)
 
     def obj(kind, **kw):
         return dict(grad_outputs=LOSS_HEADS.get(kind, ()), loss=kind, train=True, **kw)
@@ -86,6 +90,20 @@ def cases(O, LOSS_HEADS):
             [f"bert.v_embeddings.{n}" for n in ("image_embeddings.weight", "image_embeddings.bias", "image_location_embeddings.weight",
                                                "image_location_embeddings.bias", "LayerNorm.weight", "LayerNorm.bias")] +
             [f"bert.encoder.c_layer.0.biattention.{n}{i}.{w}" for n in ("query", "key", "value") for i in (1,) for w in ("weight", "bias")]))),
+        # the single-stream baseline (vilbert_b200.basebert): training with all seven outputs, eval, its embeddings and first layer
+        # frozen, and the bare BertModel with gradients into its outputs
+        ("base_train", {}, "base", 3, dict(grad_outputs=E.BASE_HEAD_NAMES, train=True), NV, base),
+        ("base_eval", {}, "base", 3, {}, NV, base),
+        ("base_frozen_embeddings_layer0", {}, "base", 3, dict(grad_outputs=E.BASE_HEAD_NAMES, train=True, frozen=frozenset(
+            [f"bert.embeddings.{n}" for n in ("word_embeddings.weight", "position_embeddings.weight", "token_type_embeddings.weight",
+                                             "LayerNorm.weight", "LayerNorm.bias")] +
+            [f"bert.image_embeddings.{n}" for n in ("image_embeddings.weight", "image_embeddings.bias", "token_type_embeddings.weight",
+                                                   "image_location_embeddings.weight", "image_location_embeddings.bias",
+                                                   "LayerNorm.weight", "LayerNorm.bias")] +
+            [f"bert.encoder.layer.0.{n}.{w}" for n in ("attention.self.query", "attention.self.key", "attention.self.value",
+                                                      "attention.output.dense", "attention.output.LayerNorm", "intermediate.dense",
+                                                      "output.dense", "output.LayerNorm") for w in ("weight", "bias")])), NV, base),
+        ("base_none_bert_outputs", {}, "base_none", 3, dict(grad_outputs=E.BASE_BERT_OUT_NAMES), NV, base),
     ]
 
 
@@ -177,18 +195,24 @@ def main():
     import torch
     from oracle import vilbert_oracle as O
     from vilbert_b200.config import BertConfig
-    from vilbert_b200.engine import LOSS_HEADS, PRECISIONS, Engine
+    from vilbert_b200 import engine as E
+    from vilbert_b200.engine import PRECISIONS, Engine
     from vilbert_b200.optim import FusedAdamW, FusedRAdam
-    tiny = json.load(open(os.path.join(root, "tests", "golden", "tiny_b4.json")))["config"]
+    golden = os.path.join(root, "tests", "golden")
+    tiny = json.load(open(os.path.join(golden, "tiny_b4.json")))["config"]
+    tiny_base = json.load(open(os.path.join(golden, "tiny_basebert.json")))
     out, n_plans, n_ops = [], 0, 0
     for prec in PRECISIONS:
-        for name, over, heads, B, kw, *nv in cases(O, LOSS_HEADS):
+        for name, over, heads, B, kw, *extra in cases(O, E, tiny_base["num_labels"]):
+            nv = extra[0] if extra else NV
+            engine_kw = extra[1] if len(extra) > 1 else {}
+            cfg = dict(tiny_base["config"] if heads.startswith("base") else tiny, **over)
             for arena in (False, True):
-                eng = Engine(BertConfig.from_dict(dict(tiny, **over)), "cpu", heads=heads, _build_only=True, precision=prec)
+                eng = Engine(BertConfig.from_dict(cfg), "cpu", heads=heads, _build_only=True, precision=prec, **engine_kw)
                 if arena:
                     eng.enable_activation_arena(ARENA_BYTES)
                 try:
-                    plan = eng.plan(B, NT, nv[0] if nv else NV, **kw)
+                    plan = eng.plan(B, NT, nv, **kw)
                 except (TypeError, ValueError) as ex:
                     print(f"plan_dump: {prec} {name} arena={int(arena)} skipped: {ex}", file=sys.stderr)
                     continue

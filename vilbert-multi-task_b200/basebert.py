@@ -1,6 +1,6 @@
 """Drop-in module surface of the single-stream baseline (vilbert/basebert.py): BaseBertForVLTasks, the model `--baseline` selects in
 train_tasks.py / eval_tasks.py / eval_retrieval.py, and its BertModel, with the reference's constructor / forward signatures, output
-tuples and state_dict key names, executing on the H100 engine (engine.Plan._build_base). A driver swaps
+tuples and state_dict key names, executing on the H100 engine (engine.BasePlan). A driver swaps
 `from vilbert.basebert import BaseBertForVLTasks` for `from vilbert_b200.basebert import BaseBertForVLTasks`.
 
 Text and image embeddings are LayerNormed into one [B, Nt+Nv, H] stream that num_hidden_layers BERT layers process under the

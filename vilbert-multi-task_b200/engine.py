@@ -228,11 +228,8 @@ class ParamStore:
         self.shadow_version = None
 
     def _add(self, name, shape):
-        n = 1
-        for s in shape:
-            n *= s
         self.entries[name] = (self._off, tuple(shape))
-        self._off += _pad8(n)
+        self._off += _pad8(math.prod(shape))
 
     def _lin(self, name, o, i):
         self._add(name + ".weight", (o, i)); self._add(name + ".bias", (o,))
@@ -253,12 +250,17 @@ class ParamStore:
         self.parts[f"{prefix}.{fused}.weight"] = tuple(f"{prefix}.{nm}.weight" for nm in names)
         self.parts[f"{prefix}.{fused}.bias"] = tuple(f"{prefix}.{nm}.bias" for nm in names)
 
+    def _layout(self, name):
+        return self.entries[name] if name in self.entries else self.fused[name]
+
+    def span(self, name):
+        """(flat offset, numel) of an entry or a fused projection."""
+        off, shape = self._layout(name)
+        return off, math.prod(shape)
+
     def _view(self, flat, name):
-        off, shape = self.entries[name] if name in self.entries else self.fused[name]
-        n = 1
-        for s in shape:
-            n *= s
-        return flat[off:off + n].view(shape)
+        off, shape = self._layout(name)
+        return flat[off:off + math.prod(shape)].view(shape)
 
     def p(self, name):
         return self._view(self.flat, name)
@@ -283,27 +285,6 @@ class ParamStore:
 
 
 # ------------------------------------------------------------------------------------------ plan
-class _TrackedParams:
-    """ParamStore proxy used while a plan is emitted: remembers, for every gradient range handed out during the
-    backward emission, the index of the backward op about to write it (the last such index per range is kept)."""
-
-    def __init__(self, ps, plan):
-        self._ps, self._plan = ps, plan
-
-    def __getattr__(self, name):
-        return getattr(self._ps, name)
-
-    def g(self, name):
-        ps, plan = self._ps, self._plan
-        off, shape = ps.entries[name] if name in ps.entries else ps.fused[name]
-        n = 1
-        for d in shape:
-            n *= d
-        if plan.cur is plan.bwd:
-            plan.grad_touch[(off, n)] = len(plan.bwd)
-        return ps.g(name)
-
-
 class Act:
     """A residual-stream activation: fp32 values, its tensor-core Operand, fp32 gradient (lazily allocated)."""
     __slots__ = ("f32", "op", "g32", "gw", "M", "H", "frozen")
@@ -408,38 +389,12 @@ class Plan:
             raise ValueError(f"frozen: {unknown[:4]} are not parameter entries of this model")
         self.out_rg = {}              # output name -> it carries a gradient (some trainable parameter lies upstream of it)
         self.grad_touch = {}           # (flat offset, numel) -> index of the last backward op writing that gradient range
-        self.ps = _TrackedParams(engine.ps, self)
+        self.ps = engine.ps
         self.lib = L.lib()
         self.dev = engine.device
-        # in_batch_pairs (vilbert.py:1008-1040): at the first connection layer every (text i, image j) combination of the input
-        # batch becomes one sample: the streams run at the input batch before it and at B^2 from there on
-        # the single-stream baseline (BaseBertForVLTasks) has none of the two-stream options: no batch pairs, task token, fast mode,
-        # gate or attention export, and its plans take no fused objective, outputs= selection or image prefix
-        self.base = engine.ps.base
-        if self.base and (vqa_loss or loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
-                          or loss_in_forward):
-            raise ValueError("single-stream baseline plans support grad_outputs, train and frozen only")
-        self.pairs = bool(getattr(engine.cfg, "in_batch_pairs", False)) and not self.base
         self.Bin = B
-        self.B, self.Nt_in, self.Nv = (B * B if self.pairs else B), Nt, Nv
-        self.has_task = bool(self.cfg.task_specific_tokens) and not self.base
-        self.Nt = Nt + (1 if self.has_task else 0)
-        # FAST_MODE (vilbert.py:1042-1053, eval_retrieval.py): one caption (text batch 1) against B images; inference only
-        # config.visualization (vilbert.py:451-458, 610-617, 813-821): export attention probabilities, queries and keys per layer
-        self.viz = bool(getattr(self.cfg, "visualization", False)) and not self.base
+        self._stream_modes(B, Nt, Nv, train, grad_outputs, vqa_loss, loss, fast_mode, image_prefix)
         self.attn_t, self.attn_v, self.attn_c = [], [], []
-        if self.viz and train:
-            raise ValueError("visualization exports the undropped attention probabilities: eval mode only")
-        self.dyn = bool(getattr(self.cfg, "dynamic_attention", False)) and not self.base
-        self.fast = (bool(getattr(self.cfg, "fast_mode", False)) if fast_mode is None else bool(fast_mode)) and not self.base
-        self.Bt = 1 if self.fast else B
-        if self.fast and (train or grad_outputs or vqa_loss or loss):
-            raise ValueError("fast_mode is an inference path (text batch 1 broadcast to the image batch): no train mode / gradients")
-        self.image_prefix = bool(image_prefix)
-        if self.image_prefix and (train or grad_outputs or vqa_loss):
-            raise ValueError("image_prefix keeps the image states across forwards: forward-only plans (no train mode, no grad_outputs)")
-        if self.image_prefix and self.pairs:
-            raise ValueError("image_prefix: in_batch_pairs re-expands the image batch inside the forward")
         self.prefix = []         # image_prefix: the image embedding and mask, run by run_image_prefix()
         self._private = False    # while set, buf() allocates private buffers (the image states of image_prefix)
         self.grad_outputs = frozenset(grad_outputs)
@@ -487,6 +442,31 @@ class Plan:
         self._arena_off = self.arena_bytes = 0
         self._build()
 
+    def _stream_modes(self, B, Nt, Nv, train, grad_outputs, vqa_loss, loss, fast_mode, image_prefix):
+        """Shapes and checks of the two-stream options: in_batch_pairs, the task token, visualization, dynamic_attention,
+        fast_mode and image_prefix."""
+        # in_batch_pairs (vilbert.py:1008-1040): at the first connection layer every (text i, image j) combination of the input
+        # batch becomes one sample: the streams run at the input batch before it and at B^2 from there on
+        self.pairs = bool(getattr(self.cfg, "in_batch_pairs", False))
+        self.B, self.Nt_in, self.Nv = (B * B if self.pairs else B), Nt, Nv
+        self.has_task = bool(self.cfg.task_specific_tokens)
+        self.Nt = Nt + (1 if self.has_task else 0)
+        # FAST_MODE (vilbert.py:1042-1053, eval_retrieval.py): one caption (text batch 1) against B images; inference only
+        # config.visualization (vilbert.py:451-458, 610-617, 813-821): export attention probabilities, queries and keys per layer
+        self.viz = bool(getattr(self.cfg, "visualization", False))
+        if self.viz and train:
+            raise ValueError("visualization exports the undropped attention probabilities: eval mode only")
+        self.dyn = bool(getattr(self.cfg, "dynamic_attention", False))
+        self.fast = bool(getattr(self.cfg, "fast_mode", False)) if fast_mode is None else bool(fast_mode)
+        self.Bt = 1 if self.fast else B
+        if self.fast and (train or grad_outputs or vqa_loss or loss):
+            raise ValueError("fast_mode is an inference path (text batch 1 broadcast to the image batch): no train mode / gradients")
+        self.image_prefix = bool(image_prefix)
+        if self.image_prefix and (train or grad_outputs or vqa_loss):
+            raise ValueError("image_prefix keeps the image states across forwards: forward-only plans (no train mode, no grad_outputs)")
+        if self.image_prefix and self.pairs:
+            raise ValueError("image_prefix: in_batch_pairs re-expands the image batch inside the forward")
+
     def _check_outputs(self):
         """Build-time checks of outputs= and results=: known head names, and every head the objective, a gradient or the results
         read is kept."""
@@ -531,19 +511,25 @@ class Plan:
         parts = self.e.ps.parts
         return any(p not in self.frozen for n in names for p in parts.get(n, (n,)))
 
+    def grad_view(self, name):
+        """Gradient view of the entry or fused projection `name` for the next backward op to write. grad_touch keeps, per range,
+        the index of the last backward op that writes it."""
+        if self.cur is self.bwd:
+            self.grad_touch[self.ps.span(name)] = len(self.bwd)
+        return self.ps.g(name)
+
     def pg(self, name):
         """Gradient view of the entry `name` for a backward op to write, or None when it is frozen."""
-        return None if name in self.frozen else self.ps.g(name)
+        return None if name in self.frozen else self.grad_view(name)
 
     def gparts(self, name):
         """Gradient views of the parts of `name` (the entries of a fused projection, or the entry itself), None for a frozen part.
         With every part trainable they are slices of one view of the whole range."""
-        ps = self.ps
-        parts = ps.parts.get(name)
+        parts = self.ps.parts.get(name)
         if parts is None:
             return [self.pg(name)]
         if not any(p in self.frozen for p in parts):
-            g = ps.g(name)
+            g = self.grad_view(name)
             n = g.shape[0] // len(parts)
             return [g[i * n:(i + 1) * n] for i in range(len(parts))]
         return [self.pg(p) for p in parts]
@@ -573,9 +559,7 @@ class Plan:
             t = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=self.dev)
             self._keep.append(t)
             return t
-        n = 1
-        for d in (shape if isinstance(shape, (tuple, list)) else (shape,)):
-            n *= int(d)
+        n = math.prod(int(d) for d in (shape if isinstance(shape, (tuple, list)) else (shape,)))
         nbytes = n * torch.empty((), dtype=dtype).element_size()
         off = self._arena_off
         if off + nbytes > arena.numel():
@@ -1158,15 +1142,7 @@ class Plan:
         if self.image_prefix:
             self.cur = self.prefix
         with self.on(0 if self.image_prefix else 1):
-            feat = self.buf16((Mv, Fv))
-            hi, lo, bw = feat.ptrs()
-            self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), hi, Mv * Fv, feat.fp16, lo, bw)
-            locp = self.buf((Mv, Hv), F32)
-            self.emit(lib.vb_loc_proj_fwd, self.in_loc.data_ptr(), ps.p(ve + ".image_location_embeddings.weight").data_ptr(),
-                      ps.p(ve + ".image_location_embeddings.bias").data_ptr(), locp.data_ptr(), Mv, Hv)
-            yv = self.buf((Mv, Hv), F32)
-            self.gemm(Mv, Hv, Fv, feat, Fv, ps.w(ve + ".image_embeddings.weight"), Fv, bias=ps.p(ve + ".image_embeddings.bias"),
-                      residual=locp, ld_res=Hv, out_f32=yv, ld_of=Hv)
+            yv, feat = self.image_embedding(ve, Hv)
             vdrop = self.drop(ve + ".dropout", c.hidden_dropout_prob)     # BertImageEmbeddings uses hidden_dropout_prob (vilbert.py:1419)
             self._private = self.image_prefix
             v32, vop, vmean, vrstd = self.ln_fwd(yv, ps.p(ve + ".LayerNorm.weight"), ps.p(ve + ".LayerNorm.bias"), Mv, Hv, out_drop=vdrop)
@@ -1184,13 +1160,39 @@ class Plan:
                     dyv16 = self.scratch("emb.dyv16", (Mv, Hv), BF16)
                     self.ln_bwd(v.g32, yv, ps.p(ve + ".LayerNorm.weight"), vmean, vrstd, dyv32, dyv16, Mv, Hv, self.pg(ve + ".LayerNorm.weight"),
                                 self.pg(ve + ".LayerNorm.bias"), gbias=self.pg(ve + ".image_embeddings.bias"), out_drop=vdrop)
-                    self.linear_wgrad(dyv16, Hv, None, 0, feat.bw, Fv, Mv, Hv, Fv, ve + ".image_embeddings")
-                    gl = (self.pg(ve + ".image_location_embeddings.weight"), self.pg(ve + ".image_location_embeddings.bias"))
-                    if gl[0] is not None or gl[1] is not None:
-                        self.emit(lib.vb_loc_proj_bwd, dyv32.data_ptr(), self.in_loc.data_ptr(), self._ptr(gl[0]), self._ptr(gl[1]), Mv, Hv)
+                    self.image_embedding_bwd(ve, Hv, feat, dyv16, dyv32)
             if not v.frozen:
                 self.push_bwd(bwd_image)
         return t, v
+
+    def image_embedding(self, prefix, H):
+        """The image embedding up to its LayerNorm (vilbert.py:1421-1432, basebert.py:324-359) on the loaded regions: feature cast to
+        an operand, the 5 -> H box projection, and the region-feature GEMM with the box term as its residual. -> (fp32 output
+        [regions, H], the feature Operand)."""
+        ps, lib = self.ps, self.lib
+        B, Nv, Fv = self.in_feat.shape
+        M = B * Nv
+        feat = self.buf16((M, Fv))
+        hi, lo, bw = feat.ptrs()
+        self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), hi, M * Fv, feat.fp16, lo, bw)
+        locp = self.buf((M, H), F32)
+        self.emit(lib.vb_loc_proj_fwd, self.in_loc.data_ptr(), ps.p(prefix + ".image_location_embeddings.weight").data_ptr(),
+                  ps.p(prefix + ".image_location_embeddings.bias").data_ptr(), locp.data_ptr(), M, H)
+        y = self.buf((M, H), F32)
+        self.gemm(M, H, Fv, feat, Fv, ps.w(prefix + ".image_embeddings.weight"), Fv, bias=ps.p(prefix + ".image_embeddings.bias"),
+                  residual=locp, ld_res=H, out_f32=y, ld_of=H)
+        return y, feat
+
+    def image_embedding_bwd(self, prefix, H, feat, dy16, dy32):
+        """Parameter gradients of image_embedding from d(output): the region-feature GEMM's weight from its bf16 copy dy16, the box
+        projection from the fp32 dy32 (either None: no gradient wanted)."""
+        M, Fv = feat.hi.shape
+        if dy16 is not None:
+            self.linear_wgrad(dy16, H, None, 0, feat.bw, Fv, M, H, Fv, prefix + ".image_embeddings")
+        if dy32 is not None:
+            gw, gb = self.pg(prefix + ".image_location_embeddings.weight"), self.pg(prefix + ".image_location_embeddings.bias")
+            if gw is not None or gb is not None:
+                self.emit(self.lib.vb_loc_proj_bwd, dy32.data_ptr(), self.in_loc.data_ptr(), self._ptr(gw), self._ptr(gb), M, H)
 
     # ------------------------------------------------------------------ poolers and heads
     def pooler(self, seq, N, wname):
@@ -1210,17 +1212,23 @@ class Plan:
             dpre32 = self.scratch("pool.dpre32", (B, Hb), F32)
             self.emit(self.lib.vb_relu_bwd, pooled.g32.data_ptr(), p32.data_ptr(), dpre.data_ptr(), dpre32.data_ptr(), B * Hb)
             self.linear_wgrad(dpre, Hb, dpre32, Hb, seq.op.bw, N * H, B, Hb, H, wname)
-            if seq.frozen:
-                return
-            g = self.grad_of(seq)
-            if not seq.gw:
-                self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
-                seq.gw = True
-            # rows b*N of the sequence gradient += dpre @ W
-            self.gemm(B, H, Hb, dpre, Hb, ps.w(wname + ".weight").bw, H, b_mn=1, residual=g, ld_res=N * H, out_f32=g, ld_of=N * H)
+            self.pooler_dgrad(seq, N, dpre, wname)
         if not pooled.frozen:
             self.push_bwd(bwd)
         return pooled
+
+    def pooler_dgrad(self, seq, N, dpre, wname):
+        """Backward of a pooler's Linear into its input: rows b*N (token 0 of every sample) of the sequence gradient += dpre @ W,
+        with the sequence gradient zeroed on its first write."""
+        if seq.frozen:
+            return
+        g = self.grad_of(seq)
+        if not seq.gw:
+            self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
+            seq.gw = True
+        B, K = dpre.shape
+        self.gemm(B, seq.H, K, dpre, K, self.ps.w(wname + ".weight").bw, seq.H, b_mn=1, residual=g, ld_res=N * seq.H, out_f32=g,
+                  ld_of=N * seq.H)
 
     def out_grad_buffer(self, name, shape):
         """Static fp32 buffer the caller's d(loss)/d(output) is copied into before backward."""
@@ -1257,9 +1265,22 @@ class Plan:
             if gw_name is None:
                 self.linear_wgrad(dl16, ldp, None, 0, x.op.bw, ld_x, M, N_out, K_in, wname)
             elif self.trainable(gw_name):
-                self.linear_wgrad(dl16, ldp, None, 0, x.op.bw, ld_x, M, N_out, K_in, None, gw=ps.g(gw_name))
+                self.linear_wgrad(dl16, ldp, None, 0, x.op.bw, ld_x, M, N_out, K_in, None, gw=self.grad_view(gw_name))
             return None if x.frozen else (dl16, ldp, W.bw)
         return bwd
+
+    def _wide_bwd(self, head_bwd, hn, tr_bwd, K, N_out):
+        """Backward of a transform + wide decoder head: d(transform output) = d(logits) W, then the transform's backward."""
+        def f():
+            r = head_bwd()
+            if r is None:
+                return
+            dl16, ldp, W16 = r
+            g = self.grad_of(hn)
+            self.gemm(hn.M, K, N_out, dl16, ldp, W16, K, b_mn=1, out_f32=g, ld_of=K)
+            hn.gw = True
+            tr_bwd()
+        return f
 
     def lm_head_compact(self, ht, ht_bwd):
         """Masked-LM head of the fused pre-training objective without the [tokens, vocab] logits: the rows with a label
@@ -1274,11 +1295,7 @@ class Plan:
         self.loss_inputs["masked_lm_labels"] = labels
         idx, cnt, lab_c = self.buf((cap,), torch.int32), self.buf((1,), torch.int32, zero=True), self.buf((cap,), I64)
         self.emit(lib.vb_compact_rows, labels.data_ptr(), -1, M, cap, idx.data_ptr(), cnt.data_ptr(), lab_c.data_ptr())
-        hc = self.buf16((cap, Ht))
-        self.emit(lib.vb_gather_rows16, ht.op.hi.data_ptr(), hc.hi.data_ptr(), self._ptr(ht.op.extra_bw), self._ptr(hc.extra_bw),
-                  idx.data_ptr(), cap, Ht)
-        if hc.lo is not None:
-            self.emit(lib.vb_gather_rows16, ht.op.lo.data_ptr(), hc.lo.data_ptr(), None, None, idx.data_ptr(), cap, Ht)
+        hc = self.gather_rows(ht.op, idx, cap, Ht)
         wn = "bert.embeddings.word_embeddings.weight"
         logits = self.buf((cap, V), F32)
         self.gemm(cap, V, Ht, hc, Ht, ps.w(wn), Ht, bias=ps.p("cls.predictions.bias"), out_f32=logits, ld_of=V)
@@ -1295,7 +1312,7 @@ class Plan:
             if gb is not None:
                 self.colsum(lc["dl32"], V, gb, cap, V)
             if self.trainable(wn):
-                self.linear_wgrad(lc["dl16"], ldp, None, 0, hc.bw, Ht, cap, V, Ht, None, gw=ps.g(wn))
+                self.linear_wgrad(lc["dl16"], ldp, None, 0, hc.bw, Ht, cap, V, Ht, None, gw=self.grad_view(wn))
             if ht.frozen:
                 return
             gc = self.scratch("lm.gc", (cap, Ht), F32)
@@ -1306,6 +1323,15 @@ class Plan:
             ht.gw = True
             ht_bwd()
         return bwd
+
+    def gather_rows(self, src, idx, rows, H):
+        """The rows `idx` (int32 [rows]) of the Operand `src` as a compact Operand: hi with its bf16 copy, and lo."""
+        op = self.buf16((rows, H))
+        self.emit(self.lib.vb_gather_rows16, src.hi.data_ptr(), op.hi.data_ptr(), self._ptr(src.extra_bw), self._ptr(op.extra_bw),
+                  idx.data_ptr(), rows, H)
+        if op.lo is not None:
+            self.emit(self.lib.vb_gather_rows16, src.lo.data_ptr(), op.lo.data_ptr(), None, None, idx.data_ptr(), rows, H)
+        return op
 
     def _lm_loss(self):
         """Where the masked-LM loss lands: the summed scalar, or the first slot of the three-slot pre-training objective."""
@@ -1407,18 +1433,6 @@ class Plan:
         else:
             fused_cls = None
 
-        def wide_bwd(head_bwd, hn, tr_bwd, K, N_out):
-            def f():
-                r = head_bwd()
-                if r is None:
-                    return
-                dl16, ldp, W16 = r        # (r is None when hn takes no gradient)
-                g = self.grad_of(hn)
-                self.gemm(hn.M, K, N_out, dl16, ldp, W16, K, b_mn=1, out_f32=g, ld_of=K)
-                hn.gw = True
-                tr_bwd()
-            return f
-
         # --- cls: masked-LM head (decoder tied to the word embeddings), image-region head, alignment head
         self.lm_c = None
         if want("linguisic_prediction"):
@@ -1435,9 +1449,9 @@ class Plan:
             im_bwd = self.big_head("vision_prediction", hv, Hv, B * Nv, Hv, c.v_target_size, "cls.imagePredictions.decoder",
                                    "cls.imagePredictions.decoder.bias")
         if want("linguisic_prediction"):
-            self.push_bwd(wide_bwd(lm_bwd, ht, ht_bwd, Ht, c.vocab_size) if lm_bwd is not None else lm_compact_bwd)
+            self.push_bwd(self._wide_bwd(lm_bwd, ht, ht_bwd, Ht, c.vocab_size) if lm_bwd is not None else lm_compact_bwd)
         if want("vision_prediction"):
-            self.push_bwd(wide_bwd(im_bwd, hv, hv_bwd, Hv, c.v_target_size))
+            self.push_bwd(self._wide_bwd(im_bwd, hv, hv_bwd, Hv, c.v_target_size))
 
         if self.heads == "pretraining":
             # BertForMultiModalPreTraining returns the alignment score of self.cls (vilbert.py:1497)
@@ -1475,7 +1489,7 @@ class Plan:
                 continue
             hh, hh_bwd = self.transform(fused, nm + ".logit_fc.0", nm + ".logit_fc.2", nm + ".tr")
             head_bwd = self.big_head(nm, hh, 2 * Hb, B, 2 * Hb, n_out, nm + ".logit_fc.3", nm + ".logit_fc.3.bias")
-            self.push_bwd(wide_bwd(head_bwd, hh, hh_bwd, 2 * Hb, n_out))
+            self.push_bwd(self._wide_bwd(head_bwd, hh, hh_bwd, 2 * Hb, n_out))
         if want("vil_logit"):
             self.small_head("vil_logit", fused, "vil_logit", 1)
         if want("vil_tri_prediction"):
@@ -1488,9 +1502,6 @@ class Plan:
 
     # ------------------------------------------------------------------ whole model
     def _build(self):
-        if self.base:
-            self._build_base()
-            return
         c, B = self.cfg, self.B
         self.outputs, self.gout = OrderedDict(), {}
         self.loss_inputs = {}
@@ -1593,9 +1604,13 @@ class Plan:
                       self.vqa_dl16.data_ptr(), _pad8(lg.shape[1]), lg.shape[0], lg.shape[1], 1.0)
         elif self.loss_kind is not None:
             self._emit_loss()
-        # gradients flowing into the BertModel outputs themselves
-        for nm, act in (("sequence_output_t", self.seq_t), ("sequence_output_v", self.seq_v), ("pooled_output_t", self.pooled_t),
-                        ("pooled_output_v", self.pooled_v)):
+        self._emit_backward((("sequence_output_t", self.seq_t), ("sequence_output_v", self.seq_v), ("pooled_output_t", self.pooled_t),
+                             ("pooled_output_v", self.pooled_v)))
+
+    def _emit_backward(self, bert_outputs):
+        """The rest of the backward list: the caller's gradients into the BertModel outputs ((name, Act) pairs), the registered
+        emitters in reverse order, and a join of every stream."""
+        for nm, act in bert_outputs:
             if nm in self.grad_outputs:
                 self.add_grad(act, self.out_grad_buffer(nm, (act.M, act.H)))
         self.sync_streams()
@@ -1610,301 +1625,6 @@ class Plan:
         self.cur.append((None, ("all",), 0))     # join every stream (incl. the weight-gradient side streams)
         self.n_kernels_bwd = sum(1 for op in self.bwd if op[0] is not None)
         self.cur = self.fwd
-
-    # ------------------------------------------------------------------ single-stream baseline (BaseBertForVLTasks)
-    def _build_base(self):
-        """basebert.BertModel.forward + BaseBertForVLTasks.forward (basebert.py:706-774, 923-962): both embeddings LayerNormed into one
-        [B, Nt+Nv, H] stream under the concatenated mask, num_hidden_layers BERT layers over it, the tanh pooler on row 0 and the seven
-        heads. The wide heads (masked-LM, region classes) read their rows gathered into compact operands and scatter their gradient
-        back; the 1-output heads run over the whole stream with a zero output gradient on the rows they do not return."""
-        c, B = self.cfg, self.B
-        self.outputs, self.gout = OrderedDict(), {}
-        self.loss_inputs, self.head_grad = {}, {}
-        self.loss = self.score = self.preds = None
-        self.N = self.Nt + self.Nv
-        self._scatter_ok = False
-        x = self.base_embeddings()
-        self.enc = []
-        for i in range(c.num_hidden_layers):
-            x = self.base_layer(x, i)
-            self.enc.append(x)
-        self.seq = x
-        self.pooled = self.base_pooler(x)
-        self.outputs["sequence_output"] = x.f32.view(B, self.N, -1)
-        self.outputs["pooled_output"] = self.pooled.f32
-        self.out_rg["sequence_output"] = not x.frozen
-        self.out_rg["pooled_output"] = not self.pooled.frozen
-        views = self.build_base_heads(x, self.pooled) if self.heads == "base" else {}
-        self.n_kernels_fwd = sum(1 for op in self.fwd if op[0] is not None)
-
-        self.cur = self.bwd
-        for nm, act in (("sequence_output", self.seq), ("pooled_output", self.pooled)):
-            if nm in self.grad_outputs:
-                self.add_grad(act, self.out_grad_buffer(nm, (act.M, act.H)))
-        self.sync_streams()
-        for entry in reversed(self._bwd_emitters):
-            if entry is None:
-                self.sync_streams()
-            else:
-                self.sid, emitter = entry
-                self._scratch_epoch += 1
-                emitter()
-        self.sid = 0
-        self.cur.append((None, ("all",), 0))
-        self.n_kernels_bwd = sum(1 for op in self.bwd if op[0] is not None)
-        self.cur = self.fwd
-        self.gout.update(views)      # the 1-output heads take their caller's gradient into their rows of the whole-stream buffer
-
-    def base_embeddings(self):
-        """BertEmbeddings + BertImageEmbeddings + torch.cat (basebert.py:284-359, 718-747). The region side (feature cast, box
-        projection, 2048 -> H GEMM) runs on the second stream under the text gather; vb_concat_embed_ln_fwd adds the image token-type
-        row, applies both LayerNorms and dropouts and writes the stream with its operand copies."""
-        ps, c, B, lib = self.ps, self.cfg, self.B, self.lib
-        H, Nt, Nv, Fv = c.hidden_size, self.Nt, self.Nv, BASE_FEATURE_SIZE
-        Mt, Mv, M = B * Nt, B * Nv, B * self.N
-        self.in_ids = self.buf((B, Nt), I64, zero=True)
-        self.in_tt = self.buf((B, Nt), I64, zero=True)
-        self.in_task = None
-        self.in_amask = self.buf((B, Nt), I64, zero=True)
-        self.in_imask = self.buf((B, Nv), I64, zero=True)
-        self.in_feat = self.buf((B, Nv, Fv), F32, zero=True)
-        self.in_loc = self.buf((B, Nv, 5), F32, zero=True)
-        self.mask = self.buf((B, self.N), F32)
-        self.emit(lib.vb_mask_concat_additive, self.in_amask.data_ptr(), self.in_imask.data_ptr(), self.mask.data_ptr(), B, Nt, Nv)
-        self.sync_streams()      # the second stream reads the inputs that load_inputs copied on the main stream
-        e, ie = "bert.embeddings", "bert.image_embeddings"
-        t_tables = [e + n for n in (".word_embeddings.weight", ".position_embeddings.weight", ".token_type_embeddings.weight")]
-        xt = self.buf((Mt, H), F32)
-        self.emit(lib.vb_embed_text_fwd, self.in_ids.data_ptr(), self.in_tt.data_ptr(), None, *[ps.p(n).data_ptr() for n in t_tables], None,
-                  xt.data_ptr(), B, Nt, H)
-        with self.on(1):
-            feat = self.buf16((Mv, Fv))
-            hi, lo, bw = feat.ptrs()
-            self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), hi, Mv * Fv, feat.fp16, lo, bw)
-            locp = self.buf((Mv, H), F32)
-            self.emit(lib.vb_loc_proj_fwd, self.in_loc.data_ptr(), ps.p(ie + ".image_location_embeddings.weight").data_ptr(),
-                      ps.p(ie + ".image_location_embeddings.bias").data_ptr(), locp.data_ptr(), Mv, H)
-            xv = self.buf((Mv, H), F32)
-            self.gemm(Mv, H, Fv, feat, Fv, ps.w(ie + ".image_embeddings.weight"), Fv, bias=ps.p(ie + ".image_embeddings.bias"),
-                      residual=locp, ld_res=H, out_f32=xv, ld_of=H)
-        self.sync_streams()
-        trow = ps.p(ie + ".token_type_embeddings.weight")[1]
-        tdrop = self.drop(e + ".dropout", c.hidden_dropout_prob)
-        vdrop = self.drop(ie + ".dropout", c.hidden_dropout_prob)
-        y32, y = self.buf((M, H), F32), self.buf16((M, H))
-        mean, rstd = self.buf((M,), F32), self.buf((M,), F32)
-        lnt, lnv = e + ".LayerNorm", ie + ".LayerNorm"
-        self.emit(lib.vb_concat_embed_ln_fwd, xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
-                  ps.p(lnt + ".bias").data_ptr(), ps.p(lnv + ".weight").data_ptr(), ps.p(lnv + ".bias").data_ptr(), y32.data_ptr(), *y.ptrs(),
-                  y.fp16, mean.data_ptr(), rstd.data_ptr(), B, Nt, Nv, H, self._ref(tdrop), self._ref(vdrop))
-        x = Act(y32, y, M, H)
-        img = [ie + n for n in (".image_embeddings.weight", ".image_embeddings.bias", ".token_type_embeddings.weight",
-                                ".image_location_embeddings.weight", ".image_location_embeddings.bias")]
-        lns = [lnt + ".weight", lnt + ".bias", lnv + ".weight", lnv + ".bias"]
-        x.frozen = not self.trainable(*t_tables, *img, *lns)
-
-        def bwd():
-            if not x.gw:
-                return
-            gt = [self.pg(n) for n in t_tables]
-            dxt = self.scratch("emb.dxt", (Mt, H), F32) if any(g is not None for g in gt) else None
-            img_w = self.trainable(ie + ".image_embeddings.weight")
-            loc = (self.pg(img[3]), self.pg(img[4]))
-            dxv32 = self.scratch("emb.dxv32", (Mv, H), F32) if (loc[0] is not None or loc[1] is not None) else None
-            dxv16 = self.scratch("emb.dxv16", (Mv, H), BF16) if img_w else None
-            gtype = self.pg(img[2])
-            self.emit(lib.vb_concat_embed_ln_bwd, x.g32.data_ptr(), xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
-                      ps.p(lnv + ".weight").data_ptr(), mean.data_ptr(), rstd.data_ptr(), self._ptr(dxt), self._ptr(dxv32), self._ptr(dxv16),
-                      *[self._ptr(self.pg(n)) for n in lns], self._ptr(self.pg(img[1])), None if gtype is None else gtype[1].data_ptr(),
-                      B, Nt, Nv, H, self._ref(tdrop), self._ref(vdrop))
-            if dxt is not None:
-                self.emit(lib.vb_embed_text_bwd_padded, dxt.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), *[self._ptr(g) for g in gt],
-                          B, Nt, H)
-            if dxv16 is not None:
-                self.linear_wgrad(dxv16, H, None, 0, feat.bw, Fv, Mv, H, Fv, ie + ".image_embeddings")
-            if dxv32 is not None:
-                self.emit(lib.vb_loc_proj_bwd, dxv32.data_ptr(), self.in_loc.data_ptr(), self._ptr(loc[0]), self._ptr(loc[1]), Mv, H)
-        if not x.frozen:
-            self.push_bwd(bwd)
-        return x
-
-    def base_layer(self, x, i):
-        """basebert.BertLayer over the whole stream at N = Nt + Nv with the concatenated mask (basebert.py:480-485)."""
-        p, c = f"bert.encoder.layer.{i}", self.cfg
-        h1 = self.self_attention_block(x, self.B, self.N, c.num_attention_heads, self.mask, p + ".attention", "t",
-                                       p_attn=c.attention_probs_dropout_prob, p_hidden=c.hidden_dropout_prob)
-        return self.ffn(h1, c.intermediate_size, p + ".intermediate.dense", p + ".output.dense", p + ".output.LayerNorm", "t.ffn",
-                        drop=self.drop(p + ".output.dropout", c.hidden_dropout_prob))
-
-    def base_pooler(self, seq):
-        """BertPooler (basebert.py:507-519): Linear on row 0 of every sample (A read with row pitch N*H), then tanh."""
-        ps, B, H, N, w = self.ps, self.B, seq.H, self.N, "bert.pooler.dense"
-        pre = self.buf((B, H), F32)
-        self.gemm(B, H, H, seq.op, N * H, ps.w(w + ".weight"), H, bias=ps.p(w + ".bias"), out_f32=pre, ld_of=H)
-        y32, y = self.buf((B, H), F32), self.buf16((B, H))
-        self.emit(self.lib.vb_tanh_fwd, pre.data_ptr(), y32.data_ptr(), *y.ptrs(), y.fp16, B * H)
-        pooled = Act(y32, y, B, H)
-        pooled.frozen = seq.frozen and not self.trainable(w + ".weight", w + ".bias")
-
-        def bwd():
-            if not pooled.gw:
-                return
-            dpre = self.scratch("pool.dpre", (B, H), BF16)
-            self.emit(self.lib.vb_tanh_bwd, pooled.g32.data_ptr(), y32.data_ptr(), dpre.data_ptr(), self._ptr(self.pg(w + ".bias")), B, H)
-            self.linear_wgrad(dpre, H, None, 0, seq.op.bw, N * H, B, H, H, w)
-            if seq.frozen:
-                return
-            g = self.grad_of(seq)
-            if not seq.gw:
-                self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
-                seq.gw = True
-            self.gemm(B, H, H, dpre, H, ps.w(w + ".weight").bw, H, b_mn=1, residual=g, ld_res=N * H, out_f32=g, ld_of=N * H)
-        if not pooled.frozen:
-            self.push_bwd(bwd)
-        return pooled
-
-    def base_rows(self, seq, a, b, tag):
-        """Rows [a, b) of every sample of the stream as a compact Act (operand copies: the head transform reads nothing else). Its
-        backward scatters the compact gradient into those rows of the stream gradient."""
-        lib, B, N, H = self.lib, self.B, self.N, seq.H
-        n = b - a
-        idx = self.buf((B * n,), torch.int32, zero=True)
-        idx.copy_((torch.arange(B).view(B, 1) * N + torch.arange(a, b).view(1, n)).reshape(-1).to(torch.int32))
-        op = self.buf16((B * n, H))
-        self.emit(lib.vb_gather_rows16, seq.op.hi.data_ptr(), op.hi.data_ptr(), self._ptr(seq.op.extra_bw), self._ptr(op.extra_bw), idx.data_ptr(),
-                  B * n, H)
-        if op.lo is not None:
-            self.emit(lib.vb_gather_rows16, seq.op.lo.data_ptr(), op.lo.data_ptr(), None, None, idx.data_ptr(), B * n, H)
-        rows = Act(None, op, B * n, H)
-        rows.frozen = seq.frozen
-
-        def bwd():
-            if not rows.gw:
-                return
-            g = self.grad_of(seq)
-            if not seq.gw:      # the gathered heads' backward runs first: zero the stream gradient once, then scatter disjoint rows
-                self.emit(lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
-                seq.gw = self._scatter_ok = True
-            if self._scatter_ok:
-                self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), g.data_ptr(), idx.data_ptr(), B * n, H, None, None)
-                return
-            full = self.scratch(tag + ".full", (B * N, H), F32)      # the stream gradient already holds other contributions
-            self.emit(lib.vb_memset_zero, full.data_ptr(), full.numel() * 4)
-            self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), full.data_ptr(), idx.data_ptr(), B * n, H, None, None)
-            self.emit(lib.vb_axpy_f32, full.data_ptr(), g.data_ptr(), full.numel(), 1.0)
-        if not seq.frozen:
-            self.push_bwd(bwd)
-        return rows
-
-    def _wide_bwd(self, head_bwd, hn, tr_bwd, K, N_out):
-        """Backward of a transform + wide decoder head: d(transform output) = d(logits) W, then the transform's backward."""
-        def f():
-            r = head_bwd()
-            if r is None:
-                return
-            dl16, ldp, W16 = r
-            g = self.grad_of(hn)
-            self.gemm(hn.M, K, N_out, dl16, ldp, W16, K, b_mn=1, out_f32=g, ld_of=K)
-            hn.gw = True
-            tr_bwd()
-        return f
-
-    def base_simple_classifier(self, x):
-        """vil_prediction = SimpleClassifier (basebert.py:965-978): weight_norm(Linear(H, 2H), dim=None) -> ReLU -> Dropout(0.5) ->
-        weight_norm(Linear(2H, num_labels), dim=None) on the pooled output. Like the reference's weight_norm pre-forward hook, every
-        forward first derives both weights from (g, v) (vb_weight_norm_fwd: fp32 and the operand copies), so a parameter update by
-        any optimizer is picked up without a separate refresh. The dropout sits in the first GEMM's epilogue after the ReLU; its
-        backward folds the 1 / (1 - p) scale into the dgrad GEMM and gates by the dropped output."""
-        ps, lib, B, H, Lb = self.ps, self.lib, self.B, x.H, self.ps.num_labels
-        H2 = 2 * H
-        W, self.wn_weights = {}, {}
-        for i in (0, 3):
-            nm = f"vil_prediction.main.{i}"
-            v, g = ps.p(nm + ".weight_v"), ps.p(nm + ".weight_g")
-            w32, op = self.buf(tuple(v.shape), F32), self.buf16(tuple(v.shape))
-            scr = self.buf((L.VB_WEIGHT_NORM_SCRATCH // 8,), torch.float64)
-            self.emit(lib.vb_weight_norm_fwd, v.data_ptr(), g.data_ptr(), v.numel(), w32.data_ptr(), *op.ptrs(), op.fp16, scr.data_ptr())
-            W[i] = (nm, v, g, op, scr)
-            self.wn_weights[nm] = w32
-        p_drop = 0.5
-        drop = self.drop("vil_prediction.main.2", p_drop)
-        h32, h = self.buf((B, H2), F32), self.buf16((B, H2))
-        self.gemm(B, H2, H, x.op, H, W[0][3], H, bias=ps.p("vil_prediction.main.0.bias"), act=L.VB_ACT_RELU, out_f32=h32, ld_of=H2,
-                  out_bf16=h, ld_ob=H2, dropout=drop)
-        logits = self.buf((B, Lb), F32)
-        self.gemm(B, Lb, H2, h, H2, W[3][3], H2, bias=ps.p("vil_prediction.main.3.bias"), out_f32=logits, ld_of=Lb)
-        self.outputs["vil_prediction"] = logits
-        part = lambda i: [f"vil_prediction.main.{i}.{s}" for s in ("weight_g", "weight_v", "bias")]
-        h_rg = not x.frozen or self.trainable(*part(0))
-        self.out_rg["vil_prediction"] = h_rg or self.trainable(*part(3))
-        scale = 1.0 / (1.0 - p_drop) if drop is not None else 1.0
-
-        def wn_wgrad(i, dy16, ld_dy, x16, ld_x, M, N_out, K_in):
-            nm, v, g, _, scr = W[i]
-            gg, gv = self.pg(nm + ".weight_g"), self.pg(nm + ".weight_v")
-            if gg is None and gv is None:
-                return
-            dw = self.scratch(f"vilp.dw{i}", (N_out, K_in), F32)
-            self.emit(lib.vb_memset_zero, dw.data_ptr(), dw.numel() * 4)
-            self.gemm(N_out, K_in, M, dy16, ld_dy, x16, ld_x, a_mn=1, b_mn=1, out_f32=dw, ld_of=K_in, atomic=1, split_k=0)
-            self.emit(lib.vb_weight_norm_bwd, dw.data_ptr(), v.data_ptr(), g.data_ptr(), v.numel(), self._ptr(gg), self._ptr(gv), scr.data_ptr())
-
-        def bwd():
-            if "vil_prediction" not in self.grad_outputs:
-                return
-            ldp = _pad8(Lb)
-            dl32 = self.out_grad_buffer("vil_prediction", (B, Lb))
-            dl16 = self.scratch("vilp.dl16", (B, ldp), BF16)
-            self.emit(lib.vb_cast2d_f32_to_bf16, dl32.data_ptr(), Lb, dl16.data_ptr(), ldp, B, Lb, 1.0)
-            gb = self.pg("vil_prediction.main.3.bias")
-            if gb is not None:
-                self.colsum(dl32, Lb, gb, B, Lb)
-            wn_wgrad(3, dl16, ldp, h.bw, H2, B, Lb, H2)
-            if not h_rg:
-                return
-            dh = self.scratch("vilp.dh32", (B, H2), F32)
-            self.gemm(B, H2, Lb, dl16, ldp, W[3][3].bw, H2, b_mn=1, out_f32=dh, ld_of=H2, alpha=scale)
-            dpre16, dpre32 = self.scratch("vilp.dpre16", (B, H2), BF16), self.scratch("vilp.dpre32", (B, H2), F32)
-            self.emit(lib.vb_relu_bwd, dh.data_ptr(), h32.data_ptr(), dpre16.data_ptr(), dpre32.data_ptr(), B * H2)
-            gb = self.pg("vil_prediction.main.0.bias")
-            if gb is not None:
-                self.colsum(dpre32, H2, gb, B, H2)
-            wn_wgrad(0, dpre16, H2, x.op.bw, H, B, H2, H)
-            self.dgrad_into(x, dpre16, H2, W[0][3].bw, B, H2, H)
-        if self.out_rg["vil_prediction"]:
-            self.push_bwd(bwd)
-
-    def build_base_heads(self, seq, pooled):
-        """The seven outputs of BaseBertForVLTasks.forward (basebert.py:929-962). Returns the views of the whole-stream output-gradient
-        buffers that the caller's gradients of the 1-output heads go into. Emission order is chosen for the backward, which runs it
-        in reverse: the gathered heads first (their scatters are the first writes to the stream gradient), then the 1-output heads
-        over the stream and the pooled heads (which accumulate), then the pooler."""
-        ps, c, B = self.ps, self.cfg, self.B
-        H, Nt, Nv, N = seq.H, self.Nt, self.Nv, self.N
-        self.base_simple_classifier(pooled)
-        self.small_head("vil_logit", pooled, "vil_logit", 1)
-        self.small_head("vil_binary_prediction", pooled, "cls.seq_relationship", 2)
-        views = {}
-        # self.dropout is one nn.Dropout called twice (basebert.py:949-952): two sites, each a mask over the whole stream
-        for name, site, a, b in (("vision_logit", "dropout.seq_v", Nt, N), ("linguisic_logit", "dropout.seq_t", 0, Nt)):
-            full = self.out_grad_buffer(name, (B * N, 1))
-            self.small_head(name, seq, name, 1, addend=self.mask if name == "vision_logit" else None,
-                            in_drop=self.drop(site, self.head_dropout_prob))
-            self.outputs[name] = self.outputs[name].view(B, N, 1)[:, a:b]
-            views[name] = full.view(B, N, 1)[:, a:b]
-        rows_t = self.base_rows(seq, 0, Nt, "rows.t")
-        rows_v = self.base_rows(seq, Nt, N, "rows.v")
-        wn = "bert.embeddings.word_embeddings.weight"
-        ht, ht_bwd = self.transform(rows_t, "cls.predictions.transform.dense", "cls.predictions.transform.LayerNorm", "lm.tr")
-        lm_bwd = self.big_head("linguisic_prediction", ht, H, B * Nt, H, c.vocab_size, None, "cls.predictions.bias", w=ps.w(wn), gw_name=wn)
-        hv, hv_bwd = self.transform(rows_v, "cls.imagePredictions.transform.dense", "cls.imagePredictions.transform.LayerNorm", "im.tr")
-        im_bwd = self.big_head("vision_prediction", hv, H, B * Nv, H, BASE_REGION_CLASSES, "cls.imagePredictions.decoder",
-                               "cls.imagePredictions.decoder.bias")
-        self.push_bwd(self._wide_bwd(lm_bwd, ht, ht_bwd, H, c.vocab_size))
-        self.push_bwd(self._wide_bwd(im_bwd, hv, hv_bwd, H, BASE_REGION_CLASSES))
-        self.outputs["linguisic_prediction"] = self.outputs["linguisic_prediction"].view(B, Nt, -1)
-        self.outputs["vision_prediction"] = self.outputs["vision_prediction"].view(B, Nv, -1)
-        return views
 
     def attention_export(self):
         """The reference's all_attention_mask triple (BertEncoder.forward, vilbert.py:1098-1107) for config.visualization: lists of
@@ -2178,9 +1898,16 @@ class Plan:
         counts as a forward of this plan there."""
         if not self.image_prefix:
             raise ValueError("run_image_prefix: the plan was built without image_prefix=True")
+        self._claim_forward(writes_grad=False)
+        self._run(self.prefix)
+
+    def _claim_forward(self, writes_grad):
+        """Every run of forward ops starts here: a new forward id, whose activations the shared arena now holds (holds_forward),
+        and with writes_grad (the run includes the backward) a flat gradient buffer that is no longer known to be zero."""
         self.fwd_id += 1
         self.e.arena_owner = (self, self.fwd_id)
-        self._run(self.prefix)
+        if writes_grad:
+            self.e.grad_clean = False
 
     def _run(self, ops):
         """Issues the ops on their streams. Markers: (None, ()) = barrier between the text and vision streams;
@@ -2218,8 +1945,7 @@ class Plan:
                 check(st, fn.__name__)
 
     def run_forward(self):
-        self.fwd_id += 1
-        self.e.arena_owner = (self, self.fwd_id)
+        self._claim_forward(writes_grad=False)
         if self.graph_fwd is not None:
             self.graph_fwd.replay()
         else:
@@ -2248,16 +1974,31 @@ class Plan:
         ~600 ctypes launches of a step become two graph replays."""
         if self.graph_fwd is None and self._eager_runs[0] >= after:
             torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._run(self.fwd)
-            self.graph_fwd = g
+            self.graph_fwd = self._record(self.fwd)
         if self.graph_bwd is None and self._eager_runs[1] >= after:
             torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._run(self.bwd)
-            self.graph_bwd = g
+            self.graph_bwd = self._record(self.bwd)
+
+    def _record(self, *op_lists):
+        """One CUDA graph of the op lists, issued one after the other."""
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            for ops in op_lists:
+                self._run(ops)
+        return g
+
+    def _warm_up(self, *op_lists):
+        """Runs the op lists once on a side stream before a capture (module load, shared-memory attributes). It runs the forward
+        and the backward: a step of this plan."""
+        self._claim_forward(writes_grad=True)
+        torch.cuda.synchronize()
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            for ops in op_lists:
+                self._run(ops)
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
 
     def enable_training_prologue(self, zero_grad=True, refresh_weights=True):
         """Makes run_step a complete training-step body: bump the dropout step counter (train mode), zero the flat
@@ -2304,9 +2045,7 @@ class Plan:
 
     def run_step(self):
         """(prologue) + forward + (loss) + backward (+ epilogue); gradients accumulate into ParamStore.grad."""
-        self.fwd_id += 1
-        self.e.arena_owner = (self, self.fwd_id)
-        self.e.grad_clean = False
+        self._claim_forward(writes_grad=True)
         if self.graph_step is not None:
             self.graph_step.replay()
         else:
@@ -2382,22 +2121,10 @@ class Plan:
         """Captures the step as CUDA graphs, one per backward piece of ddp_segments (graph 0 = prologue + forward + first
         backward piece), for the data-parallel step: see run_step_overlapped."""
         self.segments = self.ddp_segments(n_segments, tail_cut=tail_cut)
-        torch.cuda.synchronize()
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            self._run(self.prologue); self._run(self.fwd); self._run(self.bwd)
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
+        self._warm_up(self.prologue, self.fwd, self.bwd)
         barrier = [(None, ("all",), 0)]
-        self.segment_graphs = []
-        for i, (lo, hi, _, _) in enumerate(self.segments):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                if i == 0:
-                    self._run(self.prologue); self._run(self.fwd)
-                self._run(barrier + self.bwd[lo:hi] + barrier)
-            self.segment_graphs.append(g)
+        self.segment_graphs = [self._record(*([self.prologue, self.fwd] if i == 0 else []), barrier + self.bwd[lo:hi] + barrier)
+                               for i, (lo, hi, _, _) in enumerate(self.segments)]
         torch.cuda.synchronize()
 
     def live_ranges(self, lo, hi):
@@ -2446,9 +2173,7 @@ class Plan:
         torch.cuda.synchronize()
 
     def run_step_ddp(self):
-        self.fwd_id += 1
-        self.e.arena_owner = (self, self.fwd_id)
-        self.e.grad_clean = False
+        self._claim_forward(writes_grad=True)
         self.graph_step_ddp.replay()
 
     def run_step_overlapped(self, allreduce_range, comm_stream, skip_dead=True):
@@ -2458,8 +2183,7 @@ class Plan:
         Returns the list of whatever allreduce_range returned (async work handles). No epilogue runs here: a caller that
         launches the optimizer afterwards must first wait for these collectives, and with max_grad_norm so must the gradient
         norm, which is to be taken of the averaged gradient."""
-        self.fwd_id += 1
-        self.e.grad_clean = False
+        self._claim_forward(writes_grad=True)
         main = torch.cuda.current_stream()
         works = []
         for g, (_, _, lo, hi) in zip(self.segment_graphs, self.segments):
@@ -2481,30 +2205,272 @@ class Plan:
 
     def capture(self, separate=False):
         """Captures the plan into CUDA graphs (one for the whole step, or one per pass)."""
-        torch.cuda.synchronize()
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):   # warm-up outside capture (module load, smem attribute calls)
-            self._run(self.prologue)
-            self._run(self.fwd)
-            self._run(self.bwd)
-            self._run(self.epilogue)
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
+        self._warm_up(self.prologue, self.fwd, self.bwd, self.epilogue)
         if separate:
-            self.graph_fwd, self.graph_bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph_fwd):
-                self._run(self.fwd)
-            with torch.cuda.graph(self.graph_bwd):
-                self._run(self.bwd)
+            self.graph_fwd, self.graph_bwd = self._record(self.fwd), self._record(self.bwd)
         else:
-            self.graph_step = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph_step):
-                self._run(self.prologue)
-                self._run(self.fwd)
-                self._run(self.bwd)
-                self._run(self.epilogue)
+            self.graph_step = self._record(self.prologue, self.fwd, self.bwd, self.epilogue)
         torch.cuda.synchronize()
+
+
+class BasePlan(Plan):
+    """Plan of the single-stream baseline BaseBertForVLTasks (heads "base" / "base_none"; vilbert/basebert.py). It has none of the
+    two-stream options (batch pairs, task token, fast mode, gate, attention export), and its plans take grad_outputs, train and
+    frozen only: no fused objective, outputs= selection or image prefix."""
+
+    def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
+                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset()):
+        if (vqa_loss or loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
+                or loss_in_forward):
+            raise ValueError("single-stream baseline plans support grad_outputs, train and frozen only")
+        super().__init__(engine, B, Nt, Nv, grad_outputs, heads=heads, train=train, choices=choices, frozen=frozen)
+
+    def _stream_modes(self, B, Nt, Nv, *_):
+        self.pairs = self.has_task = self.viz = self.dyn = self.fast = self.image_prefix = False
+        self.B, self.Nt_in, self.Nt, self.Nv, self.Bt = B, Nt, Nt, Nv, B
+
+    def _build(self):
+        """basebert.BertModel.forward + BaseBertForVLTasks.forward (basebert.py:706-774, 923-962): both embeddings LayerNormed into one
+        [B, Nt+Nv, H] stream under the concatenated mask, num_hidden_layers BERT layers over it, the tanh pooler on row 0 and the seven
+        heads. The wide heads (masked-LM, region classes) read their rows gathered into compact operands and scatter their gradient
+        back; the 1-output heads run over the whole stream with a zero output gradient on the rows they do not return."""
+        c, B = self.cfg, self.B
+        self.outputs, self.gout = OrderedDict(), {}
+        self.loss_inputs, self.head_grad = {}, {}
+        self.loss = self.score = self.preds = None
+        self.N = self.Nt + self.Nv
+        self._scatter_ok = False
+        x = self.base_embeddings()
+        self.enc = []
+        for i in range(c.num_hidden_layers):
+            x = self.base_layer(x, i)
+            self.enc.append(x)
+        self.seq = x
+        self.pooled = self.base_pooler(x)
+        self.outputs["sequence_output"] = x.f32.view(B, self.N, -1)
+        self.outputs["pooled_output"] = self.pooled.f32
+        self.out_rg["sequence_output"] = not x.frozen
+        self.out_rg["pooled_output"] = not self.pooled.frozen
+        views = self.build_base_heads(x, self.pooled) if self.heads == "base" else {}
+        self.n_kernels_fwd = sum(1 for op in self.fwd if op[0] is not None)
+
+        self.cur = self.bwd
+        self._emit_backward((("sequence_output", self.seq), ("pooled_output", self.pooled)))
+        self.gout.update(views)      # the 1-output heads take their caller's gradient into their rows of the whole-stream buffer
+
+    def base_embeddings(self):
+        """BertEmbeddings + BertImageEmbeddings + torch.cat (basebert.py:284-359, 718-747). The region side (feature cast, box
+        projection, 2048 -> H GEMM) runs on the second stream under the text gather; vb_concat_embed_ln_fwd adds the image token-type
+        row, applies both LayerNorms and dropouts and writes the stream with its operand copies."""
+        ps, c, B, lib = self.ps, self.cfg, self.B, self.lib
+        H, Nt, Nv, Fv = c.hidden_size, self.Nt, self.Nv, BASE_FEATURE_SIZE
+        Mt, Mv, M = B * Nt, B * Nv, B * self.N
+        self.in_ids = self.buf((B, Nt), I64, zero=True)
+        self.in_tt = self.buf((B, Nt), I64, zero=True)
+        self.in_task = None
+        self.in_amask = self.buf((B, Nt), I64, zero=True)
+        self.in_imask = self.buf((B, Nv), I64, zero=True)
+        self.in_feat = self.buf((B, Nv, Fv), F32, zero=True)
+        self.in_loc = self.buf((B, Nv, 5), F32, zero=True)
+        self.mask = self.buf((B, self.N), F32)
+        self.emit(lib.vb_mask_concat_additive, self.in_amask.data_ptr(), self.in_imask.data_ptr(), self.mask.data_ptr(), B, Nt, Nv)
+        self.sync_streams()      # the second stream reads the inputs that load_inputs copied on the main stream
+        e, ie = "bert.embeddings", "bert.image_embeddings"
+        t_tables = [e + n for n in (".word_embeddings.weight", ".position_embeddings.weight", ".token_type_embeddings.weight")]
+        xt = self.buf((Mt, H), F32)
+        self.emit(lib.vb_embed_text_fwd, self.in_ids.data_ptr(), self.in_tt.data_ptr(), None, *[ps.p(n).data_ptr() for n in t_tables], None,
+                  xt.data_ptr(), B, Nt, H)
+        with self.on(1):
+            xv, feat = self.image_embedding(ie, H)
+        self.sync_streams()
+        trow = ps.p(ie + ".token_type_embeddings.weight")[1]
+        tdrop = self.drop(e + ".dropout", c.hidden_dropout_prob)
+        vdrop = self.drop(ie + ".dropout", c.hidden_dropout_prob)
+        y32, y = self.buf((M, H), F32), self.buf16((M, H))
+        mean, rstd = self.buf((M,), F32), self.buf((M,), F32)
+        lnt, lnv = e + ".LayerNorm", ie + ".LayerNorm"
+        self.emit(lib.vb_concat_embed_ln_fwd, xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
+                  ps.p(lnt + ".bias").data_ptr(), ps.p(lnv + ".weight").data_ptr(), ps.p(lnv + ".bias").data_ptr(), y32.data_ptr(), *y.ptrs(),
+                  y.fp16, mean.data_ptr(), rstd.data_ptr(), B, Nt, Nv, H, self._ref(tdrop), self._ref(vdrop))
+        x = Act(y32, y, M, H)
+        img = [ie + n for n in (".image_embeddings.weight", ".image_embeddings.bias", ".token_type_embeddings.weight",
+                                ".image_location_embeddings.weight", ".image_location_embeddings.bias")]
+        lns = [lnt + ".weight", lnt + ".bias", lnv + ".weight", lnv + ".bias"]
+        x.frozen = not self.trainable(*t_tables, *img, *lns)
+
+        def bwd():
+            if not x.gw:
+                return
+            gt = [self.pg(n) for n in t_tables]
+            dxt = self.scratch("emb.dxt", (Mt, H), F32) if any(g is not None for g in gt) else None
+            dxv32 = self.scratch("emb.dxv32", (Mv, H), F32) if self.trainable(img[3], img[4]) else None
+            dxv16 = self.scratch("emb.dxv16", (Mv, H), BF16) if self.trainable(img[0]) else None
+            gtype = self.pg(img[2])
+            self.emit(lib.vb_concat_embed_ln_bwd, x.g32.data_ptr(), xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
+                      ps.p(lnv + ".weight").data_ptr(), mean.data_ptr(), rstd.data_ptr(), self._ptr(dxt), self._ptr(dxv32), self._ptr(dxv16),
+                      *[self._ptr(self.pg(n)) for n in lns], self._ptr(self.pg(img[1])), None if gtype is None else gtype[1].data_ptr(),
+                      B, Nt, Nv, H, self._ref(tdrop), self._ref(vdrop))
+            if dxt is not None:
+                self.emit(lib.vb_embed_text_bwd_padded, dxt.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), *[self._ptr(g) for g in gt],
+                          B, Nt, H)
+            self.image_embedding_bwd(ie, H, feat, dxv16, dxv32)
+        if not x.frozen:
+            self.push_bwd(bwd)
+        return x
+
+    def base_layer(self, x, i):
+        """basebert.BertLayer over the whole stream at N = Nt + Nv with the concatenated mask (basebert.py:480-485)."""
+        p, c = f"bert.encoder.layer.{i}", self.cfg
+        h1 = self.self_attention_block(x, self.B, self.N, c.num_attention_heads, self.mask, p + ".attention", "t",
+                                       p_attn=c.attention_probs_dropout_prob, p_hidden=c.hidden_dropout_prob)
+        return self.ffn(h1, c.intermediate_size, p + ".intermediate.dense", p + ".output.dense", p + ".output.LayerNorm", "t.ffn",
+                        drop=self.drop(p + ".output.dropout", c.hidden_dropout_prob))
+
+    def base_pooler(self, seq):
+        """BertPooler (basebert.py:507-519): Linear on row 0 of every sample (A read with row pitch N*H), then tanh."""
+        ps, B, H, N, w = self.ps, self.B, seq.H, self.N, "bert.pooler.dense"
+        pre = self.buf((B, H), F32)
+        self.gemm(B, H, H, seq.op, N * H, ps.w(w + ".weight"), H, bias=ps.p(w + ".bias"), out_f32=pre, ld_of=H)
+        y32, y = self.buf((B, H), F32), self.buf16((B, H))
+        self.emit(self.lib.vb_tanh_fwd, pre.data_ptr(), y32.data_ptr(), *y.ptrs(), y.fp16, B * H)
+        pooled = Act(y32, y, B, H)
+        pooled.frozen = seq.frozen and not self.trainable(w + ".weight", w + ".bias")
+
+        def bwd():
+            if not pooled.gw:
+                return
+            dpre = self.scratch("pool.dpre", (B, H), BF16)
+            self.emit(self.lib.vb_tanh_bwd, pooled.g32.data_ptr(), y32.data_ptr(), dpre.data_ptr(), self._ptr(self.pg(w + ".bias")), B, H)
+            self.linear_wgrad(dpre, H, None, 0, seq.op.bw, N * H, B, H, H, w)
+            self.pooler_dgrad(seq, N, dpre, w)
+        if not pooled.frozen:
+            self.push_bwd(bwd)
+        return pooled
+
+    def base_rows(self, seq, a, b, tag):
+        """Rows [a, b) of every sample of the stream as a compact Act (operand copies: the head transform reads nothing else). Its
+        backward scatters the compact gradient into those rows of the stream gradient."""
+        lib, B, N, H = self.lib, self.B, self.N, seq.H
+        n = b - a
+        idx = self.buf((B * n,), torch.int32, zero=True)
+        idx.copy_((torch.arange(B).view(B, 1) * N + torch.arange(a, b).view(1, n)).reshape(-1).to(torch.int32))
+        rows = Act(None, self.gather_rows(seq.op, idx, B * n, H), B * n, H)
+        rows.frozen = seq.frozen
+
+        def bwd():
+            if not rows.gw:
+                return
+            g = self.grad_of(seq)
+            if not seq.gw:      # the gathered heads' backward runs first: zero the stream gradient once, then scatter disjoint rows
+                self.emit(lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
+                seq.gw = self._scatter_ok = True
+            if self._scatter_ok:
+                self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), g.data_ptr(), idx.data_ptr(), B * n, H, None, None)
+                return
+            full = self.scratch(tag + ".full", (B * N, H), F32)      # the stream gradient already holds other contributions
+            self.emit(lib.vb_memset_zero, full.data_ptr(), full.numel() * 4)
+            self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), full.data_ptr(), idx.data_ptr(), B * n, H, None, None)
+            self.emit(lib.vb_axpy_f32, full.data_ptr(), g.data_ptr(), full.numel(), 1.0)
+        if not seq.frozen:
+            self.push_bwd(bwd)
+        return rows
+
+    def base_simple_classifier(self, x):
+        """vil_prediction = SimpleClassifier (basebert.py:965-978): weight_norm(Linear(H, 2H), dim=None) -> ReLU -> Dropout(0.5) ->
+        weight_norm(Linear(2H, num_labels), dim=None) on the pooled output. Like the reference's weight_norm pre-forward hook, every
+        forward first derives both weights from (g, v) (vb_weight_norm_fwd: fp32 and the operand copies), so a parameter update by
+        any optimizer is picked up without a separate refresh. The dropout sits in the first GEMM's epilogue after the ReLU; its
+        backward folds the 1 / (1 - p) scale into the dgrad GEMM and gates by the dropped output."""
+        ps, lib, B, H, Lb = self.ps, self.lib, self.B, x.H, self.ps.num_labels
+        H2 = 2 * H
+        W, self.wn_weights = {}, {}
+        for i in (0, 3):
+            nm = f"vil_prediction.main.{i}"
+            v, g = ps.p(nm + ".weight_v"), ps.p(nm + ".weight_g")
+            w32, op = self.buf(tuple(v.shape), F32), self.buf16(tuple(v.shape))
+            scr = self.buf((L.VB_WEIGHT_NORM_SCRATCH // 8,), torch.float64)
+            self.emit(lib.vb_weight_norm_fwd, v.data_ptr(), g.data_ptr(), v.numel(), w32.data_ptr(), *op.ptrs(), op.fp16, scr.data_ptr())
+            W[i] = (nm, v, g, op, scr)
+            self.wn_weights[nm] = w32
+        p_drop = 0.5
+        drop = self.drop("vil_prediction.main.2", p_drop)
+        h32, h = self.buf((B, H2), F32), self.buf16((B, H2))
+        self.gemm(B, H2, H, x.op, H, W[0][3], H, bias=ps.p("vil_prediction.main.0.bias"), act=L.VB_ACT_RELU, out_f32=h32, ld_of=H2,
+                  out_bf16=h, ld_ob=H2, dropout=drop)
+        logits = self.buf((B, Lb), F32)
+        self.gemm(B, Lb, H2, h, H2, W[3][3], H2, bias=ps.p("vil_prediction.main.3.bias"), out_f32=logits, ld_of=Lb)
+        self.outputs["vil_prediction"] = logits
+        part = lambda i: [f"vil_prediction.main.{i}.{s}" for s in ("weight_g", "weight_v", "bias")]
+        h_rg = not x.frozen or self.trainable(*part(0))
+        self.out_rg["vil_prediction"] = h_rg or self.trainable(*part(3))
+        scale = 1.0 / (1.0 - p_drop) if drop is not None else 1.0
+
+        def wn_wgrad(i, dy16, ld_dy, x16, ld_x, M, N_out, K_in):
+            nm, v, g, _, scr = W[i]
+            gg, gv = self.pg(nm + ".weight_g"), self.pg(nm + ".weight_v")
+            if gg is None and gv is None:
+                return
+            dw = self.scratch(f"vilp.dw{i}", (N_out, K_in), F32)
+            self.emit(lib.vb_memset_zero, dw.data_ptr(), dw.numel() * 4)
+            self.gemm(N_out, K_in, M, dy16, ld_dy, x16, ld_x, a_mn=1, b_mn=1, out_f32=dw, ld_of=K_in, atomic=1, split_k=0)
+            self.emit(lib.vb_weight_norm_bwd, dw.data_ptr(), v.data_ptr(), g.data_ptr(), v.numel(), self._ptr(gg), self._ptr(gv), scr.data_ptr())
+
+        def bwd():
+            if "vil_prediction" not in self.grad_outputs:
+                return
+            ldp = _pad8(Lb)
+            dl32 = self.out_grad_buffer("vil_prediction", (B, Lb))
+            dl16 = self.scratch("vilp.dl16", (B, ldp), BF16)
+            self.emit(lib.vb_cast2d_f32_to_bf16, dl32.data_ptr(), Lb, dl16.data_ptr(), ldp, B, Lb, 1.0)
+            gb = self.pg("vil_prediction.main.3.bias")
+            if gb is not None:
+                self.colsum(dl32, Lb, gb, B, Lb)
+            wn_wgrad(3, dl16, ldp, h.bw, H2, B, Lb, H2)
+            if not h_rg:
+                return
+            dh = self.scratch("vilp.dh32", (B, H2), F32)
+            self.gemm(B, H2, Lb, dl16, ldp, W[3][3].bw, H2, b_mn=1, out_f32=dh, ld_of=H2, alpha=scale)
+            dpre16, dpre32 = self.scratch("vilp.dpre16", (B, H2), BF16), self.scratch("vilp.dpre32", (B, H2), F32)
+            self.emit(lib.vb_relu_bwd, dh.data_ptr(), h32.data_ptr(), dpre16.data_ptr(), dpre32.data_ptr(), B * H2)
+            gb = self.pg("vil_prediction.main.0.bias")
+            if gb is not None:
+                self.colsum(dpre32, H2, gb, B, H2)
+            wn_wgrad(0, dpre16, H2, x.op.bw, H, B, H2, H)
+            self.dgrad_into(x, dpre16, H2, W[0][3].bw, B, H2, H)
+        if self.out_rg["vil_prediction"]:
+            self.push_bwd(bwd)
+
+    def build_base_heads(self, seq, pooled):
+        """The seven outputs of BaseBertForVLTasks.forward (basebert.py:929-962). Returns the views of the whole-stream output-gradient
+        buffers that the caller's gradients of the 1-output heads go into. Emission order is chosen for the backward, which runs it
+        in reverse: the gathered heads first (their scatters are the first writes to the stream gradient), then the 1-output heads
+        over the stream and the pooled heads (which accumulate), then the pooler."""
+        ps, c, B = self.ps, self.cfg, self.B
+        H, Nt, Nv, N = seq.H, self.Nt, self.Nv, self.N
+        self.base_simple_classifier(pooled)
+        self.small_head("vil_logit", pooled, "vil_logit", 1)
+        self.small_head("vil_binary_prediction", pooled, "cls.seq_relationship", 2)
+        views = {}
+        # self.dropout is one nn.Dropout called twice (basebert.py:949-952): two sites, each a mask over the whole stream
+        for name, site, a, b in (("vision_logit", "dropout.seq_v", Nt, N), ("linguisic_logit", "dropout.seq_t", 0, Nt)):
+            full = self.out_grad_buffer(name, (B * N, 1))
+            self.small_head(name, seq, name, 1, addend=self.mask if name == "vision_logit" else None,
+                            in_drop=self.drop(site, self.head_dropout_prob))
+            self.outputs[name] = self.outputs[name].view(B, N, 1)[:, a:b]
+            views[name] = full.view(B, N, 1)[:, a:b]
+        rows_t = self.base_rows(seq, 0, Nt, "rows.t")
+        rows_v = self.base_rows(seq, Nt, N, "rows.v")
+        wn = "bert.embeddings.word_embeddings.weight"
+        ht, ht_bwd = self.transform(rows_t, "cls.predictions.transform.dense", "cls.predictions.transform.LayerNorm", "lm.tr")
+        lm_bwd = self.big_head("linguisic_prediction", ht, H, B * Nt, H, c.vocab_size, None, "cls.predictions.bias", w=ps.w(wn), gw_name=wn)
+        hv, hv_bwd = self.transform(rows_v, "cls.imagePredictions.transform.dense", "cls.imagePredictions.transform.LayerNorm", "im.tr")
+        im_bwd = self.big_head("vision_prediction", hv, H, B * Nv, H, BASE_REGION_CLASSES, "cls.imagePredictions.decoder",
+                               "cls.imagePredictions.decoder.bias")
+        self.push_bwd(self._wide_bwd(lm_bwd, ht, ht_bwd, H, c.vocab_size))
+        self.push_bwd(self._wide_bwd(im_bwd, hv, hv_bwd, H, BASE_REGION_CLASSES))
+        self.outputs["linguisic_prediction"] = self.outputs["linguisic_prediction"].view(B, Nt, -1)
+        self.outputs["vision_prediction"] = self.outputs["vision_prediction"].view(B, Nv, -1)
+        return views
 
 
 class Engine:
@@ -2557,9 +2523,9 @@ class Engine:
             return self.plans[key]
         while len(self.plans) >= self.max_plans:   # evict the least recently used plan: its buffers go back to the allocator
             self.plans.popitem(last=False)
-        self.plans[key] = Plan(self, B, Nt, Nv, grad_outputs, False, heads, train, loss=loss, choices=choices, score=score,
-                               loss_in_forward=loss_in_forward, outputs=outputs, results=results, fast_mode=fast_mode,
-                               image_prefix=image_prefix, frozen=frozen)
+        self.plans[key] = (BasePlan if self.ps.base else Plan)(
+            self, B, Nt, Nv, grad_outputs, False, heads, train, loss=loss, choices=choices, score=score, loss_in_forward=loss_in_forward,
+            outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen)
         return self.plans[key]
 
     def enable_activation_arena(self, nbytes):
