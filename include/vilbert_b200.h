@@ -229,6 +229,9 @@ vb_status vb_embed_text_bwd(const float* dout, const int64_t* ids, const int64_t
  * W [H,5]; consumed as the residual of the 2048 -> Hv region-feature GEMM. Backward accumulates dW, db (either may be NULL). */
 vb_status vb_loc_proj_fwd(const float* loc, const float* W, const float* b, float* out, int32_t M, int32_t H, void* stream);
 vb_status vb_loc_proj_bwd(const float* dy, const float* loc, float* dW, float* db, int32_t M, int32_t H, void* stream);
+/* Input gradient of the box projection: dx[m,:5] = dy[m,:] W (written, not accumulated), dy [M,H] fp32, W [H,5]. Fixed-order
+ * reductions without atomics: the result does not depend on the launch. */
+vb_status vb_loc_proj_dx(const float* dy, const float* W, float* dx, int32_t M, int32_t H, void* stream);
 
 /* Bias gradients: out[n] += sum_m X[m,n]; X is bf16 (is_bf16 != 0) or f32, [M,N] with ld. */
 vb_status vb_colsum(const void* X, int32_t is_bf16, int64_t ld, float* out, int32_t M, int32_t N, void* stream);

@@ -107,6 +107,45 @@ def cases(O, E, base_labels):
     ]
 
 
+def input_grad_cases(O, E, base_labels):
+    """Cases of plans that also differentiate the region features and boxes (input_grads=), listed after the matrix above so that
+    the listing of a tree without them is a prefix of this one. frozen="all" freezes every parameter entry (the saliency case)."""
+    both = frozenset(E.INPUT_GRAD_NAMES)
+    train = dict(grad_outputs=O.HEAD_NAMES, train=True, input_grads=both)
+    base = dict(num_labels=base_labels)
+    return [
+        ("input_grads_heads_train", {}, "vl", 4, train),
+        ("input_grads_all_frozen_eval", {}, "vl", 4, dict(grad_outputs=("vil_prediction",), input_grads=both, frozen="all")),
+        ("input_grads_in_batch_pairs", dict(in_batch_pairs=True), "vl", 4, train),
+        ("input_grads_base_train", {}, "base", 3, dict(grad_outputs=E.BASE_HEAD_NAMES, train=True, input_grads=both), NV, base),
+        ("input_grads_pretraining", {}, "pretraining", 4, dict(grad_outputs=E.LOSS_HEADS["pretraining"], loss="pretraining", train=True,
+                                                               loss_in_forward=True, input_grads=both)),
+    ]
+
+
+def dump_cases(out, case_list, prec, Engine, BertConfig, tiny, tiny_base):
+    """Lists every plan of `case_list` in precision `prec`, without and with the shared activation arena. -> (plans, op records)"""
+    n_plans = n_ops = 0
+    for name, over, heads, B, kw, *extra in case_list:
+        nv = extra[0] if extra else NV
+        engine_kw = extra[1] if len(extra) > 1 else {}
+        cfg = dict(tiny_base["config"] if heads.startswith("base") else tiny, **over)
+        for arena in (False, True):
+            eng = Engine(BertConfig.from_dict(cfg), "cpu", heads=heads, _build_only=True, precision=prec, **engine_kw)
+            if arena:
+                eng.enable_activation_arena(ARENA_BYTES)
+            plan_kw = dict(kw, frozen=frozenset(eng.ps.entries)) if kw.get("frozen") == "all" else kw
+            try:
+                plan = eng.plan(B, NT, nv, **plan_kw)
+            except (TypeError, ValueError) as ex:
+                print(f"plan_dump: {prec} {name} arena={int(arena)} skipped: {ex}", file=sys.stderr)
+                continue
+            plan.enable_training_prologue()
+            n_ops += dump_plan(out, f"{prec} {name} arena={int(arena)}", plan)
+            n_plans += 1
+    return n_plans, n_ops
+
+
 class Allocations:
     """Names pointers after the first allocation (in the order given) whose storage contains them."""
 
@@ -203,22 +242,8 @@ def main():
     tiny_base = json.load(open(os.path.join(golden, "tiny_basebert.json")))
     out, n_plans, n_ops = [], 0, 0
     for prec in PRECISIONS:
-        for name, over, heads, B, kw, *extra in cases(O, E, tiny_base["num_labels"]):
-            nv = extra[0] if extra else NV
-            engine_kw = extra[1] if len(extra) > 1 else {}
-            cfg = dict(tiny_base["config"] if heads.startswith("base") else tiny, **over)
-            for arena in (False, True):
-                eng = Engine(BertConfig.from_dict(cfg), "cpu", heads=heads, _build_only=True, precision=prec, **engine_kw)
-                if arena:
-                    eng.enable_activation_arena(ARENA_BYTES)
-                try:
-                    plan = eng.plan(B, NT, nv, **kw)
-                except (TypeError, ValueError) as ex:
-                    print(f"plan_dump: {prec} {name} arena={int(arena)} skipped: {ex}", file=sys.stderr)
-                    continue
-                plan.enable_training_prologue()
-                n_ops += dump_plan(out, f"{prec} {name} arena={int(arena)}", plan)
-                n_plans += 1
+        p, o = dump_cases(out, cases(O, E, tiny_base["num_labels"]), prec, Engine, BertConfig, tiny, tiny_base)
+        n_plans, n_ops = n_plans + p, n_ops + o
         for opt_cls in (FusedAdamW, FusedRAdam):
             n_ops += dump_optimizer_plan(out, torch, O, Engine, BertConfig, tiny, prec, opt_cls, f"{prec} {opt_cls.__name__}")
             n_plans += 1
@@ -228,6 +253,11 @@ def main():
             n_ops += dump_optimizer_plan(out, torch, O, Engine, BertConfig, tiny, prec, opt_cls, f"{prec} {opt_cls.__name__} max_grad_norm=1.0",
                                          max_grad_norm=1.0)
             n_plans += 1
+    # input gradients: listed last, so that the listing of a tree without them is a prefix of this one
+    if hasattr(E, "INPUT_GRAD_NAMES"):
+        for prec in PRECISIONS:
+            p, o = dump_cases(out, input_grad_cases(O, E, tiny_base["num_labels"]), prec, Engine, BertConfig, tiny, tiny_base)
+            n_plans, n_ops = n_plans + p, n_ops + o
     text = "\n".join(out) + "\n"
     if a.out:
         with open(a.out, "w") as f:

@@ -89,6 +89,7 @@ _SIGNATURES = {
     "vb_embed_text_bwd": [_P, _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _P],
     "vb_loc_proj_fwd": [_P, _P, _P, _P, _I32, _I32, _P],
     "vb_loc_proj_bwd": [_P, _P, _P, _P, _I32, _I32, _P],
+    "vb_loc_proj_dx": [_P, _P, _P, _I32, _I32, _P],
     "vb_colsum": [_P, _I32, _I64, _P, _I32, _I32, _P],
     "vb_small_linear_fwd": [_P, _I64, _P, _P, _P, _P, _I32, _I32, _I32, _P, _P],
     "vb_small_linear_bwd": [_P, _P, _I64, _P, _P, _I64, _I32, _P, _P, _I32, _I32, _I32, _P, _P],

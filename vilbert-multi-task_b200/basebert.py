@@ -12,7 +12,7 @@ import math
 import torch
 
 from .engine import BASE_BERT_OUT_NAMES, BASE_HEAD_NAMES
-from .modeling import BertPreTrainedModel, _BertNode, _PlanCall, _PlanFn
+from .modeling import BertPreTrainedModel, _BertNode
 
 
 class _BaseBertNode(_BertNode):
@@ -55,8 +55,8 @@ class _BaseModel(BertPreTrainedModel):
         inputs = dict(input_txt=input_txt, input_imgs=input_imgs, image_loc=image_loc, token_type_ids=token_type_ids,
                       attention_mask=attention_mask, image_attention_mask=image_attention_mask, task_ids=None)
         names = tuple(names)
-        plan = self._outputs_plan(names, inputs, bool(self.training))
-        outs = _PlanFn.apply(self._anchor, _PlanCall(self, plan, inputs, names=names))
+        plan = self._outputs_plan(names, inputs, bool(self.training), input_grads=self._input_grads(inputs))
+        outs = self._call(plan, inputs, names=names)
         return dict(zip(names, outs))
 
     def _bert_forward(self, input_txt, input_imgs, image_loc, token_type_ids=None, attention_mask=None, image_attention_mask=None,

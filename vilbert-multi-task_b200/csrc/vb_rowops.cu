@@ -355,6 +355,45 @@ __global__ void loc_proj_bwd_kernel(const float* __restrict__ dy, const float* _
   if (db) atomicAdd(db + h, acc[5]);
 }
 
+// dx[m, j] = sum_h dy[m, h] * W[h, j]  (j < 5): the input gradient of loc_proj_fwd (d image_loc). One warp per row. W is staged
+// transposed ([5][H]) in shared memory, so each 128-bit read of dy meets one 128-bit shared read per box coordinate. The five
+// lane sums go through the same xor-shuffle tree in every launch and lane 0 stores them: no atomics, replays are bitwise equal.
+template <bool VEC>
+__global__ void __launch_bounds__(ROW_THREADS) loc_proj_dx_kernel(const float* __restrict__ dy, const float* __restrict__ W,
+                                                                  float* __restrict__ dx, int M, int H) {
+  pdl_entry();
+  extern __shared__ __align__(16) float swt[];  // [5][H]
+  for (int i = threadIdx.x; i < H * 5; i += blockDim.x) swt[(i % 5) * H + i / 5] = W[i];
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  for (long long m = (long long)blockIdx.x * ROW_WARPS + (threadIdx.x >> 5); m < M; m += (long long)gridDim.x * ROW_WARPS) {
+    const float* d = dy + m * H;
+    float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+    if (VEC) {
+      for (int h = lane * 4; h < H; h += 128) {
+        const float4 v = *reinterpret_cast<const float4*>(d + h);
+#pragma unroll
+        for (int j = 0; j < 5; ++j) {
+          const float4 w = *reinterpret_cast<const float4*>(swt + j * H + h);
+          acc[j] += v.x * w.x + v.y * w.y + v.z * w.z + v.w * w.w;
+        }
+      }
+    } else {
+      for (int h = lane; h < H; h += 32) {
+        const float v = d[h];
+#pragma unroll
+        for (int j = 0; j < 5; ++j) acc[j] += v * swt[j * H + h];
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 5; ++j) acc[j] = warp_sum(acc[j]);
+    if (lane == 0) {
+#pragma unroll
+      for (int j = 0; j < 5; ++j) dx[m * 5 + j] = acc[j];
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------ column sums (bias grads)
 template <typename T>
 __device__ __forceinline__ float to_f(T v);
@@ -792,6 +831,16 @@ extern "C" vb_status vb_loc_proj_bwd(const float* dy, const float* loc, float* d
   dim3 grid((H + 127) / 128, (M + rpb - 1) / rpb);
   launch_pdl(loc_proj_bwd_kernel, dim3(grid), dim3(128), (size_t)(0), ST(stream), dy, loc, dW, db, M, H, rpb);
   return check_launch("vb_loc_proj_bwd");
+}
+
+extern "C" vb_status vb_loc_proj_dx(const float* dy, const float* W, float* dx, int32_t M, int32_t H, void* stream) {
+  if (M <= 0 || H <= 0) return set_error(VB_ERR_INVALID, "vb_loc_proj_dx: bad shape");
+  const size_t smem = (size_t)H * 5 * sizeof(float);
+  if (smem > 48 * 1024) return set_error(VB_ERR_UNSUPPORTED, "vb_loc_proj_dx: H too large");
+  const bool vec = H % 4 == 0 && (reinterpret_cast<uintptr_t>(dy) & 15) == 0;
+  if (vec) launch_pdl(loc_proj_dx_kernel<true>, dim3(row_grid(M)), dim3(ROW_THREADS), smem, ST(stream), dy, W, dx, M, H);
+  else launch_pdl(loc_proj_dx_kernel<false>, dim3(row_grid(M)), dim3(ROW_THREADS), smem, ST(stream), dy, W, dx, M, H);
+  return check_launch("vb_loc_proj_dx");
 }
 
 extern "C" vb_status vb_colsum(const void* X, int32_t is_bf16, int64_t ld, float* out, int32_t M, int32_t N, void* stream) {

@@ -38,6 +38,8 @@ BASE_FEATURE_SIZE, BASE_REGION_CLASSES = 2048, 1601
 BASE_HEAD_NAMES = ("vil_prediction", "vil_logit", "vil_binary_prediction", "vision_prediction", "vision_logit", "linguisic_prediction",
                    "linguisic_logit")
 BASE_BERT_OUT_NAMES = ("sequence_output", "pooled_output")
+# the float inputs a plan can backpropagate into (Plan(input_grads=...)): the region features and their boxes
+INPUT_GRAD_NAMES = ("input_imgs", "image_loc")
 
 
 def _pad8(n):
@@ -378,15 +380,27 @@ class Plan:
     op that produced it has a trainable parameter or an input that needs one (Act.frozen is the negation). The forward is the
     same; the backward computes no gradient of a frozen parameter (no weight-gradient GEMM, bias column sum, LayerNorm gamma /
     beta sum or embedding scatter), no gradient of an activation that needs none, and registers nothing for a block with nothing
-    to do. No range a frozen parameter owns appears in grad_touch. self.out_rg tells which outputs carry a gradient."""
+    to do. No range a frozen parameter owns appears in grad_touch. self.out_rg tells which outputs carry a gradient.
+
+    input_grads: a subset of INPUT_GRAD_NAMES whose gradient the backward also computes. The image embedding's output then needs a
+    gradient even with all of its parameters frozen, and the backward ends the image-embedding chain with d(input_imgs) = dy W (the
+    feature GEMM's dgrad) and d(image_loc) = dy W_loc (vb_loc_proj_dx). They land in private buffers outside the arena and outside
+    grad_touch; self.input_grad maps each input whose gradient the backward writes to its buffer ([B*Nv, Fv] / [B*Nv, 5] fp32). An
+    input behind a no_grad layer (fixed_v_layer > 0) gets no entry, as it gets no gradient in torch."""
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset()):
+                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
+                 input_grads=frozenset()):
         self.e, self.cfg = engine, engine.cfg
         self.frozen = frozenset(frozen)
         unknown = sorted(n for n in self.frozen if n not in engine.ps.entries)
         if unknown:
             raise ValueError(f"frozen: {unknown[:4]} are not parameter entries of this model")
+        self.input_grads = frozenset(input_grads)
+        unknown = sorted(n for n in self.input_grads if n not in INPUT_GRAD_NAMES)
+        if unknown:
+            raise ValueError(f"input_grads: {unknown} are not among the differentiable inputs {INPUT_GRAD_NAMES}")
+        self.input_grad = {}          # input name -> the buffer its gradient lands in (written by the backward)
         self.out_rg = {}              # output name -> it carries a gradient (some trainable parameter lies upstream of it)
         self.grad_touch = {}           # (flat offset, numel) -> index of the last backward op writing that gradient range
         self.ps = engine.ps
@@ -394,6 +408,8 @@ class Plan:
         self.dev = engine.device
         self.Bin = B
         self._stream_modes(B, Nt, Nv, train, grad_outputs, vqa_loss, loss, fast_mode, image_prefix)
+        if self.input_grads and (self.fast or self.image_prefix):
+            raise ValueError("fast_mode and image_prefix plans are inference paths: no input gradients")
         self.attn_t, self.attn_v, self.attn_c = [], [], []
         self.prefix = []         # image_prefix: the image embedding and mask, run by run_image_prefix()
         self._private = False    # while set, buf() allocates private buffers (the image states of image_prefix)
@@ -1149,8 +1165,9 @@ class Plan:
             self._private = False
             self.cur = self.fwd
             v = Act(v32, vop, Mv, Hv)
-            v.frozen = not self.trainable(ve + ".image_embeddings.weight", ve + ".image_embeddings.bias", ve + ".image_location_embeddings.weight",
-                                          ve + ".image_location_embeddings.bias", ve + ".LayerNorm.weight", ve + ".LayerNorm.bias")
+            v.frozen = not (self.input_grads or self.trainable(
+                ve + ".image_embeddings.weight", ve + ".image_embeddings.bias", ve + ".image_location_embeddings.weight",
+                ve + ".image_location_embeddings.bias", ve + ".LayerNorm.weight", ve + ".LayerNorm.bias"))
             if self.image_prefix:
                 self.image_states = (v32, vop.hi, vop.lo, self.mask_v)
 
@@ -1184,8 +1201,10 @@ class Plan:
         return y, feat
 
     def image_embedding_bwd(self, prefix, H, feat, dy16, dy32):
-        """Parameter gradients of image_embedding from d(output): the region-feature GEMM's weight from its bf16 copy dy16, the box
-        projection from the fp32 dy32 (either None: no gradient wanted)."""
+        """Gradients of image_embedding from d(output): the region-feature GEMM's weight from its bf16 copy dy16, the box
+        projection from the fp32 dy32 (either None: no gradient wanted), then the input gradients of input_grads: the features
+        by the dgrad GEMM dy16 W, the boxes by vb_loc_proj_dx on dy32."""
+        ps = self.ps
         M, Fv = feat.hi.shape
         if dy16 is not None:
             self.linear_wgrad(dy16, H, None, 0, feat.bw, Fv, M, H, Fv, prefix + ".image_embeddings")
@@ -1193,6 +1212,12 @@ class Plan:
             gw, gb = self.pg(prefix + ".image_location_embeddings.weight"), self.pg(prefix + ".image_location_embeddings.bias")
             if gw is not None or gb is not None:
                 self.emit(self.lib.vb_loc_proj_bwd, dy32.data_ptr(), self.in_loc.data_ptr(), self._ptr(gw), self._ptr(gb), M, H)
+        if dy16 is not None and "input_imgs" in self.input_grads:
+            g = self.input_grad["input_imgs"] = self.buf((M, Fv), F32, zero=True)
+            self.gemm(M, Fv, H, dy16, H, ps.w(prefix + ".image_embeddings.weight").bw, Fv, b_mn=1, out_f32=g, ld_of=Fv)
+        if dy32 is not None and "image_loc" in self.input_grads:
+            g = self.input_grad["image_loc"] = self.buf((M, 5), F32, zero=True)
+            self.emit(self.lib.vb_loc_proj_dx, dy32.data_ptr(), ps.p(prefix + ".image_location_embeddings.weight").data_ptr(), g.data_ptr(), M, H)
 
     # ------------------------------------------------------------------ poolers and heads
     def pooler(self, seq, N, wname):
@@ -2219,11 +2244,12 @@ class BasePlan(Plan):
     frozen only: no fused objective, outputs= selection or image prefix."""
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset()):
+                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
+                 input_grads=frozenset()):
         if (vqa_loss or loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
                 or loss_in_forward):
-            raise ValueError("single-stream baseline plans support grad_outputs, train and frozen only")
-        super().__init__(engine, B, Nt, Nv, grad_outputs, heads=heads, train=train, choices=choices, frozen=frozen)
+            raise ValueError("single-stream baseline plans support grad_outputs, train, frozen and input_grads only")
+        super().__init__(engine, B, Nt, Nv, grad_outputs, heads=heads, train=train, choices=choices, frozen=frozen, input_grads=input_grads)
 
     def _stream_modes(self, B, Nt, Nv, *_):
         self.pairs = self.has_task = self.viz = self.dyn = self.fast = self.image_prefix = False
@@ -2296,15 +2322,17 @@ class BasePlan(Plan):
         img = [ie + n for n in (".image_embeddings.weight", ".image_embeddings.bias", ".token_type_embeddings.weight",
                                 ".image_location_embeddings.weight", ".image_location_embeddings.bias")]
         lns = [lnt + ".weight", lnt + ".bias", lnv + ".weight", lnv + ".bias"]
-        x.frozen = not self.trainable(*t_tables, *img, *lns)
+        x.frozen = not (self.input_grads or self.trainable(*t_tables, *img, *lns))
 
         def bwd():
             if not x.gw:
                 return
             gt = [self.pg(n) for n in t_tables]
             dxt = self.scratch("emb.dxt", (Mt, H), F32) if any(g is not None for g in gt) else None
-            dxv32 = self.scratch("emb.dxv32", (Mv, H), F32) if self.trainable(img[3], img[4]) else None
-            dxv16 = self.scratch("emb.dxv16", (Mv, H), BF16) if self.trainable(img[0]) else None
+            want32 = self.trainable(img[3], img[4]) or "image_loc" in self.input_grads
+            want16 = self.trainable(img[0]) or "input_imgs" in self.input_grads
+            dxv32 = self.scratch("emb.dxv32", (Mv, H), F32) if want32 else None
+            dxv16 = self.scratch("emb.dxv16", (Mv, H), BF16) if want16 else None
             gtype = self.pg(img[2])
             self.emit(lib.vb_concat_embed_ln_bwd, x.g32.data_ptr(), xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
                       ps.p(lnv + ".weight").data_ptr(), mean.data_ptr(), rstd.data_ptr(), self._ptr(dxt), self._ptr(dxv32), self._ptr(dxv16),
@@ -2511,13 +2539,15 @@ class Engine:
         self.lm_capacity = 0.25          # ... with room for this fraction of the token rows (15 % are masked; more poisons the loss with NaN)
 
     def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-             loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset()):
-        """The cached plan of this shape and these options (Plan). frozen: ParamStore entry names that take no gradient."""
-        frozen = frozenset(frozen)
+             loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
+             input_grads=frozenset()):
+        """The cached plan of this shape and these options (Plan). frozen: ParamStore entry names that take no gradient;
+        input_grads: the inputs of INPUT_GRAD_NAMES the backward also differentiates."""
+        frozen, input_grads = frozenset(frozen), frozenset(input_grads)
         loss = "vqa" if vqa_loss else loss
         pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
         key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward),
-               None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix), frozen)
+               None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix), frozen, input_grads)
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]
@@ -2525,7 +2555,7 @@ class Engine:
             self.plans.popitem(last=False)
         self.plans[key] = (BasePlan if self.ps.base else Plan)(
             self, B, Nt, Nv, grad_outputs, False, heads, train, loss=loss, choices=choices, score=score, loss_in_forward=loss_in_forward,
-            outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen)
+            outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen, input_grads=input_grads)
         return self.plans[key]
 
     def enable_activation_arena(self, nbytes):

@@ -10,10 +10,11 @@ import os
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from torch.autograd.function import once_differentiable
 
 from . import _lib as L
 from .config import BertConfig
-from .engine import BERT_OUT_NAMES, HEAD_NAMES, LOSS_HEADS, PRETRAINING_HEAD_NAMES, Engine
+from .engine import BERT_OUT_NAMES, HEAD_NAMES, INPUT_GRAD_NAMES, LOSS_HEADS, PRETRAINING_HEAD_NAMES, Engine
 
 
 # Any torch.optim.Optimizer.step() (pytorch_transformers.AdamW and the reference's RAdam subclass it) may have rewritten
@@ -87,18 +88,25 @@ class _PlanCall:
     same inputs and targets. In train mode, if another forward moved the dropout step since, the step of this forward is set
     around the recomputed forward and the backward, which regenerate their dropout masks from it, and restored afterwards. The
     backward accumulates into the flat gradient buffer (the Parameters' .grad are views of it) and ends with the data-parallel
-    all-reduce when one is attached."""
+    all-reduce when one is attached.
+
+    input_names: the float inputs (INPUT_GRAD_NAMES) whose gradient the plan computes (Plan.input_grads). backward() copies them
+    out of the plan right after its backward ran, in the shape, dtype and device of the tensors the caller passed
+    (self.input_grads_out; None for an input behind a no_grad layer). They are per-rank: the all-reduce never sees them."""
 
     def __init__(self, model, plan, inputs, targets=None, names=None):
         self.model, self.plan, self.inputs, self.targets, self.names = model, plan, inputs, targets or {}, names
+        self.input_names = tuple(n for n in INPUT_GRAD_NAMES if n in plan.input_grads)
+        self.input_grads_out = (None,) * len(self.input_names)
         self.drop_step = self.fwd_id = None
 
     def _load(self):
         plan = self.plan
-        plan.load_inputs(**self.inputs)
-        li = plan.loss_inputs
-        for k, v in self.targets.items():
-            li[k].copy_(v.reshape(li[k].shape), non_blocking=True)
+        with torch.no_grad():      # the plan's input buffers never join the caller's graph, also when backward() reloads them
+            plan.load_inputs(**self.inputs)
+            li = plan.loss_inputs
+            for k, v in self.targets.items():
+                li[k].copy_(v.reshape(li[k].shape), non_blocking=True)
 
     def forward(self):
         model, plan, eng = self.model, self.plan, self.model.engine
@@ -131,12 +139,13 @@ class _PlanCall:
             return out[0:1].clone(), out[1:2].clone(), out[2:3].clone()
         return (plan.loss.detach().reshape(()).clone(),)
 
-    def backward(self, grads):
+    def backward(self, grads, wanted=()):
+        """wanted: per entry of input_names, whether its gradient is copied out (autograd's needs_input_grad)."""
         model, eng = self.model, self.model.engine
         if self.names is not None:
             live = tuple(n for n, g in zip(self.names, grads) if g is not None)
             if frozenset(live) != self.plan.grad_outputs:     # the plan's backward reaches other outputs: take the plan of this set
-                self.plan = model._outputs_plan(self.names, self.inputs, self.plan.train, live, self.plan.frozen)
+                self.plan = model._outputs_plan(self.names, self.inputs, self.plan.train, live, self.plan.frozen, self.plan.input_grads)
                 self.fwd_id = None
         plan = self.plan
         now = eng.drop_step_host
@@ -162,20 +171,32 @@ class _PlanCall:
                     else:
                         plan.loss_grad[i:i + 1].copy_(g.detach().reshape(1))
             plan.run_backward()
+            self.input_grads_out = tuple(self._input_grad(n) if w else None for n, w in zip(self.input_names, wanted))
         finally:
             if moved:
                 eng.set_dropout_step(now)
         if model._ddp_reducer is not None:     # data parallel: average the flat gradient buffer over the ranks (apex DDP, delay_allreduce=True)
             model._ddp_reducer.allreduce()
 
+    def _input_grad(self, name):
+        """A copy of the gradient of the input `name` the backward just wrote, in the shape, dtype and device of the caller's tensor
+        (autograd sums it down to an input that broadcast into the plan's buffer); None when the plan wrote none."""
+        g = self.plan.input_grad.get(name)
+        if g is None:
+            return None
+        x = self.inputs[name]
+        return g.view(self.plan.Bin, self.plan.Nv, -1).to(device=x.device, dtype=x.dtype, copy=True)
+
 
 class _PlanFn(torch.autograd.Function):
     """Bridges a _PlanCall into torch.autograd: forward runs the call's forward and returns its outputs, backward hands the
     incoming gradients to the call's backward (nothing runs when none of them is live). An output with no trainable parameter
-    upstream (every parameter it depends on has requires_grad=False) does not require grad, as in torch."""
+    or differentiable input upstream (every parameter it depends on has requires_grad=False) does not require grad, as in torch.
+    The float inputs of call.input_names follow the call as real autograd inputs and receive the gradients the plan computed;
+    the backward is not itself differentiable (double backward raises)."""
 
     @staticmethod
-    def forward(ctx, anchor, call):
+    def forward(ctx, anchor, call, *float_inputs):
         ctx.call = call
         ctx.set_materialize_grads(False)
         call.forward()
@@ -186,10 +207,13 @@ class _PlanFn(torch.autograd.Function):
         return outs
 
     @staticmethod
+    @once_differentiable
     def backward(ctx, *grads):
-        if any(g is not None for g in grads):
-            ctx.call.backward(grads)
-        return None, None
+        call = ctx.call
+        if not any(g is not None for g in grads):
+            return (None, None) + (None,) * len(call.input_names)
+        call.backward(grads, ctx.needs_input_grad[2:])
+        return (None, None) + call.input_grads_out
 
 
 class BertPreTrainedModel(nn.Module):
@@ -407,11 +431,11 @@ class BertPreTrainedModel(nn.Module):
         return (seq_t, seq_v, o["pooled_output_t"], o["pooled_output_v"], self._attention_masks(output_all_attention_masks))
 
     # ---- shared forward machinery
-    def _outputs_plan(self, names, inputs, train, live=None, frozen=None):
+    def _outputs_plan(self, names, inputs, train, live=None, frozen=None, input_grads=frozenset()):
         """The plan of the outputs `names`. A plan is specialised on the set of outputs that receive a gradient; the set `live` a
         backward found is kept as the hint for the next forward of this shape, so in a steady training loop forward and backward
         share one plan and nothing is recomputed. It is also specialised on the frozen parameters (default: the current
-        requires_grad flags)."""
+        requires_grad flags) and on the inputs it differentiates (_input_grads)."""
         if frozen is None:
             frozen = self._frozen()
         Nt = inputs["input_txt"].shape[1]
@@ -421,14 +445,33 @@ class BertPreTrainedModel(nn.Module):
             live = self._grad_hint.get(key, ())
         else:
             self._grad_hint[key] = live
-        return self.engine.plan(B, Nt, Nv, grad_outputs=live, heads=self._heads_for(names), train=train, frozen=frozen)
+        return self.engine.plan(B, Nt, Nv, grad_outputs=live, heads=self._heads_for(names), train=train, frozen=frozen,
+                                input_grads=input_grads)
+
+    @staticmethod
+    def _input_grads(inputs):
+        """The float inputs of INPUT_GRAD_NAMES a call differentiates: those that require grad while grad mode is on (under
+        torch.no_grad() none). A floating-point attention mask that requires grad is refused: its gradient would flow through the
+        additive (1 - m) * -10000 mask, which the engine does not differentiate."""
+        if not torch.is_grad_enabled():
+            return frozenset()
+        for k in ("attention_mask", "image_attention_mask"):
+            m = inputs.get(k)
+            if m is not None and m.requires_grad:
+                raise NotImplementedError(f"{k} requires grad: gradients through the attention masks are not supported")
+        return frozenset(n for n in INPUT_GRAD_NAMES if inputs[n] is not None and inputs[n].requires_grad)
+
+    def _call(self, plan, inputs, targets=None, names=None):
+        """One plan-backed call through the autograd bridge, with the inputs the plan differentiates as its autograd inputs."""
+        call = _PlanCall(self, plan, inputs, targets, names)
+        return _PlanFn.apply(self._anchor, call, *(inputs[n] for n in call.input_names))
 
     def _run(self, names, input_txt, input_imgs, image_loc, token_type_ids, attention_mask, image_attention_mask, task_ids):
         inputs = dict(input_txt=input_txt, input_imgs=input_imgs, image_loc=image_loc, token_type_ids=token_type_ids,
                       attention_mask=attention_mask, image_attention_mask=image_attention_mask, task_ids=task_ids)
         names = tuple(names)
-        plan = self._outputs_plan(names, inputs, bool(self.training))
-        outs = _PlanFn.apply(self._anchor, _PlanCall(self, plan, inputs, names=names))
+        plan = self._outputs_plan(names, inputs, bool(self.training), input_grads=self._input_grads(inputs))
+        outs = self._call(plan, inputs, names=names)
         return dict(zip(names, outs))
 
 
@@ -553,5 +596,5 @@ class BertForMultiModalPreTraining(BertPreTrainedModel):
             targets["neg_index"] = sampler(B, R, image_feat.device) if sampler is not None else self._nce_negatives(B, R, image_feat.device)
         B, Nv, Nt = image_feat.shape[0], image_feat.shape[1], input_ids.shape[1]
         plan = self.engine.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS["pretraining"] if torch.is_grad_enabled() else (), train=bool(self.training),
-                                loss="pretraining", loss_in_forward=True, frozen=self._frozen())
-        return _PlanFn.apply(self._anchor, _PlanCall(self, plan, inputs, targets))
+                                loss="pretraining", loss_in_forward=True, frozen=self._frozen(), input_grads=self._input_grads(inputs))
+        return self._call(plan, inputs, targets)

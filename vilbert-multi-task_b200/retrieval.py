@@ -101,6 +101,8 @@ class RetrievalEvaluator:
             raise ValueError("RetrievalEvaluator runs forward-only plans: call model.eval() first")
         if features.dim() != 3 or spatials.shape[:2] != features.shape[:2] or tuple(image_mask.shape) != tuple(features.shape[:2]):
             raise ValueError("gallery: features [G, Nv, F], spatials [G, Nv, 5] and image_mask [G, Nv]")
+        if torch.is_grad_enabled() and (features.requires_grad or spatials.requires_grad):
+            raise ValueError("RetrievalEvaluator runs forward-only plans: it computes no gradient of the gallery's features or spatials")
         self.G, self.Nv = int(features.shape[0]), int(features.shape[1])
         if self.G > MAX_GALLERY:
             raise ValueError(f"gallery of {self.G} images: the device ranking supports at most {MAX_GALLERY}")
