@@ -288,15 +288,18 @@ class ParamStore:
 
 # ------------------------------------------------------------------------------------------ plan
 class Act:
-    """A residual-stream activation: fp32 values, its tensor-core Operand, fp32 gradient (lazily allocated)."""
-    __slots__ = ("f32", "op", "g32", "gw", "M", "H", "frozen")
+    """A residual-stream activation: fp32 values, its tensor-core Operand, fp32 gradient (lazily allocated). Plan.act makes them.
+    Three rules carry a gradient through a plan, each kept in one place:
+    1. needs-grad (Plan.act): `rg` is set when the op that made the activation has a trainable parameter or an input that needs a
+       gradient, as autograd's requires_grad; nothing made under the reference's torch.no_grad() (fixed_t_layer / fixed_v_layer) does.
+    2. registration (Plan.push_bwd): a block whose output needs no gradient registers no backward emitter.
+    3. first write (Plan.grad_zeroed / Plan.grad_acc): `gw` tells whether a backward op has written g32 yet. The first one
+       overwrites it, or zeroes it and adds; every later one accumulates."""
+    __slots__ = ("f32", "op", "g32", "gw", "M", "H", "rg")
 
-    def __init__(self, f32, op, M, H):
-        self.f32, self.op, self.M, self.H = f32, op, M, H
+    def __init__(self, f32, op, M, H, rg):
+        self.f32, self.op, self.M, self.H, self.rg = f32, op, M, H, rg
         self.g32, self.gw = None, False
-        # no gradient flows into it: produced under the reference's torch.no_grad() (fixed_t_layer / fixed_v_layer), or by ops
-        # with no trainable parameter from inputs that need no gradient (Plan(frozen=...))
-        self.frozen = False
 
 
 # Objectives that can be fused into a plan, and the outputs each differentiates (task_utils.py:325-374, vilbert.py:1506-1590):
@@ -377,7 +380,7 @@ class Plan:
 
     frozen: ParamStore entry names whose parameters take no gradient (requires_grad=False; the tied decoder is the word-embedding
     entry). While the forward is emitted every activation records whether it needs a gradient, as autograd does: it does when the
-    op that produced it has a trainable parameter or an input that needs one (Act.frozen is the negation). The forward is the
+    op that produced it has a trainable parameter or an input that needs one (Act.rg, set by Plan.act). The forward is the
     same; the backward computes no gradient of a frozen parameter (no weight-gradient GEMM, bias column sum, LayerNorm gamma /
     beta sum or embedding scatter), no gradient of an activation that needs none, and registers nothing for a block with nothing
     to do. No range a frozen parameter owns appears in grad_touch. self.out_rg tells which outputs carry a gradient.
@@ -452,6 +455,10 @@ class Plan:
         self._keep = []          # ctypes structs / tensors referenced by raw pointer
         self._scratch = {}
         self._bwd_emitters = []
+        self._no_grad = False    # set while a layer under the reference's torch.no_grad() is built (fixed_t_layer / fixed_v_layer)
+        self._last_attn = None   # visualization: the export of the attention emitted last
+        self._scatter_ok = False          # the baseline's row heads may scatter straight into the stream gradient (base_rows)
+        self._live_ranges_cache = {}      # (lo, hi) -> live_ranges(lo, hi), for run_step_overlapped
         self.n_kernels_fwd = self.n_kernels_bwd = 0
         self.graph_fwd = self.graph_bwd = self.graph_step = None
         self._eager_runs = [0, 0]      # eager forward / backward executions (maybe_capture_passes)
@@ -523,9 +530,18 @@ class Plan:
 
     # ------------------------------------------------------------------ frozen parameters
     def trainable(self, *names):
-        """Whether any of the parameters `names` (entries or fused projections) takes a gradient."""
-        parts = self.e.ps.parts
+        """Whether any of the parameters `names` takes a gradient. A name is an entry, a fused projection, or a Linear / LayerNorm
+        module, which stands for its .weight and .bias."""
+        entries, parts = self.ps.entries, self.ps.parts
+        names = [m for n in names for m in ((n,) if n in entries or n in parts else (n + ".weight", n + ".bias"))]
         return any(p not in self.frozen for n in names for p in parts.get(n, (n,)))
+
+    def act(self, f32, op, M, H, inputs=(), params=(), rg=False):
+        """The Act an op makes from the Acts `inputs` with the parameters `params` (names as for trainable). It needs a gradient when
+        one of them does (rule 1 of Act); rg: whether an input that is not an Act does (an operand whose producer the caller tracks,
+        a plan input of input_grads). Under torch.no_grad() nothing does."""
+        rg = not self._no_grad and bool(rg or any(i.rg for i in inputs) or self.trainable(*params))
+        return Act(f32, op, M, H, rg)
 
     def grad_view(self, name):
         """Gradient view of the entry or fused projection `name` for the next backward op to write. grad_touch keeps, per range,
@@ -627,12 +643,12 @@ class Plan:
     def on(self, sid):
         return Plan._On(self, sid)
 
-    def push_bwd(self, fn):
-        """Registers a backward emitter; it will emit on the stream that is current now. Layers built while `self._no_grad` is set
-        (the reference's `with torch.no_grad()` around the first fixed_t_layer / fixed_v_layer layers) register nothing."""
-        if getattr(self, "_no_grad", False):
-            return
-        self._bwd_emitters.append((self.sid, fn))
+    def push_bwd(self, fn, rg=True):
+        """Registers a block's backward emitter; it will emit on the stream that is current now. rg: whether the block's output needs
+        a gradient (Act.rg); a block whose output needs none registers nothing (rule 2 of Act), so neither does a layer built
+        under torch.no_grad(). The wide heads register without it: their emitters decide when they run."""
+        if rg:
+            self._bwd_emitters.append((self.sid, fn))
 
     @staticmethod
     def _ptr(t):
@@ -747,12 +763,29 @@ class Plan:
             act.g32 = self.buf((act.M, act.H), F32)
         return act.g32
 
-    # dW, db of y = x W^T + b given dy (bf16 operand copy + a source for the bias column sums)
-    def linear_wgrad(self, dy16, ld_dy, dy_bias, ld_dyb, x16, ld_x, M, N_out, K_in, wname, gw=None):
+    def grad_zeroed(self, act):
+        """The gradient buffer of `act` for a backward op that adds to it: its first writer zeroes it first (rule 3 of Act)."""
+        g = self.grad_of(act)
+        if not act.gw:
+            self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
+            act.gw = True
+        return g
+
+    def grad_acc(self, act):
+        """-> (gradient buffer of `act`, accumulate flag) for a backward op that can overwrite or add: 0, overwrite, for its first
+        writer (rule 3 of Act)."""
+        g, acc = self.grad_of(act), 1 if act.gw else 0
+        act.gw = True
+        return g, acc
+
+    # dW, db of y = x W^T + b given dy (bf16 operand copy)
+    def linear_wgrad(self, dy16, ld_dy, x16, ld_x, M, N_out, K_in, wname, gw=None, bias_from=(None, 0)):
         """dW += dy^T x (split-K, atomics). Nothing on the critical chain depends on it, so with wgrad_streams it is issued on
         a side stream (2 = text chain, 3 = vision chain) right after an event marking that dy is ready; the side streams are
         joined at the data-parallel segment cuts and at the end of the backward pass. Frozen parameters (parts of a fused
-        projection) get no column sum and no GEMM: each run of trainable parts gets its own on its columns of dy."""
+        projection) get no column sum and no GEMM: each run of trainable parts gets its own on its columns of dy.
+        bias_from: (dy, its row pitch) to take db as column sums of, where no kernel upstream has fused them into its pass."""
+        dy_bias, ld_dyb = bias_from
         if dy_bias is not None:
             gb = self.gparts(wname + ".bias")
             nb = N_out // len(gb)
@@ -781,24 +814,17 @@ class Plan:
 
     # act.g32 (+)= dy16 @ W (+ extra32)
     def dgrad_into(self, act, dy16, ld_dy, W16, M, N_out, K_in, extra32=None):
-        if act.frozen:      # the activation needs no gradient (frozen producer, or fixed_*_layer's no_grad): it stops here
+        if not act.rg:      # the activation needs no gradient (frozen producer, or fixed_*_layer's no_grad): it stops here
             return
-        g = self.grad_of(act)
-        if not act.gw:
-            self.gemm(M, K_in, N_out, dy16, ld_dy, W16, K_in, b_mn=1, residual=extra32, ld_res=K_in, out_f32=g, ld_of=K_in)
-            act.gw = True
-        else:
-            if extra32 is not None:
-                self.emit(self.lib.vb_axpy_f32, extra32.data_ptr(), g.data_ptr(), M * K_in, 1.0)
-            self.gemm(M, K_in, N_out, dy16, ld_dy, W16, K_in, b_mn=1, residual=g, ld_res=K_in, out_f32=g, ld_of=K_in)
+        g, acc = self.grad_acc(act)
+        if acc and extra32 is not None:
+            self.emit(self.lib.vb_axpy_f32, extra32.data_ptr(), g.data_ptr(), M * K_in, 1.0)
+        self.gemm(M, K_in, N_out, dy16, ld_dy, W16, K_in, b_mn=1, residual=g if acc else extra32, ld_res=K_in, out_f32=g, ld_of=K_in)
 
     def add_grad(self, act, src32):
-        if act.frozen:
+        if not act.rg:
             return
-        g = self.grad_of(act)
-        if not act.gw:
-            self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
-            act.gw = True
+        g = self.grad_zeroed(act)
         self.emit(self.lib.vb_axpy_f32, src32.data_ptr(), g.data_ptr(), g.numel(), 1.0)
 
     # ------------------------------------------------------------------ blocks
@@ -810,8 +836,7 @@ class Plan:
         self.gemm(M, H, K_in, a, K_in, ps.w(wname + ".weight"), K_in, bias=ps.p(wname + ".bias"), residual=res.f32, ld_res=H,
                   out_f32=y, ld_of=H, dropout=drop)
         o32, o, mean, rstd = self.ln_fwd(y, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, H)
-        out = Act(o32, o, M, H)
-        out.frozen = not (a_rg or not res.frozen or self.trainable(wname + ".weight", wname + ".bias", lnname + ".weight", lnname + ".bias"))
+        out = self.act(o32, o, M, H, inputs=(res,), params=(wname, lnname), rg=a_rg)
 
         def bwd():
             """returns (dy16, dy32) of the dense output (== grad of the LN input); adds dy32 to res."""
@@ -821,7 +846,7 @@ class Plan:
             dy16 = self.scratch(tag + ".dy16", (M, H), BF16)
             self.ln_bwd(out.g32, y, ps.p(lnname + ".weight"), mean, rstd, dy32, dy16, M, H, self.pg(lnname + ".weight"), self.pg(lnname + ".bias"),
                         gbias=self.pg(wname + ".bias"), in_drop=drop)
-            self.linear_wgrad(dy16, H, None, 0, a.bw, K_in, M, H, K_in, wname)
+            self.linear_wgrad(dy16, H, a.bw, K_in, M, H, K_in, wname)
             return dy16, dy32
         return out, bwd
 
@@ -832,7 +857,7 @@ class Plan:
         f = self.buf16((M, I))
         self.gemm(M, I, H, x.op, H, ps.w(w1 + ".weight"), H, bias=ps.p(w1 + ".bias"), act=L.VB_ACT_GELU, out_bf16=f, ld_ob=I,
                   out_pre=pre16, ld_op=I)
-        f_rg = not x.frozen or self.trainable(w1 + ".weight", w1 + ".bias")
+        f_rg = x.rg or self.trainable(w1)
         out, out_bwd = self.dense_res_ln(f, I, x, w2, lnname, tag + ".o", drop=drop, a_rg=f_rg)
 
         def bwd():
@@ -844,10 +869,9 @@ class Plan:
             # d pre = (dy W2) * gelu'(pre)
             self.gemm(M, I, H, dy16, H, ps.w(w2 + ".weight").bw, I, b_mn=1, aux=pre16, ld_aux=I, act=L.VB_ACT_DGELU, out_bf16=dpre16, ld_ob=I,
                       out_colsum=self.pg(w1 + ".bias"))
-            self.linear_wgrad(dpre16, I, None, 0, x.op.bw, H, M, I, H, w1)
+            self.linear_wgrad(dpre16, I, x.op.bw, H, M, I, H, w1)
             self.dgrad_into(x, dpre16, I, ps.w(w1 + ".weight").bw, M, I, H, extra32=dy32)
-        if not out.frozen:
-            self.push_bwd(bwd)
+        self.push_bwd(bwd, out.rg)
         return out
 
     def self_attention_block(self, x, B, N, nh, mask, prefix, tag, p_attn=0.0, p_hidden=0.0, pool=None):
@@ -870,8 +894,8 @@ class Plan:
         self.attention(False, B, nh, N, N, D, q, 3 * H, k, 3 * H, v, 3 * H, mask, ctx, H, lse, dropout=adrop)
         if self.viz:
             (self.attn_t if tag == "t" else self.attn_v).append(self._last_attn)
-        qkv_rg = not x.frozen or self.trainable(prefix + ".self.qkv.weight", prefix + ".self.qkv.bias")
-        gate_rg = pool is not None and (not pool.frozen or self.trainable(prefix + ".self.dy.weight", prefix + ".self.dy.bias"))
+        qkv_rg = x.rg or self.trainable(prefix + ".self.qkv")
+        gate_rg = pool is not None and (pool.rg or self.trainable(prefix + ".self.dy"))
         ctx_rg = qkv_rg or gate_rg
         out, out_bwd = self.dense_res_ln(ctx, H, x, prefix + ".output.dense", prefix + ".output.LayerNorm", tag + ".ao",
                                          drop=self.drop(prefix + ".output.dropout", p_hidden), a_rg=ctx_rg)
@@ -893,7 +917,7 @@ class Plan:
                            dbq=None if gated else gq, dbk=None if gated else gk, dbv=gv, dropout=adrop)
             if gated:
                 # the gate Linear needs dz32 for its bias sum, dz16 for its weight gradient and for d pool
-                dyw_rg = self.trainable(prefix + ".self.dy.weight") or not pool.frozen
+                dyw_rg = self.trainable(prefix + ".self.dy.weight") or pool.rg
                 dz32 = self.scratch(tag + ".dz32", (B, 2 * H), F32) if self.trainable(prefix + ".self.dy.bias") else None
                 dz16 = self.scratch(tag + ".dz16", (B, 2 * H), BF16) if dyw_rg else None
                 self.emit(self.lib.vb_gate_scale_bwd, dqkv.data_ptr(), 3 * H, qkv.hi.data_ptr(), self._ptr(qkv.lo), 3 * H, z.data_ptr(), self._ptr(dz32),
@@ -901,12 +925,11 @@ class Plan:
                 for (a, b) in self._runs((gq, gk)):      # the parts of one range are adjacent in the flat buffer
                     self.colsum(dqkv[:, a * H:b * H], 3 * H, (gq, gk)[a], M, (b - a) * H)
                 if dz32 is not None or dz16 is not None:
-                    self.linear_wgrad(dz16, 2 * H, dz32, 2 * H, pool.op.bw, pool.H, B, 2 * H, pool.H, prefix + ".self.dy")
+                    self.linear_wgrad(dz16, 2 * H, pool.op.bw, pool.H, B, 2 * H, pool.H, prefix + ".self.dy", bias_from=(dz32, 2 * H))
                     self.dgrad_into(pool, dz16, 2 * H, ps.w(prefix + ".self.dy.weight").bw, B, 2 * H, pool.H)
-            self.linear_wgrad(dqkv, 3 * H, None, 0, x.op.bw, H, M, 3 * H, H, prefix + ".self.qkv")
+            self.linear_wgrad(dqkv, 3 * H, x.op.bw, H, M, 3 * H, H, prefix + ".self.qkv")
             self.dgrad_into(x, dqkv, 3 * H, ps.w(prefix + ".self.qkv.weight").bw, M, 3 * H, H, extra32=dy32)
-        if not out.frozen:
-            self.push_bwd(bwd)
+        self.push_bwd(bwd, out.rg)
         return out
 
     def connection_layer(self, v, t, idx):
@@ -940,8 +963,8 @@ class Plan:
         # biOutput: ctx2 -> vision stream (dense1 / LayerNorm1), ctx1 -> text stream (dense2 / LayerNorm2) (:890-892)
         # a side whose projections are frozen and whose input needs no gradient takes no gradient: dQ of its queries' direction
         # and dK / dV of the other are not computed
-        need1 = not v.frozen or self.trainable(p + ".biattention.qkv1.weight", p + ".biattention.qkv1.bias")
-        need2 = not t.frozen or self.trainable(p + ".biattention.qkv2.weight", p + ".biattention.qkv2.bias")
+        need1 = v.rg or self.trainable(p + ".biattention.qkv1")
+        need2 = t.rg or self.trainable(p + ".biattention.qkv2")
         ctx_rg = need1 or need2
         with self.on(1):
             v1o, v1_bwd = self.dense_res_ln(ctx2, Hb, v, p + ".biOutput.dense1", p + ".biOutput.LayerNorm1", "c.v.bo",
@@ -953,10 +976,8 @@ class Plan:
             if not (v1o.gw or t1o.gw):
                 return
             for a in (v1o, t1o):   # a stream without downstream gradient contributes zeros
-                if not a.gw and not a.frozen:
-                    g = self.grad_of(a)
-                    self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
-                    a.gw = True
+                if a.rg:
+                    self.grad_zeroed(a)
             rv, rt = v1_bwd(), t1_bwd()
             if not ctx_rg:
                 return
@@ -981,15 +1002,14 @@ class Plan:
                            dQ=part1(0, Hb), lddq=L3, dK=part2(Hb, 2 * Hb), lddk=L3, dV=part2(2 * Hb, L3), lddv=L3, delta=d2,
                            dbq=gq1, dbk=gk2, dbv=gv2, dropout=adrop2)
             if need1:
-                self.linear_wgrad(dqkv1, L3, None, 0, v.op.bw, Hv, Mv, L3, Hv, p + ".biattention.qkv1")
+                self.linear_wgrad(dqkv1, L3, v.op.bw, Hv, Mv, L3, Hv, p + ".biattention.qkv1")
             if need2:
-                self.linear_wgrad(dqkv2, L3, None, 0, t.op.bw, Ht, Mt, L3, Ht, p + ".biattention.qkv2")
+                self.linear_wgrad(dqkv2, L3, t.op.bw, Ht, Mt, L3, Ht, p + ".biattention.qkv2")
             self.dgrad_into(v, dqkv1, L3, ps.w(p + ".biattention.qkv1.weight").bw, Mv, L3, Hv, extra32=dyv32)
             self.dgrad_into(t, dqkv2, L3, ps.w(p + ".biattention.qkv2.weight").bw, Mt, L3, Ht, extra32=dyt32)
         # the cross-modal backward touches both streams' tensors: it runs on the main stream between two barriers
         self._bwd_emitters.append(None)
-        if not (v1o.frozen and t1o.frozen):
-            self.push_bwd(bwd)
+        self.push_bwd(bwd, v1o.rg or t1o.rg)
         self._bwd_emitters.append(None)
         with self.on(1):
             v2o = self.ffn(v1o, c.v_intermediate_size, p + ".v_intermediate.dense", p + ".v_output.dense", p + ".v_output.LayerNorm", "c.v.ffn",
@@ -1014,9 +1034,7 @@ class Plan:
             m = self.mask_t.new_empty((B, self.Nt)); self._keep.append(m)
             self.emit(self.lib.vb_mask_to_additive, self.in_amask_b.data_ptr(), m.data_ptr(), B, self.Nt_in, 1 if self.has_task else 0)
         self.mask_t = m
-        out = Act(f32, op, B * M1, H)
-        out.frozen = t.frozen
-        return out
+        return self.act(f32, op, B * M1, H, inputs=(t,))
 
     def expand_pairs(self, t, v):
         """in_batch_pairs (vilbert.py:1008-1040): sample p = i * b + j of the expanded batch pairs text i with image j —
@@ -1036,27 +1054,22 @@ class Plan:
                     self.emit(lib.vb_repeat_rows, src.data_ptr(), dst.data_ptr(), n * dst.element_size(), b, b)
                 else:
                     self.emit(lib.vb_broadcast_rows, src.data_ptr(), dst.data_ptr(), b * n * dst.element_size(), b)
-            out = Act(f32, op, b * b * N, act.H)
-            out.frozen = act.frozen
+            out = self.act(f32, op, b * b * N, act.H, inputs=(act,))
             outs.append(out)
 
             def bwd(act=act, out=out, n=n, is_text=is_text):
-                if not out.gw or act.frozen:
+                if not out.gw:
                     return
-                g = self.grad_of(act)
-                acc = 1 if act.gw else 0
+                g, acc = self.grad_acc(act)
                 if is_text:   # g[i] = sum_j out.g32[i * b + j]
                     self.emit(lib.vb_sum_strided, out.g32.data_ptr(), g.data_ptr(), n, b, b * n, b, n, acc)
                 else:         # g[j] = sum_i out.g32[i * b + j]
                     self.emit(lib.vb_sum_strided, out.g32.data_ptr(), g.data_ptr(), n, b, n, b, b * n, acc)
-                act.gw = True
             self._bwd_emitters.append(None)
-            if not act.frozen:
-                self.push_bwd(bwd)
+            self.push_bwd(bwd, out.rg)
             self._bwd_emitters.append(None)
         # masks: text mask rows repeated, image mask tiled (4-byte rows: plain torch-free kernels need 16-byte items -> host-side views)
         mt = self.buf((b * b, self.Nt), F32); mv = self.buf((b * b, self.Nv), F32)
-        self._pair_masks = (self.mask_t, self.mask_v, mt, mv)
         self.emit(lib.vb_mask_to_additive, self.in_amask_pairs.data_ptr(), mt.data_ptr(), b * b, self.Nt_in, 1 if self.has_task else 0)
         self.emit(lib.vb_mask_to_additive, self.in_imask_pairs.data_ptr(), mv.data_ptr(), b * b, self.Nv, 0)
         self.mask_t, self.mask_v = mt, mv
@@ -1079,18 +1092,15 @@ class Plan:
         p32 = self.buf((B, Ht), F32)
         p = self.buf16((B, Ht))
         self.emit(lib.vb_masked_mean_fwd, t.f32.data_ptr(), self.mask_t.data_ptr(), p32.data_ptr(), *p.ptrs(), p.fp16, B, self.Nt, Ht)
-        pool = Act(p32, p, B, Ht)
-        pool.frozen = t.frozen
+        pool = self.act(p32, p, B, Ht, inputs=(t,))
         mask = self.mask_t
 
         def bwd():
-            if not pool.gw or t.frozen:
+            if not pool.gw:
                 return
-            g = self.grad_of(t)
-            self.emit(lib.vb_masked_mean_bwd, pool.g32.data_ptr(), mask.data_ptr(), g.data_ptr(), 1 if t.gw else 0, B, self.Nt, Ht)
-            t.gw = True
-        if not t.frozen:
-            self.push_bwd(bwd)
+            g, acc = self.grad_acc(t)
+            self.emit(lib.vb_masked_mean_bwd, pool.g32.data_ptr(), mask.data_ptr(), g.data_ptr(), acc, B, self.Nt, Ht)
+        self.push_bwd(bwd, pool.rg)
         return pool
 
     def image_layer(self, x, i, pool=None):
@@ -1135,10 +1145,9 @@ class Plan:
                   ps.p(e + ".task_embeddings.weight").data_ptr() if self.has_task else None, xe.data_ptr(), Bt, self.Nt_in, Ht)
         tdrop = self.drop(e + ".dropout", c.hidden_dropout_prob)
         t32, top, tmean, trstd = self.ln_fwd(xe, ps.p(e + ".LayerNorm.weight"), ps.p(e + ".LayerNorm.bias"), Mt, Ht, out_drop=tdrop)
-        t = Act(t32, top, Mt, Ht)
         tables = [e + n for n in (".word_embeddings.weight", ".position_embeddings.weight", ".token_type_embeddings.weight")]
         tables.append(e + ".task_embeddings.weight" if self.has_task else None)
-        t.frozen = not self.trainable(e + ".LayerNorm.weight", e + ".LayerNorm.bias", *[n for n in tables if n is not None])
+        t = self.act(t32, top, Mt, Ht, params=(e + ".LayerNorm", *[n for n in tables if n is not None]))
 
         def bwd_text():
             if t.gw:
@@ -1149,8 +1158,7 @@ class Plan:
                 if any(g is not None for g in gt):
                     self.emit(lib.vb_embed_text_bwd, dxe.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), self._ptr(self.in_task),
                               *[self._ptr(g) for g in gt], B, self.Nt_in, Ht)
-        if not t.frozen:
-            self.push_bwd(bwd_text)
+        self.push_bwd(bwd_text, t.rg)
         # image: region features fp32 -> bf16 ingest, 2048 -> Hv GEMM with the 5 -> Hv box projection as residual, LayerNorm (:1421-1432).
         # image_prefix: the same launches go to self.prefix on the main stream, and the LayerNorm's outputs (the image states the
         # forward reads) are private buffers
@@ -1164,10 +1172,8 @@ class Plan:
             v32, vop, vmean, vrstd = self.ln_fwd(yv, ps.p(ve + ".LayerNorm.weight"), ps.p(ve + ".LayerNorm.bias"), Mv, Hv, out_drop=vdrop)
             self._private = False
             self.cur = self.fwd
-            v = Act(v32, vop, Mv, Hv)
-            v.frozen = not (self.input_grads or self.trainable(
-                ve + ".image_embeddings.weight", ve + ".image_embeddings.bias", ve + ".image_location_embeddings.weight",
-                ve + ".image_location_embeddings.bias", ve + ".LayerNorm.weight", ve + ".LayerNorm.bias"))
+            v = self.act(v32, vop, Mv, Hv, params=(ve + ".image_embeddings", ve + ".image_location_embeddings", ve + ".LayerNorm"),
+                         rg=self.input_grads)
             if self.image_prefix:
                 self.image_states = (v32, vop.hi, vop.lo, self.mask_v)
 
@@ -1178,8 +1184,7 @@ class Plan:
                     self.ln_bwd(v.g32, yv, ps.p(ve + ".LayerNorm.weight"), vmean, vrstd, dyv32, dyv16, Mv, Hv, self.pg(ve + ".LayerNorm.weight"),
                                 self.pg(ve + ".LayerNorm.bias"), gbias=self.pg(ve + ".image_embeddings.bias"), out_drop=vdrop)
                     self.image_embedding_bwd(ve, Hv, feat, dyv16, dyv32)
-            if not v.frozen:
-                self.push_bwd(bwd_image)
+            self.push_bwd(bwd_image, v.rg)
         return t, v
 
     def image_embedding(self, prefix, H):
@@ -1207,7 +1212,7 @@ class Plan:
         ps = self.ps
         M, Fv = feat.hi.shape
         if dy16 is not None:
-            self.linear_wgrad(dy16, H, None, 0, feat.bw, Fv, M, H, Fv, prefix + ".image_embeddings")
+            self.linear_wgrad(dy16, H, feat.bw, Fv, M, H, Fv, prefix + ".image_embeddings")
         if dy32 is not None:
             gw, gb = self.pg(prefix + ".image_location_embeddings.weight"), self.pg(prefix + ".image_location_embeddings.bias")
             if gw is not None or gb is not None:
@@ -1227,8 +1232,7 @@ class Plan:
         p = self.buf16((B, Hb), bw=False)
         self.gemm(B, Hb, H, seq.op, N * H, ps.w(wname + ".weight"), H, bias=ps.p(wname + ".bias"), act=L.VB_ACT_RELU, out_f32=p32, ld_of=Hb,
                   out_bf16=p, ld_ob=Hb)
-        pooled = Act(p32, p, B, Hb)
-        pooled.frozen = seq.frozen and not self.trainable(wname + ".weight", wname + ".bias")
+        pooled = self.act(p32, p, B, Hb, inputs=(seq,), params=(wname,))
 
         def bwd():
             if not pooled.gw:
@@ -1236,21 +1240,17 @@ class Plan:
             dpre = self.scratch("pool.dpre", (B, Hb), BF16)
             dpre32 = self.scratch("pool.dpre32", (B, Hb), F32)
             self.emit(self.lib.vb_relu_bwd, pooled.g32.data_ptr(), p32.data_ptr(), dpre.data_ptr(), dpre32.data_ptr(), B * Hb)
-            self.linear_wgrad(dpre, Hb, dpre32, Hb, seq.op.bw, N * H, B, Hb, H, wname)
+            self.linear_wgrad(dpre, Hb, seq.op.bw, N * H, B, Hb, H, wname, bias_from=(dpre32, Hb))
             self.pooler_dgrad(seq, N, dpre, wname)
-        if not pooled.frozen:
-            self.push_bwd(bwd)
+        self.push_bwd(bwd, pooled.rg)
         return pooled
 
     def pooler_dgrad(self, seq, N, dpre, wname):
         """Backward of a pooler's Linear into its input: rows b*N (token 0 of every sample) of the sequence gradient += dpre @ W,
         with the sequence gradient zeroed on its first write."""
-        if seq.frozen:
+        if not seq.rg:
             return
-        g = self.grad_of(seq)
-        if not seq.gw:
-            self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
-            seq.gw = True
+        g = self.grad_zeroed(seq)
         B, K = dpre.shape
         self.gemm(B, seq.H, K, dpre, K, self.ps.w(wname + ".weight").bw, seq.H, b_mn=1, residual=g, ld_res=N * seq.H, out_f32=g,
                   ld_of=N * seq.H)
@@ -1272,7 +1272,7 @@ class Plan:
         logits = self.buf((M, N_out), F32)
         self.gemm(M, N_out, K_in, x.op, ld_x, W, K_in, bias=ps.p(bias_name), out_f32=logits, ld_of=N_out)
         self.outputs[name] = logits
-        self.out_rg[name] = not x.frozen or self.trainable(wkey, bias_name)
+        self.out_rg[name] = x.rg or self.trainable(wkey, bias_name)
 
         def bwd():
             if name not in self.grad_outputs or not self.out_rg[name]:
@@ -1288,10 +1288,10 @@ class Plan:
             if gb is not None:
                 self.colsum(dl32, N_out, gb, M, N_out)
             if gw_name is None:
-                self.linear_wgrad(dl16, ldp, None, 0, x.op.bw, ld_x, M, N_out, K_in, wname)
+                self.linear_wgrad(dl16, ldp, x.op.bw, ld_x, M, N_out, K_in, wname)
             elif self.trainable(gw_name):
-                self.linear_wgrad(dl16, ldp, None, 0, x.op.bw, ld_x, M, N_out, K_in, None, gw=self.grad_view(gw_name))
-            return None if x.frozen else (dl16, ldp, W.bw)
+                self.linear_wgrad(dl16, ldp, x.op.bw, ld_x, M, N_out, K_in, None, gw=self.grad_view(gw_name))
+            return (dl16, ldp, W.bw) if x.rg else None
         return bwd
 
     def _wide_bwd(self, head_bwd, hn, tr_bwd, K, N_out):
@@ -1301,9 +1301,8 @@ class Plan:
             if r is None:
                 return
             dl16, ldp, W16 = r
-            g = self.grad_of(hn)
+            g, _ = self.grad_acc(hn)      # the head is the transform's only reader: always the first write
             self.gemm(hn.M, K, N_out, dl16, ldp, W16, K, b_mn=1, out_f32=g, ld_of=K)
-            hn.gw = True
             tr_bwd()
         return f
 
@@ -1327,7 +1326,7 @@ class Plan:
         ldp = _pad8(V)
         self.lm_c = dict(cap=cap, idx=idx, count=cnt, labels=lab_c, logits=logits, dl32=self.buf((cap, V), F32),
                          dl16=self.buf((cap, ldp), BF16, zero=True), ldp=ldp)
-        self.out_rg["linguisic_prediction"] = not ht.frozen or self.trainable(wn, "cls.predictions.bias")
+        self.out_rg["linguisic_prediction"] = ht.rg or self.trainable(wn, "cls.predictions.bias")
 
         def bwd():
             if "linguisic_prediction" not in self.grad_outputs:     # a forward-only plan of the forward-placed objective
@@ -1337,15 +1336,13 @@ class Plan:
             if gb is not None:
                 self.colsum(lc["dl32"], V, gb, cap, V)
             if self.trainable(wn):
-                self.linear_wgrad(lc["dl16"], ldp, None, 0, hc.bw, Ht, cap, V, Ht, None, gw=self.grad_view(wn))
-            if ht.frozen:
+                self.linear_wgrad(lc["dl16"], ldp, hc.bw, Ht, cap, V, Ht, None, gw=self.grad_view(wn))
+            if not ht.rg:
                 return
             gc = self.scratch("lm.gc", (cap, Ht), F32)
             self.gemm(cap, Ht, V, lc["dl16"], ldp, ps.w(wn).bw, Ht, b_mn=1, out_f32=gc, ld_of=Ht)
-            g = self.grad_of(ht)
-            self.emit(lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
+            g = self.grad_zeroed(ht)
             self.emit(lib.vb_scatter_rows_f32, gc.data_ptr(), g.data_ptr(), idx.data_ptr(), cap, Ht, cnt.data_ptr(), self._lm_loss().data_ptr())
-            ht.gw = True
             ht_bwd()
         return bwd
 
@@ -1376,8 +1373,7 @@ class Plan:
         self.gemm(M, Hh, K, x.op, K, ps.w(wdense + ".weight"), K, bias=ps.p(wdense + ".bias"), act=L.VB_ACT_GELU, out_f32=g32, ld_of=Hh,
                   out_pre=pre16, ld_op=Hh)
         _, h, mean, rstd = self.ln_fwd(g32, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, Hh, want_f32=False)
-        hn = Act(None, h, M, Hh)
-        hn.frozen = x.frozen and not self.trainable(wdense + ".weight", wdense + ".bias", lnname + ".weight", lnname + ".bias")
+        hn = self.act(None, h, M, Hh, inputs=(x,), params=(wdense, lnname))
 
         def bwd():
             if not hn.gw:
@@ -1385,7 +1381,7 @@ class Plan:
             dpre16 = self.scratch(tag + ".dpre16", (M, Hh), BF16)
             self.ln_bwd(hn.g32, g32, ps.p(lnname + ".weight"), mean, rstd, None, dpre16, M, Hh, self.pg(lnname + ".weight"), self.pg(lnname + ".bias"),
                         pre=pre16, gbias=self.pg(wdense + ".bias"))
-            self.linear_wgrad(dpre16, Hh, None, 0, x.op.bw, K, M, Hh, K, wdense)
+            self.linear_wgrad(dpre16, Hh, x.op.bw, K, M, Hh, K, wdense)
             self.dgrad_into(x, dpre16, Hh, ps.w(wdense + ".weight").bw, M, Hh, K)
         return hn, bwd
 
@@ -1398,21 +1394,16 @@ class Plan:
         self.emit(self.lib.vb_small_linear_fwd, xin.data_ptr(), K, ps.p(wname + ".weight").data_ptr(), ps.p(wname + ".bias").data_ptr(),
                   self._ptr(addend), y.data_ptr(), M, K, N_out, self._ref(in_drop))
         self.outputs[name] = y
-        self.out_rg[name] = not x.frozen or self.trainable(wname + ".weight", wname + ".bias")
+        self.out_rg[name] = x.rg or self.trainable(wname)
 
         def bwd():
             if name not in self.grad_outputs:
                 return
             dy = self.out_grad_buffer(name, (M, N_out))
-            g, acc = None, 0
-            if not x.frozen:
-                g = self.grad_of(x)
-                acc = 1 if x.gw else 0
-                x.gw = True
+            g, acc = self.grad_acc(x) if x.rg else (None, 0)
             self.emit(self.lib.vb_small_linear_bwd, dy.data_ptr(), xin.data_ptr(), K, ps.p(wname + ".weight").data_ptr(), self._ptr(g), K, acc,
                       self._ptr(self.pg(wname + ".weight")), self._ptr(self.pg(wname + ".bias")), M, K, N_out, self._ref(in_drop))
-        if self.out_rg[name]:
-            self.push_bwd(bwd)
+        self.push_bwd(bwd, self.out_rg[name])
 
     def build_heads(self, seq_t, seq_v, pooled_t, pooled_v):
         """VILBertForVLTasks.forward after self.bert (vilbert.py:1673-1708) + BertPreTrainingHeads (:1228-1243).
@@ -1426,23 +1417,17 @@ class Plan:
             hi, lo, bw = f.ptrs()
             self.emit(lib.vb_fuse_pooled_fwd, pooled_t.f32.data_ptr(), pooled_v.f32.data_ptr(), f32.data_ptr(), hi, B * Hb, mul, self._ref(drop),
                       f.fp16, lo, bw)
-            act = Act(f32, f, B, Hb)
-            act.frozen = pooled_t.frozen and pooled_v.frozen
+            act = self.act(f32, f, B, Hb, inputs=(pooled_t, pooled_v))
 
             def fuse_bwd():
                 if not act.gw:
                     return
                 for a in (pooled_t, pooled_v):
-                    if a.frozen:
-                        continue
-                    g = self.grad_of(a)
-                    if not a.gw:
-                        self.emit(lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
-                        a.gw = True
+                    if a.rg:
+                        self.grad_zeroed(a)
                 self.emit(lib.vb_fuse_pooled_bwd, act.g32.data_ptr(), pooled_t.f32.data_ptr(), pooled_v.f32.data_ptr(), self._ptr(pooled_t.g32),
                           self._ptr(pooled_v.g32), B * Hb, mul, self._ref(drop))
-            if not act.frozen:
-                self.push_bwd(fuse_bwd)
+            self.push_bwd(fuse_bwd, act.rg)
             return act
         # VILBertForVLTasks.dropout on the fused vector (vilbert.py:1677-1682); BertPreTrainingHeads has its own nn.Dropout(0.1)
         # on its own fused vector (:1233-1241) — a different mask, needed only where the alignment score is an output
@@ -1485,8 +1470,7 @@ class Plan:
             return
         if want("vil_binary_prediction") and B % 2 == 0:
             # vil_binary_prediction pairs consecutive samples: pooled.view(-1, 2*Hb) (:1686-1689)
-            pair = Act(fused.f32.view(B // 2, 2 * Hb), fused.op.view(B // 2, 2 * Hb), B // 2, 2 * Hb)
-            pair.frozen = fused.frozen
+            pair = self.act(fused.f32.view(B // 2, 2 * Hb), fused.op.view(B // 2, 2 * Hb), B // 2, 2 * Hb, inputs=(fused,))
             hb, hb_bwd = self.transform(pair, "vil_binary_prediction.logit_fc.0", "vil_binary_prediction.logit_fc.2", "bin.tr")
             # LayerNorm output is needed in fp32 for the 2-way linear: recompute it from the bf16 copy is lossy, so run the small
             # linear on an fp32 LayerNorm output
@@ -1502,8 +1486,7 @@ class Plan:
                 hb_bwd()
                 if pair.gw:   # gradient landed in pair.g32 [B/2, 2Hb] == [B, Hb]
                     self.add_grad(fused, pair.g32.view(B, Hb))
-            if not hb.frozen:
-                self.push_bwd(bin_bwd)   # registered first => runs after the 2-way linear's backward
+            self.push_bwd(bin_bwd, hb.rg)   # registered first => runs after the 2-way linear's backward
             self.small_head("vil_binary_prediction", hb, "vil_binary_prediction.logit_fc.3", 2)
         elif want("vil_binary_prediction"):
             # odd batch: the reference returns the [B, 2] alignment output of self.cls here (:1673, 1686)
@@ -1552,14 +1535,13 @@ class Plan:
         # BertEncoder.forward interleaving schedule (vilbert.py:960-1096)
         t_start = v_start = 0
         for count, (v_end, t_end) in enumerate(zip(c.v_biattention_id, c.t_biattention_id)):
-            # fixed_t_layer / fixed_v_layer (vilbert.py:968-1003): the first layers of a stream run under no_grad — their backward is
-            # not emitted and their output stops the gradient (embeddings and the frozen layers' parameters receive none)
+            # fixed_t_layer / fixed_v_layer (vilbert.py:968-1003): the first layers of a stream run under no_grad — what they make
+            # needs no gradient (Plan.act), so their backward is not emitted and their output stops the gradient (embeddings and
+            # the frozen layers' parameters receive none)
             for i in range(t_start, t_end):
-                frozen = i < getattr(c, "fixed_t_layer", 0)
-                self._no_grad = frozen
+                self._no_grad = i < getattr(c, "fixed_t_layer", 0)
                 t = self.text_layer(t, i)
                 self._no_grad = False
-                t.frozen = t.frozen or frozen
             pool = None
             if self.dyn and v_end > v_start:
                 # dynamic_attention: this segment's image layers read the pooled text states of the segment's END (the text layers
@@ -1568,11 +1550,9 @@ class Plan:
                 self.sync_streams()
             with self.on(1):
                 for i in range(v_start, v_end):
-                    frozen = i < getattr(c, "fixed_v_layer", 0)
-                    self._no_grad = frozen
+                    self._no_grad = i < getattr(c, "fixed_v_layer", 0)
                     v = self.image_layer(v, i, pool)
                     self._no_grad = False
-                    v.frozen = v.frozen or frozen
             if count == 0 and self.fast:
                 t = self.broadcast_text(t)
             if count == 0 and self.pairs:
@@ -1599,7 +1579,7 @@ class Plan:
         self.outputs["pooled_output_t"] = self.pooled_t.f32
         self.outputs["pooled_output_v"] = self.pooled_v.f32
         for nm, act in (("sequence_output_t", t), ("sequence_output_v", v), ("pooled_output_t", self.pooled_t), ("pooled_output_v", self.pooled_v)):
-            self.out_rg[nm] = not act.frozen
+            self.out_rg[nm] = act.rg
         if self.heads != "none":
             self.build_heads(t, v, self.pooled_t, self.pooled_v)
             for nm in ("vision_prediction", "vision_logit"):
@@ -2223,7 +2203,7 @@ class Plan:
         return works
 
     def _live_cache(self, lo, hi):
-        c = self.__dict__.setdefault("_live_ranges_cache", {})
+        c = self._live_ranges_cache
         if (lo, hi) not in c:
             c[(lo, hi)] = self.live_ranges(lo, hi)
         return c[(lo, hi)]
@@ -2265,7 +2245,6 @@ class BasePlan(Plan):
         self.loss_inputs, self.head_grad = {}, {}
         self.loss = self.score = self.preds = None
         self.N = self.Nt + self.Nv
-        self._scatter_ok = False
         x = self.base_embeddings()
         self.enc = []
         for i in range(c.num_hidden_layers):
@@ -2275,8 +2254,8 @@ class BasePlan(Plan):
         self.pooled = self.base_pooler(x)
         self.outputs["sequence_output"] = x.f32.view(B, self.N, -1)
         self.outputs["pooled_output"] = self.pooled.f32
-        self.out_rg["sequence_output"] = not x.frozen
-        self.out_rg["pooled_output"] = not self.pooled.frozen
+        self.out_rg["sequence_output"] = x.rg
+        self.out_rg["pooled_output"] = self.pooled.rg
         views = self.build_base_heads(x, self.pooled) if self.heads == "base" else {}
         self.n_kernels_fwd = sum(1 for op in self.fwd if op[0] is not None)
 
@@ -2318,11 +2297,10 @@ class BasePlan(Plan):
         self.emit(lib.vb_concat_embed_ln_fwd, xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
                   ps.p(lnt + ".bias").data_ptr(), ps.p(lnv + ".weight").data_ptr(), ps.p(lnv + ".bias").data_ptr(), y32.data_ptr(), *y.ptrs(),
                   y.fp16, mean.data_ptr(), rstd.data_ptr(), B, Nt, Nv, H, self._ref(tdrop), self._ref(vdrop))
-        x = Act(y32, y, M, H)
         img = [ie + n for n in (".image_embeddings.weight", ".image_embeddings.bias", ".token_type_embeddings.weight",
                                 ".image_location_embeddings.weight", ".image_location_embeddings.bias")]
         lns = [lnt + ".weight", lnt + ".bias", lnv + ".weight", lnv + ".bias"]
-        x.frozen = not (self.input_grads or self.trainable(*t_tables, *img, *lns))
+        x = self.act(y32, y, M, H, params=(*t_tables, *img, *lns), rg=self.input_grads)
 
         def bwd():
             if not x.gw:
@@ -2342,8 +2320,7 @@ class BasePlan(Plan):
                 self.emit(lib.vb_embed_text_bwd_padded, dxt.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), *[self._ptr(g) for g in gt],
                           B, Nt, H)
             self.image_embedding_bwd(ie, H, feat, dxv16, dxv32)
-        if not x.frozen:
-            self.push_bwd(bwd)
+        self.push_bwd(bwd, x.rg)
         return x
 
     def base_layer(self, x, i):
@@ -2361,18 +2338,16 @@ class BasePlan(Plan):
         self.gemm(B, H, H, seq.op, N * H, ps.w(w + ".weight"), H, bias=ps.p(w + ".bias"), out_f32=pre, ld_of=H)
         y32, y = self.buf((B, H), F32), self.buf16((B, H))
         self.emit(self.lib.vb_tanh_fwd, pre.data_ptr(), y32.data_ptr(), *y.ptrs(), y.fp16, B * H)
-        pooled = Act(y32, y, B, H)
-        pooled.frozen = seq.frozen and not self.trainable(w + ".weight", w + ".bias")
+        pooled = self.act(y32, y, B, H, inputs=(seq,), params=(w,))
 
         def bwd():
             if not pooled.gw:
                 return
             dpre = self.scratch("pool.dpre", (B, H), BF16)
             self.emit(self.lib.vb_tanh_bwd, pooled.g32.data_ptr(), y32.data_ptr(), dpre.data_ptr(), self._ptr(self.pg(w + ".bias")), B, H)
-            self.linear_wgrad(dpre, H, None, 0, seq.op.bw, N * H, B, H, H, w)
+            self.linear_wgrad(dpre, H, seq.op.bw, N * H, B, H, H, w)
             self.pooler_dgrad(seq, N, dpre, w)
-        if not pooled.frozen:
-            self.push_bwd(bwd)
+        self.push_bwd(bwd, pooled.rg)
         return pooled
 
     def base_rows(self, seq, a, b, tag):
@@ -2382,16 +2357,14 @@ class BasePlan(Plan):
         n = b - a
         idx = self.buf((B * n,), torch.int32, zero=True)
         idx.copy_((torch.arange(B).view(B, 1) * N + torch.arange(a, b).view(1, n)).reshape(-1).to(torch.int32))
-        rows = Act(None, self.gather_rows(seq.op, idx, B * n, H), B * n, H)
-        rows.frozen = seq.frozen
+        rows = self.act(None, self.gather_rows(seq.op, idx, B * n, H), B * n, H, inputs=(seq,))
 
         def bwd():
             if not rows.gw:
                 return
-            g = self.grad_of(seq)
             if not seq.gw:      # the gathered heads' backward runs first: zero the stream gradient once, then scatter disjoint rows
-                self.emit(lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
-                seq.gw = self._scatter_ok = True
+                self._scatter_ok = True
+            g = self.grad_zeroed(seq)
             if self._scatter_ok:
                 self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), g.data_ptr(), idx.data_ptr(), B * n, H, None, None)
                 return
@@ -2399,8 +2372,7 @@ class BasePlan(Plan):
             self.emit(lib.vb_memset_zero, full.data_ptr(), full.numel() * 4)
             self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), full.data_ptr(), idx.data_ptr(), B * n, H, None, None)
             self.emit(lib.vb_axpy_f32, full.data_ptr(), g.data_ptr(), full.numel(), 1.0)
-        if not seq.frozen:
-            self.push_bwd(bwd)
+        self.push_bwd(bwd, rows.rg)
         return rows
 
     def base_simple_classifier(self, x):
@@ -2429,7 +2401,7 @@ class BasePlan(Plan):
         self.gemm(B, Lb, H2, h, H2, W[3][3], H2, bias=ps.p("vil_prediction.main.3.bias"), out_f32=logits, ld_of=Lb)
         self.outputs["vil_prediction"] = logits
         part = lambda i: [f"vil_prediction.main.{i}.{s}" for s in ("weight_g", "weight_v", "bias")]
-        h_rg = not x.frozen or self.trainable(*part(0))
+        h_rg = x.rg or self.trainable(*part(0))
         self.out_rg["vil_prediction"] = h_rg or self.trainable(*part(3))
         scale = 1.0 / (1.0 - p_drop) if drop is not None else 1.0
 
@@ -2465,8 +2437,7 @@ class BasePlan(Plan):
                 self.colsum(dpre32, H2, gb, B, H2)
             wn_wgrad(0, dpre16, H2, x.op.bw, H, B, H2, H)
             self.dgrad_into(x, dpre16, H2, W[0][3].bw, B, H2, H)
-        if self.out_rg["vil_prediction"]:
-            self.push_bwd(bwd)
+        self.push_bwd(bwd, self.out_rg["vil_prediction"])
 
     def build_base_heads(self, seq, pooled):
         """The seven outputs of BaseBertForVLTasks.forward (basebert.py:929-962). Returns the views of the whole-stream output-gradient
