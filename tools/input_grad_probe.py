@@ -51,7 +51,7 @@ def main():
         plan = eng.plan(B, Nt, Nv, **kw)
         plan.load_inputs(inp["input_txt"], inp["input_imgs"], inp["image_loc"], inp["token_type_ids"], inp["attention_mask"],
                          inp["image_attention_mask"], inp["task_ids"])
-        if plan.vqa_loss:
+        if plan.loss_kind == "vqa":
             plan.vqa_target.copy_(O.synth_vqa_target(B, 3129, device="cuda"))
         else:
             plan.gout["vil_prediction"].normal_()

@@ -23,7 +23,7 @@ activations and weights exist only as tensor-core operands. Three operand precis
 import ctypes as C
 import math
 import zlib
-from collections import OrderedDict
+from collections import OrderedDict, namedtuple
 
 import torch
 
@@ -348,12 +348,19 @@ PRETRAINING_HEAD_NAMES = ("linguisic_prediction", "vision_prediction", "seq_rela
 RESULT_MODES = {"vqa": ("vil_prediction", L.VB_RESULT_ARGMAX), "gqa": ("vil_prediction_gqa", L.VB_RESULT_ARGMAX),
                 "logit_ce": ("vil_logit", L.VB_RESULT_SOFTMAX), "vlogit_bce": ("vision_logit", L.VB_RESULT_GATHER),
                 "vlogit_mc": ("vision_logit", L.VB_RESULT_ARGMAX)}
+# how the objective, score and results of a task kind address its head (Plan._head_layout): column c of row r is
+# logits[r * ld + off + c], or with ids (the loss_inputs entry of the int64 [rows, cols] choice ids) logits[r * ld + off + ids[r, c]]
+# with width the columns an id may reach; key is the loss_inputs entry of its labels (int64 [rows]) or targets (f32 [rows, cols])
+HeadLayout = namedtuple("HeadLayout", "name logits rows cols ld off ids width key")
 
 
 class Plan:
     """Static execution plan for one input shape. `grad_outputs` names the outputs that will receive a
-    gradient in backward (dead branches are not emitted); `vqa_loss` fuses the VQA BCE objective
-    (task_utils.py:325-327) and its gradient after the forward.
+    gradient in backward (dead branches are not emitted). `loss` fuses an objective of LOSS_HEADS into the plan: by default its
+    kernel starts the backward, writes its scalar to self.loss and writes d loss / d head into the head's output-gradient buffer
+    (loss="vqa", the round-1 objective of task_utils.py:325-327, also writes the head's bf16 backward operand, so no cast runs).
+    Its labels and targets are static plan inputs (self.loss_inputs); the objective, score and results of a task kind address
+    its head through one layout (_head_layout), and _objective_outputs sets up where their scalars land.
 
     Task objectives (TASK_KINDS) take three more options. loss_in_forward=True emits the objective at the END of the forward list
     (a forward-only plan yields the loss) and stores d loss / d head; the backward then starts with head gradient = stored gradient
@@ -391,7 +398,7 @@ class Plan:
     grad_touch; self.input_grad maps each input whose gradient the backward writes to its buffer ([B*Nv, Fv] / [B*Nv, 5] fp32). An
     input behind a no_grad layer (fixed_v_layer > 0) gets no entry, as it gets no gradient in torch."""
 
-    def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
+    def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
                  loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
                  input_grads=frozenset()):
         self.e, self.cfg = engine, engine.cfg
@@ -410,7 +417,7 @@ class Plan:
         self.lib = L.lib()
         self.dev = engine.device
         self.Bin = B
-        self._stream_modes(B, Nt, Nv, train, grad_outputs, vqa_loss, loss, fast_mode, image_prefix)
+        self._stream_modes(B, Nt, Nv, train, grad_outputs, loss, fast_mode, image_prefix)
         if self.input_grads and (self.fast or self.image_prefix):
             raise ValueError("fast_mode and image_prefix plans are inference paths: no input gradients")
         self.attn_t, self.attn_v, self.attn_c = [], [], []
@@ -418,8 +425,8 @@ class Plan:
         self._private = False    # while set, buf() allocates private buffers (the image states of image_prefix)
         self.grad_outputs = frozenset(grad_outputs)
         # objective fused into the step (LOSS_HEADS): its scalar lands in self.loss (device) and its gradient goes straight into the
-        # backward of the head(s) it reads; vqa_loss=True is the round-1 spelling of loss="vqa"
-        self.loss_kind = "vqa" if vqa_loss else loss
+        # backward of the head(s) it reads
+        self.loss_kind = loss
         if self.loss_kind is not None and self.loss_kind not in LOSS_HEADS:
             raise ValueError(f"loss must be one of {sorted(LOSS_HEADS)}")
         self.loss_in_forward, self.want_score, self.choices = bool(loss_in_forward), bool(score), choices
@@ -433,7 +440,6 @@ class Plan:
             raise ValueError("loss='vlogit_mc' needs choices= (multiple-choice ids per sample)")
         if self.loss_kind == "vlogit_mc" and Nv <= MC_REGION_OFFSET:
             raise ValueError(f"loss='vlogit_mc' scores the regions after the first {MC_REGION_OFFSET}: Nv must exceed it")
-        self.vqa_loss = self.loss_kind == "vqa" and not self.task_objective
         self.train = bool(train)          # nn.Dropout layers active (model.train()); False = the reference's eval mode
         self.op_dtype, self.split = engine.op_dtype, engine.split   # format of the forward operands (activations, weights)
         self.head_dropout_prob = engine.head_dropout_prob
@@ -465,7 +471,7 @@ class Plan:
         self._arena_off = self.arena_bytes = 0
         self._build()
 
-    def _stream_modes(self, B, Nt, Nv, train, grad_outputs, vqa_loss, loss, fast_mode, image_prefix):
+    def _stream_modes(self, B, Nt, Nv, train, grad_outputs, loss, fast_mode, image_prefix):
         """Shapes and checks of the two-stream options: in_batch_pairs, the task token, visualization, dynamic_attention,
         fast_mode and image_prefix."""
         # in_batch_pairs (vilbert.py:1008-1040): at the first connection layer every (text i, image j) combination of the input
@@ -482,10 +488,10 @@ class Plan:
         self.dyn = bool(getattr(self.cfg, "dynamic_attention", False))
         self.fast = bool(getattr(self.cfg, "fast_mode", False)) if fast_mode is None else bool(fast_mode)
         self.Bt = 1 if self.fast else B
-        if self.fast and (train or grad_outputs or vqa_loss or loss):
+        if self.fast and (train or grad_outputs or loss):
             raise ValueError("fast_mode is an inference path (text batch 1 broadcast to the image batch): no train mode / gradients")
         self.image_prefix = bool(image_prefix)
-        if self.image_prefix and (train or grad_outputs or vqa_loss):
+        if self.image_prefix and (train or grad_outputs):
             raise ValueError("image_prefix keeps the image states across forwards: forward-only plans (no train mode, no grad_outputs)")
         if self.image_prefix and self.pairs:
             raise ValueError("image_prefix: in_batch_pairs re-expands the image batch inside the forward")
@@ -1263,7 +1269,8 @@ class Plan:
 
     def big_head(self, name, x, ld_x, M, K_in, N_out, wname, bias_name, w=None, gw_name=None):
         """Wide linear head (N_out in the thousands): logits = x W^T + b as fp32 [M, N_out]; backward from a
-        caller-supplied fp32 d(logits) (cast to a bf16 operand with an 8-padded row pitch). w / gw_name: a weight and the entry of
+        caller-supplied fp32 d(logits), cast to a bf16 operand with an 8-padded row pitch unless the objective registered one it
+        writes itself (self.head_dl16). w / gw_name: a weight and the entry of
         its gradient not named by `wname` (the decoder tied to the word embeddings). The backward returns None when nothing
         below the logits takes a gradient."""
         ps = self.ps
@@ -1278,10 +1285,8 @@ class Plan:
             if name not in self.grad_outputs or not self.out_rg[name]:
                 return None
             ldp = _pad8(N_out)
-            if self.vqa_loss and name == "vil_prediction":
-                dl32, dl16 = self.vqa_dl32, self.vqa_dl16
-            else:
-                dl32 = self.out_grad_buffer(name, (M, N_out))
+            dl32, dl16 = self.out_grad_buffer(name, (M, N_out)), self.head_dl16.get(name)
+            if dl16 is None:
                 dl16 = self.scratch("head.dl16." + name, (M, ldp), BF16)
                 self.emit(self.lib.vb_cast2d_f32_to_bf16, dl32.data_ptr(), N_out, dl16.data_ptr(), ldp, M, N_out, 1.0)
             gb = self.pg(bias_name)
@@ -1342,7 +1347,7 @@ class Plan:
             gc = self.scratch("lm.gc", (cap, Ht), F32)
             self.gemm(cap, Ht, V, lc["dl16"], ldp, ps.w(wn).bw, Ht, b_mn=1, out_f32=gc, ld_of=Ht)
             g = self.grad_zeroed(ht)
-            self.emit(lib.vb_scatter_rows_f32, gc.data_ptr(), g.data_ptr(), idx.data_ptr(), cap, Ht, cnt.data_ptr(), self._lm_loss().data_ptr())
+            self.emit(lib.vb_scatter_rows_f32, gc.data_ptr(), g.data_ptr(), idx.data_ptr(), cap, Ht, cnt.data_ptr(), self.loss_slots[0].data_ptr())
             ht_bwd()
         return bwd
 
@@ -1354,10 +1359,6 @@ class Plan:
         if op.lo is not None:
             self.emit(self.lib.vb_gather_rows16, src.lo.data_ptr(), op.lo.data_ptr(), None, None, idx.data_ptr(), rows, H)
         return op
-
-    def _lm_loss(self):
-        """Where the masked-LM loss lands: the summed scalar, or the first slot of the three-slot pre-training objective."""
-        return self.loss if self.loss is not None else self.objective_out[0:1]
 
     def lm_rows(self):
         """(labelled rows of the last step, capacity) of the compacted masked-LM head (device sync)."""
@@ -1492,9 +1493,10 @@ class Plan:
             # odd batch: the reference returns the [B, 2] alignment output of self.cls here (:1673, 1686)
             self.small_head("vil_binary_prediction", fused_cls, "cls.bi_seq_relationship", 2)
 
-        for nm, n_out in (("vil_prediction", 3129), ("vil_prediction_gqa", 1533)):
+        for nm in ("vil_prediction", "vil_prediction_gqa"):
             if not want(nm):
                 continue
+            n_out = ps.p(nm + ".logit_fc.3.weight").shape[0]     # the answer vocabulary
             hh, hh_bwd = self.transform(fused, nm + ".logit_fc.0", nm + ".logit_fc.2", nm + ".tr")
             head_bwd = self.big_head(nm, hh, 2 * Hb, B, 2 * Hb, n_out, nm + ".logit_fc.3", nm + ".logit_fc.3.bias")
             self.push_bwd(self._wide_bwd(head_bwd, hh, hh_bwd, 2 * Hb, n_out))
@@ -1512,24 +1514,7 @@ class Plan:
     def _build(self):
         c, B = self.cfg, self.B
         self.outputs, self.gout = OrderedDict(), {}
-        self.loss_inputs = {}
-        self.head_grad = {}           # loss_in_forward: d loss / d head, written by the forward-placed objective
-        self.score = self.preds = None
-        if self.task_objective and self.loss_kind == "pretraining":
-            # masked_lm, masked_img, next_sentence side by side: one device-to-host copy reads all three
-            self.objective_out = self.buf((3,), F32, zero=True)
-            self.loss = None
-        elif self.results is not None:
-            self._alloc_results()
-            self.loss = self.objective_out[0:1] if self.task_objective else None
-            self.score = self.objective_out[1:2] if self.want_score else None
-        elif self.task_objective:
-            # loss and score side by side: one device-to-host copy reads both
-            self.objective_out = self.buf((2,), F32, zero=True)
-            self.loss = self.objective_out[0:1]
-            self.score = self.objective_out[1:2] if self.want_score else None
-        else:
-            self.loss = self.buf((1,), F32, zero=True) if (self.loss_kind is not None and not self.vqa_loss) else None
+        self._objective_outputs()
         self.enc_t, self.enc_v = [], []
         t, v = self.embeddings()
         # BertEncoder.forward interleaving schedule (vilbert.py:960-1096)
@@ -1599,14 +1584,6 @@ class Plan:
         self.cur = self.bwd
         if self.loss_in_forward:
             self._emit_grad_scale()
-        elif self.vqa_loss:
-            lg = self.outputs["vil_prediction"]
-            self.vqa_target = self.buf(tuple(lg.shape), F32, zero=True)
-            self.loss = self.buf((1,), F32, zero=True)
-            self.vqa_dl32 = self.buf(tuple(lg.shape), F32)
-            self.vqa_dl16 = self.buf((lg.shape[0], _pad8(lg.shape[1])), BF16, zero=True)
-            self.emit(self.lib.vb_bce_logits_loss, lg.data_ptr(), self.vqa_target.data_ptr(), self.loss.data_ptr(), self.vqa_dl32.data_ptr(),
-                      self.vqa_dl16.data_ptr(), _pad8(lg.shape[1]), lg.shape[0], lg.shape[1], 1.0)
         elif self.loss_kind is not None:
             self._emit_loss()
         self._emit_backward((("sequence_output_t", self.seq_t), ("sequence_output_v", self.seq_v), ("pooled_output_t", self.pooled_t),
@@ -1645,62 +1622,95 @@ class Plan:
                "attn2": a2["attn"].clone(), "querues2": qk(a2, "q", a2["Nq"]), "keys2": qk(a2, "k", a2["Nk"])} for a1, a2 in self.attn_c]
         return ts, vs, cs
 
+    def _objective_outputs(self):
+        """Where the fused objective's scalars land, for every kind of plan (all None without an objective):
+        - summed (loss= without loss_in_forward or score): self.loss, a private device f32 [1];
+        - forward-placed task objective: self.objective_out f32 [2] holds (loss, score), read with one copy; self.loss and self.score
+          (None without score=True) are its slots;
+        - forward-placed pre-training: self.objective_out f32 [3] holds (masked_lm, masked_img, next_sentence); self.loss is None;
+        - results=: self.results_out, one private byte buffer, holds objective_out (loss, score), the per-row argmax
+          (self.results_argmax, int64) and values (self.results_values, f32), read with one copy (fetch_results). VL-logit has a row
+          per question and a value per option, V-logit one value (the IoU) per row.
+        self.loss_slots are the three scalars the pre-training losses land in (the summed loss three times). self.preds (sized by the
+        head) and self.loss_grad (read by the backward) are created by _emit_score and _emit_grad_scale."""
+        k, r = self.loss_kind, self.results
+        self.loss_inputs = {}
+        self.head_grad = {}     # loss_in_forward: d loss / d head, written by the forward-placed objective
+        self.head_dl16 = {}     # head name -> the bf16 gradient operand the objective writes for big_head
+        self.loss = self.score = self.preds = self.loss_grad = self.objective_out = self.results_out = None
+        if r is not None:
+            opts = self.choices or self.e.loss_options
+            rows = self.B // opts if r == "logit_ce" else self.B
+            nval = {L.VB_RESULT_SOFTMAX: opts, L.VB_RESULT_GATHER: 1}.get(RESULT_MODES[r][1], 0)
+            self.results_out = self.buf((8 + 8 * rows + 4 * rows * nval,), torch.uint8, zero=True)
+            self.objective_out = self.results_out[:8].view(F32)
+            self.results_argmax = self.results_out[8:8 + 8 * rows].view(I64)
+            self.results_values = self.results_out[8 + 8 * rows:].view(F32).view(rows, nval) if nval else None
+        elif self.task_objective:
+            self.objective_out = self.buf((3 if k == "pretraining" else 2,), F32, zero=True)
+        elif k is not None:
+            self.loss = self.buf((1,), F32, zero=True)
+        if self.task_objective and k != "pretraining":
+            self.loss = self.objective_out[0:1]
+        if self.want_score:
+            self.score = self.objective_out[1:2]
+        pre = self.task_objective and k == "pretraining"
+        self.loss_slots = [self.objective_out[i:i + 1] for i in range(3)] if pre else [self.loss] * 3
+
+    def _head_layout(self, k):
+        """The HeadLayout of task kind k. A classifier head is read whole, a row per sample (per sample pair for the binary head at
+        even B); VL-logit has a row per question over its answer options; V-logit-mc gathers its choices from the regions after
+        the first MC_REGION_OFFSET. Describes only: the objective creates the loss_inputs entries (_emit_loss)."""
+        name = LOSS_HEADS[k][0]
+        lg = self.outputs[name]
+        rows, cols = lg.shape[0], lg.shape[1]
+        key = "labels" if k in ("logit_ce", "binary_ce", "tri_ce") else "target"
+        if k == "logit_ce":       # vil_logit.view(B / options, options)
+            opts = self.choices or self.e.loss_options
+            if rows % opts:
+                raise ValueError(f"loss='logit_ce': batch {rows} is not a multiple of {opts} options")
+            return HeadLayout(name, lg, rows // opts, opts, opts, 0, None, 0, key)
+        if k == "vlogit_mc":      # vision_logit[:, 101:].gather(1, ids)
+            return HeadLayout(name, lg, rows, int(self.choices), cols, MC_REGION_OFFSET, "multiple_choice_ids", cols, key)
+        return HeadLayout(name, lg, rows, cols, cols, 0, None, 0, key)
+
     def _emit_loss(self):
-        """Fused objectives other than "vqa": one loss kernel per head writes the scalar (self.loss, fp32 device) and the fp32
-        d(loss)/d(head output) into the plan's output-gradient buffer, from where the head's backward proceeds as for a
-        caller-supplied gradient. Labels / targets are static plan inputs (self.loss_inputs)."""
-        lib, B, k = self.lib, self.B, self.loss_kind
+        """The fused objective: one loss kernel per head writes the scalar (self.loss, fp32 device) and the fp32 d(loss)/d(head
+        output) into the plan's output-gradient buffer, from where the head's backward proceeds as for a caller-supplied gradient
+        (loss_in_forward: into a buffer of its own, _head_grad). Labels / targets are static plan inputs (self.loss_inputs), laid
+        out as the head is (_head_layout)."""
+        lib, k, li = self.lib, self.loss_kind, self.loss_inputs
         missing = [n for n in LOSS_HEADS[k] if n not in self.grad_outputs]
         if missing and not self.loss_in_forward:      # a forward-placed objective also serves forward-only (eval) plans
             raise ValueError(f"loss={k!r} differentiates {LOSS_HEADS[k]}: add them to grad_outputs")
-        li = self.loss_inputs
-
-        def ce(name, rows, cols, label_key, acc):
-            lg = self.outputs[name]
-            li[label_key] = self.buf((rows,), I64, zero=True)
-            d = self._head_grad(name, tuple(lg.shape))
-            self.emit(lib.vb_ce_loss, lg.data_ptr(), cols, li[label_key].data_ptr(), -1, self.loss.data_ptr(), d.data_ptr(), cols, None, 0,
-                      rows, cols, 1.0, 1 if acc else 0)
-
-        def bce(name, rows, cols):
-            lg = self.outputs[name]
-            li["target"] = self.buf((rows, cols), F32, zero=True)
-            d = self._head_grad(name, tuple(lg.shape))
-            self.emit(lib.vb_bce_logits_loss, lg.data_ptr(), li["target"].data_ptr(), self.loss.data_ptr(), d.data_ptr(), None, 0, rows, cols, 1.0)
-
-        def bce_gather(name, rows, width, C, off, ids, loss_mul):
-            lg = self.outputs[name]
-            li["target"] = self.buf((rows, C), F32, zero=True)
-            d = self._head_grad(name, tuple(lg.shape))
-            row_loss = self.buf((rows,), F32)
-            self.emit(lib.vb_bce_gather_loss, lg.data_ptr(), width, off, width, self._ptr(ids), li["target"].data_ptr(), rows, C, float(loss_mul),
-                      row_loss.data_ptr(), self.loss.data_ptr(), 0, d.data_ptr(), width, None, 0)
-
-        if k == "vqa":      # task objective path only (the round-1 path is vqa_loss)
-            bce("vil_prediction", B, 3129)
-        elif k == "gqa":
-            bce("vil_prediction_gqa", B, 1533)
-        elif k == "vlogit_bce":
-            bce("vision_logit", B, self.Nv)
-        elif k == "logit_ce":
-            opts = self.choices or self.e.loss_options
-            if B % opts:
-                raise ValueError(f"loss='logit_ce': batch {B} is not a multiple of {opts} options")
-            ce("vil_logit", B // opts, opts, "labels", False)
-        elif k == "binary_ce":
-            ce("vil_binary_prediction", self.outputs["vil_binary_prediction"].shape[0], 2, "labels", False)
-        elif k == "tri_ce":
-            ce("vil_tri_prediction", B, 3, "labels", False)
-        elif k == "vlogit_mc":
-            C = int(self.choices)
-            li["multiple_choice_ids"] = self.buf((B, C), I64, zero=True)
-            bce_gather("vision_logit", B, self.Nv, C, MC_REGION_OFFSET, li["multiple_choice_ids"], C)
-        elif k in ("binary_bce", "tri_bce"):
-            name = "vil_binary_prediction" if k == "binary_bce" else "vil_tri_prediction"
-            cols = 2 if k == "binary_bce" else 3
-            bce_gather(name, self.outputs[name].shape[0], cols, cols, 0, None, 1.0)
-        elif k == "pretraining":
+        if k == "pretraining":
             self._emit_pretraining_loss()
+            return
+        h = self._head_layout(k)
+        if h.ids is not None:
+            li[h.ids] = self.buf((h.rows, h.cols), I64, zero=True)
+        li[h.key] = self.buf((h.rows,), I64, zero=True) if h.key == "labels" else self.buf((h.rows, h.cols), F32, zero=True)
+        lg, inp, loss = h.logits.data_ptr(), li[h.key].data_ptr(), self.loss.data_ptr()
+        if k == "vqa":
+            self.vqa_target = li["target"]      # the VQA soft target under its round-1 name
+        if h.key == "labels":
+            d = self._head_grad(h.name, tuple(h.logits.shape))
+            self.emit(lib.vb_ce_loss, lg, h.ld, inp, -1, loss, d.data_ptr(), h.ld, None, 0, h.rows, h.cols, 1.0, 0)
+        elif k in ("vqa", "gqa", "vlogit_bce"):
+            if k == "vqa" and not self.task_objective:
+                # the summed VQA objective (the round-1 training step) also writes the bf16 operand of the wide head's backward GEMMs
+                # (8-padded rows), registered for big_head so that no cast follows; its fp32 gradient is rewritten every backward
+                d = self.gout[h.name] = self.buf(tuple(h.logits.shape), F32)
+                d16 = self.head_dl16[h.name] = self.buf((h.rows, _pad8(h.cols)), BF16, zero=True)
+            else:
+                d, d16 = self._head_grad(h.name, tuple(h.logits.shape)), None
+            self.emit(lib.vb_bce_logits_loss, lg, inp, loss, d.data_ptr(), self._ptr(d16), 0 if d16 is None else d16.shape[1], h.rows,
+                      h.cols, 1.0)
+        else:   # V-logit-mc: BCE mean x C over the gathered choices; the soft-target binary / tri heads: BCE mean
+            d = self._head_grad(h.name, tuple(h.logits.shape))
+            row_loss = self.buf((h.rows,), F32)
+            self.emit(lib.vb_bce_gather_loss, lg, h.ld, h.off, h.ld, self._ptr(li.get(h.ids)), inp, h.rows, h.cols,
+                      float(h.cols if k == "vlogit_mc" else 1.0), row_loss.data_ptr(), loss, 0, d.data_ptr(), h.ld, None, 0)
         if self.want_score:
             self._emit_score()
 
@@ -1712,8 +1722,7 @@ class Plan:
         its slot of self.objective_out and each gradient a buffer of its own (none in a forward-only plan)."""
         lib, B, Nv, li, c = self.lib, self.B, self.Nv, self.loss_inputs, self.cfg
         V, C, R = c.vocab_size, c.v_target_size, Nv - 1
-        sep = self.loss_in_forward
-        slot = [self.objective_out[i:i + 1] for i in range(3)] if sep else [self.loss] * 3
+        sep, slot = self.loss_in_forward, self.loss_slots
         acc = 0 if sep else 1           # the summed plan adds the region and alignment losses to the masked-LM loss
 
         def grad(name, shape):
@@ -1776,67 +1785,32 @@ class Plan:
 
     def _emit_score(self):
         """The batch score of the task objective (task_utils.py:121-162, 325-374, 618-623) into self.score, argmax per row into
-        self.preds, from the head logits and the objective's own inputs."""
-        k, li, B, Nv = self.loss_kind, self.loss_inputs, self.B, self.Nv
-        mode = SCORE_MODES[k]
-        ids, width, off, labels, target = None, 0, 0, None, li.get("target")
-        if k in ("vqa", "gqa", "binary_bce", "tri_bce"):
-            lg = self.outputs[LOSS_HEADS[k][0]]
-            rows, cols = lg.shape[0], lg.shape[1]
-        elif k == "logit_ce":
-            lg, labels = self.outputs["vil_logit"], li["labels"]
-            cols = self.choices or self.e.loss_options
-            rows = B // cols
-        elif k == "vlogit_bce":
-            lg, rows, cols = self.outputs["vision_logit"], B, Nv
-        else:   # vlogit_mc
-            lg, rows, cols = self.outputs["vision_logit"], B, int(self.choices)
-            ids, width, off = li["multiple_choice_ids"], Nv, MC_REGION_OFFSET
-        ld = Nv if k in ("vlogit_bce", "vlogit_mc") else cols
-        self.preds = self.buf((rows,), I64, zero=True)
-        self.emit(self.lib.vb_task_score, mode, lg.data_ptr(), ld, off, cols, self._ptr(ids), width, self._ptr(target),
-                  cols if target is not None else 0, self._ptr(labels), rows, self.score.data_ptr(), 0, self.preds.data_ptr())
-
-    def _results_shape(self):
-        """(rows, columns, values per row) of the results of self.results: VL-logit has a row per question over its options."""
-        k = self.results
-        if k in ("vqa", "gqa"):
-            return self.B, (3129 if k == "vqa" else 1533), 0
-        if k == "logit_ce":
-            opts = self.choices or self.e.loss_options
-            return self.B // opts, opts, opts
-        if k == "vlogit_bce":
-            return self.B, self.Nv, 1
-        return self.B, int(self.choices), 0          # vlogit_mc
-
-    def _alloc_results(self):
-        """One private device buffer: objective_out (f32 loss, score), the per-row argmax (int64) and the per-row values (f32)."""
-        rows, _, nval = self._results_shape()
-        self.results_out = self.buf((8 + 8 * rows + 4 * rows * nval,), torch.uint8, zero=True)
-        self.objective_out = self.results_out[:8].view(F32)
-        self.results_argmax = self.results_out[8:8 + 8 * rows].view(I64)
-        self.results_values = self.results_out[8 + 8 * rows:].view(F32).view(rows, nval) if nval else None
+        self.preds, from the head logits and the objective's own labels or targets."""
+        h, li = self._head_layout(self.loss_kind), self.loss_inputs
+        labels, target = (li["labels"], None) if h.key == "labels" else (None, li["target"])
+        self.preds = self.buf((h.rows,), I64, zero=True)
+        self.emit(self.lib.vb_task_score, SCORE_MODES[self.loss_kind], h.logits.data_ptr(), h.ld, h.off, h.cols, self._ptr(li.get(h.ids)),
+                  h.width, self._ptr(target), h.cols if target is not None else 0, self._ptr(labels), h.rows, self.score.data_ptr(), 0,
+                  self.preds.data_ptr())
 
     def _emit_results(self):
-        """vb_task_results on the head of self.results (RESULT_MODES), addressed as the score kernel addresses it."""
-        k, li, Nv = self.results, self.loss_inputs, self.Nv
-        name, mode = RESULT_MODES[k]
-        rows, cols, nval = self._results_shape()
-        ids, width, off, target, ld = None, 0, 0, None, cols
-        if k == "vlogit_bce":
-            target = li["target"]
-        elif k == "vlogit_mc":
-            ids, width, off, ld = li["multiple_choice_ids"], Nv, MC_REGION_OFFSET, Nv
-        self.emit(self.lib.vb_task_results, mode, self.outputs[name].data_ptr(), ld, off, cols, self._ptr(ids), width, self._ptr(target),
-                  Nv if target is not None else 0, rows, self.results_argmax.data_ptr(), self._ptr(self.results_values), max(nval, 1))
+        """vb_task_results on the head of self.results (RESULT_MODES), addressed as the objective and the score address it; the
+        V-logit results read the target at the chosen region (its IoU)."""
+        h, mode = self._head_layout(self.results), RESULT_MODES[self.results][1]
+        target = self.loss_inputs["target"] if mode == L.VB_RESULT_GATHER else None
+        vals = self.results_values
+        self.emit(self.lib.vb_task_results, mode, h.logits.data_ptr(), h.ld, h.off, h.cols, self._ptr(self.loss_inputs.get(h.ids)), h.width,
+                  self._ptr(target), h.cols if target is not None else 0, h.rows, self.results_argmax.data_ptr(), self._ptr(vals),
+                  1 if vals is None else vals.shape[1])
 
     def fetch_results(self):
         """Reads results_out with one device-to-host copy: (loss, score, argmax int64 [rows], values f32 [rows, n] or None) on the
         host. loss and score are 0 where the plan has no objective / score."""
         raw = self.results_out.cpu()
-        rows, _, nval = self._results_shape()
+        rows, vals = self.results_argmax.numel(), self.results_values
         loss, score = raw[:8].view(F32).tolist()
-        vals = raw[8 + 8 * rows:].view(F32).view(rows, nval) if nval else None
+        if vals is not None:
+            vals = raw[8 + 8 * rows:].view(F32).view(vals.shape)
         return loss, score, raw[8:8 + 8 * rows].view(I64), vals
 
     def _emit_grad_scale(self):
@@ -2223,10 +2197,10 @@ class BasePlan(Plan):
     two-stream options (batch pairs, task token, fast mode, gate, attention export), and its plans take grad_outputs, train and
     frozen only: no fused objective, outputs= selection or image prefix."""
 
-    def __init__(self, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
+    def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
                  loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
                  input_grads=frozenset()):
-        if (vqa_loss or loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
+        if (loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
                 or loss_in_forward):
             raise ValueError("single-stream baseline plans support grad_outputs, train, frozen and input_grads only")
         super().__init__(engine, B, Nt, Nv, grad_outputs, heads=heads, train=train, choices=choices, frozen=frozen, input_grads=input_grads)
@@ -2242,8 +2216,7 @@ class BasePlan(Plan):
         back; the 1-output heads run over the whole stream with a zero output gradient on the rows they do not return."""
         c, B = self.cfg, self.B
         self.outputs, self.gout = OrderedDict(), {}
-        self.loss_inputs, self.head_grad = {}, {}
-        self.loss = self.score = self.preds = None
+        self._objective_outputs()
         self.N = self.Nt + self.Nv
         x = self.base_embeddings()
         self.enc = []
@@ -2512,8 +2485,8 @@ class Engine:
     def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
              loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
              input_grads=frozenset()):
-        """The cached plan of this shape and these options (Plan). frozen: ParamStore entry names that take no gradient;
-        input_grads: the inputs of INPUT_GRAD_NAMES the backward also differentiates."""
+        """The cached plan of this shape and these options (Plan). vqa_loss=True is the round-1 spelling of loss="vqa"; frozen:
+        ParamStore entry names that take no gradient; input_grads: the inputs of INPUT_GRAD_NAMES the backward also differentiates."""
         frozen, input_grads = frozenset(frozen), frozenset(input_grads)
         loss = "vqa" if vqa_loss else loss
         pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
@@ -2525,7 +2498,7 @@ class Engine:
         while len(self.plans) >= self.max_plans:   # evict the least recently used plan: its buffers go back to the allocator
             self.plans.popitem(last=False)
         self.plans[key] = (BasePlan if self.ps.base else Plan)(
-            self, B, Nt, Nv, grad_outputs, False, heads, train, loss=loss, choices=choices, score=score, loss_in_forward=loss_in_forward,
+            self, B, Nt, Nv, grad_outputs, heads, train, loss=loss, choices=choices, score=score, loss_in_forward=loss_in_forward,
             outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen, input_grads=input_grads)
         return self.plans[key]
 
