@@ -205,6 +205,21 @@ vb_status vb_layernorm_bwd(const float* dy, int64_t lddy, const float* x, int64_
                            const vb_dropout* in_dropout  /* NULL or the mask applied to the dense output feeding this LN: dx_bf16 / dbias are masked */,
                            void* stream);
 
+/* The LayerNorm of the residual stream with the residual add fused in: LN(x), x = dropout(d) + residual (BertSelfOutput /
+ * BertOutput / BertBiOutput, vilbert.py:470-474, 513-517, 844-855). d f32 [M,H] is the dense output alpha*acc + bias that
+ * vb_gemm_bf16 stores without a residual; x is formed exactly as that GEMM's epilogue forms it with `residual` and `dropout`
+ * (mask index row*H + col, then one fp32 add), so both paths give the same bits. d and residual share ld (== H when dropout is
+ * set). x_out: NULL, or d itself: x is written over d (what vb_add_layernorm_bwd's x then reads). Outputs as vb_layernorm_fwd. */
+vb_status vb_add_layernorm_fwd(const float* d, const float* residual, int64_t ld, const vb_dropout* dropout /* may be NULL */,
+                               float* x_out, const float* gamma, const float* beta, float eps, float* y_f32, void* y_bf16, int64_t ldy,
+                               float* mean, float* rstd, int32_t M, int32_t H, int32_t y_fp16, void* y_lo, void* y_b16, void* stream);
+/* vb_layernorm_bwd of dy + dy2 (both f32 [M,H], pitch lddy): the gradient of the LayerNorm output arrives in two parts, the one a
+ * dgrad GEMM wrote and the residual-path gradient that GEMM's epilogue would otherwise have added (same fp32 addition). */
+vb_status vb_add_layernorm_bwd(const float* dy, const float* dy2, int64_t lddy, const float* x, int64_t ldx, const float* gamma,
+                               const float* mean, const float* rstd, float* dx_f32, void* dx_bf16, int64_t lddx,
+                               const void* gelu_pre, int64_t ld_pre, float* dgamma, float* dbeta, float* dbias,
+                               int32_t M, int32_t H, const vb_dropout* out_dropout, const vb_dropout* in_dropout, void* stream);
+
 /* fp32 -> 16-bit casts: flat (weights shadow, region-feature ingest; bf16 or fp16, optionally hi + lo) and 2-D with independent leading
  * dimensions and a scale (pads operands whose row length is not a multiple of 8). */
 vb_status vb_cast_f32_to_bf16(const float* src, void* dst, int64_t n, int32_t fp16 /* 0 = bf16, 1 = fp16 */,

@@ -83,6 +83,8 @@ _SIGNATURES = {
     "vb_attention_probs": [C.POINTER(AttnArgs), _P, _P],
     "vb_layernorm_fwd": [_P, _I64, _P, _P, _F, _P, _P, _I64, _P, _P, _I32, _I32, _P, _I32, _P, _P, _P],
     "vb_layernorm_bwd": [_P, _I64, _P, _I64, _P, _P, _P, _P, _P, _I64, _P, _I64, _P, _P, _P, _I32, _I32, _P, _P, _P],
+    "vb_add_layernorm_fwd": [_P, _P, _I64, _P, _P, _P, _P, _F, _P, _P, _I64, _P, _P, _I32, _I32, _I32, _P, _P, _P],
+    "vb_add_layernorm_bwd": [_P, _P, _I64, _P, _I64, _P, _P, _P, _P, _P, _I64, _P, _I64, _P, _P, _P, _I32, _I32, _P, _P, _P],
     "vb_cast_f32_to_bf16": [_P, _P, _I64, _I32, _P, _P, _P],
     "vb_cast2d_f32_to_bf16": [_P, _I64, _P, _I64, _I32, _I32, _F, _P],
     "vb_embed_text_fwd": [_P, _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _P],

@@ -29,17 +29,22 @@ static inline int row_grid(long long rows) {
 }
 
 // ------------------------------------------------------------------------------------------ LayerNorm fwd
-template <int NV4>
+// ADD: the LayerNorm of a residual stream, LN(dropout(d) + r) (BertSelfOutput / BertOutput / BertBiOutput): x = drop_in(d) + r is
+// formed here, in the order the GEMM epilogue would form it (mask index row*H + col, then one fp32 add), and written over d when
+// x_out is set (the backward reads it). The dense GEMM before it then stores d and reads nothing: its epilogue has no DRAM round
+// trip on the tensor cores' critical path, while this kernel has many warps per SM to hide the extra read.
+template <int NV4, bool ADD>
 __global__ void __launch_bounds__(ROW_THREADS)
-ln_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __restrict__ gamma, const float* __restrict__ beta,
+ln_fwd_kernel(const float* x, long long ldx, const float* __restrict__ gamma, const float* __restrict__ beta,
               float eps, float* __restrict__ y32, __nv_bfloat16* __restrict__ y16, long long ldy, float* __restrict__ mean_out,
               float* __restrict__ rstd_out, int M, int H, const DropCfg drop, int y_fp16, __nv_bfloat16* __restrict__ y_lo,
-              __nv_bfloat16* __restrict__ y_b16) {
+              __nv_bfloat16* __restrict__ y_b16, const float* __restrict__ r, long long ldr, const DropCfg drop_in, float* x_out) {
   pdl_entry();
   const int lane = threadIdx.x & 31;
   const int n4 = H >> 2;
   const float inv_h = 1.f / (float)H;
   const uint32_t dseed = drop.ctr ? drop_seed(drop) : 0u;
+  const uint32_t seed_in = (ADD && drop_in.ctr) ? drop_seed(drop_in) : 0u;
   for (long long row = (long long)blockIdx.x * ROW_WARPS + (threadIdx.x >> 5); row < M; row += (long long)gridDim.x * ROW_WARPS) {
     const float4* xr = reinterpret_cast<const float4*>(x + row * ldx);
     float4 v[NV4];
@@ -48,6 +53,16 @@ ln_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __restric
     for (int i = 0; i < NV4; ++i) {
       const int c = lane + i * 32;
       v[i] = (c < n4) ? xr[c] : make_float4(0.f, 0.f, 0.f, 0.f);
+      if (ADD && c < n4) {
+        const float4 rv = reinterpret_cast<const float4*>(r + row * ldr)[c];
+        if (drop_in.ctr) {
+          const uint32_t e0 = (uint32_t)(row * H + c * 4);
+          v[i].x = drop_apply(v[i].x, seed_in, e0, drop_in); v[i].y = drop_apply(v[i].y, seed_in, e0 + 1, drop_in);
+          v[i].z = drop_apply(v[i].z, seed_in, e0 + 2, drop_in); v[i].w = drop_apply(v[i].w, seed_in, e0 + 3, drop_in);
+        }
+        v[i].x += rv.x; v[i].y += rv.y; v[i].z += rv.z; v[i].w += rv.w;
+        if (x_out) reinterpret_cast<float4*>(x_out + row * ldx)[c] = v[i];
+      }
       s += v[i].x + v[i].y + v[i].z + v[i].w;
     }
     const float mean = warp_sum(s) * inv_h;
@@ -107,9 +122,12 @@ ln_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __restric
 // A row is handled by a TEAM of two warps (64 lanes x NV float4 chunks) so that the three per-column accumulators fit in
 // ~110 registers and two 256-thread CTAs (16 warps) stay resident per SM; the two row sums cross the warps through a
 // double-buffered smem slot and one 64-thread named barrier per row.
+//
+// dy2 (optional): a second fp32 gradient of the LayerNorm output, added to dy as it is read (dy + dy2: the residual-path gradient
+// that a dgrad GEMM epilogue would otherwise have added into dy, in the same fp32 addition).
 template <int NV>
 __global__ void __launch_bounds__(ROW_THREADS, 2)
-ln_bwd_kernel(const float* __restrict__ dy, long long lddy, const float* __restrict__ x, long long ldx,
+ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ dy2, long long lddy, const float* __restrict__ x, long long ldx,
               const float* __restrict__ gamma, const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
               float* __restrict__ dx32, __nv_bfloat16* __restrict__ dx16, long long lddx,
               const __nv_bfloat16* __restrict__ pre, long long ldpre, float* __restrict__ dgamma, float* __restrict__ dbeta,
@@ -139,6 +157,10 @@ ln_bwd_kernel(const float* __restrict__ dy, long long lddy, const float* __restr
       const int c = tl + i * 64;
       if (c < n4) {
         float4 d = dyr[c];
+        if (dy2) {
+          const float4 e = reinterpret_cast<const float4*>(dy2 + row * lddy)[c];
+          d.x += e.x; d.y += e.y; d.z += e.z; d.w += e.w;
+        }
         const float4 xv = xr[c], gm = reinterpret_cast<const float4*>(gamma)[c];
         if (drop_out.ctr) {
           const uint32_t e0 = (uint32_t)(row * H + c * 4);
@@ -731,45 +753,82 @@ static inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) 
 using namespace vb;
 #define ST(s) static_cast<cudaStream_t>(s)
 
-extern "C" vb_status vb_layernorm_fwd(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, float* y_f32,
-                                      void* y_bf16, int64_t ldy, float* mean, float* rstd, int32_t M, int32_t H, const vb_dropout* out_dropout,
-                                      int32_t y_fp16, void* y_lo, void* y_b16, void* stream) {
-  if (M <= 0 || H <= 0) return set_error(VB_ERR_INVALID, "vb_layernorm_fwd: empty problem");
+// r == NULL: plain LayerNorm of x; otherwise of dropout(x) + r (ln_fwd_kernel<., true>)
+static vb_status layernorm_fwd(const char* name, const float* x, int64_t ldx, const float* r, int64_t ldr, const vb_dropout* in_dropout,
+                               float* x_out, const float* gamma, const float* beta, float eps, float* y_f32, void* y_bf16, int64_t ldy, float* mean,
+                               float* rstd, int32_t M, int32_t H, const vb_dropout* out_dropout, int32_t y_fp16, void* y_lo, void* y_b16, void* stream) {
+  if (M <= 0 || H <= 0) return set_error(VB_ERR_INVALID, "%s: empty problem", name);
   if ((H & 3) || H > MAX_V4 * 128 || (ldx & 3) || (ldy & 3) || !al16(x) || !al16(gamma) || !al16(beta) || (y_f32 && !al16(y_f32)) ||
       (y_bf16 && (reinterpret_cast<uintptr_t>(y_bf16) & 7)) || (y_lo && ((reinterpret_cast<uintptr_t>(y_lo) & 7) || !y_bf16)) ||
-      (reinterpret_cast<uintptr_t>(y_b16) & 7))
-    return set_error(VB_ERR_INVALID, "vb_layernorm_fwd: need H %% 4 == 0, H <= %d, ld %% 4 == 0, 16-byte aligned rows", MAX_V4 * 128);
+      (reinterpret_cast<uintptr_t>(y_b16) & 7) || (r && ((ldr & 3) || !al16(r))) || (x_out && !al16(x_out)))
+    return set_error(VB_ERR_INVALID, "%s: need H %% 4 == 0, H <= %d, ld %% 4 == 0, 16-byte aligned rows", name, MAX_V4 * 128);
+  const DropCfg dc = make_drop(out_dropout), dc_in = make_drop(in_dropout);
+  if (dc_in.ctr && ldx != H) return set_error(VB_ERR_INVALID, "%s: the dropout mask is indexed row*H + col and needs dense rows", name);
   const int nv4 = (H / 4 + 31) / 32;
   const int grid = row_grid(M);
   __nv_bfloat16* y16 = static_cast<__nv_bfloat16*>(y_bf16);
-  const DropCfg dc = make_drop(out_dropout);
-#define LN_F(NV) launch_pdl(ln_fwd_kernel<NV>, dim3(grid), dim3(ROW_THREADS), (size_t)(0), ST(stream), x, ldx, gamma, beta, eps, y_f32, y16, ldy, mean, rstd, M, H, dc, (int)(y_fp16 ? 1 : 0), static_cast<__nv_bfloat16*>(y_lo), static_cast<__nv_bfloat16*>(y_b16))
+#define LN_F(NV) (r ? launch_pdl(ln_fwd_kernel<NV, true>, dim3(grid), dim3(ROW_THREADS), (size_t)(0), ST(stream), x, ldx, gamma, beta, eps, y_f32, y16, ldy, mean, rstd, M, H, dc, (int)(y_fp16 ? 1 : 0), static_cast<__nv_bfloat16*>(y_lo), static_cast<__nv_bfloat16*>(y_b16), r, (long long)ldr, dc_in, x_out) \
+                    : launch_pdl(ln_fwd_kernel<NV, false>, dim3(grid), dim3(ROW_THREADS), (size_t)(0), ST(stream), x, ldx, gamma, beta, eps, y_f32, y16, ldy, mean, rstd, M, H, dc, (int)(y_fp16 ? 1 : 0), static_cast<__nv_bfloat16*>(y_lo), static_cast<__nv_bfloat16*>(y_b16), r, (long long)ldr, dc_in, x_out))
   if (nv4 <= 1) LN_F(1); else if (nv4 <= 2) LN_F(2); else if (nv4 <= 4) LN_F(4); else if (nv4 <= 6) LN_F(6);
   else if (nv4 <= 8) LN_F(8); else LN_F(16);
 #undef LN_F
-  return check_launch("vb_layernorm_fwd");
+  return check_launch(name);
 }
 
-extern "C" vb_status vb_layernorm_bwd(const float* dy, int64_t lddy, const float* x, int64_t ldx, const float* gamma, const float* mean,
-                                      const float* rstd, float* dx_f32, void* dx_bf16, int64_t lddx, const void* gelu_pre,
-                                      int64_t ld_pre, float* dgamma, float* dbeta, float* dbias, int32_t M, int32_t H,
-                                      const vb_dropout* out_dropout, const vb_dropout* in_dropout, void* stream) {
-  if (M <= 0 || H <= 0) return set_error(VB_ERR_INVALID, "vb_layernorm_bwd: empty problem");
-  if ((H & 3) || H > MAX_V4 * 128 || (ldx & 3) || (lddy & 3) || (lddx & 3) || (gelu_pre && (ld_pre & 3)) || !al16(dy) || !al16(x) || !al16(gamma))
-    return set_error(VB_ERR_INVALID, "vb_layernorm_bwd: need H %% 4 == 0, H <= %d, ld %% 4 == 0, 16-byte aligned rows", MAX_V4 * 128);
+extern "C" vb_status vb_layernorm_fwd(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, float* y_f32,
+                                      void* y_bf16, int64_t ldy, float* mean, float* rstd, int32_t M, int32_t H, const vb_dropout* out_dropout,
+                                      int32_t y_fp16, void* y_lo, void* y_b16, void* stream) {
+  return layernorm_fwd("vb_layernorm_fwd", x, ldx, nullptr, 0, nullptr, nullptr, gamma, beta, eps, y_f32, y_bf16, ldy, mean, rstd, M, H,
+                       out_dropout, y_fp16, y_lo, y_b16, stream);
+}
+
+extern "C" vb_status vb_add_layernorm_fwd(const float* d, const float* residual, int64_t ld, const vb_dropout* dropout, float* x_out,
+                                          const float* gamma, const float* beta, float eps, float* y_f32, void* y_bf16, int64_t ldy, float* mean,
+                                          float* rstd, int32_t M, int32_t H, int32_t y_fp16, void* y_lo, void* y_b16, void* stream) {
+  if (!d || !residual) return set_error(VB_ERR_INVALID, "vb_add_layernorm_fwd: d and residual are required");
+  if (x_out && x_out != d) return set_error(VB_ERR_INVALID, "vb_add_layernorm_fwd: x_out must be NULL or d (the sum is written in place)");
+  return layernorm_fwd("vb_add_layernorm_fwd", d, ld, residual, ld, dropout, x_out, gamma, beta, eps, y_f32, y_bf16, ldy, mean, rstd, M, H,
+                       nullptr, y_fp16, y_lo, y_b16, stream);
+}
+
+static vb_status layernorm_bwd(const char* name, const float* dy, const float* dy2, int64_t lddy, const float* x, int64_t ldx, const float* gamma,
+                               const float* mean, const float* rstd, float* dx_f32, void* dx_bf16, int64_t lddx, const void* gelu_pre,
+                               int64_t ld_pre, float* dgamma, float* dbeta, float* dbias, int32_t M, int32_t H,
+                               const vb_dropout* out_dropout, const vb_dropout* in_dropout, void* stream) {
+  if (M <= 0 || H <= 0) return set_error(VB_ERR_INVALID, "%s: empty problem", name);
+  if ((H & 3) || H > MAX_V4 * 128 || (ldx & 3) || (lddy & 3) || (lddx & 3) || (gelu_pre && (ld_pre & 3)) || !al16(dy) || !al16(x) || !al16(gamma) ||
+      (dy2 && !al16(dy2)))
+    return set_error(VB_ERR_INVALID, "%s: need H %% 4 == 0, H <= %d, ld %% 4 == 0, 16-byte aligned rows", name, MAX_V4 * 128);
   const DropCfg dc_out = make_drop(out_dropout), dc_in = make_drop(in_dropout);
   if ((dc_out.ctr || dc_in.ctr) && (ldx != H || lddy != H || lddx != H))
-    return set_error(VB_ERR_INVALID, "vb_layernorm_bwd: dropout masks are indexed row*H + col and need dense rows");
+    return set_error(VB_ERR_INVALID, "%s: dropout masks are indexed row*H + col and need dense rows", name);
   const int nv = (H / 4 + 63) / 64;   // float4 chunks per lane of a 64-lane row team
   long long blocks = ((long long)M + 3) / 4;
   const int cap = sm_count() * 2;     // two resident CTAs per SM; fewer CTAs -> fewer dgamma/dbeta atomics
   int grid = (int)(blocks < cap || cap <= 0 ? (blocks > 0 ? blocks : 1) : cap);
   __nv_bfloat16* dx16 = static_cast<__nv_bfloat16*>(dx_bf16);
   const __nv_bfloat16* pre = static_cast<const __nv_bfloat16*>(gelu_pre);
-#define LN_B(NV) launch_pdl(ln_bwd_kernel<NV>, dim3(grid), dim3(ROW_THREADS), (size_t)(0), ST(stream), dy, lddy, x, ldx, gamma, mean, rstd, dx_f32, dx16, lddx, pre, ld_pre, dgamma, dbeta, dbias, M, H, dc_out, dc_in)
+#define LN_B(NV) launch_pdl(ln_bwd_kernel<NV>, dim3(grid), dim3(ROW_THREADS), (size_t)(0), ST(stream), dy, dy2, lddy, x, ldx, gamma, mean, rstd, dx_f32, dx16, lddx, pre, ld_pre, dgamma, dbeta, dbias, M, H, dc_out, dc_in)
   if (nv <= 1) LN_B(1); else if (nv <= 2) LN_B(2); else if (nv <= 3) LN_B(3); else if (nv <= 4) LN_B(4); else LN_B(8);
 #undef LN_B
-  return check_launch("vb_layernorm_bwd");
+  return check_launch(name);
+}
+
+extern "C" vb_status vb_layernorm_bwd(const float* dy, int64_t lddy, const float* x, int64_t ldx, const float* gamma, const float* mean,
+                                      const float* rstd, float* dx_f32, void* dx_bf16, int64_t lddx, const void* gelu_pre,
+                                      int64_t ld_pre, float* dgamma, float* dbeta, float* dbias, int32_t M, int32_t H,
+                                      const vb_dropout* out_dropout, const vb_dropout* in_dropout, void* stream) {
+  return layernorm_bwd("vb_layernorm_bwd", dy, nullptr, lddy, x, ldx, gamma, mean, rstd, dx_f32, dx_bf16, lddx, gelu_pre, ld_pre, dgamma, dbeta,
+                       dbias, M, H, out_dropout, in_dropout, stream);
+}
+
+extern "C" vb_status vb_add_layernorm_bwd(const float* dy, const float* dy2, int64_t lddy, const float* x, int64_t ldx, const float* gamma,
+                                          const float* mean, const float* rstd, float* dx_f32, void* dx_bf16, int64_t lddx, const void* gelu_pre,
+                                          int64_t ld_pre, float* dgamma, float* dbeta, float* dbias, int32_t M, int32_t H,
+                                          const vb_dropout* out_dropout, const vb_dropout* in_dropout, void* stream) {
+  if (!dy2) return set_error(VB_ERR_INVALID, "vb_add_layernorm_bwd: dy2 is required");
+  return layernorm_bwd("vb_add_layernorm_bwd", dy, dy2, lddy, x, ldx, gamma, mean, rstd, dx_f32, dx_bf16, lddx, gelu_pre, ld_pre, dgamma, dbeta,
+                       dbias, M, H, out_dropout, in_dropout, stream);
 }
 
 extern "C" vb_status vb_cast_f32_to_bf16(const float* src, void* dst, int64_t n, int32_t fp16, void* dst_lo, void* dst_b16, void* stream) {

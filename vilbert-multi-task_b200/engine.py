@@ -294,12 +294,16 @@ class Act:
        gradient, as autograd's requires_grad; nothing made under the reference's torch.no_grad() (fixed_t_layer / fixed_v_layer) does.
     2. registration (Plan.push_bwd): a block whose output needs no gradient registers no backward emitter.
     3. first write (Plan.grad_zeroed / Plan.grad_acc): `gw` tells whether a backward op has written g32 yet. The first one
-       overwrites it, or zeroes it and adds; every later one accumulates."""
-    __slots__ = ("f32", "op", "g32", "gw", "M", "H", "rg")
+       overwrites it, or zeroes it and adds; every later one accumulates.
+    The output of a residual LayerNorm (Plan.dense_res_ln) has one reader of its gradient, that LayerNorm's backward, which can add
+    a second fp32 input as it reads (ln_reads). Its first writer may leave its residual-path part in g_add instead of adding it in a
+    GEMM epilogue; a later writer adds g_add into g32 first (Plan._fold_g_add), so every sum keeps the order it has without it."""
+    __slots__ = ("f32", "op", "g32", "gw", "M", "H", "rg", "ln_reads", "g_add")
 
     def __init__(self, f32, op, M, H, rg):
         self.f32, self.op, self.M, self.H, self.rg = f32, op, M, H, rg
         self.g32, self.gw = None, False
+        self.ln_reads, self.g_add = False, None
 
 
 # Objectives that can be fused into a plan, and the outputs each differentiates (task_utils.py:325-374, vilbert.py:1506-1590):
@@ -745,21 +749,30 @@ class Plan:
             self.emit(self.lib.vb_attention_probs, C.byref(a), probs.data_ptr())
             self._last_attn = dict(attn=probs, q=Q.hi, k=K.hi, B=B, H=H, Nq=Nq, Nk=Nk, D=D)
 
-    def ln_fwd(self, x, gamma, beta, M, H, want_f32=True, out_drop=None):
-        """-> (fp32 output or None, Operand output, mean, rstd)"""
+    def ln_fwd(self, x, gamma, beta, M, H, want_f32=True, out_drop=None, res=None, in_drop=None):
+        """-> (fp32 output or None, Operand output, mean, rstd). res: LayerNorm of dropout_in(x) + res instead (the residual add is
+        fused here rather than into the GEMM that wrote x); that sum is written over x, where the backward reads it."""
         y32 = self.buf((M, H), F32) if want_f32 else None
         y = self.buf16((M, H))
         mean, rstd = self.buf((M,), F32), self.buf((M,), F32)
         hi, lo, bw = y.ptrs()
-        self.emit(self.lib.vb_layernorm_fwd, x.data_ptr(), H, gamma.data_ptr(), beta.data_ptr(), 1e-12, self._ptr(y32), hi, H,
-                  mean.data_ptr(), rstd.data_ptr(), M, H, self._ref(out_drop), y.fp16, lo, bw)
+        if res is not None:
+            self.emit(self.lib.vb_add_layernorm_fwd, x.data_ptr(), res.data_ptr(), H, self._ref(in_drop), x.data_ptr(),
+                      gamma.data_ptr(), beta.data_ptr(), 1e-12, self._ptr(y32), hi, H, mean.data_ptr(), rstd.data_ptr(), M, H, y.fp16, lo, bw)
+        else:
+            self.emit(self.lib.vb_layernorm_fwd, x.data_ptr(), H, gamma.data_ptr(), beta.data_ptr(), 1e-12, self._ptr(y32), hi, H,
+                      mean.data_ptr(), rstd.data_ptr(), M, H, self._ref(out_drop), y.fp16, lo, bw)
         return y32, y, mean, rstd
 
-    def ln_bwd(self, dy, x, gamma, mean, rstd, dx32, dx16, M, H, ggamma, gbeta, pre=None, gbias=None, out_drop=None, in_drop=None):
-        """gbias: bias gradient of the Linear feeding this LayerNorm (column sums of dx), fused into the same pass."""
-        self.emit(self.lib.vb_layernorm_bwd, dy.data_ptr(), H, x.data_ptr(), H, gamma.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
-                  self._ptr(dx32), self._ptr(dx16), H, self._ptr(pre), H, self._ptr(ggamma), self._ptr(gbeta), self._ptr(gbias), M, H,
-                  self._ref(out_drop), self._ref(in_drop))
+    def ln_bwd(self, dy, x, gamma, mean, rstd, dx32, dx16, M, H, ggamma, gbeta, pre=None, gbias=None, out_drop=None, in_drop=None, dy2=None):
+        """gbias: bias gradient of the Linear feeding this LayerNorm (column sums of dx), fused into the same pass. dy2: a second
+        part of the output gradient (Act.g_add), added to dy as it is read."""
+        tail = (x.data_ptr(), H, gamma.data_ptr(), mean.data_ptr(), rstd.data_ptr(), self._ptr(dx32), self._ptr(dx16), H, self._ptr(pre), H,
+                self._ptr(ggamma), self._ptr(gbeta), self._ptr(gbias), M, H, self._ref(out_drop), self._ref(in_drop))
+        if dy2 is not None:
+            self.emit(self.lib.vb_add_layernorm_bwd, dy.data_ptr(), dy2.data_ptr(), H, *tail)
+        else:
+            self.emit(self.lib.vb_layernorm_bwd, dy.data_ptr(), H, *tail)
 
     def colsum(self, X, ld, out, M, N):
         self.emit(self.lib.vb_colsum, X.data_ptr(), 1 if X.dtype == BF16 else 0, ld, out.data_ptr(), M, N)
@@ -775,6 +788,7 @@ class Plan:
         if not act.gw:
             self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
             act.gw = True
+        self._fold_g_add(act)
         return g
 
     def grad_acc(self, act):
@@ -782,7 +796,14 @@ class Plan:
         writer (rule 3 of Act)."""
         g, acc = self.grad_of(act), 1 if act.gw else 0
         act.gw = True
+        self._fold_g_add(act)
         return g, acc
+
+    def _fold_g_add(self, act):
+        """A later writer of g32 adds to it: the first writer's deferred part goes in first, so the sums keep their order."""
+        if act.g_add is not None:
+            self.emit(self.lib.vb_axpy_f32, act.g_add.data_ptr(), act.g32.data_ptr(), act.M * act.H, 1.0)
+            act.g_add = None
 
     # dW, db of y = x W^T + b given dy (bf16 operand copy)
     def linear_wgrad(self, dy16, ld_dy, x16, ld_x, M, N_out, K_in, wname, gw=None, bias_from=(None, 0)):
@@ -823,6 +844,8 @@ class Plan:
         if not act.rg:      # the activation needs no gradient (frozen producer, or fixed_*_layer's no_grad): it stops here
             return
         g, acc = self.grad_acc(act)
+        if not acc and extra32 is not None and act.ln_reads:
+            act.g_add, extra32 = extra32, None      # added by the LayerNorm backward that reads g32: the GEMM reads no residual
         if acc and extra32 is not None:
             self.emit(self.lib.vb_axpy_f32, extra32.data_ptr(), g.data_ptr(), M * K_in, 1.0)
         self.gemm(M, K_in, N_out, dy16, ld_dy, W16, K_in, b_mn=1, residual=g if acc else extra32, ld_res=K_in, out_f32=g, ld_of=K_in)
@@ -839,10 +862,11 @@ class Plan:
         a_rg: whether `a` needs a gradient (the caller's backward takes the returned dy16 into it)."""
         ps, M, H = self.ps, res.M, res.H
         y = self.buf((M, H), F32)
-        self.gemm(M, H, K_in, a, K_in, ps.w(wname + ".weight"), K_in, bias=ps.p(wname + ".bias"), residual=res.f32, ld_res=H,
-                  out_f32=y, ld_of=H, dropout=drop)
-        o32, o, mean, rstd = self.ln_fwd(y, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, H)
+        # the GEMM stores dense(a) only; dropout and the residual add are fused into the LayerNorm that reads it anyway
+        self.gemm(M, H, K_in, a, K_in, ps.w(wname + ".weight"), K_in, bias=ps.p(wname + ".bias"), out_f32=y, ld_of=H)
+        o32, o, mean, rstd = self.ln_fwd(y, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, H, res=res.f32, in_drop=drop)
         out = self.act(o32, o, M, H, inputs=(res,), params=(wname, lnname), rg=a_rg)
+        out.ln_reads = True
 
         def bwd():
             """returns (dy16, dy32) of the dense output (== grad of the LN input); adds dy32 to res."""
@@ -851,7 +875,8 @@ class Plan:
             dy32 = self.scratch(tag + ".dy32", (M, H), F32)
             dy16 = self.scratch(tag + ".dy16", (M, H), BF16)
             self.ln_bwd(out.g32, y, ps.p(lnname + ".weight"), mean, rstd, dy32, dy16, M, H, self.pg(lnname + ".weight"), self.pg(lnname + ".bias"),
-                        gbias=self.pg(wname + ".bias"), in_drop=drop)
+                        gbias=self.pg(wname + ".bias"), in_drop=drop, dy2=out.g_add)
+            out.g_add = None
             self.linear_wgrad(dy16, H, a.bw, K_in, M, H, K_in, wname)
             return dy16, dy32
         return out, bwd
@@ -982,7 +1007,7 @@ class Plan:
             if not (v1o.gw or t1o.gw):
                 return
             for a in (v1o, t1o):   # a stream without downstream gradient contributes zeros
-                if a.rg:
+                if a.rg and not a.gw:
                     self.grad_zeroed(a)
             rv, rt = v1_bwd(), t1_bwd()
             if not ctx_rg:
