@@ -300,7 +300,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
 }
 
 // ------------------------------------------------------------------------------------------ backward: dQ
-// DQ = false (dK / dV-only backward): the kernel writes delta, which the dK / dV kernel reads, and nothing else; it stages only dO.
+// DQ = false (dK / dV-only backward): the kernel writes delta, which the dK / dV kernel reads, and nothing else; without dropout it
+// stages only dO.
 template <int D, bool DQ = true>
 __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnParams p) {
   constexpr int LD = D + 8;
@@ -317,10 +318,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int rows_valid = min(TQ, p.Nq - q0);
+  const bool stage_qkv = DQ || p.drop.ctr;   // with dropout, delta is formed from P and dP (below)
 
-  if constexpr (DQ) load_panel<D>(sQ, p.Q + ((long long)b * p.Nq + q0) * p.ldq + h * D, p.ldq, rows_valid, TQ);
+  if (stage_qkv) load_panel<D>(sQ, p.Q + ((long long)b * p.Nq + q0) * p.ldq + h * D, p.ldq, rows_valid, TQ);
   load_panel<D>(sdO, p.dO + ((long long)b * p.Nq + q0) * p.lddo + h * D, p.lddo, rows_valid, TQ);
-  if constexpr (DQ) {
+  if (stage_qkv) {
     load_panel<D>(sK, p.K + (long long)b * p.Nk * p.ldk + h * D, p.ldk, p.Nk, nkp);
     load_panel<D>(sV, p.V + (long long)b * p.Nk * p.ldv + h * D, p.ldv, p.Nk, nkp);
     for (int j = threadIdx.x; j < nkp; j += ATT_THREADS)
@@ -328,7 +330,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
   }
   cp_async_wait_all();
   __syncthreads();
-  if (DQ && p.qkv_fp16) {
+  if (stage_qkv && p.qkv_fp16) {
     panel_f16_to_bf16<D, ATT_THREADS>(sQ, TQ); panel_f16_to_bf16<D, ATT_THREADS>(sK, nkp); panel_f16_to_bf16<D, ATT_THREADS>(sV, nkp);
     __syncthreads();
   }
@@ -336,9 +338,48 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
   const int r0 = warp * 16;
   if (r0 >= rows_valid) return;
 
+  float ls[2] = {0.f, 0.f};
+  {
+    const float* lse = p.lse + ((long long)b * p.H + h) * p.Nq + q0;
+    if (r0 + g < rows_valid) ls[0] = lse[r0 + g];
+    if (r0 + g + 8 < rows_valid) ls[1] = lse[r0 + g + 8];
+  }
+  const float c = p.scale * LOG2E;
+  const uint32_t dseed = p.drop.ctr ? drop_seed(p.drop) : 0u;
+
   // delta = rowsum(dO o O) for rows g, g+8 of this warp; each quad lane sums a quarter of the columns.
   float dl[2] = {0.f, 0.f};
-  {
+  if (p.drop.ctr) {
+    // With dropout, rowsum(dO o O_b16) no longer cancels f dP on a peaked row (bf16(f V) != f bf16(V)): form delta from the same P
+    // and f dP as the dS below, delta = sum_k P f dP / sum_k P (one extra pass of the two products over the keys)
+    float sp[2] = {0.f, 0.f}, sd[2] = {0.f, 0.f};
+    for (int kb = 0; kb < nkp; kb += KB) {
+      float s[8][4], dp[8][4];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
+        dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f;
+      }
+      mma_a_bt<D>(s, sQ, r0, sK, kb, lane, p.Nk);
+      mma_a_bt<D>(dp, sdO, r0, sV, kb, lane, p.Nk);
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        const float mk0 = sMask[kb + nt * 8 + 2 * t], mk1 = sMask[kb + nt * 8 + 2 * t + 1];
+        const float p0 = exp2f(s[nt][0] * c + mk0 - ls[0]), p1 = exp2f(s[nt][1] * c + mk1 - ls[0]);
+        const float p2 = exp2f(s[nt][2] * c + mk0 - ls[1]), p3 = exp2f(s[nt][3] * c + mk1 - ls[1]);
+        const uint32_t e0 = (uint32_t)((((long long)b * p.H + h) * p.Nq + q0 + r0 + g) * p.Nk + kb + nt * 8 + 2 * t);
+        const uint32_t e1 = e0 + 8u * (uint32_t)p.Nk;
+        sp[0] += p0 + p1; sp[1] += p2 + p3;
+        sd[0] += p0 * (dp[nt][0] * drop_factor(dseed, e0, p.drop)) + p1 * (dp[nt][1] * drop_factor(dseed, e0 + 1, p.drop));
+        sd[1] += p2 * (dp[nt][2] * drop_factor(dseed, e1, p.drop)) + p3 * (dp[nt][3] * drop_factor(dseed, e1 + 1, p.drop));
+      }
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      sp[hh] = quad_sum(sp[hh]); sd[hh] = quad_sum(sd[hh]);
+      dl[hh] = sp[hh] > 0.f ? sd[hh] / sp[hh] : 0.f;
+    }
+  } else {
     // delta = rowsum(dO o O) must cancel against dP = dO V^T formed from the bf16-rounded V: use the bf16 copy of O when the
     // forward wrote one (an fp16 O differs from P V_bf16 by the bf16 rounding of V, which peaked rows do not forgive)
     const int o_fp16 = p.Ob ? 0 : p.qkv_fp16;
@@ -364,21 +405,13 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
     }
     dl[0] = quad_sum(dl[0]); dl[1] = quad_sum(dl[1]);
   }
-  float ls[2] = {0.f, 0.f};
-  {
-    const float* lse = p.lse + ((long long)b * p.H + h) * p.Nq + q0;
-    if (r0 + g < rows_valid) ls[0] = lse[r0 + g];
-    if (r0 + g + 8 < rows_valid) ls[1] = lse[r0 + g + 8];
-    if (t == 0) {
-      float* dg = p.delta + ((long long)b * p.H + h) * p.Nq + q0;
-      if (r0 + g < rows_valid) dg[r0 + g] = dl[0];
-      if (r0 + g + 8 < rows_valid) dg[r0 + g + 8] = dl[1];
-    }
+  if (t == 0) {
+    float* dg = p.delta + ((long long)b * p.H + h) * p.Nq + q0;
+    if (r0 + g < rows_valid) dg[r0 + g] = dl[0];
+    if (r0 + g + 8 < rows_valid) dg[r0 + g + 8] = dl[1];
   }
   if constexpr (!DQ) return;
 
-  const float c = p.scale * LOG2E;
-  const uint32_t dseed = p.drop.ctr ? drop_seed(p.drop) : 0u;
   float dq[D / 8][4];
 #pragma unroll
   for (int i = 0; i < D / 8; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
@@ -397,7 +430,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
       const float mk0 = sMask[kb + nt * 8 + 2 * t], mk1 = sMask[kb + nt * 8 + 2 * t + 1];
       const float p0 = exp2f(s[nt][0] * c + mk0 - ls[0]), p1 = exp2f(s[nt][1] * c + mk1 - ls[0]);
       const float p2 = exp2f(s[nt][2] * c + mk0 - ls[1]), p3 = exp2f(s[nt][3] * c + mk1 - ls[1]);
-      if (p.drop.ctr) {   // dP = mask/(1-p) * (dO V^T); delta = rowsum(dO o O) already contains the mask through O
+      if (p.drop.ctr) {   // dP = mask/(1-p) * (dO V^T); delta was formed from these products above
         const uint32_t e0 = (uint32_t)((((long long)b * p.H + h) * p.Nq + q0 + r0 + g) * p.Nk + kb + nt * 8 + 2 * t);
         const uint32_t e1 = e0 + 8u * (uint32_t)p.Nk;
         dp[nt][0] *= drop_factor(dseed, e0, p.drop); dp[nt][1] *= drop_factor(dseed, e0 + 1, p.drop);
@@ -544,7 +577,8 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
   __nv_bfloat16* sV = sK + nkp * LD;
   __nv_bfloat16* sP = sV + nkp * LD;
   __nv_bfloat16* sdS = sP + nqp * LDP;
-  float* sMask = reinterpret_cast<float*>(DKV ? sdS + nqp * LDP : sP);
+  // the P / dS tiles are staged for phase 2, and with dropout also for phase 1 (see there)
+  float* sMask = reinterpret_cast<float*>((DKV || p.drop.ctr) ? sdS + nqp * LDP : sP);
 
   const int b = blockIdx.y, h = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -569,7 +603,7 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
   if (r0 < nqp) {
     // ---- phase 1: this warp's 16 query rows
     float dl[2] = {0.f, 0.f};   // delta = rowsum(dO o O)
-    {
+    if (!p.drop.ctr) {
       const int o_fp16 = p.Ob ? 0 : p.qkv_fp16;      // see attn_bwd_dq_kernel: the bf16 copy of O keeps delta consistent with dP
       const __nv_bfloat16* Og = (p.Ob ? p.Ob : p.O) + (long long)b * p.Nq * p.ldo + h * D;
 #pragma unroll
@@ -602,6 +636,69 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
     float dq[D / 8][4];
 #pragma unroll
     for (int i = 0; i < D / 8; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
+    if (p.drop.ctr) {
+      // With dropout, rowsum(dO o O_b16) no longer cancels f dP on a peaked row: bf16(f V) != f bf16(V), so dS of a row with one
+      // valid key would be bf16 noise instead of 0. Pass A parks P and f dP as bf16 tiles and forms delta from those same values,
+      // delta = sum_k P f dP / sum_k P (the recomputed P normalised); pass B forms dS = P (f dP - delta) from the parked values, which
+      // cancel exactly, and replaces the tiles by P f and dS for phase 2.
+      float sp[2] = {0.f, 0.f}, sd[2] = {0.f, 0.f};
+      for (int kb = 0; kb < nkp; kb += KB) {
+        float s[8][4], dp[8][4];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
+          dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f;
+        }
+        mma_a_bt<D>(s, sQ, r0, sK, kb, lane, p.Nk);
+        mma_a_bt<D>(dp, sdO, r0, sV, kb, lane, p.Nk);
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+          const int col = kb + nt * 8 + 2 * t;
+          const float mk0 = sMask[col], mk1 = sMask[col + 1];
+          const uint32_t e0 = (uint32_t)((((long long)b * p.H + h) * p.Nq + r0 + g) * p.Nk + col);
+          const uint32_t e1 = e0 + 8u * (uint32_t)p.Nk;
+          const uint32_t pa = pack_bf16(exp2f(s[nt][0] * c + mk0 - ls[0]), exp2f(s[nt][1] * c + mk1 - ls[0]));
+          const uint32_t pb = pack_bf16(exp2f(s[nt][2] * c + mk0 - ls[1]), exp2f(s[nt][3] * c + mk1 - ls[1]));
+          const uint32_t da = pack_bf16(dp[nt][0] * drop_factor(dseed, e0, p.drop), dp[nt][1] * drop_factor(dseed, e0 + 1, p.drop));
+          const uint32_t db = pack_bf16(dp[nt][2] * drop_factor(dseed, e1, p.drop), dp[nt][3] * drop_factor(dseed, e1 + 1, p.drop));
+          *reinterpret_cast<uint32_t*>(sP + (r0 + g) * LDP + col) = pa;
+          *reinterpret_cast<uint32_t*>(sP + (r0 + g + 8) * LDP + col) = pb;
+          *reinterpret_cast<uint32_t*>(sdS + (r0 + g) * LDP + col) = da;
+          *reinterpret_cast<uint32_t*>(sdS + (r0 + g + 8) * LDP + col) = db;
+          const float2 P0 = unpack16(pa, 0), P1 = unpack16(pb, 0), F0 = unpack16(da, 0), F1 = unpack16(db, 0);
+          sp[0] += P0.x + P0.y; sd[0] += P0.x * F0.x + P0.y * F0.y;
+          sp[1] += P1.x + P1.y; sd[1] += P1.x * F1.x + P1.y * F1.y;
+        }
+      }
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        sp[hh] = quad_sum(sp[hh]); sd[hh] = quad_sum(sd[hh]);
+        dl[hh] = sp[hh] > 0.f ? sd[hh] / sp[hh] : 0.f;
+      }
+      for (int kb = 0; kb < nkp; kb += KB) {
+        float s[8][4];
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {   // each lane reads back the elements it parked in pass A
+          const int col = kb + nt * 8 + 2 * t;
+          uint32_t* pp0 = reinterpret_cast<uint32_t*>(sP + (r0 + g) * LDP + col);
+          uint32_t* pp1 = reinterpret_cast<uint32_t*>(sP + (r0 + g + 8) * LDP + col);
+          uint32_t* ps0 = reinterpret_cast<uint32_t*>(sdS + (r0 + g) * LDP + col);
+          uint32_t* ps1 = reinterpret_cast<uint32_t*>(sdS + (r0 + g + 8) * LDP + col);
+          const float2 P0 = unpack16(*pp0, 0), P1 = unpack16(*pp1, 0), F0 = unpack16(*ps0, 0), F1 = unpack16(*ps1, 0);
+          s[nt][0] = P0.x * (F0.x - dl[0]); s[nt][1] = P0.y * (F0.y - dl[0]);
+          s[nt][2] = P1.x * (F1.x - dl[1]); s[nt][3] = P1.y * (F1.y - dl[1]);
+          if constexpr (DKV) {
+            const uint32_t e0 = (uint32_t)((((long long)b * p.H + h) * p.Nq + r0 + g) * p.Nk + col);
+            const uint32_t e1 = e0 + 8u * (uint32_t)p.Nk;
+            *pp0 = pack_bf16(P0.x * drop_factor(dseed, e0, p.drop), P0.y * drop_factor(dseed, e0 + 1, p.drop));
+            *pp1 = pack_bf16(P1.x * drop_factor(dseed, e1, p.drop), P1.y * drop_factor(dseed, e1 + 1, p.drop));
+            *ps0 = pack_bf16(s[nt][0], s[nt][1]);
+            *ps1 = pack_bf16(s[nt][2], s[nt][3]);
+          }
+        }
+        if constexpr (DQ) mma_p_b<D>(dq, s, sK, kb, lane, p.Nk);
+      }
+    } else
     for (int kb = 0; kb < nkp; kb += KB) {
       float s[8][4], dp[8][4];
 #pragma unroll
@@ -813,8 +910,8 @@ extern "C" vb_status vb_attention_bwd(const vb_attn_args* a, void* stream) {
     if (smem_f <= 227 * 1024) {
       dim3 gf(a->H, a->B);
       const char* what = "vb_attention_bwd(fused)";
-      // the dQ-only variant keeps no P / dS tiles
-      const size_t smem_q = smem_f - (size_t)2 * nq16 * (nkp + 8) * 2;
+      // the dQ-only variant keeps no P / dS tiles, except with dropout (phase 1 stages P and dP there)
+      const size_t smem_q = p.drop.ctr ? smem_f : smem_f - (size_t)2 * nq16 * (nkp + 8) * 2;
 #define VB_BWD_FUSED(DD)                                                                                            \
   if (!want_dkv) return launch_att(attn_bwd_fused_kernel<DD, true, false>, gf, smem_q, p, st, what, ATT1_THREADS); \
   if (!want_dq) return launch_att(attn_bwd_fused_kernel<DD, false, true>, gf, smem_f, p, st, what, ATT1_THREADS);  \
@@ -830,7 +927,7 @@ extern "C" vb_status vb_attention_bwd(const vb_attn_args* a, void* stream) {
   // two kernels: dQ (which also writes delta), then dK / dV. Without dQ the first kernel only writes delta; without dK / dV the
   // second is not launched.
   const size_t smem_q = (size_t)(2 * TQ + 2 * nkp) * (a->D + 8) * 2 + (size_t)nkp * 4;
-  const size_t smem_delta = (size_t)(2 * TQ) * (a->D + 8) * 2;
+  const size_t smem_delta = p.drop.ctr ? smem_q : (size_t)(2 * TQ) * (a->D + 8) * 2;   // with dropout delta needs Q / K / V
   const size_t smem_k = (size_t)(2 * TQ + 2 * nqp) * (a->D + 8) * 2 + (size_t)nqp * 8;
   dim3 gq((a->Nq + TQ - 1) / TQ, a->H, a->B), gk((a->Nk + TQ - 1) / TQ, a->H, a->B);
   int s;
