@@ -43,10 +43,21 @@ enum { VB_ACT_NONE = 0, VB_ACT_GELU = 1, VB_ACT_RELU = 2, VB_ACT_DGELU = 3 };
  * `step` is a device uint32 bumped once per training step; `site` names the dropout layer; `index` is the
  * row-major element index of the tensor the reference applies nn.Dropout to (mod 2^32). step == NULL or p == 0
  * disables dropout (the reference's eval mode). */
+typedef struct vb_dropout_site {
+  const uint32_t* step;
+  uint32_t site;
+  float p;
+} vb_dropout_site;
+/* The descriptor the row-wise kernels take (LayerNorms, residual LayerNorms, small linear heads): a vb_dropout_site with an
+ * optional packed-row -> padded-row map (int32 [rows], device; NULL: none). With it, element (r, c) of a row-indexed site
+ * [rows, H] draws the mask of element (row_map[r], c) of the padded tensor, so a packed plan (Plan(packed=...)) draws the padded
+ * plan's masks. The GEMM epilogue and attention carry a vb_dropout_site: attention indexes its elements at padded coordinates by
+ * itself, and no packed plan uses a GEMM-epilogue dropout. */
 typedef struct vb_dropout {
   const uint32_t* step;
   uint32_t site;
   float p;
+  const int32_t* row_map;
 } vb_dropout;
 
 /* ABI version of this header (bumped on incompatible change). */
@@ -98,7 +109,7 @@ typedef struct vb_gemm_args {
   int64_t ld_out_pre;
   int32_t atomic_out;    /* 0 store, 1 red.add into out_f32 */
   float* out_colsum;     /* [N] or NULL: += column sums of the epilogue value before the residual add (bias gradients) */
-  vb_dropout dropout;    /* applied to the epilogue value before the residual add (index m*N + n): LN(dropout(dense(x)) + res) */
+  vb_dropout_site dropout;    /* applied to the epilogue value before the residual add (index m*N + n): LN(dropout(dense(x)) + res) */
   int32_t split_k;       /* >= 1; > 1 requires atomic_out and no act / bf16 outputs */
   int32_t block_n;       /* 0 = auto, else 128 or 256 */
   int32_t max_ctas;      /* 0 = one persistent CTA per SM */
@@ -161,7 +172,7 @@ typedef struct vb_attn_args {
   float* delta;
   /* optional (backward): += column sums of dQ / dK / dV, f32 [H*D] each — the bias gradients of the projections */
   float* dbias_q; float* dbias_k; float* dbias_v;
-  vb_dropout dropout;   /* on the probabilities; element index ((b*H + h)*Nq + q)*Nk + k */
+  vb_dropout_site dropout;   /* on the probabilities; element index ((b*H + h)*Nq + q)*Nk + k */
   /* ---- ABI v2. qkv_fp16: Q, K, V and O are fp16 (forward operands) instead of bf16; dO / dQ / dK / dV are always bf16
    * (the backward converts its Q / K / V panels to bf16 in shared memory). Split precision (forward only): with Q_lo,
    * K_lo, V_lo given (same ld and indexing as Q / K / V) S = Q K^T + Q_lo K^T + Q K_lo^T and O = P V + P_lo V + P V_lo
@@ -171,6 +182,12 @@ typedef struct vb_attn_args {
   void* O_lo;
   void* O_b16;   /* forward: optional always-bf16 copy of O (same ldo): the operand of the out-projection's weight gradient.
                     backward: if given, delta = rowsum(dO o O) reads this copy (consistent with the bf16 products of the backward) */
+  /* Packed rows (varlen), all four or none (int32 [B] each, device): sample b's queries are rows q_off[b] + i, i < q_len[b], of Q /
+   * O / dO / dQ, and its keys rows k_off[b] + j, j < k_len[b], of K / V / dK / dV. Keys past k_len are excluded, so mask must be NULL;
+   * every length must be >= 1. Nq / Nk stay the maxima: the grid, lse / delta [B, H, Nq] and the dropout element index
+   * ((b*H + h)*Nq + i)*Nk + j remain at padded coordinates, so a packed step draws the padded step's masks. Rows of no sample are not
+   * written. NULL: the padded layout (rows b*Nq + i, b*Nk + j). vb_attention_probs refuses packed rows. */
+  const int32_t* q_off; const int32_t* q_len; const int32_t* k_off; const int32_t* k_len;
 } vb_attn_args;
 
 vb_status vb_attention_fwd(const vb_attn_args* args, void* stream);
@@ -428,6 +445,30 @@ vb_status vb_sum_strided(const float* src, float* dst, int64_t n, int32_t count_
 vb_status vb_step_counter_bump(uint32_t* step, void* stream);
 
 vb_status vb_memset_zero(void* ptr, int64_t bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Packed task steps (Plan(packed=...)): the valid text tokens and image regions of a batch as contiguous per-sample row ranges.
+ * A packed stream has `rows` rows (the valid-row count rounded up to a capacity bucket); sample b owns rows off[b] .. off[b] +
+ * len[b] - 1, rows off[B] .. rows - 1 belong to no sample, and map[r] is the padded row (b * N + i) of packed row r (-1: none).
+ *   vb_pack_build          off (int32 [B + 1]), len (int32 [B]) and map (int32 [rows]) of both streams from the 0/1 masks, which
+ *                          must be prefix-valid; the text length includes the task token's row when has_task (one CTA)
+ *   vb_pack_rows_f32       dst[r,:] = src[map[r],:] (zeros where map[r] < 0), f32 rows of cols
+ *   vb_pack_regions        the region features of the packed rows cast to a tensor-core operand (hi, optional split-precision lo,
+ *                          optional bf16 copy): bitwise vb_cast_f32_to_bf16 of the same elements; cols % 8 == 0
+ *   vb_unpack_rows_f32     dst[b*N + i,:] = i < len[b] ? src[off[b] + i,:] : fill (per-region logits back to the padded layout)
+ *   vb_scatter_add_rows_f32  dst[idx[r],:] += src[r,:] (distinct idx): the pooled rows' gradient into the packed sequence gradient
+ *   vb_zero_tail_rows      rows [*first, rows) of a, b, c (each optional but a; row pitch ld_bytes, row_bytes per row, both multiples
+ *                          of 16) set to zero: the rows of no sample that the attention kernels do not write */
+vb_status vb_pack_build(const int64_t* text_mask, int32_t Nt_in, int32_t has_task, const int64_t* image_mask, int32_t Nv, int32_t B,
+                        int32_t rows_t, int32_t rows_v, int32_t* off_t, int32_t* len_t, int32_t* map_t, int32_t* off_v, int32_t* len_v,
+                        int32_t* map_v, void* stream);
+vb_status vb_pack_rows_f32(const float* src, float* dst, const int32_t* map, int32_t rows, int32_t cols, void* stream);
+vb_status vb_pack_regions(const float* features, const int32_t* map, int32_t rows, int32_t cols, int32_t fp16, void* dst, void* dst_lo,
+                          void* dst_b16, void* stream);
+vb_status vb_unpack_rows_f32(const float* src, float* dst, const int32_t* off, const int32_t* len, int32_t B, int32_t N, int32_t cols,
+                             float fill, void* stream);
+vb_status vb_scatter_add_rows_f32(const float* src, float* dst, const int32_t* idx, int32_t rows, int32_t cols, void* stream);
+vb_status vb_zero_tail_rows(void* a, void* b, void* c, int64_t ld_bytes, int32_t row_bytes, const int32_t* first, int32_t rows, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused multi-tensor AdamW on flat buffers (SURVEY.md §8 f2). Replaces pytorch_transformers==1.0.0 AdamW as the reference

@@ -18,10 +18,17 @@ class VBError(RuntimeError):
     pass
 
 
-class Dropout(C.Structure):
-    """Mirror of ``struct vb_dropout``."""
+class DropoutSite(C.Structure):
+    """Mirror of ``struct vb_dropout_site`` (the dropout of the GEMM epilogue and of attention)."""
 
     _fields_ = [("step", C.c_void_p), ("site", C.c_uint32), ("p", C.c_float)]
+
+
+class Dropout(DropoutSite):
+    """Mirror of ``struct vb_dropout`` (the row-wise kernels' descriptor): a DropoutSite with an optional packed-row map. Assigned
+    to the dropout field of GemmArgs / AttnArgs it contributes its DropoutSite part."""
+
+    _fields_ = [("row_map", C.c_void_p)]
 
 
 class GemmArgs(C.Structure):
@@ -39,7 +46,7 @@ class GemmArgs(C.Structure):
         ("out_f32", C.c_void_p), ("ld_out_f32", C.c_int64),
         ("out_bf16", C.c_void_p), ("ld_out_bf16", C.c_int64),
         ("out_pre", C.c_void_p), ("ld_out_pre", C.c_int64),
-        ("atomic_out", C.c_int32), ("out_colsum", C.c_void_p), ("dropout", Dropout), ("split_k", C.c_int32), ("block_n", C.c_int32), ("max_ctas", C.c_int32),
+        ("atomic_out", C.c_int32), ("out_colsum", C.c_void_p), ("dropout", DropoutSite), ("split_k", C.c_int32), ("block_n", C.c_int32), ("max_ctas", C.c_int32),
         ("dbg_lbo_a", C.c_uint32), ("dbg_sbo_a", C.c_uint32), ("dbg_lbo_b", C.c_uint32), ("dbg_sbo_b", C.c_uint32),
         ("dbg_timeline", C.c_void_p), ("cluster_m", C.c_int32),
         ("a_fp16", C.c_int32), ("b_fp16", C.c_int32), ("out_fp16", C.c_int32),
@@ -59,9 +66,10 @@ class AttnArgs(C.Structure):
         ("dK", C.c_void_p), ("lddk", C.c_int64), ("dV", C.c_void_p), ("lddv", C.c_int64),
         ("delta", C.c_void_p),
         ("dbias_q", C.c_void_p), ("dbias_k", C.c_void_p), ("dbias_v", C.c_void_p),
-        ("dropout", Dropout),
+        ("dropout", DropoutSite),
         ("qkv_fp16", C.c_int32), ("Q_lo", C.c_void_p), ("K_lo", C.c_void_p), ("V_lo", C.c_void_p), ("O_lo", C.c_void_p),
         ("O_b16", C.c_void_p),
+        ("q_off", C.c_void_p), ("q_len", C.c_void_p), ("k_off", C.c_void_p), ("k_len", C.c_void_p),
     ]
 
 
@@ -135,6 +143,12 @@ _SIGNATURES = {
     "vb_tanh_fwd": [_P, _P, _P, _P, _P, _I32, _I64, _P],
     "vb_tanh_bwd": [_P, _P, _P, _P, _I32, _I32, _P],
     "vb_mask_concat_additive": [_P, _P, _P, _I32, _I32, _I32, _P],
+    "vb_pack_build": [_P, _I32, _I32, _P, _I32, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P],
+    "vb_pack_rows_f32": [_P, _P, _P, _I32, _I32, _P],
+    "vb_pack_regions": [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P],
+    "vb_unpack_rows_f32": [_P, _P, _P, _P, _I32, _I32, _I32, _F, _P],
+    "vb_scatter_add_rows_f32": [_P, _P, _P, _I32, _I32, _P],
+    "vb_zero_tail_rows": [_P, _P, _P, _I64, _I32, _P, _I32, _P],
 }
 # device scratch of one vb_weight_norm_fwd / _bwd launch (include/vilbert_b200.h)
 VB_WEIGHT_NORM_SCRATCH = 1024

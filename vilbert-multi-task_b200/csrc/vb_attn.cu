@@ -51,7 +51,15 @@ struct AttnParams {
   __nv_bfloat16* Ol;                   // low part of O, or NULL
   __nv_bfloat16* Ob;                   // always-bf16 copy of O, or NULL
   int kchunk;                          // forward: keys resident in shared memory at a time (multiple of KB; >= padded Nk = one pass)
+  // packed rows (varlen): sample b's queries are rows qoff[b] + i, i < qlen[b], its keys rows koff[b] + j, j < klen[b]; NULL = the
+  // padded layout (rows b * Nq + i, b * Nk + j). Nq / Nk stay the maxima: lse, delta and the dropout index are at padded coordinates
+  const int *qoff, *qlen, *koff, *klen;
 };
+
+__device__ __forceinline__ long long q_row0(const AttnParams& p, int b) { return p.qoff ? (long long)p.qoff[b] : (long long)b * p.Nq; }
+__device__ __forceinline__ long long k_row0(const AttnParams& p, int b) { return p.koff ? (long long)p.koff[b] : (long long)b * p.Nk; }
+__device__ __forceinline__ int q_count(const AttnParams& p, int b) { return p.qoff ? p.qlen[b] : p.Nq; }
+__device__ __forceinline__ int k_count(const AttnParams& p, int b) { return p.koff ? p.klen[b] : p.Nk; }
 
 // In-place fp16 -> bf16 conversion of a staged panel (rows x D at pitch D + 8): the backward kernels run their products in
 // bf16 because dO / dS are bf16 (gradient range), while Q / K / V arrive as fp16 forward operands.
@@ -197,7 +205,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
   constexpr int LD = D + 8;
   extern __shared__ __align__(16) uint8_t smem_att[];
   pdl_entry();
-  const int nkp = (p.Nk + KB - 1) / KB * KB;
+  const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * TQ;
+  const int nq = q_count(p, b), nk = k_count(p, b);
+  if (q0 >= nq) return;   // a query tile past this sample's rows (packed rows)
+  const long long qr = q_row0(p, b) + q0, kr = k_row0(p, b);
+  const int nkp = (nk + KB - 1) / KB * KB;
   const int kch = min(p.kchunk, nkp);   // keys resident at a time: the whole (padded) key range unless it does not fit (long
                                         // sequences in split precision), then chunks streamed through the same panels
   __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_att);
@@ -209,17 +221,16 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
   __nv_bfloat16* sVl = sKl + (SPLIT ? kch * LD : 0);
   float* sMask = reinterpret_cast<float*>(sVl + (SPLIT ? kch * LD : 0));
 
-  const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * TQ;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
 
-  load_panel<D>(sQ, p.Q + ((long long)b * p.Nq + q0) * p.ldq + h * D, p.ldq, min(TQ, p.Nq - q0), TQ);
-  if constexpr (SPLIT) load_panel<D>(sQl, p.Ql + ((long long)b * p.Nq + q0) * p.ldq + h * D, p.ldq, min(TQ, p.Nq - q0), TQ);
+  load_panel<D>(sQ, p.Q + qr * p.ldq + h * D, p.ldq, min(TQ, nq - q0), TQ);
+  if constexpr (SPLIT) load_panel<D>(sQl, p.Ql + qr * p.ldq + h * D, p.ldq, min(TQ, nq - q0), TQ);
   for (int j = threadIdx.x; j < nkp; j += ATT_THREADS)
-    sMask[j] = (j < p.Nk) ? (p.mask ? p.mask[(long long)b * p.Nk + j] * LOG2E : 0.f) : -CUDART_INF_F;
+    sMask[j] = (j < nk) ? (p.mask ? p.mask[(long long)b * p.Nk + j] * LOG2E : 0.f) : -CUDART_INF_F;
 
   const int r0 = warp * 16;
-  const bool active = q0 + r0 < p.Nq;   // a warp whose 16 query rows are all out of range only helps with the loads
+  const bool active = q0 + r0 < nq;   // a warp whose 16 query rows are all out of range only helps with the loads
 
   const float c = p.scale * LOG2E;
   const uint32_t dseed = p.drop.ctr ? drop_seed(p.drop) : 0u;
@@ -230,13 +241,13 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
 
   for (int k0 = 0; k0 < nkp; k0 += kch) {
     const int kc = min(kch, nkp - k0);
-    const int kvalid = max(0, min(kc, p.Nk - k0));
+    const int kvalid = max(0, min(kc, nk - k0));
     if (k0 > 0) __syncthreads();   // every warp is done with the previous chunk's panels
-    load_panel<D>(sK, p.K + ((long long)b * p.Nk + k0) * p.ldk + h * D, p.ldk, kvalid, kc);
-    load_panel<D>(sV, p.V + ((long long)b * p.Nk + k0) * p.ldv + h * D, p.ldv, kvalid, kc);
+    load_panel<D>(sK, p.K + (kr + k0) * p.ldk + h * D, p.ldk, kvalid, kc);
+    load_panel<D>(sV, p.V + (kr + k0) * p.ldv + h * D, p.ldv, kvalid, kc);
     if constexpr (SPLIT) {
-      load_panel<D>(sKl, p.Kl + ((long long)b * p.Nk + k0) * p.ldk + h * D, p.ldk, kvalid, kc);
-      load_panel<D>(sVl, p.Vl + ((long long)b * p.Nk + k0) * p.ldv + h * D, p.ldv, kvalid, kc);
+      load_panel<D>(sKl, p.Kl + (kr + k0) * p.ldk + h * D, p.ldk, kvalid, kc);
+      load_panel<D>(sVl, p.Vl + (kr + k0) * p.ldv + h * D, p.ldv, kvalid, kc);
     }
     cp_async_wait_all();
     __syncthreads();
@@ -288,10 +299,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const AttnParams 
   }
   if (!active) return;
   l[0] = quad_sum(l[0]); l[1] = quad_sum(l[1]);
-  const int rows_valid = p.Nq - q0;
-  store_tile<D>(p.O + ((long long)b * p.Nq + q0) * p.ldo + h * D, p.ldo, o, 1.f / l[0], 1.f / l[1], r0, rows_valid, lane, nullptr,
-                FP16 ? 1 : 0, (SPLIT && p.Ol) ? p.Ol + ((long long)b * p.Nq + q0) * p.ldo + h * D : nullptr);
-  if (p.Ob) store_tile<D>(p.Ob + ((long long)b * p.Nq + q0) * p.ldo + h * D, p.ldo, o, 1.f / l[0], 1.f / l[1], r0, rows_valid, lane);
+  const int rows_valid = nq - q0;
+  store_tile<D>(p.O + qr * p.ldo + h * D, p.ldo, o, 1.f / l[0], 1.f / l[1], r0, rows_valid, lane, nullptr,
+                FP16 ? 1 : 0, (SPLIT && p.Ol) ? p.Ol + qr * p.ldo + h * D : nullptr);
+  if (p.Ob) store_tile<D>(p.Ob + qr * p.ldo + h * D, p.ldo, o, 1.f / l[0], 1.f / l[1], r0, rows_valid, lane);
   if (p.lse && t == 0) {
     float* lse = p.lse + ((long long)b * p.H + h) * p.Nq + q0;
     if (r0 + g < rows_valid) lse[r0 + g] = m[0] + log2f(l[0]);
@@ -307,26 +318,29 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
   constexpr int LD = D + 8;
   extern __shared__ __align__(16) uint8_t smem_att[];
   pdl_entry();
-  const int nkp = (p.Nk + KB - 1) / KB * KB;
+  const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * TQ;
+  const int nq = q_count(p, b), nk = k_count(p, b);
+  if (q0 >= nq) return;
+  const long long qr = q_row0(p, b) + q0, kr = k_row0(p, b);
+  const int nkp = (nk + KB - 1) / KB * KB;
   __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_att);
   __nv_bfloat16* sdO = sQ + TQ * LD;
   __nv_bfloat16* sK = sdO + TQ * LD;
   __nv_bfloat16* sV = sK + nkp * LD;
   float* sMask = reinterpret_cast<float*>(sV + nkp * LD);
 
-  const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * TQ;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int rows_valid = min(TQ, p.Nq - q0);
+  const int rows_valid = min(TQ, nq - q0);
   const bool stage_qkv = DQ || p.drop.ctr;   // with dropout, delta is formed from P and dP (below)
 
-  if (stage_qkv) load_panel<D>(sQ, p.Q + ((long long)b * p.Nq + q0) * p.ldq + h * D, p.ldq, rows_valid, TQ);
-  load_panel<D>(sdO, p.dO + ((long long)b * p.Nq + q0) * p.lddo + h * D, p.lddo, rows_valid, TQ);
+  if (stage_qkv) load_panel<D>(sQ, p.Q + qr * p.ldq + h * D, p.ldq, rows_valid, TQ);
+  load_panel<D>(sdO, p.dO + qr * p.lddo + h * D, p.lddo, rows_valid, TQ);
   if (stage_qkv) {
-    load_panel<D>(sK, p.K + (long long)b * p.Nk * p.ldk + h * D, p.ldk, p.Nk, nkp);
-    load_panel<D>(sV, p.V + (long long)b * p.Nk * p.ldv + h * D, p.ldv, p.Nk, nkp);
+    load_panel<D>(sK, p.K + kr * p.ldk + h * D, p.ldk, nk, nkp);
+    load_panel<D>(sV, p.V + kr * p.ldv + h * D, p.ldv, nk, nkp);
     for (int j = threadIdx.x; j < nkp; j += ATT_THREADS)
-      sMask[j] = (j < p.Nk) ? (p.mask ? p.mask[(long long)b * p.Nk + j] * LOG2E : 0.f) : -CUDART_INF_F;
+      sMask[j] = (j < nk) ? (p.mask ? p.mask[(long long)b * p.Nk + j] * LOG2E : 0.f) : -CUDART_INF_F;
   }
   cp_async_wait_all();
   __syncthreads();
@@ -383,7 +397,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
     // delta = rowsum(dO o O) must cancel against dP = dO V^T formed from the bf16-rounded V: use the bf16 copy of O when the
     // forward wrote one (an fp16 O differs from P V_bf16 by the bf16 rounding of V, which peaked rows do not forgive)
     const int o_fp16 = p.Ob ? 0 : p.qkv_fp16;
-    const __nv_bfloat16* Og = (p.Ob ? p.Ob : p.O) + ((long long)b * p.Nq + q0) * p.ldo + h * D;
+    const __nv_bfloat16* Og = (p.Ob ? p.Ob : p.O) + qr * p.ldo + h * D;
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int r = r0 + g + hh * 8;
@@ -441,7 +455,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const AttnPara
     }
     mma_p_b<D>(dq, s, sK, kb, lane, p.Nk);
   }
-  store_tile<D>(p.dQ + ((long long)b * p.Nq + q0) * p.lddq + h * D, p.lddq, dq, p.scale, p.scale, r0, rows_valid, lane,
+  store_tile<D>(p.dQ + qr * p.lddq + h * D, p.lddq, dq, p.scale, p.scale, r0, rows_valid, lane,
                 p.dbq ? p.dbq + h * D : nullptr);
 }
 
@@ -451,7 +465,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
   constexpr int LD = D + 8;
   extern __shared__ __align__(16) uint8_t smem_att[];
   pdl_entry();
-  const int nqp = (p.Nq + KB - 1) / KB * KB;
+  const int b = blockIdx.z, h = blockIdx.y, k0 = blockIdx.x * TQ;
+  const int nq = q_count(p, b), nk = k_count(p, b);
+  if (k0 >= nk) return;
+  const long long qr = q_row0(p, b), kr = k_row0(p, b) + k0;
+  const int nqp = (nq + KB - 1) / KB * KB;
   __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(smem_att);
   __nv_bfloat16* sV = sK + TQ * LD;
   __nv_bfloat16* sQ = sV + TQ * LD;
@@ -459,21 +477,20 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
   float* sLse = reinterpret_cast<float*>(sdO + nqp * LD);
   float* sDelta = sLse + nqp;
 
-  const int b = blockIdx.z, h = blockIdx.y, k0 = blockIdx.x * TQ;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
-  const int rows_valid = min(TQ, p.Nk - k0);
+  const int rows_valid = min(TQ, nk - k0);
 
-  load_panel<D>(sK, p.K + ((long long)b * p.Nk + k0) * p.ldk + h * D, p.ldk, rows_valid, TQ);
-  load_panel<D>(sV, p.V + ((long long)b * p.Nk + k0) * p.ldv + h * D, p.ldv, rows_valid, TQ);
-  load_panel<D>(sQ, p.Q + (long long)b * p.Nq * p.ldq + h * D, p.ldq, p.Nq, nqp);
-  load_panel<D>(sdO, p.dO + (long long)b * p.Nq * p.lddo + h * D, p.lddo, p.Nq, nqp);
+  load_panel<D>(sK, p.K + kr * p.ldk + h * D, p.ldk, rows_valid, TQ);
+  load_panel<D>(sV, p.V + kr * p.ldv + h * D, p.ldv, rows_valid, TQ);
+  load_panel<D>(sQ, p.Q + qr * p.ldq + h * D, p.ldq, nq, nqp);
+  load_panel<D>(sdO, p.dO + qr * p.lddo + h * D, p.lddo, nq, nqp);
   {
     const float* lse = p.lse + ((long long)b * p.H + h) * p.Nq;
     const float* dg = p.delta + ((long long)b * p.H + h) * p.Nq;
     for (int i = threadIdx.x; i < nqp; i += ATT_THREADS) {
-      sLse[i] = (i < p.Nq) ? lse[i] : CUDART_INF_F;  // +inf -> P = 0 for padded query columns
-      sDelta[i] = (i < p.Nq) ? dg[i] : 0.f;
+      sLse[i] = (i < nq) ? lse[i] : CUDART_INF_F;  // +inf -> P = 0 for padded query columns
+      sDelta[i] = (i < nq) ? dg[i] : 0.f;
     }
   }
   cp_async_wait_all();
@@ -531,8 +548,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const AttnPar
     mma_p_b<D>(dv, pt, sdO, qb, lane, p.Nq);
     mma_p_b<D>(dk, st, sQ, qb, lane, p.Nq);
   }
-  store_tile<D>(p.dV + ((long long)b * p.Nk + k0) * p.lddv + h * D, p.lddv, dv, 1.f, 1.f, r0, rows_valid, lane, p.dbv ? p.dbv + h * D : nullptr);
-  store_tile<D>(p.dK + ((long long)b * p.Nk + k0) * p.lddk + h * D, p.lddk, dk, p.scale, p.scale, r0, rows_valid, lane, p.dbk ? p.dbk + h * D : nullptr);
+  store_tile<D>(p.dV + kr * p.lddv + h * D, p.lddv, dv, 1.f, 1.f, r0, rows_valid, lane, p.dbv ? p.dbv + h * D : nullptr);
+  store_tile<D>(p.dK + kr * p.lddk + h * D, p.lddk, dk, p.scale, p.scale, r0, rows_valid, lane, p.dbk ? p.dbk + h * D : nullptr);
 }
 
 
@@ -568,8 +585,11 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
   constexpr int LD = D + 8;
   extern __shared__ __align__(16) uint8_t smem_att[];
   pdl_entry();
-  const int nqp = (p.Nq + 15) / 16 * 16;        // query rows staged (16-row warp tiles)
-  const int nkp = (p.Nk + KB - 1) / KB * KB;    // key rows staged (64-key blocks)
+  const int b = blockIdx.y, h = blockIdx.x;
+  const int nq = q_count(p, b), nk = k_count(p, b);
+  const long long qr = q_row0(p, b), kr = k_row0(p, b);
+  const int nqp = (nq + 15) / 16 * 16;        // query rows staged (16-row warp tiles)
+  const int nkp = (nk + KB - 1) / KB * KB;    // key rows staged (64-key blocks)
   const int LDP = nkp + 8;
   __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_att);
   __nv_bfloat16* sdO = sQ + nqp * LD;
@@ -580,16 +600,15 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
   // the P / dS tiles are staged for phase 2, and with dropout also for phase 1 (see there)
   float* sMask = reinterpret_cast<float*>((DKV || p.drop.ctr) ? sdS + nqp * LDP : sP);
 
-  const int b = blockIdx.y, h = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
 
-  load_panel<D, ATT1_THREADS>(sQ, p.Q + (long long)b * p.Nq * p.ldq + h * D, p.ldq, p.Nq, nqp);
-  load_panel<D, ATT1_THREADS>(sdO, p.dO + (long long)b * p.Nq * p.lddo + h * D, p.lddo, p.Nq, nqp);
-  load_panel<D, ATT1_THREADS>(sK, p.K + (long long)b * p.Nk * p.ldk + h * D, p.ldk, p.Nk, nkp);
-  load_panel<D, ATT1_THREADS>(sV, p.V + (long long)b * p.Nk * p.ldv + h * D, p.ldv, p.Nk, nkp);
+  load_panel<D, ATT1_THREADS>(sQ, p.Q + qr * p.ldq + h * D, p.ldq, nq, nqp);
+  load_panel<D, ATT1_THREADS>(sdO, p.dO + qr * p.lddo + h * D, p.lddo, nq, nqp);
+  load_panel<D, ATT1_THREADS>(sK, p.K + kr * p.ldk + h * D, p.ldk, nk, nkp);
+  load_panel<D, ATT1_THREADS>(sV, p.V + kr * p.ldv + h * D, p.ldv, nk, nkp);
   for (int j = threadIdx.x; j < nkp; j += ATT1_THREADS)
-    sMask[j] = (j < p.Nk) ? (p.mask ? p.mask[(long long)b * p.Nk + j] * LOG2E : 0.f) : -CUDART_INF_F;
+    sMask[j] = (j < nk) ? (p.mask ? p.mask[(long long)b * p.Nk + j] * LOG2E : 0.f) : -CUDART_INF_F;
   cp_async_wait_all();
   __syncthreads();
   if (p.qkv_fp16) {
@@ -605,11 +624,11 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
     float dl[2] = {0.f, 0.f};   // delta = rowsum(dO o O)
     if (!p.drop.ctr) {
       const int o_fp16 = p.Ob ? 0 : p.qkv_fp16;      // see attn_bwd_dq_kernel: the bf16 copy of O keeps delta consistent with dP
-      const __nv_bfloat16* Og = (p.Ob ? p.Ob : p.O) + (long long)b * p.Nq * p.ldo + h * D;
+      const __nv_bfloat16* Og = (p.Ob ? p.Ob : p.O) + qr * p.ldo + h * D;
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int r = r0 + g + hh * 8;
-        if (r < p.Nq) {
+        if (r < nq) {
           float acc = 0.f;
           for (int cidx = t * 8; cidx < D; cidx += 32) {
             const uint4 ov = __ldg(reinterpret_cast<const uint4*>(Og + (long long)r * p.ldo + cidx));
@@ -630,8 +649,8 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
     float ls[2] = {CUDART_INF_F, CUDART_INF_F};   // +inf -> P = 0 on padded query rows (their tiles must be zero for phase 2)
     {
       const float* lse = p.lse + ((long long)b * p.H + h) * p.Nq;
-      if (r0 + g < p.Nq) ls[0] = lse[r0 + g];
-      if (r0 + g + 8 < p.Nq) ls[1] = lse[r0 + g + 8];
+      if (r0 + g < nq) ls[0] = lse[r0 + g];
+      if (r0 + g + 8 < nq) ls[1] = lse[r0 + g + 8];
     }
     float dq[D / 8][4];
 #pragma unroll
@@ -734,13 +753,13 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
       if constexpr (DQ) mma_p_b<D>(dq, s, sK, kb, lane, p.Nk);
     }
     if constexpr (DQ)
-      store_tile<D>(p.dQ + (long long)b * p.Nq * p.lddq + h * D, p.lddq, dq, p.scale, p.scale, r0, p.Nq, lane,
+      store_tile<D>(p.dQ + qr * p.lddq + h * D, p.lddq, dq, p.scale, p.scale, r0, nq, lane,
                     p.dbq ? p.dbq + h * D : nullptr);
   }
   if constexpr (!DKV) return;
   __syncthreads();
   // ---- phase 2: this warp's 16 key rows
-  if (r0 < p.Nk) {
+  if (r0 < nk) {
     float dk[D / 8][4], dv[D / 8][4];
 #pragma unroll
     for (int i = 0; i < D / 8; ++i) {
@@ -751,8 +770,8 @@ __global__ void __launch_bounds__(ATT1_THREADS) attn_bwd_fused_kernel(const Attn
       mma_at_b<D>(dv, sP, LDP, r0, sdO, q, lane);
       mma_at_b<D>(dk, sdS, LDP, r0, sQ, q, lane);
     }
-    store_tile<D>(p.dV + (long long)b * p.Nk * p.lddv + h * D, p.lddv, dv, 1.f, 1.f, r0, p.Nk, lane, p.dbv ? p.dbv + h * D : nullptr);
-    store_tile<D>(p.dK + (long long)b * p.Nk * p.lddk + h * D, p.lddk, dk, p.scale, p.scale, r0, p.Nk, lane, p.dbk ? p.dbk + h * D : nullptr);
+    store_tile<D>(p.dV + kr * p.lddv + h * D, p.lddv, dv, 1.f, 1.f, r0, nk, lane, p.dbv ? p.dbv + h * D : nullptr);
+    store_tile<D>(p.dK + kr * p.lddk + h * D, p.lddk, dk, p.scale, p.scale, r0, nk, lane, p.dbk ? p.dbk + h * D : nullptr);
   }
 }
 
@@ -809,6 +828,9 @@ static int validate(const vb_attn_args* a, bool bwd) {
   if (a->D != 16 && a->D != 32 && a->D != 64 && a->D != 128)
     return set_error(VB_ERR_UNSUPPORTED, "vb_attention: head dim %d not in {16,32,64,128}", a->D);
   if (!a->Q || !a->K || !a->V || !a->O) return set_error(VB_ERR_INVALID, "vb_attention: null tensor");
+  if (!a->q_off != !a->q_len || !a->q_off != !a->k_off || !a->q_off != !a->k_len)
+    return set_error(VB_ERR_INVALID, "vb_attention: packed rows need q_off, q_len, k_off and k_len together");
+  if (a->q_off && a->mask) return set_error(VB_ERR_INVALID, "vb_attention: packed rows take no additive mask (the lengths exclude the keys)");
   if ((a->ldq % 8) || (a->ldk % 8) || (a->ldv % 8) || (a->ldo % 8) || !al16(a->Q) || !al16(a->K) || !al16(a->V) || !al16(a->O))
     return set_error(VB_ERR_INVALID, "vb_attention: tensors need ld %% 8 == 0 and 16-byte aligned bases");
   if (bwd) {
@@ -845,6 +867,7 @@ static AttnParams to_params(const vb_attn_args* a) {
   p.Ol = (__nv_bfloat16*)a->O_lo;
   p.Ob = (__nv_bfloat16*)a->O_b16;
   p.kchunk = 1 << 30;
+  p.qoff = a->q_off; p.qlen = a->q_len; p.koff = a->k_off; p.klen = a->k_len;
   return p;
 }
 
@@ -948,6 +971,7 @@ extern "C" vb_status vb_attention_bwd(const vb_attn_args* a, void* stream) {
 extern "C" vb_status vb_attention_probs(const vb_attn_args* a, float* probs, void* stream) {
   using namespace vb;
   if (!a || !probs || !a->Q || !a->K) return set_error(VB_ERR_INVALID, "vb_attention_probs: null argument");
+  if (a->q_off) return set_error(VB_ERR_UNSUPPORTED, "vb_attention_probs: the probability export reads the padded layout only");
   if (a->B <= 0 || a->H <= 0 || a->Nq <= 0 || a->Nk <= 0 || (a->D % 8) || a->D > 512) return set_error(VB_ERR_INVALID, "vb_attention_probs: bad shape");
   if ((a->ldq % 8) || (a->ldk % 8) || !al16(a->Q) || !al16(a->K)) return set_error(VB_ERR_INVALID, "vb_attention_probs: Q / K need ld %% 8 == 0 and 16-byte aligned bases");
   AttnParams p = to_params(a);

@@ -46,8 +46,13 @@ struct DropCfg {
   uint32_t site;         // id of the dropout layer
   uint32_t thresh;       // p * 2^32
   float scale;           // 1 / (1 - p)
+  const int* rows = nullptr;   // row-indexed sites of a packed plan: the padded row whose mask each packed row draws (vb_dropout.row_map)
 };
 __device__ __forceinline__ uint32_t drop_seed(const DropCfg& d) { return hash32(d.site + (*d.ctr) * 0x9E3779B9U); }
+// element index of column c of row r of a row-indexed dropout site (row-major [rows, H]), at padded coordinates under a row map
+__device__ __forceinline__ uint32_t drop_index(const DropCfg& d, long long r, long long H, long long c) {
+  return (uint32_t)((d.rows ? (long long)d.rows[r] : r) * H + c);
+}
 __device__ __forceinline__ float drop_apply(float v, uint32_t seed, uint32_t idx, const DropCfg& d) {
   return hash32(idx ^ seed) >= d.thresh ? v * d.scale : 0.f;
 }

@@ -56,7 +56,7 @@ ln_fwd_kernel(const float* x, long long ldx, const float* __restrict__ gamma, co
       if (ADD && c < n4) {
         const float4 rv = reinterpret_cast<const float4*>(r + row * ldr)[c];
         if (drop_in.ctr) {
-          const uint32_t e0 = (uint32_t)(row * H + c * 4);
+          const uint32_t e0 = drop_index(drop_in, row, H, c * 4);
           v[i].x = drop_apply(v[i].x, seed_in, e0, drop_in); v[i].y = drop_apply(v[i].y, seed_in, e0 + 1, drop_in);
           v[i].z = drop_apply(v[i].z, seed_in, e0 + 2, drop_in); v[i].w = drop_apply(v[i].w, seed_in, e0 + 3, drop_in);
         }
@@ -92,7 +92,7 @@ ln_fwd_kernel(const float* x, long long ldx, const float* __restrict__ gamma, co
         o.z = (v[i].z - mean) * rstd * g.z + b.z;
         o.w = (v[i].w - mean) * rstd * g.w + b.w;
         if (drop.ctr) {   // dropout(LayerNorm(x)) of the embeddings (vilbert.py:365, 1430); element index row*H + col
-          const uint32_t e0 = (uint32_t)(row * H + c * 4);
+          const uint32_t e0 = drop_index(drop, row, H, c * 4);
           o.x = drop_apply(o.x, dseed, e0, drop); o.y = drop_apply(o.y, dseed, e0 + 1, drop);
           o.z = drop_apply(o.z, dseed, e0 + 2, drop); o.w = drop_apply(o.w, dseed, e0 + 3, drop);
         }
@@ -163,7 +163,7 @@ ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ dy2, long 
         }
         const float4 xv = xr[c], gm = reinterpret_cast<const float4*>(gamma)[c];
         if (drop_out.ctr) {
-          const uint32_t e0 = (uint32_t)(row * H + c * 4);
+          const uint32_t e0 = drop_index(drop_out, row, H, c * 4);
           d.x = drop_apply(d.x, seed_out, e0, drop_out); d.y = drop_apply(d.y, seed_out, e0 + 1, drop_out);
           d.z = drop_apply(d.z, seed_out, e0 + 2, drop_out); d.w = drop_apply(d.w, seed_out, e0 + 3, drop_out);
         }
@@ -200,7 +200,7 @@ ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ dy2, long 
             o.x *= p01.x; o.y *= p01.y; o.z *= p23.x; o.w *= p23.y;   // pre = gelu'(pre-activation) saved by the forward GEMM
           }
           if (drop_in.ctr) {   // gradient of dropout(dense(x)): same mask as the forward GEMM epilogue (index row*H + col)
-            const uint32_t e0 = (uint32_t)(row * H + c * 4);
+            const uint32_t e0 = drop_index(drop_in, row, H, c * 4);
             o.x = drop_apply(o.x, seed_in, e0, drop_in); o.y = drop_apply(o.y, seed_in, e0 + 1, drop_in);
             o.z = drop_apply(o.z, seed_in, e0 + 2, drop_in); o.w = drop_apply(o.w, seed_in, e0 + 3, drop_in);
           }
@@ -460,7 +460,7 @@ small_linear_fwd_kernel(const float* __restrict__ x, long long ldx, const float*
       float acc = 0.f;
       for (int k = lane; k < K; k += 32) {
         float xv = xr[k];
-        if (drop.ctr) xv = drop_apply(xv, dseed, (uint32_t)(row * K + k), drop);
+        if (drop.ctr) xv = drop_apply(xv, dseed, drop_index(drop, row, K, k), drop);
         acc += xv * __ldg(W + (long long)j * K + k);
       }
       acc = warp_sum(acc);
@@ -484,7 +484,7 @@ small_linear_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ 
         float acc = 0.f;
         for (long long m = blockIdx.x; m < M; m += gridDim.x) {
           float xv = x[m * ldx + k];
-          if (drop.ctr) xv = drop_apply(xv, dseed, (uint32_t)(m * K + k), drop);
+          if (drop.ctr) xv = drop_apply(xv, dseed, drop_index(drop, m, K, k), drop);
           acc += dy[m * N + j] * xv;
         }
         atomicAdd(dW + (long long)j * K + k, acc);
@@ -500,7 +500,7 @@ small_linear_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ 
       for (int k = threadIdx.x; k < K; k += ROW_THREADS) {
         float acc = 0.f;
         for (int j = 0; j < N; ++j) acc += dy[m * N + j] * __ldg(W + (long long)j * K + k);
-        if (drop.ctr) acc = drop_apply(acc, dseed, (uint32_t)(m * K + k), drop);
+        if (drop.ctr) acc = drop_apply(acc, dseed, drop_index(drop, m, K, k), drop);
         float* d = dx + m * lddx + k;
         *d = accumulate_dx ? (*d + acc) : acc;
       }
@@ -737,6 +737,7 @@ static inline DropCfg make_drop(const vb_dropout* d) {
   c.site = d ? d->site : 0u;
   c.thresh = on ? (uint32_t)((double)d->p * 4294967296.0) : 0u;
   c.scale = on && d->p < 1.f ? 1.f / (1.f - d->p) : 1.f;
+  c.rows = on ? d->row_map : nullptr;
   return c;
 }
 

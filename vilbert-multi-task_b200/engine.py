@@ -23,7 +23,7 @@ activations and weights exist only as tensor-core operands. Three operand precis
 import ctypes as C
 import math
 import zlib
-from collections import OrderedDict, namedtuple
+from collections import Counter, OrderedDict, namedtuple
 
 import torch
 
@@ -40,6 +40,23 @@ BASE_HEAD_NAMES = ("vil_prediction", "vil_logit", "vil_binary_prediction", "visi
 BASE_BERT_OUT_NAMES = ("sequence_output", "pooled_output")
 # the float inputs a plan can backpropagate into (Plan(input_grads=...)): the region features and their boxes
 INPUT_GRAD_NAMES = ("input_imgs", "image_loc")
+# heads a packed plan (Plan(packed=...)) can build: the pooled heads and the per-region logit, which it scatters back to the padded
+# layout; the per-token and per-region prediction heads of pre-training are not packed
+PACKED_HEADS = ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_prediction", "vil_tri_prediction", "vision_logit")
+# the value a masked region's logit takes in a packed plan: the reference's additive mask, which in fp32 is no further from it
+# (BCE-with-logits at target 0 of either is 0.0 with gradient 0.0)
+PACKED_MASKED_LOGIT = -10000.0
+
+
+def pack_capacity(count, padded_rows):
+    """Rows of a packed stream holding `count` valid rows of a padded [B, N] batch: count rounded up to a step of one sixteenth
+    of the padded rows, itself a multiple of the GEMMs' 128-row tile, and never more than the padded rows. The valid-row sum of a
+    64-256-sample batch moves by a few percent from batch to batch, less than one step, so a task settles on one or two
+    capacities (plans), and the rows a capacity wastes are at most a sixteenth of the padded ones."""
+    if count < 1:
+        raise ValueError("a packed stream needs at least one valid row")
+    step = max(128, -(-padded_rows // 16 // 128) * 128)
+    return min(-(-count // step) * step, padded_rows)
 
 
 def _pad8(n):
@@ -404,8 +421,9 @@ class Plan:
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
                  loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-                 input_grads=frozenset()):
+                 input_grads=frozenset(), packed=None):
         self.e, self.cfg = engine, engine.cfg
+        self.packed = None if packed is None else (int(packed[0]), int(packed[1]))
         self.frozen = frozenset(frozen)
         unknown = sorted(n for n in self.frozen if n not in engine.ps.entries)
         if unknown:
@@ -451,6 +469,8 @@ class Plan:
         self.keep = None if outputs is None else frozenset(outputs)
         self.results = results
         self._check_outputs()
+        if self.packed is not None:
+            self._check_packed(outputs)
         self.fwd_id = 0
         self.fwd, self.bwd = [], []
         self.prologue = []       # optional per-step ops run before the forward (see enable_training_prologue)
@@ -499,6 +519,22 @@ class Plan:
             raise ValueError("image_prefix keeps the image states across forwards: forward-only plans (no train mode, no grad_outputs)")
         if self.image_prefix and self.pairs:
             raise ValueError("image_prefix: in_batch_pairs re-expands the image batch inside the forward")
+
+    def _check_packed(self, outputs):
+        """packed=(rows_t, rows_v): the two streams hold the valid rows only (DESIGN.md §4g). Refused with the options that reshape
+        or export the padded streams, with input gradients (they are padded tensors) and with heads that are not packed."""
+        rows_t, rows_v = self.packed
+        if rows_t < 1 or rows_v < 1 or rows_t > self.B * self.Nt or rows_v > self.B * self.Nv:
+            raise ValueError(f"packed={self.packed}: the rows of each stream must lie in [1, B * N] = [1, {self.B * self.Nt}], "
+                             f"[1, {self.B * self.Nv}]")
+        bad = [n for n, on in (("in_batch_pairs", self.pairs), ("fast_mode", self.fast), ("dynamic_attention", self.dyn),
+                               ("visualization", self.viz), ("image_prefix", self.image_prefix), ("input_grads", bool(self.input_grads)))
+               if on]
+        if bad:
+            raise NotImplementedError(f"packed plans do not support {', '.join(bad)}")
+        if (self.e.ps.heads != "vl") or outputs is None or any(n not in PACKED_HEADS for n in outputs):
+            raise NotImplementedError(f"packed plans build heads of VILBertForVLTasks among {PACKED_HEADS} only (outputs=...), got "
+                                      f"{None if outputs is None else sorted(outputs)}")
 
     def _check_outputs(self):
         """Build-time checks of outputs= and results=: known head names, and every head the objective, a gradient or the results
@@ -666,12 +702,16 @@ class Plan:
             return None
         return t.data_ptr() if torch.is_tensor(t) else int(t)
 
-    def drop(self, name, p):
-        """ctypes byref of a vb_dropout for the dropout layer `name` with probability p, or None when inactive."""
+    def drop(self, name, p, rows=None):
+        """ctypes byref of a vb_dropout for the dropout layer `name` with probability p, or None when inactive. rows: the stream
+        ("t" / "v") of a row-indexed site; a packed plan gives it the stream's packed-row -> padded-row map, so its rows draw the
+        masks of the padded rows they hold."""
         if not self.train or p is None or p <= 0.0:
             return None
         d = L.Dropout()
         d.step, d.site, d.p = self.e.drop_step.data_ptr(), dropout_site_id(name), float(p)
+        if self.packed and rows is not None:
+            d.row_map = (self.map_t if rows == "t" else self.map_v).data_ptr()
         self._keep.append(d)
         return d
 
@@ -724,8 +764,9 @@ class Plan:
         self.emit(self.lib.vb_gemm_bf16, C.byref(g))
 
     def attention(self, bwd, B, H, Nq, Nk, D, Q, ldq, K, ldk, V, ldv, mask, O, ldo, lse, dO=None, lddo=0, dQ=None, lddq=0,
-                  dK=None, lddk=0, dV=None, lddv=0, delta=None, dbq=None, dbk=None, dbv=None, dropout=None):
-        """Q, K, V and O are Operands (the forward's; the backward re-reads them), dO / dQ / dK / dV bf16 tensors."""
+                  dK=None, lddk=0, dV=None, lddv=0, delta=None, dbq=None, dbk=None, dbv=None, dropout=None, segs=None):
+        """Q, K, V and O are Operands (the forward's; the backward re-reads them), dO / dQ / dK / dV bf16 tensors. segs: the
+        (offsets, lengths) of the query and of the key stream of a packed plan (mask is then None)."""
         self._check_operands((Q, K, V, O), (dO, dQ, dK, dV))
         a = L.AttnArgs()
         a.qkv_fp16 = Q.fp16
@@ -741,6 +782,9 @@ class Plan:
         a.dbias_q, a.dbias_k, a.dbias_v = self._ptr(dbq), self._ptr(dbk), self._ptr(dbv)
         if dropout is not None:
             a.dropout = dropout
+        if segs is not None:
+            (qo, ql), (ko, kl) = segs
+            a.q_off, a.q_len, a.k_off, a.k_len = qo.data_ptr(), ql.data_ptr(), ko.data_ptr(), kl.data_ptr()
         self._keep.append(a)
         self.emit(self.lib.vb_attention_bwd if bwd else self.lib.vb_attention_fwd, C.byref(a))
         if not bwd and self.viz:
@@ -748,6 +792,15 @@ class Plan:
             probs = self.buf((B, H, Nq, Nk), F32)
             self.emit(self.lib.vb_attention_probs, C.byref(a), probs.data_ptr())
             self._last_attn = dict(attn=probs, q=Q.hi, k=K.hi, B=B, H=H, Nq=Nq, Nk=Nk, D=D)
+
+    def zero_tail(self, stream, *ts):
+        """Packed plans: rows of no sample (past off[B] of the stream "t" / "v") of the 2-D tensors `ts` (same shape and pitch; None
+        entries skipped) set to zero. The attention kernels do not write them, and every later op reads them: a GEMM's weight
+        gradient multiplies them by a zero gradient, which garbage would turn into NaN."""
+        ts = [t for t in ts if t is not None]
+        off = self.seg[stream][0]
+        self.emit(self.lib.vb_zero_tail_rows, *[self._ptr(t) for t in ts], *([None] * (3 - len(ts))), ts[0].stride(0) * ts[0].element_size(),
+                  ts[0].shape[1] * ts[0].element_size(), off.data_ptr() + 4 * self.B, ts[0].shape[0])
 
     def ln_fwd(self, x, gamma, beta, M, H, want_f32=True, out_drop=None, res=None, in_drop=None):
         """-> (fp32 output or None, Operand output, mean, rstd). res: LayerNorm of dropout_in(x) + res instead (the residual add is
@@ -922,14 +975,17 @@ class Plan:
         lse = self.buf((B, nh, N), F32)
         q, k, v = qkv.cols(0, H), qkv.cols(H, 2 * H), qkv.cols(2 * H, 3 * H)
         adrop = self.drop(prefix + ".self.dropout", p_attn)
-        self.attention(False, B, nh, N, N, D, q, 3 * H, k, 3 * H, v, 3 * H, mask, ctx, H, lse, dropout=adrop)
+        segs = (self.seg[tag], self.seg[tag]) if self.packed else None
+        self.attention(False, B, nh, N, N, D, q, 3 * H, k, 3 * H, v, 3 * H, mask, ctx, H, lse, dropout=adrop, segs=segs)
+        if self.packed:
+            self.zero_tail(tag, ctx.hi, ctx.lo, ctx.extra_bw)
         if self.viz:
             (self.attn_t if tag == "t" else self.attn_v).append(self._last_attn)
         qkv_rg = x.rg or self.trainable(prefix + ".self.qkv")
         gate_rg = pool is not None and (pool.rg or self.trainable(prefix + ".self.dy"))
         ctx_rg = qkv_rg or gate_rg
         out, out_bwd = self.dense_res_ln(ctx, H, x, prefix + ".output.dense", prefix + ".output.LayerNorm", tag + ".ao",
-                                         drop=self.drop(prefix + ".output.dropout", p_hidden), a_rg=ctx_rg)
+                                         drop=self.drop(prefix + ".output.dropout", p_hidden, tag), a_rg=ctx_rg)
 
         def bwd():
             r = out_bwd()
@@ -945,7 +1001,9 @@ class Plan:
             gated = pool is not None                 # ... except under the gate, where the biases sit before the scaling
             self.attention(True, B, nh, N, N, D, q, 3 * H, k, 3 * H, v, 3 * H, mask, ctx, H, lse, dO=dctx, lddo=H,
                            dQ=dqkv[:, 0:H], lddq=3 * H, dK=dqkv[:, H:2 * H], lddk=3 * H, dV=dqkv[:, 2 * H:], lddv=3 * H, delta=delta,
-                           dbq=None if gated else gq, dbk=None if gated else gk, dbv=gv, dropout=adrop)
+                           dbq=None if gated else gq, dbk=None if gated else gk, dbv=gv, dropout=adrop, segs=segs)
+            if self.packed:
+                self.zero_tail(tag, dqkv)
             if gated:
                 # the gate Linear needs dz32 for its bias sum, dz16 for its weight gradient and for d pool
                 dyw_rg = self.trainable(prefix + ".self.dy.weight") or pool.rg
@@ -984,10 +1042,16 @@ class Plan:
         # dropout1 acts on attention_probs1 (text queries over regions), dropout2 on attention_probs2 (vilbert.py:730, 738, 778, 800)
         adrop1 = self.drop(p + ".biattention.dropout1", c.v_attention_probs_dropout_prob)
         adrop2 = self.drop(p + ".biattention.dropout2", c.attention_probs_dropout_prob)
-        self.attention(False, B, nh, Nt, Nv, D, q2, L3, k1, L3, v1, L3, self.mask_v, ctx1, Hb, lse1, dropout=adrop1)
+        seg_tv = (self.seg["t"], self.seg["v"]) if self.packed else None
+        seg_vt = (self.seg["v"], self.seg["t"]) if self.packed else None
+        self.attention(False, B, nh, Nt, Nv, D, q2, L3, k1, L3, v1, L3, self.mask_v, ctx1, Hb, lse1, dropout=adrop1, segs=seg_tv)
+        if self.packed:
+            self.zero_tail("t", ctx1.hi, ctx1.lo, ctx1.extra_bw)
         a1 = self._last_attn if self.viz else None
         with self.on(1):
-            self.attention(False, B, nh, Nv, Nt, D, q1, L3, k2, L3, v2, L3, self.mask_t, ctx2, Hb, lse2, dropout=adrop2)
+            self.attention(False, B, nh, Nv, Nt, D, q1, L3, k2, L3, v2, L3, self.mask_t, ctx2, Hb, lse2, dropout=adrop2, segs=seg_vt)
+            if self.packed:
+                self.zero_tail("v", ctx2.hi, ctx2.lo, ctx2.extra_bw)
             a2 = self._last_attn if self.viz else None
         if self.viz:
             self.attn_c.append((a1, a2))
@@ -999,9 +1063,9 @@ class Plan:
         ctx_rg = need1 or need2
         with self.on(1):
             v1o, v1_bwd = self.dense_res_ln(ctx2, Hb, v, p + ".biOutput.dense1", p + ".biOutput.LayerNorm1", "c.v.bo",
-                                            drop=self.drop(p + ".biOutput.dropout1", c.v_hidden_dropout_prob), a_rg=ctx_rg)
+                                            drop=self.drop(p + ".biOutput.dropout1", c.v_hidden_dropout_prob, "v"), a_rg=ctx_rg)
         t1o, t1_bwd = self.dense_res_ln(ctx1, Hb, t, p + ".biOutput.dense2", p + ".biOutput.LayerNorm2", "c.t.bo",
-                                        drop=self.drop(p + ".biOutput.dropout2", c.hidden_dropout_prob), a_rg=ctx_rg)
+                                        drop=self.drop(p + ".biOutput.dropout2", c.hidden_dropout_prob, "t"), a_rg=ctx_rg)
 
         def bwd():
             if not (v1o.gw or t1o.gw):
@@ -1028,10 +1092,14 @@ class Plan:
             part2 = (lambda a, b: dqkv2[:, a:b]) if need2 else (lambda a, b: None)
             self.attention(True, B, nh, Nt, Nv, D, q2, L3, k1, L3, v1, L3, self.mask_v, ctx1, Hb, lse1, dO=dctx1, lddo=Hb,
                            dQ=part2(0, Hb), lddq=L3, dK=part1(Hb, 2 * Hb), lddk=L3, dV=part1(2 * Hb, L3), lddv=L3, delta=d1,
-                           dbq=gq2, dbk=gk1, dbv=gv1, dropout=adrop1)
+                           dbq=gq2, dbk=gk1, dbv=gv1, dropout=adrop1, segs=seg_tv)
             self.attention(True, B, nh, Nv, Nt, D, q1, L3, k2, L3, v2, L3, self.mask_t, ctx2, Hb, lse2, dO=dctx2, lddo=Hb,
                            dQ=part1(0, Hb), lddq=L3, dK=part2(Hb, 2 * Hb), lddk=L3, dV=part2(2 * Hb, L3), lddv=L3, delta=d2,
-                           dbq=gq1, dbk=gk2, dbv=gv2, dropout=adrop2)
+                           dbq=gq1, dbk=gk2, dbv=gv2, dropout=adrop2, segs=seg_vt)
+            if self.packed:
+                for stream, need, d in (("v", need1, dqkv1), ("t", need2, dqkv2)):
+                    if need:
+                        self.zero_tail(stream, d)
             if need1:
                 self.linear_wgrad(dqkv1, L3, v.op.bw, Hv, Mv, L3, Hv, p + ".biattention.qkv1")
             if need2:
@@ -1044,9 +1112,9 @@ class Plan:
         self._bwd_emitters.append(None)
         with self.on(1):
             v2o = self.ffn(v1o, c.v_intermediate_size, p + ".v_intermediate.dense", p + ".v_output.dense", p + ".v_output.LayerNorm", "c.v.ffn",
-                           drop=self.drop(p + ".v_output.dropout", c.v_hidden_dropout_prob))
+                           drop=self.drop(p + ".v_output.dropout", c.v_hidden_dropout_prob, "v"))
         t2o = self.ffn(t1o, c.intermediate_size, p + ".t_intermediate.dense", p + ".t_output.dense", p + ".t_output.LayerNorm", "c.t.ffn",
-                       drop=self.drop(p + ".t_output.dropout", c.hidden_dropout_prob))
+                       drop=self.drop(p + ".t_output.dropout", c.hidden_dropout_prob, "t"))
         return v2o, t2o
 
     def broadcast_text(self, t):
@@ -1110,10 +1178,10 @@ class Plan:
     def text_layer(self, x, i):
         p = f"bert.encoder.layer.{i}"
         c = self.cfg
-        h1 = self.self_attention_block(x, x.M // self.Nt, self.Nt, c.num_attention_heads, self.mask_t, p + ".attention", "t",
+        h1 = self.self_attention_block(x, self.B if self.packed else x.M // self.Nt, self.Nt, c.num_attention_heads, self.mask_t, p + ".attention", "t",
                                        p_attn=c.attention_probs_dropout_prob, p_hidden=c.hidden_dropout_prob)
         return self.ffn(h1, c.intermediate_size, p + ".intermediate.dense", p + ".output.dense", p + ".output.LayerNorm", "t.ffn",
-                        drop=self.drop(p + ".output.dropout", c.hidden_dropout_prob))
+                        drop=self.drop(p + ".output.dropout", c.hidden_dropout_prob, "t"))
 
     def text_pool(self, t):
         """dynamic_attention: masked mean of the text states over the tokens (vilbert.py:578-579) as an Act [B, Ht] with GEMM operand
@@ -1137,10 +1205,10 @@ class Plan:
     def image_layer(self, x, i, pool=None):
         p = f"bert.encoder.v_layer.{i}"
         c = self.cfg
-        h1 = self.self_attention_block(x, x.M // self.Nv, self.Nv, c.v_num_attention_heads, self.mask_v, p + ".attention", "v",
+        h1 = self.self_attention_block(x, self.B if self.packed else x.M // self.Nv, self.Nv, c.v_num_attention_heads, self.mask_v, p + ".attention", "v",
                                        p_attn=c.v_attention_probs_dropout_prob, p_hidden=c.v_hidden_dropout_prob, pool=pool)
         return self.ffn(h1, c.v_intermediate_size, p + ".intermediate.dense", p + ".output.dense", p + ".output.LayerNorm", "v.ffn",
-                        drop=self.drop(p + ".output.dropout", c.v_hidden_dropout_prob))
+                        drop=self.drop(p + ".output.dropout", c.v_hidden_dropout_prob, "v"))
 
     # ------------------------------------------------------------------ embeddings
     def embeddings(self):
@@ -1160,21 +1228,37 @@ class Plan:
         self.in_imask = self.buf((B, Nv), I64, zero=True)
         self.in_feat = self.buf((B, Nv, Fv), F32, zero=True)
         self.in_loc = self.buf((B, Nv, 5), F32, zero=True)
-        self.mask_t = self.buf((Bt, Nt), F32)
-        self.mask_v = self.buf((B, Nv), F32, zero=self.image_prefix)
-        self.emit(lib.vb_mask_to_additive, self.in_amask.data_ptr(), self.mask_t.data_ptr(), Bt, self.Nt_in, 1 if self.has_task else 0)
-        if self.image_prefix:
-            self.cur = self.prefix
-        self.emit(lib.vb_mask_to_additive, self.in_imask.data_ptr(), self.mask_v.data_ptr(), B, Nv, 0)
-        self.cur = self.fwd
+        self.seg = {}
+        if self.packed:
+            # the rows of each stream and their padded rows, from the loaded masks (one kernel; the lengths exclude every masked key,
+            # so no additive mask exists)
+            (Mt, Mv), self.mask_t, self.mask_v = self.packed, None, None
+            it = torch.int32
+            self.seg = {"t": (self.buf((B + 1,), it), self.buf((B,), it)), "v": (self.buf((B + 1,), it), self.buf((B,), it))}
+            self.map_t, self.map_v = self.buf((Mt,), it), self.buf((Mv,), it)
+            self.emit(lib.vb_pack_build, self.in_amask.data_ptr(), self.Nt_in, 1 if self.has_task else 0, self.in_imask.data_ptr(), Nv, B, Mt, Mv,
+                      self.seg["t"][0].data_ptr(), self.seg["t"][1].data_ptr(), self.map_t.data_ptr(), self.seg["v"][0].data_ptr(),
+                      self.seg["v"][1].data_ptr(), self.map_v.data_ptr())
+        else:
+            self.mask_t = self.buf((Bt, Nt), F32)
+            self.mask_v = self.buf((B, Nv), F32, zero=self.image_prefix)
+            self.emit(lib.vb_mask_to_additive, self.in_amask.data_ptr(), self.mask_t.data_ptr(), Bt, self.Nt_in, 1 if self.has_task else 0)
+            if self.image_prefix:
+                self.cur = self.prefix
+            self.emit(lib.vb_mask_to_additive, self.in_imask.data_ptr(), self.mask_v.data_ptr(), B, Nv, 0)
+            self.cur = self.fwd
         self.sync_streams()
-        # text: gather-sum (+ task row) then LayerNorm (vilbert.py:346-367)
-        xe = self.buf((Mt, Ht), F32)
+        # text: gather-sum (+ task row) then LayerNorm (vilbert.py:346-367). Packed: the sums of the padded rows (cheap), their valid
+        # rows gathered, and the LayerNorm on those
+        xe = xe_pad = self.buf((Bt * Nt, Ht), F32)
         e = "bert.embeddings"
         self.emit(lib.vb_embed_text_fwd, self.in_ids.data_ptr(), self.in_tt.data_ptr(), self._ptr(self.in_task), ps.p(e + ".word_embeddings.weight").data_ptr(),
                   ps.p(e + ".position_embeddings.weight").data_ptr(), ps.p(e + ".token_type_embeddings.weight").data_ptr(),
                   ps.p(e + ".task_embeddings.weight").data_ptr() if self.has_task else None, xe.data_ptr(), Bt, self.Nt_in, Ht)
-        tdrop = self.drop(e + ".dropout", c.hidden_dropout_prob)
+        if self.packed:
+            xe = self.buf((Mt, Ht), F32)
+            self.emit(lib.vb_pack_rows_f32, xe_pad.data_ptr(), xe.data_ptr(), self.map_t.data_ptr(), Mt, Ht)
+        tdrop = self.drop(e + ".dropout", c.hidden_dropout_prob, "t")
         t32, top, tmean, trstd = self.ln_fwd(xe, ps.p(e + ".LayerNorm.weight"), ps.p(e + ".LayerNorm.bias"), Mt, Ht, out_drop=tdrop)
         tables = [e + n for n in (".word_embeddings.weight", ".position_embeddings.weight", ".token_type_embeddings.weight")]
         tables.append(e + ".task_embeddings.weight" if self.has_task else None)
@@ -1185,6 +1269,11 @@ class Plan:
                 dxe = self.scratch("emb.dxe", (Mt, Ht), F32)
                 self.ln_bwd(t.g32, xe, ps.p(e + ".LayerNorm.weight"), tmean, trstd, dxe, None, Mt, Ht, self.pg(e + ".LayerNorm.weight"),
                             self.pg(e + ".LayerNorm.bias"), out_drop=tdrop)
+                if self.packed:     # back to the padded rows the embedding sums were gathered from (zeros on the masked ones)
+                    dxe_pad = self.scratch("emb.dxe_pad", (B * Nt, Ht), F32)
+                    self.emit(lib.vb_unpack_rows_f32, dxe.data_ptr(), dxe_pad.data_ptr(), self.seg["t"][0].data_ptr(), self.seg["t"][1].data_ptr(),
+                              B, Nt, Ht, 0.0)
+                    dxe = dxe_pad
                 gt = [None if n is None else self.pg(n) for n in tables]
                 if any(g is not None for g in gt):
                     self.emit(lib.vb_embed_text_bwd, dxe.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), self._ptr(self.in_task),
@@ -1198,7 +1287,7 @@ class Plan:
             self.cur = self.prefix
         with self.on(0 if self.image_prefix else 1):
             yv, feat = self.image_embedding(ve, Hv)
-            vdrop = self.drop(ve + ".dropout", c.hidden_dropout_prob)     # BertImageEmbeddings uses hidden_dropout_prob (vilbert.py:1419)
+            vdrop = self.drop(ve + ".dropout", c.hidden_dropout_prob, "v")     # BertImageEmbeddings uses hidden_dropout_prob (vilbert.py:1419)
             self._private = self.image_prefix
             v32, vop, vmean, vrstd = self.ln_fwd(yv, ps.p(ve + ".LayerNorm.weight"), ps.p(ve + ".LayerNorm.bias"), Mv, Hv, out_drop=vdrop)
             self._private = False
@@ -1224,12 +1313,18 @@ class Plan:
         [regions, H], the feature Operand)."""
         ps, lib = self.ps, self.lib
         B, Nv, Fv = self.in_feat.shape
-        M = B * Nv
+        M = self.packed[1] if self.packed else B * Nv
         feat = self.buf16((M, Fv))
         hi, lo, bw = feat.ptrs()
-        self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), hi, M * Fv, feat.fp16, lo, bw)
+        self.loc_rows = self.in_loc
+        if self.packed:     # the valid regions' features cast straight into packed operand rows, and their boxes
+            self.emit(lib.vb_pack_regions, self.in_feat.data_ptr(), self.map_v.data_ptr(), M, Fv, feat.fp16, hi, lo, bw)
+            self.loc_rows = self.buf((M, 5), F32)
+            self.emit(lib.vb_pack_rows_f32, self.in_loc.data_ptr(), self.loc_rows.data_ptr(), self.map_v.data_ptr(), M, 5)
+        else:
+            self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), hi, M * Fv, feat.fp16, lo, bw)
         locp = self.buf((M, H), F32)
-        self.emit(lib.vb_loc_proj_fwd, self.in_loc.data_ptr(), ps.p(prefix + ".image_location_embeddings.weight").data_ptr(),
+        self.emit(lib.vb_loc_proj_fwd, self.loc_rows.data_ptr(), ps.p(prefix + ".image_location_embeddings.weight").data_ptr(),
                   ps.p(prefix + ".image_location_embeddings.bias").data_ptr(), locp.data_ptr(), M, H)
         y = self.buf((M, H), F32)
         self.gemm(M, H, Fv, feat, Fv, ps.w(prefix + ".image_embeddings.weight"), Fv, bias=ps.p(prefix + ".image_embeddings.bias"),
@@ -1247,7 +1342,7 @@ class Plan:
         if dy32 is not None:
             gw, gb = self.pg(prefix + ".image_location_embeddings.weight"), self.pg(prefix + ".image_location_embeddings.bias")
             if gw is not None or gb is not None:
-                self.emit(self.lib.vb_loc_proj_bwd, dy32.data_ptr(), self.in_loc.data_ptr(), self._ptr(gw), self._ptr(gb), M, H)
+                self.emit(self.lib.vb_loc_proj_bwd, dy32.data_ptr(), self.loc_rows.data_ptr(), self._ptr(gw), self._ptr(gb), M, H)
         if dy16 is not None and "input_imgs" in self.input_grads:
             g = self.input_grad["input_imgs"] = self.buf((M, Fv), F32, zero=True)
             self.gemm(M, Fv, H, dy16, H, ps.w(prefix + ".image_embeddings.weight").bw, Fv, b_mn=1, out_f32=g, ld_of=Fv)
@@ -1261,7 +1356,11 @@ class Plan:
         ps, B, H, Hb = self.ps, self.B, seq.H, self.cfg.bi_hidden_size
         p32 = self.buf((B, Hb), F32)
         p = self.buf16((B, Hb), bw=False)
-        self.gemm(B, Hb, H, seq.op, N * H, ps.w(wname + ".weight"), H, bias=ps.p(wname + ".bias"), act=L.VB_ACT_RELU, out_f32=p32, ld_of=Hb,
+        x, ldx = seq.op, N * H
+        if self.packed:      # each sample's first row, through the stream's offsets
+            first = self.seg["t" if wname == "bert.t_pooler.dense" else "v"][0][:B]
+            x, ldx = self.gather_rows(seq.op, first, B, H), H
+        self.gemm(B, Hb, H, x, ldx, ps.w(wname + ".weight"), H, bias=ps.p(wname + ".bias"), act=L.VB_ACT_RELU, out_f32=p32, ld_of=Hb,
                   out_bf16=p, ld_ob=Hb)
         pooled = self.act(p32, p, B, Hb, inputs=(seq,), params=(wname,))
 
@@ -1271,18 +1370,23 @@ class Plan:
             dpre = self.scratch("pool.dpre", (B, Hb), BF16)
             dpre32 = self.scratch("pool.dpre32", (B, Hb), F32)
             self.emit(self.lib.vb_relu_bwd, pooled.g32.data_ptr(), p32.data_ptr(), dpre.data_ptr(), dpre32.data_ptr(), B * Hb)
-            self.linear_wgrad(dpre, Hb, seq.op.bw, N * H, B, Hb, H, wname, bias_from=(dpre32, Hb))
-            self.pooler_dgrad(seq, N, dpre, wname)
+            self.linear_wgrad(dpre, Hb, x.bw, ldx, B, Hb, H, wname, bias_from=(dpre32, Hb))
+            self.pooler_dgrad(seq, N, dpre, wname, first if self.packed else None)
         self.push_bwd(bwd, pooled.rg)
         return pooled
 
-    def pooler_dgrad(self, seq, N, dpre, wname):
-        """Backward of a pooler's Linear into its input: rows b*N (token 0 of every sample) of the sequence gradient += dpre @ W,
-        with the sequence gradient zeroed on its first write."""
+    def pooler_dgrad(self, seq, N, dpre, wname, rows=None):
+        """Backward of a pooler's Linear into its input: rows b*N (token 0 of every sample; packed: the rows `rows`) of the sequence
+        gradient += dpre @ W, with the sequence gradient zeroed on its first write."""
         if not seq.rg:
             return
         g = self.grad_zeroed(seq)
         B, K = dpre.shape
+        if rows is not None:
+            d = self.scratch("pool.dx", (B, seq.H), F32)
+            self.gemm(B, seq.H, K, dpre, K, self.ps.w(wname + ".weight").bw, seq.H, b_mn=1, out_f32=d, ld_of=seq.H)
+            self.emit(self.lib.vb_scatter_add_rows_f32, d.data_ptr(), g.data_ptr(), rows.data_ptr(), B, seq.H)
+            return
         self.gemm(B, seq.H, K, dpre, K, self.ps.w(wname + ".weight").bw, seq.H, b_mn=1, residual=g, ld_res=N * seq.H, out_f32=g,
                   ld_of=N * seq.H)
 
@@ -1431,6 +1535,31 @@ class Plan:
                       self._ptr(self.pg(wname + ".weight")), self._ptr(self.pg(wname + ".bias")), M, K, N_out, self._ref(in_drop))
         self.push_bwd(bwd, self.out_rg[name])
 
+    def packed_vision_logit(self, seq_v, in_drop):
+        """vision_logit of a packed plan: the Linear on the packed region rows, scattered to the padded [B * Nv, 1] layout with
+        PACKED_MASKED_LOGIT on the masked regions, so the objective, score and results read it as in the padded plan. The backward
+        gathers the padded gradient back to the packed rows."""
+        ps, lib, B, Nv, name = self.ps, self.lib, self.B, self.Nv, "vision_logit"
+        M, K = seq_v.M, seq_v.H
+        off, ln = self.seg["v"]
+        y = self.buf((M, 1), F32)
+        self.emit(lib.vb_small_linear_fwd, seq_v.f32.data_ptr(), K, ps.p(name + ".weight").data_ptr(), ps.p(name + ".bias").data_ptr(), None,
+                  y.data_ptr(), M, K, 1, self._ref(in_drop))
+        out = self.buf((B * Nv, 1), F32)
+        self.emit(lib.vb_unpack_rows_f32, y.data_ptr(), out.data_ptr(), off.data_ptr(), ln.data_ptr(), B, Nv, 1, PACKED_MASKED_LOGIT)
+        self.outputs[name] = out
+        self.out_rg[name] = seq_v.rg or self.trainable(name)
+
+        def bwd():
+            if name not in self.grad_outputs:
+                return
+            dy = self.scratch("vlogit.dy", (M, 1), F32)
+            self.emit(lib.vb_pack_rows_f32, self.out_grad_buffer(name, (B * Nv, 1)).data_ptr(), dy.data_ptr(), self.map_v.data_ptr(), M, 1)
+            g, acc = self.grad_acc(seq_v) if seq_v.rg else (None, 0)
+            self.emit(lib.vb_small_linear_bwd, dy.data_ptr(), seq_v.f32.data_ptr(), K, ps.p(name + ".weight").data_ptr(), self._ptr(g), K, acc,
+                      self._ptr(self.pg(name + ".weight")), self._ptr(self.pg(name + ".bias")), M, K, 1, self._ref(in_drop))
+        self.push_bwd(bwd, self.out_rg[name])
+
     def build_heads(self, seq_t, seq_v, pooled_t, pooled_v):
         """VILBertForVLTasks.forward after self.bert (vilbert.py:1673-1708) + BertPreTrainingHeads (:1228-1243).
         Dropout layers are identity (eval-mode / p = 0 parity protocol)."""
@@ -1529,7 +1658,9 @@ class Plan:
             self.small_head("vil_logit", fused, "vil_logit", 1)
         if want("vil_tri_prediction"):
             self.small_head("vil_tri_prediction", fused, "vil_tri_prediction", 3)
-        if want("vision_logit"):
+        if want("vision_logit") and self.packed:
+            self.packed_vision_logit(seq_v, self.drop("dropout.seq_v", self.head_dropout_prob, "v"))
+        elif want("vision_logit"):
             self.small_head("vision_logit", seq_v, "vision_logit", 1, addend=self.mask_v,
                             in_drop=self.drop("dropout.seq_v", self.head_dropout_prob))
         if want("linguisic_logit"):
@@ -1584,8 +1715,9 @@ class Plan:
         self.seq_t, self.seq_v = t, v
         self.pooled_t = self.pooler(t, self.Nt, "bert.t_pooler.dense")
         self.pooled_v = self.pooler(v, self.Nv, "bert.v_pooler.dense")
-        self.outputs["sequence_output_t"] = t.f32.view(B, self.Nt, -1)
-        self.outputs["sequence_output_v"] = v.f32.view(B, self.Nv, -1)
+        # packed: the sequence outputs are the packed rows [rows, H] (map_t / map_v give their padded rows)
+        self.outputs["sequence_output_t"] = t.f32 if self.packed else t.f32.view(B, self.Nt, -1)
+        self.outputs["sequence_output_v"] = v.f32 if self.packed else v.f32.view(B, self.Nv, -1)
         self.outputs["pooled_output_t"] = self.pooled_t.f32
         self.outputs["pooled_output_v"] = self.pooled_v.f32
         for nm, act in (("sequence_output_t", t), ("sequence_output_v", v), ("pooled_output_t", self.pooled_t), ("pooled_output_v", self.pooled_v)):
@@ -2506,25 +2638,39 @@ class Engine:
         self.bwd_gemm_max_ctas = 0       # persistent CTAs of the backward GEMMs (0 = one per SM); data parallel: leave SMs to NCCL (DESIGN §4c)
         self.lm_compact = True           # fused pre-training objective: masked-LM decoder + CE on the labelled rows only (Plan.lm_head_compact)
         self.lm_capacity = 0.25          # ... with room for this fraction of the token rows (15 % are masked; more poisons the loss with NaN)
+        # task steps (vilbert_b200.tasks) on packed plans: the valid text tokens and image regions only (Plan(packed=...)), batches
+        # that cannot be packed run padded and are counted by reason in pack_fallbacks; plan_builds counts plans built per
+        # (B, Nt, Nv). A packed task holds one or two capacities (pack_capacity) per shape: the plan cache keeps room for them
+        self.pack_padding = False
+        self.pack_fallbacks = Counter()
+        self.plan_builds = Counter()
 
     def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
              loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-             input_grads=frozenset()):
+             input_grads=frozenset(), packed=None):
         """The cached plan of this shape and these options (Plan). vqa_loss=True is the round-1 spelling of loss="vqa"; frozen:
-        ParamStore entry names that take no gradient; input_grads: the inputs of INPUT_GRAD_NAMES the backward also differentiates."""
+        ParamStore entry names that take no gradient; input_grads: the inputs of INPUT_GRAD_NAMES the backward also differentiates;
+        packed: (rows_t, rows_v) of a packed plan."""
         frozen, input_grads = frozenset(frozen), frozenset(input_grads)
         loss = "vqa" if vqa_loss else loss
         pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
         key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward),
-               None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix), frozen, input_grads)
+               None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix), frozen, input_grads,
+               None if packed is None else tuple(packed))
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]
-        while len(self.plans) >= self.max_plans:   # evict the least recently used plan: its buffers go back to the allocator
+        # packed task steps add up to two capacities per task shape: a 12-task mix then holds ~36 plans in steady state
+        while len(self.plans) >= self.max_plans * (3 if self.pack_padding else 1):   # evict the least recently used plan
             self.plans.popitem(last=False)
+        if packed is not None and self.ps.base:
+            raise NotImplementedError("packed plans run the two-stream VILBertForVLTasks only")
+        extra = {} if packed is None else {"packed": packed}
         self.plans[key] = (BasePlan if self.ps.base else Plan)(
             self, B, Nt, Nv, grad_outputs, heads, train, loss=loss, choices=choices, score=score, loss_in_forward=loss_in_forward,
-            outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen, input_grads=input_grads)
+            outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen, input_grads=input_grads,
+            **extra)
+        self.plan_builds[(B, Nt, Nv)] += 1
         return self.plans[key]
 
     def enable_activation_arena(self, nbytes):

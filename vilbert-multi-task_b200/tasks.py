@@ -20,7 +20,7 @@ import torch
 import torch.nn as nn
 
 from .data import expand_batch
-from .engine import LOSS_HEADS, RESULT_MODES
+from .engine import LOSS_HEADS, MC_REGION_OFFSET, RESULT_MODES, pack_capacity
 from .modeling import _PlanCall, _PlanFn
 
 LossMap = {
@@ -83,10 +83,66 @@ def _unpack(task_id, batch):
     return features, spatials, image_mask, question, target, input_mask, segment_ids, mc_ids, co_attention_mask
 
 
+_PACK_REFUSED = ("in_batch_pairs", "fast_mode", "dynamic_attention", "visualization")
+
+
+def _prefix_lengths(mask):
+    """Valid length per row of a 0/1 mask [rows, N], or None when some row is not prefix-valid (a 0 before a 1) or has no 1."""
+    m = mask.ne(0)
+    n = m.sum(1)
+    ok = bool((n >= 1).all()) and bool(m.eq(torch.arange(m.size(1)).unsqueeze(0) < n.unsqueeze(1)).all())
+    return n if ok else None
+
+
+def packed_rows(model, task_cfg, task_id, batch, processes):
+    """The (rows_t, rows_v) capacities of a packed plan for this batch when model.engine.pack_padding is set and the batch can be
+    packed, else None. Decided from the host tensors before the batch moves, so it forces no sync. The masks are replicated as the
+    task's `process` replicates them. A batch can be packed when both masks are prefix-valid with at least one valid entry per row
+    ("mask"), no V-logit target is non-zero on a masked region ("target": the padded loss would read that region's logit and send
+    it a gradient) and no gathered V-logit-mc choice with a non-zero target sits on a masked region, nor do all of a sample's choices
+    (its argmax would then fall among masked logits, which the padded plan leaves at logit - 10000) ("choice"); otherwise it runs
+    padded and engine.pack_fallbacks counts the reason ("device": the masks are already on the device). Train mode packs too: the
+    packed plan draws the padded plan's dropout masks."""
+    eng = model.engine
+    if not eng.pack_padding:
+        return None
+    cfg = eng.cfg
+    bad = [f for f in _PACK_REFUSED if getattr(cfg, f, False)]
+    if bad:
+        raise NotImplementedError(f"engine.pack_padding does not support config.{bad[0]}")
+
+    def fallback(reason):
+        eng.pack_fallbacks[reason] += 1
+        return None
+
+    features, spatials, image_mask, question, target, input_mask, segment_ids, mc_ids, _ = _unpack(task_id, batch)
+    if any(t is not None and t.is_cuda for t in (image_mask, input_mask, target, mc_ids)):
+        return fallback("device")
+    process = task_cfg[task_id]["process"]
+    if process in processes:     # the masks as expand_batch lays them out (a one-wide stand-in for the features and boxes)
+        stand_in = image_mask.unsqueeze(-1)
+        _, _, image_mask, _, input_mask, _, _, _, _ = expand_batch(process, stand_in, stand_in, image_mask, question, input_mask, input_mask)
+    lt, lv = _prefix_lengths(input_mask), _prefix_lengths(image_mask)
+    if lt is None or lv is None:
+        return fallback("mask")
+    kind = task_kind(task_cfg, task_id)
+    if kind == "vlogit_bce" and target.numel() == image_mask.numel():
+        if bool((target.reshape(image_mask.shape).ne(0) & image_mask.eq(0)).any()):
+            return fallback("target")
+    if mc_ids is not None and kind == "vlogit_mc":
+        region = mc_ids.long() + MC_REGION_OFFSET
+        masked = region.ge(lv.unsqueeze(1))
+        if bool((target.reshape(mc_ids.shape).ne(0) & masked).any()) or bool(masked.all(1).any()):
+            return fallback("choice")
+    B, Nt, Nv = input_mask.size(0), input_mask.size(1) + (1 if cfg.task_specific_tokens else 0), image_mask.size(1)
+    rows_t = int(lt.sum()) + (B if cfg.task_specific_tokens else 0)
+    return pack_capacity(rows_t, B * Nt), pack_capacity(int(lv.sum()), B * Nv)
+
+
 class _Step:
     """One task batch on the device, reshaped for the model, with the plan of its objective and the call that runs it."""
 
-    def __init__(self, task_cfg, task_id, batch, model, train, grad, processes, evaluate=False):
+    def __init__(self, task_cfg, task_id, batch, model, train, grad, processes, evaluate=False, packed=None):
         eng = model.engine
         self.kind = kind = task_kind(task_cfg, task_id)
         features, spatials, image_mask, question, target, input_mask, segment_ids, mc_ids, _ = _unpack(task_id, batch)
@@ -114,10 +170,12 @@ class _Step:
             has_loss = kind not in ("vqa", "gqa")
             plan = eng.plan(B, Nt, Nv, train=train, loss=kind if has_loss else None, choices=choices,
                             score=has_loss and kind not in _NO_SCORE, loss_in_forward=has_loss, outputs=LOSS_HEADS[kind],
-                            results=kind if kind in RESULT_MODES else None)
+                            results=kind if kind in RESULT_MODES else None, packed=packed)
         else:
+            # a packed plan builds the objective's head only: the step returns nothing else, and a kept head is bitwise the same
             plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS[kind] if grad else (), train=train, loss=kind, choices=choices,
-                            score=kind not in _NO_SCORE, loss_in_forward=True, frozen=model._frozen())
+                            score=kind not in _NO_SCORE, loss_in_forward=True, frozen=model._frozen(),
+                            outputs=None if packed is None else LOSS_HEADS[kind], packed=packed)
         inputs = dict(input_txt=question, input_imgs=features, image_loc=spatials, token_type_ids=segment_ids, attention_mask=input_mask,
                       image_attention_mask=image_mask, task_ids=task_tokens)
         targets = {}
@@ -154,10 +212,12 @@ def ForwardModelsTrain(args, task_cfg, device, task_id, task_count, task_iter_tr
         task_iter_train[task_id] = iter(task_dataloader_train[task_id])
     task_count[task_id] += 1
     batch = next(task_iter_train[task_id])
-    batch = tuple(t.cuda(device=device, non_blocking=True) for t in batch)
     m = _model(model)
+    processes = ("dialog", "expand", "retrieval", "nlvr")
+    packed = packed_rows(m, task_cfg, task_id, batch, processes)
+    batch = tuple(t.cuda(device=device, non_blocking=True) for t in batch)
     _check_loss(task_cfg, task_id, task_losses)
-    step = _Step(task_cfg, task_id, batch, m, bool(m.training), True, ("dialog", "expand", "retrieval", "nlvr"))
+    step = _Step(task_cfg, task_id, batch, m, bool(m.training), True, processes, packed=packed)
     loss, = _PlanFn.apply(m._anchor, step.call)
     step.score_error()
     score = step.plan.score.reshape(()) / float(step.batch_size)
@@ -167,11 +227,13 @@ def ForwardModelsTrain(args, task_cfg, device, task_id, task_count, task_iter_tr
 def ForwardModelsVal(args, task_cfg, device, task_id, batch, model, task_losses):
     """task_utils.py:31-164: (float(loss), float(batch_score), batch_size) from a forward-only plan in the model's current mode,
     with one device-to-host copy of (loss, score). The reference's validation step has no `dialog` reshape; neither has this one."""
-    batch = tuple(t.cuda(device=device, non_blocking=True) for t in batch)
     m = _model(model)
+    processes = ("expand", "retrieval", "nlvr")
+    packed = packed_rows(m, task_cfg, task_id, batch, processes)
+    batch = tuple(t.cuda(device=device, non_blocking=True) for t in batch)
     _check_loss(task_cfg, task_id, task_losses)
     with torch.no_grad():
-        step = _Step(task_cfg, task_id, batch, m, bool(m.training), False, ("expand", "retrieval", "nlvr"))
+        step = _Step(task_cfg, task_id, batch, m, bool(m.training), False, processes, packed=packed)
         step.call.forward()
         step.score_error()
         loss, score = step.plan.objective_out.tolist()
@@ -194,12 +256,14 @@ def EvaluatingModel(args, task_cfg, device, task_id, batch, model, task_dataload
         raise NotImplementedError(f"{task_id}: EvaluatingModel has no result for task type {task_cfg[task_id]['type']!r} with loss "
                                   f"{task_cfg[task_id]['loss']!r}")
     question_id = batch[-1].tolist()
-    batch = tuple(t.cuda(device=device, non_blocking=True) for t in batch)
     m = _model(model)
+    processes = ("dialog", "expand", "retrieval", "nlvr")
+    packed = packed_rows(m, task_cfg, task_id, batch, processes)
+    batch = tuple(t.cuda(device=device, non_blocking=True) for t in batch)
     if kind not in ("vqa", "gqa"):            # VL-classifier / GQA do not read task_losses
         _check_loss(task_cfg, task_id, task_losses)
     with torch.no_grad():
-        step = _Step(task_cfg, task_id, batch, m, bool(m.training), False, ("dialog", "expand", "retrieval", "nlvr"), evaluate=True)
+        step = _Step(task_cfg, task_id, batch, m, bool(m.training), False, processes, evaluate=True, packed=packed)
         step.score_error()
         step.call.forward()
         plan = step.plan
@@ -226,4 +290,4 @@ def EvaluatingModel(args, task_cfg, device, task_id, batch, model, task_dataload
     return loss, score, step.batch_size, results, others
 
 
-__all__ = ["EvaluatingModel", "ForwardModelsTrain", "ForwardModelsVal", "LoadLosses", "TASK_KINDS", "task_kind"]
+__all__ = ["EvaluatingModel", "ForwardModelsTrain", "ForwardModelsVal", "LoadLosses", "TASK_KINDS", "packed_rows", "task_kind"]
