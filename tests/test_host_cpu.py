@@ -207,6 +207,30 @@ def test_plan_rejects_operands_in_the_wrong_format(golden_dir):
     assert plan.bwd[-1][0].__name__ == "vb_gemm_bf16"
 
 
+def test_emit_checks_launch_arguments_while_the_plan_is_built(golden_dir):
+    """Plan.emit makes C values of its arguments (a tensor its data pointer, a dropout descriptor a reference to it) and refuses,
+    while the plan is built, a launch whose argument count does not match its prototype and an argument with no C form, such as
+    an Operand passed whole where one of its pointers belongs. ctypes would only refuse them when the launch first runs."""
+    from vilbert_b200.engine import Operand
+    cfgj = json.load(open(os.path.join(golden_dir, "tiny_b4.json")))["config"]
+    plan = Engine(BertConfig.from_dict(cfgj), "cpu", _build_only=True).plan(4, 9, 11)
+    axpy = plan.lib.vb_axpy_f32
+    x, y, h = torch.zeros(8), torch.zeros(8), torch.zeros(8, dtype=torch.float16)
+    n = len(plan.fwd)
+    with pytest.raises(TypeError, match="vb_axpy_f32 takes 4"):
+        plan.emit(axpy, x, y, 8)                                    # one short
+    with pytest.raises(TypeError, match="vb_axpy_f32 takes 4"):
+        plan.emit(axpy, x, y, 8, 1.0, None)                         # a stream: the plan passes the one the op runs on
+    with pytest.raises(TypeError, match="Operand"):
+        plan.emit(plan.lib.vb_gather_rows16, Operand(h), h, None, None, x, 8, 1)
+    assert len(plan.fwd) == n
+    plan.emit(axpy, x, y, 8, 1.0)
+    assert plan.fwd[-1][1] == (x.data_ptr(), y.data_ptr(), 8, 1.0)
+    d = L.Dropout()
+    plan.emit(plan.lib.vb_fuse_pooled_bwd, x, x, y, None, y, 8, 1, d)
+    assert plan.fwd[-1][1][3] is None and plan.fwd[-1][1][-1]._obj is d
+
+
 def test_shared_activation_arena_layout(golden_dir):
     """Engine.enable_activation_arena: activation / scratch buffers of every plan are sub-allocated from one arena (plans overlay
     each other), while everything loaded or initialised outside a run (inputs, targets, output gradients) stays private."""

@@ -123,6 +123,24 @@ def input_grad_cases(O, E, base_labels):
     ]
 
 
+def packed_cases(E):
+    """Packed task steps (packed=(rows_t, rows_v)) building heads of PACKED_HEADS only: a train-mode VQA step, a V-logit evaluation
+    step with its results, a VL-logit step over two options and a train-mode V-logit step with the text stream frozen (frozen= as
+    entry-name prefixes). Listed after every case above, so that the listing of a tree without them is a prefix of this one."""
+    rows = (24, 32)
+
+    def step(kind, **kw):
+        return dict(grad_outputs=E.LOSS_HEADS[kind], loss=kind, train=True, score=True, loss_in_forward=True, outputs=E.LOSS_HEADS[kind],
+                    packed=rows, **kw)
+    return [
+        ("packed_task_vqa", {}, "vl", 4, step("vqa")),
+        ("packed_eval_vlogit_bce", {}, "vl", 4, dict(loss="vlogit_bce", score=True, loss_in_forward=True, outputs=("vision_logit",),
+                                                     results="vlogit_bce", packed=rows)),
+        ("packed_task_logit_ce", {}, "vl", 4, step("logit_ce", choices=2)),
+        ("packed_task_vlogit_bce_frozen_text", {}, "vl", 4, step("vlogit_bce", frozen=("bert.embeddings.", "bert.encoder.layer."))),
+    ]
+
+
 def dump_cases(out, case_list, prec, Engine, BertConfig, tiny, tiny_base):
     """Lists every plan of `case_list` in precision `prec`, without and with the shared activation arena. -> (plans, op records)"""
     n_plans = n_ops = 0
@@ -134,7 +152,11 @@ def dump_cases(out, case_list, prec, Engine, BertConfig, tiny, tiny_base):
             eng = Engine(BertConfig.from_dict(cfg), "cpu", heads=heads, _build_only=True, precision=prec, **engine_kw)
             if arena:
                 eng.enable_activation_arena(ARENA_BYTES)
-            plan_kw = dict(kw, frozen=frozenset(eng.ps.entries)) if kw.get("frozen") == "all" else kw
+            frozen = kw.get("frozen")
+            if frozen == "all" or isinstance(frozen, tuple):     # every entry, or the entries under these name prefixes
+                plan_kw = dict(kw, frozen=frozenset(n for n in eng.ps.entries if frozen == "all" or n.startswith(frozen)))
+            else:
+                plan_kw = kw
             try:
                 plan = eng.plan(B, NT, nv, **plan_kw)
             except (TypeError, ValueError) as ex:
@@ -257,6 +279,11 @@ def main():
     if hasattr(E, "INPUT_GRAD_NAMES"):
         for prec in PRECISIONS:
             p, o = dump_cases(out, input_grad_cases(O, E, tiny_base["num_labels"]), prec, Engine, BertConfig, tiny, tiny_base)
+            n_plans, n_ops = n_plans + p, n_ops + o
+    # packed task steps: listed last, so that the listing of a tree without them is a prefix of this one
+    if hasattr(E, "PACKED_HEADS"):
+        for prec in PRECISIONS:
+            p, o = dump_cases(out, packed_cases(E), prec, Engine, BertConfig, tiny, tiny_base)
             n_plans, n_ops = n_plans + p, n_ops + o
     text = "\n".join(out) + "\n"
     if a.out:

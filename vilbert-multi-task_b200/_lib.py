@@ -6,6 +6,8 @@ returns a non-zero status this module raises — nothing here ever routes to a C
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvilbert_b200.so")
 
@@ -178,6 +180,37 @@ def check(status, what=""):
     if status != 0:
         msg = lib().vb_last_error().decode("utf-8", "replace")
         raise VBError(f"{what or 'libvilbert_b200'} failed with status {status}: {msg}")
+
+
+_BYREF = type(C.byref(C.c_int()))
+
+
+def arg(v):
+    """The C value of one launch argument: a tensor's data pointer, a descriptor struct (Dropout, GemmArgs, ...) by reference.
+    None, Python and ctypes scalars and byref objects are C values already. Anything else (an Operand passed whole where one of
+    its pointers belongs) raises TypeError, so a wrong value fails when the launch is built, not when it first runs."""
+    if v is None or isinstance(v, (int, float, C._SimpleCData, _BYREF)):
+        return v
+    if isinstance(v, torch.Tensor):
+        return v.data_ptr()
+    if isinstance(v, C.Structure):
+        return C.byref(v)
+    raise TypeError(f"{type(v).__name__} is not a C launch argument")
+
+
+def launch_args(fn, *values):
+    """The C arguments of one launch of the entry point `fn` without its trailing stream, each converted by arg(). Their count
+    is checked against fn's prototype here: ctypes would check it only when the launch first runs."""
+    if len(values) != len(fn.argtypes) - 1:
+        raise TypeError(f"{fn.__name__} takes {len(fn.argtypes) - 1} arguments before the stream, got {len(values)}")
+    return tuple(arg(v) for v in values)
+
+
+def call(fn, *values, stream=None):
+    """One launch of `fn` on `stream` (default: the current stream), outside a plan; raises VBError on a non-zero status."""
+    if stream is None:
+        stream = torch.cuda.current_stream().cuda_stream
+    check(fn(*launch_args(fn, *values), stream), fn.__name__)
 
 
 def exported_symbols():

@@ -22,7 +22,7 @@ def repeat_rows(x, repeats):
     if not x.is_cuda or item_bytes % 16 or x.data_ptr() % 16:
         return x.unsqueeze(1).expand(x.shape[0], repeats, *x.shape[1:]).reshape(x.shape[0] * repeats, *x.shape[1:])
     out = torch.empty((x.shape[0] * repeats,) + tuple(x.shape[1:]), dtype=x.dtype, device=x.device)
-    L.check(L.lib().vb_repeat_rows(x.data_ptr(), out.data_ptr(), item_bytes, x.shape[0], repeats, torch.cuda.current_stream().cuda_stream), "vb_repeat_rows")
+    L.call(L.lib().vb_repeat_rows, x, out, item_bytes, x.shape[0], repeats)
     return out
 
 

@@ -20,7 +20,6 @@ activations and weights exist only as tensor-core operands. Three operand precis
                     runs as three tensor-core passes (hi.hi + lo.hi + hi.lo), ~fp32 accuracy (north_star 1e-3);
   "bf16"            every operand bf16 (round-1 arithmetic; kept for A/B measurements).
 """
-import ctypes as C
 import math
 import zlib
 from collections import Counter, OrderedDict, namedtuple
@@ -297,10 +296,10 @@ class ParamStore:
         hi, lo, bw = self.shadows.ptrs(off)
         return (self.flat.data_ptr() + 4 * off, hi, n, self.shadows.fp16, lo, bw)
 
-    def refresh_shadow(self, stream):
-        """16-bit operand copy (hi, and lo in split precision) of every parameter in one launch (belongs with the
-        optimizer step in training)."""
-        L.check(L.lib().vb_cast_f32_to_bf16(*self.cast_args(0, self.numel), stream), "vb_cast_f32_to_bf16")
+    def refresh_shadow(self):
+        """16-bit operand copy (hi, and lo in split precision) of every parameter in one launch on the current stream (belongs
+        with the optimizer step in training)."""
+        L.call(L.lib().vb_cast_f32_to_bf16, *self.cast_args(0, self.numel))
 
 
 # ------------------------------------------------------------------------------------------ plan
@@ -662,7 +661,9 @@ class Plan:
         return self._scratch[key]
 
     def emit(self, fn, *args):
-        self.cur.append((fn, args, self.sid if self.two_streams else 0))
+        """Appends a launch of `fn` to the pass being built. Tensors, None and descriptor structs are passed as they are: the
+        arguments become C values here (_lib.launch_args), which also checks their count against fn's prototype."""
+        self.cur.append((fn, L.launch_args(fn, *args), self.sid if self.two_streams else 0))
 
     def sync_streams(self, mirror=True):
         """Both streams wait for each other here. Between two connection layers the text and the vision segments are
@@ -696,28 +697,18 @@ class Plan:
         if rg:
             self._bwd_emitters.append((self.sid, fn))
 
-    @staticmethod
-    def _ptr(t):
-        if t is None:
-            return None
-        return t.data_ptr() if torch.is_tensor(t) else int(t)
-
     def drop(self, name, p, rows=None):
-        """ctypes byref of a vb_dropout for the dropout layer `name` with probability p, or None when inactive. rows: the stream
+        """The vb_dropout descriptor of the dropout layer `name` with probability p, or None when inactive. rows: the stream
         ("t" / "v") of a row-indexed site; a packed plan gives it the stream's packed-row -> padded-row map, so its rows draw the
         masks of the padded rows they hold."""
         if not self.train or p is None or p <= 0.0:
             return None
         d = L.Dropout()
-        d.step, d.site, d.p = self.e.drop_step.data_ptr(), dropout_site_id(name), float(p)
+        d.step, d.site, d.p = L.arg(self.e.drop_step), dropout_site_id(name), float(p)
         if self.packed and rows is not None:
-            d.row_map = (self.map_t if rows == "t" else self.map_v).data_ptr()
+            d.row_map = L.arg(self.map_t if rows == "t" else self.map_v)
         self._keep.append(d)
         return d
-
-    @staticmethod
-    def _ref(d):
-        return C.byref(d) if d is not None else None
 
     def _check_operands(self, fwd_ops, bwd_ops):
         """The kernels are told a format flag, not typed pointers: a buffer of the other format would be read as its bits.
@@ -739,29 +730,29 @@ class Plan:
         if fwd:
             self._check_operands((A, B, out_bf16), ())
             g.a_fp16 = g.b_fp16 = g.out_fp16 = A.fp16
-            g.A_lo, g.B_lo = self._ptr(A.lo), self._ptr(B.lo)
+            g.A_lo, g.B_lo = L.arg(A.lo), L.arg(B.lo)
             if out_bf16 is not None:
-                g.out_lo, g.out_b16, out_bf16 = self._ptr(out_bf16.lo), self._ptr(out_bf16.extra_bw), out_bf16.hi
+                g.out_lo, g.out_b16, out_bf16 = L.arg(out_bf16.lo), L.arg(out_bf16.extra_bw), out_bf16.hi
             A, B = A.hi, B.hi
         else:
             self._check_operands((), (A, B, out_bf16))      # the format flags stay 0 (bf16)
         g.M, g.N, g.K = M, N, K
-        g.A, g.lda, g.a_mn_major = self._ptr(A), lda, a_mn
-        g.B, g.ldb, g.b_mn_major = self._ptr(B), ldb, b_mn
+        g.A, g.lda, g.a_mn_major = L.arg(A), lda, a_mn
+        g.B, g.ldb, g.b_mn_major = L.arg(B), ldb, b_mn
         g.alpha = alpha
-        g.bias = self._ptr(bias)
-        g.residual, g.ld_res = self._ptr(residual), ld_res
-        g.aux, g.ld_aux = self._ptr(aux), ld_aux
+        g.bias = L.arg(bias)
+        g.residual, g.ld_res = L.arg(residual), ld_res
+        g.aux, g.ld_aux = L.arg(aux), ld_aux
         g.act = act
-        g.out_f32, g.ld_out_f32 = self._ptr(out_f32), ld_of
-        g.out_bf16, g.ld_out_bf16 = self._ptr(out_bf16), ld_ob
-        g.out_pre, g.ld_out_pre = self._ptr(out_pre), ld_op
+        g.out_f32, g.ld_out_f32 = L.arg(out_f32), ld_of
+        g.out_bf16, g.ld_out_bf16 = L.arg(out_bf16), ld_ob
+        g.out_pre, g.ld_out_pre = L.arg(out_pre), ld_op
         g.atomic_out, g.split_k, g.block_n, g.max_ctas = atomic, split_k, 0, (0 if fwd else self.e.bwd_gemm_max_ctas)
-        g.out_colsum = self._ptr(out_colsum)
+        g.out_colsum = L.arg(out_colsum)
         if dropout is not None:
             g.dropout = dropout
         self._keep.append(g)
-        self.emit(self.lib.vb_gemm_bf16, C.byref(g))
+        self.emit(self.lib.vb_gemm_bf16, g)
 
     def attention(self, bwd, B, H, Nq, Nk, D, Q, ldq, K, ldk, V, ldv, mask, O, ldo, lse, dO=None, lddo=0, dQ=None, lddq=0,
                   dK=None, lddk=0, dV=None, lddv=0, delta=None, dbq=None, dbk=None, dbv=None, dropout=None, segs=None):
@@ -770,27 +761,27 @@ class Plan:
         self._check_operands((Q, K, V, O), (dO, dQ, dK, dV))
         a = L.AttnArgs()
         a.qkv_fp16 = Q.fp16
-        a.O_b16 = self._ptr(O.extra_bw)     # forward: written; backward: read for delta (consistent with the bf16 backward products)
+        a.O_b16 = L.arg(O.extra_bw)     # forward: written; backward: read for delta (consistent with the bf16 backward products)
         if not bwd:
-            a.Q_lo, a.K_lo, a.V_lo, a.O_lo = self._ptr(Q.lo), self._ptr(K.lo), self._ptr(V.lo), self._ptr(O.lo)
+            a.Q_lo, a.K_lo, a.V_lo, a.O_lo = L.arg(Q.lo), L.arg(K.lo), L.arg(V.lo), L.arg(O.lo)
         a.B, a.H, a.Nq, a.Nk, a.D = B, H, Nq, Nk, D
-        a.Q, a.ldq, a.K, a.ldk, a.V, a.ldv = self._ptr(Q.hi), ldq, self._ptr(K.hi), ldk, self._ptr(V.hi), ldv
-        a.mask, a.scale = self._ptr(mask), 1.0 / math.sqrt(D)
-        a.O, a.ldo, a.lse = self._ptr(O.hi), ldo, self._ptr(lse)
-        a.dO, a.lddo, a.dQ, a.lddq = self._ptr(dO), lddo, self._ptr(dQ), lddq
-        a.dK, a.lddk, a.dV, a.lddv, a.delta = self._ptr(dK), lddk, self._ptr(dV), lddv, self._ptr(delta)
-        a.dbias_q, a.dbias_k, a.dbias_v = self._ptr(dbq), self._ptr(dbk), self._ptr(dbv)
+        a.Q, a.ldq, a.K, a.ldk, a.V, a.ldv = L.arg(Q.hi), ldq, L.arg(K.hi), ldk, L.arg(V.hi), ldv
+        a.mask, a.scale = L.arg(mask), 1.0 / math.sqrt(D)
+        a.O, a.ldo, a.lse = L.arg(O.hi), ldo, L.arg(lse)
+        a.dO, a.lddo, a.dQ, a.lddq = L.arg(dO), lddo, L.arg(dQ), lddq
+        a.dK, a.lddk, a.dV, a.lddv, a.delta = L.arg(dK), lddk, L.arg(dV), lddv, L.arg(delta)
+        a.dbias_q, a.dbias_k, a.dbias_v = L.arg(dbq), L.arg(dbk), L.arg(dbv)
         if dropout is not None:
             a.dropout = dropout
         if segs is not None:
             (qo, ql), (ko, kl) = segs
-            a.q_off, a.q_len, a.k_off, a.k_len = qo.data_ptr(), ql.data_ptr(), ko.data_ptr(), kl.data_ptr()
+            a.q_off, a.q_len, a.k_off, a.k_len = L.arg(qo), L.arg(ql), L.arg(ko), L.arg(kl)
         self._keep.append(a)
-        self.emit(self.lib.vb_attention_bwd if bwd else self.lib.vb_attention_fwd, C.byref(a))
+        self.emit(self.lib.vb_attention_bwd if bwd else self.lib.vb_attention_fwd, a)
         if not bwd and self.viz:
             # config.visualization: the probabilities (fp32 [B, heads, Nq, Nk]) and views of the queries / keys the reference returns
             probs = self.buf((B, H, Nq, Nk), F32)
-            self.emit(self.lib.vb_attention_probs, C.byref(a), probs.data_ptr())
+            self.emit(self.lib.vb_attention_probs, a, probs)
             self._last_attn = dict(attn=probs, q=Q.hi, k=K.hi, B=B, H=H, Nq=Nq, Nk=Nk, D=D)
 
     def zero_tail(self, stream, *ts):
@@ -799,7 +790,7 @@ class Plan:
         gradient multiplies them by a zero gradient, which garbage would turn into NaN."""
         ts = [t for t in ts if t is not None]
         off = self.seg[stream][0]
-        self.emit(self.lib.vb_zero_tail_rows, *[self._ptr(t) for t in ts], *([None] * (3 - len(ts))), ts[0].stride(0) * ts[0].element_size(),
+        self.emit(self.lib.vb_zero_tail_rows, *ts, *([None] * (3 - len(ts))), ts[0].stride(0) * ts[0].element_size(),
                   ts[0].shape[1] * ts[0].element_size(), off.data_ptr() + 4 * self.B, ts[0].shape[0])
 
     def ln_fwd(self, x, gamma, beta, M, H, want_f32=True, out_drop=None, res=None, in_drop=None):
@@ -810,25 +801,22 @@ class Plan:
         mean, rstd = self.buf((M,), F32), self.buf((M,), F32)
         hi, lo, bw = y.ptrs()
         if res is not None:
-            self.emit(self.lib.vb_add_layernorm_fwd, x.data_ptr(), res.data_ptr(), H, self._ref(in_drop), x.data_ptr(),
-                      gamma.data_ptr(), beta.data_ptr(), 1e-12, self._ptr(y32), hi, H, mean.data_ptr(), rstd.data_ptr(), M, H, y.fp16, lo, bw)
+            self.emit(self.lib.vb_add_layernorm_fwd, x, res, H, in_drop, x, gamma, beta, 1e-12, y32, hi, H, mean, rstd, M, H, y.fp16, lo, bw)
         else:
-            self.emit(self.lib.vb_layernorm_fwd, x.data_ptr(), H, gamma.data_ptr(), beta.data_ptr(), 1e-12, self._ptr(y32), hi, H,
-                      mean.data_ptr(), rstd.data_ptr(), M, H, self._ref(out_drop), y.fp16, lo, bw)
+            self.emit(self.lib.vb_layernorm_fwd, x, H, gamma, beta, 1e-12, y32, hi, H, mean, rstd, M, H, out_drop, y.fp16, lo, bw)
         return y32, y, mean, rstd
 
     def ln_bwd(self, dy, x, gamma, mean, rstd, dx32, dx16, M, H, ggamma, gbeta, pre=None, gbias=None, out_drop=None, in_drop=None, dy2=None):
         """gbias: bias gradient of the Linear feeding this LayerNorm (column sums of dx), fused into the same pass. dy2: a second
         part of the output gradient (Act.g_add), added to dy as it is read."""
-        tail = (x.data_ptr(), H, gamma.data_ptr(), mean.data_ptr(), rstd.data_ptr(), self._ptr(dx32), self._ptr(dx16), H, self._ptr(pre), H,
-                self._ptr(ggamma), self._ptr(gbeta), self._ptr(gbias), M, H, self._ref(out_drop), self._ref(in_drop))
+        tail = (x, H, gamma, mean, rstd, dx32, dx16, H, pre, H, ggamma, gbeta, gbias, M, H, out_drop, in_drop)
         if dy2 is not None:
-            self.emit(self.lib.vb_add_layernorm_bwd, dy.data_ptr(), dy2.data_ptr(), H, *tail)
+            self.emit(self.lib.vb_add_layernorm_bwd, dy, dy2, H, *tail)
         else:
-            self.emit(self.lib.vb_layernorm_bwd, dy.data_ptr(), H, *tail)
+            self.emit(self.lib.vb_layernorm_bwd, dy, H, *tail)
 
     def colsum(self, X, ld, out, M, N):
-        self.emit(self.lib.vb_colsum, X.data_ptr(), 1 if X.dtype == BF16 else 0, ld, out.data_ptr(), M, N)
+        self.emit(self.lib.vb_colsum, X, 1 if X.dtype == BF16 else 0, ld, out, M, N)
 
     def grad_of(self, act):
         if act.g32 is None:
@@ -839,7 +827,7 @@ class Plan:
         """The gradient buffer of `act` for a backward op that adds to it: its first writer zeroes it first (rule 3 of Act)."""
         g = self.grad_of(act)
         if not act.gw:
-            self.emit(self.lib.vb_memset_zero, g.data_ptr(), g.numel() * 4)
+            self.emit(self.lib.vb_memset_zero, g, g.numel() * 4)
             act.gw = True
         self._fold_g_add(act)
         return g
@@ -855,7 +843,7 @@ class Plan:
     def _fold_g_add(self, act):
         """A later writer of g32 adds to it: the first writer's deferred part goes in first, so the sums keep their order."""
         if act.g_add is not None:
-            self.emit(self.lib.vb_axpy_f32, act.g_add.data_ptr(), act.g32.data_ptr(), act.M * act.H, 1.0)
+            self.emit(self.lib.vb_axpy_f32, act.g_add, act.g32, act.M * act.H, 1.0)
             act.g_add = None
 
     # dW, db of y = x W^T + b given dy (bf16 operand copy)
@@ -900,14 +888,14 @@ class Plan:
         if not acc and extra32 is not None and act.ln_reads:
             act.g_add, extra32 = extra32, None      # added by the LayerNorm backward that reads g32: the GEMM reads no residual
         if acc and extra32 is not None:
-            self.emit(self.lib.vb_axpy_f32, extra32.data_ptr(), g.data_ptr(), M * K_in, 1.0)
+            self.emit(self.lib.vb_axpy_f32, extra32, g, M * K_in, 1.0)
         self.gemm(M, K_in, N_out, dy16, ld_dy, W16, K_in, b_mn=1, residual=g if acc else extra32, ld_res=K_in, out_f32=g, ld_of=K_in)
 
     def add_grad(self, act, src32):
         if not act.rg:
             return
         g = self.grad_zeroed(act)
-        self.emit(self.lib.vb_axpy_f32, src32.data_ptr(), g.data_ptr(), g.numel(), 1.0)
+        self.emit(self.lib.vb_axpy_f32, src32, g, g.numel(), 1.0)
 
     # ------------------------------------------------------------------ blocks
     def dense_res_ln(self, a, K_in, res, wname, lnname, tag, drop=None, a_rg=True):
@@ -970,7 +958,7 @@ class Plan:
             Kp = pool.H
             z = self.buf((B, 2 * H), F32)
             self.gemm(B, 2 * H, Kp, pool.op, Kp, ps.w(prefix + ".self.dy.weight"), Kp, bias=ps.p(prefix + ".self.dy.bias"), out_f32=z, ld_of=2 * H)
-            self.emit(self.lib.vb_gate_scale_fwd, qkv.hi.data_ptr(), self._ptr(qkv.lo), 3 * H, z.data_ptr(), B, N, 2 * H, qkv.fp16)
+            self.emit(self.lib.vb_gate_scale_fwd, qkv.hi, qkv.lo, 3 * H, z, B, N, 2 * H, qkv.fp16)
         ctx = self.buf16((M, H))
         lse = self.buf((B, nh, N), F32)
         q, k, v = qkv.cols(0, H), qkv.cols(H, 2 * H), qkv.cols(2 * H, 3 * H)
@@ -1009,8 +997,7 @@ class Plan:
                 dyw_rg = self.trainable(prefix + ".self.dy.weight") or pool.rg
                 dz32 = self.scratch(tag + ".dz32", (B, 2 * H), F32) if self.trainable(prefix + ".self.dy.bias") else None
                 dz16 = self.scratch(tag + ".dz16", (B, 2 * H), BF16) if dyw_rg else None
-                self.emit(self.lib.vb_gate_scale_bwd, dqkv.data_ptr(), 3 * H, qkv.hi.data_ptr(), self._ptr(qkv.lo), 3 * H, z.data_ptr(), self._ptr(dz32),
-                          self._ptr(dz16), B, N, 2 * H, qkv.fp16)
+                self.emit(self.lib.vb_gate_scale_bwd, dqkv, 3 * H, qkv.hi, qkv.lo, 3 * H, z, dz32, dz16, B, N, 2 * H, qkv.fp16)
                 for (a, b) in self._runs((gq, gk)):      # the parts of one range are adjacent in the flat buffer
                     self.colsum(dqkv[:, a * H:b * H], 3 * H, (gq, gk)[a], M, (b - a) * H)
                 if dz32 is not None or dz16 is not None:
@@ -1124,14 +1111,14 @@ class Plan:
         op = self.buf16((B * M1, H), bw=False)      # FAST_MODE is inference only: no backward copy
         for src, dst in ((t.f32, f32), (t.op.hi, op.hi), (t.op.lo, op.lo)):
             if dst is not None:
-                self.emit(self.lib.vb_broadcast_rows, src.data_ptr(), dst.data_ptr(), M1 * H * dst.element_size(), B)
+                self.emit(self.lib.vb_broadcast_rows, src, dst, M1 * H * dst.element_size(), B)
         nt4 = (self.Nt * 4 + 15) // 16 * 16           # the mask row is padded to 16 bytes for the broadcast kernel
         if nt4 == self.Nt * 4:
             m = self.buf((B, self.Nt), F32)
-            self.emit(self.lib.vb_broadcast_rows, self.mask_t.data_ptr(), m.data_ptr(), self.Nt * 4, B)
+            self.emit(self.lib.vb_broadcast_rows, self.mask_t, m, self.Nt * 4, B)
         else:
             m = self.mask_t.new_empty((B, self.Nt)); self._keep.append(m)
-            self.emit(self.lib.vb_mask_to_additive, self.in_amask_b.data_ptr(), m.data_ptr(), B, self.Nt_in, 1 if self.has_task else 0)
+            self.emit(self.lib.vb_mask_to_additive, self.in_amask_b, m, B, self.Nt_in, 1 if self.has_task else 0)
         self.mask_t = m
         return self.act(f32, op, B * M1, H, inputs=(t,))
 
@@ -1150,9 +1137,9 @@ class Plan:
                 if dst is None:
                     continue
                 if is_text:
-                    self.emit(lib.vb_repeat_rows, src.data_ptr(), dst.data_ptr(), n * dst.element_size(), b, b)
+                    self.emit(lib.vb_repeat_rows, src, dst, n * dst.element_size(), b, b)
                 else:
-                    self.emit(lib.vb_broadcast_rows, src.data_ptr(), dst.data_ptr(), b * n * dst.element_size(), b)
+                    self.emit(lib.vb_broadcast_rows, src, dst, b * n * dst.element_size(), b)
             out = self.act(f32, op, b * b * N, act.H, inputs=(act,))
             outs.append(out)
 
@@ -1161,16 +1148,16 @@ class Plan:
                     return
                 g, acc = self.grad_acc(act)
                 if is_text:   # g[i] = sum_j out.g32[i * b + j]
-                    self.emit(lib.vb_sum_strided, out.g32.data_ptr(), g.data_ptr(), n, b, b * n, b, n, acc)
+                    self.emit(lib.vb_sum_strided, out.g32, g, n, b, b * n, b, n, acc)
                 else:         # g[j] = sum_i out.g32[i * b + j]
-                    self.emit(lib.vb_sum_strided, out.g32.data_ptr(), g.data_ptr(), n, b, n, b, b * n, acc)
+                    self.emit(lib.vb_sum_strided, out.g32, g, n, b, n, b, b * n, acc)
             self._bwd_emitters.append(None)
             self.push_bwd(bwd, out.rg)
             self._bwd_emitters.append(None)
         # masks: text mask rows repeated, image mask tiled (4-byte rows: plain torch-free kernels need 16-byte items -> host-side views)
         mt = self.buf((b * b, self.Nt), F32); mv = self.buf((b * b, self.Nv), F32)
-        self.emit(lib.vb_mask_to_additive, self.in_amask_pairs.data_ptr(), mt.data_ptr(), b * b, self.Nt_in, 1 if self.has_task else 0)
-        self.emit(lib.vb_mask_to_additive, self.in_imask_pairs.data_ptr(), mv.data_ptr(), b * b, self.Nv, 0)
+        self.emit(lib.vb_mask_to_additive, self.in_amask_pairs, mt, b * b, self.Nt_in, 1 if self.has_task else 0)
+        self.emit(lib.vb_mask_to_additive, self.in_imask_pairs, mv, b * b, self.Nv, 0)
         self.mask_t, self.mask_v = mt, mv
         self.sync_streams()
         return outs[0], outs[1]
@@ -1190,7 +1177,7 @@ class Plan:
         B, Ht, lib = self.B, t.H, self.lib
         p32 = self.buf((B, Ht), F32)
         p = self.buf16((B, Ht))
-        self.emit(lib.vb_masked_mean_fwd, t.f32.data_ptr(), self.mask_t.data_ptr(), p32.data_ptr(), *p.ptrs(), p.fp16, B, self.Nt, Ht)
+        self.emit(lib.vb_masked_mean_fwd, t.f32, self.mask_t, p32, *p.ptrs(), p.fp16, B, self.Nt, Ht)
         pool = self.act(p32, p, B, Ht, inputs=(t,))
         mask = self.mask_t
 
@@ -1198,7 +1185,7 @@ class Plan:
             if not pool.gw:
                 return
             g, acc = self.grad_acc(t)
-            self.emit(lib.vb_masked_mean_bwd, pool.g32.data_ptr(), mask.data_ptr(), g.data_ptr(), acc, B, self.Nt, Ht)
+            self.emit(lib.vb_masked_mean_bwd, pool.g32, mask, g, acc, B, self.Nt, Ht)
         self.push_bwd(bwd, pool.rg)
         return pool
 
@@ -1236,28 +1223,27 @@ class Plan:
             it = torch.int32
             self.seg = {"t": (self.buf((B + 1,), it), self.buf((B,), it)), "v": (self.buf((B + 1,), it), self.buf((B,), it))}
             self.map_t, self.map_v = self.buf((Mt,), it), self.buf((Mv,), it)
-            self.emit(lib.vb_pack_build, self.in_amask.data_ptr(), self.Nt_in, 1 if self.has_task else 0, self.in_imask.data_ptr(), Nv, B, Mt, Mv,
-                      self.seg["t"][0].data_ptr(), self.seg["t"][1].data_ptr(), self.map_t.data_ptr(), self.seg["v"][0].data_ptr(),
-                      self.seg["v"][1].data_ptr(), self.map_v.data_ptr())
+            self.emit(lib.vb_pack_build, self.in_amask, self.Nt_in, 1 if self.has_task else 0, self.in_imask, Nv, B, Mt, Mv, self.seg["t"][0],
+                      self.seg["t"][1], self.map_t, self.seg["v"][0], self.seg["v"][1], self.map_v)
         else:
             self.mask_t = self.buf((Bt, Nt), F32)
             self.mask_v = self.buf((B, Nv), F32, zero=self.image_prefix)
-            self.emit(lib.vb_mask_to_additive, self.in_amask.data_ptr(), self.mask_t.data_ptr(), Bt, self.Nt_in, 1 if self.has_task else 0)
+            self.emit(lib.vb_mask_to_additive, self.in_amask, self.mask_t, Bt, self.Nt_in, 1 if self.has_task else 0)
             if self.image_prefix:
                 self.cur = self.prefix
-            self.emit(lib.vb_mask_to_additive, self.in_imask.data_ptr(), self.mask_v.data_ptr(), B, Nv, 0)
+            self.emit(lib.vb_mask_to_additive, self.in_imask, self.mask_v, B, Nv, 0)
             self.cur = self.fwd
         self.sync_streams()
         # text: gather-sum (+ task row) then LayerNorm (vilbert.py:346-367). Packed: the sums of the padded rows (cheap), their valid
         # rows gathered, and the LayerNorm on those
         xe = xe_pad = self.buf((Bt * Nt, Ht), F32)
         e = "bert.embeddings"
-        self.emit(lib.vb_embed_text_fwd, self.in_ids.data_ptr(), self.in_tt.data_ptr(), self._ptr(self.in_task), ps.p(e + ".word_embeddings.weight").data_ptr(),
-                  ps.p(e + ".position_embeddings.weight").data_ptr(), ps.p(e + ".token_type_embeddings.weight").data_ptr(),
-                  ps.p(e + ".task_embeddings.weight").data_ptr() if self.has_task else None, xe.data_ptr(), Bt, self.Nt_in, Ht)
+        self.emit(lib.vb_embed_text_fwd, self.in_ids, self.in_tt, self.in_task, ps.p(e + ".word_embeddings.weight"),
+                  ps.p(e + ".position_embeddings.weight"), ps.p(e + ".token_type_embeddings.weight"),
+                  ps.p(e + ".task_embeddings.weight") if self.has_task else None, xe, Bt, self.Nt_in, Ht)
         if self.packed:
             xe = self.buf((Mt, Ht), F32)
-            self.emit(lib.vb_pack_rows_f32, xe_pad.data_ptr(), xe.data_ptr(), self.map_t.data_ptr(), Mt, Ht)
+            self.emit(lib.vb_pack_rows_f32, xe_pad, xe, self.map_t, Mt, Ht)
         tdrop = self.drop(e + ".dropout", c.hidden_dropout_prob, "t")
         t32, top, tmean, trstd = self.ln_fwd(xe, ps.p(e + ".LayerNorm.weight"), ps.p(e + ".LayerNorm.bias"), Mt, Ht, out_drop=tdrop)
         tables = [e + n for n in (".word_embeddings.weight", ".position_embeddings.weight", ".token_type_embeddings.weight")]
@@ -1271,13 +1257,11 @@ class Plan:
                             self.pg(e + ".LayerNorm.bias"), out_drop=tdrop)
                 if self.packed:     # back to the padded rows the embedding sums were gathered from (zeros on the masked ones)
                     dxe_pad = self.scratch("emb.dxe_pad", (B * Nt, Ht), F32)
-                    self.emit(lib.vb_unpack_rows_f32, dxe.data_ptr(), dxe_pad.data_ptr(), self.seg["t"][0].data_ptr(), self.seg["t"][1].data_ptr(),
-                              B, Nt, Ht, 0.0)
+                    self.emit(lib.vb_unpack_rows_f32, dxe, dxe_pad, self.seg["t"][0], self.seg["t"][1], B, Nt, Ht, 0.0)
                     dxe = dxe_pad
                 gt = [None if n is None else self.pg(n) for n in tables]
                 if any(g is not None for g in gt):
-                    self.emit(lib.vb_embed_text_bwd, dxe.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), self._ptr(self.in_task),
-                              *[self._ptr(g) for g in gt], B, self.Nt_in, Ht)
+                    self.emit(lib.vb_embed_text_bwd, dxe, self.in_ids, self.in_tt, self.in_task, *gt, B, self.Nt_in, Ht)
         self.push_bwd(bwd_text, t.rg)
         # image: region features fp32 -> bf16 ingest, 2048 -> Hv GEMM with the 5 -> Hv box projection as residual, LayerNorm (:1421-1432).
         # image_prefix: the same launches go to self.prefix on the main stream, and the LayerNorm's outputs (the image states the
@@ -1318,14 +1302,14 @@ class Plan:
         hi, lo, bw = feat.ptrs()
         self.loc_rows = self.in_loc
         if self.packed:     # the valid regions' features cast straight into packed operand rows, and their boxes
-            self.emit(lib.vb_pack_regions, self.in_feat.data_ptr(), self.map_v.data_ptr(), M, Fv, feat.fp16, hi, lo, bw)
+            self.emit(lib.vb_pack_regions, self.in_feat, self.map_v, M, Fv, feat.fp16, hi, lo, bw)
             self.loc_rows = self.buf((M, 5), F32)
-            self.emit(lib.vb_pack_rows_f32, self.in_loc.data_ptr(), self.loc_rows.data_ptr(), self.map_v.data_ptr(), M, 5)
+            self.emit(lib.vb_pack_rows_f32, self.in_loc, self.loc_rows, self.map_v, M, 5)
         else:
-            self.emit(lib.vb_cast_f32_to_bf16, self.in_feat.data_ptr(), hi, M * Fv, feat.fp16, lo, bw)
+            self.emit(lib.vb_cast_f32_to_bf16, self.in_feat, hi, M * Fv, feat.fp16, lo, bw)
         locp = self.buf((M, H), F32)
-        self.emit(lib.vb_loc_proj_fwd, self.loc_rows.data_ptr(), ps.p(prefix + ".image_location_embeddings.weight").data_ptr(),
-                  ps.p(prefix + ".image_location_embeddings.bias").data_ptr(), locp.data_ptr(), M, H)
+        self.emit(lib.vb_loc_proj_fwd, self.loc_rows, ps.p(prefix + ".image_location_embeddings.weight"),
+                  ps.p(prefix + ".image_location_embeddings.bias"), locp, M, H)
         y = self.buf((M, H), F32)
         self.gemm(M, H, Fv, feat, Fv, ps.w(prefix + ".image_embeddings.weight"), Fv, bias=ps.p(prefix + ".image_embeddings.bias"),
                   residual=locp, ld_res=H, out_f32=y, ld_of=H)
@@ -1342,13 +1326,13 @@ class Plan:
         if dy32 is not None:
             gw, gb = self.pg(prefix + ".image_location_embeddings.weight"), self.pg(prefix + ".image_location_embeddings.bias")
             if gw is not None or gb is not None:
-                self.emit(self.lib.vb_loc_proj_bwd, dy32.data_ptr(), self.loc_rows.data_ptr(), self._ptr(gw), self._ptr(gb), M, H)
+                self.emit(self.lib.vb_loc_proj_bwd, dy32, self.loc_rows, gw, gb, M, H)
         if dy16 is not None and "input_imgs" in self.input_grads:
             g = self.input_grad["input_imgs"] = self.buf((M, Fv), F32, zero=True)
             self.gemm(M, Fv, H, dy16, H, ps.w(prefix + ".image_embeddings.weight").bw, Fv, b_mn=1, out_f32=g, ld_of=Fv)
         if dy32 is not None and "image_loc" in self.input_grads:
             g = self.input_grad["image_loc"] = self.buf((M, 5), F32, zero=True)
-            self.emit(self.lib.vb_loc_proj_dx, dy32.data_ptr(), ps.p(prefix + ".image_location_embeddings.weight").data_ptr(), g.data_ptr(), M, H)
+            self.emit(self.lib.vb_loc_proj_dx, dy32, ps.p(prefix + ".image_location_embeddings.weight"), g, M, H)
 
     # ------------------------------------------------------------------ poolers and heads
     def pooler(self, seq, N, wname):
@@ -1369,7 +1353,7 @@ class Plan:
                 return
             dpre = self.scratch("pool.dpre", (B, Hb), BF16)
             dpre32 = self.scratch("pool.dpre32", (B, Hb), F32)
-            self.emit(self.lib.vb_relu_bwd, pooled.g32.data_ptr(), p32.data_ptr(), dpre.data_ptr(), dpre32.data_ptr(), B * Hb)
+            self.emit(self.lib.vb_relu_bwd, pooled.g32, p32, dpre, dpre32, B * Hb)
             self.linear_wgrad(dpre, Hb, x.bw, ldx, B, Hb, H, wname, bias_from=(dpre32, Hb))
             self.pooler_dgrad(seq, N, dpre, wname, first if self.packed else None)
         self.push_bwd(bwd, pooled.rg)
@@ -1385,7 +1369,7 @@ class Plan:
         if rows is not None:
             d = self.scratch("pool.dx", (B, seq.H), F32)
             self.gemm(B, seq.H, K, dpre, K, self.ps.w(wname + ".weight").bw, seq.H, b_mn=1, out_f32=d, ld_of=seq.H)
-            self.emit(self.lib.vb_scatter_add_rows_f32, d.data_ptr(), g.data_ptr(), rows.data_ptr(), B, seq.H)
+            self.emit(self.lib.vb_scatter_add_rows_f32, d, g, rows, B, seq.H)
             return
         self.gemm(B, seq.H, K, dpre, K, self.ps.w(wname + ".weight").bw, seq.H, b_mn=1, residual=g, ld_res=N * seq.H, out_f32=g,
                   ld_of=N * seq.H)
@@ -1417,7 +1401,7 @@ class Plan:
             dl32, dl16 = self.out_grad_buffer(name, (M, N_out)), self.head_dl16.get(name)
             if dl16 is None:
                 dl16 = self.scratch("head.dl16." + name, (M, ldp), BF16)
-                self.emit(self.lib.vb_cast2d_f32_to_bf16, dl32.data_ptr(), N_out, dl16.data_ptr(), ldp, M, N_out, 1.0)
+                self.emit(self.lib.vb_cast2d_f32_to_bf16, dl32, N_out, dl16, ldp, M, N_out, 1.0)
             gb = self.pg(bias_name)
             if gb is not None:
                 self.colsum(dl32, N_out, gb, M, N_out)
@@ -1452,7 +1436,7 @@ class Plan:
         labels.fill_(-1)
         self.loss_inputs["masked_lm_labels"] = labels
         idx, cnt, lab_c = self.buf((cap,), torch.int32), self.buf((1,), torch.int32, zero=True), self.buf((cap,), I64)
-        self.emit(lib.vb_compact_rows, labels.data_ptr(), -1, M, cap, idx.data_ptr(), cnt.data_ptr(), lab_c.data_ptr())
+        self.emit(lib.vb_compact_rows, labels, -1, M, cap, idx, cnt, lab_c)
         hc = self.gather_rows(ht.op, idx, cap, Ht)
         wn = "bert.embeddings.word_embeddings.weight"
         logits = self.buf((cap, V), F32)
@@ -1476,17 +1460,16 @@ class Plan:
             gc = self.scratch("lm.gc", (cap, Ht), F32)
             self.gemm(cap, Ht, V, lc["dl16"], ldp, ps.w(wn).bw, Ht, b_mn=1, out_f32=gc, ld_of=Ht)
             g = self.grad_zeroed(ht)
-            self.emit(lib.vb_scatter_rows_f32, gc.data_ptr(), g.data_ptr(), idx.data_ptr(), cap, Ht, cnt.data_ptr(), self.loss_slots[0].data_ptr())
+            self.emit(lib.vb_scatter_rows_f32, gc, g, idx, cap, Ht, cnt, self.loss_slots[0])
             ht_bwd()
         return bwd
 
     def gather_rows(self, src, idx, rows, H):
         """The rows `idx` (int32 [rows]) of the Operand `src` as a compact Operand: hi with its bf16 copy, and lo."""
         op = self.buf16((rows, H))
-        self.emit(self.lib.vb_gather_rows16, src.hi.data_ptr(), op.hi.data_ptr(), self._ptr(src.extra_bw), self._ptr(op.extra_bw),
-                  idx.data_ptr(), rows, H)
+        self.emit(self.lib.vb_gather_rows16, src.hi, op.hi, src.extra_bw, op.extra_bw, idx, rows, H)
         if op.lo is not None:
-            self.emit(self.lib.vb_gather_rows16, src.lo.data_ptr(), op.lo.data_ptr(), None, None, idx.data_ptr(), rows, H)
+            self.emit(self.lib.vb_gather_rows16, src.lo, op.lo, None, None, idx, rows, H)
         return op
 
     def lm_rows(self):
@@ -1521,8 +1504,7 @@ class Plan:
         K = x.H if K is None else K
         xin = x.f32 if x32 is None else x32
         y = self.buf((M, N_out), F32)
-        self.emit(self.lib.vb_small_linear_fwd, xin.data_ptr(), K, ps.p(wname + ".weight").data_ptr(), ps.p(wname + ".bias").data_ptr(),
-                  self._ptr(addend), y.data_ptr(), M, K, N_out, self._ref(in_drop))
+        self.emit(self.lib.vb_small_linear_fwd, xin, K, ps.p(wname + ".weight"), ps.p(wname + ".bias"), addend, y, M, K, N_out, in_drop)
         self.outputs[name] = y
         self.out_rg[name] = x.rg or self.trainable(wname)
 
@@ -1531,8 +1513,8 @@ class Plan:
                 return
             dy = self.out_grad_buffer(name, (M, N_out))
             g, acc = self.grad_acc(x) if x.rg else (None, 0)
-            self.emit(self.lib.vb_small_linear_bwd, dy.data_ptr(), xin.data_ptr(), K, ps.p(wname + ".weight").data_ptr(), self._ptr(g), K, acc,
-                      self._ptr(self.pg(wname + ".weight")), self._ptr(self.pg(wname + ".bias")), M, K, N_out, self._ref(in_drop))
+            self.emit(self.lib.vb_small_linear_bwd, dy, xin, K, ps.p(wname + ".weight"), g, K, acc,
+                      self.pg(wname + ".weight"), self.pg(wname + ".bias"), M, K, N_out, in_drop)
         self.push_bwd(bwd, self.out_rg[name])
 
     def packed_vision_logit(self, seq_v, in_drop):
@@ -1543,10 +1525,9 @@ class Plan:
         M, K = seq_v.M, seq_v.H
         off, ln = self.seg["v"]
         y = self.buf((M, 1), F32)
-        self.emit(lib.vb_small_linear_fwd, seq_v.f32.data_ptr(), K, ps.p(name + ".weight").data_ptr(), ps.p(name + ".bias").data_ptr(), None,
-                  y.data_ptr(), M, K, 1, self._ref(in_drop))
+        self.emit(lib.vb_small_linear_fwd, seq_v.f32, K, ps.p(name + ".weight"), ps.p(name + ".bias"), None, y, M, K, 1, in_drop)
         out = self.buf((B * Nv, 1), F32)
-        self.emit(lib.vb_unpack_rows_f32, y.data_ptr(), out.data_ptr(), off.data_ptr(), ln.data_ptr(), B, Nv, 1, PACKED_MASKED_LOGIT)
+        self.emit(lib.vb_unpack_rows_f32, y, out, off, ln, B, Nv, 1, PACKED_MASKED_LOGIT)
         self.outputs[name] = out
         self.out_rg[name] = seq_v.rg or self.trainable(name)
 
@@ -1554,10 +1535,10 @@ class Plan:
             if name not in self.grad_outputs:
                 return
             dy = self.scratch("vlogit.dy", (M, 1), F32)
-            self.emit(lib.vb_pack_rows_f32, self.out_grad_buffer(name, (B * Nv, 1)).data_ptr(), dy.data_ptr(), self.map_v.data_ptr(), M, 1)
+            self.emit(lib.vb_pack_rows_f32, self.out_grad_buffer(name, (B * Nv, 1)), dy, self.map_v, M, 1)
             g, acc = self.grad_acc(seq_v) if seq_v.rg else (None, 0)
-            self.emit(lib.vb_small_linear_bwd, dy.data_ptr(), seq_v.f32.data_ptr(), K, ps.p(name + ".weight").data_ptr(), self._ptr(g), K, acc,
-                      self._ptr(self.pg(name + ".weight")), self._ptr(self.pg(name + ".bias")), M, K, 1, self._ref(in_drop))
+            self.emit(lib.vb_small_linear_bwd, dy, seq_v.f32, K, ps.p(name + ".weight"), g, K, acc,
+                      self.pg(name + ".weight"), self.pg(name + ".bias"), M, K, 1, in_drop)
         self.push_bwd(bwd, self.out_rg[name])
 
     def build_heads(self, seq_t, seq_v, pooled_t, pooled_v):
@@ -1570,8 +1551,7 @@ class Plan:
             f32 = self.buf((B, Hb), F32)
             f = self.buf16((B, Hb))
             hi, lo, bw = f.ptrs()
-            self.emit(lib.vb_fuse_pooled_fwd, pooled_t.f32.data_ptr(), pooled_v.f32.data_ptr(), f32.data_ptr(), hi, B * Hb, mul, self._ref(drop),
-                      f.fp16, lo, bw)
+            self.emit(lib.vb_fuse_pooled_fwd, pooled_t.f32, pooled_v.f32, f32, hi, B * Hb, mul, drop, f.fp16, lo, bw)
             act = self.act(f32, f, B, Hb, inputs=(pooled_t, pooled_v))
 
             def fuse_bwd():
@@ -1580,8 +1560,7 @@ class Plan:
                 for a in (pooled_t, pooled_v):
                     if a.rg:
                         self.grad_zeroed(a)
-                self.emit(lib.vb_fuse_pooled_bwd, act.g32.data_ptr(), pooled_t.f32.data_ptr(), pooled_v.f32.data_ptr(), self._ptr(pooled_t.g32),
-                          self._ptr(pooled_v.g32), B * Hb, mul, self._ref(drop))
+                self.emit(lib.vb_fuse_pooled_bwd, act.g32, pooled_t.f32, pooled_v.f32, pooled_t.g32, pooled_v.g32, B * Hb, mul, drop)
             self.push_bwd(fuse_bwd, act.rg)
             return act
         # VILBertForVLTasks.dropout on the fused vector (vilbert.py:1677-1682); BertPreTrainingHeads has its own nn.Dropout(0.1)
@@ -1632,7 +1611,7 @@ class Plan:
             hb32 = self.buf((B // 2, 2 * Hb), F32)
             # re-emit LN with an fp32 output (cheap: B/2 rows)
             fwd_fn, fwd_args, fwd_sid = self.fwd[-1]
-            args = list(fwd_args); args[5] = hb32.data_ptr(); self.fwd[-1] = (fwd_fn, tuple(args), fwd_sid)
+            args = list(fwd_args); args[5] = L.arg(hb32); self.fwd[-1] = (fwd_fn, tuple(args), fwd_sid)
             hb.f32 = hb32
 
             def bin_bwd():
@@ -1847,12 +1826,12 @@ class Plan:
         if h.ids is not None:
             li[h.ids] = self.buf((h.rows, h.cols), I64, zero=True)
         li[h.key] = self.buf((h.rows,), I64, zero=True) if h.key == "labels" else self.buf((h.rows, h.cols), F32, zero=True)
-        lg, inp, loss = h.logits.data_ptr(), li[h.key].data_ptr(), self.loss.data_ptr()
+        lg, inp, loss = h.logits, li[h.key], self.loss
         if k == "vqa":
             self.vqa_target = li["target"]      # the VQA soft target under its round-1 name
         if h.key == "labels":
             d = self._head_grad(h.name, tuple(h.logits.shape))
-            self.emit(lib.vb_ce_loss, lg, h.ld, inp, -1, loss, d.data_ptr(), h.ld, None, 0, h.rows, h.cols, 1.0, 0)
+            self.emit(lib.vb_ce_loss, lg, h.ld, inp, -1, loss, d, h.ld, None, 0, h.rows, h.cols, 1.0, 0)
         elif k in ("vqa", "gqa", "vlogit_bce"):
             if k == "vqa" and not self.task_objective:
                 # the summed VQA objective (the round-1 training step) also writes the bf16 operand of the wide head's backward GEMMs
@@ -1861,13 +1840,12 @@ class Plan:
                 d16 = self.head_dl16[h.name] = self.buf((h.rows, _pad8(h.cols)), BF16, zero=True)
             else:
                 d, d16 = self._head_grad(h.name, tuple(h.logits.shape)), None
-            self.emit(lib.vb_bce_logits_loss, lg, inp, loss, d.data_ptr(), self._ptr(d16), 0 if d16 is None else d16.shape[1], h.rows,
-                      h.cols, 1.0)
+            self.emit(lib.vb_bce_logits_loss, lg, inp, loss, d, d16, 0 if d16 is None else d16.shape[1], h.rows, h.cols, 1.0)
         else:   # V-logit-mc: BCE mean x C over the gathered choices; the soft-target binary / tri heads: BCE mean
             d = self._head_grad(h.name, tuple(h.logits.shape))
             row_loss = self.buf((h.rows,), F32)
-            self.emit(lib.vb_bce_gather_loss, lg, h.ld, h.off, h.ld, self._ptr(li.get(h.ids)), inp, h.rows, h.cols,
-                      float(h.cols if k == "vlogit_mc" else 1.0), row_loss.data_ptr(), loss, 0, d.data_ptr(), h.ld, None, 0)
+            self.emit(lib.vb_bce_gather_loss, lg, h.ld, h.off, h.ld, li.get(h.ids), inp, h.rows, h.cols,
+                      float(h.cols if k == "vlogit_mc" else 1.0), row_loss, loss, 0, d, h.ld, None, 0)
         if self.want_score:
             self._emit_score()
 
@@ -1891,46 +1869,40 @@ class Plan:
             lc = self.lm_c
             d32 = grad("linguisic_prediction", (lc["cap"], V)) if sep else lc["dl32"]
             d16 = None if sep else lc["dl16"]      # loss_in_forward: the backward scales d32, then casts it into dl16
-            self.emit(lib.vb_ce_loss, lc["logits"].data_ptr(), V, lc["labels"].data_ptr(), -1, slot[0].data_ptr(), self._ptr(d32), V,
-                      self._ptr(d16), lc["ldp"], lc["cap"], V, 1.0, 0)
+            self.emit(lib.vb_ce_loss, lc["logits"], V, lc["labels"], -1, slot[0], d32, V, d16, lc["ldp"], lc["cap"], V, 1.0, 0)
             if sep:
                 # more labelled rows than the capacity must already show in the forward (eval plans have no backward): the scatter
                 # kernel's count check poisons the masked-LM slot; the rows it moves are a 4-column dummy
                 src = self.scratch("lm.cap.src", (lc["cap"], 4), F32)
                 dst = self.scratch("lm.cap.dst", (B * self.Nt, 4), F32)
-                self.emit(lib.vb_scatter_rows_f32, src.data_ptr(), dst.data_ptr(), lc["idx"].data_ptr(), lc["cap"], 4, lc["count"].data_ptr(),
-                          slot[0].data_ptr())
+                self.emit(lib.vb_scatter_rows_f32, src, dst, lc["idx"], lc["cap"], 4, lc["count"], slot[0])
         else:
             lg, rows = self.outputs["linguisic_prediction"], B * self.Nt
             li["masked_lm_labels"] = self.buf((rows,), I64, zero=True)
             d = grad("linguisic_prediction", tuple(lg.shape))
-            self.emit(lib.vb_ce_loss, lg.data_ptr(), V, li["masked_lm_labels"].data_ptr(), -1, slot[0].data_ptr(), self._ptr(d), V, None, 0,
-                      rows, V, 1.0, 0)
+            self.emit(lib.vb_ce_loss, lg, V, li["masked_lm_labels"], -1, slot[0], d, V, None, 0, rows, V, 1.0, 0)
         sv = self.outputs["vision_prediction"]
         li["image_target"] = self.buf((B, R, C), F32, zero=True)
         li["image_label"] = self.buf((B, R), I64, zero=True)
         dv = grad("vision_prediction", tuple(sv.shape))
         vt = c.visual_target
         if vt == 0:
-            self.emit(lib.vb_kl_masked_loss, sv.data_ptr(), li["image_target"].data_ptr(), li["image_label"].data_ptr(), slot[1].data_ptr(),
-                      self._ptr(dv), None, 0, B, Nv, C, 1.0, acc)
+            self.emit(lib.vb_kl_masked_loss, sv, li["image_target"], li["image_label"], slot[1], dv, None, 0, B, Nv, C, 1.0, acc)
         elif vt == 1:
             row_loss = self.buf((B * Nv,), F32)
-            self.emit(lib.vb_mse_masked_loss, sv.data_ptr(), li["image_target"].data_ptr(), li["image_label"].data_ptr(), B, Nv, C, 1.0,
-                      row_loss.data_ptr(), slot[1].data_ptr(), acc, self._ptr(dv))
+            self.emit(lib.vb_mse_masked_loss, sv, li["image_target"], li["image_label"], B, Nv, C, 1.0, row_loss, slot[1], acc, dv)
         elif vt == 2:
             n = nce_negative_count(c)
             li["neg_index"] = self.buf((B, R, n), I64, zero=True)
             row_loss = self.buf((B * Nv,), F32)
-            self.emit(lib.vb_nce_region_loss, sv.data_ptr(), li["image_target"].data_ptr(), li["image_label"].data_ptr(), li["neg_index"].data_ptr(),
-                      B, Nv, C, n, 1.0, row_loss.data_ptr(), slot[1].data_ptr(), acc, self._ptr(dv))
+            self.emit(lib.vb_nce_region_loss, sv, li["image_target"], li["image_label"], li["neg_index"],
+                      B, Nv, C, n, 1.0, row_loss, slot[1], acc, dv)
         else:
             raise ValueError(f"visual_target must be 0, 1 or 2, got {vt!r}")
         ns = self.outputs["seq_relationship_score"]
         li["next_sentence_label"] = self.buf((B,), I64, zero=True)
         d = grad("seq_relationship_score", tuple(ns.shape))
-        self.emit(lib.vb_ce_loss, ns.data_ptr(), 2, li["next_sentence_label"].data_ptr(), -1, slot[2].data_ptr(), self._ptr(d), 2, None, 0, B, 2,
-                  1.0, acc)
+        self.emit(lib.vb_ce_loss, ns, 2, li["next_sentence_label"], -1, slot[2], d, 2, None, 0, B, 2, 1.0, acc)
 
     def _head_grad(self, name, shape):
         """Where the objective writes d loss / d head: the head's output-gradient buffer, or with loss_in_forward a buffer of its own
@@ -1946,9 +1918,8 @@ class Plan:
         h, li = self._head_layout(self.loss_kind), self.loss_inputs
         labels, target = (li["labels"], None) if h.key == "labels" else (None, li["target"])
         self.preds = self.buf((h.rows,), I64, zero=True)
-        self.emit(self.lib.vb_task_score, SCORE_MODES[self.loss_kind], h.logits.data_ptr(), h.ld, h.off, h.cols, self._ptr(li.get(h.ids)),
-                  h.width, self._ptr(target), h.cols if target is not None else 0, self._ptr(labels), h.rows, self.score.data_ptr(), 0,
-                  self.preds.data_ptr())
+        self.emit(self.lib.vb_task_score, SCORE_MODES[self.loss_kind], h.logits, h.ld, h.off, h.cols, li.get(h.ids), h.width, target,
+                  h.cols if target is not None else 0, labels, h.rows, self.score, 0, self.preds)
 
     def _emit_results(self):
         """vb_task_results on the head of self.results (RESULT_MODES), addressed as the objective and the score address it; the
@@ -1956,9 +1927,8 @@ class Plan:
         h, mode = self._head_layout(self.results), RESULT_MODES[self.results][1]
         target = self.loss_inputs["target"] if mode == L.VB_RESULT_GATHER else None
         vals = self.results_values
-        self.emit(self.lib.vb_task_results, mode, h.logits.data_ptr(), h.ld, h.off, h.cols, self._ptr(self.loss_inputs.get(h.ids)), h.width,
-                  self._ptr(target), h.cols if target is not None else 0, h.rows, self.results_argmax.data_ptr(), self._ptr(vals),
-                  1 if vals is None else vals.shape[1])
+        self.emit(self.lib.vb_task_results, mode, h.logits, h.ld, h.off, h.cols, self.loss_inputs.get(h.ids), h.width, target,
+                  h.cols if target is not None else 0, h.rows, self.results_argmax, vals, 1 if vals is None else vals.shape[1])
 
     def fetch_results(self):
         """Reads results_out with one device-to-host copy: (loss, score, argmax int64 [rows], values f32 [rows, n] or None) on the
@@ -1983,11 +1953,11 @@ class Plan:
                 if name == "linguisic_prediction" and self.lm_c is not None:
                     lc = self.lm_c
                     V = self.cfg.vocab_size
-                    self.emit(self.lib.vb_scale_by_device, d.data_ptr(), lc["dl32"].data_ptr(), d.numel(), s.data_ptr())
-                    self.emit(self.lib.vb_cast2d_f32_to_bf16, lc["dl32"].data_ptr(), V, lc["dl16"].data_ptr(), lc["ldp"], lc["cap"], V, 1.0)
+                    self.emit(self.lib.vb_scale_by_device, d, lc["dl32"], d.numel(), s)
+                    self.emit(self.lib.vb_cast2d_f32_to_bf16, lc["dl32"], V, lc["dl16"], lc["ldp"], lc["cap"], V, 1.0)
                     continue
                 g = self.out_grad_buffer(name, tuple(d.shape))
-                self.emit(self.lib.vb_scale_by_device, d.data_ptr(), g.data_ptr(), d.numel(), s.data_ptr())
+                self.emit(self.lib.vb_scale_by_device, d, g, d.numel(), s)
 
     # ------------------------------------------------------------------ execution
     def load_inputs(self, input_txt, input_imgs, image_loc, token_type_ids=None, attention_mask=None, image_attention_mask=None,
@@ -2144,23 +2114,21 @@ class Plan:
         the vision stream underneath those text layers (the vision stream's own first consumer, the image embedding, is
         queued behind them and is not needed before the first connection layer)."""
         ps, lib = self.ps, self.lib
-        self.prologue = []
+        self.prologue = self.cur = []
         if self.train:
-            self.prologue.append((lib.vb_step_counter_bump, (self.e.drop_step.data_ptr(),), 0))
+            self.emit(lib.vb_step_counter_bump, self.e.drop_step)
         n = ps.numel
         first_c = [off for name, (off, _) in ps.entries.items() if ".c_layer." in name]
         split = min(first_c) if (self.two_streams and first_c) else n
         if refresh_weights and split > 0:
-            self.prologue.append((lib.vb_cast_f32_to_bf16, ps.cast_args(0, split), 0))
-        tail = []
-        if zero_grad:
-            tail.append((lib.vb_memset_zero, (ps.grad.data_ptr(), ps.grad.numel() * 4), 1 if self.two_streams else 0))
-        if refresh_weights and split < n:
-            tail.append((lib.vb_cast_f32_to_bf16, ps.cast_args(split, n - split), 1))
-        if self.two_streams:
-            self.prologue += [(None, (), 0)] + tail       # barrier: the vision stream starts after the main-stream part
-        else:
-            self.prologue += tail
+            self.emit(lib.vb_cast_f32_to_bf16, *ps.cast_args(0, split))
+        self.sync_streams(mirror=False)       # the vision stream starts after the main-stream part
+        with self.on(1):
+            if zero_grad:
+                self.emit(lib.vb_memset_zero, ps.grad, ps.grad.numel() * 4)
+            if refresh_weights and split < n:
+                self.emit(lib.vb_cast_f32_to_bf16, *ps.cast_args(split, n - split))
+        self.cur = self.fwd
         self.graph_step = None
 
     def enable_optimizer(self, opt, dropout_bump=True):
@@ -2169,9 +2137,10 @@ class Plan:
         gradient memset in the step. (The host-side lr table of `opt` is refreshed by opt.step(); here the launch alone is
         replayed, e.g. inside the step graph, with the table currently on the device.) With `max_grad_norm` the gradient-norm
         launch precedes it, so every replay clips and skips a non-finite step on the device."""
-        self.prologue = []
+        self.prologue = self.cur = []
         if self.train and dropout_bump:
-            self.prologue.append((self.lib.vb_step_counter_bump, (self.e.drop_step.data_ptr(),), 0))
+            self.emit(self.lib.vb_step_counter_bump, self.e.drop_step)
+        self.cur = self.fwd
         self.epilogue = [(fn, args, 0) for fn, args in opt.ops()]
         self.graph_step = None
 
@@ -2408,13 +2377,12 @@ class BasePlan(Plan):
         self.in_feat = self.buf((B, Nv, Fv), F32, zero=True)
         self.in_loc = self.buf((B, Nv, 5), F32, zero=True)
         self.mask = self.buf((B, self.N), F32)
-        self.emit(lib.vb_mask_concat_additive, self.in_amask.data_ptr(), self.in_imask.data_ptr(), self.mask.data_ptr(), B, Nt, Nv)
+        self.emit(lib.vb_mask_concat_additive, self.in_amask, self.in_imask, self.mask, B, Nt, Nv)
         self.sync_streams()      # the second stream reads the inputs that load_inputs copied on the main stream
         e, ie = "bert.embeddings", "bert.image_embeddings"
         t_tables = [e + n for n in (".word_embeddings.weight", ".position_embeddings.weight", ".token_type_embeddings.weight")]
         xt = self.buf((Mt, H), F32)
-        self.emit(lib.vb_embed_text_fwd, self.in_ids.data_ptr(), self.in_tt.data_ptr(), None, *[ps.p(n).data_ptr() for n in t_tables], None,
-                  xt.data_ptr(), B, Nt, H)
+        self.emit(lib.vb_embed_text_fwd, self.in_ids, self.in_tt, None, *[ps.p(n) for n in t_tables], None, xt, B, Nt, H)
         with self.on(1):
             xv, feat = self.image_embedding(ie, H)
         self.sync_streams()
@@ -2424,9 +2392,8 @@ class BasePlan(Plan):
         y32, y = self.buf((M, H), F32), self.buf16((M, H))
         mean, rstd = self.buf((M,), F32), self.buf((M,), F32)
         lnt, lnv = e + ".LayerNorm", ie + ".LayerNorm"
-        self.emit(lib.vb_concat_embed_ln_fwd, xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
-                  ps.p(lnt + ".bias").data_ptr(), ps.p(lnv + ".weight").data_ptr(), ps.p(lnv + ".bias").data_ptr(), y32.data_ptr(), *y.ptrs(),
-                  y.fp16, mean.data_ptr(), rstd.data_ptr(), B, Nt, Nv, H, self._ref(tdrop), self._ref(vdrop))
+        self.emit(lib.vb_concat_embed_ln_fwd, xt, xv, trow, ps.p(lnt + ".weight"), ps.p(lnt + ".bias"), ps.p(lnv + ".weight"), ps.p(lnv + ".bias"),
+                  y32, *y.ptrs(), y.fp16, mean, rstd, B, Nt, Nv, H, tdrop, vdrop)
         img = [ie + n for n in (".image_embeddings.weight", ".image_embeddings.bias", ".token_type_embeddings.weight",
                                 ".image_location_embeddings.weight", ".image_location_embeddings.bias")]
         lns = [lnt + ".weight", lnt + ".bias", lnv + ".weight", lnv + ".bias"]
@@ -2442,13 +2409,10 @@ class BasePlan(Plan):
             dxv32 = self.scratch("emb.dxv32", (Mv, H), F32) if want32 else None
             dxv16 = self.scratch("emb.dxv16", (Mv, H), BF16) if want16 else None
             gtype = self.pg(img[2])
-            self.emit(lib.vb_concat_embed_ln_bwd, x.g32.data_ptr(), xt.data_ptr(), xv.data_ptr(), trow.data_ptr(), ps.p(lnt + ".weight").data_ptr(),
-                      ps.p(lnv + ".weight").data_ptr(), mean.data_ptr(), rstd.data_ptr(), self._ptr(dxt), self._ptr(dxv32), self._ptr(dxv16),
-                      *[self._ptr(self.pg(n)) for n in lns], self._ptr(self.pg(img[1])), None if gtype is None else gtype[1].data_ptr(),
-                      B, Nt, Nv, H, self._ref(tdrop), self._ref(vdrop))
+            self.emit(lib.vb_concat_embed_ln_bwd, x.g32, xt, xv, trow, ps.p(lnt + ".weight"), ps.p(lnv + ".weight"), mean, rstd, dxt, dxv32, dxv16,
+                      *[self.pg(n) for n in lns], self.pg(img[1]), None if gtype is None else gtype[1], B, Nt, Nv, H, tdrop, vdrop)
             if dxt is not None:
-                self.emit(lib.vb_embed_text_bwd_padded, dxt.data_ptr(), self.in_ids.data_ptr(), self.in_tt.data_ptr(), *[self._ptr(g) for g in gt],
-                          B, Nt, H)
+                self.emit(lib.vb_embed_text_bwd_padded, dxt, self.in_ids, self.in_tt, *gt, B, Nt, H)
             self.image_embedding_bwd(ie, H, feat, dxv16, dxv32)
         self.push_bwd(bwd, x.rg)
         return x
@@ -2467,14 +2431,14 @@ class BasePlan(Plan):
         pre = self.buf((B, H), F32)
         self.gemm(B, H, H, seq.op, N * H, ps.w(w + ".weight"), H, bias=ps.p(w + ".bias"), out_f32=pre, ld_of=H)
         y32, y = self.buf((B, H), F32), self.buf16((B, H))
-        self.emit(self.lib.vb_tanh_fwd, pre.data_ptr(), y32.data_ptr(), *y.ptrs(), y.fp16, B * H)
+        self.emit(self.lib.vb_tanh_fwd, pre, y32, *y.ptrs(), y.fp16, B * H)
         pooled = self.act(y32, y, B, H, inputs=(seq,), params=(w,))
 
         def bwd():
             if not pooled.gw:
                 return
             dpre = self.scratch("pool.dpre", (B, H), BF16)
-            self.emit(self.lib.vb_tanh_bwd, pooled.g32.data_ptr(), y32.data_ptr(), dpre.data_ptr(), self._ptr(self.pg(w + ".bias")), B, H)
+            self.emit(self.lib.vb_tanh_bwd, pooled.g32, y32, dpre, self.pg(w + ".bias"), B, H)
             self.linear_wgrad(dpre, H, seq.op.bw, N * H, B, H, H, w)
             self.pooler_dgrad(seq, N, dpre, w)
         self.push_bwd(bwd, pooled.rg)
@@ -2496,12 +2460,12 @@ class BasePlan(Plan):
                 self._scatter_ok = True
             g = self.grad_zeroed(seq)
             if self._scatter_ok:
-                self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), g.data_ptr(), idx.data_ptr(), B * n, H, None, None)
+                self.emit(lib.vb_scatter_rows_f32, rows.g32, g, idx, B * n, H, None, None)
                 return
             full = self.scratch(tag + ".full", (B * N, H), F32)      # the stream gradient already holds other contributions
-            self.emit(lib.vb_memset_zero, full.data_ptr(), full.numel() * 4)
-            self.emit(lib.vb_scatter_rows_f32, rows.g32.data_ptr(), full.data_ptr(), idx.data_ptr(), B * n, H, None, None)
-            self.emit(lib.vb_axpy_f32, full.data_ptr(), g.data_ptr(), full.numel(), 1.0)
+            self.emit(lib.vb_memset_zero, full, full.numel() * 4)
+            self.emit(lib.vb_scatter_rows_f32, rows.g32, full, idx, B * n, H, None, None)
+            self.emit(lib.vb_axpy_f32, full, g, full.numel(), 1.0)
         self.push_bwd(bwd, rows.rg)
         return rows
 
@@ -2519,7 +2483,7 @@ class BasePlan(Plan):
             v, g = ps.p(nm + ".weight_v"), ps.p(nm + ".weight_g")
             w32, op = self.buf(tuple(v.shape), F32), self.buf16(tuple(v.shape))
             scr = self.buf((L.VB_WEIGHT_NORM_SCRATCH // 8,), torch.float64)
-            self.emit(lib.vb_weight_norm_fwd, v.data_ptr(), g.data_ptr(), v.numel(), w32.data_ptr(), *op.ptrs(), op.fp16, scr.data_ptr())
+            self.emit(lib.vb_weight_norm_fwd, v, g, v.numel(), w32, *op.ptrs(), op.fp16, scr)
             W[i] = (nm, v, g, op, scr)
             self.wn_weights[nm] = w32
         p_drop = 0.5
@@ -2541,9 +2505,9 @@ class BasePlan(Plan):
             if gg is None and gv is None:
                 return
             dw = self.scratch(f"vilp.dw{i}", (N_out, K_in), F32)
-            self.emit(lib.vb_memset_zero, dw.data_ptr(), dw.numel() * 4)
+            self.emit(lib.vb_memset_zero, dw, dw.numel() * 4)
             self.gemm(N_out, K_in, M, dy16, ld_dy, x16, ld_x, a_mn=1, b_mn=1, out_f32=dw, ld_of=K_in, atomic=1, split_k=0)
-            self.emit(lib.vb_weight_norm_bwd, dw.data_ptr(), v.data_ptr(), g.data_ptr(), v.numel(), self._ptr(gg), self._ptr(gv), scr.data_ptr())
+            self.emit(lib.vb_weight_norm_bwd, dw, v, g, v.numel(), gg, gv, scr)
 
         def bwd():
             if "vil_prediction" not in self.grad_outputs:
@@ -2551,7 +2515,7 @@ class BasePlan(Plan):
             ldp = _pad8(Lb)
             dl32 = self.out_grad_buffer("vil_prediction", (B, Lb))
             dl16 = self.scratch("vilp.dl16", (B, ldp), BF16)
-            self.emit(lib.vb_cast2d_f32_to_bf16, dl32.data_ptr(), Lb, dl16.data_ptr(), ldp, B, Lb, 1.0)
+            self.emit(lib.vb_cast2d_f32_to_bf16, dl32, Lb, dl16, ldp, B, Lb, 1.0)
             gb = self.pg("vil_prediction.main.3.bias")
             if gb is not None:
                 self.colsum(dl32, Lb, gb, B, Lb)
@@ -2561,7 +2525,7 @@ class BasePlan(Plan):
             dh = self.scratch("vilp.dh32", (B, H2), F32)
             self.gemm(B, H2, Lb, dl16, ldp, W[3][3].bw, H2, b_mn=1, out_f32=dh, ld_of=H2, alpha=scale)
             dpre16, dpre32 = self.scratch("vilp.dpre16", (B, H2), BF16), self.scratch("vilp.dpre32", (B, H2), F32)
-            self.emit(lib.vb_relu_bwd, dh.data_ptr(), h32.data_ptr(), dpre16.data_ptr(), dpre32.data_ptr(), B * H2)
+            self.emit(lib.vb_relu_bwd, dh, h32, dpre16, dpre32, B * H2)
             gb = self.pg("vil_prediction.main.0.bias")
             if gb is not None:
                 self.colsum(dpre32, H2, gb, B, H2)
@@ -2688,7 +2652,7 @@ class Engine:
 
     def bump_dropout_step(self):
         """New dropout masks for the next forward (plans with a training prologue do this inside their graph)."""
-        L.check(L.lib().vb_step_counter_bump(self.drop_step.data_ptr(), torch.cuda.current_stream().cuda_stream), "vb_step_counter_bump")
+        L.call(L.lib().vb_step_counter_bump, self.drop_step)
         self.drop_step_host = (self.drop_step_host + 1) & 0xFFFFFFFF
 
     def set_dropout_step(self, step):
@@ -2696,12 +2660,12 @@ class Engine:
         self.drop_step.fill_(self.drop_step_host if self.drop_step_host < 2 ** 31 else self.drop_step_host - 2 ** 32)
 
     def refresh_weights(self):
-        self.ps.refresh_shadow(torch.cuda.current_stream().cuda_stream)
+        self.ps.refresh_shadow()
         self.shadow_clean = True
 
     def zero_grad(self, force=False):
         """Zeroes the flat gradient buffer unless it is known to be clean (the fused optimizer zeroes it in its own pass)."""
         if self.grad_clean and not force:
             return
-        L.check(L.lib().vb_memset_zero(self.ps.grad.data_ptr(), self.ps.grad.numel() * 4, torch.cuda.current_stream().cuda_stream))
+        L.call(L.lib().vb_memset_zero, self.ps.grad, self.ps.grad.numel() * 4)
         self.grad_clean = True

@@ -155,15 +155,18 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
     def _buffer_args(self):
         """The leading arguments of vb_adamw_step / vb_radam_step: buffers, 16-bit copies, chunk table and group table."""
         ps = self.engine.ps
-        return (ps.flat.data_ptr(), ps.grad.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), *ps.shadows.ptrs(),
-                ps.shadows.fp16, self._chunk_start.data_ptr(), self._chunk_count.data_ptr(), self._chunk_group.data_ptr(), self.n_chunks,
-                self._groups_dev.data_ptr())
+        return (ps.flat, ps.grad, self.exp_avg, self.exp_avg_sq, *ps.shadows.ptrs(), ps.shadows.fp16, self._chunk_start,
+                self._chunk_count, self._chunk_group, self.n_chunks, self._groups_dev)
 
-    def _norm_op(self, step_ptr):
-        """(fn, args) of vb_grad_norm over the chunk table; it advances the counter at step_ptr (None: none) unless it skips."""
-        return (L.lib().vb_grad_norm, (self.engine.ps.grad.data_ptr(), self._chunk_start.data_ptr(), self._chunk_count.data_ptr(),
-                                       self.n_chunks, C.c_float(self.grad_scale), C.c_float(self.max_grad_norm),
-                                       self._norm_partials.data_ptr(), self._clip_record.data_ptr(), step_ptr))
+    @staticmethod
+    def _op(fn, *args):
+        """(fn, C arguments) of one launch for an engine op list."""
+        return fn, L.launch_args(fn, *args)
+
+    def _norm_op(self, step):
+        """(fn, args) of vb_grad_norm over the chunk table; it advances the counter `step` (None: none) unless it skips."""
+        return self._op(L.lib().vb_grad_norm, self.engine.ps.grad, self._chunk_start, self._chunk_count, self.n_chunks,
+                        C.c_float(self.grad_scale), C.c_float(self.max_grad_norm), self._norm_partials, self._clip_record, step)
 
     def op(self):
         """(fn, args) of the step launch for an engine op list when max_grad_norm is None (the step is then one operation)."""
@@ -174,10 +177,8 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
 
     @staticmethod
     def _run(ops, stream):
-        if stream is None:
-            stream = torch.cuda.current_stream().cuda_stream
         for fn, args in ops:
-            L.check(fn(*args, stream), fn.__name__)
+            L.call(fn, *args, stream=stream)
 
     def _after_step(self):
         eng = self.engine
@@ -237,10 +238,10 @@ class FusedAdamW(_FlatBufferOptimizer):
     def ops(self):
         """[(fn, args)] of one step for an engine op list (Plan.epilogue): the step launch, preceded by the gradient norm when
         max_grad_norm is set."""
-        args = self._buffer_args() + (self._step_dev.data_ptr(), C.c_float(self.grad_scale), 1 if self.fused_zero_grad else 0)
+        args = self._buffer_args() + (self._step_dev, C.c_float(self.grad_scale), 1 if self.fused_zero_grad else 0)
         if self.max_grad_norm is None:
-            return [(L.lib().vb_adamw_step, args)]
-        return [self._norm_op(self._step_dev.data_ptr()), (L.lib().vb_adamw_step_clipped, args + (self._clip_record.data_ptr(),))]
+            return [self._op(L.lib().vb_adamw_step, *args)]
+        return [self._norm_op(self._step_dev), self._op(L.lib().vb_adamw_step_clipped, *args, self._clip_record)]
 
     @torch.no_grad()
     def step(self, closure=None):
@@ -280,7 +281,7 @@ class FusedRAdam(_FlatBufferOptimizer):
         self.leader_group = next((gi for gi, g in enumerate(self.param_groups) if any(id(p) in trainable for p in g["params"])), 0)
 
     def _args(self, advance_step):
-        return self._buffer_args() + (self.leader_group, self._step_dev.data_ptr(), advance_step, C.c_float(self.grad_scale),
+        return self._buffer_args() + (self.leader_group, self._step_dev, advance_step, C.c_float(self.grad_scale),
                                       1 if self.fused_zero_grad else 0)
 
     # ------------------------------------------------------------------ stepping
@@ -295,9 +296,9 @@ class FusedRAdam(_FlatBufferOptimizer):
         max_grad_norm is set. Advancing the step counter is part of the step, so every replay of a captured step moves one step
         along the rectification schedule."""
         if self.max_grad_norm is None:
-            return [(L.lib().vb_radam_step, self._args(1 if advance_step else 0))]
-        return [self._norm_op(self._step_dev.data_ptr() if advance_step else None),
-                (L.lib().vb_radam_step_clipped, self._args(0) + (self._clip_record.data_ptr(),))]
+            return [self._op(L.lib().vb_radam_step, *self._args(1 if advance_step else 0))]
+        return [self._norm_op(self._step_dev if advance_step else None),
+                self._op(L.lib().vb_radam_step_clipped, *self._args(0), self._clip_record)]
 
     @torch.no_grad()
     def step(self, closure=None):

@@ -179,8 +179,8 @@ class RetrievalEvaluator:
             raise ValueError(f"target_image: one per caption ({C}), got {target.numel()}")
         ranks = torch.empty(C, dtype=torch.int32, device=scores.device)
         topk = torch.empty((C, int(k)), dtype=torch.int32, device=scores.device)
-        L.check(L.lib().vb_retrieval_rank(scores.data_ptr(), scores.stride(0), C, G, target.data_ptr(), int(k), ranks.data_ptr(),
-                                          topk.data_ptr(), torch.cuda.current_stream(scores.device).cuda_stream), "vb_retrieval_rank")
+        L.call(L.lib().vb_retrieval_rank, scores, scores.stride(0), C, G, target, int(k), ranks, topk,
+               stream=torch.cuda.current_stream(scores.device).cuda_stream)
         return ranks, topk
 
 
