@@ -418,6 +418,11 @@ vb_status vb_gate_scale_bwd(void* dqk, int64_t ldd, const void* qk, const void* 
  *                        poison given, *poison = NaN when *count > cap (rows were dropped: the loss must not look valid) */
 vb_status vb_compact_rows(const int64_t* labels, int64_t ignore_index, int32_t rows, int32_t cap, int32_t* idx, int32_t* count,
                           int64_t* labels_compact, void* stream);
+/* vb_compact_rows on a packed stream (Plan(packed=...)): row r < rows stands for padded row map[r] and is selected when map[r] >= 0
+ * and labels[map[r]] != ignore_index (labels in the padded layout); idx holds packed rows, ascending, so the selected rows come in
+ * the order vb_compact_rows gives their padded rows. */
+vb_status vb_compact_rows_mapped(const int64_t* labels, int64_t ignore_index, const int32_t* map, int32_t rows, int32_t cap, int32_t* idx,
+                                 int32_t* count, int64_t* labels_compact, void* stream);
 vb_status vb_gather_rows16(const void* src, void* dst, const void* src2, void* dst2, const int32_t* idx, int32_t cap, int32_t cols, void* stream);
 vb_status vb_scatter_rows_f32(const float* src, float* dst, const int32_t* idx, int32_t cap, int32_t cols, const int32_t* count, float* poison,
                               void* stream);
@@ -469,6 +474,17 @@ vb_status vb_unpack_rows_f32(const float* src, float* dst, const int32_t* off, c
                              float fill, void* stream);
 vb_status vb_scatter_add_rows_f32(const float* src, float* dst, const int32_t* idx, int32_t rows, int32_t cols, void* stream);
 vb_status vb_zero_tail_rows(void* a, void* b, void* c, int64_t ld_bytes, int32_t row_bytes, const int32_t* first, int32_t rows, void* stream);
+
+/* Whether a pre-training batch can be packed, from its device-resident masks and labels in one launch (one CTA): text_mask /
+ * lm_labels int64 [B, Nt], image_mask int64 [B, Nv], image_label int64 [B, Nv - 1] (regions 1 .. Nv - 1). A NULL mask is all
+ * valid; NULL labels count nothing. out (int32 [2B + 5]):
+ *   out[b], out[B + b]   valid entries of sample b's text / image mask
+ *   out[2B], out[2B + 1] samples whose text / image mask is not prefix-valid or has no valid entry
+ *   out[2B + 2]          tokens with lm_labels != -1 where text_mask == 0
+ *   out[2B + 3]          regions with image_label == 1 where image_mask == 0
+ *   out[2B + 4]          tokens with lm_labels != -1 */
+vb_status vb_pack_summary(const int64_t* text_mask, const int64_t* image_mask, int32_t B, int32_t Nt, int32_t Nv, const int64_t* lm_labels,
+                          const int64_t* image_label, int32_t* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused multi-tensor AdamW on flat buffers (SURVEY.md §8 f2). Replaces pytorch_transformers==1.0.0 AdamW as the reference

@@ -141,6 +141,23 @@ def packed_cases(E):
     ]
 
 
+def packed_pretraining_cases(E):
+    """Packed pre-training steps: the fused objective with its three losses in the forward (BertForMultiModalPreTraining with
+    engine.pack_padding) for every config.visual_target, in train mode and as a forward-only evaluation plan, and a train-mode step
+    with the text stream frozen. Listed after every case above, so that the listing of a tree without them is a prefix of this one."""
+    rows = (24, 32)
+    train = dict(grad_outputs=E.LOSS_HEADS["pretraining"], train=True)
+
+    def step(**kw):
+        return dict(loss="pretraining", loss_in_forward=True, packed=rows, **kw)
+    return [
+        *[case for vt, over in ((0, {}), (1, dict(visual_target=1, v_target_size=48)), (2, dict(visual_target=2, v_target_size=48)))
+          for case in ((f"packed_pretraining_vt{vt}", over, "pretraining", 4, step(**train)),
+                       (f"packed_pretraining_vt{vt}_eval", over, "pretraining", 4, step()))],
+        ("packed_pretraining_frozen_text", {}, "pretraining", 4, step(frozen=("bert.embeddings.", "bert.encoder.layer."), **train)),
+    ]
+
+
 def dump_cases(out, case_list, prec, Engine, BertConfig, tiny, tiny_base):
     """Lists every plan of `case_list` in precision `prec`, without and with the shared activation arena. -> (plans, op records)"""
     n_plans = n_ops = 0
@@ -284,6 +301,11 @@ def main():
     if hasattr(E, "PACKED_HEADS"):
         for prec in PRECISIONS:
             p, o = dump_cases(out, packed_cases(E), prec, Engine, BertConfig, tiny, tiny_base)
+            n_plans, n_ops = n_plans + p, n_ops + o
+    # packed pre-training steps: listed last, so that the listing of a tree without them is a prefix of this one
+    if hasattr(E, "pretraining_pack_rows"):
+        for prec in PRECISIONS:
+            p, o = dump_cases(out, packed_pretraining_cases(E), prec, Engine, BertConfig, tiny, tiny_base)
             n_plans, n_ops = n_plans + p, n_ops + o
     text = "\n".join(out) + "\n"
     if a.out:

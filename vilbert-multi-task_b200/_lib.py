@@ -130,6 +130,7 @@ _SIGNATURES = {
     "vb_gate_scale_fwd": [_P, _P, _I64, _P, _I32, _I32, _I32, _I32, _P],
     "vb_gate_scale_bwd": [_P, _I64, _P, _P, _I64, _P, _P, _P, _I32, _I32, _I32, _I32, _P],
     "vb_compact_rows": [_P, _I64, _I32, _I32, _P, _P, _P, _P],
+    "vb_compact_rows_mapped": [_P, _I64, _P, _I32, _I32, _P, _P, _P, _P],
     "vb_gather_rows16": [_P, _P, _P, _P, _P, _I32, _I32, _P],
     "vb_scatter_rows_f32": [_P, _P, _P, _I32, _I32, _P, _P, _P],
     "vb_adamw_step": [_P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _P, _F, _I32, _P],
@@ -151,6 +152,7 @@ _SIGNATURES = {
     "vb_unpack_rows_f32": [_P, _P, _P, _P, _I32, _I32, _I32, _F, _P],
     "vb_scatter_add_rows_f32": [_P, _P, _P, _I32, _I32, _P],
     "vb_zero_tail_rows": [_P, _P, _P, _I64, _I32, _P, _I32, _P],
+    "vb_pack_summary": [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P],
 }
 # device scratch of one vb_weight_norm_fwd / _bwd launch (include/vilbert_b200.h)
 VB_WEIGHT_NORM_SCRATCH = 1024

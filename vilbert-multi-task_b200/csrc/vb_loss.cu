@@ -144,9 +144,12 @@ kl_masked_loss_kernel(const float* __restrict__ scores, const float* __restrict_
 // ------------------------------------------------------------------------------------------ masked-row compaction (masked-LM head)
 // Only the rows whose label != ignore_index contribute to the masked-LM cross-entropy (15 % of the tokens, vilbert.py:1578-1583),
 // so when only the loss is wanted the 30522-way tied decoder runs on those rows alone: idx[r] = r-th selected row (ascending),
-// -1 beyond the count; *count = number of selected rows (may exceed cap: the caller checks).
-__global__ void __launch_bounds__(1024) compact_rows_kernel(const long long* __restrict__ labels, long long ignore_index, int rows, int cap,
-                                                             int* __restrict__ idx, int* __restrict__ count, long long* __restrict__ labels_c) {
+// -1 beyond the count; *count = number of selected rows (may exceed cap: the caller checks). With a row map (a packed stream,
+// vb_pack.cu) row r stands for padded row map[r] and is selected when map[r] >= 0 and labels[map[r]] != ignore_index; idx then
+// holds packed rows, in the order of their padded rows.
+__global__ void __launch_bounds__(1024) compact_rows_kernel(const long long* __restrict__ labels, long long ignore_index, const int* __restrict__ map,
+                                                             int rows, int cap, int* __restrict__ idx, int* __restrict__ count,
+                                                             long long* __restrict__ labels_c) {
   pdl_entry();
   __shared__ int wsum[32];
   __shared__ int carry;
@@ -155,7 +158,8 @@ __global__ void __launch_bounds__(1024) compact_rows_kernel(const long long* __r
   __syncthreads();
   for (int base = 0; base < rows; base += 1024) {
     const int r = base + threadIdx.x;
-    const int sel = (r < rows && labels[r] != ignore_index) ? 1 : 0;
+    const int src = r < rows ? (map ? map[r] : r) : -1;
+    const int sel = (src >= 0 && labels[src] != ignore_index) ? 1 : 0;
     int v = sel;                                   // inclusive warp scan
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) { const int n = __shfl_up_sync(0xffffffffu, v, o); if ((threadIdx.x & 31) >= o) v += n; }
@@ -169,7 +173,7 @@ __global__ void __launch_bounds__(1024) compact_rows_kernel(const long long* __r
     }
     __syncthreads();
     const int before = carry + (threadIdx.x >= 32 ? wsum[(threadIdx.x >> 5) - 1] : 0) + v - sel;
-    if (sel && before < cap) { idx[before] = r; labels_c[before] = labels[r]; }
+    if (sel && before < cap) { idx[before] = r; labels_c[before] = labels[src]; }
     __syncthreads();
     if (threadIdx.x == 0) carry += wsum[31];
     __syncthreads();
@@ -718,12 +722,23 @@ extern "C" vb_status vb_nce_region_loss(const float* scores, const float* target
   return check_launch("vb_nce_region_loss");
 }
 
+static vb_status compact_rows(const char* name, const int64_t* labels, int64_t ignore_index, const int32_t* map, int32_t rows, int32_t cap,
+                              int32_t* idx, int32_t* count, int64_t* labels_compact, void* stream) {
+  if (rows <= 0 || cap <= 0 || !labels || !idx || !count || !labels_compact) return set_error(VB_ERR_INVALID, "%s: bad arguments", name);
+  launch_pdl(compact_rows_kernel, dim3(1), dim3(1024), (size_t)0, static_cast<cudaStream_t>(stream), reinterpret_cast<const long long*>(labels),
+             (long long)ignore_index, map, (int)rows, (int)cap, idx, count, reinterpret_cast<long long*>(labels_compact));
+  return check_launch(name);
+}
+
 extern "C" vb_status vb_compact_rows(const int64_t* labels, int64_t ignore_index, int32_t rows, int32_t cap, int32_t* idx, int32_t* count,
                                      int64_t* labels_compact, void* stream) {
-  if (rows <= 0 || cap <= 0 || !labels || !idx || !count || !labels_compact) return set_error(VB_ERR_INVALID, "vb_compact_rows: bad arguments");
-  launch_pdl(compact_rows_kernel, dim3(1), dim3(1024), (size_t)0, static_cast<cudaStream_t>(stream), reinterpret_cast<const long long*>(labels),
-             (long long)ignore_index, (int)rows, (int)cap, idx, count, reinterpret_cast<long long*>(labels_compact));
-  return check_launch("vb_compact_rows");
+  return compact_rows("vb_compact_rows", labels, ignore_index, nullptr, rows, cap, idx, count, labels_compact, stream);
+}
+
+extern "C" vb_status vb_compact_rows_mapped(const int64_t* labels, int64_t ignore_index, const int32_t* map, int32_t rows, int32_t cap,
+                                            int32_t* idx, int32_t* count, int64_t* labels_compact, void* stream) {
+  if (!map) return set_error(VB_ERR_INVALID, "vb_compact_rows_mapped: no row map");
+  return compact_rows("vb_compact_rows_mapped", labels, ignore_index, map, rows, cap, idx, count, labels_compact, stream);
 }
 
 extern "C" vb_status vb_gather_rows16(const void* src, void* dst, const void* src2, void* dst2, const int32_t* idx, int32_t cap, int32_t cols,

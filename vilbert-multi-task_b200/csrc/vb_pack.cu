@@ -137,6 +137,48 @@ __global__ void zero_tail_rows_kernel(uint8_t* __restrict__ a, uint8_t* __restri
   }
 }
 
+// Whether a pre-training batch can be packed, in one small buffer read back with one copy (layout: vb_pack_summary in
+// include/vilbert_b200.h). One CTA, a
+// thread per sample. A sample's mask is prefix-valid and non-empty when it has n >= 1 valid entries and the last one sits at n - 1.
+// A NULL mask is all valid; NULL labels count nothing.
+constexpr int SUMMARY_THREADS = 256;
+
+__global__ void __launch_bounds__(SUMMARY_THREADS) pack_summary_kernel(const long long* __restrict__ mt, const long long* __restrict__ mv, int B,
+                                                                       int Nt, int Nv, const long long* __restrict__ lm,
+                                                                       const long long* __restrict__ il, int* __restrict__ out) {
+  pdl_entry();
+  __shared__ int total[5];
+  if (threadIdx.x < 5) total[threadIdx.x] = 0;
+  __syncthreads();
+  int bad_t = 0, bad_v = 0, lab_t = 0, lab_v = 0, n_lab = 0;
+  for (int b = threadIdx.x; b < B; b += SUMMARY_THREADS) {
+    int n = 0, last = -1;
+    for (int j = 0; j < Nt; ++j) {
+      const long long e = (long long)b * Nt + j;
+      const bool on = !mt || mt[e] != 0;
+      if (on) { ++n; last = j; }
+      if (lm && lm[e] != -1) { ++n_lab; lab_t += !on; }
+    }
+    out[b] = n;
+    bad_t += n == 0 || last != n - 1;
+    n = 0; last = -1;
+    for (int j = 0; j < Nv; ++j) {
+      const bool on = !mv || mv[(long long)b * Nv + j] != 0;
+      if (on) { ++n; last = j; }
+      if (il && j > 0 && il[(long long)b * (Nv - 1) + j - 1] == 1) lab_v += !on;    // image_label covers regions 1 .. Nv - 1
+    }
+    out[B + b] = n;
+    bad_v += n == 0 || last != n - 1;
+  }
+  if (bad_t) atomicAdd(&total[0], bad_t);
+  if (bad_v) atomicAdd(&total[1], bad_v);
+  if (lab_t) atomicAdd(&total[2], lab_t);
+  if (lab_v) atomicAdd(&total[3], lab_v);
+  if (n_lab) atomicAdd(&total[4], n_lab);
+  __syncthreads();
+  if (threadIdx.x < 5) out[2 * B + threadIdx.x] = total[threadIdx.x];
+}
+
 static inline int grid_for(long long n) {
   long long blocks = (n + 255) / 256, cap = (long long)sm_count() * 8;
   if (cap <= 0) cap = 132 * 8;
@@ -201,4 +243,13 @@ extern "C" vb_status vb_zero_tail_rows(void* a, void* b, void* c, int64_t ld_byt
   launch_pdl(zero_tail_rows_kernel, dim3(grid_for((long long)rows * (row_bytes / 16))), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream),
              static_cast<uint8_t*>(a), static_cast<uint8_t*>(b), static_cast<uint8_t*>(c), (long long)ld_bytes, (int)row_bytes, first, (int)rows);
   return check_launch("vb_zero_tail_rows");
+}
+
+extern "C" vb_status vb_pack_summary(const int64_t* text_mask, const int64_t* image_mask, int32_t B, int32_t Nt, int32_t Nv,
+                                     const int64_t* lm_labels, const int64_t* image_label, int32_t* out, void* stream) {
+  if (B <= 0 || Nt <= 0 || Nv <= 1 || !out) return set_error(VB_ERR_INVALID, "vb_pack_summary: bad arguments");
+  launch_pdl(pack_summary_kernel, dim3(1), dim3(SUMMARY_THREADS), (size_t)0, static_cast<cudaStream_t>(stream),
+             reinterpret_cast<const long long*>(text_mask), reinterpret_cast<const long long*>(image_mask), (int)B, (int)Nt, (int)Nv,
+             reinterpret_cast<const long long*>(lm_labels), reinterpret_cast<const long long*>(image_label), out);
+  return check_launch("vb_pack_summary");
 }

@@ -40,8 +40,11 @@ BASE_BERT_OUT_NAMES = ("sequence_output", "pooled_output")
 # the float inputs a plan can backpropagate into (Plan(input_grads=...)): the region features and their boxes
 INPUT_GRAD_NAMES = ("input_imgs", "image_loc")
 # heads a packed plan (Plan(packed=...)) can build: the pooled heads and the per-region logit, which it scatters back to the padded
-# layout; the per-token and per-region prediction heads of pre-training are not packed
+# layout. The prediction heads of pre-training are packed only inside the fused objective (loss="pretraining", loss_in_forward=True):
+# the masked-LM head compacts its labelled rows through the text row map, the region head scatters its rows to the padded layout
 PACKED_HEADS = ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_prediction", "vil_tri_prediction", "vision_logit")
+# config options packed plans refuse: they reshape or export the padded streams
+PACK_REFUSED_CONFIG = ("in_batch_pairs", "fast_mode", "dynamic_attention", "visualization")
 # the value a masked region's logit takes in a packed plan: the reference's additive mask, which in fp32 is no further from it
 # (BCE-with-logits at target 0 of either is 0.0 with gradient 0.0)
 PACKED_MASKED_LOGIT = -10000.0
@@ -56,6 +59,59 @@ def pack_capacity(count, padded_rows):
         raise ValueError("a packed stream needs at least one valid row")
     step = max(128, -(-padded_rows // 16 // 128) * 128)
     return min(-(-count // step) * step, padded_rows)
+
+
+def prefix_lengths(mask):
+    """Valid length per row of a 0/1 host mask [rows, N], or None when some row is not prefix-valid (a 0 before a 1) or has no 1."""
+    m = mask.ne(0)
+    n = m.sum(1)
+    ok = bool((n >= 1).all()) and bool(m.eq(torch.arange(m.size(1)).unsqueeze(0) < n.unsqueeze(1)).all())
+    return n if ok else None
+
+
+def check_pack_config(cfg):
+    """engine.pack_padding with a config option packed plans refuse (PACK_REFUSED_CONFIG) raises NotImplementedError."""
+    bad = [f for f in PACK_REFUSED_CONFIG if getattr(cfg, f, False)]
+    if bad:
+        raise NotImplementedError(f"engine.pack_padding does not support config.{bad[0]}")
+
+
+def pretraining_pack_rows(attention_mask, image_attention_mask, masked_lm_labels, image_label, B, Nt, Nv):
+    """Host decision of a packed pre-training step from host tensors (None: a mask of all ones, labels that select nothing), with
+    no device read: (rows_t, rows_v) of the packed plan, or the reason the batch runs padded. "mask": a mask is not prefix-valid
+    or has an empty row; "label": a token with masked_lm_labels != -1 sits where attention_mask == 0, or a region with
+    image_label == 1 (image_label covers regions 1 .. Nv - 1) where image_attention_mask == 0 — the padded loss reads those rows."""
+    mt = torch.ones(B, Nt, dtype=I64) if attention_mask is None else attention_mask.reshape(B, Nt)
+    mv = torch.ones(B, Nv, dtype=I64) if image_attention_mask is None else image_attention_mask.reshape(B, Nv)
+    lt, lv = prefix_lengths(mt), prefix_lengths(mv)
+    if lt is None or lv is None:
+        return "mask"
+    if masked_lm_labels is not None and bool((masked_lm_labels.reshape(B, Nt).ne(-1) & mt.eq(0)).any()):
+        return "label"
+    if image_label is not None and bool((image_label.reshape(B, Nv - 1).eq(1) & mv[:, 1:].eq(0)).any()):
+        return "label"
+    return pack_capacity(int(lt.sum()), B * Nt), pack_capacity(int(lv.sum()), B * Nv)
+
+
+def pack_summary(attention_mask, image_attention_mask, masked_lm_labels, image_label, B, Nt, Nv):
+    """vb_pack_summary of device-resident masks and labels (None as in pretraining_pack_rows) on the current stream, read back with
+    one device-to-host copy: the host waits for the stream here. -> int32 host tensor [2B + 5] (layout: include/vilbert_b200.h)."""
+    dev = next(t.device for t in (attention_mask, image_attention_mask, masked_lm_labels, image_label) if t is not None and t.is_cuda)
+    as_dev = lambda t: None if t is None else t.to(device=dev, dtype=I64, non_blocking=True).contiguous()
+    ins = [as_dev(t) for t in (attention_mask, image_attention_mask, masked_lm_labels, image_label)]
+    out = torch.empty(2 * B + 5, dtype=torch.int32, device=dev)
+    L.call(L.lib().vb_pack_summary, ins[0], ins[1], B, Nt, Nv, ins[2], ins[3], out)
+    return out.cpu()
+
+
+def pretraining_pack_rows_from_summary(summary, B, Nt, Nv):
+    """The decision of pretraining_pack_rows from a vb_pack_summary result (pack_summary)."""
+    s = summary.tolist()
+    if s[2 * B] or s[2 * B + 1]:
+        return "mask"
+    if s[2 * B + 2] or s[2 * B + 3]:
+        return "label"
+    return pack_capacity(sum(s[:B]), B * Nt), pack_capacity(sum(s[B:2 * B]), B * Nv)
 
 
 def _pad8(n):
@@ -521,7 +577,9 @@ class Plan:
 
     def _check_packed(self, outputs):
         """packed=(rows_t, rows_v): the two streams hold the valid rows only (DESIGN.md §4g). Refused with the options that reshape
-        or export the padded streams, with input gradients (they are padded tensors) and with heads that are not packed."""
+        or export the padded streams, with input gradients (they are padded tensors) and with heads that are not packed: the heads
+        of VILBertForVLTasks among PACKED_HEADS (outputs=), or the three heads of BertForMultiModalPreTraining under the fused
+        objective with its losses in the forward (loss="pretraining", loss_in_forward=True, engine.lm_compact, all three heads)."""
         rows_t, rows_v = self.packed
         if rows_t < 1 or rows_v < 1 or rows_t > self.B * self.Nt or rows_v > self.B * self.Nv:
             raise ValueError(f"packed={self.packed}: the rows of each stream must lie in [1, B * N] = [1, {self.B * self.Nt}], "
@@ -531,6 +589,12 @@ class Plan:
                if on]
         if bad:
             raise NotImplementedError(f"packed plans do not support {', '.join(bad)}")
+        if self.heads == "pretraining":
+            if not (self.loss_kind == "pretraining" and self.loss_in_forward and self.e.lm_compact and
+                    (outputs is None or frozenset(outputs) == frozenset(PRETRAINING_HEAD_NAMES))):
+                raise NotImplementedError("packed pre-training plans run the fused objective only: loss='pretraining', "
+                                          "loss_in_forward=True, engine.lm_compact and all three heads")
+            return
         if (self.e.ps.heads != "vl") or outputs is None or any(n not in PACKED_HEADS for n in outputs):
             raise NotImplementedError(f"packed plans build heads of VILBertForVLTasks among {PACKED_HEADS} only (outputs=...), got "
                                       f"{None if outputs is None else sorted(outputs)}")
@@ -1380,12 +1444,13 @@ class Plan:
             self.gout[name] = self.buf(shape, F32, zero=True)
         return self.gout[name]
 
-    def big_head(self, name, x, ld_x, M, K_in, N_out, wname, bias_name, w=None, gw_name=None):
+    def big_head(self, name, x, ld_x, M, K_in, N_out, wname, bias_name, w=None, gw_name=None, dl32=None):
         """Wide linear head (N_out in the thousands): logits = x W^T + b as fp32 [M, N_out]; backward from a
         caller-supplied fp32 d(logits), cast to a bf16 operand with an 8-padded row pitch unless the objective registered one it
         writes itself (self.head_dl16). w / gw_name: a weight and the entry of
-        its gradient not named by `wname` (the decoder tied to the word embeddings). The backward returns None when nothing
-        below the logits takes a gradient."""
+        its gradient not named by `wname` (the decoder tied to the word embeddings). dl32: the buffer the backward reads d(logits)
+        from when it is not the output-gradient buffer of `name` (a packed head, whose output is the padded layout). The backward
+        returns None when nothing below the logits takes a gradient."""
         ps = self.ps
         W = w if w is not None else ps.w(wname + ".weight")
         wkey = gw_name if gw_name is not None else wname + ".weight"
@@ -1398,13 +1463,13 @@ class Plan:
             if name not in self.grad_outputs or not self.out_rg[name]:
                 return None
             ldp = _pad8(N_out)
-            dl32, dl16 = self.out_grad_buffer(name, (M, N_out)), self.head_dl16.get(name)
+            dl, dl16 = self.out_grad_buffer(name, (M, N_out)) if dl32 is None else dl32, self.head_dl16.get(name)
             if dl16 is None:
                 dl16 = self.scratch("head.dl16." + name, (M, ldp), BF16)
-                self.emit(self.lib.vb_cast2d_f32_to_bf16, dl32, N_out, dl16, ldp, M, N_out, 1.0)
+                self.emit(self.lib.vb_cast2d_f32_to_bf16, dl, N_out, dl16, ldp, M, N_out, 1.0)
             gb = self.pg(bias_name)
             if gb is not None:
-                self.colsum(dl32, N_out, gb, M, N_out)
+                self.colsum(dl, N_out, gb, M, N_out)
             if gw_name is None:
                 self.linear_wgrad(dl16, ldp, x.op.bw, ld_x, M, N_out, K_in, wname)
             elif self.trainable(gw_name):
@@ -1428,15 +1493,21 @@ class Plan:
         """Masked-LM head of the fused pre-training objective without the [tokens, vocab] logits: the rows with a label
         (masked_lm_labels != -1, 15 % of the tokens; vilbert.py:1578-1583) are compacted on the device into a fixed-capacity
         operand (engine.lm_capacity of the rows), the tied decoder GEMM, the cross-entropy and both backward GEMMs run on those
-        rows, and the gradient is scattered back to the token rows. More labelled rows than the capacity poison the loss (NaN)."""
+        rows, and the gradient is scattered back to the token rows. More labelled rows than the capacity poison the loss (NaN).
+        Packed: the labels stay in the padded layout, the labelled packed rows are found through the text row map (in the order of
+        their padded rows), and the capacity is that of the padded rows, so both plans poison the loss under the same condition."""
         ps, c, lib = self.ps, self.cfg, self.lib
         M, Ht, V = ht.M, ht.H, c.vocab_size
-        cap = min(_pad8(M), _pad8(max(64, int(math.ceil(self.e.lm_capacity * M)))))
-        labels = self.buf((M,), I64, zero=True)      # a plan input (loaded from outside a run): private, never in the shared arena
+        M_pad = self.B * self.Nt if self.packed else M
+        cap = min(_pad8(M_pad), _pad8(max(64, int(math.ceil(self.e.lm_capacity * M_pad)))))
+        labels = self.buf((M_pad,), I64, zero=True)      # a plan input (loaded from outside a run): private, never in the shared arena
         labels.fill_(-1)
         self.loss_inputs["masked_lm_labels"] = labels
         idx, cnt, lab_c = self.buf((cap,), torch.int32), self.buf((1,), torch.int32, zero=True), self.buf((cap,), I64)
-        self.emit(lib.vb_compact_rows, labels, -1, M, cap, idx, cnt, lab_c)
+        if self.packed:
+            self.emit(lib.vb_compact_rows_mapped, labels, -1, self.map_t, M, cap, idx, cnt, lab_c)
+        else:
+            self.emit(lib.vb_compact_rows, labels, -1, M, cap, idx, cnt, lab_c)
         hc = self.gather_rows(ht.op, idx, cap, Ht)
         wn = "bert.embeddings.word_embeddings.weight"
         logits = self.buf((cap, V), F32)
@@ -1541,6 +1612,25 @@ class Plan:
                       self.pg(name + ".weight"), self.pg(name + ".bias"), M, K, 1, in_drop)
         self.push_bwd(bwd, self.out_rg[name])
 
+    def packed_vision_prediction(self, hv):
+        """The region decoder of a packed plan: the [rows_v, C] logits of the packed region rows, scattered to the padded
+        [B * Nv, C] layout (0 on the masked regions, which no region objective reads), so the KL / MSE / NCE kernels run as in the
+        padded plan. Its backward gathers the padded gradient back to the packed rows before the decoder's backward (big_head)."""
+        lib, B, Nv, C_, name = self.lib, self.B, self.Nv, self.cfg.v_target_size, "vision_prediction"
+        M, K = hv.M, hv.H
+        dl = self.buf((M, C_), F32) if name in self.grad_outputs else None
+        head_bwd = self.big_head(name, hv, K, M, K, C_, "cls.imagePredictions.decoder", "cls.imagePredictions.decoder.bias", dl32=dl)
+        off, ln = self.seg["v"]
+        out = self.buf((B * Nv, C_), F32)
+        self.emit(lib.vb_unpack_rows_f32, self.outputs[name], out, off, ln, B, Nv, C_, 0.0)
+        self.outputs[name] = out
+
+        def bwd():
+            if name in self.grad_outputs and self.out_rg[name]:
+                self.emit(lib.vb_pack_rows_f32, self.out_grad_buffer(name, (B * Nv, C_)), dl, self.map_v, M, C_)
+            return head_bwd()
+        return bwd
+
     def build_heads(self, seq_t, seq_v, pooled_t, pooled_v):
         """VILBertForVLTasks.forward after self.bert (vilbert.py:1673-1708) + BertPreTrainingHeads (:1228-1243).
         Dropout layers are identity (eval-mode / p = 0 parity protocol)."""
@@ -1590,8 +1680,11 @@ class Plan:
                                        w=ps.w("bert.embeddings.word_embeddings.weight"), gw_name="bert.embeddings.word_embeddings.weight")
         if want("vision_prediction"):
             hv, hv_bwd = self.transform(seq_v, "cls.imagePredictions.transform.dense", "cls.imagePredictions.transform.LayerNorm", "im.tr")
-            im_bwd = self.big_head("vision_prediction", hv, Hv, B * Nv, Hv, c.v_target_size, "cls.imagePredictions.decoder",
-                                   "cls.imagePredictions.decoder.bias")
+            if self.packed:
+                im_bwd = self.packed_vision_prediction(hv)
+            else:
+                im_bwd = self.big_head("vision_prediction", hv, Hv, B * Nv, Hv, c.v_target_size, "cls.imagePredictions.decoder",
+                                       "cls.imagePredictions.decoder.bias")
         if want("linguisic_prediction"):
             self.push_bwd(self._wide_bwd(lm_bwd, ht, ht_bwd, Ht, c.vocab_size) if lm_bwd is not None else lm_compact_bwd)
         if want("vision_prediction"):

@@ -14,7 +14,8 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib as L
 from .config import BertConfig
-from .engine import BERT_OUT_NAMES, HEAD_NAMES, INPUT_GRAD_NAMES, LOSS_HEADS, PRETRAINING_HEAD_NAMES, Engine
+from .engine import (BERT_OUT_NAMES, HEAD_NAMES, INPUT_GRAD_NAMES, LOSS_HEADS, PRETRAINING_HEAD_NAMES, Engine, check_pack_config, pack_summary,
+                     pretraining_pack_rows, pretraining_pack_rows_from_summary)
 
 
 # Any torch.optim.Optimizer.step() (pytorch_transformers.AdamW and the reference's RAdam subclass it) may have rewritten
@@ -524,7 +525,11 @@ class BertForMultiModalPreTraining(BertPreTrainedModel):
     kernels at the end of the forward (Plan(loss="pretraining", loss_in_forward=True)); no head output is cloned and the tied
     decoder runs on the labelled token rows only. The losses come back as [1]-shaped CUDA tensors whose backward scales each head
     gradient by its own d(total)/d(loss) on the device. Unlike the torch path, more labelled tokens than engine.lm_capacity of the
-    rows make the masked-LM loss NaN."""
+    rows make the masked-LM loss NaN.
+
+    With engine.pack_padding set, such a call runs on a packed plan (Plan(packed=...), DESIGN.md §4g): the encoder and the three
+    heads see the valid tokens and regions only, and the losses and gradients are those of the padded step up to fp32 summation
+    order (_packed_rows says which batches pack)."""
     _heads = "pretraining"
 
     def __init__(self, config, device=None, precision=None, fused_objective=False):
@@ -595,6 +600,31 @@ class BertForMultiModalPreTraining(BertPreTrainedModel):
             sampler = getattr(self, "nce_sampler", None)
             targets["neg_index"] = sampler(B, R, image_feat.device) if sampler is not None else self._nce_negatives(B, R, image_feat.device)
         B, Nv, Nt = image_feat.shape[0], image_feat.shape[1], input_ids.shape[1]
+        input_grads = self._input_grads(inputs)
+        packed = self._packed_rows(attention_mask, image_attention_mask, masked_lm_labels, image_label, B, Nt, Nv, input_grads)
         plan = self.engine.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS["pretraining"] if torch.is_grad_enabled() else (), train=bool(self.training),
-                                loss="pretraining", loss_in_forward=True, frozen=self._frozen(), input_grads=self._input_grads(inputs))
+                                loss="pretraining", loss_in_forward=True, frozen=self._frozen(), input_grads=input_grads, packed=packed)
         return self._call(plan, inputs, targets)
+
+    def _packed_rows(self, attention_mask, image_attention_mask, masked_lm_labels, image_label, B, Nt, Nv, input_grads):
+        """(rows_t, rows_v) of the packed plan of a fused call when engine.pack_padding is set and the batch can be packed, else None;
+        a batch that cannot is counted in engine.pack_fallbacks by reason (engine.pretraining_pack_rows). Host masks and labels
+        are decided on the host with no device read. When any of them is on the device, one vb_pack_summary launch decides and one
+        device-to-host copy reads its result: the host then waits for the work queued so far, once per forward."""
+        eng = self.engine
+        if not eng.pack_padding:
+            return None
+        check_pack_config(self.config)
+        if not eng.lm_compact:
+            raise NotImplementedError("engine.pack_padding packs the compacted masked-LM head only: set engine.lm_compact")
+        if input_grads:
+            raise NotImplementedError("engine.pack_padding does not compute input gradients (they are padded tensors)")
+        ts = (attention_mask, image_attention_mask, masked_lm_labels, image_label)
+        if any(t is not None and t.is_cuda for t in ts):
+            rows = pretraining_pack_rows_from_summary(pack_summary(*ts, B, Nt, Nv), B, Nt, Nv)
+        else:
+            rows = pretraining_pack_rows(*ts, B, Nt, Nv)
+        if isinstance(rows, str):
+            eng.pack_fallbacks[rows] += 1
+            return None
+        return rows

@@ -20,7 +20,7 @@ import torch
 import torch.nn as nn
 
 from .data import expand_batch
-from .engine import LOSS_HEADS, MC_REGION_OFFSET, RESULT_MODES, pack_capacity
+from .engine import LOSS_HEADS, MC_REGION_OFFSET, RESULT_MODES, check_pack_config, pack_capacity, prefix_lengths
 from .modeling import _PlanCall, _PlanFn
 
 LossMap = {
@@ -83,17 +83,6 @@ def _unpack(task_id, batch):
     return features, spatials, image_mask, question, target, input_mask, segment_ids, mc_ids, co_attention_mask
 
 
-_PACK_REFUSED = ("in_batch_pairs", "fast_mode", "dynamic_attention", "visualization")
-
-
-def _prefix_lengths(mask):
-    """Valid length per row of a 0/1 mask [rows, N], or None when some row is not prefix-valid (a 0 before a 1) or has no 1."""
-    m = mask.ne(0)
-    n = m.sum(1)
-    ok = bool((n >= 1).all()) and bool(m.eq(torch.arange(m.size(1)).unsqueeze(0) < n.unsqueeze(1)).all())
-    return n if ok else None
-
-
 def packed_rows(model, task_cfg, task_id, batch, processes):
     """The (rows_t, rows_v) capacities of a packed plan for this batch when model.engine.pack_padding is set and the batch can be
     packed, else None. Decided from the host tensors before the batch moves, so it forces no sync. The masks are replicated as the
@@ -107,9 +96,7 @@ def packed_rows(model, task_cfg, task_id, batch, processes):
     if not eng.pack_padding:
         return None
     cfg = eng.cfg
-    bad = [f for f in _PACK_REFUSED if getattr(cfg, f, False)]
-    if bad:
-        raise NotImplementedError(f"engine.pack_padding does not support config.{bad[0]}")
+    check_pack_config(cfg)
 
     def fallback(reason):
         eng.pack_fallbacks[reason] += 1
@@ -122,7 +109,7 @@ def packed_rows(model, task_cfg, task_id, batch, processes):
     if process in processes:     # the masks as expand_batch lays them out (a one-wide stand-in for the features and boxes)
         stand_in = image_mask.unsqueeze(-1)
         _, _, image_mask, _, input_mask, _, _, _, _ = expand_batch(process, stand_in, stand_in, image_mask, question, input_mask, input_mask)
-    lt, lv = _prefix_lengths(input_mask), _prefix_lengths(image_mask)
+    lt, lv = prefix_lengths(input_mask), prefix_lengths(image_mask)
     if lt is None or lv is None:
         return fallback("mask")
     kind = task_kind(task_cfg, task_id)
