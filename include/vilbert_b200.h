@@ -107,7 +107,7 @@ typedef struct vb_gemm_args {
   int64_t ld_out_bf16;
   void* out_pre;         /* bf16 gelu'(pre-activation) (GELU) or NULL */
   int64_t ld_out_pre;
-  int32_t atomic_out;    /* 0 store, 1 red.add into out_f32 */
+  int32_t atomic_out;    /* 0 store, 1 red.add into out_f32, VB_GEMM_PARTIALS: split s stores into rows [s*M, s*M + M) of out_f32 */
   float* out_colsum;     /* [N] or NULL: += column sums of the epilogue value before the residual add (bias gradients) */
   vb_dropout_site dropout;    /* applied to the epilogue value before the residual add (index m*N + n): LN(dropout(dense(x)) + res) */
   int32_t split_k;       /* >= 1; > 1 requires atomic_out and no act / bf16 outputs */
@@ -592,6 +592,47 @@ vb_status vb_tanh_fwd(const float* x, float* y_f32, void* y16, void* y_lo, void*
 vb_status vb_tanh_bwd(const float* dy, const float* y, void* dx_bf16, float* dbias, int32_t M, int32_t N, void* stream);
 /* out [B, Nt+Nv] = cat((1 - mask_t) * -10000, (1 - mask_v) * -10000) (basebert.py:723-750); masks int64 0/1. */
 vb_status vb_mask_concat_additive(const int64_t* mask_t, const int64_t* mask_v, float* out, int32_t B, int32_t Nt, int32_t Nv, void* stream);
+
+/* ---- deterministic variants (plans built under torch.use_deterministic_algorithms(True), DESIGN.md §4h)
+ * Each replaces the float atomics of its default entry point by per-block partial sums in a caller-owned fp32 workspace `ws`
+ * followed by one ordered sum (vb_reduce_slices), with block counts that depend on the shape only: two runs on the same GPU model
+ * and build give bitwise identical results. Arguments are those of the default entry point, plus ws.
+ *
+ * vb_gemm_bf16 with atomic_out = VB_GEMM_PARTIALS (weight gradients): split s of the k dimension stores its fp32 tile into rows
+ * [s*M, s*M + M) of out_f32 (pitch ld_out_f32), a workspace of split_k * M rows; split_k must be the value vb_gemm_plan resolves for
+ * the same arguments. The caller then adds the slices to the gradient with vb_reduce_slices. */
+#define VB_GEMM_PARTIALS 2
+#define VB_DET_SLICES 64          /* row blocks of vb_colsum_det / vb_loc_proj_bwd_det, CTAs of vb_small_linear_bwd_det, at most */
+#define VB_DET_LN_SLICES 256      /* CTAs of vb_layernorm_bwd_det, at most */
+#define VB_DET_LOSS_SLICES 1024   /* CTAs of the _det losses, at most */
+/* dst[i] += part[0*stride + i] + part[1*stride + i] + ... + part[(slices-1)*stride + i], summed in slice order, i < n */
+vb_status vb_reduce_slices(const float* part, int64_t stride, int32_t slices, int64_t n, float* dst, void* stream);
+/* vb_colsum: ws holds VB_DET_SLICES * N floats */
+vb_status vb_colsum_det(const void* X, int32_t is_bf16, int64_t ld, float* out, int32_t M, int32_t N, float* ws, void* stream);
+/* vb_layernorm_bwd (dy2 == NULL) and vb_add_layernorm_bwd: ws holds 3 * VB_DET_LN_SLICES * H floats (unused when no sum is asked) */
+vb_status vb_layernorm_bwd_det(const float* dy, const float* dy2, int64_t lddy, const float* x, int64_t ldx, const float* gamma,
+                               const float* mean, const float* rstd, float* dx_f32, void* dx_bf16, int64_t lddx, const void* gelu_pre,
+                               int64_t ld_pre, float* dgamma, float* dbeta, float* dbias, int32_t M, int32_t H,
+                               const vb_dropout* out_dropout, const vb_dropout* in_dropout, float* ws, void* stream);
+/* vb_embed_text_bwd without a workspace: each table row that takes a gradient is summed by one warp over the rows that select it,
+ * in row order, and written once (H <= 1024) */
+vb_status vb_embed_text_bwd_det(const float* dout, const int64_t* ids, const int64_t* token_type_ids, const int64_t* task_ids,
+                                float* dword, float* dpos, float* dtype, float* dtask, int32_t B, int32_t Nt, int32_t H, void* stream);
+/* vb_loc_proj_bwd: ws holds VB_DET_SLICES * 6 * H floats */
+vb_status vb_loc_proj_bwd_det(const float* dy, const float* loc, float* dW, float* db, int32_t M, int32_t H, float* ws, void* stream);
+/* vb_small_linear_bwd: ws holds VB_DET_SLICES * (N * K + N) floats */
+vb_status vb_small_linear_bwd_det(const float* dy, const float* x, int64_t ldx, const float* W, float* dx, int64_t lddx,
+                                  int32_t accumulate_dx, float* dW, float* db, int32_t M, int32_t K, int32_t N,
+                                  const vb_dropout* in_dropout, float* ws, void* stream);
+/* the losses: ws holds VB_DET_LOSS_SLICES floats */
+vb_status vb_bce_logits_loss_det(const float* logits, const float* target, float* loss, float* dlogits_f32, void* dlogits_bf16,
+                                 int64_t ld_dlogits_bf16, int32_t rows, int32_t cols, float grad_scale, float* ws, void* stream);
+vb_status vb_ce_loss_det(const float* logits, int64_t ld_logits, const int64_t* labels, int64_t ignore_index, float* loss,
+                         float* dlogits_f32, int64_t ld_d32, void* dlogits_bf16, int64_t ld_d16, int32_t rows, int32_t cols,
+                         float grad_scale, int32_t accumulate_loss, float* ws, void* stream);
+vb_status vb_kl_masked_loss_det(const float* scores, const float* target, const int64_t* label, float* loss, float* dscores_f32,
+                                void* dscores_bf16, int64_t ld_d16, int32_t B, int32_t Nv, int32_t C, float grad_scale,
+                                int32_t accumulate_loss, float* ws, void* stream);
 
 #ifdef __cplusplus
 }

@@ -158,6 +158,13 @@ def packed_pretraining_cases(E):
     ]
 
 
+def deterministic_cases(O, E, base_labels):
+    """The two-stream cases of every matrix above with deterministic=True (named det_...)."""
+    every = (cases(O, E, base_labels) + input_grad_cases(O, E, base_labels) + packed_cases(E) + packed_pretraining_cases(E))
+    return [(f"det_{name}", over, heads, B, dict(kw, deterministic=True), *extra)
+            for name, over, heads, B, kw, *extra in every if not heads.startswith("base")]
+
+
 def dump_cases(out, case_list, prec, Engine, BertConfig, tiny, tiny_base):
     """Lists every plan of `case_list` in precision `prec`, without and with the shared activation arena. -> (plans, op records)"""
     n_plans = n_ops = 0
@@ -306,6 +313,12 @@ def main():
     if hasattr(E, "pretraining_pack_rows"):
         for prec in PRECISIONS:
             p, o = dump_cases(out, packed_pretraining_cases(E), prec, Engine, BertConfig, tiny, tiny_base)
+            n_plans, n_ops = n_plans + p, n_ops + o
+    # deterministic plans (torch.use_deterministic_algorithms(True)): every two-stream case above again with deterministic=True,
+    # listed last, so that the listing of a tree without them is a prefix of this one (the baseline refuses them)
+    if hasattr(E, "DET_WORKSPACE"):
+        for prec in PRECISIONS:
+            p, o = dump_cases(out, deterministic_cases(O, E, tiny_base["num_labels"]), prec, Engine, BertConfig, tiny, tiny_base)
             n_plans, n_ops = n_plans + p, n_ops + o
     text = "\n".join(out) + "\n"
     if a.out:

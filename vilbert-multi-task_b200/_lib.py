@@ -153,9 +153,21 @@ _SIGNATURES = {
     "vb_scatter_add_rows_f32": [_P, _P, _P, _I32, _I32, _P],
     "vb_zero_tail_rows": [_P, _P, _P, _I64, _I32, _P, _I32, _P],
     "vb_pack_summary": [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P],
+    "vb_reduce_slices": [_P, _I64, _I32, _I64, _P, _P],
+    "vb_colsum_det": [_P, _I32, _I64, _P, _I32, _I32, _P, _P],
+    "vb_layernorm_bwd_det": [_P, _P, _I64, _P, _I64, _P, _P, _P, _P, _P, _I64, _P, _I64, _P, _P, _P, _I32, _I32, _P, _P, _P, _P],
+    "vb_embed_text_bwd_det": [_P, _P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _P],
+    "vb_loc_proj_bwd_det": [_P, _P, _P, _P, _I32, _I32, _P, _P],
+    "vb_small_linear_bwd_det": [_P, _P, _I64, _P, _P, _I64, _I32, _P, _P, _I32, _I32, _I32, _P, _P, _P],
+    "vb_bce_logits_loss_det": [_P, _P, _P, _P, _P, _I64, _I32, _I32, _F, _P, _P],
+    "vb_ce_loss_det": [_P, _I64, _P, _I64, _P, _P, _I64, _P, _I64, _I32, _I32, _F, _I32, _P, _P],
+    "vb_kl_masked_loss_det": [_P, _P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _F, _I32, _P, _P],
 }
 # device scratch of one vb_weight_norm_fwd / _bwd launch (include/vilbert_b200.h)
 VB_WEIGHT_NORM_SCRATCH = 1024
+# deterministic variants (include/vilbert_b200.h): the partials mode of vb_gemm_bf16 and the workspace slices of the _det entry points
+VB_GEMM_PARTIALS = 2
+VB_DET_SLICES, VB_DET_LN_SLICES, VB_DET_LOSS_SLICES = 64, 256, 1024
 
 _lib = None
 

@@ -97,7 +97,8 @@ enum { EPI_F32 = 0,     // v = alpha*acc (+bias) (ReLU) (+fp32 residual) -> out_
        EPI_DGELU = 3,   // v = acc * aux (aux = saved gelu'(pre)) -> out_bf16 (+ column sums)
        EPI_ATOMIC = 4,  // red.global.add.v4.f32 into out_f32 (split-K wgrad)
        EPI_GENERIC = 5, // runtime flags only (ReLU poolers, unusual output combinations)
-       EPI_COUNT = 6 };
+       EPI_PARTIAL = 6, // deterministic split-K wgrad: split s stores its fp32 tile into rows [s*M, s*M + M) of out_f32 (a workspace)
+       EPI_COUNT = 7 };
 
 // Generic, compact (non-unrolled) path: any flags, any alignment, ragged rows / columns.
 __device__ __noinline__ void epi_generic_chunk(const GemmKernelParams& p, const float* stg, int m_base, int n, int rr, int cc) {
@@ -141,6 +142,20 @@ __device__ __noinline__ void epi_generic_chunk(const GemmKernelParams& p, const 
   if (p.out_colsum) {
 #pragma unroll 1
     for (int j = 0; j < nv; ++j) atomicAdd(p.out_colsum + n + j, cs[j]);
+  }
+}
+
+// Ragged chunks of EPI_PARTIAL: plain stores of alpha * acc into the split's slice (row m + slice_row), bounds-checked.
+__device__ __noinline__ void epi_partial_chunk(const GemmKernelParams& p, const float* stg, int m_base, int n, int rr, int cc, long long slice_row) {
+  const int nv = min(4, p.N - n);
+  if (nv <= 0) return;
+#pragma unroll 1
+  for (int ps = 0; ps < EPI_PS; ++ps) {
+    const int row = ps * 4 + rr;
+    const long long m = m_base + row;
+    if (m >= p.M) break;
+#pragma unroll 1
+    for (int j = 0; j < nv; ++j) p.out_f32[(m + slice_row) * p.ld_of + n + j] = stg[stg_off(row, cc + j)] * p.alpha;
   }
 }
 
@@ -230,6 +245,8 @@ __device__ __forceinline__ void epi_fast_chunk(const GemmKernelParams& p, const 
       store16x4<OUT16>(p, m * p.ld_ob + n, v0, v1, v2, v3);
     } else if (EPI == EPI_ATOMIC) {
       asm volatile("red.global.v4.f32.add [%0], {%1, %2, %3, %4};" ::"l"(p.out_f32 + m * p.ld_of + n), "f"(v0), "f"(v1), "f"(v2), "f"(v3) : "memory");
+    } else if (EPI == EPI_PARTIAL) {   // m already points into the split's slice
+      *reinterpret_cast<float4*>(p.out_f32 + m * p.ld_of + n) = make_float4(v0, v1, v2, v3);
     }
   }
   if (EPI == EPI_DGELU && p.out_colsum) {
@@ -475,7 +492,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           for (int c2 = 0; c2 < NC; ++c2)
             if (c2 == c) stage_chunk(acc[c2 >> 2], c2 & 3, stg, lane);
           __syncwarp();
-          if (EPI == EPI_F32 && p.act == VB_ACT_RELU && fast) epi_pool_chunk(p, stg, m_base, n, rr, cc, b4);
+          if (EPI == EPI_PARTIAL) {
+            if (fast) epi_fast_chunk<EPI, OUT16>(p, stg, m_base + split * p.M, n, rr, cc, resv, auxv, b4);
+            else      epi_partial_chunk(p, stg, m_base, n, rr, cc, (long long)split * p.M);
+          }
+          else if (EPI == EPI_F32 && p.act == VB_ACT_RELU && fast) epi_pool_chunk(p, stg, m_base, n, rr, cc, b4);
           else if (fast) epi_fast_chunk<EPI, OUT16>(p, stg, m_base, n, rr, cc, resv, auxv, b4);
           else           epi_generic_chunk(p, stg, m_base, n, rr, cc);
           __syncwarp();
@@ -580,6 +601,7 @@ static int launch_gemm_epi(int epi, int out16, const CUtensorMap* tm, GemmKernel
       return launch_gemm<BN, EPI_GELU, CG, 0>(tm, p, work, max_ctas, stream);
     case EPI_DGELU: return launch_gemm<BN, EPI_DGELU, CG>(tm, p, work, max_ctas, stream);
     case EPI_ATOMIC: return launch_gemm<BN, EPI_ATOMIC, CG>(tm, p, work, max_ctas, stream);
+    case EPI_PARTIAL: return launch_gemm<BN, EPI_PARTIAL, CG>(tm, p, work, max_ctas, stream);
     default: return launch_gemm<BN, EPI_GENERIC, CG>(tm, p, work, max_ctas, stream);
   }
 }
@@ -668,6 +690,8 @@ extern "C" vb_status vb_gemm_bf16(const vb_gemm_args* a, void* stream_) {
   if (a->bias && !aligned(a->bias, 16)) return set_error(VB_ERR_INVALID, "vb_gemm_bf16: bias must be 16-byte aligned");
   if (a->atomic_out && (!a->out_f32 || a->out_bf16 || a->out_pre))
     return set_error(VB_ERR_INVALID, "vb_gemm_bf16: atomic_out supports only out_f32");
+  if (a->atomic_out != 0 && a->atomic_out != 1 && a->atomic_out != VB_GEMM_PARTIALS)
+    return set_error(VB_ERR_INVALID, "vb_gemm_bf16: atomic_out must be 0, 1 or VB_GEMM_PARTIALS");
   if ((a->A_lo && !aligned(a->A_lo, 16)) || (a->B_lo && !aligned(a->B_lo, 16)))
     return set_error(VB_ERR_INVALID, "vb_gemm_bf16: A_lo / B_lo must be 16-byte aligned");
   if ((a->out_lo || a->out_b16) && !a->out_bf16) return set_error(VB_ERR_INVALID, "vb_gemm_bf16: out_lo / out_b16 need out_bf16");
@@ -756,7 +780,13 @@ extern "C" vb_status vb_gemm_bf16(const vb_gemm_args* a, void* stream_) {
   int epi = EPI_GENERIC;
   const bool no_extra = !a->out_colsum;
   const bool has_drop = p.drop.ctr != nullptr;   // only the F32 specialisation (and the generic path) implement it
-  if (a->atomic_out) {
+  if (a->atomic_out == VB_GEMM_PARTIALS) {
+    // split s owns rows [s*M, s*M + M) of out_f32; the caller reduces them (vb_reduce_slices) and must know the split count
+    if (a->act != VB_ACT_NONE || a->bias || a->residual || !no_extra || has_drop || a->split_k != split_k)
+      return set_error(VB_ERR_INVALID, "vb_gemm_bf16: VB_GEMM_PARTIALS needs a plain epilogue and split_k as vb_gemm_plan resolves it "
+                       "(asked %d, resolved %d)", a->split_k, split_k);
+    epi = EPI_PARTIAL; p.fast_ok = p.vec_f32;
+  } else if (a->atomic_out) {
     if (a->act == VB_ACT_NONE && !a->bias && !a->residual && no_extra && !has_drop) { epi = EPI_ATOMIC; p.fast_ok = p.vec_f32; }
   } else if (a->act == VB_ACT_GELU) {
     if (a->out_pre && !a->residual && no_extra && !has_drop && (a->out_bf16 || a->out_f32)) {

@@ -13,6 +13,8 @@ inline int check_launch(const char* what) {
   return VB_OK;
 }
 int sm_count();
+// dst[i] += part[0 * stride + i] + part[1 * stride + i] + ... (slices terms, in slice order): the ordered sum of deterministic plans
+int launch_reduce_slices(const float* part, long long stride, int slices, long long n, float* dst, cudaStream_t stream);
 
 // Programmatic dependent launch (PDL): every kernel of the library starts with `griddepcontrol.wait` (all global
 // traffic happens after it) followed by `griddepcontrol.launch_dependents`, and is launched with

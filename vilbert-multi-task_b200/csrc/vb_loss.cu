@@ -48,10 +48,13 @@ __device__ __forceinline__ float block_count(const long long* labels, int n, flo
 
 // F.cross_entropy(logits [rows, cols], labels [rows], ignore_index), reduction = mean over the non-ignored rows.
 // One CTA per row (grid-stride). loss += sum over its rows of (lse - z[label]) / n_valid; dlogits = (softmax - onehot) * gs / n_valid.
-__global__ void __launch_bounds__(LOSS_THREADS)
-ce_loss_kernel(const float* __restrict__ z, long long ldz, const long long* __restrict__ labels, long long ignore_index,
-               float* __restrict__ loss, float* __restrict__ d32, long long ldd32, __nv_bfloat16* __restrict__ d16, long long ldd16,
-               int rows, int cols, float grad_scale) {
+// PARTIALS (deterministic plans): CTA b stores its share, with the NaN of "no valid row" in CTA 0's, into part[b] instead of adding
+// it to *loss; vb_ce_loss_det sums the shares in CTA order.
+template <bool PARTIALS>
+__device__ __forceinline__ void
+ce_loss_body(const float* __restrict__ z, long long ldz, const long long* __restrict__ labels, long long ignore_index,
+             float* __restrict__ loss, float* __restrict__ d32, long long ldd32, __nv_bfloat16* __restrict__ d16, long long ldd16,
+             int rows, int cols, float grad_scale, float* __restrict__ part) {
   pdl_entry();
   __shared__ float red[LOSS_THREADS / 32];
   const float n_valid = block_count(labels, rows, red, [&](long long l) { return l != ignore_index; });
@@ -85,8 +88,24 @@ ce_loss_kernel(const float* __restrict__ z, long long ldz, const long long* __re
     }
     if (threadIdx.x == 0) local += (lse - zr[lab]) * inv;
   }
+  if (PARTIALS) {
+    if (threadIdx.x == 0) part[blockIdx.x] = (blockIdx.x == 0 && n_valid == 0.f) ? local + CUDART_NAN_F : local;
+    return;
+  }
   if (threadIdx.x == 0 && local != 0.f) atomicAdd(loss, local);
   if (threadIdx.x == 0 && blockIdx.x == 0 && n_valid == 0.f) atomicAdd(loss, CUDART_NAN_F);   // torch: mean over no rows = nan
+}
+__global__ void __launch_bounds__(LOSS_THREADS)
+ce_loss_kernel(const float* __restrict__ z, long long ldz, const long long* __restrict__ labels, long long ignore_index,
+               float* __restrict__ loss, float* __restrict__ d32, long long ldd32, __nv_bfloat16* __restrict__ d16, long long ldd16,
+               int rows, int cols, float grad_scale) {
+  ce_loss_body<false>(z, ldz, labels, ignore_index, loss, d32, ldd32, d16, ldd16, rows, cols, grad_scale, nullptr);
+}
+__global__ void __launch_bounds__(LOSS_THREADS)
+ce_loss_det_kernel(const float* __restrict__ z, long long ldz, const long long* __restrict__ labels, long long ignore_index,
+                   float* __restrict__ d32, long long ldd32, __nv_bfloat16* __restrict__ d16, long long ldd16, int rows, int cols,
+                   float grad_scale, float* __restrict__ part) {
+  ce_loss_body<true>(z, ldz, labels, ignore_index, nullptr, d32, ldd32, d16, ldd16, rows, cols, grad_scale, part);
 }
 
 // Masked-region objective (vilbert.py:1506-1525, visual_target == 0):
@@ -94,10 +113,12 @@ ce_loss_kernel(const float* __restrict__ z, long long ldz, const long long* __re
 //   loss   = sum_{b,r: label[b,r] == 1} sum_c t * (log t - log_softmax(scores)_c)  /  max(#(label == 1), 0)
 // scores: f32 [B, Nv, C] (ld = C between regions), target f32 [B, Nv-1, C], label int64 [B, Nv-1]. One CTA per (b, r) row.
 // d scores_c = ((sum_c t) * softmax_c - t_c) * gs / n_pos on masked rows, 0 elsewhere (incl. region 0).
-__global__ void __launch_bounds__(LOSS_THREADS)
-kl_masked_loss_kernel(const float* __restrict__ scores, const float* __restrict__ target, const long long* __restrict__ label,
-                      float* __restrict__ loss, float* __restrict__ d32, __nv_bfloat16* __restrict__ d16, long long ldd16, int B, int Nv,
-                      int C, float grad_scale) {
+// PARTIALS: as ce_loss_body
+template <bool PARTIALS>
+__device__ __forceinline__ void
+kl_masked_loss_body(const float* __restrict__ scores, const float* __restrict__ target, const long long* __restrict__ label,
+                    float* __restrict__ loss, float* __restrict__ d32, __nv_bfloat16* __restrict__ d16, long long ldd16, int B, int Nv,
+                    int C, float grad_scale, float* __restrict__ part) {
   pdl_entry();
   __shared__ float red[LOSS_THREADS / 32];
   const int rows_t = B * (Nv - 1);
@@ -137,8 +158,24 @@ kl_masked_loss_kernel(const float* __restrict__ scores, const float* __restrict_
     acc = block_reduce(acc, red, false);
     if (threadIdx.x == 0) local += acc * inv;
   }
+  if (PARTIALS) {
+    if (threadIdx.x == 0) part[blockIdx.x] = (blockIdx.x == 0 && n_pos == 0.f) ? local + CUDART_NAN_F : local;
+    return;
+  }
   if (threadIdx.x == 0 && local != 0.f) atomicAdd(loss, local);
   if (threadIdx.x == 0 && blockIdx.x == 0 && n_pos == 0.f) atomicAdd(loss, CUDART_NAN_F);   // 0 / max(0, 0) in the reference
+}
+__global__ void __launch_bounds__(LOSS_THREADS)
+kl_masked_loss_kernel(const float* __restrict__ scores, const float* __restrict__ target, const long long* __restrict__ label,
+                      float* __restrict__ loss, float* __restrict__ d32, __nv_bfloat16* __restrict__ d16, long long ldd16, int B, int Nv,
+                      int C, float grad_scale) {
+  kl_masked_loss_body<false>(scores, target, label, loss, d32, d16, ldd16, B, Nv, C, grad_scale, nullptr);
+}
+__global__ void __launch_bounds__(LOSS_THREADS)
+kl_masked_loss_det_kernel(const float* __restrict__ scores, const float* __restrict__ target, const long long* __restrict__ label,
+                          float* __restrict__ d32, __nv_bfloat16* __restrict__ d16, long long ldd16, int B, int Nv, int C, float grad_scale,
+                          float* __restrict__ part) {
+  kl_masked_loss_body<true>(scores, target, label, nullptr, d32, d16, ldd16, B, Nv, C, grad_scale, part);
 }
 
 // ------------------------------------------------------------------------------------------ masked-row compaction (masked-LM head)
@@ -601,6 +638,23 @@ extern "C" vb_status vb_ce_loss(const float* logits, int64_t ld_logits, const in
   return check_launch("vb_ce_loss");
 }
 
+extern "C" vb_status vb_ce_loss_det(const float* logits, int64_t ld_logits, const int64_t* labels, int64_t ignore_index, float* loss,
+                                    float* dlogits_f32, int64_t ld_d32, void* dlogits_bf16, int64_t ld_d16, int32_t rows, int32_t cols,
+                                    float grad_scale, int32_t accumulate_loss, float* ws, void* stream) {
+  if (rows <= 0 || cols <= 0 || !logits || !labels || !loss || !ws) return set_error(VB_ERR_INVALID, "vb_ce_loss_det: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!accumulate_loss) {
+    cudaError_t e = cudaMemsetAsync(loss, 0, sizeof(float), st);
+    if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_ce_loss_det: memset: %s", cudaGetErrorString(e));
+  }
+  const int grid = loss_grid(rows) < VB_DET_LOSS_SLICES ? loss_grid(rows) : VB_DET_LOSS_SLICES;
+  launch_pdl(ce_loss_det_kernel, dim3(grid), dim3(LOSS_THREADS), (size_t)0, st, logits, (long long)ld_logits,
+             reinterpret_cast<const long long*>(labels), (long long)ignore_index, dlogits_f32, (long long)ld_d32,
+             static_cast<__nv_bfloat16*>(dlogits_bf16), (long long)ld_d16, (int)rows, (int)cols, grad_scale, ws);
+  if (int s = check_launch("vb_ce_loss_det")) return s;
+  return launch_reduce_slices(ws, 1, grid, 1, loss, st);
+}
+
 extern "C" vb_status vb_bce_gather_loss(const float* logits, int64_t ld_logits, int32_t col_off, int32_t width, const int64_t* ids,
                                         const float* target, int32_t rows, int32_t C, float loss_mul, float* row_loss, float* loss,
                                         int32_t accumulate_loss, float* dlogits_f32, int64_t ld_d32, void* dlogits_bf16, int64_t ld_d16,
@@ -687,6 +741,24 @@ extern "C" vb_status vb_kl_masked_loss(const float* scores, const float* target,
              reinterpret_cast<const long long*>(label), loss, dscores_f32, static_cast<__nv_bfloat16*>(dscores_bf16), (long long)ld_d16,
              (int)B, (int)Nv, (int)C, grad_scale);
   return check_launch("vb_kl_masked_loss");
+}
+
+extern "C" vb_status vb_kl_masked_loss_det(const float* scores, const float* target, const int64_t* label, float* loss, float* dscores_f32,
+                                           void* dscores_bf16, int64_t ld_d16, int32_t B, int32_t Nv, int32_t C, float grad_scale,
+                                           int32_t accumulate_loss, float* ws, void* stream) {
+  if (B <= 0 || Nv <= 1 || C <= 0 || !scores || !target || !label || !loss || !ws)
+    return set_error(VB_ERR_INVALID, "vb_kl_masked_loss_det: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!accumulate_loss) {
+    cudaError_t e = cudaMemsetAsync(loss, 0, sizeof(float), st);
+    if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_kl_masked_loss_det: memset: %s", cudaGetErrorString(e));
+  }
+  const int grid = loss_grid(B * Nv) < VB_DET_LOSS_SLICES ? loss_grid(B * Nv) : VB_DET_LOSS_SLICES;
+  launch_pdl(kl_masked_loss_det_kernel, dim3(grid), dim3(LOSS_THREADS), (size_t)0, st, scores, target,
+             reinterpret_cast<const long long*>(label), dscores_f32, static_cast<__nv_bfloat16*>(dscores_bf16), (long long)ld_d16,
+             (int)B, (int)Nv, (int)C, grad_scale, ws);
+  if (int s = check_launch("vb_kl_masked_loss_det")) return s;
+  return launch_reduce_slices(ws, 1, grid, 1, loss, st);
 }
 
 extern "C" vb_status vb_mse_masked_loss(const float* scores, const float* target, const int64_t* label, int32_t B, int32_t Nv, int32_t D,

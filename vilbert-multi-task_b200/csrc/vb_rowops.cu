@@ -125,13 +125,16 @@ ln_fwd_kernel(const float* x, long long ldx, const float* __restrict__ gamma, co
 //
 // dy2 (optional): a second fp32 gradient of the LayerNorm output, added to dy as it is read (dy + dy2: the residual-path gradient
 // that a dgrad GEMM epilogue would otherwise have added into dy, in the same fp32 addition).
-template <int NV>
-__global__ void __launch_bounds__(ROW_THREADS, 2)
-ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ dy2, long long lddy, const float* __restrict__ x, long long ldx,
-              const float* __restrict__ gamma, const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
-              float* __restrict__ dx32, __nv_bfloat16* __restrict__ dx16, long long lddx,
-              const __nv_bfloat16* __restrict__ pre, long long ldpre, float* __restrict__ dgamma, float* __restrict__ dbeta,
-              float* __restrict__ dbias, int M, int H, const DropCfg drop_out, const DropCfg drop_in) {
+//
+// PARTIALS (ln_bwd_det_kernel, deterministic plans): instead of one atomic per column and CTA, CTA b stores its column sums of pass
+// k (dgamma, dbeta, dbias) into part[(k * gridDim.x + b) * H + col]; vb_reduce_slices adds them up in CTA order.
+template <int NV, bool PARTIALS>
+__device__ __forceinline__ void
+ln_bwd_body(const float* __restrict__ dy, const float* __restrict__ dy2, long long lddy, const float* __restrict__ x, long long ldx,
+            const float* __restrict__ gamma, const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
+            float* __restrict__ dx32, __nv_bfloat16* __restrict__ dx16, long long lddx,
+            const __nv_bfloat16* __restrict__ pre, long long ldpre, float* __restrict__ dgamma, float* __restrict__ dbeta,
+            float* __restrict__ dbias, int M, int H, const DropCfg drop_out, const DropCfg drop_in, float* __restrict__ part) {
   pdl_entry();
   constexpr int TEAMS = ROW_THREADS / 64;
   const uint32_t seed_out = drop_out.ctr ? drop_seed(drop_out) : 0u;   // mask applied to this LayerNorm's output in forward
@@ -227,11 +230,33 @@ ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ dy2, long 
 #pragma unroll
         for (int w = 0; w < TEAMS; ++w) sacc += red[w][threadIdx.x];
         const int col = (i * 64 + (threadIdx.x >> 2)) * 4 + (threadIdx.x & 3);
-        if (col < H) atomicAdd(dst + col, sacc);
+        if (PARTIALS) {
+          if (col < H) part[((long long)pass * gridDim.x + blockIdx.x) * H + col] = sacc;
+        } else {
+          if (col < H) atomicAdd(dst + col, sacc);
+        }
       }
     }
   }
 }
+
+#define VB_LN_BWD_PARAMS                                                                                                                   \
+  const float* __restrict__ dy, const float* __restrict__ dy2, long long lddy, const float* __restrict__ x, long long ldx,                  \
+      const float* __restrict__ gamma, const float* __restrict__ mean_in, const float* __restrict__ rstd_in, float* __restrict__ dx32,     \
+      __nv_bfloat16* __restrict__ dx16, long long lddx, const __nv_bfloat16* __restrict__ pre, long long ldpre,                           \
+      float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M, int H, const DropCfg drop_out,             \
+      const DropCfg drop_in
+template <int NV>
+__global__ void __launch_bounds__(ROW_THREADS, 2) ln_bwd_kernel(VB_LN_BWD_PARAMS) {
+  ln_bwd_body<NV, false>(dy, dy2, lddy, x, ldx, gamma, mean_in, rstd_in, dx32, dx16, lddx, pre, ldpre, dgamma, dbeta, dbias, M, H, drop_out,
+                         drop_in, nullptr);
+}
+template <int NV>
+__global__ void __launch_bounds__(ROW_THREADS, 2) ln_bwd_det_kernel(VB_LN_BWD_PARAMS, float* __restrict__ part) {
+  ln_bwd_body<NV, true>(dy, dy2, lddy, x, ldx, gamma, mean_in, rstd_in, dx32, dx16, lddx, pre, ldpre, dgamma, dbeta, dbias, M, H, drop_out,
+                        drop_in, part);
+}
+#undef VB_LN_BWD_PARAMS
 
 // ------------------------------------------------------------------------------------------ casts
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n4, long long n, int fp16,
@@ -557,9 +582,11 @@ __global__ void axpy_kernel(const float* __restrict__ x, float* __restrict__ y, 
 
 // ------------------------------------------------------------------------------------------ VQA loss
 // loss = mean(BCEWithLogits(z, t)) * n_cols  (task_utils.py:325-327); dz = (sigmoid(z) - t) / n_rows * grad_scale
-__global__ void bce_logits_kernel(const float* __restrict__ z, const float* __restrict__ t, float* __restrict__ loss,
-                                  float* __restrict__ dz32, __nv_bfloat16* __restrict__ dz16, long long lddz16, int rows, int cols,
-                                  float grad_scale) {
+// PARTIALS: CTA b stores its share into part[b] instead of adding it to *loss (deterministic plans; vb_reduce_slices sums them).
+template <bool PARTIALS>
+__device__ __forceinline__ void bce_logits_body(const float* __restrict__ z, const float* __restrict__ t, float* __restrict__ loss,
+                                                float* __restrict__ dz32, __nv_bfloat16* __restrict__ dz16, long long lddz16, int rows,
+                                                int cols, float grad_scale, float* __restrict__ part) {
   pdl_entry();
   __shared__ float red[32];
   const long long n = (long long)rows * cols;
@@ -578,8 +605,21 @@ __global__ void bce_logits_kernel(const float* __restrict__ z, const float* __re
   if (threadIdx.x < 32) {
     float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
     v = warp_sum(v);
-    if (threadIdx.x == 0) atomicAdd(loss, v * inv_rows);
+    if (threadIdx.x == 0) {
+      if (PARTIALS) part[blockIdx.x] = v * inv_rows;
+      else atomicAdd(loss, v * inv_rows);
+    }
   }
+}
+__global__ void bce_logits_kernel(const float* __restrict__ z, const float* __restrict__ t, float* __restrict__ loss,
+                                  float* __restrict__ dz32, __nv_bfloat16* __restrict__ dz16, long long lddz16, int rows, int cols,
+                                  float grad_scale) {
+  bce_logits_body<false>(z, t, loss, dz32, dz16, lddz16, rows, cols, grad_scale, nullptr);
+}
+__global__ void bce_logits_det_kernel(const float* __restrict__ z, const float* __restrict__ t, float* __restrict__ dz32,
+                                      __nv_bfloat16* __restrict__ dz16, long long lddz16, int rows, int cols, float grad_scale,
+                                      float* __restrict__ part) {
+  bce_logits_body<true>(z, t, nullptr, dz32, dz16, lddz16, rows, cols, grad_scale, part);
 }
 
 // additive attention mask (vilbert.py:1341-1362): out[b, j] = (1 - m[b, j]) * -10000; with prepend_one the
@@ -741,6 +781,158 @@ static inline DropCfg make_drop(const vb_dropout* d) {
   return c;
 }
 
+// ------------------------------------------------------------------------------------------ deterministic reductions
+// The kernels of deterministic plans (DESIGN.md §4h) replace "per-block partial, then a float atomic" by "per-block partial into a
+// workspace slice, then one ordered sum": dst[i] += part[0 * stride + i] + part[1 * stride + i] + ... in slice order. The slice
+// count is a function of the problem shape only, so the sum has the same order in every run.
+__global__ void reduce_slices_kernel(const float* __restrict__ part, long long stride, int slices, long long n, float* __restrict__ dst) {
+  pdl_entry();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int k = 0; k < slices; ++k) s += part[k * stride + i];
+    dst[i] += s;
+  }
+}
+
+// colsum_kernel with the CTA's column sums stored into part[blockIdx.y * N + col]
+template <typename T>
+__global__ void colsum_partial_kernel(const T* __restrict__ X, long long ld, float* __restrict__ part, int M, int N, int rows_per_block) {
+  pdl_entry();
+  __shared__ float red[8][33];
+  const int col = blockIdx.x * 32 + threadIdx.x;
+  const long long m0 = (long long)blockIdx.y * rows_per_block;
+  const long long m1 = min((long long)M, m0 + rows_per_block);
+  float acc = 0.f;
+  if (col < N)
+    for (long long m = m0 + threadIdx.y; m < m1; m += 8) acc += to_f<T>(X[m * ld + col]);
+  red[threadIdx.y][threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.y == 0 && col < N) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s += red[i][threadIdx.x];
+    part[(long long)blockIdx.y * N + col] = s;
+  }
+}
+
+// loc_proj_bwd_kernel with the row block's sums stored into part[blockIdx.y * 6H + ...]: dW (h * 5 + j) then db (5H + h)
+__global__ void loc_proj_bwd_partial_kernel(const float* __restrict__ dy, const float* __restrict__ loc, float* __restrict__ part, int M,
+                                            int H, int rows_per_block) {
+  pdl_entry();
+  const long long m0 = (long long)blockIdx.y * rows_per_block;
+  const long long m1 = min((long long)M, m0 + rows_per_block);
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= H) return;
+  float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (long long m = m0; m < m1; ++m) {
+    const float d = dy[m * H + h];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) acc[j] += d * __ldg(loc + m * 5 + j);
+    acc[5] += d;
+  }
+  float* o = part + (long long)blockIdx.y * 6 * H;
+#pragma unroll
+  for (int j = 0; j < 5; ++j) o[(long long)h * 5 + j] = acc[j];
+  o[5LL * H + h] = acc[5];
+}
+
+// the dW / db sums of small_linear_bwd_kernel with CTA b's share stored into part[b * (N K + N) + ...]: dW (j * K + k) then db (N K + j)
+__global__ void __launch_bounds__(ROW_THREADS)
+small_linear_wgrad_partial_kernel(const float* __restrict__ dy, const float* __restrict__ x, long long ldx, float* __restrict__ part,
+                                  int M, int K, int N, const DropCfg drop) {
+  pdl_entry();
+  const uint32_t dseed = drop.ctr ? drop_seed(drop) : 0u;
+  float* o = part + (long long)blockIdx.x * ((long long)N * K + N);
+  for (int j = 0; j < N; ++j) {
+    for (int k = threadIdx.x; k < K; k += ROW_THREADS) {
+      float acc = 0.f;
+      for (long long m = blockIdx.x; m < M; m += gridDim.x) {
+        float xv = x[m * ldx + k];
+        if (drop.ctr) xv = drop_apply(xv, dseed, drop_index(drop, m, K, k), drop);
+        acc += dy[m * N + j] * xv;
+      }
+      o[(long long)j * K + k] = acc;
+    }
+    if (threadIdx.x == 0) {
+      float dbp = 0.f;
+      for (long long m = blockIdx.x; m < M; m += gridDim.x) dbp += dy[m * N + j];
+      o[(long long)N * K + j] = dbp;
+    }
+  }
+}
+
+// Embedding-table gradients without atomics. Output row r of the text embedding selects one row of each table (embed_key: the word
+// id, the token type, the task id of the task-token row, the position); -1 = none (word id 0 is padding_idx, vilbert.py:328-330).
+// One warp per (table, output row): the warp of the FIRST output row that selects a table row (found by a ballot scan over the
+// earlier rows) owns that table row, adds d(out) of every output row that selects it in row order, and adds the sum to the table
+// row with a plain store. Each table row has one writer, each sum one order. The scans cost rows^2 / 32 key reads per table (2.4k
+// rows at B = 64 x 37 tokens: ~0.2M), which is small next to the step; H <= 1024 (8 float4 columns per lane).
+constexpr int EMBED_DET_V4 = 8;
+__device__ __forceinline__ long long embed_key(int table, long long row, const long long* __restrict__ ids, const long long* __restrict__ tts,
+                                               const long long* __restrict__ task_ids, int Nt, int has_task) {
+  const int No = Nt + has_task;
+  const int b = (int)(row / No), p = (int)(row % No);
+  if (has_task && p == 1) return table == 2 ? task_ids[b] : -1;
+  const int t = (has_task && p > 1) ? p - 1 : p;
+  if (table == 0) { const long long id = ids[(long long)b * Nt + t]; return id != 0 ? id : -1; }
+  if (table == 1) return tts[(long long)b * Nt + t];
+  if (table == 3) return t;
+  return -1;
+}
+__global__ void __launch_bounds__(ROW_THREADS)
+embed_text_bwd_det_kernel(const float* __restrict__ dout, const long long* __restrict__ ids, const long long* __restrict__ tts,
+                          const long long* __restrict__ task_ids, float* __restrict__ dword, float* __restrict__ dpos,
+                          float* __restrict__ dtype, float* __restrict__ dtask, int B, int Nt, int H, int has_task) {
+  pdl_entry();
+  const int lane = threadIdx.x & 31;
+  const long long rows = (long long)B * (Nt + has_task);
+  const int n4 = H >> 2;
+  for (long long item = (long long)blockIdx.x * ROW_WARPS + (threadIdx.x >> 5); item < 4 * rows; item += (long long)gridDim.x * ROW_WARPS) {
+    const int table = (int)(item / rows);
+    const long long row = item % rows;
+    float* dst = table == 0 ? dword : (table == 1 ? dtype : (table == 2 ? dtask : dpos));
+    if (!dst) continue;
+    const long long key = embed_key(table, row, ids, tts, task_ids, Nt, has_task);
+    if (key < 0) continue;
+    bool first = true;
+    for (long long base = 0; base < row && first; base += 32) {
+      const long long r = base + lane;
+      first = !__any_sync(0xffffffffu, r < row && embed_key(table, r, ids, tts, task_ids, Nt, has_task) == key);
+    }
+    if (!first) continue;
+    float4 acc[EMBED_DET_V4];
+#pragma unroll
+    for (int i = 0; i < EMBED_DET_V4; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long base = row; base < rows; base += 32) {
+      const long long r = base + lane;
+      unsigned hit = __ballot_sync(0xffffffffu, r < rows && embed_key(table, r, ids, tts, task_ids, Nt, has_task) == key);
+      while (hit) {
+        const int j = __ffs(hit) - 1;
+        hit &= hit - 1;
+        const float4* d = reinterpret_cast<const float4*>(dout + (base + j) * H);
+#pragma unroll
+        for (int i = 0; i < EMBED_DET_V4; ++i) {
+          const int c = lane + 32 * i;
+          if (c < n4) {
+            const float4 v = d[c];
+            acc[i].x += v.x; acc[i].y += v.y; acc[i].z += v.z; acc[i].w += v.w;
+          }
+        }
+      }
+    }
+    float4* o = reinterpret_cast<float4*>(dst + key * H);
+#pragma unroll
+    for (int i = 0; i < EMBED_DET_V4; ++i) {
+      const int c = lane + 32 * i;
+      if (c < n4) {
+        float4 v = o[c];
+        v.x += acc[i].x; v.y += acc[i].y; v.z += acc[i].z; v.w += acc[i].w;
+        o[c] = v;
+      }
+    }
+  }
+}
+
 static inline int ew_grid(long long n, int threads = 256) {
   long long blocks = (n + threads - 1) / threads;
   long long cap = (long long)sm_count() * 8;
@@ -815,6 +1007,51 @@ static vb_status layernorm_bwd(const char* name, const float* dy, const float* d
   return check_launch(name);
 }
 
+namespace vb {
+int launch_reduce_slices(const float* part, long long stride, int slices, long long n, float* dst, cudaStream_t stream) {
+  if (n <= 0 || slices <= 0 || !dst) return VB_OK;
+  launch_pdl(reduce_slices_kernel, dim3(ew_grid(n)), dim3(256), (size_t)0, stream, part, stride, slices, n, dst);
+  return check_launch("vb_reduce_slices");
+}
+}  // namespace vb
+
+extern "C" vb_status vb_reduce_slices(const float* part, int64_t stride, int32_t slices, int64_t n, float* dst, void* stream) {
+  if (slices < 0 || n < 0 || stride < n || (slices > 0 && n > 0 && (!part || !dst)))
+    return set_error(VB_ERR_INVALID, "vb_reduce_slices: bad arguments (slices %d, n %lld, stride %lld)", (int)slices, (long long)n, (long long)stride);
+  return launch_reduce_slices(part, stride, slices, n, dst, ST(stream));
+}
+
+// vb_layernorm_bwd / vb_add_layernorm_bwd (dy2 may be NULL) of deterministic plans: the column sums go through `ws`
+extern "C" vb_status vb_layernorm_bwd_det(const float* dy, const float* dy2, int64_t lddy, const float* x, int64_t ldx, const float* gamma,
+                                          const float* mean, const float* rstd, float* dx_f32, void* dx_bf16, int64_t lddx, const void* gelu_pre,
+                                          int64_t ld_pre, float* dgamma, float* dbeta, float* dbias, int32_t M, int32_t H,
+                                          const vb_dropout* out_dropout, const vb_dropout* in_dropout, float* ws, void* stream) {
+  const char* name = "vb_layernorm_bwd_det";
+  if (M <= 0 || H <= 0) return set_error(VB_ERR_INVALID, "%s: empty problem", name);
+  if ((H & 3) || H > MAX_V4 * 128 || (ldx & 3) || (lddy & 3) || (lddx & 3) || (gelu_pre && (ld_pre & 3)) || !al16(dy) || !al16(x) || !al16(gamma) ||
+      (dy2 && !al16(dy2)))
+    return set_error(VB_ERR_INVALID, "%s: need H %% 4 == 0, H <= %d, ld %% 4 == 0, 16-byte aligned rows", name, MAX_V4 * 128);
+  const bool sums = dgamma || dbeta || dbias;
+  if (sums && !ws) return set_error(VB_ERR_INVALID, "%s: the column sums need a workspace", name);
+  const DropCfg dc_out = make_drop(out_dropout), dc_in = make_drop(in_dropout);
+  if ((dc_out.ctr || dc_in.ctr) && (ldx != H || lddy != H || lddx != H))
+    return set_error(VB_ERR_INVALID, "%s: dropout masks are indexed row*H + col and need dense rows", name);
+  const int nv = (H / 4 + 63) / 64;
+  const long long blocks = ((long long)M + 3) / 4;
+  const int grid = (int)(blocks < VB_DET_LN_SLICES ? blocks : VB_DET_LN_SLICES);   // a function of M only: the sums keep their order
+  __nv_bfloat16* dx16 = static_cast<__nv_bfloat16*>(dx_bf16);
+  const __nv_bfloat16* pre = static_cast<const __nv_bfloat16*>(gelu_pre);
+#define LN_BD(NV) launch_pdl(ln_bwd_det_kernel<NV>, dim3(grid), dim3(ROW_THREADS), (size_t)(0), ST(stream), dy, dy2, lddy, x, ldx, gamma, mean, rstd, dx_f32, dx16, lddx, pre, ld_pre, dgamma, dbeta, dbias, M, H, dc_out, dc_in, ws)
+  if (nv <= 1) LN_BD(1); else if (nv <= 2) LN_BD(2); else if (nv <= 3) LN_BD(3); else if (nv <= 4) LN_BD(4); else LN_BD(8);
+#undef LN_BD
+  if (int st = check_launch(name)) return st;
+  float* dst[3] = {dgamma, dbeta, dbias};
+  for (int k = 0; k < 3; ++k)
+    if (dst[k])
+      if (int st = launch_reduce_slices(ws + (long long)k * grid * H, H, grid, H, dst[k], ST(stream))) return st;
+  return VB_OK;
+}
+
 extern "C" vb_status vb_layernorm_bwd(const float* dy, int64_t lddy, const float* x, int64_t ldx, const float* gamma, const float* mean,
                                       const float* rstd, float* dx_f32, void* dx_bf16, int64_t lddx, const void* gelu_pre,
                                       int64_t ld_pre, float* dgamma, float* dbeta, float* dbias, int32_t M, int32_t H,
@@ -875,6 +1112,20 @@ extern "C" vb_status vb_embed_text_bwd(const float* dout, const int64_t* ids, co
   return check_launch("vb_embed_text_bwd");
 }
 
+extern "C" vb_status vb_embed_text_bwd_det(const float* dout, const int64_t* ids, const int64_t* token_type_ids, const int64_t* task_ids,
+                                           float* dword, float* dpos, float* dtype, float* dtask, int32_t B, int32_t Nt, int32_t H,
+                                           void* stream) {
+  if (B <= 0 || Nt <= 0 || (H & 3) || H > EMBED_DET_V4 * 128 || !al16(dout))
+    return set_error(VB_ERR_INVALID, "vb_embed_text_bwd_det: bad shape (H %% 4 == 0, H <= %d, 16-byte aligned rows)", EMBED_DET_V4 * 128);
+  const int has_task = task_ids != nullptr;
+  if (!dword && !dpos && !dtype && !(has_task && dtask)) return VB_OK;
+  const long long rows = (long long)B * (Nt + has_task);
+  launch_pdl(embed_text_bwd_det_kernel, dim3(row_grid(4 * rows)), dim3(ROW_THREADS), (size_t)(0), ST(stream),
+      dout, reinterpret_cast<const long long*>(ids), reinterpret_cast<const long long*>(token_type_ids),
+      reinterpret_cast<const long long*>(task_ids), dword, dpos, dtype, has_task ? dtask : nullptr, B, Nt, H, has_task);
+  return check_launch("vb_embed_text_bwd_det");
+}
+
 extern "C" vb_status vb_loc_proj_fwd(const float* loc, const float* W, const float* b, float* out, int32_t M, int32_t H, void* stream) {
   if (M <= 0 || H <= 0) return set_error(VB_ERR_INVALID, "vb_loc_proj_fwd: bad shape");
   const size_t smem = (size_t)H * 6 * sizeof(float);
@@ -891,6 +1142,19 @@ extern "C" vb_status vb_loc_proj_bwd(const float* dy, const float* loc, float* d
   dim3 grid((H + 127) / 128, (M + rpb - 1) / rpb);
   launch_pdl(loc_proj_bwd_kernel, dim3(grid), dim3(128), (size_t)(0), ST(stream), dy, loc, dW, db, M, H, rpb);
   return check_launch("vb_loc_proj_bwd");
+}
+
+extern "C" vb_status vb_loc_proj_bwd_det(const float* dy, const float* loc, float* dW, float* db, int32_t M, int32_t H, float* ws, void* stream) {
+  if (M <= 0 || H <= 0) return set_error(VB_ERR_INVALID, "vb_loc_proj_bwd_det: bad shape");
+  if (!dW && !db) return VB_OK;
+  if (!ws) return set_error(VB_ERR_INVALID, "vb_loc_proj_bwd_det: no workspace");
+  int rpb = (M + VB_DET_SLICES - 1) / VB_DET_SLICES; if (rpb < 64) rpb = 64;
+  const int slices = (M + rpb - 1) / rpb;
+  launch_pdl(loc_proj_bwd_partial_kernel, dim3((H + 127) / 128, slices), dim3(128), (size_t)(0), ST(stream), dy, loc, ws, M, H, rpb);
+  if (int st = check_launch("vb_loc_proj_bwd_det")) return st;
+  if (dW) if (int st = launch_reduce_slices(ws, 6LL * H, slices, 5LL * H, dW, ST(stream))) return st;
+  if (db) if (int st = launch_reduce_slices(ws + 5LL * H, 6LL * H, slices, H, db, ST(stream))) return st;
+  return VB_OK;
 }
 
 extern "C" vb_status vb_loc_proj_dx(const float* dy, const float* W, float* dx, int32_t M, int32_t H, void* stream) {
@@ -912,6 +1176,17 @@ extern "C" vb_status vb_colsum(const void* X, int32_t is_bf16, int64_t ld, float
   return check_launch("vb_colsum");
 }
 
+extern "C" vb_status vb_colsum_det(const void* X, int32_t is_bf16, int64_t ld, float* out, int32_t M, int32_t N, float* ws, void* stream) {
+  if (M <= 0 || N <= 0 || !ws) return set_error(VB_ERR_INVALID, "vb_colsum_det: bad shape or no workspace");
+  int rpb = (M + VB_DET_SLICES - 1) / VB_DET_SLICES; if (rpb < 64) rpb = 64;
+  const int slices = (M + rpb - 1) / rpb;
+  dim3 grid((N + 31) / 32, slices), block(32, 8);
+  if (is_bf16) launch_pdl(colsum_partial_kernel<__nv_bfloat16>, dim3(grid), dim3(block), (size_t)(0), ST(stream), static_cast<const __nv_bfloat16*>(X), ld, ws, M, N, rpb);
+  else launch_pdl(colsum_partial_kernel<float>, dim3(grid), dim3(block), (size_t)(0), ST(stream), static_cast<const float*>(X), ld, ws, M, N, rpb);
+  if (int st = check_launch("vb_colsum_det")) return st;
+  return launch_reduce_slices(ws, N, slices, N, out, ST(stream));
+}
+
 extern "C" vb_status vb_small_linear_fwd(const float* x, int64_t ldx, const float* W, const float* b, const float* row_addend, float* y,
                                          int32_t M, int32_t K, int32_t N, const vb_dropout* in_dropout, void* stream) {
   if (M <= 0 || K <= 0 || N <= 0 || N > 8) return set_error(VB_ERR_INVALID, "vb_small_linear_fwd: bad shape (N <= 8)");
@@ -927,6 +1202,28 @@ extern "C" vb_status vb_small_linear_bwd(const float* dy, const float* x, int64_
   int grid = sm_count(); if (grid > M) grid = M; if (grid <= 0) grid = 1;
   launch_pdl(small_linear_bwd_kernel, dim3(grid), dim3(ROW_THREADS), (size_t)(0), ST(stream), dy, x, ldx, W, dx, lddx, accumulate_dx, dW, db, M, K, N, make_drop(in_dropout));
   return check_launch("vb_small_linear_bwd");
+}
+
+extern "C" vb_status vb_small_linear_bwd_det(const float* dy, const float* x, int64_t ldx, const float* W, float* dx, int64_t lddx,
+                                             int32_t accumulate_dx, float* dW, float* db, int32_t M, int32_t K, int32_t N,
+                                             const vb_dropout* in_dropout, float* ws, void* stream) {
+  if (M <= 0 || K <= 0 || N <= 0 || N > 8) return set_error(VB_ERR_INVALID, "vb_small_linear_bwd_det: bad shape (N <= 8)");
+  if ((dW || db) && !ws) return set_error(VB_ERR_INVALID, "vb_small_linear_bwd_det: no workspace");
+  const DropCfg dc = make_drop(in_dropout);
+  if (dx) {   // the input gradient has no atomics: the default kernel without its dW / db sums
+    int grid = sm_count(); if (grid > M) grid = M; if (grid <= 0) grid = 1;
+    launch_pdl(small_linear_bwd_kernel, dim3(grid), dim3(ROW_THREADS), (size_t)(0), ST(stream), dy, x, ldx, W, dx, lddx, accumulate_dx,
+               (float*)nullptr, (float*)nullptr, M, K, N, dc);
+    if (int st = check_launch("vb_small_linear_bwd_det")) return st;
+  }
+  if (!dW && !db) return VB_OK;
+  const int slices = M < VB_DET_SLICES ? M : VB_DET_SLICES;
+  const long long stride = (long long)N * K + N;
+  launch_pdl(small_linear_wgrad_partial_kernel, dim3(slices), dim3(ROW_THREADS), (size_t)(0), ST(stream), dy, x, ldx, ws, M, K, N, dc);
+  if (int st = check_launch("vb_small_linear_bwd_det")) return st;
+  if (dW) if (int st = launch_reduce_slices(ws, stride, slices, (long long)N * K, dW, ST(stream))) return st;
+  if (db) if (int st = launch_reduce_slices(ws + (long long)N * K, stride, slices, N, db, ST(stream))) return st;
+  return VB_OK;
 }
 
 extern "C" vb_status vb_fuse_pooled_fwd(const float* a, const float* b, float* out_f32, void* out_bf16, int64_t n, int32_t mul,
@@ -961,6 +1258,18 @@ extern "C" vb_status vb_bce_logits_loss(const float* logits, const float* target
                                                                               static_cast<__nv_bfloat16*>(dlogits_bf16), ld_dlogits_bf16, rows,
                                                                               cols, grad_scale);
   return check_launch("vb_bce_logits_loss");
+}
+extern "C" vb_status vb_bce_logits_loss_det(const float* logits, const float* target, float* loss, float* dlogits_f32, void* dlogits_bf16,
+                                            int64_t ld_dlogits_bf16, int32_t rows, int32_t cols, float grad_scale, float* ws, void* stream) {
+  if (rows <= 0 || cols <= 0 || !ws) return set_error(VB_ERR_INVALID, "vb_bce_logits_loss_det: bad shape or no workspace");
+  cudaError_t e = cudaMemsetAsync(loss, 0, sizeof(float), ST(stream));
+  if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_bce_logits_loss_det: memset: %s", cudaGetErrorString(e));
+  int grid = ew_grid((long long)rows * cols);
+  if (grid > VB_DET_LOSS_SLICES) grid = VB_DET_LOSS_SLICES;
+  launch_pdl(bce_logits_det_kernel, dim3(grid), dim3(256), (size_t)(0), ST(stream), logits, target, dlogits_f32,
+             static_cast<__nv_bfloat16*>(dlogits_bf16), ld_dlogits_bf16, rows, cols, grad_scale, ws);
+  if (int st = check_launch("vb_bce_logits_loss_det")) return st;
+  return launch_reduce_slices(ws, 1, grid, 1, loss, ST(stream));
 }
 extern "C" vb_status vb_mask_to_additive(const int64_t* mask, float* out, int32_t B, int32_t N, int32_t prepend_one, void* stream) {
   if (B <= 0 || N <= 0) return set_error(VB_ERR_INVALID, "vb_mask_to_additive: bad shape");

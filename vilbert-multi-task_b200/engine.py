@@ -21,6 +21,7 @@ activations and weights exist only as tensor-core operands. Three operand precis
   "bf16"            every operand bf16 (round-1 arithmetic; kept for A/B measurements).
 """
 import math
+import warnings
 import zlib
 from collections import Counter, OrderedDict, namedtuple
 
@@ -430,6 +431,22 @@ RESULT_MODES = {"vqa": ("vil_prediction", L.VB_RESULT_ARGMAX), "gqa": ("vil_pred
 HeadLayout = namedtuple("HeadLayout", "name logits rows cols ld off ids width key")
 
 
+# deterministic plans (Plan(deterministic=True), DESIGN.md §4h): entry points whose float atomics make the summation order depend on
+# scheduling, and the workspace floats their _det twin (same arguments + a trailing workspace) needs, from the arguments of the launch.
+# vb_layernorm_bwd / vb_add_layernorm_bwd (Plan.ln_bwd) and the atomic GEMMs (Plan.gemm) are switched where they are emitted.
+DET_WORKSPACE = {
+    "vb_colsum": lambda X, bf16, ld, out, M, N: L.VB_DET_SLICES * N,
+    "vb_loc_proj_bwd": lambda dy, loc, dW, db, M, H: L.VB_DET_SLICES * 6 * H,
+    "vb_small_linear_bwd": lambda dy, x, ldx, W, dx, lddx, acc, dW, db, M, K, N, drop: L.VB_DET_SLICES * (N * K + N),
+    "vb_embed_text_bwd": None,
+    "vb_ce_loss": lambda *a: L.VB_DET_LOSS_SLICES,
+    "vb_kl_masked_loss": lambda *a: L.VB_DET_LOSS_SLICES,
+    "vb_bce_logits_loss": lambda *a: L.VB_DET_LOSS_SLICES,
+}
+# kernels of the single-stream baseline (BaseBertForVLTasks) with float atomics and no deterministic variant
+DET_MISSING_BASELINE = ("vb_concat_embed_ln_bwd", "vb_embed_text_bwd_padded")
+
+
 class Plan:
     """Static execution plan for one input shape. `grad_outputs` names the outputs that will receive a
     gradient in backward (dead branches are not emitted). `loss` fuses an objective of LOSS_HEADS into the plan: by default its
@@ -472,12 +489,21 @@ class Plan:
     gradient even with all of its parameters frozen, and the backward ends the image-embedding chain with d(input_imgs) = dy W (the
     feature GEMM's dgrad) and d(image_loc) = dy W_loc (vb_loc_proj_dx). They land in private buffers outside the arena and outside
     grad_touch; self.input_grad maps each input whose gradient the backward writes to its buffer ([B*Nv, Fv] / [B*Nv, 5] fp32). An
-    input behind a no_grad layer (fixed_v_layer > 0) gets no entry, as it gets no gradient in torch."""
+    input behind a no_grad layer (fixed_v_layer > 0) gets no entry, as it gets no gradient in torch.
+
+    deterministic=True (torch.use_deterministic_algorithms(True), DESIGN.md §4h): every sum that float atomics would make
+    order-dependent goes through the _det variant of its kernel (per-block partials in a workspace of the plan, then one ordered
+    sum), the GEMM weight gradients that split K store their splits apart and add them in split order, and all launches go to one
+    stream, so no two kernels add into the same range concurrently. Two runs give bitwise identical results on the same GPU model
+    and build. self.det_ws_bytes: the workspace the plan allocated for it."""
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
                  loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-                 input_grads=frozenset(), packed=None):
+                 input_grads=frozenset(), packed=None, deterministic=False):
         self.e, self.cfg = engine, engine.cfg
+        self.det = bool(deterministic)
+        self._det_ws, self.det_ws_bytes = None, 0
+        self._det_bias = []      # deterministic plans: attention bias sums (bias, d(Q|K|V), pitch) left to det_bias_sums
         self.packed = None if packed is None else (int(packed[0]), int(packed[1]))
         self.frozen = frozenset(frozen)
         unknown = sorted(n for n in self.frozen if n not in engine.ps.entries)
@@ -532,8 +558,8 @@ class Plan:
         self.epilogue = []       # optional per-step ops run after the backward (the fused optimizer: enable_optimizer)
         self.cur = self.fwd
         self.sid = 0             # stream the next emitted op goes to: 0 = text/main stream, 1 = vision stream
-        self.two_streams = engine.two_streams
-        self.wgrad_streams = engine.wgrad_streams and engine.two_streams   # weight-gradient GEMMs off the critical chain
+        self.two_streams = engine.two_streams and not self.det
+        self.wgrad_streams = engine.wgrad_streams and self.two_streams   # weight-gradient GEMMs off the critical chain
         self._streams = None
         self._n_events = 0
         self._scratch_epoch = 0
@@ -726,8 +752,32 @@ class Plan:
 
     def emit(self, fn, *args):
         """Appends a launch of `fn` to the pass being built. Tensors, None and descriptor structs are passed as they are: the
-        arguments become C values here (_lib.launch_args), which also checks their count against fn's prototype."""
+        arguments become C values here (_lib.launch_args), which also checks their count against fn's prototype. A deterministic
+        plan launches the _det twin of an entry point of DET_WORKSPACE instead, with its workspace."""
+        if self.det and fn.__name__ in DET_WORKSPACE:
+            size = DET_WORKSPACE[fn.__name__]
+            fn = getattr(self.lib, fn.__name__ + "_det")
+            if size is not None:
+                args = args + (self.det_ws(size(*args)),)
         self.cur.append((fn, L.launch_args(fn, *args), self.sid if self.two_streams else 0))
+
+    def det_ws(self, n):
+        """fp32 workspace of at least n floats for a deterministic launch. A deterministic plan runs on one stream, so launches share
+        the current buffer: each partials kernel and the ordered sum after it are done before the next launch writes it. A request
+        larger than the current buffer allocates a new one; the launches emitted before keep the old one, so the plan holds every
+        size the workspace grew through (all counted in det_ws_bytes)."""
+        if self._det_ws is None or self._det_ws.numel() < n:
+            self._det_ws = torch.empty(max(int(n), 1), dtype=F32, device=self.dev)
+            self._keep.append(self._det_ws)
+            self.det_ws_bytes += self._det_ws.numel() * 4
+        return self._det_ws
+
+    def det_bias_sums(self):
+        """Deterministic plans: the attention bias gradients the backward kernels would have summed with atomics, as ordered column
+        sums of d(Q|K|V) (after the packed tail rows are zeroed)."""
+        pending, self._det_bias = self._det_bias, []
+        for db, dx, ld in pending:
+            self.colsum(dx, ld, db, dx.shape[0], dx.shape[1])
 
     def sync_streams(self, mirror=True):
         """Both streams wait for each other here. Between two connection layers the text and the vision segments are
@@ -812,11 +862,31 @@ class Plan:
         g.out_bf16, g.ld_out_bf16 = L.arg(out_bf16), ld_ob
         g.out_pre, g.ld_out_pre = L.arg(out_pre), ld_op
         g.atomic_out, g.split_k, g.block_n, g.max_ctas = atomic, split_k, 0, (0 if fwd else self.e.bwd_gemm_max_ctas)
-        g.out_colsum = L.arg(out_colsum)
+        g.out_colsum = L.arg(None if self.det else out_colsum)
         if dropout is not None:
             g.dropout = dropout
         self._keep.append(g)
+        if self.det and atomic:
+            # split-K weight gradients: each split stores its tile into its own slice of the workspace, one ordered sum adds them
+            g.atomic_out, g.split_k = L.VB_GEMM_PARTIALS, 0
+            bn, cl, sp = (L.C.c_int32() for _ in range(3))
+            L.check(self.lib.vb_gemm_plan(L.C.byref(g), 132 if self.dev.type != "cuda" else 0, L.C.byref(bn), L.C.byref(cl), L.C.byref(sp)),
+                    "vb_gemm_plan")
+            if sp.value == 1:
+                g.atomic_out, g.split_k = 1, 1      # one CTA per output tile: a single add per element, in launch order
+                self.emit(self.lib.vb_gemm_bf16, g)
+                return
+            if ld_of != N:
+                raise L.VBError(f"deterministic split-K GEMM needs a dense output (ld {ld_of} != N {N})")
+            ws = self.det_ws(sp.value * M * N)
+            g.out_f32, g.split_k = L.arg(ws), sp.value
+            self.emit(self.lib.vb_gemm_bf16, g)
+            self.emit(self.lib.vb_reduce_slices, ws, M * N, sp.value, M * N, out_f32)
+            return
         self.emit(self.lib.vb_gemm_bf16, g)
+        if self.det and out_colsum is not None:
+            # the bias gradient fused into the epilogue: an ordered column sum of the operand the GEMM stored
+            self.colsum(out_bf16, ld_ob, out_colsum, M, N)
 
     def attention(self, bwd, B, H, Nq, Nk, D, Q, ldq, K, ldk, V, ldv, mask, O, ldo, lse, dO=None, lddo=0, dQ=None, lddq=0,
                   dK=None, lddk=0, dV=None, lddv=0, delta=None, dbq=None, dbk=None, dbv=None, dropout=None, segs=None):
@@ -834,6 +904,9 @@ class Plan:
         a.O, a.ldo, a.lse = L.arg(O.hi), ldo, L.arg(lse)
         a.dO, a.lddo, a.dQ, a.lddq = L.arg(dO), lddo, L.arg(dQ), lddq
         a.dK, a.lddk, a.dV, a.lddv, a.delta = L.arg(dK), lddk, L.arg(dV), lddv, L.arg(delta)
+        if self.det and bwd:     # no atomics in the kernel: det_bias_sums takes ordered column sums of dQ / dK / dV instead
+            self._det_bias += [(db, dx, ld) for db, dx, ld in ((dbq, dQ, lddq), (dbk, dK, lddk), (dbv, dV, lddv)) if db is not None]
+            dbq = dbk = dbv = None
         a.dbias_q, a.dbias_k, a.dbias_v = L.arg(dbq), L.arg(dbk), L.arg(dbv)
         if dropout is not None:
             a.dropout = dropout
@@ -874,7 +947,10 @@ class Plan:
         """gbias: bias gradient of the Linear feeding this LayerNorm (column sums of dx), fused into the same pass. dy2: a second
         part of the output gradient (Act.g_add), added to dy as it is read."""
         tail = (x, H, gamma, mean, rstd, dx32, dx16, H, pre, H, ggamma, gbeta, gbias, M, H, out_drop, in_drop)
-        if dy2 is not None:
+        if self.det:
+            sums = any(g is not None for g in (ggamma, gbeta, gbias))
+            self.emit(self.lib.vb_layernorm_bwd_det, dy, dy2, H, *tail, self.det_ws(3 * L.VB_DET_LN_SLICES * H) if sums else None)
+        elif dy2 is not None:
             self.emit(self.lib.vb_add_layernorm_bwd, dy, dy2, H, *tail)
         else:
             self.emit(self.lib.vb_layernorm_bwd, dy, H, *tail)
@@ -1056,6 +1132,7 @@ class Plan:
                            dbq=None if gated else gq, dbk=None if gated else gk, dbv=gv, dropout=adrop, segs=segs)
             if self.packed:
                 self.zero_tail(tag, dqkv)
+            self.det_bias_sums()
             if gated:
                 # the gate Linear needs dz32 for its bias sum, dz16 for its weight gradient and for d pool
                 dyw_rg = self.trainable(prefix + ".self.dy.weight") or pool.rg
@@ -1151,6 +1228,7 @@ class Plan:
                 for stream, need, d in (("v", need1, dqkv1), ("t", need2, dqkv2)):
                     if need:
                         self.zero_tail(stream, d)
+            self.det_bias_sums()
             if need1:
                 self.linear_wgrad(dqkv1, L3, v.op.bw, Hv, Mv, L3, Hv, p + ".biattention.qkv1")
             if need2:
@@ -2704,16 +2782,27 @@ class Engine:
 
     def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
              loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-             input_grads=frozenset(), packed=None):
+             input_grads=frozenset(), packed=None, deterministic=None):
         """The cached plan of this shape and these options (Plan). vqa_loss=True is the round-1 spelling of loss="vqa"; frozen:
         ParamStore entry names that take no gradient; input_grads: the inputs of INPUT_GRAD_NAMES the backward also differentiates;
-        packed: (rows_t, rows_v) of a packed plan."""
+        packed: (rows_t, rows_v) of a packed plan. deterministic: bitwise-reproducible kernels (Plan); None reads
+        torch.are_deterministic_algorithms_enabled() now. The single-stream baseline has kernels without a deterministic variant: it
+        raises RuntimeError, or with torch's warn_only=True warns and builds the default plan."""
         frozen, input_grads = frozenset(frozen), frozenset(input_grads)
+        det = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
+        if det and self.ps.base:
+            msg = (f"{' and '.join(DET_MISSING_BASELINE)} (the backward of BaseBertForVLTasks' embeddings) add with float atomics and "
+                   "have no deterministic implementation; build the plan without torch.use_deterministic_algorithms(True), or with "
+                   "warn_only=True to run the default kernels")
+            if not torch.is_deterministic_algorithms_warn_only_enabled():
+                raise RuntimeError(msg)
+            warnings.warn(msg)
+            det = False
         loss = "vqa" if vqa_loss else loss
         pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
         key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward),
                None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix), frozen, input_grads,
-               None if packed is None else tuple(packed))
+               None if packed is None else tuple(packed), det)
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]
@@ -2723,6 +2812,8 @@ class Engine:
         if packed is not None and self.ps.base:
             raise NotImplementedError("packed plans run the two-stream VILBertForVLTasks only")
         extra = {} if packed is None else {"packed": packed}
+        if det:
+            extra["deterministic"] = True
         self.plans[key] = (BasePlan if self.ps.base else Plan)(
             self, B, Nt, Nv, grad_outputs, heads, train, loss=loss, choices=choices, score=score, loss_in_forward=loss_in_forward,
             outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen, input_grads=input_grads,
