@@ -1,8 +1,9 @@
-"""Times one evaluation batch (eval_tasks.py:290, EvaluatingModel) per task type on one GPU in two ways, alternating them in the
+"""Times one evaluation batch (eval_tasks.py:290, EvaluatingModel) per task type on one GPU in three ways, alternating them in the
 same process:
 
   fused      vilbert_b200.tasks.EvaluatingModel: a forward-only plan with only the type's head, objective, score and
              vb_task_results; one device-to-host copy
+  recycled   the same with engine.recycle_forward_only: the plan's buffers placed by lifetime (Plan(recycle=True))
   module     the module surface (VILBertForVLTasks.forward, all nine heads cloned) + the reference's step restated in
              tests/_eval_oracle.py (torch loss / score / softmax and one .item() per value)
 
@@ -10,10 +11,11 @@ same process:
 
 Model: bert_base_6layer_6conect with task tokens, random weights, eval mode. Shapes: the regions and tokens of the 12-in-1 tasks of
 each evaluation type (bench.py's config 5) at eval_tasks.py's default --batch_size 30 and at 256. Batches are synthetic CPU tensors
-(the arms move them to the GPU as the reference does). Both arms' plans share one activation arena; a shape whose plan does not fit
+(the arms move them to the GPU as the reference does). The arms' plans share one activation arena; an arm whose plan does not fit
 is reported as not measured. Prints one JSON line (also written to DIR/eval_step_probe.json): per (type, batch) the median ms per
-call of each arm and the bytes of each arm's plan, with the card name and power limit. Needs a GPU."""
+call of each arm and the bytes each arm's plan holds (Plan.held_bytes), with the card name and power limit. Needs a GPU."""
 import argparse
+import gc
 import json
 import os
 import statistics
@@ -34,11 +36,6 @@ SHAPES = [("VL-classifier", "TASK1", 101, 23, 0), ("VL-classifier-GQA", "TASK15"
 def card():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
     return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else "unknown"
-
-
-def plan_bytes(plan):
-    import torch
-    return plan.arena_bytes + sum(t.numel() * t.element_size() for t in plan._keep if torch.is_tensor(t))
 
 
 def main():
@@ -76,27 +73,39 @@ def main():
                 EvaluatingModel(None, cfg, dev, task, batch, model, loader, losses, [], [])
                 plans["fused"] = model._last_plan
 
+            def recycled():
+                model.engine.recycle_forward_only = True
+                try:
+                    EvaluatingModel(None, cfg, dev, task, batch, model, loader, losses, [], [])
+                finally:
+                    model.engine.recycle_forward_only = False
+                plans["recycled"] = model._last_plan
+
             def module():
                 E.evaluating_step(cfg, task, tuple(t.to(dev, non_blocking=True) for t in batch), model, label2ans, [], [])
                 plans["module"] = model._last_plan
-            arms = {"fused": fused, "module": module}
+            arms = {"fused": fused, "recycled": recycled, "module": module}
             times = {k: [] for k in arms}
             row = {"type": typ, "task": task, "B": B, "regions": Nv, "tokens": Nt + 1, "options": opts or None}
-            try:
-                for i in range(a.warmup + a.iters):
-                    for name, fn in arms.items():
-                        torch.cuda.synchronize()
-                        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                        e0.record()
+            for i in range(a.warmup + a.iters):
+                for name, fn in list(arms.items()):
+                    torch.cuda.synchronize()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    try:
                         fn()
-                        e1.record()
-                        torch.cuda.synchronize()
-                        if i >= a.warmup:
-                            times[name].append(e0.elapsed_time(e1))
-                row.update({f"ms_{k}_median": statistics.median(v) for k, v in times.items()})
-                row.update({f"plan_bytes_{k}": plan_bytes(p) for k, p in plans.items()})
-            except (L.VBError, torch.OutOfMemoryError) as ex:
-                row["not_measured"] = str(ex).splitlines()[0][:200]
+                    except (L.VBError, torch.OutOfMemoryError) as ex:
+                        row[f"not_measured_{name}"] = str(ex).splitlines()[0][:200]
+                        del arms[name], times[name]
+                        gc.collect()
+                        torch.cuda.empty_cache()
+                        continue
+                    e1.record()
+                    torch.cuda.synchronize()
+                    if i >= a.warmup:
+                        times[name].append(e0.elapsed_time(e1))
+            row.update({f"ms_{k}_median": statistics.median(v) for k, v in times.items()})
+            row.update({f"plan_bytes_{k}": p.held_bytes for k, p in plans.items() if k in arms})
             print(json.dumps(row), flush=True)
             rows.append(row)
             model.engine.release_plans()

@@ -1,14 +1,18 @@
 """Times caption-to-image retrieval at the reference's real shapes: bert_base_6layer_6conect with task tokens, 101 regions, 30 + 1
-tokens, a gallery of 1,000 random-feature images, random weights. Two arms alternate in one process after a warm-up:
+tokens, a gallery of 1,000 random-feature images, random weights. The arms of --arms alternate in one process after a warm-up:
 
-  (a) RetrievalEvaluator(chunk=500): each 500-image chunk loaded and embedded once, one graph replay per caption and chunk;
-  (b) the reference loop (eval_retrieval.py:264-313) restated on the module surface: model(...) per caption and gallery half with
-      config.fast_mode set, the half's features copied from pinned host memory on every call, the scores read back with .cpu().
+  plain     RetrievalEvaluator(chunk=--chunk): each chunk loaded and embedded once, one graph replay per caption and chunk;
+  recycled  the same with recycle=True at chunk=--recycled-chunk (default --chunk): the plans' buffers placed by lifetime;
+  module    the reference loop (eval_retrieval.py:264-313) restated on the module surface: model(...) per caption and gallery half
+            with config.fast_mode set, the half's features copied from pinned host memory on every call, the scores read back
+            with .cpu().
 
-    python tools/retrieval_probe.py [--captions 200] [--rounds 3] [--out retrieval_probe.json]
+    python tools/retrieval_probe.py [--captions 200] [--rounds 3] [--arms plain,module] [--chunk 500] [--recycled-chunk N]
+                                    [--out retrieval_probe.json]
 
-Reports ms per caption (median and min-max over the rounds), model TFLOP/s from the FLOPs of the plans' GEMMs and attentions, the
-evaluator's plan bytes, the card's name, power limit and SM clock, and how far the two arms' outputs agree."""
+Reports per arm ms per caption (median and min-max over the rounds), model TFLOP/s from the FLOPs of the plans' GEMMs and attentions,
+and for the evaluator arms the bytes their plans hold (Plan.held_bytes); the card's name, power limit and SM clock; and how far
+each arm's scores and ranks are from the first arm's."""
 import argparse
 import json
 import os
@@ -54,6 +58,9 @@ def main():
     ap.add_argument("--captions", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--images", type=int, default=1000)
+    ap.add_argument("--arms", default="plain,module")
+    ap.add_argument("--chunk", type=int, default=500)
+    ap.add_argument("--recycled-chunk", type=int, default=0)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     import vilbert_b200
@@ -73,12 +80,17 @@ def main():
     seg = torch.zeros(C, Nt, dtype=torch.long)
     target = torch.arange(C) % G
 
-    ev = RetrievalEvaluator(model, feats, locs, imask, chunk=half)
+    arms = a.arms.split(",")
+    bad = [x for x in arms if x not in ("plain", "recycled", "module")]
+    if bad:
+        raise SystemExit(f"retrieval_probe: unknown arm(s) {bad}")
+    evs = {"plain": RetrievalEvaluator(model, feats, locs, imask, chunk=a.chunk, recycle=False),
+           "recycled": RetrievalEvaluator(model, feats, locs, imask, chunk=a.recycled_chunk or a.chunk, recycle=True)}
 
-    def arm_a(n):
-        return ev.score(caps[:n], amask[:n], seg[:n], task_id=8)
+    def evaluator(name):
+        return lambda n: evs[name].score(caps[:n], amask[:n], seg[:n], task_id=8)
 
-    def arm_b(n):
+    def module_loop(n):
         model.config.fast_mode = True
         out = np.zeros((n, G), dtype=np.float32)
         task = torch.full((1, 1), 8, dtype=torch.long, device="cuda")
@@ -91,7 +103,8 @@ def main():
                                   imask[sl].cuda(non_blocking=True), task_ids=task)[2]
                     out[c, sl] = logit.view(-1).cpu().numpy()
         model.config.fast_mode = False
-        return out
+        return torch.from_numpy(out).cuda()
+    fns = {name: module_loop if name == "module" else evaluator(name) for name in arms}
 
     def timed(f, n):
         torch.cuda.synchronize()
@@ -100,34 +113,32 @@ def main():
         torch.cuda.synchronize()
         return (time.perf_counter() - t0) * 1e3 / n, r
 
-    timed(arm_a, 4)        # warm-up: plans, graph capture, kernels loaded
-    timed(arm_b, 4)
-    ta, tb = [], []
-    sa = sb = None
+    for f in fns.values():
+        timed(f, 4)        # warm-up: plans, graph capture, kernels loaded
+    times, scores = {k: [] for k in fns}, {}
     for _ in range(a.rounds):
-        t, sa = timed(arm_a, C)
-        ta.append(t)
-        t, sb = timed(arm_b, C)
-        tb.append(t)
+        for name, f in fns.items():
+            t, scores[name] = timed(f, C)
+            times[name].append(t)
     eng = model.engine
-    pa = [p for p in eng.plans.values() if p.image_prefix]
-    pb = [p for p in eng.plans.values() if not p.image_prefix and p.B == half]
-    flops_caption = sum(plan_flops(p) * (G // p.B) for p in pa if p.B == half) + sum(plan_flops(p) for p in pa if p.B != half and G % half)
-    flops_module = plan_flops(pb[0]) * (G // half) if pb else 0
-    ranks_a, _ = ev.rank(sa, target, k=20)
-    ranks_b, _ = ev.rank(torch.from_numpy(sb).cuda(), target, k=20)
-    res = dict(
-        card=card(), config="bert_base_6layer_6conect + task tokens", images=G, regions=Nv, tokens=Nt + 1, captions=C, rounds=a.rounds,
-        precision=eng.precision,
-        evaluator_ms_per_caption=dict(median=statistics.median(ta), min=min(ta), max=max(ta)),
-        module_loop_ms_per_caption=dict(median=statistics.median(tb), min=min(tb), max=max(tb)),
-        evaluator_tflops=flops_caption / (statistics.median(ta) * 1e-3) / 1e12,
-        module_loop_tflops=flops_module / (statistics.median(tb) * 1e-3) / 1e12,
-        flops_per_caption=flops_caption, module_flops_per_caption=flops_module,
-        evaluator_plan_bytes=sum(sum(t.numel() * t.element_size() for t in p._keep if torch.is_tensor(t)) for p in pa),
-        max_abs_score_diff=float((sa.cpu() - torch.from_numpy(sb)).abs().max()),
-        ranks_differing=int((ranks_a != ranks_b).sum()),
-    )
+    res = dict(card=card(), config="bert_base_6layer_6conect + task tokens", images=G, regions=Nv, tokens=Nt + 1, captions=C,
+               rounds=a.rounds, precision=eng.precision, arms={})
+    ranks0, _ = RetrievalEvaluator.rank(scores[arms[0]], target, k=20)
+    for name in arms:
+        med = statistics.median(times[name])
+        if name == "module":
+            pb = [p for p in eng.plans.values() if not p.image_prefix and p.B == half]
+            flops, held = (plan_flops(pb[0]) * (G // half) if pb else 0), None
+        else:
+            ps = [p for p in eng.plans.values() if p.image_prefix and p.recycle == (name == "recycled")]
+            flops = sum(plan_flops(p) for p in ps for _ in range(G // p.B if p.B == evs[name].chunk else 1))
+            held = {p.B: p.held_bytes for p in ps}
+        ranks, _ = RetrievalEvaluator.rank(scores[name], target, k=20)
+        res["arms"][name] = dict(chunk=None if name == "module" else evs[name].chunk,
+                                 ms_per_caption=dict(median=med, min=min(times[name]), max=max(times[name])),
+                                 tflops=flops / (med * 1e-3) / 1e12, flops_per_caption=flops, plan_held_bytes=held,
+                                 max_abs_score_diff_vs_first=float((scores[name] - scores[arms[0]]).abs().max()),
+                                 ranks_differing_vs_first=int((ranks != ranks0).sum()))
     text = json.dumps(res, indent=1)
     print(text)
     if a.out:

@@ -20,6 +20,7 @@ activations and weights exist only as tensor-core operands. Three operand precis
                     runs as three tensor-core passes (hi.hi + lo.hi + hi.lo), ~fp32 accuracy (north_star 1e-3);
   "bf16"            every operand bf16 (round-1 arithmetic; kept for A/B measurements).
 """
+import bisect
 import math
 import warnings
 import zlib
@@ -445,6 +446,114 @@ DET_WORKSPACE = {
 }
 # kernels of the single-stream baseline (BaseBertForVLTasks) with float atomics and no deterministic variant
 DET_MISSING_BASELINE = ("vb_concat_embed_ln_bwd", "vb_embed_text_bwd_padded")
+# streams an op list can name: main, vision, and the two weight-gradient side streams (Plan._run)
+N_STREAMS = 4
+# alignment of every buffer a plan places in a region of its own or in the shared arena
+BUF_ALIGN = 256
+
+
+def _struct_pointers(s):
+    for cls in reversed(type(s).__mro__):
+        for f, t in cls.__dict__.get("_fields_", ()):
+            v = getattr(s, f)
+            if t is L.C.c_void_p:
+                if v:
+                    yield v
+            elif isinstance(t, type) and issubclass(t, L.C.Structure):
+                yield from _struct_pointers(v)
+
+
+def op_pointers(fn, args):
+    """Every address one emitted launch passes: its void* arguments and the void* fields of the descriptor structs it passes by
+    reference (nested ones included)."""
+    for a, t in zip(args, fn.argtypes):
+        if a is None:
+            continue
+        if hasattr(a, "_obj"):
+            yield from _struct_pointers(a._obj)
+        elif t is L.C.c_void_p:
+            yield a
+
+
+def happens_before_clocks(sections):
+    """Vector clocks of the ops of `sections` (op lists run one after the other, every stream joined in between), from the stream
+    markers Plan._run issues: -> [(op, stream, own count, clock before the op)]. An op x happens before an op y exactly when
+    x's own count is at most y's clock-before entry for x's stream."""
+    vc = [[0] * N_STREAMS for _ in range(N_STREAMS)]
+    out, events = [], {}
+
+    def join(dst, src):
+        vc[dst] = [max(a, b) for a, b in zip(vc[dst], src)]
+    for ops in sections:
+        for s in range(N_STREAMS):              # a run starts after everything before it
+            join(0, vc[s])
+        for s in range(1, N_STREAMS):
+            join(s, vc[0])
+        for op in ops:
+            fn, args, sid = op
+            if fn is None:
+                if not args:                    # text <-> vision barrier
+                    join(1, vc[0]); join(0, vc[1])
+                elif args[0] == "all":
+                    for s in range(1, N_STREAMS):
+                        join(s, vc[0])
+                    for s in range(1, N_STREAMS):
+                        join(0, vc[s])
+                elif args[0] == "rec":
+                    events[args[1]] = list(vc[sid])
+                elif args[0] == "wait":
+                    join(sid, events[args[1]])
+                continue
+            before = list(vc[sid])
+            vc[sid][sid] += 1
+            out.append((op, sid, vc[sid][sid], before))
+    return out
+
+
+def lifetime_layout(sections, spans, pinned):
+    """First-fit placement by decreasing size of the byte ranges `spans` ((address, nbytes) of the buffers of a recording build,
+    indexed) over their conflict graph. Two buffers conflict unless every use of one happens before every use of the other
+    (happens_before_clocks) on the ops of `sections`; the buffers in `pinned` conflict with every used buffer (they live for the
+    whole plan), and a buffer no op uses with none (it sits at offset 0, and the extent covers it). -> (offset per index, extent),
+    offsets aligned to BUF_ALIGN."""
+    n, S = len(spans), N_STREAMS
+    big = 1 << 62
+    last = [[0] * S for _ in range(n)]          # per stream: the latest own count of a use
+    first = [[big] * S for _ in range(n)]       # per stream: the least clock-before entry over the uses
+    used = [False] * n
+    order = sorted((a, i) for i, (a, nb) in enumerate(spans) if nb > 0)
+    starts = [a for a, _ in order]
+    for op, s, own, before in happens_before_clocks(sections):
+        fn, args, _ = op
+        for p in op_pointers(fn, args):
+            k = bisect.bisect_right(starts, p) - 1
+            if k < 0:
+                continue
+            i = order[k][1]
+            if p >= spans[i][0] + spans[i][1]:
+                continue
+            used[i] = True
+            last[i][s] = max(last[i][s], own)
+            first[i] = [min(a, b) for a, b in zip(first[i], before)]
+    for i in pinned:
+        last[i], first[i], used[i] = [big] * S, [0] * S, True
+
+    def before(i, j):
+        return all(a <= b for a, b in zip(last[i], first[j]))
+    size = [-(-nb // BUF_ALIGN) * BUF_ALIGN for _, nb in spans]
+    offset, placed = [0] * n, []
+    extent = max([0] + [size[i] for i in range(n) if not used[i]])
+    for i in sorted((i for i in range(n) if used[i] and size[i]), key=lambda i: (-size[i], i)):
+        taken = sorted((offset[j], offset[j] + size[j]) for j in placed if not (before(i, j) or before(j, i)))
+        off = 0
+        for a, b in taken:
+            if off + size[i] <= a:
+                break
+            off = max(off, b)
+        offset[i] = off
+        placed.append(i)
+        extent = max(extent, off + size[i])
+    return offset, extent
 
 
 class Plan:
@@ -495,11 +604,36 @@ class Plan:
     order-dependent goes through the _det variant of its kernel (per-block partials in a workspace of the plan, then one ordered
     sum), the GEMM weight gradients that split K store their splits apart and add them in split order, and all launches go to one
     stream, so no two kernels add into the same range concurrently. Two runs give bitwise identical results on the same GPU model
-    and build. self.det_ws_bytes: the workspace the plan allocated for it."""
+    and build. self.det_ws_bytes: the workspace the plan allocated for it.
+
+    recycle=True (forward-only plans: no train mode, no grad_outputs, no input_grads; DESIGN.md §3): buffers whose lifetimes are
+    disjoint share bytes. The plan is built twice in the same order. The first build records every buffer request in host memory
+    that it does not fill (also under torch.use_deterministic_algorithms(True)); the vector clocks of its ops (happens_before_clocks) give each buffer its uses, and lifetime_layout
+    places them. The second build emits the same launches with each buffer at its place, in one region of the plan or, with the
+    shared arena, at the start of the arena (arena_bytes is the extent). Private buffers and the buffers the host reads after a run
+    (_host_reads) keep bytes of their own. self.held_bytes: arena extent + the plan's own device buffers."""
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
                  loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-                 input_grads=frozenset(), packed=None, deterministic=False):
+                 input_grads=frozenset(), packed=None, deterministic=False, recycle=False, _recording=False):
+        self.recycle = bool(recycle)
+        if self.recycle and (train or grad_outputs or input_grads):
+            raise ValueError("recycle=True shares the bytes of buffers whose lifetimes are disjoint, which only a forward-only plan "
+                             "has: no train mode, no grad_outputs, no input_grads (the backward reads the saved activations)")
+        self._requests = [] if _recording else None     # recording build: (tensor, bytes, private) per buffer request
+        self._place, self._n_req, self._region = None, 0, None
+        if self.recycle:
+            # the recording build's buffers are address ranges only: torch.use_deterministic_algorithms(True) would fill each
+            # torch.empty with NaN, writing host memory as large as the plain plan
+            fill = torch.utils.deterministic.fill_uninitialized_memory
+            torch.utils.deterministic.fill_uninitialized_memory = False
+            try:
+                rec = Plan.__new__(type(self))
+                Plan.__init__(rec, engine, B, Nt, Nv, grad_outputs, heads, train, loss, choices, score, loss_in_forward, outputs,
+                              results, fast_mode, image_prefix, frozen, input_grads, packed, deterministic, _recording=True)
+            finally:
+                torch.utils.deterministic.fill_uninitialized_memory = fill
+            self._place = rec._lifetime_placement()
         self.e, self.cfg = engine, engine.cfg
         self.det = bool(deterministic)
         self._det_ws, self.det_ws_bytes = None, 0
@@ -574,7 +708,11 @@ class Plan:
         self.graph_fwd = self.graph_bwd = self.graph_step = None
         self._eager_runs = [0, 0]      # eager forward / backward executions (maybe_capture_passes)
         self._arena_off = self.arena_bytes = 0
+        if self._place is not None:
+            self._open_region()
         self._build()
+        if self._place is not None and self._n_req != len(self._place[0]):
+            raise L.VBError(f"recycled plan: the second build made {self._n_req} buffer requests, the first {len(self._place[0])}")
 
     def _stream_modes(self, B, Nt, Nv, train, grad_outputs, loss, fast_mode, image_prefix):
         """Shapes and checks of the two-stream options: in_batch_pairs, the task token, visualization, dynamic_attention,
@@ -719,15 +857,30 @@ class Plan:
         that hold no state between runs (activations, scratch: everything a run writes before reading) are sub-allocated from the
         arena at the same offsets in every plan, so the plans of different shapes overlay each other; buffers that are
         initialised at build time or loaded from outside a run (zero=True: inputs, labels, output gradients, zero-padded
-        operands) stay private."""
+        operands) stay private.
+
+        A recycled plan (recycle=True) places the other buffers where its recording build's lifetimes put them (_place), in
+        its region (_open_region); the recording build itself hands out host memory it does not fill."""
         arena = self.e.arena
         zero = zero or self._private
+        n = math.prod(int(d) for d in (shape if isinstance(shape, (tuple, list)) else (shape,)))
+        nbytes = n * torch.empty((), dtype=dtype).element_size()
+        if self._requests is not None:
+            t = torch.empty(shape, dtype=dtype)
+            self._requests.append((t, nbytes, zero))
+            return t
+        if self._place is not None:
+            sigs, offsets, _ = self._place
+            i = self._n_req
+            self._n_req += 1
+            if i >= len(sigs) or sigs[i] != (nbytes, zero):
+                raise L.VBError(f"recycled plan: buffer request {i} ({nbytes} bytes, private={zero}) differs from the recording build's")
+            if not zero:
+                return self._region[offsets[i]:offsets[i] + nbytes].view(dtype).view(shape)
         if arena is None or zero:
             t = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=self.dev)
             self._keep.append(t)
             return t
-        n = math.prod(int(d) for d in (shape if isinstance(shape, (tuple, list)) else (shape,)))
-        nbytes = n * torch.empty((), dtype=dtype).element_size()
         off = self._arena_off
         if off + nbytes > arena.numel():
             raise L.VBError(f"activation arena of {arena.numel() / 2**30:.2f} GiB is too small for plan B={self.B} Nt={self.Nt} Nv={self.Nv} "
@@ -735,6 +888,45 @@ class Plan:
         self._arena_off = (off + nbytes + 255) // 256 * 256
         self.arena_bytes = self._arena_off
         return arena[off:off + nbytes].view(dtype).view(shape)
+
+    def _host_reads(self):
+        """The tensors the host may read after a run, besides the private buffers: the outputs, the encoded layers
+        (output_all_encoded_layers) and the attention exports of config.visualization."""
+        acts = getattr(self, "enc_t", []) + getattr(self, "enc_v", []) + getattr(self, "enc", [])
+        attn = self.attn_t + self.attn_v + [d for pair in self.attn_c for d in pair]
+        return list(self.outputs.values()) + [a.f32 for a in acts] + [d[k] for d in attn for k in ("attn", "q", "k")]
+
+    def _lifetime_placement(self):
+        """Of a recording build: (per request (bytes, private), per request its offset in the recycled region or None when
+        private, the region's extent). The one rule of what is not recycled: a private buffer stays private, and a buffer the host
+        reads after a run (_host_reads) lives for the whole plan."""
+        reqs = self._requests
+        spans = [(t.data_ptr(), 0 if zero else nb) for t, nb, zero in reqs]
+        pinned = set()
+        for t in self._host_reads():
+            p = t.data_ptr()
+            pinned.update(i for i, (a, nb) in enumerate(spans) if a <= p < a + nb)
+        offsets, extent = lifetime_layout((self.prefix, self.fwd, self.bwd), spans, pinned)
+        return ([(nb, zero) for _, nb, zero in reqs], [None if zero else off for (_, _, zero), off in zip(reqs, offsets)], extent)
+
+    def _open_region(self):
+        """The bytes a recycled plan places its buffers in: the start of the shared arena (its extent is arena_bytes), or one
+        device buffer of its own."""
+        extent, arena = max(self._place[2], 1), self.e.arena
+        if arena is None:
+            self._region = torch.empty(extent, dtype=torch.uint8, device=self.dev)
+            self._keep.append(self._region)
+            return
+        if extent > arena.numel():
+            raise L.VBError(f"activation arena of {arena.numel() / 2**30:.2f} GiB is too small for plan B={self.B} Nt={self.Nt} Nv={self.Nv} "
+                            f"(needs {extent / 2**30:.2f} GiB): pass a larger size to Engine.enable_activation_arena")
+        self._region = arena
+        self.arena_bytes = extent
+
+    @property
+    def held_bytes(self):
+        """Device bytes the plan holds: its extent of the shared arena and its own buffers."""
+        return self.arena_bytes + sum(t.numel() * t.element_size() for t in self._keep if torch.is_tensor(t))
 
     def buf16(self, shape, bw=True):
         """Forward-operand buffer in the engine's operand format; bw=False: no bf16 copy (nothing in the backward reads it)."""
@@ -767,7 +959,7 @@ class Plan:
         larger than the current buffer allocates a new one; the launches emitted before keep the old one, so the plan holds every
         size the workspace grew through (all counted in det_ws_bytes)."""
         if self._det_ws is None or self._det_ws.numel() < n:
-            self._det_ws = torch.empty(max(int(n), 1), dtype=F32, device=self.dev)
+            self._det_ws = torch.empty(max(int(n), 1), dtype=F32, device="cpu" if self._requests is not None else self.dev)
             self._keep.append(self._det_ws)
             self.det_ws_bytes += self._det_ws.numel() * 4
         return self._det_ws
@@ -2496,11 +2688,12 @@ class BasePlan(Plan):
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
                  loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-                 input_grads=frozenset()):
+                 input_grads=frozenset(), recycle=False):
         if (loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
                 or loss_in_forward):
-            raise ValueError("single-stream baseline plans support grad_outputs, train, frozen and input_grads only")
-        super().__init__(engine, B, Nt, Nv, grad_outputs, heads=heads, train=train, choices=choices, frozen=frozen, input_grads=input_grads)
+            raise ValueError("single-stream baseline plans support grad_outputs, train, frozen, input_grads and recycle only")
+        super().__init__(engine, B, Nt, Nv, grad_outputs, heads=heads, train=train, choices=choices, frozen=frozen, input_grads=input_grads,
+                         recycle=recycle)
 
     def _stream_modes(self, B, Nt, Nv, *_):
         self.pairs = self.has_task = self.viz = self.dyn = self.fast = self.image_prefix = False
@@ -2767,6 +2960,9 @@ class Engine:
         self.shadow_trusted = False      # True while the engine's own fused optimizer is the only writer of the parameters
         self.grad_clean = False          # the flat gradient buffer is all zeros (set by zero_grad / the fused optimizer)
         self.loss_options = 4            # answer options per question of the VL-logit objective (retrieval / VCR: 4)
+        # forward-only plans (no train mode, no grad_outputs, no input_grads) share the bytes of buffers with disjoint lifetimes
+        # (Plan(recycle=True)); the default of Engine.plan(recycle=None)
+        self.recycle_forward_only = False
         self.auto_graph = True           # module surface: capture a plan's passes into CUDA graphs after two eager runs
         self.arena = None                # optional shared activation arena (enable_activation_arena)
         self.arena_owner = None          # (plan, forward id) whose activations the arena currently holds
@@ -2782,13 +2978,16 @@ class Engine:
 
     def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
              loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-             input_grads=frozenset(), packed=None, deterministic=None):
+             input_grads=frozenset(), packed=None, deterministic=None, recycle=None):
         """The cached plan of this shape and these options (Plan). vqa_loss=True is the round-1 spelling of loss="vqa"; frozen:
         ParamStore entry names that take no gradient; input_grads: the inputs of INPUT_GRAD_NAMES the backward also differentiates;
         packed: (rows_t, rows_v) of a packed plan. deterministic: bitwise-reproducible kernels (Plan); None reads
         torch.are_deterministic_algorithms_enabled() now. The single-stream baseline has kernels without a deterministic variant: it
-        raises RuntimeError, or with torch's warn_only=True warns and builds the default plan."""
+        raises RuntimeError, or with torch's warn_only=True warns and builds the default plan. recycle: buffers placed by lifetime
+        (Plan); None takes engine.recycle_forward_only for a forward-only plan and leaves any other plan as it is."""
         frozen, input_grads = frozenset(frozen), frozenset(input_grads)
+        if recycle is None:
+            recycle = self.recycle_forward_only and not (train or grad_outputs or input_grads)
         det = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
         if det and self.ps.base:
             msg = (f"{' and '.join(DET_MISSING_BASELINE)} (the backward of BaseBertForVLTasks' embeddings) add with float atomics and "
@@ -2802,7 +3001,7 @@ class Engine:
         pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
         key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward),
                None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix), frozen, input_grads,
-               None if packed is None else tuple(packed), det)
+               None if packed is None else tuple(packed), det, bool(recycle))
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]
@@ -2814,6 +3013,8 @@ class Engine:
         extra = {} if packed is None else {"packed": packed}
         if det:
             extra["deterministic"] = True
+        if recycle:
+            extra["recycle"] = True
         self.plans[key] = (BasePlan if self.ps.base else Plan)(
             self, B, Nt, Nv, grad_outputs, heads, train, loss=loss, choices=choices, score=score, loss_in_forward=loss_in_forward,
             outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen, input_grads=input_grads,

@@ -436,13 +436,16 @@ class BertPreTrainedModel(nn.Module):
         """The plan of the outputs `names`. A plan is specialised on the set of outputs that receive a gradient; the set `live` a
         backward found is kept as the hint for the next forward of this shape, so in a steady training loop forward and backward
         share one plan and nothing is recomputed. It is also specialised on the frozen parameters (default: the current
-        requires_grad flags) and on the inputs it differentiates (_input_grads)."""
+        requires_grad flags) and on the inputs it differentiates (_input_grads). With engine.recycle_forward_only an eval-mode call
+        under torch.no_grad() takes the forward-only plan, whose buffers are placed by lifetime (Plan(recycle=True))."""
         if frozen is None:
             frozen = self._frozen()
         Nt = inputs["input_txt"].shape[1]
         B, Nv = inputs["input_imgs"].shape[:2]     # FAST_MODE: the text batch is 1, the image batch sets the plan
         key = (B, Nt, Nv, names, train)
-        if live is None:
+        if live is None and self.engine.recycle_forward_only and not train and not torch.is_grad_enabled():
+            live = ()
+        elif live is None:
             live = self._grad_hint.get(key, ())
         else:
             self._grad_hint[key] = live

@@ -90,9 +90,11 @@ class RetrievalEvaluator:
 
     model: VILBertForVLTasks (scores = vil_logit) or BertForMultiModalPreTraining (zero shot: softmax(seq_relationship_score, 1)[:, 0]),
     in eval mode. features f32 [G, Nv, 2048], spatials f32 [G, Nv, 5], image_mask [G, Nv], on the host (staged through pinned memory
-    one chunk at a time) or on the model's device. Chunks of `chunk` images share one plan; a smaller last chunk gets its own."""
+    one chunk at a time) or on the model's device. Chunks of `chunk` images share one plan; a smaller last chunk gets its own.
+    recycle: build the plans with their buffers placed by lifetime (Plan(recycle=True)), which holds a fraction of the bytes at the
+    same launches and scores; None takes engine.recycle_forward_only."""
 
-    def __init__(self, model, features, spatials, image_mask, chunk=500):
+    def __init__(self, model, features, spatials, image_mask, chunk=500, recycle=None):
         self.model = model
         heads = getattr(model, "_heads", None)
         if heads not in SCORE_HEAD:
@@ -112,9 +114,11 @@ class RetrievalEvaluator:
         self.chunk = min(int(chunk), self.G)
         self.heads = heads
         self.head = SCORE_HEAD[heads]
+        self.recycle = recycle
 
     def _plan(self, n, Nt):
-        return self.model.engine.plan(n, Nt, self.Nv, heads=self.heads, outputs=(self.head,), fast_mode=True, image_prefix=True)
+        return self.model.engine.plan(n, Nt, self.Nv, heads=self.heads, outputs=(self.head,), fast_mode=True, image_prefix=True,
+                                      recycle=self.recycle)
 
     def _load_chunk(self, plan, lo, n):
         dev = self.model.engine.device
