@@ -301,7 +301,8 @@ vb_status vb_bce_logits_loss(const float* logits, const float* target, float* lo
  * used at vilbert.py:1578-1590 for the masked-LM (30522-way, ignore_index -1) and alignment objectives and at
  * task_utils.py:339-343, 366-374 for the VL-logit / binary / tri heads). *loss (device scalar) = the mean (+= when
  * accumulate_loss); dlogits = grad_scale * d loss / d logits as f32 and/or bf16 (the operand of the head's backward GEMMs),
- * zero on ignored rows. No rows to average -> loss = NaN like torch, gradients 0. */
+ * zero on ignored rows. No rows to average -> loss = NaN like torch, gradients 0. A label outside [0, cols) other than ignore_index
+ * reads nothing: its row's gradient is 0 and the loss is NaN. */
 vb_status vb_ce_loss(const float* logits, int64_t ld_logits, const int64_t* labels, int64_t ignore_index, float* loss,
                      float* dlogits_f32, int64_t ld_d32, void* dlogits_bf16, int64_t ld_d16, int32_t rows, int32_t cols,
                      float grad_scale, int32_t accumulate_loss, void* stream);

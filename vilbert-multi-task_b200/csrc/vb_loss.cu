@@ -48,6 +48,7 @@ __device__ __forceinline__ float block_count(const long long* labels, int n, flo
 
 // F.cross_entropy(logits [rows, cols], labels [rows], ignore_index), reduction = mean over the non-ignored rows.
 // One CTA per row (grid-stride). loss += sum over its rows of (lse - z[label]) / n_valid; dlogits = (softmax - onehot) * gs / n_valid.
+// A label outside [0, cols) (and != ignore_index) reads nothing: its row's gradient is 0 and the loss is NaN, as in bce_gather_rows.
 // PARTIALS (deterministic plans): CTA b stores its share, with the NaN of "no valid row" in CTA 0's, into part[b] instead of adding
 // it to *loss; vb_ce_loss_det sums the shares in CTA order.
 template <bool PARTIALS>
@@ -64,11 +65,13 @@ ce_loss_body(const float* __restrict__ z, long long ldz, const long long* __rest
     const long long lab = labels[r];
     const float* zr = z + (long long)r * ldz;
     const bool live = lab != ignore_index;
-    if (!live) {   // ignored row: zero gradient
+    const bool in_range = lab >= 0 && lab < cols;
+    if (!live || !in_range) {   // ignored row: zero gradient; a label outside [0, cols) reads nothing and makes the loss NaN
       for (int c = threadIdx.x; c < cols; c += LOSS_THREADS) {
         if (d32) d32[(long long)r * ldd32 + c] = 0.f;
         if (d16) d16[(long long)r * ldd16 + c] = __float2bfloat16(0.f);
       }
+      if (live && threadIdx.x == 0) local += CUDART_NAN_F;
       continue;
     }
     float mx = -CUDART_INF_F;
