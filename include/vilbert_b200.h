@@ -635,6 +635,21 @@ vb_status vb_kl_masked_loss_det(const float* scores, const float* target, const 
                                 void* dscores_bf16, int64_t ld_d16, int32_t B, int32_t Nv, int32_t C, float grad_scale,
                                 int32_t accumulate_loss, float* ws, void* stream);
 
+/* ---- anomaly detection (torch.autograd.set_detect_anomaly(True); plans built with Plan(anomaly=True), DESIGN.md §4i)
+ * vb_nan_check scans the regions of a device table on `stream`: region r is rows x cols elements of dtype at ptr, row pitch ld
+ * ELEMENTS; only that logical extent is read, never the pitch padding. When a region holds a NaN (an exponent of all ones and a
+ * non-zero mantissa, either sign, any payload; an inf is not one) the launch does atomicMin(flag, id). The test is on the bits,
+ * so it holds under --use_fast_math. 128-bit loads where a run is 16-byte aligned; every CTA strides over every region, so one
+ * launch covers many small regions and a few large ones. reset != 0 (n_regions == 0): *flag = INT32_MAX instead. */
+enum { VB_NAN_F32 = 0, VB_NAN_F16 = 1, VB_NAN_BF16 = 2 };
+typedef struct vb_nan_region {
+  const void* ptr;
+  int64_t rows, cols, ld;
+  int32_t dtype;   /* VB_NAN_F32 | VB_NAN_F16 | VB_NAN_BF16 */
+  int32_t id;
+} vb_nan_region;
+vb_status vb_nan_check(const vb_nan_region* regions, int32_t n_regions, int32_t* flag, int32_t reset, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -165,6 +165,15 @@ def deterministic_cases(O, E, base_labels):
             for name, over, heads, B, kw, *extra in every if not heads.startswith("base")]
 
 
+def anomaly_cases(O, E, base_labels):
+    """Every case above that has a backward (grad_outputs or input_grads) again with anomaly=True (named anomaly_...), the
+    deterministic ones included: the plans torch.autograd.set_detect_anomaly(True) selects."""
+    every = (cases(O, E, base_labels) + input_grad_cases(O, E, base_labels) + packed_cases(E) + packed_pretraining_cases(E) +
+             deterministic_cases(O, E, base_labels))
+    return [(f"anomaly_{name}", over, heads, B, dict(kw, anomaly=True), *extra)
+            for name, over, heads, B, kw, *extra in every if kw.get("grad_outputs") or kw.get("input_grads")]
+
+
 def dump_cases(out, case_list, prec, Engine, BertConfig, tiny, tiny_base):
     """Lists every plan of `case_list` in precision `prec`, without and with the shared activation arena. -> (plans, op records)"""
     n_plans = n_ops = 0
@@ -319,6 +328,12 @@ def main():
     if hasattr(E, "DET_WORKSPACE"):
         for prec in PRECISIONS:
             p, o = dump_cases(out, deterministic_cases(O, E, tiny_base["num_labels"]), prec, Engine, BertConfig, tiny, tiny_base)
+            n_plans, n_ops = n_plans + p, n_ops + o
+    # anomaly checks (torch.autograd.set_detect_anomaly(True)): listed last, so that the listing of a tree without them is a prefix
+    # of this one
+    if hasattr(E, "ANOMALY_OUTPUTS"):
+        for prec in PRECISIONS:
+            p, o = dump_cases(out, anomaly_cases(O, E, tiny_base["num_labels"]), prec, Engine, BertConfig, tiny, tiny_base)
             n_plans, n_ops = n_plans + p, n_ops + o
     text = "\n".join(out) + "\n"
     if a.out:

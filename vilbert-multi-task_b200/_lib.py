@@ -162,7 +162,17 @@ _SIGNATURES = {
     "vb_bce_logits_loss_det": [_P, _P, _P, _P, _P, _I64, _I32, _I32, _F, _P, _P],
     "vb_ce_loss_det": [_P, _I64, _P, _I64, _P, _P, _I64, _P, _I64, _I32, _I32, _F, _I32, _P, _P],
     "vb_kl_masked_loss_det": [_P, _P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _F, _I32, _P, _P],
+    "vb_nan_check": [_P, _I32, _P, _I32, _P],
 }
+# anomaly detection (include/vilbert_b200.h): the dtype codes of a vb_nan_region
+VB_NAN_F32, VB_NAN_F16, VB_NAN_BF16 = 0, 1, 2
+
+
+class NanRegion(C.Structure):
+    """Mirror of ``struct vb_nan_region``."""
+
+    _fields_ = [("ptr", C.c_void_p), ("rows", C.c_int64), ("cols", C.c_int64), ("ld", C.c_int64), ("dtype", C.c_int32),
+                ("id", C.c_int32)]
 # device scratch of one vb_weight_norm_fwd / _bwd launch (include/vilbert_b200.h)
 VB_WEIGHT_NORM_SCRATCH = 1024
 # deterministic variants (include/vilbert_b200.h): the partials mode of vb_gemm_bf16 and the workspace slices of the _det entry points

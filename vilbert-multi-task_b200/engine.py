@@ -372,12 +372,13 @@ class Act:
     The output of a residual LayerNorm (Plan.dense_res_ln) has one reader of its gradient, that LayerNorm's backward, which can add
     a second fp32 input as it reads (ln_reads). Its first writer may leave its residual-path part in g_add instead of adding it in a
     GEMM epilogue; a later writer adds g_add into g32 first (Plan._fold_g_add), so every sum keeps the order it has without it."""
-    __slots__ = ("f32", "op", "g32", "gw", "M", "H", "rg", "ln_reads", "g_add")
+    __slots__ = ("f32", "op", "g32", "gw", "M", "H", "rg", "ln_reads", "g_add", "mod")
 
     def __init__(self, f32, op, M, H, rg):
         self.f32, self.op, self.M, self.H, self.rg = f32, op, M, H, rg
         self.g32, self.gw = None, False
         self.ln_reads, self.g_add = False, None
+        self.mod = None          # module path of the block whose output this is (anomaly labels of the gradient delivered into it)
 
 
 # Objectives that can be fused into a plan, and the outputs each differentiates (task_utils.py:325-374, vilbert.py:1506-1590):
@@ -448,6 +449,110 @@ DET_WORKSPACE = {
 DET_MISSING_BASELINE = ("vb_concat_embed_ln_bwd", "vb_embed_text_bwd_padded")
 # streams an op list can name: main, vision, and the two weight-gradient side streams (Plan._run)
 N_STREAMS = 4
+
+# anomaly detection (Plan(anomaly=True), torch.autograd.set_detect_anomaly(True), DESIGN.md §4i): per entry point that runs in the
+# backward role, the gradient values one launch writes, read from the launch's own arguments (C values as emitted) as
+# (output name, pointer, rows, cols, ld in elements, VB_NAN_* dtype); a null pointer is an output the launch does not write. `p` is
+# the plan, for the extents no argument carries: the rows of a packed stream (_attn_rows), of a scattered-into buffer (_buf_rows)
+# and the ranges of parameter gradients (_param_numel). The workspaces of the row-wise _det kernels are not listed: a launch
+# writes only the slices it uses. An entry point emitted in the backward role without an entry fails when the plan is built.
+_F32, _BF16 = L.VB_NAN_F32, L.VB_NAN_BF16
+
+
+def _gemm_outputs(p, a):
+    g = a[0]._obj
+    rows = g.M * (g.split_k if g.atomic_out == L.VB_GEMM_PARTIALS else 1)     # deterministic split-K: one slice per split
+    return [("out_f32", g.out_f32, rows, g.N, g.ld_out_f32, _F32),
+            ("out_bf16", g.out_bf16, g.M, g.N, g.ld_out_bf16, L.VB_NAN_F16 if g.out_fp16 else _BF16),
+            ("out_colsum", g.out_colsum, 1, g.N, g.N, _F32)]
+
+
+def _attn_bwd_outputs(p, a):
+    x = a[0]._obj
+    hd, rq, rk = x.H * x.D, p._attn_rows(x.q_off, x.B, x.Nq), p._attn_rows(x.k_off, x.B, x.Nk)
+    return [("dQ", x.dQ, rq, hd, x.lddq, _BF16), ("dK", x.dK, rk, hd, x.lddk, _BF16), ("dV", x.dV, rk, hd, x.lddv, _BF16),
+            ("dbias_q", x.dbias_q, 1, hd, hd, _F32), ("dbias_k", x.dbias_k, 1, hd, hd, _F32), ("dbias_v", x.dbias_v, 1, hd, hd, _F32)]
+
+
+def _ln_bwd_outputs(o):
+    """vb_layernorm_bwd (o = 0) and vb_add_layernorm_bwd / vb_layernorm_bwd_det (o = 1: the dy2 argument)."""
+    def f(p, a):
+        M, H, ld = a[15 + o], a[16 + o], a[9 + o]
+        return [("dx_f32", a[7 + o], M, H, ld, _F32), ("dx_bf16", a[8 + o], M, H, ld, _BF16), ("dgamma", a[12 + o], 1, H, H, _F32),
+                ("dbeta", a[13 + o], 1, H, H, _F32), ("dbias", a[14 + o], 1, H, H, _F32)]
+    return f
+
+
+def _vec(name, ptr, n, dt=_F32):
+    return (name, ptr, 1, n, n, dt)
+
+
+def _tables(names, first):
+    """Embedding-table gradients at arguments first, first + 1, ...: whole parameter ranges."""
+    return lambda p, a: [_vec(n, a[first + i], p._param_numel(a[first + i])) for i, n in enumerate(names)]
+
+
+_small_linear = lambda p, a: [("dx", a[4], a[9], a[10], a[5], _F32), _vec("dW", a[7], a[11] * a[10]), _vec("db", a[8], a[11])]
+_loc_proj = lambda p, a: [_vec("dW", a[2], 5 * a[5]), _vec("db", a[3], a[5])]
+_ce = lambda p, a: [("dlogits_f32", a[5], a[9], a[10], a[6], _F32), ("dlogits_bf16", a[7], a[9], a[10], a[8], _BF16)]
+_bce = lambda p, a: [("dlogits_f32", a[3], a[6], a[7], a[7], _F32), ("dlogits_bf16", a[4], a[6], a[7], a[5], _BF16)]
+_kl = lambda p, a: [("dscores_f32", a[4], a[7] * a[8], a[9], a[9], _F32), ("dscores_bf16", a[5], a[7] * a[8], a[9], a[6], _BF16)]
+_region_loss = lambda i: lambda p, a: [("dscores_f32", a[i], a[3 if i == 10 else 4] * a[4 if i == 10 else 5],
+                                         a[5 if i == 10 else 6], a[5 if i == 10 else 6], _F32)]
+ANOMALY_OUTPUTS = {
+    "vb_gemm_bf16": _gemm_outputs,
+    "vb_attention_bwd": _attn_bwd_outputs,
+    "vb_layernorm_bwd": _ln_bwd_outputs(0),
+    "vb_add_layernorm_bwd": _ln_bwd_outputs(1),
+    "vb_layernorm_bwd_det": _ln_bwd_outputs(1),
+    "vb_colsum": lambda p, a: [_vec("out", a[3], a[5])],
+    "vb_colsum_det": lambda p, a: [_vec("out", a[3], a[5])],
+    "vb_reduce_slices": lambda p, a: [_vec("dst", a[4], a[3])],
+    "vb_memset_zero": lambda p, a: [_vec("ptr", a[0], a[1] // 4)],
+    "vb_axpy_f32": lambda p, a: [_vec("y", a[1], a[2])],
+    "vb_embed_text_bwd": _tables(("dword", "dpos", "dtype", "dtask"), 4),
+    "vb_embed_text_bwd_det": _tables(("dword", "dpos", "dtype", "dtask"), 4),
+    "vb_embed_text_bwd_padded": _tables(("dword", "dpos", "dtype"), 3),
+    "vb_loc_proj_bwd": _loc_proj,
+    "vb_loc_proj_bwd_det": _loc_proj,
+    "vb_loc_proj_dx": lambda p, a: [("dx", a[2], a[3], 5, 5, _F32)],
+    "vb_small_linear_bwd": _small_linear,
+    "vb_small_linear_bwd_det": _small_linear,
+    "vb_fuse_pooled_bwd": lambda p, a: [_vec("da", a[3], a[5]), _vec("db", a[4], a[5])],
+    "vb_relu_bwd": lambda p, a: [_vec("dx_bf16", a[2], a[4], _BF16), _vec("dx_f32", a[3], a[4])],
+    "vb_sum_strided": lambda p, a: [_vec("dst", a[1], a[3] * a[2])],
+    "vb_masked_mean_bwd": lambda p, a: [("dx", a[2], a[4] * a[5], a[6], a[6], _F32)],
+    "vb_gate_scale_bwd": lambda p, a: [("dqk", a[0], a[8] * a[9], a[10], a[1], _BF16), ("dz", a[6], a[8], a[10], a[10], _F32),
+                                       ("dz16", a[7], a[8], a[10], a[10], _BF16)],
+    "vb_scatter_rows_f32": lambda p, a: [("dst", a[1], p._buf_rows[a[1]], a[4], a[4], _F32)],
+    "vb_scatter_add_rows_f32": lambda p, a: [("dst", a[1], p._buf_rows[a[1]], a[4], a[4], _F32)],
+    "vb_pack_rows_f32": lambda p, a: [("dst", a[1], a[3], a[4], a[4], _F32)],
+    "vb_unpack_rows_f32": lambda p, a: [("dst", a[1], a[4] * a[5], a[6], a[6], _F32)],
+    "vb_zero_tail_rows": lambda p, a: [],      # zeros into the rows of no sample; the launch before it declared those buffers
+    "vb_cast2d_f32_to_bf16": lambda p, a: [("dst", a[2], a[4], a[5], a[3], _BF16)],
+    "vb_weight_norm_bwd": lambda p, a: [_vec("dg", a[4], 1), _vec("dv", a[5], a[3])],
+    "vb_tanh_bwd": lambda p, a: [("dx_bf16", a[2], a[4], a[5], a[5], _BF16), _vec("dbias", a[3], a[5])],
+    "vb_concat_embed_ln_bwd": lambda p, a: [
+        ("dxt", a[8], a[17] * a[18], a[20], a[20], _F32), ("dxv", a[9], a[17] * a[19], a[20], a[20], _F32),
+        ("dxv_bf16", a[10], a[17] * a[19], a[20], a[20], _BF16)] + [_vec(n, a[11 + i], a[20]) for i, n in enumerate(
+            ("dgamma_t", "dbeta_t", "dgamma_v", "dbeta_v", "dcol_v", "dcol_v2"))],
+    "vb_ce_loss": _ce,
+    "vb_ce_loss_det": _ce,
+    "vb_bce_logits_loss": _bce,
+    "vb_bce_logits_loss_det": _bce,
+    "vb_bce_gather_loss": lambda p, a: [("dlogits_f32", a[12], a[6], a[3], a[13], _F32), ("dlogits_bf16", a[14], a[6], a[3], a[15], _BF16)],
+    "vb_kl_masked_loss": _kl,
+    "vb_kl_masked_loss_det": _kl,
+    "vb_mse_masked_loss": _region_loss(10),
+    "vb_nce_region_loss": _region_loss(12),
+    "vb_scale_by_device": lambda p, a: [_vec("dst", a[1], a[2])],
+}
+# one checked region: its id (the index into Plan.nan_records) and where it comes from — the op (its index in Plan.fwd or Plan.bwd,
+# `section`), the op's entry point and stream, the output (its index among the op's checked outputs and its name) and the module path
+# of the block that emitted the op (a fused objective: its kind)
+NanRecord = namedtuple("NanRecord", "region section op entry output name module stream")
+C_SIZEOF_NAN_REGION = L.C.sizeof(L.NanRegion)
+NAN_FLAG_CLEAR = 2 ** 31 - 1
 # alignment of every buffer a plan places in a region of its own or in the shared arena
 BUF_ALIGN = 256
 
@@ -611,12 +716,22 @@ class Plan:
     that it does not fill (also under torch.use_deterministic_algorithms(True)); the vector clocks of its ops (happens_before_clocks) give each buffer its uses, and lifetime_layout
     places them. The second build emits the same launches with each buffer at its place, in one region of the plan or, with the
     shared arena, at the start of the arena (arena_bytes is the extent). Private buffers and the buffers the host reads after a run
-    (_host_reads) keep bytes of their own. self.held_bytes: arena extent + the plan's own device buffers."""
+    (_host_reads) keep bytes of their own. self.held_bytes: arena extent + the plan's own device buffers.
+
+    anomaly=True (torch.autograd.set_detect_anomaly(True), DESIGN.md §4i): every op in the backward role — the backward list, the
+    head-gradient writes of a forward-placed objective, vb_scale_by_device — is tagged with the module path of the block that
+    emitted it, and after each block one vb_nan_check per stream the block used scans the gradients its ops wrote (ANOMALY_OUTPUTS)
+    on that stream. Region ids follow op-list order and the flag (reset at the start of every forward) keeps the least id that held
+    a NaN, so anomaly_report() names the first op whose outputs held one. Removing the checks and the reset leaves the unchecked
+    plan's launches. The checks only read."""
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
                  loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-                 input_grads=frozenset(), packed=None, deterministic=False, recycle=False, _recording=False):
+                 input_grads=frozenset(), packed=None, deterministic=False, recycle=False, anomaly=False, _recording=False):
         self.recycle = bool(recycle)
+        self.anomaly = bool(anomaly)
+        if self.anomaly and self.recycle:
+            raise ValueError("anomaly checks read the gradients of a backward: a recycled (forward-only) plan has none")
         if self.recycle and (train or grad_outputs or input_grads):
             raise ValueError("recycle=True shares the bytes of buffers whose lifetimes are disjoint, which only a forward-only plan "
                              "has: no train mode, no grad_outputs, no input_grads (the backward reads the saved activations)")
@@ -710,7 +825,17 @@ class Plan:
         self._arena_off = self.arena_bytes = 0
         if self._place is not None:
             self._open_region()
+        self._label = None       # module path of the backward-role ops being emitted (role()); None: not the backward role
+        self._pending = []       # anomaly: (op list, index, module path) of the backward-role ops since the last check
+        self._buf_rows = {}      # anomaly: data pointer -> leading dimension of the plan's buffers (extents of scattered-into rows)
+        self.nan_records, self._nan_checks = [], []
+        self.nan_flag = None
+        if self.anomaly:
+            self.nan_flag = torch.full((1,), NAN_FLAG_CLEAR, dtype=torch.int32, device=self.dev)
+            self.emit(self.lib.vb_nan_check, None, 0, self.nan_flag, 1)       # the reset: first launch of every forward
         self._build()
+        if self.anomaly:
+            self._nan_table()
         if self._place is not None and self._n_req != len(self._place[0]):
             raise L.VBError(f"recycled plan: the second build made {self._n_req} buffer requests, the first {len(self._place[0])}")
 
@@ -880,14 +1005,17 @@ class Plan:
         if arena is None or zero:
             t = (torch.zeros if zero else torch.empty)(shape, dtype=dtype, device=self.dev)
             self._keep.append(t)
-            return t
-        off = self._arena_off
-        if off + nbytes > arena.numel():
-            raise L.VBError(f"activation arena of {arena.numel() / 2**30:.2f} GiB is too small for plan B={self.B} Nt={self.Nt} Nv={self.Nv} "
-                            f"(needs more than {(off + nbytes) / 2**30:.2f} GiB): pass a larger size to Engine.enable_activation_arena")
-        self._arena_off = (off + nbytes + 255) // 256 * 256
-        self.arena_bytes = self._arena_off
-        return arena[off:off + nbytes].view(dtype).view(shape)
+        else:
+            off = self._arena_off
+            if off + nbytes > arena.numel():
+                raise L.VBError(f"activation arena of {arena.numel() / 2**30:.2f} GiB is too small for plan B={self.B} Nt={self.Nt} Nv={self.Nv} "
+                                f"(needs more than {(off + nbytes) / 2**30:.2f} GiB): pass a larger size to Engine.enable_activation_arena")
+            self._arena_off = (off + nbytes + 255) // 256 * 256
+            self.arena_bytes = self._arena_off
+            t = arena[off:off + nbytes].view(dtype).view(shape)
+        if self.anomaly and t.dim():
+            self._buf_rows[t.data_ptr()] = t.shape[0]
+        return t
 
     def _host_reads(self):
         """The tensors the host may read after a run, besides the private buffers: the outputs, the encoded layers
@@ -952,6 +1080,89 @@ class Plan:
             if size is not None:
                 args = args + (self.det_ws(size(*args)),)
         self.cur.append((fn, L.launch_args(fn, *args), self.sid if self.two_streams else 0))
+        if self.anomaly and self._label is not None:
+            self._pending.append((self.cur, len(self.cur) - 1, self._label))
+        elif self.anomaly and self.cur is self.bwd:
+            raise L.VBError(f"{fn.__name__}: a launch of the backward list emitted outside a role() (anomaly checks need its module)")
+
+    # ------------------------------------------------------------------ anomaly detection
+    class _Role:
+        def __init__(self, plan, label):
+            self.plan, self.label = plan, label
+
+        def __enter__(self):
+            self.prev = self.plan._label
+            self.plan._label = self.label
+
+        def __exit__(self, *exc):
+            self.plan._label = self.prev
+            if self.prev is None and exc[0] is None:
+                self.plan._emit_nan_checks()
+            return False
+
+    def role(self, label):
+        """Context in which the emitted ops are backward-role ops of the module `label` (None: not backward-role ops). Leaving the
+        outermost role ends a block: a checked plan emits its checks there (_emit_nan_checks)."""
+        return Plan._Role(self, label)
+
+    def _emit_nan_checks(self):
+        """After a block: the checked outputs (ANOMALY_OUTPUTS) of its backward-role ops become regions with ids in op-list order,
+        and one vb_nan_check per stream the block used scans that stream's regions, on that stream after the block's ops. The
+        launch's arguments are set by _nan_table once every region is known."""
+        pending, self._pending = self._pending, []
+        streams = OrderedDict()
+        for ops, i, label in pending:
+            fn, args, sid = ops[i]
+            spec = ANOMALY_OUTPUTS.get(fn.__name__)
+            if spec is None:
+                raise L.VBError(f"{fn.__name__} runs in the backward role ({label}) but has no entry in engine.ANOMALY_OUTPUTS")
+            k, section = 0, "fwd" if ops is self.fwd else "bwd"
+            for name, ptr, rows, cols, ld, dt in spec(self, args):
+                if not ptr or rows <= 0 or cols <= 0:
+                    continue
+                rid = len(self.nan_records)
+                self.nan_records.append(NanRecord(rid, section, i, fn.__name__, k, name, label, sid))
+                streams.setdefault(sid, []).append((ptr, rows, cols, ld, dt, rid))
+                k += 1
+        for sid, regions in streams.items():
+            self.cur.append((self.lib.vb_nan_check, None, sid))
+            self._nan_checks.append((self.cur, len(self.cur) - 1, regions))
+
+    def _nan_table(self):
+        """The static device table of every check's regions (contiguous per launch) and the arguments of the check launches."""
+        regions = [r for _, _, rs in self._nan_checks for r in rs]
+        arr = (L.NanRegion * max(len(regions), 1))()
+        for e, (ptr, rows, cols, ld, dt, rid) in zip(arr, regions):
+            e.ptr, e.rows, e.cols, e.ld, e.dtype, e.id = ptr, rows, cols, ld, dt, rid
+        raw = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
+        self.nan_table = raw.to(self.dev) if self.dev.type == "cuda" else raw
+        size, first = C_SIZEOF_NAN_REGION, 0
+        for ops, i, rs in self._nan_checks:
+            fn = self.lib.vb_nan_check
+            ops[i] = (fn, L.launch_args(fn, self.nan_table.data_ptr() + size * first, len(rs), self.nan_flag, 0), ops[i][2])
+            first += len(rs)
+        self.nan_regions = regions
+
+    def anomaly_report(self):
+        """After a backward of a checked plan (anomaly=True): the NanRecord of the first region, in op-list order, that held a NaN,
+        or None. One device-to-host read of the flag (the host waits for the current stream)."""
+        if not self.anomaly:
+            raise ValueError("anomaly_report: the plan was built without anomaly checks")
+        v = int(self.nan_flag.item())
+        return None if v == NAN_FLAG_CLEAR else self.nan_records[v]
+
+    def _attn_rows(self, off, B, N):
+        """Query or key rows of an attention launch: B * N, or the rows of the packed stream whose offsets `off` points at."""
+        if not off:
+            return B * N
+        return next(self.packed[k] for k, s in enumerate(("t", "v")) if self.seg[s][0].data_ptr() == off)
+
+    def _param_numel(self, ptr):
+        """Elements of the parameter-gradient entry that starts at `ptr` (0 for a null pointer)."""
+        if not ptr:
+            return 0
+        off = (ptr - self.ps.grad.data_ptr()) // 4
+        return next(math.prod(shape) for o, shape in self.ps.entries.values() if o == off)
 
     def det_ws(self, n):
         """fp32 workspace of at least n floats for a deterministic launch. A deterministic plan runs on one stream, so launches share
@@ -996,12 +1207,13 @@ class Plan:
     def on(self, sid):
         return Plan._On(self, sid)
 
-    def push_bwd(self, fn, rg=True):
+    def push_bwd(self, fn, rg, label):
         """Registers a block's backward emitter; it will emit on the stream that is current now. rg: whether the block's output needs
         a gradient (Act.rg); a block whose output needs none registers nothing (rule 2 of Act), so neither does a layer built
-        under torch.no_grad(). The wide heads register without it: their emitters decide when they run."""
+        under torch.no_grad(). The wide heads register with rg=True: their emitters decide when they run. label: the module path
+        of the block (the reference's parameter-name prefix), which names its ops in an anomaly report."""
         if rg:
-            self._bwd_emitters.append((self.sid, fn))
+            self._bwd_emitters.append((self.sid, fn, label))
 
     def drop(self, name, p, rows=None):
         """The vb_dropout descriptor of the dropout layer `name` with probability p, or None when inactive. rows: the stream
@@ -1240,6 +1452,7 @@ class Plan:
         o32, o, mean, rstd = self.ln_fwd(y, ps.p(lnname + ".weight"), ps.p(lnname + ".bias"), M, H, res=res.f32, in_drop=drop)
         out = self.act(o32, o, M, H, inputs=(res,), params=(wname, lnname), rg=a_rg)
         out.ln_reads = True
+        out.mod = lnname.rsplit(".", 1)[0]
 
         def bwd():
             """returns (dy16, dy32) of the dense output (== grad of the LN input); adds dy32 to res."""
@@ -1275,7 +1488,7 @@ class Plan:
                       out_colsum=self.pg(w1 + ".bias"))
             self.linear_wgrad(dpre16, I, x.op.bw, H, M, I, H, w1)
             self.dgrad_into(x, dpre16, I, ps.w(w1 + ".weight").bw, M, I, H, extra32=dy32)
-        self.push_bwd(bwd, out.rg)
+        self.push_bwd(bwd, out.rg, out.mod)
         return out
 
     def self_attention_block(self, x, B, N, nh, mask, prefix, tag, p_attn=0.0, p_hidden=0.0, pool=None):
@@ -1338,7 +1551,7 @@ class Plan:
                     self.dgrad_into(pool, dz16, 2 * H, ps.w(prefix + ".self.dy.weight").bw, B, 2 * H, pool.H)
             self.linear_wgrad(dqkv, 3 * H, x.op.bw, H, M, 3 * H, H, prefix + ".self.qkv")
             self.dgrad_into(x, dqkv, 3 * H, ps.w(prefix + ".self.qkv.weight").bw, M, 3 * H, H, extra32=dy32)
-        self.push_bwd(bwd, out.rg)
+        self.push_bwd(bwd, out.rg, prefix)
         return out
 
     def connection_layer(self, v, t, idx):
@@ -1429,7 +1642,7 @@ class Plan:
             self.dgrad_into(t, dqkv2, L3, ps.w(p + ".biattention.qkv2.weight").bw, Mt, L3, Ht, extra32=dyt32)
         # the cross-modal backward touches both streams' tensors: it runs on the main stream between two barriers
         self._bwd_emitters.append(None)
-        self.push_bwd(bwd, v1o.rg or t1o.rg)
+        self.push_bwd(bwd, v1o.rg or t1o.rg, p + ".biOutput")
         self._bwd_emitters.append(None)
         with self.on(1):
             v2o = self.ffn(v1o, c.v_intermediate_size, p + ".v_intermediate.dense", p + ".v_output.dense", p + ".v_output.LayerNorm", "c.v.ffn",
@@ -1486,7 +1699,7 @@ class Plan:
                 else:         # g[j] = sum_i out.g32[i * b + j]
                     self.emit(lib.vb_sum_strided, out.g32, g, n, b, n, b, b * n, acc)
             self._bwd_emitters.append(None)
-            self.push_bwd(bwd, out.rg)
+            self.push_bwd(bwd, out.rg, "bert.encoder")
             self._bwd_emitters.append(None)
         # masks: text mask rows repeated, image mask tiled (4-byte rows: plain torch-free kernels need 16-byte items -> host-side views)
         mt = self.buf((b * b, self.Nt), F32); mv = self.buf((b * b, self.Nv), F32)
@@ -1520,7 +1733,7 @@ class Plan:
                 return
             g, acc = self.grad_acc(t)
             self.emit(lib.vb_masked_mean_bwd, pool.g32, mask, g, acc, B, self.Nt, Ht)
-        self.push_bwd(bwd, pool.rg)
+        self.push_bwd(bwd, pool.rg, "bert.encoder")
         return pool
 
     def image_layer(self, x, i, pool=None):
@@ -1596,7 +1809,7 @@ class Plan:
                 gt = [None if n is None else self.pg(n) for n in tables]
                 if any(g is not None for g in gt):
                     self.emit(lib.vb_embed_text_bwd, dxe, self.in_ids, self.in_tt, self.in_task, *gt, B, self.Nt_in, Ht)
-        self.push_bwd(bwd_text, t.rg)
+        self.push_bwd(bwd_text, t.rg, e)
         # image: region features fp32 -> bf16 ingest, 2048 -> Hv GEMM with the 5 -> Hv box projection as residual, LayerNorm (:1421-1432).
         # image_prefix: the same launches go to self.prefix on the main stream, and the LayerNorm's outputs (the image states the
         # forward reads) are private buffers
@@ -1622,7 +1835,7 @@ class Plan:
                     self.ln_bwd(v.g32, yv, ps.p(ve + ".LayerNorm.weight"), vmean, vrstd, dyv32, dyv16, Mv, Hv, self.pg(ve + ".LayerNorm.weight"),
                                 self.pg(ve + ".LayerNorm.bias"), gbias=self.pg(ve + ".image_embeddings.bias"), out_drop=vdrop)
                     self.image_embedding_bwd(ve, Hv, feat, dyv16, dyv32)
-            self.push_bwd(bwd_image, v.rg)
+            self.push_bwd(bwd_image, v.rg, ve)
         return t, v
 
     def image_embedding(self, prefix, H):
@@ -1681,6 +1894,7 @@ class Plan:
         self.gemm(B, Hb, H, x, ldx, ps.w(wname + ".weight"), H, bias=ps.p(wname + ".bias"), act=L.VB_ACT_RELU, out_f32=p32, ld_of=Hb,
                   out_bf16=p, ld_ob=Hb)
         pooled = self.act(p32, p, B, Hb, inputs=(seq,), params=(wname,))
+        pooled.mod = wname.rsplit(".", 1)[0]
 
         def bwd():
             if not pooled.gw:
@@ -1690,7 +1904,7 @@ class Plan:
             self.emit(self.lib.vb_relu_bwd, pooled.g32, p32, dpre, dpre32, B * Hb)
             self.linear_wgrad(dpre, Hb, x.bw, ldx, B, Hb, H, wname, bias_from=(dpre32, Hb))
             self.pooler_dgrad(seq, N, dpre, wname, first if self.packed else None)
-        self.push_bwd(bwd, pooled.rg)
+        self.push_bwd(bwd, pooled.rg, pooled.mod)
         return pooled
 
     def pooler_dgrad(self, seq, N, dpre, wname, rows=None):
@@ -1856,7 +2070,7 @@ class Plan:
             g, acc = self.grad_acc(x) if x.rg else (None, 0)
             self.emit(self.lib.vb_small_linear_bwd, dy, xin, K, ps.p(wname + ".weight"), g, K, acc,
                       self.pg(wname + ".weight"), self.pg(wname + ".bias"), M, K, N_out, in_drop)
-        self.push_bwd(bwd, self.out_rg[name])
+        self.push_bwd(bwd, self.out_rg[name], wname)
 
     def packed_vision_logit(self, seq_v, in_drop):
         """vision_logit of a packed plan: the Linear on the packed region rows, scattered to the padded [B * Nv, 1] layout with
@@ -1880,7 +2094,7 @@ class Plan:
             g, acc = self.grad_acc(seq_v) if seq_v.rg else (None, 0)
             self.emit(lib.vb_small_linear_bwd, dy, seq_v.f32, K, ps.p(name + ".weight"), g, K, acc,
                       self.pg(name + ".weight"), self.pg(name + ".bias"), M, K, 1, in_drop)
-        self.push_bwd(bwd, self.out_rg[name])
+        self.push_bwd(bwd, self.out_rg[name], name)
 
     def packed_vision_prediction(self, hv):
         """The region decoder of a packed plan: the [rows_v, C] logits of the packed region rows, scattered to the padded
@@ -1907,7 +2121,7 @@ class Plan:
         ps, c, B, lib = self.ps, self.cfg, self.B, self.lib
         Hb, Ht, Hv, Nt, Nv = c.bi_hidden_size, c.hidden_size, c.v_hidden_size, self.Nt, self.Nv
         mul = 1 if c.fusion_method == "mul" else 0
-        def fuse(drop):
+        def fuse(drop, label):
             f32 = self.buf((B, Hb), F32)
             f = self.buf16((B, Hb))
             hi, lo, bw = f.ptrs()
@@ -1921,7 +2135,7 @@ class Plan:
                     if a.rg:
                         self.grad_zeroed(a)
                 self.emit(lib.vb_fuse_pooled_bwd, act.g32, pooled_t.f32, pooled_v.f32, pooled_t.g32, pooled_v.g32, B * Hb, mul, drop)
-            self.push_bwd(fuse_bwd, act.rg)
+            self.push_bwd(fuse_bwd, act.rg, label)
             return act
         # VILBertForVLTasks.dropout on the fused vector (vilbert.py:1677-1682); BertPreTrainingHeads has its own nn.Dropout(0.1)
         # on its own fused vector (:1233-1241) — a different mask, needed only where the alignment score is an output
@@ -1929,11 +2143,11 @@ class Plan:
         want = self.want
         need_fused = any(want(n) for n in ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_tri_prediction")) or (
             want("vil_binary_prediction") and B % 2 == 0)
-        fused = fuse(self.drop("dropout.pooled", self.head_dropout_prob)) if self.heads == "vl" and need_fused else None
+        fused = fuse(self.drop("dropout.pooled", self.head_dropout_prob), "dropout") if self.heads == "vl" and need_fused else None
         need_cls_fused = (self.heads == "pretraining" and want("seq_relationship_score")) or (B % 2 == 1 and want("vil_binary_prediction"))
         cls_drop = self.drop("cls.dropout", 0.1)
         if need_cls_fused:
-            fused_cls = fuse(cls_drop) if (cls_drop is not None or fused is None) else fused
+            fused_cls = fuse(cls_drop, "cls.dropout") if (cls_drop is not None or fused is None) else fused
         else:
             fused_cls = None
 
@@ -1956,9 +2170,10 @@ class Plan:
                 im_bwd = self.big_head("vision_prediction", hv, Hv, B * Nv, Hv, c.v_target_size, "cls.imagePredictions.decoder",
                                        "cls.imagePredictions.decoder.bias")
         if want("linguisic_prediction"):
-            self.push_bwd(self._wide_bwd(lm_bwd, ht, ht_bwd, Ht, c.vocab_size) if lm_bwd is not None else lm_compact_bwd)
+            self.push_bwd(self._wide_bwd(lm_bwd, ht, ht_bwd, Ht, c.vocab_size) if lm_bwd is not None else lm_compact_bwd, True,
+                          "cls.predictions")
         if want("vision_prediction"):
-            self.push_bwd(self._wide_bwd(im_bwd, hv, hv_bwd, Hv, c.v_target_size))
+            self.push_bwd(self._wide_bwd(im_bwd, hv, hv_bwd, Hv, c.v_target_size), True, "cls.imagePredictions")
 
         if self.heads == "pretraining":
             # BertForMultiModalPreTraining returns the alignment score of self.cls (vilbert.py:1497)
@@ -1983,7 +2198,7 @@ class Plan:
                 hb_bwd()
                 if pair.gw:   # gradient landed in pair.g32 [B/2, 2Hb] == [B, Hb]
                     self.add_grad(fused, pair.g32.view(B, Hb))
-            self.push_bwd(bin_bwd, hb.rg)   # registered first => runs after the 2-way linear's backward
+            self.push_bwd(bin_bwd, hb.rg, "vil_binary_prediction.logit_fc")   # registered first => runs after the 2-way linear's backward
             self.small_head("vil_binary_prediction", hb, "vil_binary_prediction.logit_fc.3", 2)
         elif want("vil_binary_prediction"):
             # odd batch: the reference returns the [B, 2] alignment output of self.cls here (:1673, 1686)
@@ -1995,7 +2210,7 @@ class Plan:
             n_out = ps.p(nm + ".logit_fc.3.weight").shape[0]     # the answer vocabulary
             hh, hh_bwd = self.transform(fused, nm + ".logit_fc.0", nm + ".logit_fc.2", nm + ".tr")
             head_bwd = self.big_head(nm, hh, 2 * Hb, B, 2 * Hb, n_out, nm + ".logit_fc.3", nm + ".logit_fc.3.bias")
-            self.push_bwd(self._wide_bwd(head_bwd, hh, hh_bwd, 2 * Hb, n_out))
+            self.push_bwd(self._wide_bwd(head_bwd, hh, hh_bwd, 2 * Hb, n_out), True, nm + ".logit_fc")
         if want("vil_logit"):
             self.small_head("vil_logit", fused, "vil_logit", 1)
         if want("vil_tri_prediction"):
@@ -2074,17 +2289,19 @@ class Plan:
                     self.outputs[nm] = self.outputs[nm].view(B, self.Nt, -1)
         self.sync_streams(mirror=False)
         if self.loss_in_forward:
-            self._emit_loss()
+            with self.role(self.loss_kind):      # its head-gradient writes stand for torch's loss node
+                self._emit_loss()
         if self.results is not None:
             self._emit_results()
         self.n_kernels_fwd = sum(1 for op in self.fwd if op[0] is not None)
 
         # ---------------- backward
         self.cur = self.bwd
-        if self.loss_in_forward:
-            self._emit_grad_scale()
-        elif self.loss_kind is not None:
-            self._emit_loss()
+        with self.role(self.loss_kind):
+            if self.loss_in_forward:
+                self._emit_grad_scale()
+            elif self.loss_kind is not None:
+                self._emit_loss()
         self._emit_backward((("sequence_output_t", self.seq_t), ("sequence_output_v", self.seq_v), ("pooled_output_t", self.pooled_t),
                              ("pooled_output_v", self.pooled_v)))
 
@@ -2093,15 +2310,17 @@ class Plan:
         emitters in reverse order, and a join of every stream."""
         for nm, act in bert_outputs:
             if nm in self.grad_outputs:
-                self.add_grad(act, self.out_grad_buffer(nm, (act.M, act.H)))
+                with self.role(act.mod or "bert"):
+                    self.add_grad(act, self.out_grad_buffer(nm, (act.M, act.H)))
         self.sync_streams()
         for entry in reversed(self._bwd_emitters):
             if entry is None:
                 self.sync_streams()
             else:
-                self.sid, emitter = entry
+                self.sid, emitter, label = entry
                 self._scratch_epoch += 1
-                emitter()
+                with self.role(label):
+                    emitter()
         self.sid = 0
         self.cur.append((None, ("all",), 0))     # join every stream (incl. the weight-gradient side streams)
         self.n_kernels_bwd = sum(1 for op in self.bwd if op[0] is not None)
@@ -2210,7 +2429,8 @@ class Plan:
             self.emit(lib.vb_bce_gather_loss, lg, h.ld, h.off, h.ld, li.get(h.ids), inp, h.rows, h.cols,
                       float(h.cols if k == "vlogit_mc" else 1.0), row_loss, loss, 0, d, h.ld, None, 0)
         if self.want_score:
-            self._emit_score()
+            with self.role(None):
+                self._emit_score()
 
     def _emit_pretraining_loss(self):
         """vilbert.py:1578-1590: masked-LM CE (ignore_index -1), the masked-region objective of config.visual_target (0: KL to the
@@ -2238,7 +2458,8 @@ class Plan:
                 # kernel's count check poisons the masked-LM slot; the rows it moves are a 4-column dummy
                 src = self.scratch("lm.cap.src", (lc["cap"], 4), F32)
                 dst = self.scratch("lm.cap.dst", (B * self.Nt, 4), F32)
-                self.emit(lib.vb_scatter_rows_f32, src, dst, lc["idx"], lc["cap"], 4, lc["count"], slot[0])
+                with self.role(None):
+                    self.emit(lib.vb_scatter_rows_f32, src, dst, lc["idx"], lc["cap"], 4, lc["count"], slot[0])
         else:
             lg, rows = self.outputs["linguisic_prediction"], B * self.Nt
             li["masked_lm_labels"] = self.buf((rows,), I64, zero=True)
@@ -2499,7 +2720,11 @@ class Plan:
         backward + ONE AdamW launch that also rewrites the 16-bit weight copy and zeroes the gradients — no weight cast and no
         gradient memset in the step. (The host-side lr table of `opt` is refreshed by opt.step(); here the launch alone is
         replayed, e.g. inside the step graph, with the table currently on the device.) With `max_grad_norm` the gradient-norm
-        launch precedes it, so every replay clips and skips a non-finite step on the device."""
+        launch precedes it, so every replay clips and skips a non-finite step on the device. A plan with anomaly checks refuses:
+        the step would apply a NaN gradient before the host could raise."""
+        if self.anomaly:
+            raise ValueError("enable_optimizer: a plan with anomaly checks (torch.autograd.set_detect_anomaly(True)) reports a NaN "
+                             "gradient on the host after the backward; a step placed in the plan would apply it first")
         self.prologue = self.cur = []
         if self.train and dropout_bump:
             self.emit(self.lib.vb_step_counter_bump, self.e.drop_step)
@@ -2688,12 +2913,12 @@ class BasePlan(Plan):
 
     def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
                  loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-                 input_grads=frozenset(), recycle=False):
+                 input_grads=frozenset(), recycle=False, anomaly=False):
         if (loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
                 or loss_in_forward):
             raise ValueError("single-stream baseline plans support grad_outputs, train, frozen, input_grads and recycle only")
         super().__init__(engine, B, Nt, Nv, grad_outputs, heads=heads, train=train, choices=choices, frozen=frozen, input_grads=input_grads,
-                         recycle=recycle)
+                         recycle=recycle, anomaly=anomaly)
 
     def _stream_modes(self, B, Nt, Nv, *_):
         self.pairs = self.has_task = self.viz = self.dyn = self.fast = self.image_prefix = False
@@ -2778,7 +3003,7 @@ class BasePlan(Plan):
             if dxt is not None:
                 self.emit(lib.vb_embed_text_bwd_padded, dxt, self.in_ids, self.in_tt, *gt, B, Nt, H)
             self.image_embedding_bwd(ie, H, feat, dxv16, dxv32)
-        self.push_bwd(bwd, x.rg)
+        self.push_bwd(bwd, x.rg, e)
         return x
 
     def base_layer(self, x, i):
@@ -2797,6 +3022,7 @@ class BasePlan(Plan):
         y32, y = self.buf((B, H), F32), self.buf16((B, H))
         self.emit(self.lib.vb_tanh_fwd, pre, y32, *y.ptrs(), y.fp16, B * H)
         pooled = self.act(y32, y, B, H, inputs=(seq,), params=(w,))
+        pooled.mod = "bert.pooler"
 
         def bwd():
             if not pooled.gw:
@@ -2805,10 +3031,10 @@ class BasePlan(Plan):
             self.emit(self.lib.vb_tanh_bwd, pooled.g32, y32, dpre, self.pg(w + ".bias"), B, H)
             self.linear_wgrad(dpre, H, seq.op.bw, N * H, B, H, H, w)
             self.pooler_dgrad(seq, N, dpre, w)
-        self.push_bwd(bwd, pooled.rg)
+        self.push_bwd(bwd, pooled.rg, pooled.mod)
         return pooled
 
-    def base_rows(self, seq, a, b, tag):
+    def base_rows(self, seq, a, b, tag, label):
         """Rows [a, b) of every sample of the stream as a compact Act (operand copies: the head transform reads nothing else). Its
         backward scatters the compact gradient into those rows of the stream gradient."""
         lib, B, N, H = self.lib, self.B, self.N, seq.H
@@ -2830,7 +3056,7 @@ class BasePlan(Plan):
             self.emit(lib.vb_memset_zero, full, full.numel() * 4)
             self.emit(lib.vb_scatter_rows_f32, rows.g32, full, idx, B * n, H, None, None)
             self.emit(lib.vb_axpy_f32, full, g, full.numel(), 1.0)
-        self.push_bwd(bwd, rows.rg)
+        self.push_bwd(bwd, rows.rg, label)
         return rows
 
     def base_simple_classifier(self, x):
@@ -2895,7 +3121,7 @@ class BasePlan(Plan):
                 self.colsum(dpre32, H2, gb, B, H2)
             wn_wgrad(0, dpre16, H2, x.op.bw, H, B, H2, H)
             self.dgrad_into(x, dpre16, H2, W[0][3].bw, B, H2, H)
-        self.push_bwd(bwd, self.out_rg["vil_prediction"])
+        self.push_bwd(bwd, self.out_rg["vil_prediction"], "vil_prediction")
 
     def build_base_heads(self, seq, pooled):
         """The seven outputs of BaseBertForVLTasks.forward (basebert.py:929-962). Returns the views of the whole-stream output-gradient
@@ -2915,16 +3141,16 @@ class BasePlan(Plan):
                             in_drop=self.drop(site, self.head_dropout_prob))
             self.outputs[name] = self.outputs[name].view(B, N, 1)[:, a:b]
             views[name] = full.view(B, N, 1)[:, a:b]
-        rows_t = self.base_rows(seq, 0, Nt, "rows.t")
-        rows_v = self.base_rows(seq, Nt, N, "rows.v")
+        rows_t = self.base_rows(seq, 0, Nt, "rows.t", "cls.predictions")
+        rows_v = self.base_rows(seq, Nt, N, "rows.v", "cls.imagePredictions")
         wn = "bert.embeddings.word_embeddings.weight"
         ht, ht_bwd = self.transform(rows_t, "cls.predictions.transform.dense", "cls.predictions.transform.LayerNorm", "lm.tr")
         lm_bwd = self.big_head("linguisic_prediction", ht, H, B * Nt, H, c.vocab_size, None, "cls.predictions.bias", w=ps.w(wn), gw_name=wn)
         hv, hv_bwd = self.transform(rows_v, "cls.imagePredictions.transform.dense", "cls.imagePredictions.transform.LayerNorm", "im.tr")
         im_bwd = self.big_head("vision_prediction", hv, H, B * Nv, H, BASE_REGION_CLASSES, "cls.imagePredictions.decoder",
                                "cls.imagePredictions.decoder.bias")
-        self.push_bwd(self._wide_bwd(lm_bwd, ht, ht_bwd, H, c.vocab_size))
-        self.push_bwd(self._wide_bwd(im_bwd, hv, hv_bwd, H, BASE_REGION_CLASSES))
+        self.push_bwd(self._wide_bwd(lm_bwd, ht, ht_bwd, H, c.vocab_size), True, "cls.predictions")
+        self.push_bwd(self._wide_bwd(im_bwd, hv, hv_bwd, H, BASE_REGION_CLASSES), True, "cls.imagePredictions")
         self.outputs["linguisic_prediction"] = self.outputs["linguisic_prediction"].view(B, Nt, -1)
         self.outputs["vision_prediction"] = self.outputs["vision_prediction"].view(B, Nv, -1)
         return views
@@ -2978,17 +3204,22 @@ class Engine:
 
     def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
              loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-             input_grads=frozenset(), packed=None, deterministic=None, recycle=None):
+             input_grads=frozenset(), packed=None, deterministic=None, recycle=None, anomaly=None):
         """The cached plan of this shape and these options (Plan). vqa_loss=True is the round-1 spelling of loss="vqa"; frozen:
         ParamStore entry names that take no gradient; input_grads: the inputs of INPUT_GRAD_NAMES the backward also differentiates;
         packed: (rows_t, rows_v) of a packed plan. deterministic: bitwise-reproducible kernels (Plan); None reads
         torch.are_deterministic_algorithms_enabled() now. The single-stream baseline has kernels without a deterministic variant: it
         raises RuntimeError, or with torch's warn_only=True warns and builds the default plan. recycle: buffers placed by lifetime
-        (Plan); None takes engine.recycle_forward_only for a forward-only plan and leaves any other plan as it is."""
+        (Plan); None takes engine.recycle_forward_only for a forward-only plan and leaves any other plan as it is. anomaly: NaN checks
+        of the backward's gradients (Plan); None reads torch.is_anomaly_enabled() and torch.is_anomaly_check_nan_enabled() now. A plan
+        with no backward (no grad_outputs, no input_grads) has nothing to check and is the unchecked plan."""
         frozen, input_grads = frozenset(frozen), frozenset(input_grads)
         if recycle is None:
             recycle = self.recycle_forward_only and not (train or grad_outputs or input_grads)
         det = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
+        if anomaly is None:
+            anomaly = torch.is_anomaly_enabled() and torch.is_anomaly_check_nan_enabled()
+        anomaly = bool(anomaly) and bool(grad_outputs or input_grads)
         if det and self.ps.base:
             msg = (f"{' and '.join(DET_MISSING_BASELINE)} (the backward of BaseBertForVLTasks' embeddings) add with float atomics and "
                    "have no deterministic implementation; build the plan without torch.use_deterministic_algorithms(True), or with "
@@ -3001,7 +3232,7 @@ class Engine:
         pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
         key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward),
                None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix), frozen, input_grads,
-               None if packed is None else tuple(packed), det, bool(recycle))
+               None if packed is None else tuple(packed), det, bool(recycle), anomaly)
         if key in self.plans:
             self.plans.move_to_end(key)
             return self.plans[key]
@@ -3015,6 +3246,8 @@ class Engine:
             extra["deterministic"] = True
         if recycle:
             extra["recycle"] = True
+        if anomaly:
+            extra["anomaly"] = True
         self.plans[key] = (BasePlan if self.ps.base else Plan)(
             self, B, Nt, Nv, grad_outputs, heads, train, loss=loss, choices=choices, score=score, loss_in_forward=loss_in_forward,
             outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen, input_grads=input_grads,

@@ -6,6 +6,8 @@ non-CUDA device or without the built extension raises.
 """
 import operator
 import os
+import traceback
+import warnings
 
 import torch
 import torch.nn as nn
@@ -93,13 +95,20 @@ class _PlanCall:
 
     input_names: the float inputs (INPUT_GRAD_NAMES) whose gradient the plan computes (Plan.input_grads). backward() copies them
     out of the plan right after its backward ran, in the shape, dtype and device of the tensors the caller passed
-    (self.input_grads_out; None for an input behind a no_grad layer). They are per-rank: the all-reduce never sees them."""
+    (self.input_grads_out; None for an input behind a no_grad layer). They are per-rank: the all-reduce never sees them.
+
+    Anomaly mode (torch.autograd.set_detect_anomaly(True), or the detect_anomaly() context, with check_nan): the plans are built with
+    NaN checks (Plan(anomaly=True)) and forward() keeps the Python stack of the call. backward() reads the plan's report right after
+    its backward ran; when a gradient held a NaN it warns with that stack and raises RuntimeError naming the first op, as torch
+    names the backward node — before the input gradients are copied out and before the all-reduce, so the caller's optimizer step is
+    never reached. The flat gradient buffer keeps what the backward wrote."""
 
     def __init__(self, model, plan, inputs, targets=None, names=None):
         self.model, self.plan, self.inputs, self.targets, self.names = model, plan, inputs, targets or {}, names
         self.input_names = tuple(n for n in INPUT_GRAD_NAMES if n in plan.input_grads)
         self.input_grads_out = (None,) * len(self.input_names)
         self.drop_step = self.fwd_id = None
+        self.stack = None
 
     def _load(self):
         plan = self.plan
@@ -115,6 +124,8 @@ class _PlanCall:
         if plan.train:
             eng.bump_dropout_step()      # fresh nn.Dropout masks for this forward
         self.drop_step = eng.drop_step_host
+        if torch.is_anomaly_enabled() and torch.is_anomaly_check_nan_enabled():
+            self.stack = traceback.format_stack()[:-1]
         self._load()
         if eng.auto_graph:
             plan.maybe_capture_passes()
@@ -172,12 +183,23 @@ class _PlanCall:
                     else:
                         plan.loss_grad[i:i + 1].copy_(g.detach().reshape(1))
             plan.run_backward()
+            if plan.anomaly and torch.is_anomaly_enabled() and torch.is_anomaly_check_nan_enabled():
+                self._raise_on_nan(plan.anomaly_report())
             self.input_grads_out = tuple(self._input_grad(n) if w else None for n, w in zip(self.input_names, wanted))
         finally:
             if moved:
                 eng.set_dropout_step(now)
         if model._ddp_reducer is not None:     # data parallel: average the flat gradient buffer over the ranks (apex DDP, delay_allreduce=True)
             model._ddp_reducer.allreduce()
+
+    def _raise_on_nan(self, r):
+        """torch's anomaly-mode report for the NanRecord `r` (None: nothing to report)."""
+        if r is None:
+            return
+        fn = f"{r.module}: {r.entry}"
+        stack = "".join(self.stack) if self.stack else "(the forward ran with anomaly detection off)\n"
+        warnings.warn(f"Error detected in {fn}. Traceback of forward call that caused the error:\n{stack}", UserWarning, stacklevel=2)
+        raise RuntimeError(f"Function '{fn}' returned nan values in its {r.output}th output.")
 
     def _input_grad(self, name):
         """A copy of the gradient of the input `name` the backward just wrote, in the shape, dtype and device of the caller's tensor
