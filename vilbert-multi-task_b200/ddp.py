@@ -1,6 +1,7 @@
 """Data-parallel plumbing: the only distributed step of the path is the gradient all-reduce
 (reference: apex DistributedDataParallel(model, delay_allreduce=True) at train_tasks.py:497 — one flattened
-all-reduce after backward, averaged over the world size; batch split per rank at task_utils.py:435-437).
+all-reduce after backward, averaged over the world size; apex's default delay_allreduce=False at train_concap.py:513 —
+bucketed all-reduces overlapped with the backward; batch split per rank at task_utils.py:435-437).
 
 Here the gradients already live in ONE flat fp32 buffer (engine.ParamStore.grad), so the all-reduce runs in place
 on contiguous, fixed-address buckets (NCCL over NVLink/NVSwitch on GPUs; gloo in the CPU tests)."""
@@ -40,11 +41,14 @@ class FlatGradAllReducer:
         self.set_ranges([(0, n)])
         # NCCL has a fused average; gloo only sums
         self.use_avg = dist.is_initialized() and dist.get_backend(group) == "nccl"
+        self._comm = None        # communication stream of overlapped_backward
 
     def set_ranges(self, ranges):
         """Restricts allreduce() to the flat ranges [lo, hi) of `ranges` (the trainable parameters; frozen ones have no gradient
-        to exchange): every bucket is cut to its parts inside them. The whole buffer gives the full buckets."""
-        self.buckets = [self.flat[max(lo, a):min(hi, b)] for (lo, hi) in self._bounds for (a, b) in ranges if min(hi, b) > max(lo, a)]
+        to exchange): every bucket is cut to its parts inside them. The whole buffer gives the full buckets. self.table: their
+        (lo, hi) in ascending order, the same on every rank (Plan.bucket_schedule is keyed on it)."""
+        self.table = tuple((max(lo, a), min(hi, b)) for (lo, hi) in self._bounds for (a, b) in ranges if min(hi, b) > max(lo, a))
+        self.buckets = [self.flat[lo:hi] for lo, hi in self.table]
 
     def allreduce(self, stream=None):
         """Averages the flat gradient buffer over all ranks, bucket by bucket (in place)."""
@@ -80,6 +84,23 @@ class FlatGradAllReducer:
             dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
             t.div_(self.world)
 
+    def overlapped_backward(self, plan):
+        """Runs the backward of `plan` in the pieces of plan.bucket_schedule(self.table) and averages each bucket (allreduce_range,
+        asynchronous) on a communication stream as soon as the piece that finishes it has run, so the exchange overlaps the rest of
+        the backward. Returns once the current stream waits for every collective: work queued after it (an optimizer step, a
+        gradient-norm clip) sees the averaged buffer."""
+        if self._comm is None:
+            self._comm = torch.cuda.Stream(device=self.flat.device)
+        works = []
+
+        def handover(ranges):
+            works.extend(self.allreduce_range(lo, hi) for lo, hi in ranges)
+        plan.run_backward_pieces(self.table, handover, self._comm)
+        torch.cuda.current_stream().wait_stream(self._comm)
+        for w in works:
+            if w is not None:
+                w.wait()
+
     def broadcast_params(self, flat_params, src=0):
         """Rank-`src` parameters to every rank (what apex DDP does at wrap time)."""
         if self.world > 1:
@@ -87,10 +108,17 @@ class FlatGradAllReducer:
 
 
 class DistributedDataParallel:
-    """Drop-in for `apex.parallel.DistributedDataParallel(model, delay_allreduce=True)` as the reference uses it
-    (train_tasks.py:490-497): rank 0's parameters are broadcast at wrap time and every `loss.backward()` ends with ONE all-reduce
-    (average over the world) of the flat fp32 gradient buffer, restricted to the ranges of the trainable parameters. Not an nn.Module wrapper with hooks: the engine's backward calls
-    the reducer itself. `.module` is the wrapped model, calls are forwarded."""
+    """Drop-in for `apex.parallel.DistributedDataParallel(model, delay_allreduce=...)` as the reference uses it
+    (train_tasks.py:490-497, train_concap.py:513): rank 0's parameters are broadcast at wrap time and every `loss.backward()`
+    averages the flat fp32 gradient buffer over the world, restricted to the ranges of the trainable parameters. Not an nn.Module
+    wrapper with hooks: the engine's backward calls the reducer itself. `.module` is the wrapped model, calls and attributes
+    (model.no_sync()) are forwarded.
+
+    delay_allreduce=True (the default here, and train_tasks.py's choice): one all-reduce of the buffer after the backward.
+    delay_allreduce=False (apex's default): the buckets of the buffer are averaged in descending offset order while the backward
+    still runs, each as soon as no later backward op writes it (Plan.bucket_schedule). Both modes send the same messages, so they
+    give bitwise the same parameters. A world of one, and a plan with anomaly checks (whose NaN report must come before any
+    collective), take the first path. Backwards under model.no_sync() exchange nothing in either mode."""
 
     def __init__(self, model, delay_allreduce=True, n_buckets=8, group=None):
         self.module = model
@@ -99,6 +127,7 @@ class DistributedDataParallel:
         self.reducer.broadcast_params(eng.ps.flat)
         eng.shadow_clean = False
         model._ddp_reducer = self.reducer
+        model._ddp_overlap = not delay_allreduce
         # only the ranges of trainable parameters are exchanged; the model updates them when a requires_grad flag changes
         model._ddp_set_ranges = self.reducer.set_ranges
         self.reducer.set_ranges(model._trainable_ranges())

@@ -819,6 +819,8 @@ class Plan:
         self._last_attn = None   # visualization: the export of the attention emitted last
         self._scatter_ok = False          # the baseline's row heads may scatter straight into the stream gradient (base_rows)
         self._live_ranges_cache = {}      # (lo, hi) -> live_ranges(lo, hi), for run_step_overlapped
+        self._bucket_schedules = {}       # bucket table -> bucket_schedule(table)
+        self._piece_runs, self._piece_graphs = Counter(), {}     # schedule -> eager runs / its graphs (run_backward_pieces)
         self.n_kernels_fwd = self.n_kernels_bwd = 0
         self.graph_fwd = self.graph_bwd = self.graph_step = None
         self._eager_runs = [0, 0]      # eager forward / backward executions (maybe_capture_passes)
@@ -2747,6 +2749,21 @@ class Plan:
             self._run(self.bwd)
             self._run(self.epilogue)
 
+    def _straddled(self):
+        """Per position i of the backward list (a cut before bwd[i], 0..len): how many side-stream event edges it straddles. A piece
+        ends with a join of every stream and the next one starts with a fork, so any position works as long as no event recorded
+        in one piece is waited for in a later one (rec/wait markers of the side streams): a legal cut straddles none."""
+        rec_pos, last_wait = {}, {}
+        for i, op in enumerate(self.bwd):
+            if op[0] is None and len(op[1]) == 2:
+                if op[1][0] == "rec": rec_pos[op[1][1]] = i
+                elif op[1][0] == "wait": last_wait[op[1][1]] = i
+        straddle = [0] * (len(self.bwd) + 1)
+        for ev, r in rec_pos.items():
+            for i in range(r + 1, last_wait.get(ev, r) + 1):
+                straddle[i] += 1
+        return straddle
+
     def ddp_segments(self, n_segments=4, tail_cut=True):
         """Cuts the backward op list at stream barriers into `n_segments` pieces and returns
         [(bwd_op_lo, bwd_op_hi, grad_lo, grad_hi)]: after piece i has run, the flat gradient range [grad_lo, grad_hi) is
@@ -2754,17 +2771,7 @@ class Plan:
         whole flat buffer from its end (heads, last layers) to its start (embeddings). With `tail_cut` one extra piece holds
         only the last few kernels, so up to n_segments + 1 pieces are returned."""
         n_ops = len(self.bwd)
-        # legal cut positions: a piece ends with a join of every stream and the next one starts with a fork, so any position
-        # works as long as no event recorded in one piece is waited for in a later one (rec/wait markers of the side streams)
-        rec_pos, last_wait = {}, {}
-        for i, op in enumerate(self.bwd):
-            if op[0] is None and len(op[1]) == 2:
-                if op[1][0] == "rec": rec_pos[op[1][1]] = i
-                elif op[1][0] == "wait": last_wait[op[1][1]] = i
-        straddle = [0] * (n_ops + 1)
-        for ev, r in rec_pos.items():
-            for i in range(r + 1, last_wait.get(ev, r) + 1):
-                straddle[i] += 1
+        straddle = self._straddled()
         n_kern = [0] * (n_ops + 1)                      # kernels in bwd[:i]
         for i, op in enumerate(self.bwd):
             n_kern[i + 1] = n_kern[i] + (op[0] is not None)
@@ -2895,6 +2902,107 @@ class Plan:
         if (lo, hi) not in c:
             c[(lo, hi)] = self.live_ranges(lo, hi)
         return c[(lo, hi)]
+
+    def bucket_schedule(self, buckets):
+        """The backward of the module surface's overlapped data parallelism (ddp.DistributedDataParallel(delay_allreduce=False)) cut
+        into pieces: -> ((op_lo, op_hi, ranges), ...), where `ranges` are the buckets to all-reduce once bwd[op_lo:op_hi] has run.
+
+        `buckets` is the reducer's table, the same on every rank: (lo, hi) ranges of the flat gradient buffer in ascending order.
+        They are handed over in descending order, each exactly once, whatever this plan is, so ranks whose plans differ (packed
+        capacities, a padded fallback, frozen or deterministic variants) issue the same collectives in the same order; only where
+        the backward pauses for them depends on the plan. A bucket is ready one past the last backward op that passes an address
+        inside a gradient range of grad_touch overlapping it (0 when none does): grad_touch records when a gradient view was
+        taken, which side-stream event markers and, in deterministic plans, the ordered sums of split-K and bias gradients follow,
+        so the launches themselves are read. The op writes from that address to the end of the outermost range containing it.
+        The cut of bucket k is the latest readiness of the buckets at or above it, moved forward to the next position that
+        straddles no side-stream event edge (_straddled). Cached per table: ddp.trainable_ranges changes it with requires_grad."""
+        key = tuple((int(lo), int(hi)) for lo, hi in buckets)
+        sched = self._bucket_schedules.get(key)
+        if sched is not None:
+            return sched
+        if self.anomaly:
+            raise ValueError("bucket_schedule: the NaN checks of an anomaly plan read the gradients after the backward, and their "
+                             "report comes before any collective; such plans all-reduce after the backward")
+        if any(b[0] >= b[1] for b in key) or any(a[1] > b[0] for a, b in zip(key, key[1:])):
+            raise ValueError("bucket_schedule: the buckets must be non-empty, disjoint and in ascending order")
+        spans = sorted(self.grad_touch)
+        starts = [off for off, _ in spans]
+        outer_end, m = [], 0
+        for off, n in spans:          # ranges nest (a fused projection holds its parts): the end of the outermost range so far
+            m = max(m, off + n)
+            outer_end.append(m)
+        base, numel = self.ps.grad.data_ptr(), self.ps.numel
+        ready = [0] * len(key)
+        for i, (fn, args, _) in enumerate(self.bwd):
+            if fn is None:
+                continue
+            for p in op_pointers(fn, args):
+                if not base <= p < base + 4 * numel:
+                    continue
+                o = (p - base) // 4
+                j = bisect.bisect_right(starts, o) - 1
+                if j < 0 or outer_end[j] <= o:
+                    continue
+                for k, (lo, hi) in enumerate(key):
+                    if lo < outer_end[j] and o < hi:
+                        ready[k] = i + 1
+        straddle = self._straddled()
+        pieces, op_lo, cut, pending = [], 0, 0, []
+        for k in reversed(range(len(key))):
+            c = max(cut, ready[k])
+            while straddle[c]:
+                c += 1
+            if c != cut and pending:
+                pieces.append((op_lo, cut, tuple(pending)))
+                op_lo, pending = cut, []
+            cut = c
+            pending.append(key[k])
+        pieces.append((op_lo, cut, tuple(pending)))
+        if any(op[0] is not None for op in self.bwd[cut:]):     # kernels that write no bucket (input gradients): a last piece
+            pieces.append((cut, len(self.bwd), ()))
+        sched = self._bucket_schedules[key] = tuple(pieces)
+        return sched
+
+    def _piece(self, lo, hi):
+        """bwd[lo:hi] between two joins of every stream: a piece starts with a fork, so that in a graph capture every side stream it
+        uses joins the capture, and ends with a join, so that everything it wrote is done when the main stream's event fires."""
+        barrier = [(None, ("all",), 0)]
+        return barrier + self.bwd[lo:hi] + barrier
+
+    def run_backward_pieces(self, buckets, handover, comm_stream):
+        """The backward as the pieces of bucket_schedule(buckets). After each piece that finished buckets, `comm_stream` waits for an
+        event recorded on the current stream and handover(ranges) is called under comm_stream with them; it enqueues the
+        collectives, which stay outside any graph (DESIGN.md §4c). Pieces run eagerly, or as one CUDA graph each once
+        maybe_capture_pieces captured them. The caller makes the current stream wait for the collectives before reading the buffer."""
+        if not self.holds_forward(self.fwd_id):
+            raise L.VBError("shared activation arena: another plan's forward ran between this plan's forward and backward "
+                            "(its saved activations are gone); run forward + backward per batch, or disable the arena")
+        self.e.grad_clean = False
+        sched = self.bucket_schedule(buckets)
+        graphs = self._piece_graphs.get(sched)
+        main = torch.cuda.current_stream()
+        for i, (lo, hi, ranges) in enumerate(sched):
+            if hi > lo:
+                if graphs is not None:
+                    graphs[i].replay()
+                else:
+                    self._run(self._piece(lo, hi))
+            if ranges:
+                ev = torch.cuda.Event()
+                ev.record(main)
+                comm_stream.wait_event(ev)
+                with torch.cuda.stream(comm_stream):
+                    handover(ranges)
+        if graphs is None:
+            self._piece_runs[sched] += 1
+
+    def maybe_capture_pieces(self, buckets, after=2):
+        """maybe_capture_passes for the pieces of bucket_schedule(buckets): once they have run eagerly `after` times, one CUDA graph
+        per non-empty piece, captured without a warm-up run (it would accumulate into the gradient buffer)."""
+        sched = self.bucket_schedule(buckets)
+        if sched not in self._piece_graphs and self._piece_runs[sched] >= after:
+            torch.cuda.synchronize()
+            self._piece_graphs[sched] = [self._record(self._piece(lo, hi)) if hi > lo else None for lo, hi, _ in sched]
 
     def capture(self, separate=False):
         """Captures the plan into CUDA graphs (one for the whole step, or one per pass)."""

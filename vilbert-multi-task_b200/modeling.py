@@ -4,6 +4,7 @@ reference's constructor / forward signatures, output tuples and state_dict key n
 (engine.py -> libvilbert_b200.so). There is no PyTorch / CPU fallback: constructing a model on a
 non-CUDA device or without the built extension raises.
 """
+import contextlib
 import operator
 import os
 import traceback
@@ -90,8 +91,10 @@ class _PlanCall:
     overwrote the shared arena, or the backward switched to the plan of another gradient set), the forward is recomputed from the
     same inputs and targets. In train mode, if another forward moved the dropout step since, the step of this forward is set
     around the recomputed forward and the backward, which regenerate their dropout masks from it, and restored afterwards. The
-    backward accumulates into the flat gradient buffer (the Parameters' .grad are views of it) and ends with the data-parallel
-    all-reduce when one is attached.
+    backward accumulates into the flat gradient buffer (the Parameters' .grad are views of it) and, when a data-parallel reducer
+    is attached and the model is not under no_sync(), averages it over the ranks: after the backward (delay_allreduce=True, a
+    world of one, a plan with anomaly checks), or bucket by bucket while the backward runs in pieces (delay_allreduce=False,
+    ddp.FlatGradAllReducer.overlapped_backward).
 
     input_names: the float inputs (INPUT_GRAD_NAMES) whose gradient the plan computes (Plan.input_grads). backward() copies them
     out of the plan right after its backward ran, in the shape, dtype and device of the tensors the caller passed
@@ -160,6 +163,8 @@ class _PlanCall:
                 self.plan = model._outputs_plan(self.names, self.inputs, self.plan.train, live, self.plan.frozen, self.plan.input_grads)
                 self.fwd_id = None
         plan = self.plan
+        red = model._ddp_reducer if model._ddp_sync else None
+        overlap = red is not None and model._ddp_overlap and red.world > 1 and not plan.anomaly
         now = eng.drop_step_host
         moved = plan.train and now != self.drop_step
         if moved:
@@ -172,6 +177,8 @@ class _PlanCall:
             model._attach_grads()
             if eng.auto_graph:
                 plan.maybe_capture_passes()
+                if overlap:
+                    plan.maybe_capture_pieces(red.table)
             if self.names is not None:
                 for n, g in zip(self.names, grads):
                     if g is not None:
@@ -182,15 +189,18 @@ class _PlanCall:
                         plan.loss_grad[i:i + 1].zero_()
                     else:
                         plan.loss_grad[i:i + 1].copy_(g.detach().reshape(1))
-            plan.run_backward()
+            if overlap:
+                red.overlapped_backward(plan)
+            else:
+                plan.run_backward()
             if plan.anomaly and torch.is_anomaly_enabled() and torch.is_anomaly_check_nan_enabled():
                 self._raise_on_nan(plan.anomaly_report())
             self.input_grads_out = tuple(self._input_grad(n) if w else None for n, w in zip(self.input_names, wanted))
         finally:
             if moved:
                 eng.set_dropout_step(now)
-        if model._ddp_reducer is not None:     # data parallel: average the flat gradient buffer over the ranks (apex DDP, delay_allreduce=True)
-            model._ddp_reducer.allreduce()
+        if red is not None and not overlap:     # data parallel: average the flat gradient buffer over the ranks (apex DDP, delay_allreduce=True)
+            red.allreduce()
 
     def _raise_on_nan(self, r):
         """torch's anomaly-mode report for the NanRecord `r` (None: nothing to report)."""
@@ -269,6 +279,8 @@ class BertPreTrainedModel(nn.Module):
         self._opt_epoch = -1
         self._ddp_reducer = None
         self._ddp_set_ranges = None     # data parallel: restricts the reducer to the trainable ranges (ddp.DistributedDataParallel)
+        self._ddp_overlap = False       # ... all-reduces the buckets during the backward (delay_allreduce=False)
+        self._ddp_sync = True           # False under no_sync()
         self.init_weights()
 
     # ---- reference init (vilbert.py:1274-1285): N(0, initializer_range) for Linear/Embedding weights, zero bias, LN 1/0
@@ -325,6 +337,17 @@ class BertPreTrainedModel(nn.Module):
         frozen Parameter's (requires_grad=False) .grad is None."""
         self.engine.zero_grad()
         self._attach_grads(zero_if_detached=False)
+
+    @contextlib.contextmanager
+    def no_sync(self):
+        """Gradient-accumulation micro-batches under data parallelism, as torch's DistributedDataParallel.no_sync(): the backwards
+        inside the context exchange nothing and accumulate into the flat gradient buffer; the first backward outside it averages
+        the accumulated buffer over the ranks. Without a data-parallel wrapper it changes nothing."""
+        prev, self._ddp_sync = self._ddp_sync, False
+        try:
+            yield
+        finally:
+            self._ddp_sync = prev
 
     def _frozen(self):
         """ParamStore entry names of the Parameters with requires_grad=False: the set every plan-backed call is specialised on.
