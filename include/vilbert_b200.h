@@ -151,7 +151,12 @@ vb_status vb_gemm_plan(const vb_gemm_args* args, int32_t sm_count, int32_t* bloc
  *   mask: f32 [B, Nk] additive (0 / -10000, vilbert.py:1350-1362) or NULL
  *   lse:  f32 [B, H, Nq] row log-sum-exp in the log2 domain (saved for backward; may be NULL in fwd)
  * Backward recomputes P from lse: needs dO (bf16), writes dQ/dK/dV (bf16, same indexing as Q/K/V with
- * their own ld) and uses delta [B, H, Nq] f32 as scratch. D in {16, 32, 64, 128}; Nq, Nk <= ~320.
+ * their own ld) and uses delta [B, H, Nq] f32 as scratch. D in {16, 32, 64, 128}.
+ * Sequence limits: the forward streams keys through shared memory in chunks when the K / V panels do not fit. The backward runs
+ * one fused kernel for Nq, Nk <= 128 and D >= 32; otherwise two kernels that keep whole panels resident (227 KiB of shared
+ * memory): for D = 128 / 64 / 32 / 16 they take Nk <= 320 / 704 / 1344 / 2240 when dQ is requested or dropout is on, and
+ * Nq <= 320 / 704 / 1280 / 2176 when dK / dV are requested. Past these vb_attention_bwd returns VB_ERR_UNSUPPORTED and launches
+ * nothing.
  * Partial backward: dQ may be NULL (dK / dV only), or dK and dV may both be NULL (dQ only); what is written is bitwise what the
  * full backward writes there. dK without dV (or the reverse) and all three NULL return VB_ERR_INVALID. A bias sum follows its
  * gradient: dbias_q is ignored when dQ is NULL, dbias_k / dbias_v when dK / dV are.

@@ -25,15 +25,28 @@ def test_attention_fwd_bwd(B, H, Nq, Nk, D, cross):
     assert max(errs.values()) < 2e-2, errs
 
 
+# The backward's dispatch edges (vb_attention_bwd): the fused single-pass kernel runs for Nq, Nk <= 128 and D >= 32, and is at its
+# largest (~205 KiB of shared memory) at Nq = Nk = 128, D = 128; one query or one key more, or D = 16, takes the dQ + dK / dV
+# pair, which holds whole panels up to Nq = Nk = 320 at D = 128. Each shape asserts the variant it reaches.
+_FUSED = r"attn_bwd_fused_kernel<{D}, true, true>"
+_TWO = (r"attn_bwd_dq_kernel<{D}, true>", r"attn_bwd_dkv_kernel<{D}>")
+BWD_EDGES = {(Nq, Nk, D): ((_FUSED,) if Nq <= 128 and Nk <= 128 else _TWO)
+             for D in (32, 64, 128) for Nq, Nk in [(128, 128), (128, 129), (129, 128), (1, 128), (128, 1), (1, 1), (320, 320),
+                                                   (320, 36), (36, 320)]}
+BWD_EDGES[(128, 128, 16)] = _TWO
+
+
 @pytest.mark.parametrize("B,H,Nq,Nk,D,cross", [
     (3, 3, 11, 11, 32, False), (4, 12, 36, 36, 64, False), (4, 8, 100, 100, 128, False), (4, 8, 36, 100, 128, True),
-    (4, 8, 100, 36, 128, True), (2, 8, 257, 306, 128, True), (2, 2, 7, 12, 16, True)])
+    (4, 8, 100, 36, 128, True), (2, 8, 257, 306, 128, True), (2, 2, 7, 12, 16, True)]
+    + [(2, 2, Nq, Nk, D, Nq != Nk) for (Nq, Nk, D) in BWD_EDGES])
 def test_attention_fp16_operands(B, H, Nq, Nk, D, cross):
     """The engine's default arithmetic: Q/K/V/O fp16 (forward operands), dO/dQ/dK/dV bf16. The forward is checked at fp16
     accuracy; the backward converts its Q/K/V panels to bf16 (dS and dO are bf16 MMA operands); whole-model gradient parity is
     bounded in tests/test_model_gpu.py."""
-    from _gpu_util import attn_case
-    errs, _ = attn_case(B, H, Nq, Nk, D, cross, fp16=True)
+    from _gpu_util import attn_case, launched
+    run = lambda: attn_case(B, H, Nq, Nk, D, cross, fp16=True)
+    errs, _ = launched(run, *(p.format(D=D) for p in BWD_EDGES[(Nq, Nk, D)]))[0] if (Nq, Nk, D) in BWD_EDGES else run()
     assert errs["lse"] < 1e-5 and errs["O"] < 2e-3 and errs["O_b16"] < 1e-3, errs
     # gradients vs the attention of the bf16-rounded inputs (what the backward kernels contract); the saved row log-sum-exp comes
     # from the fp16 forward, so the recomputed probabilities differ from the reference's by the bf16 rounding of the scores

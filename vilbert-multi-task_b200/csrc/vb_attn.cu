@@ -953,6 +953,9 @@ extern "C" vb_status vb_attention_bwd(const vb_attn_args* a, void* stream) {
   const size_t smem_delta = p.drop.ctr ? smem_q : (size_t)(2 * TQ) * (a->D + 8) * 2;   // with dropout delta needs Q / K / V
   const size_t smem_k = (size_t)(2 * TQ + 2 * nqp) * (a->D + 8) * 2 + (size_t)nqp * 8;
   dim3 gq((a->Nq + TQ - 1) / TQ, a->H, a->B), gk((a->Nk + TQ - 1) / TQ, a->H, a->B);
+  // refuse a query range the dK / dV panels cannot hold before the dQ kernel runs: a refused call writes nothing
+  if (want_dkv && smem_k > 227 * 1024)
+    return set_error(VB_ERR_UNSUPPORTED, "vb_attention_bwd(dkv): sequence too long for the smem-resident panel (%zu bytes)", smem_k);
   int s;
 #define VB_BWD_TWO(DD)                                                                                                         \
   s = want_dq ? launch_att(attn_bwd_dq_kernel<DD>, gq, smem_q, p, st, "vb_attention_bwd(dq)")                                  \

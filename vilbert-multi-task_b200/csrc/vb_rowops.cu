@@ -638,7 +638,9 @@ __global__ void mask_to_additive_kernel(const long long* __restrict__ m, float* 
 // ------------------------------------------------------------------------------------------ dynamic_attention (vilbert.py:577-586)
 // BertImageSelfAttention with config.dynamic_attention: pool = masked mean of the current text states over the tokens,
 // gate = 1 + sigmoid(dyLinear(pool)) per (sample, channel), queries and keys of the image self-attention are multiplied by it.
-__device__ __forceinline__ float mask_weight(float add) { return 1.f + add / 10000.f; }   // (1 - m) * -10000 -> m
+// (1 - m) * -10000 -> m, exactly: a correctly rounded division (not the approximate one of --use_fast_math, which leaves a masked
+// token a weight of about 6e-8 in the mean and a non-zero gradient)
+__device__ __forceinline__ float mask_weight(float add) { return 1.f + __fdiv_rn(add, 10000.f); }
 __device__ __forceinline__ float sigmoidf_(float z) { return 1.f / (1.f + expf(-z)); }
 
 // pool[b, c] = sum_n w[b, n] x[b, n, c] / sum_n w[b, n]   (x fp32 [B, N, H]; also the 16-bit GEMM operand copies of pool)
