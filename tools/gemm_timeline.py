@@ -29,7 +29,7 @@ def run(M, N, K, bn, res=False, a_mn=False, b_mn=False, atomic=False, split_k=1,
     t = full[:, :8]
     ns0, ns1 = full[:, 8], full[:, 9]
     d = (t - t[:, :1]).float()
-    names = ["entry", "setup done", "first TMA issued", "first full_bar", "last MMA committed", "epi: tmem_full", "epi: done", "exit sync"]
+    names = ["entry", "setup done", "first TMA issued", "first full_bar", "(not recorded)", "tile 0: k-loop retired", "tile 0: epilogue done", "exit sync"]
     print(f"--- M{M} N{N} K{K} bn{bn} res{int(res)} a_mn{int(a_mn)} b_mn{int(b_mn)} atomic{int(atomic)} split{split_k} bf16out{int(bf16)}: event time {e0.elapsed_time(e1)*1e3:.1f} us, {int(live.sum())} CTAs; cycles since CTA entry (median / max over CTAs):")
     for i, n in enumerate(names):
         print(f"     {n:20s} {d[:, i].median().item():10.0f} {d[:, i].max().item():10.0f}")

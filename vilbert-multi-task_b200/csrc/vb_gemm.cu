@@ -7,8 +7,9 @@
 // SURVEY.md appendix A). Design:
 //   warpgroup 0      TMA producer: one elected lane of warp 0 issues cp.async.bulk.tensor 2D boxes (64 x rows, 128B swizzle)
 //                    into a NUM_STAGES-deep smem ring, completion on mbarriers (complete_tx); warps 1..3 only hold the
-//                    warpgroup slot so that the consumers start at a warpgroup boundary;
-//   warpgroups 1, 2  consumers, 64 rows of the 128 x BN tile each: wgmma.mma_async (m64 n128 k16, two per k step when BN = 256)
+//                    warpgroup slot so that the consumers start at a warpgroup boundary; the warpgroup keeps 40 registers
+//                    per thread and hands the rest to the consumers (setmaxnreg);
+//   warpgroups 1, 2  consumers, 64 rows of the 128 x BN tile each: wgmma.mma_async (m64 nBN k16)
 //                    from the swizzled stages into fp32 register accumulators; a stage is released once the wgmma group
 //                    reading it has retired (one group stays in flight). Then the epilogue of the warp's 16 rows: registers ->
 //                    XOR-swizzled smem tile -> row-wise, 128-bit coalesced pass doing bias / erf-GELU / GELU' / residual /
@@ -21,6 +22,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "vb_internal.h"
 #include "vb_ptx.cuh"
@@ -262,24 +265,26 @@ __device__ __forceinline__ void epi_fast_chunk(const GemmKernelParams& p, const 
   }
 }
 
-// One 64-deep k-block of a consumer warpgroup: 4 k steps of wgmma (NACC n128 halves each), committed as one group.
+// One 64-deep k-block of a consumer warpgroup: 4 k steps of one wgmma each (m64 n128 or n256), committed as one group.
 // MN-major operands advance 16 k rows = two 8-row groups (2 KB) per step, K-major ones 32 bytes inside the swizzle span.
-template <int NACC, int F16, int TA, int TB>
-__device__ __forceinline__ void mma_kblock(float (&acc)[NACC][64], uint32_t sa, uint32_t sb, const GemmKernelParams& p, bool accumulate) {
+// The n256 B operand continues the n128 layout: K-major rows 16 KB on, MN-major 64-wide boxes LBO = BK * 128 apart.
+template <int BN, int F16, int TA, int TB>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint32_t sa, uint32_t sb, uint64_t desc_base_a, uint64_t desc_base_b,
+                                           bool accumulate) {
   wgmma_fence();
 #pragma unroll
   for (int k = 0; k < BK / UK; ++k) {
-    const uint64_t da = gmma_desc_at(p.desc_base_a, sa + k * (TA ? 2048 : UK * 2));
-#pragma unroll
-    for (int j = 0; j < NACC; ++j)
-      wgmma_m64n128k16<F16, TA, TB>(acc[j], da, gmma_desc_at(p.desc_base_b, sb + j * (128 * BK * 2) + k * (TB ? 2048 : UK * 2)),
-                                    (accumulate || k > 0) ? 1u : 0u);
+    const uint64_t da = gmma_desc_at(desc_base_a, sa + k * (TA ? 2048 : UK * 2));
+    const uint64_t db = gmma_desc_at(desc_base_b, sb + k * (TB ? 2048 : UK * 2));
+    if constexpr (BN == 256) wgmma_m64n256k16<F16, TA, TB>(acc, da, db, (accumulate || k > 0) ? 1u : 0u);
+    else                     wgmma_m64n128k16<F16, TA, TB>(acc, da, db, (accumulate || k > 0) ? 1u : 0u);
   }
   wgmma_commit();
 }
 
-// Columns [32 c4, +32) of one n128 accumulator half -> the warp's staging tile (row = fragment row within the warp's 16).
-__device__ __forceinline__ void stage_chunk(const float (&d)[64], int c4, float* stg, int lane) {
+// Columns [32 c4, +32) of the accumulator fragment -> the warp's staging tile (row = fragment row within the warp's 16).
+template <int NR>
+__device__ __forceinline__ void stage_chunk(const float (&d)[NR], int c4, float* stg, int lane) {
   const int r0 = lane >> 2, c0 = 2 * (lane & 3);
 #pragma unroll
   for (int ii = 0; ii < 4; ++ii) {
@@ -293,11 +298,10 @@ template <int BN, int EPI, int CG, int OUT16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_a_lo, const __grid_constant__ CUtensorMap tmap_b_lo,
-                  const GemmKernelParams p) {
+                  const __grid_constant__ GemmKernelParams p) {
   using Cfg = GemmCfg<BN>;
   constexpr bool pair = (CG == 2);
   constexpr int NUM_STAGES = Cfg::NUM_STAGES;
-  constexpr int NACC = BN / 128;
 
   // SWIZZLE_128B tiles need 1024-byte alignment: the kernel has no static shared memory, so the dynamic window starts at
   // the CTA's (1024-aligned) shared base; checked once below.
@@ -339,6 +343,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const int num_groups = gridDim.x / CG;
   const int total_work = p.num_m_groups * p.num_n_blocks * p.split_k;
 
+  // Register split: one lane of the producer warpgroup issues the loads, the consumers hold the accumulators (BN / 2 per thread
+  // at BN = 256). 128 x 40 + 256 x 232 = 64512 of the 65536 registers the launch bounds give the CTA (168 per thread). Each
+  // setmaxnreg sits inside its role's branch (ptxas ignores it if code needing more registers is reachable after it), and all
+  // four warps of a warpgroup execute it.
+  if (warp_idx < 4) setmaxnreg_dec<40>();
   if (warp_idx == 0) {
     // ================================================================ TMA producer (one elected lane issues; the warp stays converged)
     int stage = 0;
@@ -401,6 +410,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     }
   } else if (warp_idx >= 4) {
     // ================================================================ consumers (warps 4..11 = warpgroups 1, 2)
+    setmaxnreg_inc<232>();
     const int cw = warp_idx - 4;
     const int wg = cw >> 2;                 // rows [64 wg, +64) of the tile
     float* stg = staging + cw * (EPI_ROWS * 32);
@@ -415,9 +425,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         if constexpr (pair) mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[s]), (uint32_t)(crank ^ 1)));
       }
     };
-    float acc[NACC][64];
+    float acc[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
+    const int mma_kind = p.mma_kind;
+    const uint64_t desc_base_a = p.desc_base_a, desc_base_b = p.desc_base_b;
     for (int w = group; w < total_work; w += num_groups) {
       const int split = w % p.split_k;
       const int t2 = w / p.split_k;
@@ -426,33 +438,35 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       const int kb0 = split * p.k_blocks_per_split;
       const int kb1 = min(kb0 + p.k_blocks_per_split, p.num_k_blocks);
       int prev = -1;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(smem_u32(&full_bar[stage]), phase);
-        if (kb == kb0 && w == group && threadIdx.x == 128) VB_DBG(3);
-        const uint32_t sa = smem_u32(smem_tiles + stage * Cfg::STAGE_BYTES) + a_off;
-        const uint32_t sb = smem_u32(smem_tiles + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
-        const bool accum = kb > kb0;
-        switch (p.mma_kind) {
-          case 0: mma_kblock<NACC, 0, 0, 0>(acc, sa, sb, p, accum); break;
-          case 1: mma_kblock<NACC, 0, 0, 1>(acc, sa, sb, p, accum); break;
-          case 2: mma_kblock<NACC, 0, 1, 0>(acc, sa, sb, p, accum); break;
-          case 3: mma_kblock<NACC, 0, 1, 1>(acc, sa, sb, p, accum); break;
-          case 4: mma_kblock<NACC, 1, 0, 0>(acc, sa, sb, p, accum); break;
-          case 5: mma_kblock<NACC, 1, 0, 1>(acc, sa, sb, p, accum); break;
-          case 6: mma_kblock<NACC, 1, 1, 0>(acc, sa, sb, p, accum); break;
-          default: mma_kblock<NACC, 1, 1, 1>(acc, sa, sb, p, accum); break;
+      // the k-loop of the tile, one copy per operand kind (formats and majors are wgmma immediates)
+      auto kloop = [&](auto kind) {
+        constexpr int KIND = decltype(kind)::value;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(smem_u32(&full_bar[stage]), phase);
+          if (kb == kb0 && w == group && threadIdx.x == 128) VB_DBG(3);
+          const uint32_t sa = smem_u32(smem_tiles + stage * Cfg::STAGE_BYTES) + a_off;
+          const uint32_t sb = smem_u32(smem_tiles + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+          mma_kblock<BN, (KIND >> 2) & 1, (KIND >> 1) & 1, KIND & 1>(acc, sa, sb, desc_base_a, desc_base_b, kb > kb0);
+          // the group of the previous k-block has retired: its stage may be refilled
+          wgmma_wait<1>();
+          if (prev >= 0) release(prev);
+          prev = stage;
+          if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
         }
-        // the group of the previous k-block has retired: its stage may be refilled
-        wgmma_wait<1>();
-        if (prev >= 0) release(prev);
-        prev = stage;
-        if (++stage == NUM_STAGES) { stage = 0; phase ^= 1; }
+      };
+      switch (mma_kind) {
+        case 0: kloop(std::integral_constant<int, 0>{}); break;
+        case 1: kloop(std::integral_constant<int, 1>{}); break;
+        case 2: kloop(std::integral_constant<int, 2>{}); break;
+        case 3: kloop(std::integral_constant<int, 3>{}); break;
+        case 4: kloop(std::integral_constant<int, 4>{}); break;
+        case 5: kloop(std::integral_constant<int, 5>{}); break;
+        case 6: kloop(std::integral_constant<int, 6>{}); break;
+        default: kloop(std::integral_constant<int, 7>{}); break;
       }
       wgmma_wait<0>();
 #pragma unroll
-      for (int j = 0; j < NACC; ++j)
-#pragma unroll
-        for (int i = 0; i < 64; ++i) reg_fence(acc[j][i]);
+      for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
       if (prev >= 0) release(prev);
       if (w == group && threadIdx.x == 128) VB_DBG(5);
 
@@ -487,10 +501,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             }
             if (p.bias) b4 = *reinterpret_cast<const float4*>(p.bias + n);
           }
-          // registers -> staging tile: the accumulator half and its 32-column quarter must be compile-time indices
+          // registers -> staging tile: the 32-column chunk of the fragment must be a compile-time index
 #pragma unroll
           for (int c2 = 0; c2 < NC; ++c2)
-            if (c2 == c) stage_chunk(acc[c2 >> 2], c2 & 3, stg, lane);
+            if (c2 == c) stage_chunk(acc, c2, stg, lane);
           __syncwarp();
           if (EPI == EPI_PARTIAL) {
             if (fast) epi_fast_chunk<EPI, OUT16>(p, stg, m_base + split * p.M, n, rr, cc, resv, auxv, b4);
