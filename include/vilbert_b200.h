@@ -60,7 +60,8 @@ typedef struct vb_dropout {
   const int32_t* row_map;
 } vb_dropout;
 
-/* ABI version of this header (bumped on incompatible change). */
+/* ABI version of this header (bumped on incompatible change). v3: vb_gemm_args has no CTA-pair field and no smem descriptor
+ * overrides, and vb_gemm_plan returns (block_n, split_k). */
 int vb_version(void);
 /* Message for the last non-OK status returned on this thread ("" if none). */
 const char* vb_last_error(void);
@@ -113,10 +114,7 @@ typedef struct vb_gemm_args {
   int32_t split_k;       /* >= 1; > 1 requires atomic_out and no act / bf16 outputs */
   int32_t block_n;       /* 0 = auto, else 128 or 256 */
   int32_t max_ctas;      /* 0 = one persistent CTA per SM */
-  /* debug/test overrides for the smem matrix descriptors (0 = library default) */
-  uint32_t dbg_lbo_a, dbg_sbo_a, dbg_lbo_b, dbg_sbo_b;
   void* dbg_timeline;    /* NULL, or u64 [grid][10]: per-CTA clock64 / globaltimer stamps (development only) */
-  int32_t cluster_m;     /* 0 = auto, 1 = no clusters, 2 = CTA pairs (2-CTA clusters sharing B by TMA multicast) on adjacent row blocks */
   /* ---- ABI v2: 16-bit operand formats and split precision -------------------------------------------------
    * Forward operands (activations, weights) are IEEE fp16 (11 significant bits; the reference's own reduced
    * precision mode is fp16, train_concap.py:504-505), gradient operands are bf16 (range). a_fp16 / b_fp16 / out_fp16:
@@ -136,10 +134,10 @@ typedef struct vb_gemm_args {
 
 vb_status vb_gemm_bf16(const vb_gemm_args* args, void* stream);
 
-/* Host-only query: the tile configuration vb_gemm_bf16 would use for `args` (fields block_n / cluster_m / split_k that are
-   non-zero in `args` are honoured) on a device with `sm_count` SMs (0 = the current CUDA device). No GPU work, no device
+/* Host-only query: the tile configuration vb_gemm_bf16 would use for `args` (fields block_n / split_k that are non-zero
+   in `args` are honoured) on a device with `sm_count` SMs (0 = the current CUDA device). No GPU work, no device
    needed when sm_count > 0; only the shape, layout, epilogue and output fields of `args` are read. */
-vb_status vb_gemm_plan(const vb_gemm_args* args, int32_t sm_count, int32_t* block_n, int32_t* cluster_m, int32_t* split_k);
+vb_status vb_gemm_plan(const vb_gemm_args* args, int32_t sm_count, int32_t* block_n, int32_t* split_k);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused attention:  P = softmax(Q K^T * scale + mask[b, key]),  O = P V, heads merged in the output.

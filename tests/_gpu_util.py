@@ -58,7 +58,7 @@ def assert_launched(names, *patterns):
 
 # ------------------------------------------------------------------------------------------ GEMM
 def gemm_case(M, N, K, a_mn=False, b_mn=False, bias=False, res=False, act=0, out_bf16=False, atomic=False, split_k=1, block_n=0,
-              alpha=1.0, check=True, iters=0, seed=0, both_outputs=False, cluster_m=0, a_fp16=False, b_fp16=False, out_fp16=False,
+              alpha=1.0, check=True, iters=0, seed=0, both_outputs=False, a_fp16=False, b_fp16=False, out_fp16=False,
               split=False):
     """Returns (max relative error vs fp32 matmul of the 16-bit operands, ms per launch or None). a_fp16 / b_fp16 / out_fp16
     pick fp16 instead of bf16 per operand (mixed formats = the dgrad / wgrad configuration). split=True stores A and B as
@@ -103,7 +103,6 @@ def gemm_case(M, N, K, a_mn=False, b_mn=False, bias=False, res=False, act=0, out
     g.out_bf16, g.ld_out_bf16 = (out16.data_ptr(), N) if out_bf16 and not atomic else (None, 0)
     g.out_pre, g.ld_out_pre = (pre16.data_ptr(), N) if pre16 is not None else (None, 0)
     g.atomic_out, g.split_k, g.block_n, g.max_ctas = int(atomic), split_k, block_n, 0
-    g.cluster_m = cluster_m
     g.a_fp16, g.b_fp16, g.out_fp16 = int(a_fp16), int(b_fp16), int(out_fp16)
     if split:
         g.A_lo, g.B_lo = Al_st.data_ptr(), Bl_st.data_ptr()

@@ -318,8 +318,8 @@ def _wgrad_args(M, N, K, ldb, g):
 def test_gemm_split_k_partials(M, N, K, ldb):
     lib, g = L.lib(), _gen(M + N + K)
     a, dy, x = _wgrad_args(M, N, K, ldb, g)
-    bn, cl, sp = C.c_int32(), C.c_int32(), C.c_int32()
-    L.check(lib.vb_gemm_plan(C.byref(a), 0, C.byref(bn), C.byref(cl), C.byref(sp)))
+    bn, sp = C.c_int32(), C.c_int32()
+    L.check(lib.vb_gemm_plan(C.byref(a), 0, C.byref(bn), C.byref(sp)))
     S = sp.value
     ws = _ws(S * M * N)
     base = torch.randn(M, N, device=DEV, generator=g)

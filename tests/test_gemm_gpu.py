@@ -43,17 +43,18 @@ def test_mn_major_operands(a_mn, b_mn, M, N, K, bn):
 @pytest.mark.parametrize("bn", [128, 256])
 @pytest.mark.parametrize("kw,shape", [
     (dict(bias=True, res=True), (2304, 768, 768)),                       # even number of row blocks
-    (dict(bias=True, out_bf16=True), (6400, 3072, 1024)),                # several items per cluster, accumulator double buffering
-    (dict(bias=True, res=True), (333, 1601, 1024)),                      # 3 row blocks: the last pair has an idle half; ragged N
+    (dict(bias=True, out_bf16=True), (6400, 3072, 1024)),                # several tiles per CTA
+    (dict(bias=True, res=True), (333, 1601, 1024)),                      # odd number of row blocks (3); ragged N
     (dict(bias=True, act=L.VB_ACT_GELU, out_bf16=True), (1000, 520, 200)),
-    (dict(b_mn=True, res=True), (2304, 768, 3072)),                      # dgrad form: B read MN-major, its 64-column boxes split across the pair
+    (dict(b_mn=True, res=True), (2304, 768, 3072)),                      # dgrad form: B read MN-major
     (dict(a_mn=True, b_mn=True, atomic=True, split_k=0), (1024, 1024, 6400)),   # wgrad form with split-K
     (dict(a_mn=True, b_mn=True, atomic=True, split_k=3), (768, 520, 2304)),
 ])
-def test_cta_pairs(kw, shape, bn):
-    """cluster_m=2: CTA pairs (2-CTA clusters) on adjacent row blocks; each CTA loads half of the B tile and multicasts it to both (vb_gemm.cu)."""
+def test_forced_tile_widths(kw, shape, bn):
+    """block_n fixed by the caller: both tile widths on even and odd row-block counts, the dgrad and wgrad operand forms and
+    split-K."""
     from _gpu_util import gemm_case
-    err, _ = gemm_case(*shape, block_n=bn, cluster_m=2, **kw)
+    err, _ = gemm_case(*shape, block_n=bn, **kw)
     assert err < 2e-3, err
 
 
@@ -64,7 +65,7 @@ def test_cta_pairs(kw, shape, bn):
     (dict(b_mn=True, res=True), (2304, 768, 3072)),
     (dict(a_mn=True, b_mn=True, atomic=True, split_k=0), (1024, 1024, 6400)),
     (dict(b_mn=True, out_bf16=True), (333, 1601, 1024)),
-    (dict(bias=True, out_bf16=True, out_fp16=True, cluster_m=2, block_n=256), (1000, 520, 200)),
+    (dict(bias=True, out_bf16=True, out_fp16=True, block_n=256), (1000, 520, 200)),
 ])
 def test_fp16_operands(kw, shape):
     """fp16 x fp16 (the forward operand format of the default precision), fp16 16-bit outputs, every operand major."""
@@ -89,11 +90,11 @@ def test_mixed_operand_formats_are_rejected():
 @pytest.mark.parametrize("kw,shape", [
     (dict(bias=True, res=True), (2304, 768, 768)),
     (dict(bias=True, out_bf16=True), (6400, 3072, 1024)),
-    (dict(bias=True, out_bf16=True, cluster_m=1, block_n=128), (1000, 520, 200)),
+    (dict(bias=True, out_bf16=True, block_n=128), (1000, 520, 200)),
     (dict(bias=True, act=L.VB_ACT_GELU, out_bf16=True), (300, 200, 136)),
     (dict(bias=True, act=L.VB_ACT_RELU, out_bf16=True, both_outputs=True), (64, 1024, 768)),
     (dict(bias=True), (130, 30522, 768)),
-    (dict(bias=True, res=True, cluster_m=2), (6400, 1024, 4096)),
+    (dict(bias=True, res=True), (6400, 1024, 4096)),
 ])
 def test_split_precision(kw, shape):
     """fp32 parity mode: operands as fp16 hi + lo, three passes (hi.hi + lo.hi + hi.lo) into one register accumulator; the

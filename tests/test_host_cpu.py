@@ -19,7 +19,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/vilbert_b200.h but not exported"
     assert set(L._SIGNATURES) <= set(declared)
-    assert lib.vb_version() == 2
+    assert lib.vb_version() == 3
     assert ctypes.sizeof(L.GemmArgs) >= 160 and ctypes.sizeof(L.AttnArgs) >= 150
 
 
@@ -285,9 +285,9 @@ def test_ddp_segments_partition_the_gradient_buffer(golden_dir):
 
 
 def test_gemm_tile_configuration_cost_model():
-    """vb_gemm_plan (host only): the (tile width, CTA pairing, k splits) vb_gemm_bf16 picks for the model's GEMM shapes on a
-    132-SM device — 256-wide tiles for the large image-stream problems, 128-wide tiles where the tile count binds, split-K only
-    for the weight-gradient form, CTA pairs only when asked for; caller-fixed values are honoured, nonsense is rejected."""
+    """vb_gemm_plan (host only): the (tile width, k splits) vb_gemm_bf16 picks for the model's GEMM shapes on a 132-SM device
+    — 256-wide tiles for the large image-stream problems, 128-wide tiles where the tile count binds, split-K only for the
+    weight-gradient form; caller-fixed values are honoured, nonsense is rejected."""
     import ctypes as C
     from vilbert_b200 import _lib as L
     lib = L.lib()
@@ -295,7 +295,7 @@ def test_gemm_tile_configuration_cost_model():
     def plan(M, N, K, sms=132, **kw):
         g = L.GemmArgs(); g.M, g.N, g.K, g.alpha = M, N, K, 1.0
         g.A = g.B = 0x1000                                     # never dereferenced by the query
-        g.block_n, g.cluster_m = kw.get("block_n", 0), kw.get("cluster_m", 0)
+        g.block_n = kw.get("block_n", 0)
         if kw.get("atomic"):
             g.atomic_out, g.out_f32, g.split_k = 1, 0x1000, kw.get("split_k", 0)
         else:
@@ -303,24 +303,21 @@ def test_gemm_tile_configuration_cost_model():
             if kw.get("bf16"): g.out_bf16 = 0x1000
             else: g.out_f32 = 0x1000
             if kw.get("res"): g.residual = 0x1000
-        bn, cl, sp = C.c_int32(), C.c_int32(), C.c_int32()
-        st = lib.vb_gemm_plan(C.byref(g), sms, C.byref(bn), C.byref(cl), C.byref(sp))
-        return st, (bn.value, cl.value, sp.value)
+        bn, sp = C.c_int32(), C.c_int32()
+        st = lib.vb_gemm_plan(C.byref(g), sms, C.byref(bn), C.byref(sp))
+        return st, (bn.value, sp.value)
 
-    assert plan(6400, 3072, 1024, bf16=True) == (0, (256, 1, 1))          # image QKV: 256-wide tiles
-    assert plan(8192, 8192, 8192, bf16=True) == (0, (256, 1, 1))
-    assert plan(2304, 768, 768, res=True) == (0, (128, 1, 1))             # text out-proj: 108 tiles on 132 SMs
-    st, (bn, cl, sp) = plan(3072, 1024, 6400, atomic=True)                # image QKV weight gradient
-    assert st == 0 and cl == 1 and sp > 1
-    st, (bn, cl, sp) = plan(768, 768, 2304, atomic=True)
+    assert plan(6400, 3072, 1024, bf16=True) == (0, (256, 1))             # image QKV: 256-wide tiles
+    assert plan(8192, 8192, 8192, bf16=True) == (0, (256, 1))
+    assert plan(2304, 768, 768, res=True) == (0, (128, 1))                # text out-proj: 108 tiles on 132 SMs
+    st, (bn, sp) = plan(3072, 1024, 6400, atomic=True)                    # image QKV weight gradient
+    assert st == 0 and sp > 1
+    st, (bn, sp) = plan(768, 768, 2304, atomic=True)
     assert st == 0 and sp > 1                                             # 36 tiles: split K to fill the SMs
-    assert plan(6400, 1024, 1024, res=True)[1][2] == 1                    # no split-K outside the atomic form
-    assert plan(6400, 3072, 1024, bf16=True, block_n=128, cluster_m=1) == (0, (128, 1, 1))
-    assert plan(6400, 3072, 1024, bf16=True, cluster_m=2) == (0, (256, 2, 1))
-    assert plan(3072, 1024, 6400, atomic=True, split_k=5)[1][2] == 5
-    assert plan(64, 1024, 768, cluster_m=2)[1][1] == 1                    # one row block: nothing to pair
+    assert plan(6400, 1024, 1024, res=True)[1][1] == 1                    # no split-K outside the atomic form
+    assert plan(6400, 3072, 1024, bf16=True, block_n=128) == (0, (128, 1))
+    assert plan(3072, 1024, 6400, atomic=True, split_k=5)[1][1] == 5
     assert plan(6400, 1024, 1024, block_n=64)[0] == 1 and b"block_n" in lib.vb_last_error()
-    assert plan(6400, 1024, 1024, cluster_m=3)[0] == 1 and b"cluster_m" in lib.vb_last_error()
     assert plan(6400, 1024, 1024, res=True, split_k=2)[0] == 1 and b"split_k" in lib.vb_last_error()
 
 

@@ -260,18 +260,17 @@ def _pad8(n):
 
 
 def _plan(g):
-    bn, cl, sp = C.c_int32(), C.c_int32(), C.c_int32()
-    L.check(L.lib().vb_gemm_plan(C.byref(g), 0, C.byref(bn), C.byref(cl), C.byref(sp)), "vb_gemm_plan")
-    return bn.value, cl.value, sp.value
+    bn, sp = C.c_int32(), C.c_int32()
+    L.check(L.lib().vb_gemm_plan(C.byref(g), 0, C.byref(bn), C.byref(sp)), "vb_gemm_plan")
+    return bn.value, sp.value
 
 
 @pytest.mark.parametrize("block_n", [128, 256])
-@pytest.mark.parametrize("cluster_m", [1, 2])
 @pytest.mark.parametrize("M,N,K,aux_pad", [
     (2304, 3072, 768, 0), (6400, 1024, 1024, 0),      # config 2's text / image FFN dgrads: every chunk full -> fast column sum
     (1000, 520, 200, 0), (333, 1601, 1024, 0),        # ragged rows / columns: fast chunks plus the generic tail
     (1000, 520, 200, 1)])                             # ld_aux % 4 != 0: no vector aux loads -> generic column sum everywhere
-def test_gemm_dgelu_colsum(M, N, K, aux_pad, block_n, cluster_m):
+def test_gemm_dgelu_colsum(M, N, K, aux_pad, block_n):
     """dgrad of the FFN intermediate: dx = (dy W) * gelu'(pre) as bf16, out_colsum += column sums (the intermediate bias
     gradient). B is the weight stored [K, N] (MN-major), operands bf16. EPI_DGELU: the fast path reduces each 16 x 32 chunk over
     its 4 row lanes by shuffles, then one atomic per column; ragged chunks and unaligned aux run the generic epilogue."""
@@ -294,15 +293,15 @@ def test_gemm_dgelu_colsum(M, N, K, aux_pad, block_n, cluster_m):
     g.aux, g.ld_aux = aux.data_ptr(), ld_aux
     g.out_bf16, g.ld_out_bf16 = out.data_ptr(), ldn
     g.out_colsum = cs.data_ptr()
-    g.block_n, g.cluster_m = block_n, cluster_m
-    assert _plan(g) == (block_n, cluster_m, 1)
+    g.block_n = block_n
+    assert _plan(g) == (block_n, 1)
     L.check(L.lib().vb_gemm_bf16(C.byref(g), _st()), "vb_gemm_bf16")
     torch.cuda.synchronize()
     v = (A[:, :K].to(F64) @ W[:, :N].to(F64)) * aux[:, :N].to(F64)
     errs = dict(out=relmax(out[:, :N], v), colsum=colsum_err(cs, base, v))
     # a column sum that loses one 16-row epilogue chunk (the last one)
     wrongs = {"lost chunk": dict(colsum=colsum_err(cs, base, v[:M - 16]))}
-    verdict(f"gemm dgelu colsum {M}x{N}x{K} bn{block_n} cl{cluster_m} ld_aux%4={ld_aux % 4}", errs, dict(out=5e-3, colsum=1e-5), wrongs)
+    verdict(f"gemm dgelu colsum {M}x{N}x{K} bn{block_n} ld_aux%4={ld_aux % 4}", errs, dict(out=5e-3, colsum=1e-5), wrongs)
 
 
 GEMM_SITE = dropout_site_id("bert.encoder.v_layer.2.output.dropout")

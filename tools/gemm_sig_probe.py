@@ -28,7 +28,7 @@ from vilbert_b200 import _lib as L  # noqa: E402
 PEAK_TFLOPS, PEAK_TBS = 989.0, 3.35
 PTR_FIELDS = ("A", "B", "bias", "residual", "aux", "out_f32", "out_bf16", "out_pre", "out_colsum", "A_lo", "B_lo", "out_lo", "out_b16")
 SCALAR_FIELDS = ("M", "N", "K", "lda", "a_mn_major", "ldb", "b_mn_major", "alpha", "ld_res", "ld_aux", "act", "ld_out_f32", "ld_out_bf16",
-                 "ld_out_pre", "atomic_out", "split_k", "block_n", "max_ctas", "cluster_m", "a_fp16", "b_fp16", "out_fp16")
+                 "ld_out_pre", "atomic_out", "split_k", "block_n", "max_ctas", "a_fp16", "b_fp16", "out_fp16")
 
 
 def signature(g):
@@ -84,9 +84,9 @@ def resolved_tiles(s):
         setattr(g, f, s[f])
     for f in s["set"]:
         setattr(g, f, 256)   # non-null placeholder: vb_gemm_plan reads only which pointers are set
-    bn, cl, sp = C.c_int32(), C.c_int32(), C.c_int32()
-    L.check(L.lib().vb_gemm_plan(C.byref(g), 132, C.byref(bn), C.byref(cl), C.byref(sp)), "vb_gemm_plan")
-    return bn.value, cl.value, sp.value
+    bn, sp = C.c_int32(), C.c_int32()
+    L.check(L.lib().vb_gemm_plan(C.byref(g), 132, C.byref(bn), C.byref(sp)), "vb_gemm_plan")
+    return bn.value, sp.value
 
 
 class Launch:
@@ -100,7 +100,7 @@ class Launch:
         dev = torch.device("cuda")
         gen = torch.Generator(device=dev).manual_seed(seed)
         f16 = lambda fmt: torch.float16 if fmt else torch.bfloat16
-        _, _, sp = resolved_tiles(s)
+        _, sp = resolved_tiles(s)
         rows = {"A": K if s["a_mn_major"] else M, "B": K if s["b_mn_major"] else N, "bias": 1, "residual": M, "aux": M,
                 "out_f32": M * (sp if s["atomic_out"] == L.VB_GEMM_PARTIALS else 1), "out_bf16": M, "out_pre": M, "out_colsum": 1,
                 "A_lo": K if s["a_mn_major"] else M, "B_lo": K if s["b_mn_major"] else N, "out_lo": M, "out_b16": M}
@@ -179,13 +179,13 @@ def probe(sig, iters, stream):
     ln.g.dbg_timeline = None
     t = dbg.view(-1, 10).cpu()
     t = t[t[:, 0] != 0][:, :8].double()
-    bn, cl, sp = resolved_tiles(ln.s)
+    bn, sp = resolved_tiles(ln.s)
     s = ln.s
     kbs = -(-s["K"] // 64) * (1 + ("A_lo" in s["set"]) + ("B_lo" in s["set"]))
     kps = -(-kbs // sp)
     med = lambda x: float(x.median()) if len(x) else float("nan")
     fl, by = ln.flops(), ln.bytes()
-    return dict(sig=short(s), args=s, block_n=bn, cluster=cl, split_k=sp, us=us, tflops=fl / us / 1e6,
+    return dict(sig=short(s), args=s, block_n=bn, split_k=sp, us=us, tflops=fl / us / 1e6,
                 floor_us=max(fl / PEAK_TFLOPS / 1e6, by / PEAK_TBS / 1e6), bytes=by, flops=fl,
                 cyc_first_full=med(t[:, 3] - t[:, 0]), cyc_per_kblock=med((t[:, 5] - t[:, 3]) / kps), cyc_epilogue=med(t[:, 6] - t[:, 5]))
 
@@ -211,8 +211,8 @@ def main():
         for k, cnt in sigs.items():
             s = describe(k)
             if a.list:
-                bn, cl, sp = resolved_tiles(s)
-                print(f"  {short(s):64s} x{cnt:3d}  bn{bn} cl{cl} sk{sp}")
+                bn, sp = resolved_tiles(s)
+                print(f"  {short(s):64s} x{cnt:3d}  bn{bn} sk{sp}")
                 continue
             r = probe(k, a.iters, stream)
             r["per_step"] = cnt
@@ -221,10 +221,10 @@ def main():
         if a.list:
             continue
         rows.sort(key=lambda r: -r["us_per_step"])
-        print(f"  {'signature':64s} {'bn/cl/sk':>9s} {'n':>3s} {'us':>8s} {'TFLOP/s':>8s} {'floor':>7s} {'us/step':>8s} "
+        print(f"  {'signature':64s} {'bn/sk':>7s} {'n':>3s} {'us':>8s} {'TFLOP/s':>8s} {'floor':>7s} {'us/step':>8s} "
               f"{'cyc->full':>9s} {'cyc/kblk':>8s} {'cyc epi':>8s}")
         for r in rows:
-            print(f"  {r['sig']:64s} {r['block_n']:4d}/{r['cluster']}/{r['split_k']:<2d} {r['per_step']:3d} {r['us']:8.1f} {r['tflops']:8.1f} "
+            print(f"  {r['sig']:64s} {r['block_n']:4d}/{r['split_k']:<2d} {r['per_step']:3d} {r['us']:8.1f} {r['tflops']:8.1f} "
                   f"{r['floor_us']:7.1f} {r['us_per_step']:8.1f} {r['cyc_first_full']:9.0f} {r['cyc_per_kblock']:8.0f} {r['cyc_epilogue']:8.0f}")
         tot = sum(r["us_per_step"] for r in rows)
         print(f"  total {tot / 1e3:.3f} ms of GEMM per step (serial), floor {sum(r['floor_us'] * r['per_step'] for r in rows) / 1e3:.3f} ms", flush=True)

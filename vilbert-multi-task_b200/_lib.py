@@ -49,8 +49,7 @@ class GemmArgs(C.Structure):
         ("out_bf16", C.c_void_p), ("ld_out_bf16", C.c_int64),
         ("out_pre", C.c_void_p), ("ld_out_pre", C.c_int64),
         ("atomic_out", C.c_int32), ("out_colsum", C.c_void_p), ("dropout", DropoutSite), ("split_k", C.c_int32), ("block_n", C.c_int32), ("max_ctas", C.c_int32),
-        ("dbg_lbo_a", C.c_uint32), ("dbg_sbo_a", C.c_uint32), ("dbg_lbo_b", C.c_uint32), ("dbg_sbo_b", C.c_uint32),
-        ("dbg_timeline", C.c_void_p), ("cluster_m", C.c_int32),
+        ("dbg_timeline", C.c_void_p),
         ("a_fp16", C.c_int32), ("b_fp16", C.c_int32), ("out_fp16", C.c_int32),
         ("A_lo", C.c_void_p), ("B_lo", C.c_void_p), ("out_lo", C.c_void_p), ("out_b16", C.c_void_p),
     ]
@@ -87,7 +86,7 @@ _P, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 _SIGNATURES = {
     "vb_device_info": [C.POINTER(C.c_int), C.POINTER(C.c_int)],
     "vb_gemm_bf16": [C.POINTER(GemmArgs), _P],
-    "vb_gemm_plan": [C.POINTER(GemmArgs), C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)],
+    "vb_gemm_plan": [C.POINTER(GemmArgs), C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)],
     "vb_attention_fwd": [C.POINTER(AttnArgs), _P],
     "vb_attention_bwd": [C.POINTER(AttnArgs), _P],
     "vb_attention_probs": [C.POINTER(AttnArgs), _P, _P],

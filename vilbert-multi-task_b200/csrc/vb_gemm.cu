@@ -16,8 +16,6 @@
 //                    16-bit conversion, while the producer already loads the next tile's stages.
 // Operands may be K-major (nn.Linear forward) or MN-major (dgrad / wgrad operands read in place, no transposed copies); both
 // are the canonical SWIZZLE_128B layouts TMA writes, wgmma reads the MN-major ones with its transpose flag.
-// CTA pairs (cluster_m = 2): a 2-CTA cluster on adjacent row blocks of one column block; each CTA loads half of the common B
-// tile and multicasts it into both, so B crosses from L2 once per pair.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -43,8 +41,8 @@ constexpr int EPI_PS = EPI_ROWS / 4;      // passes of the coalesced epilogue (4
 constexpr int STAGING_BYTES_PER_WARP = EPI_ROWS * 32 * 4;
 __device__ __forceinline__ int stg_off(int row, int col) { return row * 32 + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3)); }
 
-// One stage = the 128 x 64 A box and the BN x 64 B box (in a CTA pair each CTA still holds the whole B box: half loaded by
-// itself, half multicast by the peer). 192 KB of stages leave room for the staging tiles within the 227 KB of an H100 block.
+// One stage = the 128 x 64 A box and the BN x 64 B box. 192 KB of stages leave room for the staging tiles within the 227 KB of
+// an H100 block.
 template <int BN>
 struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
@@ -84,9 +82,6 @@ struct GemmKernelParams {
   int mma_kind;              // bit 0: B MN-major, bit 1: A MN-major, bit 2: fp16 operands (else bf16)
   DropCfg drop;              // dropout on the epilogue value before the residual add (EPI_F32 / generic)
   int a_mn, b_mn;            // operand majors
-  int cluster;               // 1, or 2 = CTA pairs: the two CTAs of a cluster take adjacent row blocks of one column block and
-                             // share its B tile through TMA multicast
-  int num_m_groups;          // ceil(num_m_blocks / cluster)
   int fast_ok;               // every buffer the specialised epilogue touches allows 128/64-bit accesses
   unsigned long long* dbg;   // optional per-CTA timeline [grid][10] (8 x clock64 + 2 x globaltimer ns), NULL in production
 };
@@ -294,13 +289,12 @@ __device__ __forceinline__ void stage_chunk(const float (&d)[NR], int c4, float*
   }
 }
 
-template <int BN, int EPI, int CG, int OUT16>
+template <int BN, int EPI, int OUT16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_a_lo, const __grid_constant__ CUtensorMap tmap_b_lo,
                   const __grid_constant__ GemmKernelParams p) {
   using Cfg = GemmCfg<BN>;
-  constexpr bool pair = (CG == 2);
   constexpr int NUM_STAGES = Cfg::NUM_STAGES;
 
   // SWIZZLE_128B tiles need 1024-byte alignment: the kernel has no static shared memory, so the dynamic window starts at
@@ -325,23 +319,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (p.npass > 1) { tma_prefetch_desc(&tmap_a_lo); tma_prefetch_desc(&tmap_b_lo); }
     for (int s = 0; s < NUM_STAGES; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), CONSUMER_WARPS * CG);   // one arrive per consumer warp (of both CTAs of a pair)
+      mbar_init(smem_u32(&empty_bar[s]), CONSUMER_WARPS);   // one arrive per consumer warp
     }
     fence_mbar_init();
   }
   __syncthreads();
-  // the barriers of both CTAs of a pair must exist before the peer's multicast loads / arrives reach them
-  if constexpr (pair) cluster_sync_all();
   pdl_entry();   // everything above (barrier init, descriptor prefetch) overlapped the previous kernel's tail
   if (threadIdx.x == 0) VB_DBG(1);
 
-  // work items = (row-block group, column block, k split); the CTAs of a pair walk the same items in lockstep, CTA
-  // `crank` takes row block group * cluster + crank (possibly past the matrix: it then loads zero rows and stores
-  // nothing, but still loads and multicasts its half of B)
-  const int crank = pair ? (int)cluster_ctarank() : 0;
-  const int group = blockIdx.x / CG;
-  const int num_groups = gridDim.x / CG;
-  const int total_work = p.num_m_groups * p.num_n_blocks * p.split_k;
+  // work items = (row block, column block, k split), walked by the persistent CTAs in grid-stride order
+  const int group = blockIdx.x;
+  const int num_groups = gridDim.x;
+  const int total_work = p.num_m_blocks * p.num_n_blocks * p.split_k;
 
   // Register split: one lane of the producer warpgroup issues the loads, the consumers hold the accumulators (BN / 2 per thread
   // at BN = 256). 128 x 40 + 256 x 232 = 64512 of the 65536 registers the launch bounds give the CTA (168 per thread). Each
@@ -355,41 +344,28 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     for (int w = group; w < total_work; w += num_groups) {
       const int split = w % p.split_k;
       const int t2 = w / p.split_k;
-      const int m_blk = (t2 % p.num_m_groups) * CG + crank;
-      const int n_blk = t2 / p.num_m_groups;
+      const int m_blk = t2 % p.num_m_blocks;
+      const int n_blk = t2 / p.num_m_blocks;
       const int kb0 = split * p.k_blocks_per_split;
       const int kb1 = min(kb0 + p.k_blocks_per_split, p.num_k_blocks);
       // loads of one (real) k-block from the given tensor maps; split precision selects hi / lo maps per pass
       auto issue_loads = [&](const CUtensorMap* tma_a, const CUtensorMap* tma_b, int kb) {
-        // in a pair this stage of BOTH CTAs is free: each consumer warp arrives on its own and on the peer's empty barrier
         mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
         const uint32_t sa = smem_u32(smem_tiles + stage * Cfg::STAGE_BYTES);
         const uint32_t sb = sa + Cfg::A_BYTES;
         const uint32_t fb = smem_u32(&full_bar[stage]);
-        mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);   // a pair's B bytes arrive half from this CTA, half from the peer
+        mbar_arrive_expect_tx(fb, Cfg::STAGE_BYTES);
         if (p.a_mn) {
 #pragma unroll
           for (int j = 0; j < BM / 64; ++j) tma_load_2d(sa + j * (BK * 128), tma_a, m_blk * BM + j * 64, kb * BK, fb);
         } else {
           tma_load_2d(sa, tma_a, kb * BK, m_blk * BM, fb);
         }
-        if constexpr (!pair) {
-          if (p.b_mn) {
+        if (p.b_mn) {
 #pragma unroll
-            for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * (BK * 128), tma_b, n_blk * BN + j * 64, kb * BK, fb);
-          } else {
-            tma_load_2d(sb, tma_b, kb * BK, n_blk * BN, fb);
-          }
+          for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * (BK * 128), tma_b, n_blk * BN + j * 64, kb * BK, fb);
         } else {
-          if (p.b_mn) {   // 64-column boxes [crank * BN/128, +BN/128) of the tile
-#pragma unroll
-            for (int j = 0; j < BN / 128; ++j) {
-              const int jj = crank * (BN / 128) + j;
-              tma_load_2d_multicast(sb + jj * (BK * 128), tma_b, n_blk * BN + jj * 64, kb * BK, fb, 0x3);
-            }
-          } else {        // rows [crank * BN/2, +BN/2) of the tile (tensor-map box = BN/2 rows)
-            tma_load_2d_multicast(sb + crank * (BN / 2) * 128, tma_b, kb * BK, n_blk * BN + crank * (BN / 2), fb, 0x3);
-          }
+          tma_load_2d(sb, tma_b, kb * BK, n_blk * BN, fb);
         }
       };
       for (int kbv = kb0; kbv < kb1; ++kbv) {
@@ -420,10 +396,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const uint32_t a_off = wg * (64 * 128);
     auto release = [&](int s) {
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(smem_u32(&empty_bar[s]));
-        if constexpr (pair) mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[s]), (uint32_t)(crank ^ 1)));
-      }
+      if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));
     };
     float acc[BN / 2];
     int stage = 0;
@@ -433,8 +406,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     for (int w = group; w < total_work; w += num_groups) {
       const int split = w % p.split_k;
       const int t2 = w / p.split_k;
-      const int m_blk = (t2 % p.num_m_groups) * CG + crank;
-      const int n_blk = t2 / p.num_m_groups;
+      const int m_blk = t2 % p.num_m_blocks;
+      const int n_blk = t2 / p.num_m_blocks;
       const int kb0 = split * p.k_blocks_per_split;
       const int kb1 = min(kb0 + p.k_blocks_per_split, p.num_k_blocks);
       int prev = -1;
@@ -520,8 +493,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     }
   }
 
-  // a pair's peer may still multicast into this CTA's stages / arrive on its barriers until both are done
-  if constexpr (pair) cluster_sync_all();
   if (threadIdx.x == 0) { VB_DBG(7); VB_DBG_NS(9); }
 #undef VB_DBG
 #undef VB_DBG_NS
@@ -561,90 +532,58 @@ static int make_tmap(CUtensorMap* tm, const void* ptr, uint64_t inner, uint64_t 
   return VB_OK;
 }
 
-template <int BN, int EPI, int CG, int OUT16 = 0>
+template <int BN, int EPI, int OUT16 = 0>
 static int launch_gemm(const CUtensorMap* tm, GemmKernelParams& p, long long total_work, int max_ctas,
                        cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_wgmma_kernel<BN, EPI, CG, OUT16>;
+  auto kern = gemm_wgmma_kernel<BN, EPI, OUT16>;
   static bool attr_set = false;  // per template instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  // persistent grid: one CTA per SM; with clusters, as many clusters as the device can keep resident at once (a GPC
-  // with an odd number of SMs cannot host a pair on all of them) so that no cluster waits for a second wave
-  int groups_cap = max_ctas;
-  if (CG > 1) {
-    static int max_clusters = -1;   // per template instantiation; cluster size is 2 whenever it is not 1
-    if (max_clusters < 0) {
-      cudaLaunchConfig_t cfg{};
-      cfg.gridDim = dim3(2 * sm_count()); cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeClusterDimension;
-      at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-      cfg.attrs = at; cfg.numAttrs = 1;
-      int n = 0;
-      cudaError_t eo = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
-      if (eo != cudaSuccess || n <= 0) return set_error(VB_ERR_CUDA, "cudaOccupancyMaxActiveClusters: %s", cudaGetErrorString(eo));
-      max_clusters = n;
-    }
-    groups_cap = max_ctas / CG < max_clusters ? max_ctas / CG : max_clusters;
-  }
-  const int groups = (int)(total_work < groups_cap ? total_work : groups_cap);
-  const int grid = groups * CG;
-  cudaError_t e = launch_pdl_cluster(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)Cfg::SMEM_BYTES, stream, CG, tm[0], tm[1], tm[2], tm[3], p);
+  // persistent grid: one CTA per SM, fewer when there are fewer work items
+  const int grid = (int)(total_work < max_ctas ? total_work : max_ctas);
+  cudaError_t e = launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)Cfg::SMEM_BYTES, stream, tm[0], tm[1], tm[2], tm[3], p);
   if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "gemm launch: %s", cudaGetErrorString(e));
   return VB_OK;
 }
 
-template <int BN, int CG>
+template <int BN>
 static int launch_gemm_epi(int epi, int out16, const CUtensorMap* tm, GemmKernelParams& p, long long work, int max_ctas,
                            cudaStream_t stream) {
   switch (epi) {
-    case EPI_F32: return launch_gemm<BN, EPI_F32, CG>(tm, p, work, max_ctas, stream);
+    case EPI_F32: return launch_gemm<BN, EPI_F32>(tm, p, work, max_ctas, stream);
     case EPI_BF16:
-      if (out16 == 1) return launch_gemm<BN, EPI_BF16, CG, 1>(tm, p, work, max_ctas, stream);
-      if (out16 == 2) return launch_gemm<BN, EPI_BF16, CG, 2>(tm, p, work, max_ctas, stream);
-      if (out16 == 3) return launch_gemm<BN, EPI_BF16, CG, 3>(tm, p, work, max_ctas, stream);
-      return launch_gemm<BN, EPI_BF16, CG, 0>(tm, p, work, max_ctas, stream);
+      if (out16 == 1) return launch_gemm<BN, EPI_BF16, 1>(tm, p, work, max_ctas, stream);
+      if (out16 == 2) return launch_gemm<BN, EPI_BF16, 2>(tm, p, work, max_ctas, stream);
+      if (out16 == 3) return launch_gemm<BN, EPI_BF16, 3>(tm, p, work, max_ctas, stream);
+      return launch_gemm<BN, EPI_BF16, 0>(tm, p, work, max_ctas, stream);
     case EPI_GELU:
-      if (out16 == 1) return launch_gemm<BN, EPI_GELU, CG, 1>(tm, p, work, max_ctas, stream);
-      if (out16 == 2) return launch_gemm<BN, EPI_GELU, CG, 2>(tm, p, work, max_ctas, stream);
-      if (out16 == 3) return launch_gemm<BN, EPI_GELU, CG, 3>(tm, p, work, max_ctas, stream);
-      return launch_gemm<BN, EPI_GELU, CG, 0>(tm, p, work, max_ctas, stream);
-    case EPI_DGELU: return launch_gemm<BN, EPI_DGELU, CG>(tm, p, work, max_ctas, stream);
-    case EPI_ATOMIC: return launch_gemm<BN, EPI_ATOMIC, CG>(tm, p, work, max_ctas, stream);
-    case EPI_PARTIAL: return launch_gemm<BN, EPI_PARTIAL, CG>(tm, p, work, max_ctas, stream);
-    default: return launch_gemm<BN, EPI_GENERIC, CG>(tm, p, work, max_ctas, stream);
+      if (out16 == 1) return launch_gemm<BN, EPI_GELU, 1>(tm, p, work, max_ctas, stream);
+      if (out16 == 2) return launch_gemm<BN, EPI_GELU, 2>(tm, p, work, max_ctas, stream);
+      if (out16 == 3) return launch_gemm<BN, EPI_GELU, 3>(tm, p, work, max_ctas, stream);
+      return launch_gemm<BN, EPI_GELU, 0>(tm, p, work, max_ctas, stream);
+    case EPI_DGELU: return launch_gemm<BN, EPI_DGELU>(tm, p, work, max_ctas, stream);
+    case EPI_ATOMIC: return launch_gemm<BN, EPI_ATOMIC>(tm, p, work, max_ctas, stream);
+    case EPI_PARTIAL: return launch_gemm<BN, EPI_PARTIAL>(tm, p, work, max_ctas, stream);
+    default: return launch_gemm<BN, EPI_GENERIC>(tm, p, work, max_ctas, stream);
   }
 }
 
 static inline bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
 
-// cluster_m = 0 resolves to this (env VB_GEMM_CLUSTER=1|2 forces one mode, for experiments)
-static int default_cluster() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("VB_GEMM_CLUSTER");
-    v = (e && (e[0] == '1' || e[0] == '2')) ? (e[0] - '0') : 0;   // 0 = chosen per problem by the cost model
-  }
-  return v;
-}
-
-// Chooses (tile width, CTAs per tile group, k splits) for a problem; honours the values the caller fixed. Pure host code.
-static int choose_config(const vb_gemm_args* a, int max_ctas, int* bn_out, int* cluster_out, int* split_out) {
+// Chooses (tile width, k splits) for a problem; honours the values the caller fixed. Pure host code.
+static int choose_config(const vb_gemm_args* a, int max_ctas, int* bn_out, int* split_out) {
   const int num_m = (a->M + BM - 1) / BM;
   const int num_k = (a->K + BK - 1) / BK * (1 + (a->A_lo ? 1 : 0) + (a->B_lo ? 1 : 0));   // virtual k-blocks (split precision passes)
-  // Tile configuration = (tile width bn, CTAs per tile group cg, k splits): minimise the modelled time of the busiest CTA,
+  // Tile configuration = (tile width bn, k splits): minimise the modelled time of the busiest CTA,
   // in SM cycles. The constants are estimates, not measurements: a 64-deep k-block of a 128 x 128 tile is 2.1 MFLOP, ~512
   // cycles at the dense BF16 / FP16 rate of an H100 SM (4096 FLOP per cycle), plus ~10 % for barrier waits and wgmma issue
   // (128 x 256: twice that); the epilogue of a tile follows its main loop (the accumulators live in the consumers' registers)
-  // while the producer already loads the next tile; ~3k cycles of prologue + first-load latency per launch. CTA pairs only
-  // save L2 -> SM traffic of B, which this model does not charge, so they are used when the caller asks for them.
+  // while the producer already loads the next tile; ~3k cycles of prologue + first-load latency per launch.
   if (a->block_n != 0 && a->block_n != 128 && a->block_n != 256) return set_error(VB_ERR_INVALID, "vb_gemm_bf16: block_n must be 0, 128 or 256");
-  int cluster_req = a->cluster_m ? a->cluster_m : default_cluster();
-  if (cluster_req != 0 && cluster_req != 1 && cluster_req != 2) return set_error(VB_ERR_INVALID, "vb_gemm_bf16: cluster_m must be 0, 1 or 2");
   if (a->split_k > 1 && (!a->atomic_out || a->act != VB_ACT_NONE || a->bias || a->residual || a->out_colsum))
     return set_error(VB_ERR_INVALID, "vb_gemm_bf16: split_k > 1 needs atomic_out and a plain epilogue");
   const bool can_split = a->atomic_out && a->act == VB_ACT_NONE && !a->bias && !a->residual && !a->out_colsum;
@@ -653,38 +592,32 @@ static int choose_config(const vb_gemm_args* a, int max_ctas, int* bn_out, int* 
   else if (a->act == VB_ACT_GELU || a->act == VB_ACT_DGELU) epi_base = 4200;
   else if (a->act == VB_ACT_NONE && a->out_f32 && !a->out_bf16) epi_base = a->residual ? 4800 : 3000;
   else if (a->act == VB_ACT_NONE && a->out_bf16 && !a->out_f32) epi_base = 3000;
-  int bn = 128, cluster = 1, split_k = 1;
+  int bn = 128, split_k = 1;
   {
     long long best = -1;
     static const int split_cand[] = {1, 2, 3, 4, 5, 6, 8, 10, 12, 16, 24, 32};
     for (int w = 128; w <= 256; w += 128) {
       if (a->block_n && a->block_n != w) continue;
       if (!a->block_n && w == 256 && a->N <= 128) continue;
-      for (int cg = 1; cg <= 2; ++cg) {
-        if (cluster_req != 2 && cg == 2) continue;
-        if (cluster_req == 2 && cg == 1 && num_m >= 2 && max_ctas >= 2) continue;
-        if (cg == 2 && (num_m < 2 || max_ctas < 2)) continue;
-        const long long t_kb = (w == 128) ? 560 : 1100;
-        const long long epi = epi_base * (w / 128);
-        const long long groups = (cg == 1) ? max_ctas : max_ctas / 2;
-        const long long tiles = (long long)((num_m + cg - 1) / cg) * ((a->N + w - 1) / w);
-        for (int sc : split_cand) {
-          if (a->split_k > 0 && sc != 1) break;
-          int sp = a->split_k > 0 ? a->split_k : sc;
-          if (sp > 1 && !can_split) break;
-          if (sp > num_k) { if (a->split_k > 0) sp = num_k; else break; }
-          const long long kps_ = (num_k + sp - 1) / sp;
-          sp = (int)((num_k + kps_ - 1) / kps_);   // no empty splits
-          const long long rounds = (tiles * sp + groups - 1) / groups;
-          const long long ml = kps_ * t_kb;
-          const long long c = 3000 + rounds * (ml + epi);
-          if (best < 0 || c < best) { best = c; bn = w; cluster = cg; split_k = sp; }
-        }
+      const long long t_kb = (w == 128) ? 560 : 1100;
+      const long long epi = epi_base * (w / 128);
+      const long long tiles = (long long)num_m * ((a->N + w - 1) / w);
+      for (int sc : split_cand) {
+        if (a->split_k > 0 && sc != 1) break;
+        int sp = a->split_k > 0 ? a->split_k : sc;
+        if (sp > 1 && !can_split) break;
+        if (sp > num_k) { if (a->split_k > 0) sp = num_k; else break; }
+        const long long kps_ = (num_k + sp - 1) / sp;
+        sp = (int)((num_k + kps_ - 1) / kps_);   // no empty splits
+        const long long rounds = (tiles * sp + max_ctas - 1) / max_ctas;
+        const long long ml = kps_ * t_kb;
+        const long long c = 3000 + rounds * (ml + epi);
+        if (best < 0 || c < best) { best = c; bn = w; split_k = sp; }
       }
     }
-    if (best < 0) return set_error(VB_ERR_INVALID, "vb_gemm_bf16: no tile configuration for block_n=%d cluster_m=%d split_k=%d", a->block_n, a->cluster_m, a->split_k);
+    if (best < 0) return set_error(VB_ERR_INVALID, "vb_gemm_bf16: no tile configuration for block_n=%d split_k=%d", a->block_n, a->split_k);
   }
-  *bn_out = bn; *cluster_out = cluster; *split_out = split_k;
+  *bn_out = bn; *split_out = split_k;
   return VB_OK;
 }
 
@@ -721,8 +654,8 @@ extern "C" vb_status vb_gemm_bf16(const vb_gemm_args* a, void* stream_) {
   const int num_k = real_k * npass;   // virtual k-blocks (split precision: K is walked once per pass)
   int max_ctas = a->max_ctas > 0 ? a->max_ctas : dev_sms;
 
-  int bn = 128, cluster = 1, split_k = 1;
-  if (int st = choose_config(a, max_ctas, &bn, &cluster, &split_k)) return st;
+  int bn = 128, split_k = 1;
+  if (int st = choose_config(a, max_ctas, &bn, &split_k)) return st;
   const int num_n = (a->N + bn - 1) / bn;
   const int kps = (num_k + split_k - 1) / split_k;
 
@@ -755,18 +688,12 @@ extern "C" vb_status vb_gemm_bf16(const vb_gemm_args* a, void* stream_) {
   // smem matrix descriptors (see vb_ptx.cuh). K-major: rows of 128 B, 8-row groups 1024 B apart (SBO),
   // K advance of 16 elements = 32 B inside the swizzle span. MN-major: 64-element (128 B) rows indexed
   // by k, 8-k groups 1024 B apart (SBO), next 64 MN elements BK*128 B further (LBO); K advance of 16 = 2 groups.
-  const uint32_t lbo_a = a->dbg_lbo_a ? a->dbg_lbo_a : (a->a_mn_major ? BK * 128 : 16);
-  const uint32_t sbo_a = a->dbg_sbo_a ? a->dbg_sbo_a : 1024;
-  const uint32_t lbo_b = a->dbg_lbo_b ? a->dbg_lbo_b : (a->b_mn_major ? BK * 128 : 16);
-  const uint32_t sbo_b = a->dbg_sbo_b ? a->dbg_sbo_b : 1024;
-  p.desc_base_a = gmma_desc_base(lbo_a, sbo_a);
-  p.desc_base_b = gmma_desc_base(lbo_b, sbo_b);
+  p.desc_base_a = gmma_desc_base(a->a_mn_major ? BK * 128 : 16, 1024);
+  p.desc_base_b = gmma_desc_base(a->b_mn_major ? BK * 128 : 16, 1024);
   p.mma_kind = (a->b_mn_major ? 1 : 0) | (a->a_mn_major ? 2 : 0) | (a->a_fp16 ? 4 : 0);
   p.dbg = reinterpret_cast<unsigned long long*>(a->dbg_timeline);
   p.a_mn = a->a_mn_major ? 1 : 0;
   p.b_mn = a->b_mn_major ? 1 : 0;
-  p.cluster = cluster;
-  p.num_m_groups = (num_m + cluster - 1) / cluster;
   p.fast_ok = 0;
   p.drop.ctr = (a->dropout.step && a->dropout.p > 0.f) ? a->dropout.step : nullptr;
   p.drop.site = a->dropout.site;
@@ -784,12 +711,12 @@ extern "C" vb_status vb_gemm_bf16(const vb_gemm_args* a, void* stream_) {
       else               st = make_tmap(&tm[i], ptr, (uint64_t)a->K, (uint64_t)a->M, (uint64_t)a->lda, BK, BM);
     } else {
       if (a->b_mn_major) st = make_tmap(&tm[i], ptr, (uint64_t)a->N, (uint64_t)a->K, (uint64_t)a->ldb, 64, BK);
-      else               st = make_tmap(&tm[i], ptr, (uint64_t)a->K, (uint64_t)a->N, (uint64_t)a->ldb, BK, (uint32_t)(bn / cluster));   // a pair CTA loads half the tile
+      else               st = make_tmap(&tm[i], ptr, (uint64_t)a->K, (uint64_t)a->N, (uint64_t)a->ldb, BK, (uint32_t)bn);
     }
     if (st) return st;
   }
 
-  const long long total_work = (long long)p.num_m_groups * num_n * split_k;
+  const long long total_work = (long long)num_m * num_n * split_k;
   // pick the epilogue specialisation; anything unusual runs the generic one
   int epi = EPI_GENERIC;
   const bool no_extra = !a->out_colsum;
@@ -822,17 +749,13 @@ extern "C" vb_status vb_gemm_bf16(const vb_gemm_args* a, void* stream_) {
   } else if (epi == EPI_DGELU && (a->out_fp16 || a->out_lo || a->out_b16)) {
     epi = EPI_GENERIC;
   }
-  if (cluster == 2) {
-    if (bn == 256) return launch_gemm_epi<256, 2>(epi, out16, tm, p, total_work, max_ctas, stream);
-    return launch_gemm_epi<128, 2>(epi, out16, tm, p, total_work, max_ctas, stream);
-  }
-  if (bn == 256) return launch_gemm_epi<256, 1>(epi, out16, tm, p, total_work, max_ctas, stream);
-  return launch_gemm_epi<128, 1>(epi, out16, tm, p, total_work, max_ctas, stream);
+  if (bn == 256) return launch_gemm_epi<256>(epi, out16, tm, p, total_work, max_ctas, stream);
+  return launch_gemm_epi<128>(epi, out16, tm, p, total_work, max_ctas, stream);
 }
 
-extern "C" vb_status vb_gemm_plan(const vb_gemm_args* a, int32_t sm_count_, int32_t* block_n, int32_t* cluster_m, int32_t* split_k) {
+extern "C" vb_status vb_gemm_plan(const vb_gemm_args* a, int32_t sm_count_, int32_t* block_n, int32_t* split_k) {
   using namespace vb;
-  if (!a || !block_n || !cluster_m || !split_k) return set_error(VB_ERR_INVALID, "vb_gemm_plan: null argument");
+  if (!a || !block_n || !split_k) return set_error(VB_ERR_INVALID, "vb_gemm_plan: null argument");
   if (a->M <= 0 || a->N <= 0 || a->K <= 0) return set_error(VB_ERR_INVALID, "vb_gemm_plan: empty problem %dx%dx%d", a->M, a->N, a->K);
   int sms = sm_count_;
   if (sms <= 0) {
@@ -840,8 +763,8 @@ extern "C" vb_status vb_gemm_plan(const vb_gemm_args* a, int32_t sm_count_, int3
     if (int s = vb_device_info(&sms, &cc)) return s;
   }
   const int max_ctas = a->max_ctas > 0 ? a->max_ctas : sms;
-  int bn, cl, sp;
-  if (int s = choose_config(a, max_ctas, &bn, &cl, &sp)) return s;
-  *block_n = bn; *cluster_m = cl; *split_k = sp;
+  int bn, sp;
+  if (int s = choose_config(a, max_ctas, &bn, &sp)) return s;
+  *block_n = bn; *split_k = sp;
   return VB_OK;
 }

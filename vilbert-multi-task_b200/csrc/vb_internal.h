@@ -37,32 +37,4 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
-
-// Same with a thread-block cluster of `cluster_x` CTAs along x (grid.x must be a multiple of it).
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl_cluster(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, int cluster_x,
-                                      Args&&... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute at[2];
-  int n = 0;
-  if (cluster_x > 1) {
-    at[n].id = cudaLaunchAttributeClusterDimension;
-    at[n].val.clusterDim.x = (unsigned)cluster_x;
-    at[n].val.clusterDim.y = 1;
-    at[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  if (pdl_enabled()) {
-    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  cfg.attrs = at;
-  cfg.numAttrs = n;
-  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-}
 }  // namespace vb

@@ -1,4 +1,4 @@
-// sm_90a PTX wrappers used by the ViLBERT kernels: mbarrier, TMA (cp.async.bulk.tensor, cluster multicast),
+// sm_90a PTX wrappers used by the ViLBERT kernels: mbarrier, TMA (cp.async.bulk.tensor),
 // wgmma (warpgroup MMA from shared-memory descriptors), ldmatrix + mma.sync for the attention tiles.
 // Everything here is inline PTX; no CUTLASS/CuTe dependency.
 #pragma once
@@ -107,38 +107,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* tmap,
       " [%0], [%1, {%2, %3}], [%4];"
       ::"r"(smem_dst), "l"(tmap), "r"(c0), "r"(c1), "r"(bar)
       : "memory");
-}
-
-// Multicast variant: the box lands at the same shared-memory offset in every CTA of `cta_mask`, and its bytes complete on the
-// mbarrier at the same offset in each of them.
-__device__ __forceinline__ void tma_load_2d_multicast(uint32_t smem_dst, const void* tmap, int c0, int c1, uint32_t bar,
-                                                      uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%2, %3}], [%4], %5;"
-      ::"r"(smem_dst), "l"(tmap), "r"(c0), "r"(c1), "r"(bar), "h"(cta_mask)
-      : "memory");
-}
-
-// ---------------------------------------------------------------- thread-block clusters
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster.
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-// Arrive on an mbarrier of another CTA of the cluster (address from mapa_shared).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
-}
-// Full cluster barrier (every thread of every CTA of the cluster executes it).
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- wgmma (Hopper warpgroup MMA)

@@ -1275,8 +1275,8 @@ class Plan:
         if self.det and atomic:
             # split-K weight gradients: each split stores its tile into its own slice of the workspace, one ordered sum adds them
             g.atomic_out, g.split_k = L.VB_GEMM_PARTIALS, 0
-            bn, cl, sp = (L.C.c_int32() for _ in range(3))
-            L.check(self.lib.vb_gemm_plan(L.C.byref(g), 132 if self.dev.type != "cuda" else 0, L.C.byref(bn), L.C.byref(cl), L.C.byref(sp)),
+            bn, sp = L.C.c_int32(), L.C.c_int32()
+            L.check(self.lib.vb_gemm_plan(L.C.byref(g), 132 if self.dev.type != "cuda" else 0, L.C.byref(bn), L.C.byref(sp)),
                     "vb_gemm_plan")
             if sp.value == 1:
                 g.atomic_out, g.split_k = 1, 1      # one CTA per output tile: a single add per element, in launch order
