@@ -68,7 +68,7 @@ def test_checked_plan_is_the_unchecked_plan_plus_its_checks(case):
     plain = _plan(name, over, heads, B, dict(kw, anomaly=False), *extra)
     assert _listing(checked, drop_checks=True) == _listing(plain)
     fn, args, sid = checked.fwd[0]
-    assert fn.__name__ == "vb_nan_check" and args[3] == 1 and sid == 0       # the flag reset opens every forward
+    assert fn.__name__ == "vb_nan_check" and args.reset == 1 and sid == 0       # the flag reset opens every forward
 
 
 def _span(ptr, rows, cols, ld, dt):
@@ -92,9 +92,9 @@ def test_every_backward_gradient_is_checked_after_its_op(case, precision):
     scanned, table = {}, plan.nan_table.data_ptr()
     for section in ("fwd", "bwd"):
         for i, (fn, args, sid) in enumerate(getattr(plan, section)):
-            if fn is not None and fn.__name__ == "vb_nan_check" and not args[3]:
-                first = (args[0] - table) // E.C_SIZEOF_NAN_REGION
-                for k in range(args[1]):
+            if fn is not None and fn.__name__ == "vb_nan_check" and not args.reset:
+                first = (args.regions - table) // E.C_SIZEOF_NAN_REGION
+                for k in range(args.n_regions):
                     scanned[plan.nan_regions[first + k][5]] = (section, i, sid)
     assert sorted(scanned) == list(range(len(plan.nan_records)))
     assert [r.region for r in plan.nan_records] == sorted(scanned)       # ids follow op-list order (fwd objective first)

@@ -127,8 +127,10 @@ def test_baseline_refuses_deterministic_plans():
 
 
 def test_det_prototypes_take_the_default_arguments_plus_a_workspace():
-    lib = E.L.lib()
+    """The parameter names of each _det twin are its default entry point's plus a trailing ws: DET_WORKSPACE sizes the workspace
+    and a twin's engine.ANOMALY_OUTPUTS entry, its default entry point's, reads its launch by those names."""
+    args = E.L.ARGS
     for name, size in E.DET_WORKSPACE.items():
-        base, det = getattr(lib, name).argtypes, getattr(lib, name + "_det").argtypes
-        extra = 0 if size is None else 1
-        assert det[:len(base) - 1] == base[:-1] and len(det) == len(base) + extra, name
+        assert args[name + "_det"]._fields == args[name]._fields + (() if size is None else ("ws",)), name
+    assert args["vb_layernorm_bwd_det"]._fields == args["vb_add_layernorm_bwd"]._fields + ("ws",)
+    assert {n for n in args if n.endswith("_det")} == {n + "_det" for n in E.DET_WORKSPACE} | {"vb_layernorm_bwd_det"}

@@ -161,7 +161,7 @@ def test_layernorm_parameters_frozen(golden_dir):
     full, plan = _plan(cfg), _plan(cfg, frozen)
     _check_frozen_untouched(plan, frozen)
     ln = _ops(plan, "vb_layernorm_bwd")
-    assert len(ln) == len(_ops(full, "vb_layernorm_bwd")) and all(a[12] is None and a[13] is None for a in ln)
+    assert len(ln) == len(_ops(full, "vb_layernorm_bwd")) and all(a.dgamma is None and a.dbeta is None for a in ln)
     assert len(_ops(plan, "vb_gemm_bf16")) == len(_ops(full, "vb_gemm_bf16"))
 
 
@@ -171,7 +171,7 @@ def test_frozen_word_embeddings_with_task_tokens(golden_dir):
     plan = _plan(cfg, frozenset({wn}))
     _check_frozen_untouched(plan, {wn})
     (emb,) = _ops(plan, "vb_embed_text_bwd")
-    assert emb[4] is None and all(a is not None for a in emb[5:8])        # dword NULL; position, type and task tables written
+    assert emb.dword is None and all(a is not None for a in (emb.dpos, emb.dtype, emb.dtask))   # position, type and task tables written
     # the masked-LM decoder tied to it gets no weight gradient either
     assert plan.out_rg["linguisic_prediction"]
 
@@ -198,7 +198,7 @@ def test_dynamic_attention_and_pairs_with_a_frozen_vision_stream(golden_dir, ove
         # the image layers' gate Linears are frozen but their input, the pooled text states, needs a gradient: the gate backward
         # still runs for d pool, without the bias sum (dz NULL) and without the gate's weight gradient
         gates = _ops(plan, "vb_gate_scale_bwd")
-        assert len(gates) == len(_ops(full, "vb_gate_scale_bwd")) and all(a[6] is None and a[7] is not None for a in gates)
+        assert len(gates) == len(_ops(full, "vb_gate_scale_bwd")) and all(a.dz is None and a.dz16 is not None for a in gates)
         assert _ops(plan, "vb_masked_mean_bwd")
 
 

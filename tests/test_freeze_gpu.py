@@ -16,7 +16,6 @@ from vilbert_b200 import _lib as L
 
 pytestmark = pytest.mark.gpu
 BF = torch.bfloat16
-VB_ERR_INVALID = 1        # include/vilbert_b200.h
 
 
 def S():
@@ -98,11 +97,11 @@ def test_partial_attention_backward_rejects_invalid_sets():
     delta = torch.zeros(B, H, Nq, device="cuda")
     a.delta = delta.data_ptr()
     a.dQ = a.dK = a.dV = None
-    assert L.lib().vb_attention_bwd(C.byref(a), S()) == VB_ERR_INVALID
+    assert L.lib().vb_attention_bwd(C.byref(a), S()) == L.VB_ERR_INVALID
     a.dK, a.lddk = dk.data_ptr(), H * D                       # dK without dV
-    assert L.lib().vb_attention_bwd(C.byref(a), S()) == VB_ERR_INVALID
+    assert L.lib().vb_attention_bwd(C.byref(a), S()) == L.VB_ERR_INVALID
     a.dK, a.dV, a.lddv = None, dk.data_ptr(), H * D           # dV without dK
-    assert L.lib().vb_attention_bwd(C.byref(a), S()) == VB_ERR_INVALID
+    assert L.lib().vb_attention_bwd(C.byref(a), S()) == L.VB_ERR_INVALID
     torch.cuda.synchronize()
     del keep
 

@@ -2,6 +2,7 @@
 import ctypes
 import json
 import os
+import re
 
 import pytest
 import torch
@@ -12,15 +13,54 @@ from vilbert_b200.config import BertConfig
 from vilbert_b200.engine import Engine, ParamStore
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_header_function():
     lib = L.lib()
     declared = L.exported_symbols()
     assert len(declared) >= 20
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/vilbert_b200.h but not exported"
-    assert set(L._SIGNATURES) <= set(declared)
     assert lib.vb_version() == 3
     assert ctypes.sizeof(L.GemmArgs) >= 160 and ctypes.sizeof(L.AttnArgs) >= 150
+
+
+def test_header_parser_reads_every_prototype():
+    """The functions bound from the header are every name the header calls like a function: a prototype the parser cannot read
+    fails here instead of going unbound. A type without a ctypes counterpart fails the binding."""
+    assert set(L.FUNCTIONS) == set(re.findall(r"\b(vb_\w+)\s*\(", L.header_text()))
+    funcs, consts, _ = L._parse_header("enum { VB_A = 4, VB_B };\n#define VB_C 7\nvb_status vb_x(int32_t n, void* stream);")
+    assert consts == {"VB_A": 4, "VB_B": 5, "VB_C": 7} and L._bindings(funcs)[1]["vb_x"]._fields == ("n",)
+    with pytest.raises(L.VBError, match="double"):
+        L._bindings(L._parse_header("vb_status vb_x(double d, void* stream);")[0])
+
+
+# the hand-written ctypes mirrors and the header structs they mirror; the optimizers hold the vb_clip_record as an int32 tensor
+MIRRORS = {L.DropoutSite: "vb_dropout_site", L.Dropout: "vb_dropout", L.GemmArgs: "vb_gemm_args", L.AttnArgs: "vb_attn_args",
+           L.AdamWGroup: "vb_adamw_group", L.NanRegion: "vb_nan_region"}
+
+
+def _mirror_fields(cls, prefix=""):
+    """(name, ctypes type) of every field of a mirror, base-class fields first, nested structs flattened."""
+    out = []
+    for c in reversed(cls.__mro__):
+        for f, t in c.__dict__.get("_fields_", ()):
+            out += _mirror_fields(t, f"{prefix}{f}.") if issubclass(t, ctypes.Structure) else [(prefix + f, t)]
+    return out
+
+
+def _header_fields(struct, prefix=""):
+    out = []
+    for t, f in L.STRUCTS[struct]:
+        out += _header_fields(t, f"{prefix}{f}.") if t in L.STRUCTS else [(prefix + f, L.ctype(t))]
+    return out
+
+
+@pytest.mark.parametrize("cls", list(MIRRORS), ids=[c.__name__ for c in MIRRORS])
+def test_struct_mirror_matches_the_header(cls):
+    assert _mirror_fields(cls) == _header_fields(MIRRORS[cls])
+
+
+def test_every_header_struct_but_the_clip_record_has_a_mirror():
+    assert set(MIRRORS.values()) == set(L.STRUCTS) - {"vb_clip_record"}
 
 
 def test_no_fallback_without_gpu():

@@ -149,7 +149,7 @@ def test_input_grad_plan_adds_exactly_two_launches(golden_dir, kind):
     Fv = plan.in_feat.shape[-1]
     g = gemm[1][0]._obj
     assert (g.M, g.N, g.b_mn_major, g.atomic_out, g.residual) == (B * NV, Fv, 1, 0, None)
-    assert dx[1][2] == plan.input_grad["image_loc"].data_ptr() and dx[1][3] == B * NV
+    assert dx[1].dx == plan.input_grad["image_loc"].data_ptr() and dx[1].M == B * NV
     assert tuple(plan.input_grad["input_imgs"].shape) == (B * NV, Fv) and tuple(plan.input_grad["image_loc"].shape) == (B * NV, 5)
     for t in plan.input_grad.values():
         assert _outside_arena(eng, t)

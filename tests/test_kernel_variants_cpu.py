@@ -1,5 +1,6 @@
-"""Every C entry point the Python side binds (vilbert_b200._lib._SIGNATURES) is called by name from a test that runs on the GPU, or is
-listed below with the test that covers it. A new entry point without a kernel test then fails here, on any machine."""
+"""Every C entry point the Python side binds (every function of include/vilbert_b200.h: vilbert_b200._lib.FUNCTIONS) is called by
+name from a test that runs on the GPU, or is listed below with the test that covers it. A new entry point without a kernel test
+then fails here, on any machine."""
 import glob
 import os
 import re
@@ -16,6 +17,7 @@ COVERED_ELSEWHERE = {
     "vb_adamw_step_clipped": "tests/test_clip_gpu.py: FusedAdamW(max_grad_norm=...) steps against the clipped float64 oracle",
     "vb_radam_step_clipped": "tests/test_clip_gpu.py: FusedRAdam(max_grad_norm=...) steps against the clipped float64 oracle",
     "vb_gemm_plan": "tests/test_host_cpu.py: host-only tile-plan query, no GPU work",
+    "vb_version": "tests/test_host_cpu.py: the ABI version the library reports, no GPU work",
 }
 
 
@@ -25,17 +27,17 @@ def _gpu_run_sources():
     return {os.path.basename(f): open(f).read() for f in files if os.path.exists(f)}
 
 
-def test_every_entry_point_has_a_gpu_test():
+def test_every_header_function_has_a_gpu_test():
     sources = _gpu_run_sources()
-    missing = [n for n in L._SIGNATURES
+    missing = [n for n in L.FUNCTIONS
                if n not in COVERED_ELSEWHERE and not any(re.search(rf"\b{n}\b", t) for t in sources.values())]
     assert not missing, f"entry points no GPU test calls: {missing}"
 
 
-def test_covered_elsewhere_is_current():
+def test_covered_elsewhere_names_header_functions():
     """Each listed entry point still exists, and the test file named for it exists and mentions it or the wrapper that calls it."""
     for name, where in COVERED_ELSEWHERE.items():
-        assert name in L._SIGNATURES, name
+        assert name in L.FUNCTIONS, name
         path = os.path.join(os.path.dirname(TESTS), where.split(":")[0])
         assert os.path.exists(path), (name, where)
         text = open(path).read()

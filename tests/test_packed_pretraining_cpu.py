@@ -142,12 +142,12 @@ def test_packed_plan_launches_the_padded_ops_at_packed_rows(vt, train):
     # scattered to the padded layout (and, with a backward, its padded gradient gathered back)
     fwd = [op for op in b.fwd if op[0] is not None]
     comp = [args for fn, args, _ in fwd if fn.__name__ == "vb_compact_rows_mapped"]
-    assert len(comp) == 1 and comp[0][2] == b.map_t.data_ptr() and comp[0][3] == rows_t
-    assert comp[0][4] == a.lm_c["cap"] == b.lm_c["cap"]      # the capacity of the padded token rows
+    assert len(comp) == 1 and comp[0].map == b.map_t.data_ptr() and comp[0].rows == rows_t
+    assert comp[0].cap == a.lm_c["cap"] == b.lm_c["cap"]      # the capacity of the padded token rows
     C_ = eng.cfg.v_target_size
-    unpack = [args for fn, args, _ in fwd if fn.__name__ == "vb_unpack_rows_f32" and args[6] == C_]
-    assert len(unpack) == 1 and unpack[0][1] == b.outputs["vision_prediction"].data_ptr()
-    gathers = [args for fn, args, _ in b.bwd if fn is not None and fn.__name__ == "vb_pack_rows_f32" and args[4] == C_]
+    unpack = [args for fn, args, _ in fwd if fn.__name__ == "vb_unpack_rows_f32" and args.cols == C_]
+    assert len(unpack) == 1 and unpack[0].dst == b.outputs["vision_prediction"].data_ptr()
+    gathers = [args for fn, args, _ in b.bwd if fn is not None and fn.__name__ == "vb_pack_rows_f32" and args.cols == C_]
     assert len(gathers) == (1 if train else 0)
     assert b.outputs["vision_prediction"].shape == a.outputs["vision_prediction"].shape == (B, NV, C_)
     assert b.loss_inputs["masked_lm_labels"].shape == a.loss_inputs["masked_lm_labels"].shape == (B * NT,)

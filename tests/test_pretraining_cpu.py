@@ -47,16 +47,15 @@ def test_three_slot_plan_structure(golden_dir, vt):
     assert plan.loss_grad.tolist() == [1.0, 1.0, 1.0]
     lm, cap, region, ns = f[-4:]
     assert [op[0].__name__ for op in (lm, cap, region, ns)] == ["vb_ce_loss", "vb_scatter_rows_f32", REGION_FN[vt], "vb_ce_loss"]
-    slot_arg = {"vb_ce_loss": 4, "vb_kl_masked_loss": 3, "vb_mse_masked_loss": 8, "vb_nce_region_loss": 10}
-    assert lm[1][4] == out.data_ptr() and cap[1][6] == out.data_ptr()      # the capacity check poisons the masked-LM slot
-    assert region[1][slot_arg[REGION_FN[vt]]] == out.data_ptr() + 4 and ns[1][4] == out.data_ptr() + 8
+    assert lm[1].loss == out.data_ptr() and cap[1].poison == out.data_ptr()      # the capacity check poisons the masked-LM slot
+    assert region[1].loss == out.data_ptr() + 4 and ns[1].loss == out.data_ptr() + 8
     b = _kernels(plan.bwd)
     assert [op[0].__name__ for op in b[:4]] == ["vb_scale_by_device", "vb_cast2d_f32_to_bf16", "vb_scale_by_device", "vb_scale_by_device"]
     lg = plan.loss_grad.data_ptr()
-    assert (b[0][1][3], b[2][1][3], b[3][1][3]) == (lg, lg + 4, lg + 8)
-    assert b[0][1][0] == plan.head_grad["linguisic_prediction"].data_ptr() and b[0][1][1] == plan.lm_c["dl32"].data_ptr()
-    assert b[1][1][2] == plan.lm_c["dl16"].data_ptr()
-    assert b[2][1][1] == plan.gout["vision_prediction"].data_ptr() and b[3][1][1] == plan.gout["seq_relationship_score"].data_ptr()
+    assert (b[0][1].scale, b[2][1].scale, b[3][1].scale) == (lg, lg + 4, lg + 8)
+    assert b[0][1].src == plan.head_grad["linguisic_prediction"].data_ptr() and b[0][1].dst == plan.lm_c["dl32"].data_ptr()
+    assert b[1][1].dst == plan.lm_c["dl16"].data_ptr()
+    assert b[2][1].dst == plan.gout["vision_prediction"].data_ptr() and b[3][1].dst == plan.gout["seq_relationship_score"].data_ptr()
     # the objective is computed in the forward only
     assert not {REGION_FN[vt], "vb_ce_loss"} & set(_names(plan.bwd))
 
@@ -67,8 +66,8 @@ def test_eval_plan_has_no_backward_and_writes_no_gradient(golden_dir, vt):
     plan = eng.plan(4, NT, NV, loss="pretraining", loss_in_forward=True)
     assert _names(plan.bwd) == [] and not plan.head_grad
     lm, cap, region, ns = _kernels(plan.fwd)[-4:]
-    assert lm[1][5] is None and lm[1][7] is None and ns[1][5] is None    # CE: no f32 / bf16 gradient
-    assert region[1][{0: 4, 1: 10, 2: 12}[vt]] is None
+    assert lm[1].dlogits_f32 is None and lm[1].dlogits_bf16 is None and ns[1].dlogits_f32 is None    # CE: no f32 / bf16 gradient
+    assert region[1].dscores_f32 is None
 
 
 def test_new_inputs_and_loss_grad_are_private(golden_dir):

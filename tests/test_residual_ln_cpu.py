@@ -32,11 +32,10 @@ def test_dense_res_ln_gemms_read_no_residual(golden_dir):
             gemm_out[g.out_f32] = g
     for i in adds:
         args = fwd[i][1]
-        d, x_out = args[0], args[4]
-        assert x_out == d                         # the sum is kept for the backward, over the dense output
-        g = gemm_out[d]
+        assert args.x_out == args.d               # the sum is kept for the backward, over the dense output
+        g = gemm_out[args.d]
         assert g.residual is None and g.bias is not None and g.dropout.step is None
-        assert args[3] is not None                # train mode: the hidden dropout moved along with the add
+        assert args.dropout is not None           # train mode: the hidden dropout moved along with the add
     # the only forward GEMM that still adds a residual is the image embedding's (+ the 5-wide location projection)
     res_fwd = [a[0]._obj for n, a in fwd if n == "vb_gemm_bf16" and a[0]._obj.residual is not None]
     assert [(g.M, g.N) for g in res_fwd] == [(4 * NV, c.v_hidden_size)]
@@ -58,4 +57,4 @@ def test_residual_gradients_go_to_the_layernorm_backward(golden_dir):
     assert sum(1 for g in res if g.residual != g.out_f32) == 2
     for n, args in bwd:
         if n == "vb_add_layernorm_bwd":
-            assert args[1] is not None and args[1] != args[0]
+            assert args.dy2 is not None and args.dy2 != args.dy

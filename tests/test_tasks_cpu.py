@@ -137,7 +137,7 @@ def test_task_plan_structure(golden_dir, kind, choices, Nv):
     assert plan.loss_grad.item() == 1.0 and plan.preds.dtype == torch.int64
     head = LOSS_HEADS[kind][0]
     scale = [op for op in plan.bwd if op[0] is not None][0]
-    assert scale[1][1] == plan.gout[head].data_ptr() and scale[1][0] == plan.head_grad[head].data_ptr()
+    assert scale[1].dst == plan.gout[head].data_ptr() and scale[1].src == plan.head_grad[head].data_ptr()
     ev = eng.plan(4, NT, Nv, loss=kind, choices=choices, score=True, loss_in_forward=True)
     assert ev is not plan and _names(ev.fwd)[-2:] == [loss_fn, "vb_task_score"] and _names(ev.bwd) == []
     if kind == "vlogit_mc":

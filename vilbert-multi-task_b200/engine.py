@@ -434,16 +434,17 @@ HeadLayout = namedtuple("HeadLayout", "name logits rows cols ld off ids width ke
 
 
 # deterministic plans (Plan(deterministic=True), DESIGN.md §4h): entry points whose float atomics make the summation order depend on
-# scheduling, and the workspace floats their _det twin (same arguments + a trailing workspace) needs, from the arguments of the launch.
+# scheduling, and the workspace floats their _det twin (same arguments + a trailing workspace) needs, from the arguments of the launch
+# (_lib.launch_args: named after the parameters of the default entry point).
 # vb_layernorm_bwd / vb_add_layernorm_bwd (Plan.ln_bwd) and the atomic GEMMs (Plan.gemm) are switched where they are emitted.
 DET_WORKSPACE = {
-    "vb_colsum": lambda X, bf16, ld, out, M, N: L.VB_DET_SLICES * N,
-    "vb_loc_proj_bwd": lambda dy, loc, dW, db, M, H: L.VB_DET_SLICES * 6 * H,
-    "vb_small_linear_bwd": lambda dy, x, ldx, W, dx, lddx, acc, dW, db, M, K, N, drop: L.VB_DET_SLICES * (N * K + N),
+    "vb_colsum": lambda a: L.VB_DET_SLICES * a.N,
+    "vb_loc_proj_bwd": lambda a: L.VB_DET_SLICES * 6 * a.H,
+    "vb_small_linear_bwd": lambda a: L.VB_DET_SLICES * (a.N * a.K + a.N),
     "vb_embed_text_bwd": None,
-    "vb_ce_loss": lambda *a: L.VB_DET_LOSS_SLICES,
-    "vb_kl_masked_loss": lambda *a: L.VB_DET_LOSS_SLICES,
-    "vb_bce_logits_loss": lambda *a: L.VB_DET_LOSS_SLICES,
+    "vb_ce_loss": lambda a: L.VB_DET_LOSS_SLICES,
+    "vb_kl_masked_loss": lambda a: L.VB_DET_LOSS_SLICES,
+    "vb_bce_logits_loss": lambda a: L.VB_DET_LOSS_SLICES,
 }
 # kernels of the single-stream baseline (BaseBertForVLTasks) with float atomics and no deterministic variant
 DET_MISSING_BASELINE = ("vb_concat_embed_ln_bwd", "vb_embed_text_bwd_padded")
@@ -451,11 +452,12 @@ DET_MISSING_BASELINE = ("vb_concat_embed_ln_bwd", "vb_embed_text_bwd_padded")
 N_STREAMS = 4
 
 # anomaly detection (Plan(anomaly=True), torch.autograd.set_detect_anomaly(True), DESIGN.md §4i): per entry point that runs in the
-# backward role, the gradient values one launch writes, read from the launch's own arguments (C values as emitted) as
-# (output name, pointer, rows, cols, ld in elements, VB_NAN_* dtype); a null pointer is an output the launch does not write. `p` is
-# the plan, for the extents no argument carries: the rows of a packed stream (_attn_rows), of a scattered-into buffer (_buf_rows)
-# and the ranges of parameter gradients (_param_numel). The workspaces of the row-wise _det kernels are not listed: a launch
-# writes only the slices it uses. An entry point emitted in the backward role without an entry fails when the plan is built.
+# backward role, the gradient values one launch writes, read by parameter name from the launch's own arguments (C values as
+# emitted, _lib.launch_args) as (output name, pointer, rows, cols, ld in elements, VB_NAN_* dtype); a null pointer is an output the
+# launch does not write. `p` is the plan, for the extents no argument carries: the rows of a packed stream (_attn_rows), of a
+# scattered-into buffer (_buf_rows) and the ranges of parameter gradients (_param_numel). A _det twin shares the entry of its
+# default entry point; the workspaces of the row-wise _det kernels are not listed: a launch writes only the slices it uses. An
+# entry point emitted in the backward role without an entry fails when the plan is built.
 _F32, _BF16 = L.VB_NAN_F32, L.VB_NAN_BF16
 
 
@@ -474,79 +476,69 @@ def _attn_bwd_outputs(p, a):
             ("dbias_q", x.dbias_q, 1, hd, hd, _F32), ("dbias_k", x.dbias_k, 1, hd, hd, _F32), ("dbias_v", x.dbias_v, 1, hd, hd, _F32)]
 
 
-def _ln_bwd_outputs(o):
-    """vb_layernorm_bwd (o = 0) and vb_add_layernorm_bwd / vb_layernorm_bwd_det (o = 1: the dy2 argument)."""
-    def f(p, a):
-        M, H, ld = a[15 + o], a[16 + o], a[9 + o]
-        return [("dx_f32", a[7 + o], M, H, ld, _F32), ("dx_bf16", a[8 + o], M, H, ld, _BF16), ("dgamma", a[12 + o], 1, H, H, _F32),
-                ("dbeta", a[13 + o], 1, H, H, _F32), ("dbias", a[14 + o], 1, H, H, _F32)]
-    return f
-
-
 def _vec(name, ptr, n, dt=_F32):
     return (name, ptr, 1, n, n, dt)
 
 
-def _tables(names, first):
-    """Embedding-table gradients at arguments first, first + 1, ...: whole parameter ranges."""
-    return lambda p, a: [_vec(n, a[first + i], p._param_numel(a[first + i])) for i, n in enumerate(names)]
+def _tables(*names):
+    """Embedding-table gradients: whole parameter ranges."""
+    return lambda p, a: [_vec(n, getattr(a, n), p._param_numel(getattr(a, n))) for n in names]
 
 
-_small_linear = lambda p, a: [("dx", a[4], a[9], a[10], a[5], _F32), _vec("dW", a[7], a[11] * a[10]), _vec("db", a[8], a[11])]
-_loc_proj = lambda p, a: [_vec("dW", a[2], 5 * a[5]), _vec("db", a[3], a[5])]
-_ce = lambda p, a: [("dlogits_f32", a[5], a[9], a[10], a[6], _F32), ("dlogits_bf16", a[7], a[9], a[10], a[8], _BF16)]
-_bce = lambda p, a: [("dlogits_f32", a[3], a[6], a[7], a[7], _F32), ("dlogits_bf16", a[4], a[6], a[7], a[5], _BF16)]
-_kl = lambda p, a: [("dscores_f32", a[4], a[7] * a[8], a[9], a[9], _F32), ("dscores_bf16", a[5], a[7] * a[8], a[9], a[6], _BF16)]
-_region_loss = lambda i: lambda p, a: [("dscores_f32", a[i], a[3 if i == 10 else 4] * a[4 if i == 10 else 5],
-                                         a[5 if i == 10 else 6], a[5 if i == 10 else 6], _F32)]
+_ln_bwd = lambda p, a: [("dx_f32", a.dx_f32, a.M, a.H, a.lddx, _F32), ("dx_bf16", a.dx_bf16, a.M, a.H, a.lddx, _BF16),
+                        _vec("dgamma", a.dgamma, a.H), _vec("dbeta", a.dbeta, a.H), _vec("dbias", a.dbias, a.H)]
+_region_loss = lambda p, a: [("dscores_f32", a.dscores_f32, a.B * a.Nv, a.D, a.D, _F32)]
+_scattered = lambda p, a: [("dst", a.dst, p._buf_rows[a.dst], a.cols, a.cols, _F32)]
 ANOMALY_OUTPUTS = {
     "vb_gemm_bf16": _gemm_outputs,
     "vb_attention_bwd": _attn_bwd_outputs,
-    "vb_layernorm_bwd": _ln_bwd_outputs(0),
-    "vb_add_layernorm_bwd": _ln_bwd_outputs(1),
-    "vb_layernorm_bwd_det": _ln_bwd_outputs(1),
-    "vb_colsum": lambda p, a: [_vec("out", a[3], a[5])],
-    "vb_colsum_det": lambda p, a: [_vec("out", a[3], a[5])],
-    "vb_reduce_slices": lambda p, a: [_vec("dst", a[4], a[3])],
-    "vb_memset_zero": lambda p, a: [_vec("ptr", a[0], a[1] // 4)],
-    "vb_axpy_f32": lambda p, a: [_vec("y", a[1], a[2])],
-    "vb_embed_text_bwd": _tables(("dword", "dpos", "dtype", "dtask"), 4),
-    "vb_embed_text_bwd_det": _tables(("dword", "dpos", "dtype", "dtask"), 4),
-    "vb_embed_text_bwd_padded": _tables(("dword", "dpos", "dtype"), 3),
-    "vb_loc_proj_bwd": _loc_proj,
-    "vb_loc_proj_bwd_det": _loc_proj,
-    "vb_loc_proj_dx": lambda p, a: [("dx", a[2], a[3], 5, 5, _F32)],
-    "vb_small_linear_bwd": _small_linear,
-    "vb_small_linear_bwd_det": _small_linear,
-    "vb_fuse_pooled_bwd": lambda p, a: [_vec("da", a[3], a[5]), _vec("db", a[4], a[5])],
-    "vb_relu_bwd": lambda p, a: [_vec("dx_bf16", a[2], a[4], _BF16), _vec("dx_f32", a[3], a[4])],
-    "vb_sum_strided": lambda p, a: [_vec("dst", a[1], a[3] * a[2])],
-    "vb_masked_mean_bwd": lambda p, a: [("dx", a[2], a[4] * a[5], a[6], a[6], _F32)],
-    "vb_gate_scale_bwd": lambda p, a: [("dqk", a[0], a[8] * a[9], a[10], a[1], _BF16), ("dz", a[6], a[8], a[10], a[10], _F32),
-                                       ("dz16", a[7], a[8], a[10], a[10], _BF16)],
-    "vb_scatter_rows_f32": lambda p, a: [("dst", a[1], p._buf_rows[a[1]], a[4], a[4], _F32)],
-    "vb_scatter_add_rows_f32": lambda p, a: [("dst", a[1], p._buf_rows[a[1]], a[4], a[4], _F32)],
-    "vb_pack_rows_f32": lambda p, a: [("dst", a[1], a[3], a[4], a[4], _F32)],
-    "vb_unpack_rows_f32": lambda p, a: [("dst", a[1], a[4] * a[5], a[6], a[6], _F32)],
+    "vb_layernorm_bwd": _ln_bwd,
+    "vb_add_layernorm_bwd": _ln_bwd,
+    "vb_colsum": lambda p, a: [_vec("out", a.out, a.N)],
+    "vb_reduce_slices": lambda p, a: [_vec("dst", a.dst, a.n)],
+    "vb_memset_zero": lambda p, a: [_vec("ptr", a.ptr, a.bytes // 4)],
+    "vb_axpy_f32": lambda p, a: [_vec("y", a.y, a.n)],
+    "vb_embed_text_bwd": _tables("dword", "dpos", "dtype", "dtask"),
+    "vb_embed_text_bwd_padded": _tables("dword", "dpos", "dtype"),
+    "vb_loc_proj_bwd": lambda p, a: [_vec("dW", a.dW, 5 * a.H), _vec("db", a.db, a.H)],
+    "vb_loc_proj_dx": lambda p, a: [("dx", a.dx, a.M, 5, 5, _F32)],
+    "vb_small_linear_bwd": lambda p, a: [("dx", a.dx, a.M, a.K, a.lddx, _F32), _vec("dW", a.dW, a.N * a.K), _vec("db", a.db, a.N)],
+    "vb_fuse_pooled_bwd": lambda p, a: [_vec("da", a.da, a.n), _vec("db", a.db, a.n)],
+    "vb_relu_bwd": lambda p, a: [_vec("dx_bf16", a.dx_bf16, a.n, _BF16), _vec("dx_f32", a.dx_f32, a.n)],
+    "vb_sum_strided": lambda p, a: [_vec("dst", a.dst, a.count_k * a.n)],
+    "vb_masked_mean_bwd": lambda p, a: [("dx", a.dx, a.B * a.N, a.H, a.H, _F32)],
+    "vb_gate_scale_bwd": lambda p, a: [("dqk", a.dqk, a.B * a.N, a.cols, a.ldd, _BF16), ("dz", a.dz, a.B, a.cols, a.cols, _F32),
+                                       ("dz16", a.dz16, a.B, a.cols, a.cols, _BF16)],
+    "vb_scatter_rows_f32": _scattered,
+    "vb_scatter_add_rows_f32": _scattered,
+    "vb_pack_rows_f32": lambda p, a: [("dst", a.dst, a.rows, a.cols, a.cols, _F32)],
+    "vb_unpack_rows_f32": lambda p, a: [("dst", a.dst, a.B * a.N, a.cols, a.cols, _F32)],
     "vb_zero_tail_rows": lambda p, a: [],      # zeros into the rows of no sample; the launch before it declared those buffers
-    "vb_cast2d_f32_to_bf16": lambda p, a: [("dst", a[2], a[4], a[5], a[3], _BF16)],
-    "vb_weight_norm_bwd": lambda p, a: [_vec("dg", a[4], 1), _vec("dv", a[5], a[3])],
-    "vb_tanh_bwd": lambda p, a: [("dx_bf16", a[2], a[4], a[5], a[5], _BF16), _vec("dbias", a[3], a[5])],
+    "vb_cast2d_f32_to_bf16": lambda p, a: [("dst", a.dst, a.rows, a.cols, a.ldd, _BF16)],
+    "vb_weight_norm_bwd": lambda p, a: [_vec("dg", a.dg, 1), _vec("dv", a.dv, a.n)],
+    "vb_tanh_bwd": lambda p, a: [("dx_bf16", a.dx_bf16, a.M, a.N, a.N, _BF16), _vec("dbias", a.dbias, a.N)],
     "vb_concat_embed_ln_bwd": lambda p, a: [
-        ("dxt", a[8], a[17] * a[18], a[20], a[20], _F32), ("dxv", a[9], a[17] * a[19], a[20], a[20], _F32),
-        ("dxv_bf16", a[10], a[17] * a[19], a[20], a[20], _BF16)] + [_vec(n, a[11 + i], a[20]) for i, n in enumerate(
-            ("dgamma_t", "dbeta_t", "dgamma_v", "dbeta_v", "dcol_v", "dcol_v2"))],
-    "vb_ce_loss": _ce,
-    "vb_ce_loss_det": _ce,
-    "vb_bce_logits_loss": _bce,
-    "vb_bce_logits_loss_det": _bce,
-    "vb_bce_gather_loss": lambda p, a: [("dlogits_f32", a[12], a[6], a[3], a[13], _F32), ("dlogits_bf16", a[14], a[6], a[3], a[15], _BF16)],
-    "vb_kl_masked_loss": _kl,
-    "vb_kl_masked_loss_det": _kl,
-    "vb_mse_masked_loss": _region_loss(10),
-    "vb_nce_region_loss": _region_loss(12),
-    "vb_scale_by_device": lambda p, a: [_vec("dst", a[1], a[2])],
+        ("dxt", a.dxt, a.B * a.Nt, a.H, a.H, _F32), ("dxv", a.dxv, a.B * a.Nv, a.H, a.H, _F32),
+        ("dxv_bf16", a.dxv_bf16, a.B * a.Nv, a.H, a.H, _BF16)] + [_vec(n, getattr(a, n), a.H) for n in (
+            "dgamma_t", "dbeta_t", "dgamma_v", "dbeta_v", "dcol_v", "dcol_v2")],
+    "vb_ce_loss": lambda p, a: [("dlogits_f32", a.dlogits_f32, a.rows, a.cols, a.ld_d32, _F32),
+                                ("dlogits_bf16", a.dlogits_bf16, a.rows, a.cols, a.ld_d16, _BF16)],
+    "vb_bce_logits_loss": lambda p, a: [("dlogits_f32", a.dlogits_f32, a.rows, a.cols, a.cols, _F32),
+                                        ("dlogits_bf16", a.dlogits_bf16, a.rows, a.cols, a.ld_dlogits_bf16, _BF16)],
+    "vb_bce_gather_loss": lambda p, a: [("dlogits_f32", a.dlogits_f32, a.rows, a.width, a.ld_d32, _F32),
+                                        ("dlogits_bf16", a.dlogits_bf16, a.rows, a.width, a.ld_d16, _BF16)],
+    "vb_kl_masked_loss": lambda p, a: [("dscores_f32", a.dscores_f32, a.B * a.Nv, a.C, a.C, _F32),
+                                       ("dscores_bf16", a.dscores_bf16, a.B * a.Nv, a.C, a.ld_d16, _BF16)],
+    "vb_mse_masked_loss": _region_loss,
+    "vb_nce_region_loss": _region_loss,
+    "vb_scale_by_device": lambda p, a: [_vec("dst", a.dst, a.n)],
 }
+# a _det twin takes its default entry point's parameters plus a trailing ws (vb_layernorm_bwd_det: those of vb_add_layernorm_bwd),
+# so it shares that entry point's entry
+ANOMALY_OUTPUTS.update({n: ANOMALY_OUTPUTS["vb_add_layernorm_bwd" if n == "vb_layernorm_bwd_det" else n[:-len("_det")]]
+                        for n in L.FUNCTIONS if n.endswith("_det")})
+
+
 # one checked region: its id (the index into Plan.nan_records) and where it comes from — the op (its index in Plan.fwd or Plan.bwd,
 # `section`), the op's entry point and stream, the output (its index among the op's checked outputs and its name) and the module path
 # of the block that emitted the op (a fused objective: its kind)
@@ -1078,9 +1070,9 @@ class Plan:
         plan launches the _det twin of an entry point of DET_WORKSPACE instead, with its workspace."""
         if self.det and fn.__name__ in DET_WORKSPACE:
             size = DET_WORKSPACE[fn.__name__]
-            fn = getattr(self.lib, fn.__name__ + "_det")
             if size is not None:
-                args = args + (self.det_ws(size(*args)),)
+                args = args + (self.det_ws(size(L.launch_args(fn, *args))),)
+            fn = getattr(self.lib, fn.__name__ + "_det")
         self.cur.append((fn, L.launch_args(fn, *args), self.sid if self.two_streams else 0))
         if self.anomaly and self._label is not None:
             self._pending.append((self.cur, len(self.cur) - 1, self._label))
@@ -2191,7 +2183,7 @@ class Plan:
             hb32 = self.buf((B // 2, 2 * Hb), F32)
             # re-emit LN with an fp32 output (cheap: B/2 rows)
             fwd_fn, fwd_args, fwd_sid = self.fwd[-1]
-            args = list(fwd_args); args[5] = L.arg(hb32); self.fwd[-1] = (fwd_fn, tuple(args), fwd_sid)
+            self.fwd[-1] = (fwd_fn, fwd_args._replace(y_f32=L.arg(hb32)), fwd_sid)
             hb.f32 = hb32
 
             def bin_bwd():
