@@ -467,7 +467,12 @@ vb_status vb_memset_zero(void* ptr, int64_t bytes, void* stream);
  *   vb_unpack_rows_f32     dst[b*N + i,:] = i < len[b] ? src[off[b] + i,:] : fill (per-region logits back to the padded layout)
  *   vb_scatter_add_rows_f32  dst[idx[r],:] += src[r,:] (distinct idx): the pooled rows' gradient into the packed sequence gradient
  *   vb_zero_tail_rows      rows [*first, rows) of a, b, c (each optional but a; row pitch ld_bytes, row_bytes per row, both multiples
- *                          of 16) set to zero: the rows of no sample that the attention kernels do not write */
+ *                          of 16) set to zero: the rows of no sample that the attention kernels do not write
+ *   vb_pack_segments       off, len and map of ONE stream from its 0/1 mask [B, N_in] (vb_pack_build's layout and clamp): the image
+ *                          stream of a packed retrieval plan's prefix, and its caption's text stream
+ *   vb_broadcast_segment_rows  a one-sample packed stream of L = len[0] valid rows (read on the device) repeated as `repeats`
+ *                          contiguous segments: dst row b * L + i (b < repeats) = src row i, every other of the `rows` rows zero;
+ *                          row_bytes a multiple of 16 (fp32 rows and each 16-bit operand copy, one launch per tensor) */
 vb_status vb_pack_build(const int64_t* text_mask, int32_t Nt_in, int32_t has_task, const int64_t* image_mask, int32_t Nv, int32_t B,
                         int32_t rows_t, int32_t rows_v, int32_t* off_t, int32_t* len_t, int32_t* map_t, int32_t* off_v, int32_t* len_v,
                         int32_t* map_v, void* stream);
@@ -478,6 +483,10 @@ vb_status vb_unpack_rows_f32(const float* src, float* dst, const int32_t* off, c
                              float fill, void* stream);
 vb_status vb_scatter_add_rows_f32(const float* src, float* dst, const int32_t* idx, int32_t rows, int32_t cols, void* stream);
 vb_status vb_zero_tail_rows(void* a, void* b, void* c, int64_t ld_bytes, int32_t row_bytes, const int32_t* first, int32_t rows, void* stream);
+vb_status vb_pack_segments(const int64_t* mask, int32_t N_in, int32_t has_task, int32_t B, int32_t rows, int32_t* off, int32_t* len,
+                           int32_t* map, void* stream);
+vb_status vb_broadcast_segment_rows(const void* src, void* dst, int32_t row_bytes, const int32_t* len, int32_t repeats, int32_t rows,
+                                    void* stream);
 
 /* Whether a pre-training batch can be packed, from its device-resident masks and labels in one launch (one CTA): text_mask /
  * lm_labels int64 [B, Nt], image_mask int64 [B, Nv], image_label int64 [B, Nv - 1] (regions 1 .. Nv - 1). A NULL mask is all

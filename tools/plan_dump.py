@@ -158,6 +158,21 @@ def packed_pretraining_cases(E):
     ]
 
 
+def packed_retrieval_cases(E):
+    """Packed retrieval plans (fast_mode and image_prefix with packed=(rows_t, rows_v), the score head alone): VILBertForVLTasks with
+    and without task tokens, the zero-shot pre-training model, recycled and deterministic. Listed after every case above, so that
+    the listing of a tree without them is a prefix of this one."""
+    rows = (20, 24)
+    kw = dict(outputs=("vil_logit",), fast_mode=True, image_prefix=True, packed=rows)
+    return [
+        ("packed_retrieval", {}, "vl", 4, kw),
+        ("packed_retrieval_task_tokens", dict(task_specific_tokens=True), "vl", 4, kw),
+        ("packed_retrieval_zero_shot", {}, "pretraining", 4, dict(kw, outputs=("seq_relationship_score",))),
+        ("packed_retrieval_recycled", dict(task_specific_tokens=True), "vl", 4, dict(kw, recycle=True)),
+        ("det_packed_retrieval_task_tokens", dict(task_specific_tokens=True), "vl", 4, dict(kw, deterministic=True)),
+    ]
+
+
 def deterministic_cases(O, E, base_labels):
     """The two-stream cases of every matrix above with deterministic=True (named det_...)."""
     every = (cases(O, E, base_labels) + input_grad_cases(O, E, base_labels) + packed_cases(E) + packed_pretraining_cases(E))
@@ -334,6 +349,11 @@ def main():
     if hasattr(E, "ANOMALY_OUTPUTS"):
         for prec in PRECISIONS:
             p, o = dump_cases(out, anomaly_cases(O, E, tiny_base["num_labels"]), prec, Engine, BertConfig, tiny, tiny_base)
+            n_plans, n_ops = n_plans + p, n_ops + o
+    # packed retrieval plans: listed last, so that the listing of a tree without them is a prefix of this one
+    if hasattr(E, "RETRIEVAL_SCORE_HEADS"):
+        for prec in PRECISIONS:
+            p, o = dump_cases(out, packed_retrieval_cases(E), prec, Engine, BertConfig, tiny, tiny_base)
             n_plans, n_ops = n_plans + p, n_ops + o
     text = "\n".join(out) + "\n"
     if a.out:

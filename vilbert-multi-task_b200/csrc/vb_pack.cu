@@ -50,6 +50,46 @@ __global__ void __launch_bounds__(PACK_THREADS) pack_build_kernel(const long lon
   }
 }
 
+// pack_build_kernel for one stream: the image stream of a retrieval chunk (built once per chunk, in the image prefix) or the text
+// stream of a caption (built per caption from its loaded mask). Same layout, same clamp.
+__global__ void __launch_bounds__(PACK_THREADS) pack_segments_kernel(const long long* __restrict__ mask, int N_in, int has_task, int B,
+                                                                     int rows, int* __restrict__ off, int* __restrict__ len,
+                                                                     int* __restrict__ map) {
+  pdl_entry();
+  const int N = N_in + has_task;
+  for (int b = threadIdx.x; b < B; b += PACK_THREADS) {
+    int n = 0;
+    for (int j = 0; j < N_in; ++j) n += mask[(long long)b * N_in + j] != 0;
+    len[b] = n + has_task;
+  }
+  for (int r = threadIdx.x; r < rows; r += PACK_THREADS) map[r] = -1;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int o = 0;
+    for (int b = 0; b < B; ++b) {
+      len[b] = min(len[b], rows - o); off[b] = o; o += len[b];
+    }
+    off[B] = o;
+  }
+  __syncthreads();
+  for (int b = 0; b < B; ++b)
+    for (int i = threadIdx.x; i < len[b]; i += PACK_THREADS) map[off[b] + i] = b * N + i;
+}
+
+// A one-sample packed stream of L = *len valid rows repeated as `repeats` contiguous segments: dst row r = b * L + i (b < repeats)
+// is src row i, every other row of the `rows` is zero. 16-byte units (c16 per row); L is read on the device, so the launch stays
+// graph-capturable while the caption length changes.
+__global__ void broadcast_segment_rows_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int c16, const int* __restrict__ len,
+                                              int repeats, int rows) {
+  pdl_entry();
+  const int L = max(*len, 1);
+  const long long n = (long long)rows * c16, stride = (long long)gridDim.x * blockDim.x;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += stride) {
+    const int r = (int)(e / c16), c = (int)(e % c16), b = r / L;
+    dst[e] = b < repeats ? __ldg(src + (long long)(r - b * L) * c16 + c) : make_uint4(0u, 0u, 0u, 0u);
+  }
+}
+
 // dst[r, :] = src[map[r], :] (0 where map[r] < 0), f32 rows of `cols`
 __global__ void pack_rows_f32_kernel(const float* __restrict__ src, float* __restrict__ dst, const int* __restrict__ map, int rows, int cols) {
   pdl_entry();
@@ -200,6 +240,24 @@ extern "C" vb_status vb_pack_build(const int64_t* text_mask, int32_t Nt_in, int3
              reinterpret_cast<const long long*>(text_mask), (int)Nt_in, (int)(has_task ? 1 : 0), reinterpret_cast<const long long*>(image_mask),
              (int)Nv, (int)B, (int)rows_t, (int)rows_v, off_t, len_t, map_t, off_v, len_v, map_v);
   return check_launch("vb_pack_build");
+}
+
+extern "C" vb_status vb_pack_segments(const int64_t* mask, int32_t N_in, int32_t has_task, int32_t B, int32_t rows, int32_t* off, int32_t* len,
+                                      int32_t* map, void* stream) {
+  if (B <= 0 || N_in <= 0 || rows <= 0 || !mask || !off || !len || !map) return set_error(VB_ERR_INVALID, "vb_pack_segments: bad arguments");
+  launch_pdl(pack_segments_kernel, dim3(1), dim3(PACK_THREADS), (size_t)0, static_cast<cudaStream_t>(stream),
+             reinterpret_cast<const long long*>(mask), (int)N_in, (int)(has_task ? 1 : 0), (int)B, (int)rows, off, len, map);
+  return check_launch("vb_pack_segments");
+}
+
+extern "C" vb_status vb_broadcast_segment_rows(const void* src, void* dst, int32_t row_bytes, const int32_t* len, int32_t repeats, int32_t rows,
+                                               void* stream) {
+  if (row_bytes <= 0 || (row_bytes & 15) || repeats <= 0 || rows <= 0 || !src || !dst || !len || !a16(src) || !a16(dst))
+    return set_error(VB_ERR_INVALID, "vb_broadcast_segment_rows: bad arguments (16-byte rows and bases)");
+  launch_pdl(broadcast_segment_rows_kernel, dim3(grid_for((long long)rows * (row_bytes / 16))), dim3(256), (size_t)0,
+             static_cast<cudaStream_t>(stream), static_cast<const uint4*>(src), static_cast<uint4*>(dst), (int)(row_bytes / 16), len,
+             (int)repeats, (int)rows);
+  return check_launch("vb_broadcast_segment_rows");
 }
 
 extern "C" vb_status vb_pack_rows_f32(const float* src, float* dst, const int32_t* map, int32_t rows, int32_t cols, void* stream) {

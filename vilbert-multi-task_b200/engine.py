@@ -45,6 +45,9 @@ INPUT_GRAD_NAMES = ("input_imgs", "image_loc")
 # layout. The prediction heads of pre-training are packed only inside the fused objective (loss="pretraining", loss_in_forward=True):
 # the masked-LM head compacts its labelled rows through the text row map, the region head scatters its rows to the padded layout
 PACKED_HEADS = ("vil_prediction", "vil_prediction_gqa", "vil_logit", "vil_binary_prediction", "vil_tri_prediction", "vision_logit")
+# the score head a packed retrieval plan (fast_mode and image_prefix) builds, per model kind: VILBertForVLTasks' vil_logit, the
+# pre-training model's alignment logits (zero-shot retrieval)
+RETRIEVAL_SCORE_HEADS = {"vl": "vil_logit", "pretraining": "seq_relationship_score"}
 # config options packed plans refuse: they reshape or export the padded streams
 PACK_REFUSED_CONFIG = ("in_batch_pairs", "fast_mode", "dynamic_attention", "visualization")
 # the value a masked region's logit takes in a packed plan: the reference's additive mask, which in fp32 is no further from it
@@ -514,6 +517,9 @@ ANOMALY_OUTPUTS = {
     "vb_pack_rows_f32": lambda p, a: [("dst", a.dst, a.rows, a.cols, a.cols, _F32)],
     "vb_unpack_rows_f32": lambda p, a: [("dst", a.dst, a.B * a.N, a.cols, a.cols, _F32)],
     "vb_zero_tail_rows": lambda p, a: [],      # zeros into the rows of no sample; the launch before it declared those buffers
+    # packed retrieval (forward-only plans): int32 segments, and copies of rows some earlier launch wrote
+    "vb_pack_segments": lambda p, a: [],
+    "vb_broadcast_segment_rows": lambda p, a: [],
     "vb_cast2d_f32_to_bf16": lambda p, a: [("dst", a.dst, a.rows, a.cols, a.ldd, _BF16)],
     "vb_weight_norm_bwd": lambda p, a: [_vec("dg", a.dg, 1), _vec("dv", a.dv, a.n)],
     "vb_tanh_bwd": lambda p, a: [("dx_bf16", a.dx_bf16, a.M, a.N, a.N, _BF16), _vec("dbias", a.dbias, a.N)],
@@ -862,16 +868,26 @@ class Plan:
         """packed=(rows_t, rows_v): the two streams hold the valid rows only (DESIGN.md §4g). Refused with the options that reshape
         or export the padded streams, with input gradients (they are padded tensors) and with heads that are not packed: the heads
         of VILBertForVLTasks among PACKED_HEADS (outputs=), or the three heads of BertForMultiModalPreTraining under the fused
-        objective with its losses in the forward (loss="pretraining", loss_in_forward=True, engine.lm_compact, all three heads)."""
+        objective with its losses in the forward (loss="pretraining", loss_in_forward=True, engine.lm_compact, all three heads).
+        Retrieval (fast_mode and image_prefix together, forward-only) packs with the score head alone (RETRIEVAL_SCORE_HEADS):
+        rows_t then counts the caption's rows after its broadcast to the B images."""
         rows_t, rows_v = self.packed
         if rows_t < 1 or rows_v < 1 or rows_t > self.B * self.Nt or rows_v > self.B * self.Nv:
             raise ValueError(f"packed={self.packed}: the rows of each stream must lie in [1, B * N] = [1, {self.B * self.Nt}], "
                              f"[1, {self.B * self.Nv}]")
-        bad = [n for n, on in (("in_batch_pairs", self.pairs), ("fast_mode", self.fast), ("dynamic_attention", self.dyn),
-                               ("visualization", self.viz), ("image_prefix", self.image_prefix), ("input_grads", bool(self.input_grads)))
+        retrieval = self.fast and self.image_prefix
+        bad = [n for n, on in (("in_batch_pairs", self.pairs), ("fast_mode", self.fast and not retrieval), ("dynamic_attention", self.dyn),
+                               ("visualization", self.viz), ("image_prefix", self.image_prefix and not retrieval),
+                               ("input_grads", bool(self.input_grads)))
                if on]
         if bad:
             raise NotImplementedError(f"packed plans do not support {', '.join(bad)}")
+        if retrieval:
+            head = RETRIEVAL_SCORE_HEADS.get(self.heads)
+            if head is None or outputs is None or frozenset(outputs) != {head} or self.loss_kind is not None or self.results:
+                raise NotImplementedError(f"packed retrieval plans build the score head alone: outputs=({head!r},), no objective, got "
+                                          f"{None if outputs is None else sorted(outputs)}")
+            return
         if self.heads == "pretraining":
             if not (self.loss_kind == "pretraining" and self.loss_in_forward and self.e.lm_compact and
                     (outputs is None or frozenset(outputs) == frozenset(PRETRAINING_HEAD_NAMES))):
@@ -1326,7 +1342,7 @@ class Plan:
         ts = [t for t in ts if t is not None]
         off = self.seg[stream][0]
         self.emit(self.lib.vb_zero_tail_rows, *ts, *([None] * (3 - len(ts))), ts[0].stride(0) * ts[0].element_size(),
-                  ts[0].shape[1] * ts[0].element_size(), off.data_ptr() + 4 * self.B, ts[0].shape[0])
+                  ts[0].shape[1] * ts[0].element_size(), off.data_ptr() + 4 * self.n_seg[stream], ts[0].shape[0])
 
     def ln_fwd(self, x, gamma, beta, M, H, want_f32=True, out_drop=None, res=None, in_drop=None):
         """-> (fp32 output or None, Operand output, mean, rstd). res: LayerNorm of dropout_in(x) + res instead (the residual add is
@@ -1646,8 +1662,22 @@ class Plan:
         return v2o, t2o
 
     def broadcast_text(self, t):
-        """FAST_MODE: t [1*Nt, H] -> [B*Nt, H] (fp32 values and operand copies), and the text mask [1, Nt] -> [B, Nt]."""
+        """FAST_MODE: t [1*Nt, H] -> [B*Nt, H] (fp32 values and operand copies), and the text mask [1, Nt] -> [B, Nt]. Packed
+        (retrieval): the caption's L valid rows -> B contiguous segments (b*L, L) of the rows_t rows, zeros after B*L, with the B
+        segments written from the broadcast mask; L is read on the device."""
         B, M1, H = self.B, t.M, t.H
+        if self.packed:
+            rows, it = self.packed[0], torch.int32
+            seg = (self.buf((B + 1,), it), self.buf((B,), it))
+            self.map_t = self.buf((rows,), it)
+            self.emit(self.lib.vb_pack_segments, self.in_amask_b, self.Nt_in, 1 if self.has_task else 0, B, rows, *seg, self.map_t)
+            f32 = self.buf((rows, H), F32)
+            op = self.buf16((rows, H), bw=False)
+            for src, dst in ((t.f32, f32), (t.op.hi, op.hi), (t.op.lo, op.lo)):
+                if dst is not None:
+                    self.emit(self.lib.vb_broadcast_segment_rows, src, dst, H * dst.element_size(), self.seg["t"][1], B, rows)
+            self.seg["t"], self.n_seg["t"] = seg, B
+            return self.act(f32, op, rows, H, inputs=(t,))
         f32 = self.buf((B * M1, H), F32)
         op = self.buf16((B * M1, H), bw=False)      # FAST_MODE is inference only: no backward copy
         for src, dst in ((t.f32, f32), (t.op.hi, op.hi), (t.op.lo, op.lo)):
@@ -1706,7 +1736,7 @@ class Plan:
     def text_layer(self, x, i):
         p = f"bert.encoder.layer.{i}"
         c = self.cfg
-        h1 = self.self_attention_block(x, self.B if self.packed else x.M // self.Nt, self.Nt, c.num_attention_heads, self.mask_t, p + ".attention", "t",
+        h1 = self.self_attention_block(x, self.n_seg["t"] if self.packed else x.M // self.Nt, self.Nt, c.num_attention_heads, self.mask_t, p + ".attention", "t",
                                        p_attn=c.attention_probs_dropout_prob, p_hidden=c.hidden_dropout_prob)
         return self.ffn(h1, c.intermediate_size, p + ".intermediate.dense", p + ".output.dense", p + ".output.LayerNorm", "t.ffn",
                         drop=self.drop(p + ".output.dropout", c.hidden_dropout_prob, "t"))
@@ -1762,10 +1792,22 @@ class Plan:
             # so no additive mask exists)
             (Mt, Mv), self.mask_t, self.mask_v = self.packed, None, None
             it = torch.int32
-            self.seg = {"t": (self.buf((B + 1,), it), self.buf((B,), it)), "v": (self.buf((B + 1,), it), self.buf((B,), it))}
-            self.map_t, self.map_v = self.buf((Mt,), it), self.buf((Mv,), it)
-            self.emit(lib.vb_pack_build, self.in_amask, self.Nt_in, 1 if self.has_task else 0, self.in_imask, Nv, B, Mt, Mv, self.seg["t"][0],
-                      self.seg["t"][1], self.map_t, self.seg["v"][0], self.seg["v"][1], self.map_v)
+            self.n_seg = {"t": Bt, "v": B}       # samples of each stream (the text has one until broadcast_text)
+            if self.fast:
+                # retrieval: the caption is one segment of the Nt rows until broadcast_text; the image segments are written by the
+                # prefix into private buffers, so they outlive every caption forward like the image states
+                Mt = Nt
+                self.seg["t"], self.map_t = (self.buf((2,), it), self.buf((1,), it)), self.buf((Mt,), it)
+                self.emit(lib.vb_pack_segments, self.in_amask, self.Nt_in, 1 if self.has_task else 0, 1, Mt, *self.seg["t"], self.map_t)
+                self.seg["v"], self.map_v = (self.buf((B + 1,), it, zero=True), self.buf((B,), it, zero=True)), self.buf((Mv,), it, zero=True)
+                self.cur = self.prefix
+                self.emit(lib.vb_pack_segments, self.in_imask, Nv, 0, B, Mv, *self.seg["v"], self.map_v)
+                self.cur = self.fwd
+            else:
+                self.seg = {"t": (self.buf((B + 1,), it), self.buf((B,), it)), "v": (self.buf((B + 1,), it), self.buf((B,), it))}
+                self.map_t, self.map_v = self.buf((Mt,), it), self.buf((Mv,), it)
+                self.emit(lib.vb_pack_build, self.in_amask, self.Nt_in, 1 if self.has_task else 0, self.in_imask, Nv, B, Mt, Mv,
+                          self.seg["t"][0], self.seg["t"][1], self.map_t, self.seg["v"][0], self.seg["v"][1], self.map_v)
         else:
             self.mask_t = self.buf((Bt, Nt), F32)
             self.mask_v = self.buf((B, Nv), F32, zero=self.image_prefix)
@@ -1820,7 +1862,7 @@ class Plan:
             v = self.act(v32, vop, Mv, Hv, params=(ve + ".image_embeddings", ve + ".image_location_embeddings", ve + ".LayerNorm"),
                          rg=self.input_grads)
             if self.image_prefix:
-                self.image_states = (v32, vop.hi, vop.lo, self.mask_v)
+                self.image_states = (v32, vop.hi, vop.lo, self.mask_v) + ((*self.seg["v"], self.map_v) if self.packed else ())
 
             def bwd_image():
                 if v.gw:

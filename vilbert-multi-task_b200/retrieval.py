@@ -15,17 +15,21 @@ the half's region features to the device and embeds them again. Here the work ru
 is loaded and embedded once (Plan(image_prefix=True).run_image_prefix()), then every caption costs a few device-to-device copies
 from a caption bank uploaded once and one replay of a fast-mode forward (text batch 1 broadcast to the chunk) that builds only the
 score head. Scores stay on the device; vb_retrieval_rank ranks them there, and one read-back returns ranks and top-k lists.
+With pack=True (or engine.pack_padding) each pair runs on a plan that holds the chunk's valid regions and the caption's valid
+tokens only (retrieval_pack_plan, DESIGN.md §4e).
 
 Differences from the reference: equal scores are ordered by image index (the reference's default argsort leaves their order
 unspecified), and progress is logged once per chunk rather than after every caption (no caption has a full score row before the
 last chunk).
 """
 import logging
+from collections import OrderedDict
 
 import numpy as np
 import torch
 
 from . import _lib as L
+from .engine import pack_capacity
 
 logger = logging.getLogger(__name__)
 
@@ -85,6 +89,43 @@ def read_retrieval_dataset(dataset):
             torch.tensor(targets, dtype=torch.int64))
 
 
+def _row_lengths(mask):
+    """(valid entries per row, whether the row is prefix-valid and non-empty) of a 0/1 host mask [rows, N]."""
+    m = mask.ne(0)
+    n = m.sum(1)
+    return n, (n >= 1) & m.eq(torch.arange(m.size(1)).unsqueeze(0) < n.unsqueeze(1)).all(1)
+
+
+def retrieval_pack_plan(image_mask, caption_mask, chunk, has_task):
+    """The host decision of a packed retrieval evaluation from the gallery's and the captions' host masks ([G, Nv], [C, Nt]):
+    -> (chunks, fallback chunks, fallback captions). Each chunk is (first image, images n, rows_v, groups); groups maps the text
+    capacity rows_t of a packed plan to its captions, in ascending order, after the padded group (key None) if there is one.
+    A chunk packs its valid regions, rows_v = pack_capacity(valid regions, n * Nv); a caption of L valid rows (task token
+    included) is broadcast to the n images as n * L rows, rows_t = pack_capacity(n * L, n * Nt). A chunk with an image row that
+    is not prefix-valid or empty runs every caption padded (rows_v None); a caption whose mask is not prefix-valid runs padded on
+    every chunk."""
+    G, Nv = image_mask.shape
+    Nt = caption_mask.shape[1] + has_task
+    nv, ok_v = _row_lengths(image_mask)
+    nt, ok_t = _row_lengths(caption_mask)
+    lengths = (nt + has_task).tolist()
+    ok_t = ok_t.tolist()
+    chunks, bad_chunks = [], 0
+    for lo in range(0, G, chunk):
+        n = min(chunk, G - lo)
+        if not bool(ok_v[lo:lo + n].all()):
+            chunks.append((lo, n, None, {None: list(range(len(lengths)))}))
+            bad_chunks += 1
+            continue
+        cap = {L: pack_capacity(n * L, n * Nt) for L in set(lengths)}
+        groups = {}
+        for c, (L, ok) in enumerate(zip(lengths, ok_t)):
+            groups.setdefault(cap[L] if ok else None, []).append(c)
+        order = sorted(groups, key=lambda k: -1 if k is None else k)
+        chunks.append((lo, n, pack_capacity(int(nv[lo:lo + n].sum()), n * Nv), OrderedDict((k, groups[k]) for k in order)))
+    return chunks, bad_chunks, ok_t.count(False)
+
+
 class RetrievalEvaluator:
     """Scores captions against a fixed image gallery on fast-mode forward-only plans with a precomputed image prefix.
 
@@ -92,9 +133,14 @@ class RetrievalEvaluator:
     in eval mode. features f32 [G, Nv, 2048], spatials f32 [G, Nv, 5], image_mask [G, Nv], on the host (staged through pinned memory
     one chunk at a time) or on the model's device. Chunks of `chunk` images share one plan; a smaller last chunk gets its own.
     recycle: build the plans with their buffers placed by lifetime (Plan(recycle=True)), which holds a fraction of the bytes at the
-    same launches and scores; None takes engine.recycle_forward_only."""
+    same launches and scores; None takes engine.recycle_forward_only.
 
-    def __init__(self, model, features, spatials, image_mask, chunk=500, recycle=None):
+    pack: score each (caption, chunk) pair on a packed plan (Plan(packed=...), DESIGN.md §4g) that holds the chunk's valid regions and
+    the caption's valid tokens only; None follows engine.pack_padding. The decision is taken on the host from the masks
+    (retrieval_pack_plan): a chunk whose image mask is not prefix-valid or has an empty row, and a caption whose mask is not
+    prefix-valid, run on the padded plan and are counted in engine.pack_fallbacks["mask"]."""
+
+    def __init__(self, model, features, spatials, image_mask, chunk=500, recycle=None, pack=None):
         self.model = model
         heads = getattr(model, "_heads", None)
         if heads not in SCORE_HEAD:
@@ -115,10 +161,24 @@ class RetrievalEvaluator:
         self.heads = heads
         self.head = SCORE_HEAD[heads]
         self.recycle = recycle
+        self.pack = pack
 
-    def _plan(self, n, Nt):
+    def _plan(self, n, Nt, packed=None):
         return self.model.engine.plan(n, Nt, self.Nv, heads=self.heads, outputs=(self.head,), fast_mode=True, image_prefix=True,
-                                      recycle=self.recycle)
+                                      recycle=self.recycle, packed=packed)
+
+    def _chunks(self, input_mask, has_task):
+        """The chunks of a score() call as retrieval_pack_plan gives them; without packing every chunk has the padded group only.
+        Packing counts its fallbacks in engine.pack_fallbacks["mask"]. Masks already on the device are copied to the host once
+        here, never per caption."""
+        eng = self.model.engine
+        if not (self.pack if self.pack is not None else eng.pack_padding):
+            C = int(input_mask.shape[0])
+            return [(lo, min(self.chunk, self.G - lo), None, {None: range(C)}) for lo in range(0, self.G, self.chunk)]
+        chunks, bad_chunks, bad_captions = retrieval_pack_plan(self.image_mask.cpu(), input_mask.cpu(), self.chunk, int(has_task))
+        if bad_chunks + bad_captions:
+            eng.pack_fallbacks["mask"] += bad_chunks + bad_captions
+        return chunks
 
     def _load_chunk(self, plan, lo, n):
         dev = self.model.engine.device
@@ -145,6 +205,7 @@ class RetrievalEvaluator:
             raise ValueError("config.task_specific_tokens is set: task_id is required")
         dev = eng.device
         C, Nt = int(captions.shape[0]), int(captions.shape[1])
+        chunks = self._chunks(input_mask, has_task)
         # the caption bank: uploaded once, read row by row with device-to-device copies
         ids = captions.to(dev, torch.int64, non_blocking=True)
         mask = input_mask.to(dev, torch.int64, non_blocking=True)
@@ -152,22 +213,23 @@ class RetrievalEvaluator:
         task = torch.full((1, 1), _task_number(task_id), dtype=torch.int64, device=dev) if has_task else None
         scores = torch.empty((C, self.G), dtype=torch.float32, device=dev)
         model._sync_weights()
-        n_chunks = (self.G + self.chunk - 1) // self.chunk
-        for ci, lo in enumerate(range(0, self.G, self.chunk)):
-            n = min(self.chunk, self.G - lo)
-            plan = self._plan(n, Nt)
-            self._load_chunk(plan, lo, n)
-            out = plan.outputs[self.head]
-            for c in range(C):
-                plan.load_inputs(ids[c:c + 1], None, None, seg[c:c + 1], mask[c:c + 1], None, task)
-                if eng.auto_graph:
-                    plan.maybe_capture_passes(after=1)
-                plan.run_forward()
-                if self.heads == "vl":
-                    scores[c, lo:lo + n].copy_(out.view(-1))
-                else:
-                    scores[c, lo:lo + n].copy_(torch.softmax(out, dim=1)[:, 0])
-            logger.info("retrieval: chunk %d/%d (images %d-%d) scored against %d captions", ci + 1, n_chunks, lo, lo + n - 1, C)
+        # chunk outer, plan (padded, or one packed capacity of the captions) middle, caption inner: each plan embeds the chunk
+        # once in its prefix, and every caption lands at its own row
+        for ci, (lo, n, rows_v, groups) in enumerate(chunks):
+            for rows_t, group in groups.items():
+                plan = self._plan(n, Nt, None if rows_t is None else (rows_t, rows_v))
+                self._load_chunk(plan, lo, n)
+                out = plan.outputs[self.head]
+                for c in group:
+                    plan.load_inputs(ids[c:c + 1], None, None, seg[c:c + 1], mask[c:c + 1], None, task)
+                    if eng.auto_graph:
+                        plan.maybe_capture_passes(after=1)
+                    plan.run_forward()
+                    if self.heads == "vl":
+                        scores[c, lo:lo + n].copy_(out.view(-1))
+                    else:
+                        scores[c, lo:lo + n].copy_(torch.softmax(out, dim=1)[:, 0])
+            logger.info("retrieval: chunk %d/%d (images %d-%d) scored against %d captions", ci + 1, len(chunks), lo, lo + n - 1, C)
         return scores
 
     @staticmethod
@@ -188,15 +250,15 @@ class RetrievalEvaluator:
         return ranks, topk
 
 
-def evaluate_retrieval(model, dataset, task_id=None, chunk=500, k=20):
+def evaluate_retrieval(model, dataset, task_id=None, chunk=500, k=20, pack=None):
     """The loop of eval_retrieval.py:253-358 (and, with the pre-training model and task_id=None, of eval_coco_retrieval.py:336-412):
     (r1, r5, r10, medr, meanr, results), results being each caption's top-k image list (the reference dumps the top 20 into
     *_result.json). The dataset is read through the reference's item protocol (read_retrieval_dataset); metrics are taken over the
     captions evaluated, which with the reference's 5,000 x 1,000 sizes is exactly its number. Puts the model in eval mode, as the
-    reference loop does."""
+    reference loop does. pack: score on packed plans (RetrievalEvaluator); None follows model.engine.pack_padding."""
     model.eval()
     feats, spats, imask, caps, masks, segs, targets = read_retrieval_dataset(dataset)
-    ev = RetrievalEvaluator(model, feats, spats, imask, chunk=chunk)
+    ev = RetrievalEvaluator(model, feats, spats, imask, chunk=chunk, pack=pack)
     scores = ev.score(caps, masks, segs, task_id=task_id)
     ranks, topk = ev.rank(scores, targets, k=k)
     both = torch.cat((ranks.view(-1, 1), topk), dim=1).cpu()       # the one read-back
