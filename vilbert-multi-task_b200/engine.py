@@ -21,6 +21,7 @@ activations and weights exist only as tensor-core operands. Three operand precis
   "bf16"            every operand bf16 (round-1 arithmetic; kept for A/B measurements).
 """
 import bisect
+import dataclasses
 import math
 import warnings
 import zlib
@@ -659,9 +660,15 @@ def lifetime_layout(sections, spans, pinned):
     return offset, extent
 
 
-class Plan:
-    """Static execution plan for one input shape. `grad_outputs` names the outputs that will receive a
-    gradient in backward (dead branches are not emitted). `loss` fuses an objective of LOSS_HEADS into the plan: by default its
+@dataclasses.dataclass(frozen=True)
+class PlanSpec:
+    """A plan's shape, options and the engine values its build reads (head_dropout_prob, bwd_gemm_max_ctas, the streams as the plan
+    uses them), each in one normal form, so that one plan has exactly one spec: Engine.plan caches plans by it. PlanSpec.of makes it.
+
+    grad_outputs: the outputs that will receive a gradient in backward (dead branches are not emitted). heads: "vl" | "pretraining"
+    | "none" | the baseline's "base" | "base_none" (engine.ps.heads by default). train: nn.Dropout layers active (model.train()).
+
+    loss fuses an objective of LOSS_HEADS into the plan (vqa_loss=True is the round-1 spelling of loss="vqa"): by default its
     kernel starts the backward, writes its scalar to self.loss and writes d loss / d head into the head's output-gradient buffer
     (loss="vqa", the round-1 objective of task_utils.py:325-327, also writes the head's bf16 backward operand, so no cast runs).
     Its labels and targets are static plan inputs (self.loss_inputs); the objective, score and results of a task kind address
@@ -670,12 +677,13 @@ class Plan:
     Task objectives (TASK_KINDS) take three more options. loss_in_forward=True emits the objective at the END of the forward list
     (a forward-only plan yields the loss) and stores d loss / d head; the backward then starts with head gradient = stored gradient
     x self.loss_grad (a device scalar, 1 by default: what the caller's d(total)/d(loss) is copied into). score=True also emits the
-    on-device batch score of the kind (self.score, device f32 [1]; self.preds, the per-row argmax). `choices`: answer options of
-    logit_ce (default engine.loss_options) and multiple-choice ids per sample of vlogit_mc.
+    on-device batch score of the kind (self.score, device f32 [1]; self.preds, the per-row argmax). choices: answer options of
+    logit_ce (engine.loss_options by default) and multiple-choice ids per sample of vlogit_mc; None for every other objective.
 
     loss="pretraining" with loss_in_forward=True keeps the three pre-training losses apart: self.objective_out (device f32 [3]) holds
     masked_lm, masked_img and next_sentence, self.loss is None, and self.loss_grad (f32 [3]) scales each head gradient by its own
-    slot. A plan without grad_outputs computes the losses only and writes no gradient.
+    slot. A plan without grad_outputs computes the losses only and writes no gradient. pretraining: the engine and config values
+    its build reads (engine.lm_compact, engine.lm_capacity, config.visual_target, nce_negative_count), None for other plans.
 
     outputs: the heads (names of HEAD_NAMES) the plan builds; None builds all of them. A head not named gets no kernel, no buffer
     and no entry in self.outputs (the four BertModel outputs are always there); what a kept head reads (the fused pooled vector,
@@ -685,10 +693,10 @@ class Plan:
     With heads="pretraining", outputs= names heads of PRETRAINING_HEAD_NAMES: ("seq_relationship_score",) builds no masked-LM or
     region decoder.
 
-    fast_mode: text batch 1 broadcast to the image batch (None: config.fast_mode). image_prefix=True (forward-only plans): the image
-    embedding (feature cast, box projection, embedding GEMM, LayerNorm) and the additive image mask are emitted into self.prefix,
-    run by run_image_prefix() on what load_images() loaded, and write private buffers that no op of the forward writes; the forward
-    starts at the text embeddings and reads those image states as they are, so one image batch serves many text forwards.
+    fast_mode: text batch 1 broadcast to the image batch (config.fast_mode by default). image_prefix=True (forward-only plans): the
+    image embedding (feature cast, box projection, embedding GEMM, LayerNorm) and the additive image mask are emitted into
+    self.prefix, run by run_image_prefix() on what load_images() loaded, and write private buffers that no op of the forward writes;
+    the forward starts at the text embeddings and reads those image states as they are, so one image batch serves many text forwards.
 
     frozen: ParamStore entry names whose parameters take no gradient (requires_grad=False; the tied decoder is the word-embedding
     entry). While the forward is emitted every activation records whether it needs a gradient, as autograd does: it does when the
@@ -703,110 +711,254 @@ class Plan:
     grad_touch; self.input_grad maps each input whose gradient the backward writes to its buffer ([B*Nv, Fv] / [B*Nv, 5] fp32). An
     input behind a no_grad layer (fixed_v_layer > 0) gets no entry, as it gets no gradient in torch.
 
-    deterministic=True (torch.use_deterministic_algorithms(True), DESIGN.md §4h): every sum that float atomics would make
-    order-dependent goes through the _det variant of its kernel (per-block partials in a workspace of the plan, then one ordered
-    sum), the GEMM weight gradients that split K store their splits apart and add them in split order, and all launches go to one
-    stream, so no two kernels add into the same range concurrently. Two runs give bitwise identical results on the same GPU model
-    and build. self.det_ws_bytes: the workspace the plan allocated for it.
+    packed=(rows_t, rows_v): the two streams hold the valid rows only (DESIGN.md §4g). Refused with the options that reshape or
+    export the padded streams, with input gradients (they are padded tensors) and with heads that are not packed: the heads of
+    VILBertForVLTasks among PACKED_HEADS (outputs=), or the three heads of BertForMultiModalPreTraining under the fused objective
+    with its losses in the forward (loss="pretraining", loss_in_forward=True, engine.lm_compact, all three heads). Retrieval
+    (fast_mode and image_prefix together, forward-only) packs with the score head alone (RETRIEVAL_SCORE_HEADS): rows_t then counts
+    the caption's rows after its broadcast to the B images.
 
-    recycle=True (forward-only plans: no train mode, no grad_outputs, no input_grads; DESIGN.md §3): buffers whose lifetimes are
-    disjoint share bytes. The plan is built twice in the same order. The first build records every buffer request in host memory
-    that it does not fill (also under torch.use_deterministic_algorithms(True)); the vector clocks of its ops (happens_before_clocks) give each buffer its uses, and lifetime_layout
-    places them. The second build emits the same launches with each buffer at its place, in one region of the plan or, with the
-    shared arena, at the start of the arena (arena_bytes is the extent). Private buffers and the buffers the host reads after a run
-    (_host_reads) keep bytes of their own. self.held_bytes: arena extent + the plan's own device buffers.
+    deterministic=True (torch.use_deterministic_algorithms(True), DESIGN.md §4h; None reads torch's flag at the call): every sum
+    that float atomics would make order-dependent goes through the _det variant of its kernel (per-block partials in a workspace of
+    the plan, then one ordered sum), the GEMM weight gradients that split K store their splits apart and add them in split order,
+    and all launches go to one stream, so no two kernels add into the same range concurrently. Two runs give bitwise identical
+    results on the same GPU model and build. self.det_ws_bytes: the workspace the plan allocated for it. The single-stream
+    baseline has kernels without a deterministic variant: it raises RuntimeError, or with torch's warn_only=True warns and builds
+    the default plan.
 
-    anomaly=True (torch.autograd.set_detect_anomaly(True), DESIGN.md §4i): every op in the backward role — the backward list, the
-    head-gradient writes of a forward-placed objective, vb_scale_by_device — is tagged with the module path of the block that
-    emitted it, and after each block one vb_nan_check per stream the block used scans the gradients its ops wrote (ANOMALY_OUTPUTS)
-    on that stream. Region ids follow op-list order and the flag (reset at the start of every forward) keeps the least id that held
-    a NaN, so anomaly_report() names the first op whose outputs held one. Removing the checks and the reset leaves the unchecked
-    plan's launches. The checks only read."""
+    recycle=True (forward-only plans: no train mode, no grad_outputs, no input_grads; DESIGN.md §3; None takes
+    engine.recycle_forward_only for a forward-only plan): buffers whose lifetimes are disjoint share bytes. The plan is built twice
+    in the same order. The first build records every buffer request in host memory that it does not fill (also under
+    torch.use_deterministic_algorithms(True)); the vector clocks of its ops (happens_before_clocks) give each buffer its uses, and
+    lifetime_layout places them. The second build emits the same launches with each buffer at its place, in one region of the
+    plan or, with the shared arena, at the start of the arena (arena_bytes is the extent). Private buffers and the buffers the host
+    reads after a run (_host_reads) keep bytes of their own. self.held_bytes: arena extent + the plan's own device buffers.
 
-    def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
-                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-                 input_grads=frozenset(), packed=None, deterministic=False, recycle=False, anomaly=False, _recording=False):
-        self.recycle = bool(recycle)
-        self.anomaly = bool(anomaly)
-        if self.anomaly and self.recycle:
+    anomaly=True (torch.autograd.set_detect_anomaly(True), DESIGN.md §4i; None reads torch.is_anomaly_enabled() and
+    torch.is_anomaly_check_nan_enabled() at the call; a plan with no backward has nothing to check and is the unchecked plan):
+    every op in the backward role — the backward list, the head-gradient writes of a forward-placed objective, vb_scale_by_device —
+    is tagged with the module path of the block that emitted it, and after each block one vb_nan_check per stream the block used
+    scans the gradients its ops wrote (ANOMALY_OUTPUTS) on that stream. Region ids follow op-list order and the flag (reset at the
+    start of every forward) keeps the least id that held a NaN, so anomaly_report() names the first op whose outputs held one.
+    Removing the checks and the reset leaves the unchecked plan's launches. The checks only read."""
+    B: int
+    Nt: int
+    Nv: int
+    grad_outputs: frozenset
+    heads: str
+    train: bool
+    loss: str
+    choices: int
+    score: bool
+    loss_in_forward: bool
+    outputs: frozenset
+    results: str
+    fast_mode: bool
+    image_prefix: bool
+    frozen: frozenset
+    input_grads: frozenset
+    packed: tuple
+    deterministic: bool
+    recycle: bool
+    anomaly: bool
+    head_dropout_prob: float
+    bwd_gemm_max_ctas: int
+    two_streams: bool
+    wgrad_streams: bool
+    pretraining: tuple
+
+    @classmethod
+    def of(cls, engine, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
+           loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
+           input_grads=frozenset(), packed=None, deterministic=None, recycle=None, anomaly=None):
+        """The spec of the plan of `engine` with this shape and these options; raises what the options ask that no plan does."""
+        cfg, base = engine.cfg, engine.ps.base
+        grad_outputs, frozen, input_grads = frozenset(grad_outputs), frozenset(frozen), frozenset(input_grads)
+        outputs = None if outputs is None else frozenset(outputs)
+        packed = None if packed is None else (int(packed[0]), int(packed[1]))
+        train, score, loss_in_forward, image_prefix = bool(train), bool(score), bool(loss_in_forward), bool(image_prefix)
+        loss = "vqa" if vqa_loss else loss
+        backward = bool(grad_outputs or input_grads)
+        recycle = bool(engine.recycle_forward_only and not (train or backward) if recycle is None else recycle)
+        det = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
+        if anomaly is None:
+            anomaly = torch.is_anomaly_enabled() and torch.is_anomaly_check_nan_enabled()
+        anomaly = bool(anomaly) and backward
+        if det and base:
+            msg = (f"{' and '.join(DET_MISSING_BASELINE)} (the backward of BaseBertForVLTasks' embeddings) add with float atomics and "
+                   "have no deterministic implementation; build the plan without torch.use_deterministic_algorithms(True), or with "
+                   "warn_only=True to run the default kernels")
+            if not torch.is_deterministic_algorithms_warn_only_enabled():
+                raise RuntimeError(msg)
+            warnings.warn(msg)
+            det = False
+        if packed is not None and base:
+            raise NotImplementedError("packed plans run the two-stream VILBertForVLTasks only")
+        if base and (loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
+                     or loss_in_forward):
+            raise ValueError("single-stream baseline plans support grad_outputs, train, frozen, input_grads and recycle only")
+        if anomaly and recycle:
             raise ValueError("anomaly checks read the gradients of a backward: a recycled (forward-only) plan has none")
-        if self.recycle and (train or grad_outputs or input_grads):
+        if recycle and (train or backward):
             raise ValueError("recycle=True shares the bytes of buffers whose lifetimes are disjoint, which only a forward-only plan "
                              "has: no train mode, no grad_outputs, no input_grads (the backward reads the saved activations)")
+        unknown = sorted(n for n in frozen if n not in engine.ps.entries)
+        if unknown:
+            raise ValueError(f"frozen: {unknown[:4]} are not parameter entries of this model")
+        unknown = sorted(n for n in input_grads if n not in INPUT_GRAD_NAMES)
+        if unknown:
+            raise ValueError(f"input_grads: {unknown} are not among the differentiable inputs {INPUT_GRAD_NAMES}")
+
+        # the two-stream options (Plan._stream_modes); the baseline has none of them
+        pairs, viz, dyn = [not base and bool(getattr(cfg, f, False)) for f in ("in_batch_pairs", "visualization", "dynamic_attention")]
+        fast = not base and bool(getattr(cfg, "fast_mode", False) if fast_mode is None else fast_mode)
+        if viz and train:
+            raise ValueError("visualization exports the undropped attention probabilities: eval mode only")
+        if fast and (train or grad_outputs or loss):
+            raise ValueError("fast_mode is an inference path (text batch 1 broadcast to the image batch): no train mode / gradients")
+        if image_prefix and (train or grad_outputs):
+            raise ValueError("image_prefix keeps the image states across forwards: forward-only plans (no train mode, no grad_outputs)")
+        if image_prefix and pairs:
+            raise ValueError("image_prefix: in_batch_pairs re-expands the image batch inside the forward")
+        if input_grads and (fast or image_prefix):
+            raise ValueError("fast_mode and image_prefix plans are inference paths: no input gradients")
+
+        # the fused objective
+        if loss is not None and loss not in LOSS_HEADS:
+            raise ValueError(f"loss must be one of {sorted(LOSS_HEADS)}")
+        if (loss_in_forward or score) and loss not in TASK_KINDS and not (loss == "pretraining" and not score):
+            raise ValueError(f"loss_in_forward needs a task objective, one of {TASK_KINDS}, or 'pretraining'; score needs a task objective")
+        if score and loss not in SCORE_MODES:
+            raise ValueError(f"loss={loss!r} has no batch score: with int labels the reference's compute_score_with_logits "
+                             "raises (task_utils.py:618-623)")
+        if loss == "vlogit_mc" and not (choices and choices > 0):
+            raise ValueError("loss='vlogit_mc' needs choices= (multiple-choice ids per sample)")
+        if loss == "vlogit_mc" and Nv <= MC_REGION_OFFSET:
+            raise ValueError(f"loss='vlogit_mc' scores the regions after the first {MC_REGION_OFFSET}: Nv must exceed it")
+
+        # outputs= and results=: known head names, and every head the objective, a gradient or the results read is kept
+        heads = engine.ps.heads if heads is None else heads
+        if results is not None:
+            if results not in RESULT_MODES:
+                raise ValueError(f"results must be one of {sorted(RESULT_MODES)}, got {results!r}")
+            if loss is not None and (loss != results or not loss_in_forward):
+                raise ValueError(f"results={results!r} goes with loss=None or loss={results!r}, loss_in_forward=True (got loss={loss!r})")
+            if results not in ("vqa", "gqa") and loss != results:
+                raise ValueError(f"results={results!r} reads the inputs of its objective: build it with loss={results!r}, loss_in_forward=True")
+        if outputs is not None:
+            if heads == "pretraining" and all(n in HEAD_NAMES + PRETRAINING_HEAD_NAMES for n in outputs):
+                other = sorted(n for n in outputs if n not in PRETRAINING_HEAD_NAMES)
+                if other:
+                    raise ValueError(f"outputs: {other} are heads of VILBertForVLTasks (heads='vl'); the heads of heads='pretraining' are "
+                                     f"{PRETRAINING_HEAD_NAMES}")
+            else:
+                unknown = sorted(n for n in outputs if n not in HEAD_NAMES)
+                if unknown:
+                    raise ValueError(f"outputs: unknown head name(s) {unknown}; the heads are {HEAD_NAMES}")
+                if heads != "vl":
+                    raise ValueError(f"outputs= selects among the heads of VILBertForVLTasks (heads='vl') or of BertForMultiModalPreTraining "
+                                     f"(heads='pretraining'), not heads={heads!r}")
+            need = {n for n in grad_outputs if n in HEAD_NAMES + PRETRAINING_HEAD_NAMES}
+            if loss is not None:
+                need |= set(LOSS_HEADS[loss])
+            if results is not None:
+                need.add(RESULT_MODES[results][0])
+            missing = sorted(need - outputs)
+            if missing:
+                raise ValueError(f"outputs={sorted(outputs)} misses {missing}, which the plan's objective, gradients or results read")
+
+        # packed=: the rows of each stream at the batch and text length the streams run at
+        if packed is not None:
+            rows_t, rows_v = packed
+            Bs, Nts = B * B if pairs else B, Nt + (1 if cfg.task_specific_tokens else 0)
+            if rows_t < 1 or rows_v < 1 or rows_t > Bs * Nts or rows_v > Bs * Nv:
+                raise ValueError(f"packed={packed}: the rows of each stream must lie in [1, B * N] = [1, {Bs * Nts}], [1, {Bs * Nv}]")
+            retrieval = fast and image_prefix
+            bad = [n for n, on in (("in_batch_pairs", pairs), ("fast_mode", fast and not retrieval), ("dynamic_attention", dyn),
+                                   ("visualization", viz), ("image_prefix", image_prefix and not retrieval),
+                                   ("input_grads", bool(input_grads)))
+                   if on]
+            if bad:
+                raise NotImplementedError(f"packed plans do not support {', '.join(bad)}")
+            if retrieval:
+                head = RETRIEVAL_SCORE_HEADS.get(heads)
+                if head is None or outputs != {head} or loss is not None or results:
+                    raise NotImplementedError(f"packed retrieval plans build the score head alone: outputs=({head!r},), no objective, got "
+                                              f"{None if outputs is None else sorted(outputs)}")
+            elif heads == "pretraining":
+                if not (loss == "pretraining" and loss_in_forward and engine.lm_compact and
+                        (outputs is None or outputs == frozenset(PRETRAINING_HEAD_NAMES))):
+                    raise NotImplementedError("packed pre-training plans run the fused objective only: loss='pretraining', "
+                                              "loss_in_forward=True, engine.lm_compact and all three heads")
+            elif engine.ps.heads != "vl" or outputs is None or any(n not in PACKED_HEADS for n in outputs):
+                raise NotImplementedError(f"packed plans build heads of VILBertForVLTasks among {PACKED_HEADS} only (outputs=...), got "
+                                          f"{None if outputs is None else sorted(outputs)}")
+
+        # what the objective's head layout reads (_head_layout)
+        if loss is not None and not loss_in_forward:      # a forward-placed objective also serves forward-only (eval) plans
+            if any(n not in grad_outputs for n in LOSS_HEADS[loss]):
+                raise ValueError(f"loss={loss!r} differentiates {LOSS_HEADS[loss]}: add them to grad_outputs")
+        if loss == "logit_ce":        # vil_logit.view(B / options, options); results="logit_ce" goes with this loss
+            choices = choices or engine.loss_options
+            rows = B * B if pairs else B
+            if rows % choices:
+                raise ValueError(f"loss='logit_ce': batch {rows} is not a multiple of {choices} options")
+        else:
+            choices = int(choices) if loss == "vlogit_mc" else None
+        pre = (engine.lm_compact, engine.lm_capacity, cfg.visual_target, nce_negative_count(cfg)) if loss == "pretraining" else None
+        two = engine.two_streams and not det
+        return cls(B, Nt, Nv, grad_outputs, heads, train, loss, choices, score, loss_in_forward, outputs, results, fast, image_prefix,
+                   frozen, input_grads, packed, det, recycle, anomaly, engine.head_dropout_prob, engine.bwd_gemm_max_ctas, bool(two),
+                   bool(engine.wgrad_streams and two), pre)
+
+
+class Plan:
+    """Static execution plan of one PlanSpec, which documents its options."""
+
+    def __init__(self, engine, spec, _recording=False):
+        self.spec = spec
+        self.recycle, self.anomaly = spec.recycle, spec.anomaly
         self._requests = [] if _recording else None     # recording build: (tensor, bytes, private) per buffer request
         self._place, self._n_req, self._region = None, 0, None
-        if self.recycle:
+        if self.recycle and not _recording:
             # the recording build's buffers are address ranges only: torch.use_deterministic_algorithms(True) would fill each
             # torch.empty with NaN, writing host memory as large as the plain plan
             fill = torch.utils.deterministic.fill_uninitialized_memory
             torch.utils.deterministic.fill_uninitialized_memory = False
             try:
-                rec = Plan.__new__(type(self))
-                Plan.__init__(rec, engine, B, Nt, Nv, grad_outputs, heads, train, loss, choices, score, loss_in_forward, outputs,
-                              results, fast_mode, image_prefix, frozen, input_grads, packed, deterministic, _recording=True)
+                rec = type(self)(engine, spec, _recording=True)
             finally:
                 torch.utils.deterministic.fill_uninitialized_memory = fill
             self._place = rec._lifetime_placement()
         self.e, self.cfg = engine, engine.cfg
-        self.det = bool(deterministic)
+        self.det, self.packed, self.frozen, self.input_grads = spec.deterministic, spec.packed, spec.frozen, spec.input_grads
+        self.train, self.heads, self.keep, self.fast, self.image_prefix = spec.train, spec.heads, spec.outputs, spec.fast_mode, spec.image_prefix
+        # objective fused into the step (LOSS_HEADS): its scalar lands in self.loss (device) and its gradient goes straight into the
+        # backward of the head(s) it reads
+        self.grad_outputs, self.loss_kind, self.choices, self.results = spec.grad_outputs, spec.loss, spec.choices, spec.results
+        self.loss_in_forward, self.want_score = spec.loss_in_forward, spec.score
+        self.head_dropout_prob, self.two_streams, self.wgrad_streams = spec.head_dropout_prob, spec.two_streams, spec.wgrad_streams
         self._det_ws, self.det_ws_bytes = None, 0
         self._det_bias = []      # deterministic plans: attention bias sums (bias, d(Q|K|V), pitch) left to det_bias_sums
-        self.packed = None if packed is None else (int(packed[0]), int(packed[1]))
-        self.frozen = frozenset(frozen)
-        unknown = sorted(n for n in self.frozen if n not in engine.ps.entries)
-        if unknown:
-            raise ValueError(f"frozen: {unknown[:4]} are not parameter entries of this model")
-        self.input_grads = frozenset(input_grads)
-        unknown = sorted(n for n in self.input_grads if n not in INPUT_GRAD_NAMES)
-        if unknown:
-            raise ValueError(f"input_grads: {unknown} are not among the differentiable inputs {INPUT_GRAD_NAMES}")
         self.input_grad = {}          # input name -> the buffer its gradient lands in (written by the backward)
         self.out_rg = {}              # output name -> it carries a gradient (some trainable parameter lies upstream of it)
         self.grad_touch = {}           # (flat offset, numel) -> index of the last backward op writing that gradient range
         self.ps = engine.ps
         self.lib = L.lib()
         self.dev = engine.device
-        self.Bin = B
-        self._stream_modes(B, Nt, Nv, train, grad_outputs, loss, fast_mode, image_prefix)
-        if self.input_grads and (self.fast or self.image_prefix):
-            raise ValueError("fast_mode and image_prefix plans are inference paths: no input gradients")
+        self.Bin = spec.B
+        self._stream_modes(spec.B, spec.Nt, spec.Nv)
         self.attn_t, self.attn_v, self.attn_c = [], [], []
         self.prefix = []         # image_prefix: the image embedding and mask, run by run_image_prefix()
         self._private = False    # while set, buf() allocates private buffers (the image states of image_prefix)
-        self.grad_outputs = frozenset(grad_outputs)
-        # objective fused into the step (LOSS_HEADS): its scalar lands in self.loss (device) and its gradient goes straight into the
-        # backward of the head(s) it reads
-        self.loss_kind = loss
-        if self.loss_kind is not None and self.loss_kind not in LOSS_HEADS:
-            raise ValueError(f"loss must be one of {sorted(LOSS_HEADS)}")
-        self.loss_in_forward, self.want_score, self.choices = bool(loss_in_forward), bool(score), choices
         self.task_objective = self.loss_in_forward or self.want_score     # the objective's scalars live in self.objective_out
-        if self.task_objective and self.loss_kind not in TASK_KINDS and not (self.loss_kind == "pretraining" and not self.want_score):
-            raise ValueError(f"loss_in_forward needs a task objective, one of {TASK_KINDS}, or 'pretraining'; score needs a task objective")
-        if self.want_score and self.loss_kind not in SCORE_MODES:
-            raise ValueError(f"loss={self.loss_kind!r} has no batch score: with int labels the reference's compute_score_with_logits "
-                             "raises (task_utils.py:618-623)")
-        if self.loss_kind == "vlogit_mc" and not (choices and choices > 0):
-            raise ValueError("loss='vlogit_mc' needs choices= (multiple-choice ids per sample)")
-        if self.loss_kind == "vlogit_mc" and Nv <= MC_REGION_OFFSET:
-            raise ValueError(f"loss='vlogit_mc' scores the regions after the first {MC_REGION_OFFSET}: Nv must exceed it")
-        self.train = bool(train)          # nn.Dropout layers active (model.train()); False = the reference's eval mode
         self.op_dtype, self.split = engine.op_dtype, engine.split   # format of the forward operands (activations, weights)
-        self.head_dropout_prob = engine.head_dropout_prob
-        self.heads = engine.ps.heads if heads is None else heads   # "vl" | "pretraining" | "none"
-        self.keep = None if outputs is None else frozenset(outputs)
-        self.results = results
-        self._check_outputs()
-        if self.packed is not None:
-            self._check_packed(outputs)
         self.fwd_id = 0
         self.fwd, self.bwd = [], []
         self.prologue = []       # optional per-step ops run before the forward (see enable_training_prologue)
         self.epilogue = []       # optional per-step ops run after the backward (the fused optimizer: enable_optimizer)
         self.cur = self.fwd
         self.sid = 0             # stream the next emitted op goes to: 0 = text/main stream, 1 = vision stream
-        self.two_streams = engine.two_streams and not self.det
-        self.wgrad_streams = engine.wgrad_streams and self.two_streams   # weight-gradient GEMMs off the critical chain
         self._streams = None
         self._n_events = 0
         self._scratch_epoch = 0
@@ -839,9 +991,8 @@ class Plan:
         if self._place is not None and self._n_req != len(self._place[0]):
             raise L.VBError(f"recycled plan: the second build made {self._n_req} buffer requests, the first {len(self._place[0])}")
 
-    def _stream_modes(self, B, Nt, Nv, train, grad_outputs, loss, fast_mode, image_prefix):
-        """Shapes and checks of the two-stream options: in_batch_pairs, the task token, visualization, dynamic_attention,
-        fast_mode and image_prefix."""
+    def _stream_modes(self, B, Nt, Nv):
+        """Shapes of the two-stream options: in_batch_pairs, the task token, visualization, dynamic_attention and fast_mode."""
         # in_batch_pairs (vilbert.py:1008-1040): at the first connection layer every (text i, image j) combination of the input
         # batch becomes one sample: the streams run at the input batch before it and at B^2 from there on
         self.pairs = bool(getattr(self.cfg, "in_batch_pairs", False))
@@ -851,86 +1002,8 @@ class Plan:
         # FAST_MODE (vilbert.py:1042-1053, eval_retrieval.py): one caption (text batch 1) against B images; inference only
         # config.visualization (vilbert.py:451-458, 610-617, 813-821): export attention probabilities, queries and keys per layer
         self.viz = bool(getattr(self.cfg, "visualization", False))
-        if self.viz and train:
-            raise ValueError("visualization exports the undropped attention probabilities: eval mode only")
         self.dyn = bool(getattr(self.cfg, "dynamic_attention", False))
-        self.fast = bool(getattr(self.cfg, "fast_mode", False)) if fast_mode is None else bool(fast_mode)
         self.Bt = 1 if self.fast else B
-        if self.fast and (train or grad_outputs or loss):
-            raise ValueError("fast_mode is an inference path (text batch 1 broadcast to the image batch): no train mode / gradients")
-        self.image_prefix = bool(image_prefix)
-        if self.image_prefix and (train or grad_outputs):
-            raise ValueError("image_prefix keeps the image states across forwards: forward-only plans (no train mode, no grad_outputs)")
-        if self.image_prefix and self.pairs:
-            raise ValueError("image_prefix: in_batch_pairs re-expands the image batch inside the forward")
-
-    def _check_packed(self, outputs):
-        """packed=(rows_t, rows_v): the two streams hold the valid rows only (DESIGN.md §4g). Refused with the options that reshape
-        or export the padded streams, with input gradients (they are padded tensors) and with heads that are not packed: the heads
-        of VILBertForVLTasks among PACKED_HEADS (outputs=), or the three heads of BertForMultiModalPreTraining under the fused
-        objective with its losses in the forward (loss="pretraining", loss_in_forward=True, engine.lm_compact, all three heads).
-        Retrieval (fast_mode and image_prefix together, forward-only) packs with the score head alone (RETRIEVAL_SCORE_HEADS):
-        rows_t then counts the caption's rows after its broadcast to the B images."""
-        rows_t, rows_v = self.packed
-        if rows_t < 1 or rows_v < 1 or rows_t > self.B * self.Nt or rows_v > self.B * self.Nv:
-            raise ValueError(f"packed={self.packed}: the rows of each stream must lie in [1, B * N] = [1, {self.B * self.Nt}], "
-                             f"[1, {self.B * self.Nv}]")
-        retrieval = self.fast and self.image_prefix
-        bad = [n for n, on in (("in_batch_pairs", self.pairs), ("fast_mode", self.fast and not retrieval), ("dynamic_attention", self.dyn),
-                               ("visualization", self.viz), ("image_prefix", self.image_prefix and not retrieval),
-                               ("input_grads", bool(self.input_grads)))
-               if on]
-        if bad:
-            raise NotImplementedError(f"packed plans do not support {', '.join(bad)}")
-        if retrieval:
-            head = RETRIEVAL_SCORE_HEADS.get(self.heads)
-            if head is None or outputs is None or frozenset(outputs) != {head} or self.loss_kind is not None or self.results:
-                raise NotImplementedError(f"packed retrieval plans build the score head alone: outputs=({head!r},), no objective, got "
-                                          f"{None if outputs is None else sorted(outputs)}")
-            return
-        if self.heads == "pretraining":
-            if not (self.loss_kind == "pretraining" and self.loss_in_forward and self.e.lm_compact and
-                    (outputs is None or frozenset(outputs) == frozenset(PRETRAINING_HEAD_NAMES))):
-                raise NotImplementedError("packed pre-training plans run the fused objective only: loss='pretraining', "
-                                          "loss_in_forward=True, engine.lm_compact and all three heads")
-            return
-        if (self.e.ps.heads != "vl") or outputs is None or any(n not in PACKED_HEADS for n in outputs):
-            raise NotImplementedError(f"packed plans build heads of VILBertForVLTasks among {PACKED_HEADS} only (outputs=...), got "
-                                      f"{None if outputs is None else sorted(outputs)}")
-
-    def _check_outputs(self):
-        """Build-time checks of outputs= and results=: known head names, and every head the objective, a gradient or the results
-        read is kept."""
-        k, r = self.loss_kind, self.results
-        if r is not None:
-            if r not in RESULT_MODES:
-                raise ValueError(f"results must be one of {sorted(RESULT_MODES)}, got {r!r}")
-            if k is not None and (k != r or not self.loss_in_forward):
-                raise ValueError(f"results={r!r} goes with loss=None or loss={r!r}, loss_in_forward=True (got loss={k!r})")
-            if r not in ("vqa", "gqa") and k != r:
-                raise ValueError(f"results={r!r} reads the inputs of its objective: build it with loss={r!r}, loss_in_forward=True")
-        if self.keep is None:
-            return
-        if self.heads == "pretraining" and all(n in HEAD_NAMES + PRETRAINING_HEAD_NAMES for n in self.keep):
-            other = sorted(n for n in self.keep if n not in PRETRAINING_HEAD_NAMES)
-            if other:
-                raise ValueError(f"outputs: {other} are heads of VILBertForVLTasks (heads='vl'); the heads of heads='pretraining' are "
-                                 f"{PRETRAINING_HEAD_NAMES}")
-        else:
-            unknown = sorted(n for n in self.keep if n not in HEAD_NAMES)
-            if unknown:
-                raise ValueError(f"outputs: unknown head name(s) {unknown}; the heads are {HEAD_NAMES}")
-            if self.heads != "vl":
-                raise ValueError(f"outputs= selects among the heads of VILBertForVLTasks (heads='vl') or of BertForMultiModalPreTraining "
-                                 f"(heads='pretraining'), not heads={self.heads!r}")
-        need = {n for n in self.grad_outputs if n in HEAD_NAMES + PRETRAINING_HEAD_NAMES}
-        if k is not None:
-            need |= set(LOSS_HEADS[k])
-        if r is not None:
-            need.add(RESULT_MODES[r][0])
-        missing = sorted(need - self.keep)
-        if missing:
-            raise ValueError(f"outputs={sorted(self.keep)} misses {missing}, which the plan's objective, gradients or results read")
 
     def want(self, name):
         """Whether the head `name` is built (outputs=)."""
@@ -1275,7 +1348,7 @@ class Plan:
         g.out_f32, g.ld_out_f32 = L.arg(out_f32), ld_of
         g.out_bf16, g.ld_out_bf16 = L.arg(out_bf16), ld_ob
         g.out_pre, g.ld_out_pre = L.arg(out_pre), ld_op
-        g.atomic_out, g.split_k, g.block_n, g.max_ctas = atomic, split_k, 0, (0 if fwd else self.e.bwd_gemm_max_ctas)
+        g.atomic_out, g.split_k, g.block_n, g.max_ctas = atomic, split_k, 0, (0 if fwd else self.spec.bwd_gemm_max_ctas)
         g.out_colsum = L.arg(None if self.det else out_colsum)
         if dropout is not None:
             g.dropout = dropout
@@ -2393,7 +2466,7 @@ class Plan:
         self.head_dl16 = {}     # head name -> the bf16 gradient operand the objective writes for big_head
         self.loss = self.score = self.preds = self.loss_grad = self.objective_out = self.results_out = None
         if r is not None:
-            opts = self.choices or self.e.loss_options
+            opts = self.choices
             rows = self.B // opts if r == "logit_ce" else self.B
             nval = {L.VB_RESULT_SOFTMAX: opts, L.VB_RESULT_GATHER: 1}.get(RESULT_MODES[r][1], 0)
             self.results_out = self.buf((8 + 8 * rows + 4 * rows * nval,), torch.uint8, zero=True)
@@ -2420,12 +2493,10 @@ class Plan:
         rows, cols = lg.shape[0], lg.shape[1]
         key = "labels" if k in ("logit_ce", "binary_ce", "tri_ce") else "target"
         if k == "logit_ce":       # vil_logit.view(B / options, options)
-            opts = self.choices or self.e.loss_options
-            if rows % opts:
-                raise ValueError(f"loss='logit_ce': batch {rows} is not a multiple of {opts} options")
+            opts = self.choices
             return HeadLayout(name, lg, rows // opts, opts, opts, 0, None, 0, key)
         if k == "vlogit_mc":      # vision_logit[:, 101:].gather(1, ids)
-            return HeadLayout(name, lg, rows, int(self.choices), cols, MC_REGION_OFFSET, "multiple_choice_ids", cols, key)
+            return HeadLayout(name, lg, rows, self.choices, cols, MC_REGION_OFFSET, "multiple_choice_ids", cols, key)
         return HeadLayout(name, lg, rows, cols, cols, 0, None, 0, key)
 
     def _emit_loss(self):
@@ -2434,9 +2505,6 @@ class Plan:
         (loss_in_forward: into a buffer of its own, _head_grad). Labels / targets are static plan inputs (self.loss_inputs), laid
         out as the head is (_head_layout)."""
         lib, k, li = self.lib, self.loss_kind, self.loss_inputs
-        missing = [n for n in LOSS_HEADS[k] if n not in self.grad_outputs]
-        if missing and not self.loss_in_forward:      # a forward-placed objective also serves forward-only (eval) plans
-            raise ValueError(f"loss={k!r} differentiates {LOSS_HEADS[k]}: add them to grad_outputs")
         if k == "pretraining":
             self._emit_pretraining_loss()
             return
@@ -3050,20 +3118,11 @@ class Plan:
 
 class BasePlan(Plan):
     """Plan of the single-stream baseline BaseBertForVLTasks (heads "base" / "base_none"; vilbert/basebert.py). It has none of the
-    two-stream options (batch pairs, task token, fast mode, gate, attention export), and its plans take grad_outputs, train and
-    frozen only: no fused objective, outputs= selection or image prefix."""
+    two-stream options (batch pairs, task token, fast mode, gate, attention export), and its plans take grad_outputs, train,
+    frozen, input_grads and recycle only: no fused objective, outputs= selection or image prefix (PlanSpec.of)."""
 
-    def __init__(self, engine, B, Nt, Nv, grad_outputs=(), heads=None, train=False, loss=None, choices=None, score=False,
-                 loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-                 input_grads=frozenset(), recycle=False, anomaly=False):
-        if (loss is not None or outputs is not None or results is not None or fast_mode or image_prefix or score
-                or loss_in_forward):
-            raise ValueError("single-stream baseline plans support grad_outputs, train, frozen, input_grads and recycle only")
-        super().__init__(engine, B, Nt, Nv, grad_outputs, heads=heads, train=train, choices=choices, frozen=frozen, input_grads=input_grads,
-                         recycle=recycle, anomaly=anomaly)
-
-    def _stream_modes(self, B, Nt, Nv, *_):
-        self.pairs = self.has_task = self.viz = self.dyn = self.fast = self.image_prefix = False
+    def _stream_modes(self, B, Nt, Nv):
+        self.pairs = self.has_task = self.viz = self.dyn = False
         self.B, self.Nt_in, self.Nt, self.Nv, self.Bt = B, Nt, Nt, Nv, B
 
     def _build(self):
@@ -3344,58 +3403,20 @@ class Engine:
         self.pack_fallbacks = Counter()
         self.plan_builds = Counter()
 
-    def plan(self, B, Nt, Nv, grad_outputs=(), vqa_loss=False, heads=None, train=False, loss=None, choices=None, score=False,
-             loss_in_forward=False, outputs=None, results=None, fast_mode=None, image_prefix=False, frozen=frozenset(),
-             input_grads=frozenset(), packed=None, deterministic=None, recycle=None, anomaly=None):
-        """The cached plan of this shape and these options (Plan). vqa_loss=True is the round-1 spelling of loss="vqa"; frozen:
-        ParamStore entry names that take no gradient; input_grads: the inputs of INPUT_GRAD_NAMES the backward also differentiates;
-        packed: (rows_t, rows_v) of a packed plan. deterministic: bitwise-reproducible kernels (Plan); None reads
-        torch.are_deterministic_algorithms_enabled() now. The single-stream baseline has kernels without a deterministic variant: it
-        raises RuntimeError, or with torch's warn_only=True warns and builds the default plan. recycle: buffers placed by lifetime
-        (Plan); None takes engine.recycle_forward_only for a forward-only plan and leaves any other plan as it is. anomaly: NaN checks
-        of the backward's gradients (Plan); None reads torch.is_anomaly_enabled() and torch.is_anomaly_check_nan_enabled() now. A plan
-        with no backward (no grad_outputs, no input_grads) has nothing to check and is the unchecked plan."""
-        frozen, input_grads = frozenset(frozen), frozenset(input_grads)
-        if recycle is None:
-            recycle = self.recycle_forward_only and not (train or grad_outputs or input_grads)
-        det = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
-        if anomaly is None:
-            anomaly = torch.is_anomaly_enabled() and torch.is_anomaly_check_nan_enabled()
-        anomaly = bool(anomaly) and bool(grad_outputs or input_grads)
-        if det and self.ps.base:
-            msg = (f"{' and '.join(DET_MISSING_BASELINE)} (the backward of BaseBertForVLTasks' embeddings) add with float atomics and "
-                   "have no deterministic implementation; build the plan without torch.use_deterministic_algorithms(True), or with "
-                   "warn_only=True to run the default kernels")
-            if not torch.is_deterministic_algorithms_warn_only_enabled():
-                raise RuntimeError(msg)
-            warnings.warn(msg)
-            det = False
-        loss = "vqa" if vqa_loss else loss
-        pre = (self.lm_compact, self.lm_capacity, self.cfg.visual_target, nce_negative_count(self.cfg)) if loss == "pretraining" else None
-        key = (B, Nt, Nv, frozenset(grad_outputs), loss, heads, bool(train), pre, choices, bool(score), bool(loss_in_forward),
-               None if outputs is None else frozenset(outputs), results, fast_mode, bool(image_prefix), frozen, input_grads,
-               None if packed is None else tuple(packed), det, bool(recycle), anomaly)
-        if key in self.plans:
-            self.plans.move_to_end(key)
-            return self.plans[key]
+    def plan(self, B, Nt, Nv, **options):
+        """The cached plan of this shape and these options (the arguments of PlanSpec.of, which resolves and checks them). A call
+        the spec refuses leaves the cache as it was."""
+        spec = PlanSpec.of(self, B, Nt, Nv, **options)
+        plan = self.plans.get(spec)
+        if plan is not None:
+            self.plans.move_to_end(spec)
+            return plan
         # packed task steps add up to two capacities per task shape: a 12-task mix then holds ~36 plans in steady state
         while len(self.plans) >= self.max_plans * (3 if self.pack_padding else 1):   # evict the least recently used plan
             self.plans.popitem(last=False)
-        if packed is not None and self.ps.base:
-            raise NotImplementedError("packed plans run the two-stream VILBertForVLTasks only")
-        extra = {} if packed is None else {"packed": packed}
-        if det:
-            extra["deterministic"] = True
-        if recycle:
-            extra["recycle"] = True
-        if anomaly:
-            extra["anomaly"] = True
-        self.plans[key] = (BasePlan if self.ps.base else Plan)(
-            self, B, Nt, Nv, grad_outputs, heads, train, loss=loss, choices=choices, score=score, loss_in_forward=loss_in_forward,
-            outputs=outputs, results=results, fast_mode=fast_mode, image_prefix=image_prefix, frozen=frozen, input_grads=input_grads,
-            **extra)
+        plan = self.plans[spec] = (BasePlan if self.ps.base else Plan)(self, spec)
         self.plan_builds[(B, Nt, Nv)] += 1
-        return self.plans[key]
+        return plan
 
     def enable_activation_arena(self, nbytes):
         """One activation arena shared by all plans built afterwards (12-in-1 training holds a plan per task shape, but runs one
