@@ -61,7 +61,7 @@ typedef struct vb_dropout {
 } vb_dropout;
 
 /* ABI version of this header (bumped on incompatible change). v3: vb_gemm_args has no CTA-pair field and no smem descriptor
- * overrides, and vb_gemm_plan returns (block_n, split_k). */
+ * overrides, and vb_gemm_plan returns (block_n, split_k). v4: vb_adamw_group carries one_minus_beta1 / one_minus_beta2. */
 int vb_version(void);
 /* Message for the last non-OK status returned on this thread ("" if none). */
 const char* vb_last_error(void);
@@ -504,7 +504,11 @@ vb_status vb_pack_summary(const int64_t* text_mask, const int64_t* image_mask, i
  * builds it (train_tasks.py:401-426: one param group per tensor with its own lr / weight_decay, correct_bias=False),
  * optimizer.step() + model.zero_grad() (train_tasks.py:550-551), and the engine's own weight-shadow cast:
  *   m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;  p -= step_size m / (sqrt(v) + eps);  p -= lr wd p   (decay after, on the new p)
- *   step_size = lr, or lr sqrt(1-b2^t)/(1-b1^t) when correct_bias (t = *step, a device int32 the caller advances)
+ *   step_size = lr, or lr sqrt(1-b2^t)/(1-b1^t) when correct_bias (t = max(*step, 1), a device int32 the caller advances;
+ *   a counter still at 0 steps like t = 1 instead of dividing by 1 - b1^0 = 0), formed in float64 and rounded to fp32 once
+ * The (1-b1), (1-b2) factors are the group's one_minus_beta1 / one_minus_beta2: fp32(1 - b) of the host's float64 b, as the
+ * reference's fp32 torch ops see `1.0 - beta2`. 1 - fp32(b) would differ: fp32(0.999) rounds 1 - b2 to 0.00099998713.
+ * The bias corrections and RAdam's rectification use b = 1 - one_minus_beta in float64 for the same reason.
  * p / g / m / v: flat f32 buffers with one layout. Work list: chunk c covers elements [chunk_start[c], +chunk_count[c]) of one
  * tensor (starts multiples of 4) and uses groups[chunk_group[c]] (a DEVICE array, rewritten by the host when a scheduler
  * changes an lr). g is multiplied by grad_scale on read (gradient accumulation / loss scaling) and zeroed when zero_grad.
@@ -513,6 +517,7 @@ vb_status vb_pack_summary(const int64_t* text_mask, const int64_t* image_mask, i
 typedef struct vb_adamw_group {
   float lr, beta1, beta2, eps, weight_decay;
   int32_t correct_bias;
+  float one_minus_beta1, one_minus_beta2;
 } vb_adamw_group;
 
 vb_status vb_adamw_step(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
@@ -528,7 +533,8 @@ vb_status vb_adamw_step(float* p, float* g, float* m, float* v, void* p16, void*
  *             = lr / (1-b1^t)  otherwise
  * N_sma and step_size are computed in float64 from the lr / b1 / b2 of groups[leader_group] and used for every tensor: the
  * reference caches them per step in one buffer shared by all groups, so the first tensor's group supplies them.
- * advance_step != 0: *step += 1 on `stream` first (one call = one capturable step). Other arguments as vb_adamw_step. */
+ * advance_step != 0: *step += 1 on `stream` first (one call = one capturable step); a call refused for its arguments leaves the
+ * counter alone. t = max(*step, 1). Other arguments as vb_adamw_step. */
 vb_status vb_radam_step(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
                         const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
                         const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step, float grad_scale,

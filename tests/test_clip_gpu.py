@@ -92,12 +92,11 @@ def test_norm_matches_float64_and_is_bitwise_reproducible(golden_dir, chunk, gra
 
 
 # ---------------------------------------------------------------------------------------------------- clipped steps
-@pytest.mark.parametrize("kind", ["adamw", "radam"])
-@pytest.mark.parametrize("ratio", [0.3, 3.0])
-def test_clipped_step_matches_torch_clip_then_fused_step(golden_dir, kind, ratio):
+def _clipped_step_case(golden_dir, kind, ratio):
     """FusedX(max_grad_norm=c) == clip_grad_norm_(c) over the trainable parameters followed by FusedX(), with c below (ratio 0.3:
     clipped) and above (3.0: coefficient 1) the norm, over four steps with the reference grouping; both match the float64
-    restatement."""
+    restatement, which takes the betas as the Python floats the user passes (the kernels use fp32(1 - beta), as the reference's
+    fp32 torch ops do)."""
     model_a, _ = _tiny_model(golden_dir)
     model_b, _ = _tiny_model(golden_dir)
     _fill_grad(model_a.engine, 10)
@@ -109,7 +108,7 @@ def test_clipped_step_matches_torch_clip_then_fused_step(golden_dir, kind, ratio
     ref = [p.detach().clone().double() for _, p in named]
     mom = [(torch.zeros_like(r), torch.zeros_like(r)) for r in ref]
     ora = RO.RAdamOracle([dict(gr, params=[torch.nn.Parameter(r)], lr=_f32(gr["lr"])) for gr, r in zip(groups, ref)], lr=_f32(1e-3),
-                         betas=(_f32(0.9), _f32(0.999)), eps=_f32(1e-8)) if kind == "radam" else None
+                         betas=(0.9, 0.999), eps=_f32(1e-8)) if kind == "radam" else None
     for t in range(1, 5):
         for m in (model_a, model_b):
             _fill_grad(m.engine, 10 + t)
@@ -122,7 +121,7 @@ def test_clipped_step_matches_torch_clip_then_fused_step(golden_dir, kind, ratio
         cg = CO.clipped_grads(grads, c)
         if kind == "adamw":
             for r, (m1, m2), g, gr in zip(ref, mom, cg, groups):
-                AO.adamw_step(r, g, m1, m2, t, _f32(gr["lr"]), beta1=_f32(0.9), beta2=_f32(0.999), eps=_f32(1e-6),
+                AO.adamw_step(r, g, m1, m2, t, _f32(gr["lr"]), beta1=0.9, beta2=0.999, eps=_f32(1e-6),
                               weight_decay=_f32(gr["weight_decay"]), correct_bias=False)
         else:
             for grp, g in zip(ora.param_groups, cg):
@@ -134,6 +133,19 @@ def test_clipped_step_matches_torch_clip_then_fused_step(golden_dir, kind, ratio
         assert _rel(pa.detach(), r, 1e-6) < 2e-6, k
     ps = model_a.engine.ps
     assert torch.equal(ps.shadow, ps.flat.to(ps.op_dtype)) and model_a.engine.grad_clean and model_a.engine.shadow_clean
+
+
+@pytest.mark.parametrize("kind", ["radam"])
+@pytest.mark.parametrize("ratio", [0.3, 3.0])
+def test_clipped_step_matches_torch_clip_then_fused_step(golden_dir, kind, ratio):
+    _clipped_step_case(golden_dir, kind, ratio)
+
+
+@pytest.mark.parametrize("ratio", [0.3, 3.0])
+def test_clipped_adamw_step_matches_clip_then_step_with_python_betas(golden_dir, ratio):
+    """AdamW's float64 restatement with betas (0.9, 0.999), not their fp32 neighbours: with fp32 betas it would form
+    1 - fp32(0.999) = 0.00099998713 and sit 6e-6 relative off every update of a step from fresh moments."""
+    _clipped_step_case(golden_dir, "adamw", ratio)
 
 
 # ---------------------------------------------------------------------------------------------------- skipped steps

@@ -13,13 +13,14 @@ from vilbert_b200.config import BertConfig
 from vilbert_b200.engine import Engine, ParamStore
 
 
-def test_library_exports_every_header_function():
+def test_library_exports_every_header_function_at_abi_v4():
+    """v4: vb_adamw_group carries one_minus_beta1 / one_minus_beta2."""
     lib = L.lib()
     declared = L.exported_symbols()
     assert len(declared) >= 20
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/vilbert_b200.h but not exported"
-    assert lib.vb_version() == 3
+    assert lib.vb_version() == 4
     assert ctypes.sizeof(L.GemmArgs) >= 160 and ctypes.sizeof(L.AttnArgs) >= 150
 
 

@@ -11,11 +11,6 @@ TESTS = os.path.dirname(os.path.abspath(__file__))
 
 # entry points reached through a wrapper rather than by name: {name: "test that covers it and how"}
 COVERED_ELSEWHERE = {
-    "vb_adamw_step": "tests/test_optim.py: FusedAdamW.step against the AdamW oracle (oracle/adamw_oracle.py)",
-    "vb_radam_step": "tests/test_radam.py: FusedRAdam.step against the RAdam oracle (tests/_radam_oracle.py)",
-    "vb_grad_norm": "tests/test_clip_gpu.py: FusedAdamW / FusedRAdam with max_grad_norm, norm and skip record against float64",
-    "vb_adamw_step_clipped": "tests/test_clip_gpu.py: FusedAdamW(max_grad_norm=...) steps against the clipped float64 oracle",
-    "vb_radam_step_clipped": "tests/test_clip_gpu.py: FusedRAdam(max_grad_norm=...) steps against the clipped float64 oracle",
     "vb_gemm_plan": "tests/test_host_cpu.py: host-only tile-plan query, no GPU work",
     "vb_version": "tests/test_host_cpu.py: the ABI version the library reports, no GPU work",
 }

@@ -80,7 +80,8 @@ def test_fused_adamw_matches_oracle_over_steps(golden_dir, precision, correct_bi
         scale_ = max(ref[k].abs().max().item(), 1e-6)
         assert ((named[k].detach().double() - ref[k]).abs().max() / scale_).item() < 2e-6, k
         assert ((opt.state[named[k]]["exp_avg"].double() - mom[k][0]).abs().max() / max(mom[k][0].abs().max().item(), 1e-12)).item() < 1e-5, k
-        assert ((opt.state[named[k]]["exp_avg_sq"].double() - mom[k][1]).abs().max() / max(mom[k][1].abs().max().item(), 1e-12)).item() < 1e-4, k   # fp32 kernel vs float64 restatement
+        # fp32 kernel vs float64 restatement: a few roundings per step (1 - fp32(0.999) in place of fp32(1 - 0.999) is 1.3e-5)
+        assert ((opt.state[named[k]]["exp_avg_sq"].double() - mom[k][1]).abs().max() / max(mom[k][1].abs().max().item(), 1e-12)).item() < 2e-6, k
     # the 16-bit operand copy was produced by the same launch
     ps = eng.ps
     assert torch.equal(ps.shadow, ps.flat.to(ps.op_dtype)) and torch.equal(ps.shadow_b, ps.flat.to(torch.bfloat16))

@@ -141,14 +141,15 @@ def _rel(a, b, floor):
 
 
 def _f32(x):
-    """A hyper-parameter as the kernel's fp32 group table holds it (0.999 -> 0.99900001287...): the oracle computes in float64
-    from the same values, so the comparison measures the kernel's arithmetic, not the table's storage precision."""
+    """A learning rate as the kernel's fp32 group table holds it: the oracle computes in float64 from the same value, so the
+    comparison measures the kernel's arithmetic, not the table's storage precision. The betas stay the Python floats: the table
+    carries fp32(1 - beta) beside them, and the kernel's rectification and moments follow the Python values."""
     return float(np.float32(x))
 
 
 def _oracle_for(groups, params, lr):
     return RO.RAdamOracle([dict(g, params=[p], lr=_f32(g["lr"])) for g, p in zip(groups, params)], lr=_f32(lr),
-                          betas=(_f32(0.9), _f32(0.999)), eps=_f32(1e-8))
+                          betas=(0.9, 0.999), eps=1e-8)
 
 
 @pytest.mark.gpu
@@ -181,7 +182,7 @@ def test_fused_radam_matches_float64_oracle_over_steps(golden_dir, precision):
     for r, (k, p) in zip(ref, named):
         assert _rel(p.detach(), r.detach(), 1e-6) < 2e-6, k
         assert _rel(opt.state[p]["exp_avg"], ora.state[r]["exp_avg"], 1e-12) < 1e-5, k
-        assert _rel(opt.state[p]["exp_avg_sq"], ora.state[r]["exp_avg_sq"], 1e-12) < 1e-4, k
+        assert _rel(opt.state[p]["exp_avg_sq"], ora.state[r]["exp_avg_sq"], 1e-12) < 2e-6, k
     ps = eng.ps
     assert torch.equal(ps.shadow, ps.flat.to(ps.op_dtype)) and torch.equal(ps.shadow_b, ps.flat.to(torch.bfloat16))
     if precision == "fp32":
@@ -272,7 +273,7 @@ def test_checkpoint_round_trip_continues_like_an_uninterrupted_run(golden_dir, r
     ora = _oracle_for(groups_a, ref, 1e-3)
     ora.load_state_dict(ck["optimizer"])
     for g in ora.param_groups:
-        g["betas"], g["eps"] = (_f32(0.9), _f32(0.999)), _f32(1e-8)
+        g["betas"], g["eps"] = (0.9, 0.999), 1e-8
     flat = model_a.engine.ps.flat
     for t in range(resume_at + 1, total + 1):
         for g, b in zip(ora.param_groups, base):

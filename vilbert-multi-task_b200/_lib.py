@@ -81,7 +81,7 @@ class AdamWGroup(C.Structure):
     """Mirror of ``struct vb_adamw_group``."""
 
     _fields_ = [("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float), ("weight_decay", C.c_float),
-                ("correct_bias", C.c_int32)]
+                ("correct_bias", C.c_int32), ("one_minus_beta1", C.c_float), ("one_minus_beta2", C.c_float)]
 
 
 class NanRegion(C.Structure):

@@ -38,7 +38,7 @@ int sm_count() {
 }
 }  // namespace vb
 
-extern "C" int vb_version(void) { return 3; }
+extern "C" int vb_version(void) { return 4; }
 
 extern "C" const char* vb_last_error(void) { return vb::g_err; }
 

@@ -7,6 +7,10 @@
 // with step_size = lr (correct_bias False) or lr sqrt(1 - b2^t) / (1 - b1^t). The decoupled weight decay is applied
 // AFTER the Adam update and uses the updated p, like the reference.
 //
+// Hyper-parameters enter as the reference's fp32 torch ops see its Python floats: b and fp32(1 - b) as the moment factors
+// (the host forms 1 - b in float64: 1 - fp32(0.999) would be 0.00099998713, 1.3e-5 low), and the step sizes in float64
+// (fp32 1 - b2^t loses ~1e-5 to cancellation at small t, and fast-math powf adds its approximation on top).
+//
 // All parameters live in ONE flat fp32 buffer (engine.ParamStore), so the whole optimizer step is one HBM-bound
 // launch: per element read p, g, m, v (16 B), write p, m, v (12 B) + the 16-bit tensor-core operand copy of the new
 // weight (2 B, + 2 B low part in split precision) + the zeroed gradient (4 B). That removes the separate weight
@@ -151,6 +155,9 @@ __device__ __forceinline__ bool step_scale(const vb_clip_record* __restrict__ re
   return true;
 }
 
+// 1 - b^t in float64 for b = 1 - om, without the cancellation of forming b^t first.
+__device__ __forceinline__ double one_minus_pow(float om, double t) { return -expm1(t * log1p(-(double)om)); }
+
 __global__ void __launch_bounds__(OPT_THREADS)
 adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
              uint16_t* __restrict__ p16, uint16_t* __restrict__ p16_lo, __nv_bfloat16* __restrict__ p16_b, int fp16,
@@ -164,15 +171,16 @@ adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
     if (zero_grad) zero_chunks(g, chunk_start, chunk_count, n_chunks);
     return;
   }
-  const int t = step ? *step : 1;
+  // a counter still at 0 steps like t = 1 (the counter is advanced before the first step; 1 - b1^0 would divide by zero)
+  const double t = step ? (double)max(*step, 1) : 1.0;
   for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
     const long long s0 = chunk_start[c];
     const int n = chunk_count[c];
     const vb_adamw_group G = groups[chunk_group[c]];
-    float step_size = G.lr;
-    if (G.correct_bias) step_size = G.lr * sqrtf(1.f - powf(G.beta2, (float)t)) / (1.f - powf(G.beta1, (float)t));
+    const float step_size = G.correct_bias ? (float)((double)G.lr * sqrt(one_minus_pow(G.one_minus_beta2, t)) / one_minus_pow(G.one_minus_beta1, t))
+                                           : G.lr;
     const float decay = 1.f - G.lr * G.weight_decay;   // p <- p - lr wd p  (weight_decay > 0 only)
-    const float ob1 = 1.f - G.beta1, ob2 = 1.f - G.beta2;
+    const float ob1 = G.one_minus_beta1, ob2 = G.one_minus_beta2;
     auto upd = [&](float pv, float gv, float& mv, float& vv) -> float {
       gv *= gs;
       mv = G.beta1 * mv + ob1 * gv;
@@ -215,7 +223,8 @@ adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
 // The reference caches (N_sma, step_size) per step in one buffer shared by all param groups (optimization.py:59-86), so
 // within a step every tensor uses the values computed from the FIRST tensor's group: the lr, b1 and b2 of the leader group
 // `leader` drive the rectified step of all tensors. Both scalars are computed in float64 like the reference's Python floats:
-// in fp32, 1 - b2^t cancels (at b2 = 0.999 N_sma(6) comes out 6.0005 instead of 5.994).
+// in fp32, 1 - b2^t cancels (at b2 = 0.999 N_sma(6) comes out 6.0005 instead of 5.994). b = 1 - one_minus_beta, not the fp32 b:
+// 2 / (1 - fp32(0.999)) - 1 is N_sma_max = 1999.03 instead of 1999.
 __global__ void __launch_bounds__(OPT_THREADS)
 radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
              uint16_t* __restrict__ p16, uint16_t* __restrict__ p16_lo, __nv_bfloat16* __restrict__ p16_b, int fp16,
@@ -233,13 +242,13 @@ radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
   if (threadIdx.x == 0) {
     const vb_adamw_group L = groups[leader];
     const double t = (double)max(*step, 1);   // the counter is advanced before the first step; 0 would divide by zero
-    const double b1 = L.beta1, b2 = L.beta2, lr = L.lr;
-    const double b2t = pow(b2, t);
-    const double n_max = 2.0 / (1.0 - b2) - 1.0;
-    const double n_sma = n_max - 2.0 * t * b2t / (1.0 - b2t);
+    const double lr = L.lr, ob2 = L.one_minus_beta2;
+    const double obt1 = one_minus_pow(L.one_minus_beta1, t), obt2 = one_minus_pow(L.one_minus_beta2, t);   // 1 - b1^t, 1 - b2^t
+    const double n_max = 2.0 / ob2 - 1.0;
+    const double n_sma = n_max - 2.0 * t * (1.0 - obt2) / obt2;
     const int rect = n_sma >= 5.0;
-    const double ss = rect ? lr * sqrt((1.0 - b2t) * (n_sma - 4.0) / (n_max - 4.0) * (n_sma - 2.0) / n_sma * n_max / (n_max - 2.0)) / (1.0 - pow(b1, t))
-                           : lr / (1.0 - pow(b1, t));
+    const double ss = rect ? lr * sqrt(obt2 * (n_sma - 4.0) / (n_max - 4.0) * (n_sma - 2.0) / n_sma * n_max / (n_max - 2.0)) / obt1
+                           : lr / obt1;
     s_step_size = (float)ss;
     s_rect = rect;
   }
@@ -251,7 +260,7 @@ radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
     const int n = chunk_count[c];
     const vb_adamw_group G = groups[chunk_group[c]];
     const float decay = G.weight_decay * G.lr;
-    const float ob1 = 1.f - G.beta1, ob2 = 1.f - G.beta2;
+    const float ob1 = G.one_minus_beta1, ob2 = G.one_minus_beta2;
     auto upd = [&](float pv, float gv, float& mv, float& vv) -> float {
       gv *= gs;
       vv = G.beta2 * vv + ob2 * gv * gv;
@@ -320,15 +329,18 @@ static vb_status radam_launch(const char* name, float* p, float* g, float* m, fl
                               int32_t n_chunks, const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step,
                               float grad_scale, int32_t zero_grad, const vb_clip_record* rec, void* stream) {
   if (!step || leader_group < 0) return set_error(VB_ERR_INVALID, "%s: null step counter or negative leader group", name);
+  // every argument is checked before the counter moves: a refused call changes nothing
+  if (n_chunks > 0) {
+    if (!p || !g || !m || !v || !chunk_start || !chunk_count || !chunk_group || !groups)
+      return set_error(VB_ERR_INVALID, "%s: null argument", name);
+    if (!opt_buffers_aligned(p, g, m, v, p16, p16_lo, p16_b))
+      return set_error(VB_ERR_INVALID, "%s: buffers must be 16-byte aligned (16-bit copies 8-byte)", name);
+  }
   if (advance_step) {
     const vb_status st = vb_step_counter_bump(reinterpret_cast<uint32_t*>(step), stream);
     if (st != VB_OK) return st;
   }
   if (n_chunks <= 0) return VB_OK;
-  if (!p || !g || !m || !v || !chunk_start || !chunk_count || !chunk_group || !groups)
-    return set_error(VB_ERR_INVALID, "%s: null argument", name);
-  if (!opt_buffers_aligned(p, g, m, v, p16, p16_lo, p16_b))
-    return set_error(VB_ERR_INVALID, "%s: buffers must be 16-byte aligned (16-bit copies 8-byte)", name);
   cudaError_t e = launch_pdl(radam_kernel, dim3(opt_grid(n_chunks)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
                              static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),
                              reinterpret_cast<const long long*>(chunk_start), chunk_count, chunk_group, (int)n_chunks, groups, (int)leader_group,

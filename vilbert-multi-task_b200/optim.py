@@ -26,7 +26,15 @@ import torch
 
 from . import _lib as L
 
-_GROUP_DT = np.dtype([("lr", "<f4"), ("beta1", "<f4"), ("beta2", "<f4"), ("eps", "<f4"), ("weight_decay", "<f4"), ("correct_bias", "<i4")])
+_GROUP_DT = np.dtype([("lr", "<f4"), ("beta1", "<f4"), ("beta2", "<f4"), ("eps", "<f4"), ("weight_decay", "<f4"), ("correct_bias", "<i4"),
+                      ("one_minus_beta1", "<f4"), ("one_minus_beta2", "<f4")])
+
+
+def group_row(lr, betas, eps, weight_decay, correct_bias=False):
+    """The vb_adamw_group row of one param group. 1 - beta is formed here from the Python floats and rounded to fp32 once, as the
+    reference's fp32 torch ops see `1.0 - beta2`: the kernel forming 1 - fp32(beta2) instead would shrink every second-moment
+    increment by 1.3e-5 at beta2 = 0.999."""
+    return (lr, betas[0], betas[1], eps, weight_decay, 1 if correct_bias else 0, 1.0 - betas[0], 1.0 - betas[1])
 
 
 def build_chunks(ranges, chunk=32768):
@@ -141,7 +149,7 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
     # ------------------------------------------------------------------ hyper-parameter table
     def _group_row(self, grp):
         """The vb_adamw_group row of one param group."""
-        return (grp["lr"], grp["betas"][0], grp["betas"][1], grp["eps"], grp["weight_decay"], 0)
+        return group_row(grp["lr"], grp["betas"], grp["eps"], grp["weight_decay"])
 
     def _upload_groups(self):
         g = self._groups_np
@@ -226,7 +234,7 @@ class FusedAdamW(_FlatBufferOptimizer):
                          model, engine, zero_grad, chunk, max_grad_norm)
 
     def _group_row(self, grp):
-        return super()._group_row(grp)[:5] + (1 if grp["correct_bias"] else 0,)
+        return group_row(grp["lr"], grp["betas"], grp["eps"], grp["weight_decay"], grp["correct_bias"])
 
     # ------------------------------------------------------------------ stepping
     def launch(self, stream=None):
