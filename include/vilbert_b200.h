@@ -361,6 +361,18 @@ vb_status vb_task_results(int32_t mode, const float* logits, int64_t ld_logits, 
  * for the top-k; no atomics, results are deterministic. cols <= 50000, 1 <= k <= 64; otherwise VB_ERR_INVALID. */
 vb_status vb_retrieval_rank(const float* scores, int64_t ld_scores, int32_t rows, int32_t cols, const int64_t* target, int32_t k,
                             int32_t* rank_out, int32_t* topk_out, void* stream);
+/* vb_retrieval_rank_sets: image-to-text retrieval ranks, where a row has a set of targets (an image and its ground-truth
+ * captions). Row r of scores is ordered exactly as vb_retrieval_rank orders it; its targets are the columns
+ * set_idx[set_off[r] .. set_off[r+1]) (int64, CSR: set_off has rows + 1 entries).
+ *   rank_out[r] (int32)     the smallest position any target of the set takes in that order (its best-placed target); targets
+ *                           outside [0, cols) are ignored, and a set with no target inside gives -1
+ *   topk_out[r, 0..k) (int32, NULL: none)  as vb_retrieval_rank: the first min(k, cols) columns of the order, -1 after them
+ * The best-placed target is the one with the largest key, so the rank is one block-wide count as in vb_retrieval_rank (one
+ * kernel serves both). set_off and set_idx are read on the device only and are trusted: the offsets must index set_idx. A row
+ * whose offsets are negative or decreasing has an empty set. No atomics, results are deterministic. cols <= 50000,
+ * 1 <= k <= 64, set_off and set_idx not NULL; otherwise VB_ERR_INVALID, before any launch. */
+vb_status vb_retrieval_rank_sets(const float* scores, int64_t ld_scores, int32_t rows, int32_t cols, const int64_t* set_off,
+                                 const int64_t* set_idx, int32_t k, int32_t* rank_out, int32_t* topk_out, void* stream);
 /* dst = src * (*scale), f32, scale read on the device: the backward of a forward-placed objective starts from the stored
  * d loss / d head times d(total) / d loss (loss_scale[task] / gradient_accumulation_steps, train_tasks.py:247-251, 545-548)
  * without a host synchronisation. */

@@ -17,7 +17,7 @@ def __getattr__(name):
     if name in ("ForwardModelsTrain", "ForwardModelsVal", "LoadLosses"):
         from . import tasks
         return getattr(tasks, name)
-    if name in ("RetrievalEvaluator", "evaluate_retrieval", "retrieval_metrics"):
+    if name in ("RetrievalEvaluator", "evaluate_retrieval", "evaluate_retrieval_both", "retrieval_metrics", "i2t_metrics"):
         from . import retrieval
         return getattr(retrieval, name)
     if name in ("Engine", "Plan", "ParamStore"):

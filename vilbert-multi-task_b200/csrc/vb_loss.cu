@@ -423,7 +423,7 @@ task_results_kernel(int mode, const float* __restrict__ logits, long long ld, in
   for (int c = lane; c < cols; c += 32) out[c] = (float)(exp((double)(result_logit(zr, off, idr, width, c) - v)) * inv);
 }
 
-// ------------------------------------------------------------------------------------------ retrieval ranks (vb_retrieval_rank)
+// ------------------------------------------------------------------------------------------ retrieval ranks (vb_retrieval_rank[_sets])
 // Stable descending order of a score row as one 64-bit key per column, higher = earlier: the high word maps the float to an
 // unsigned integer that orders like the number (-0.0 folded onto +0.0, every NaN to 0, below -inf), the low word is ~column, so
 // equal scores keep the column order. Integer keys only: no float comparison, so --use_fast_math's flush-to-zero does not tie
@@ -458,11 +458,13 @@ __device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v
   return r;
 }
 
-// one CTA per row: the row's keys are staged in dynamic shared memory (4 bytes per column); the rank is one block-wide count of
-// the keys above the target's, the top-k k block-wide arg-max rounds, each bounded by the previous pick. No atomics.
+// one CTA per row: the row's keys are staged in dynamic shared memory (4 bytes per column). Row r's targets are
+// idx[off[r] .. off[r+1]), or idx[r] alone when off is NULL (vb_retrieval_rank). The best-placed target is the largest of their
+// keys, found with one block-wide max; the rank is one block-wide count of the keys above it, the top-k k block-wide arg-max
+// rounds, each bounded by the previous pick. No atomics.
 __global__ void __launch_bounds__(RANK_THREADS)
-retrieval_rank_kernel(const float* __restrict__ scores, long long ld, int N, const long long* __restrict__ target, int k,
-                      int* __restrict__ rank_out, int* __restrict__ topk_out) {
+retrieval_rank_kernel(const float* __restrict__ scores, long long ld, int N, const long long* __restrict__ off,
+                      const long long* __restrict__ idx, int k, int* __restrict__ rank_out, int* __restrict__ topk_out) {
   pdl_entry();
   extern __shared__ uint32_t keys[];
   __shared__ unsigned long long red64[RANK_THREADS / 32];
@@ -471,12 +473,21 @@ retrieval_rank_kernel(const float* __restrict__ scores, long long ld, int N, con
   const float* row = scores + (long long)r * ld;
   for (int j = threadIdx.x; j < N; j += RANK_THREADS) keys[j] = rank_key_hi(row[j]);
   __syncthreads();
-  const long long t = target[r];
-  int above = 0;
-  if (t >= 0 && t < N) {
-    const unsigned long long kt = rank_key(keys, (int)t);
-    for (int j = threadIdx.x; j < N; j += RANK_THREADS) above += rank_key(keys, j) > kt ? 1 : 0;
+  // 0 stands for "no target in [0, N)": every key is at least 2^31, its low word being ~column. A negative or decreasing range
+  // is empty, so it reads nothing before idx.
+  const long long lo = off ? off[r] : r, hi = off ? off[r + 1] : r + 1;
+  unsigned long long kt = 0ull;
+  for (long long i = (lo >= 0 ? lo : hi) + threadIdx.x; i < hi; i += RANK_THREADS) {
+    const long long t = idx[i];
+    if (t >= 0 && t < N) {
+      const unsigned long long x = rank_key(keys, (int)t);
+      kt = x > kt ? x : kt;
+    }
   }
+  kt = block_max_u64(kt, red64);
+  int above = 0;
+  if (kt)
+    for (int j = threadIdx.x; j < N; j += RANK_THREADS) above += rank_key(keys, j) > kt ? 1 : 0;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) above += __shfl_xor_sync(0xffffffffu, above, o);
   if ((threadIdx.x & 31) == 0) red32[threadIdx.x >> 5] = above;
@@ -484,7 +495,7 @@ retrieval_rank_kernel(const float* __restrict__ scores, long long ld, int N, con
   if (threadIdx.x == 0) {
     int s = 0;
     for (int w = 0; w < RANK_THREADS / 32; ++w) s += red32[w];
-    rank_out[r] = (t >= 0 && t < N) ? s : -1;
+    rank_out[r] = kt ? s : -1;
   }
   if (!topk_out) return;
   int* out = topk_out + (long long)r * k;
@@ -706,22 +717,35 @@ extern "C" vb_status vb_task_results(int32_t mode, const float* logits, int64_t 
   return check_launch("vb_task_results");
 }
 
-extern "C" vb_status vb_retrieval_rank(const float* scores, int64_t ld_scores, int32_t rows, int32_t cols, const int64_t* target, int32_t k,
-                                       int32_t* rank_out, int32_t* topk_out, void* stream) {
-  if (rows <= 0 || cols <= 0 || ld_scores < cols || !scores || !target || !rank_out || (topk_out && (k <= 0 || k > RANK_MAX_K)))
-    return set_error(VB_ERR_INVALID, "vb_retrieval_rank: bad arguments (rows %d, cols %d, ld %lld, k %d; 1 <= k <= %d)", (int)rows,
+// both retrieval entry points: every refusal comes before the launch, so a refused call writes nothing
+static vb_status retrieval_rank_launch(const char* name, const float* scores, int64_t ld_scores, int32_t rows, int32_t cols,
+                                       const int64_t* off, const int64_t* idx, int32_t k, int32_t* rank_out, int32_t* topk_out,
+                                       void* stream) {
+  if (rows <= 0 || cols <= 0 || ld_scores < cols || !scores || !idx || !rank_out || (topk_out && (k <= 0 || k > RANK_MAX_K)))
+    return set_error(VB_ERR_INVALID, "%s: bad arguments (rows %d, cols %d, ld %lld, k %d; 1 <= k <= %d)", name, (int)rows,
                      (int)cols, (long long)ld_scores, (int)k, RANK_MAX_K);
   if (cols > RANK_MAX_COLS)
-    return set_error(VB_ERR_INVALID, "vb_retrieval_rank: %d columns exceed the %d a row of shared memory holds", (int)cols, RANK_MAX_COLS);
+    return set_error(VB_ERR_INVALID, "%s: %d columns exceed the %d a row of shared memory holds", name, (int)cols, RANK_MAX_COLS);
   const size_t smem = (size_t)cols * sizeof(uint32_t);
   if (smem > 48 * 1024) {      // set per call, as the attention kernels do: it holds for the current device only
     cudaError_t e = cudaFuncSetAttribute(retrieval_rank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_retrieval_rank: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "%s: cudaFuncSetAttribute: %s", name, cudaGetErrorString(e));
   }
   launch_pdl(retrieval_rank_kernel, dim3(rows), dim3(RANK_THREADS), smem, static_cast<cudaStream_t>(stream), scores, (long long)ld_scores,
-             (int)cols, reinterpret_cast<const long long*>(target), (int)(topk_out ? k : 0), reinterpret_cast<int*>(rank_out),
-             reinterpret_cast<int*>(topk_out));
-  return check_launch("vb_retrieval_rank");
+             (int)cols, reinterpret_cast<const long long*>(off), reinterpret_cast<const long long*>(idx), (int)(topk_out ? k : 0),
+             reinterpret_cast<int*>(rank_out), reinterpret_cast<int*>(topk_out));
+  return check_launch(name);
+}
+
+extern "C" vb_status vb_retrieval_rank(const float* scores, int64_t ld_scores, int32_t rows, int32_t cols, const int64_t* target, int32_t k,
+                                       int32_t* rank_out, int32_t* topk_out, void* stream) {
+  return retrieval_rank_launch("vb_retrieval_rank", scores, ld_scores, rows, cols, nullptr, target, k, rank_out, topk_out, stream);
+}
+
+extern "C" vb_status vb_retrieval_rank_sets(const float* scores, int64_t ld_scores, int32_t rows, int32_t cols, const int64_t* set_off,
+                                            const int64_t* set_idx, int32_t k, int32_t* rank_out, int32_t* topk_out, void* stream) {
+  if (!set_off) return set_error(VB_ERR_INVALID, "vb_retrieval_rank_sets: set_off is NULL");
+  return retrieval_rank_launch("vb_retrieval_rank_sets", scores, ld_scores, rows, cols, set_off, set_idx, k, rank_out, topk_out, stream);
 }
 
 extern "C" vb_status vb_scale_by_device(const float* src, float* dst, int64_t n, const float* scale, void* stream) {

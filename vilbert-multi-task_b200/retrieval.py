@@ -10,6 +10,13 @@ TASK8 model) and of evaluation/eval_coco_retrieval.py:336-412 (zero-shot pre-tra
 
     r1, r5, r10, medr, meanr, results = evaluate_retrieval(model, dataset, task_id="TASK8")
 
+Image-to-text retrieval (text retrieval) from the same score matrix: each image's rank is that of its best-placed ground-truth
+caption (vb_retrieval_rank_sets), with the same tie and NaN order.
+
+    ranks_i, topk_i = ev.rank_captions(scores, target_image, k=20)              # device int32 [G], [G, k]
+    (r1, r5, r10, medr, meanr), n_without = i2t_metrics(ranks_i)
+    out = evaluate_retrieval_both(model, dataset, task_id="TASK8")             # {"t2i", "i2t", "rsum", "images_without_caption"}
+
 The reference scores every caption against the same gallery with one model call per caption and gallery half, so each call moves
 the half's region features to the device and embeds them again. Here the work runs chunk outer, caption inner: a chunk of images
 is loaded and embedded once (Plan(image_prefix=True).run_image_prefix()), then every caption costs a few device-to-device copies
@@ -36,8 +43,8 @@ logger = logging.getLogger(__name__)
 # the score head of each model kind (Engine heads): VILBertForVLTasks' vil_logit (eval_retrieval.py:299-310), the pre-training
 # model's alignment logits, scored as softmax(logits, 1)[:, 0] (eval_coco_retrieval.py:357-363)
 SCORE_HEAD = {"vl": "vil_logit", "pretraining": "seq_relationship_score"}
-MAX_TOPK = 64            # vb_retrieval_rank: k <= 64
-MAX_GALLERY = 50000      # ... and at most 50,000 images per row
+MAX_TOPK = 64            # vb_retrieval_rank[_sets]: k <= 64
+MAX_GALLERY = 50000      # ... and at most 50,000 columns per row (images, or captions for rank_captions)
 
 
 def retrieval_metrics(ranks):
@@ -249,6 +256,48 @@ class RetrievalEvaluator:
                stream=torch.cuda.current_stream(scores.device).cuda_stream)
         return ranks, topk
 
+    @staticmethod
+    def rank_captions(scores, target_image, k=20):
+        """Image-to-text ranks from the same score matrix: (ranks int32 [G], topk int32 [G, k]) on the device. ranks[g] is the
+        0-based position of image g's best-placed ground-truth caption (the captions c with target_image[c] == g) in the stable
+        descending order of column g of scores (ties by caption index, NaN last), -1 for an image without a caption; topk[g] is
+        the first k captions of that order (-1 past the last caption). k <= 64, at most 50,000 captions."""
+        if scores.dim() != 2 or scores.dtype != torch.float32 or not scores.is_cuda or scores.stride(1) != 1:
+            raise ValueError("scores: device f32 [C, G] with contiguous rows")
+        if not 1 <= int(k) <= MAX_TOPK:
+            raise ValueError(f"k = {k}: the device ranking returns 1 to {MAX_TOPK} entries per image")
+        C, G = scores.shape
+        target = torch.as_tensor(target_image).to(scores.device, torch.int64).reshape(-1)
+        if target.numel() != C:
+            raise ValueError(f"target_image: one per caption ({C}), got {target.numel()}")
+        set_off, set_idx = caption_sets(target, G)
+        by_image = scores.t().contiguous()                              # [G, C]: one row per image
+        ranks = torch.empty(G, dtype=torch.int32, device=scores.device)
+        topk = torch.empty((G, int(k)), dtype=torch.int32, device=scores.device)
+        L.call(L.lib().vb_retrieval_rank_sets, by_image, C, G, C, set_off, set_idx, int(k), ranks, topk,
+               stream=torch.cuda.current_stream(scores.device).cuda_stream)
+        return ranks, topk
+
+
+def caption_sets(target_image, G):
+    """Each image's ground-truth captions as CSR on target_image's device, with no host synchronisation: (set_off int64 [G + 1],
+    set_idx int64) with image g's captions, in ascending order, at set_idx[set_off[g]:set_off[g + 1]]. A caption whose target is
+    outside [0, G) belongs to no image; an image without a caption has an empty range."""
+    target = torch.as_tensor(target_image).to(torch.int64).reshape(-1)
+    sorted_target, set_idx = torch.sort(target, stable=True)
+    set_off = torch.searchsorted(sorted_target, torch.arange(G + 1, dtype=torch.int64, device=target.device))
+    return set_off, set_idx
+
+
+def i2t_metrics(ranks):
+    """((r1, r5, r10, medr, meanr), images without a caption) of image-to-text ranks (rank_captions): retrieval_metrics over the
+    images with at least one caption; an image without one (rank -1) is counted, not ranked."""
+    r = ranks.detach().cpu().numpy() if torch.is_tensor(ranks) else np.asarray(ranks)
+    ranked = r[r >= 0]
+    if len(ranked) == 0:
+        raise ValueError("i2t_metrics: no image has a caption")
+    return retrieval_metrics(ranked), int(len(r) - len(ranked))
+
 
 def evaluate_retrieval(model, dataset, task_id=None, chunk=500, k=20, pack=None):
     """The loop of eval_retrieval.py:253-358 (and, with the pre-training model and task_id=None, of eval_coco_retrieval.py:336-412):
@@ -265,3 +314,26 @@ def evaluate_retrieval(model, dataset, task_id=None, chunk=500, k=20, pack=None)
     r1, r5, r10, medr, meanr = retrieval_metrics(both[:, 0])
     logger.info("Final r1:%.3f, r5:%.3f, r10:%.3f, mder:%.3f, meanr:%.3f", r1, r5, r10, medr, meanr)
     return r1, r5, r10, medr, meanr, both[:, 1:1 + min(k, ev.G)].tolist()
+
+
+def evaluate_retrieval_both(model, dataset, task_id=None, chunk=500, k=20, pack=None):
+    """Both retrieval directions from one scoring pass, with the arguments of evaluate_retrieval:
+    {"t2i": (r1, r5, r10, medr, meanr, results), "i2t": (r1, r5, r10, medr, meanr, results), "rsum": float,
+    "images_without_caption": n}. t2i (caption-to-image, image retrieval) is what evaluate_retrieval returns. i2t (image-to-text,
+    text retrieval) ranks each image's best-placed ground-truth caption (rank_captions); its metrics are retrieval_metrics over the
+    images with at least one caption (i2t_metrics), and its results are every image's top-k caption list. rsum is the sum of both
+    directions' r1, r5 and r10. Both directions' ranks and top-k lists are read back in one copy."""
+    model.eval()
+    feats, spats, imask, caps, masks, segs, targets = read_retrieval_dataset(dataset)
+    ev = RetrievalEvaluator(model, feats, spats, imask, chunk=chunk, pack=pack)
+    scores = ev.score(caps, masks, segs, task_id=task_id)
+    C, G = scores.shape
+    ranks_t, topk_t = ev.rank(scores, targets, k=k)
+    ranks_i, topk_i = ev.rank_captions(scores, targets, k=k)
+    both = torch.cat((torch.cat((ranks_t.view(-1, 1), topk_t), 1), torch.cat((ranks_i.view(-1, 1), topk_i), 1))).cpu()
+    t2i = retrieval_metrics(both[:C, 0])
+    i2t, without = i2t_metrics(both[C:, 0])
+    logger.info("Final t2i r1:%.3f, r5:%.3f, r10:%.3f, mder:%.3f, meanr:%.3f", *t2i)
+    logger.info("Final i2t r1:%.3f, r5:%.3f, r10:%.3f, mder:%.3f, meanr:%.3f (%d images without a caption)", *i2t, without)
+    return {"t2i": (*t2i, both[:C, 1:1 + min(k, G)].tolist()), "i2t": (*i2t, both[C:, 1:1 + min(k, C)].tolist()),
+            "rsum": float(sum(t2i[:3]) + sum(i2t[:3])), "images_without_caption": without}
