@@ -25,6 +25,15 @@ score head. Scores stay on the device; vb_retrieval_rank ranks them there, and o
 With pack=True (or engine.pack_padding) each pair runs on a plan that holds the chunk's valid regions and the caption's valid
 tokens only (retrieval_pack_plan, DESIGN.md §4e).
 
+Across GPUs (torchrun, one rank per GPU): pass group= (e.g. dist.group.WORLD) to score() / evaluate_retrieval*(). Each of the W
+ranks scores its contiguous caption block (shard_bounds) against the whole gallery, the blocks are gathered into the same [C, G]
+matrix on every rank (gather_rows), and every rank ranks it and returns the same metrics and lists. A fixed-length vector of the
+shapes, options and exact checksums of the inputs and weights is compared first (check_agreement), so ranks called with other
+data or weights raise ValueError instead of hanging or gathering a wrong matrix. group=None runs on one GPU with no
+torch.distributed call.
+
+    out = evaluate_retrieval_both(model, dataset, task_id="TASK8", group=dist.group.WORLD)     # same result on every rank
+
 Differences from the reference: equal scores are ordered by image index (the reference's default argsort leaves their order
 unspecified), and progress is logged once per chunk rather than after every caption (no caption has a full score row before the
 last chunk).
@@ -34,9 +43,10 @@ from collections import OrderedDict
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from . import _lib as L
-from .engine import pack_capacity
+from .engine import PRECISIONS, pack_capacity
 
 logger = logging.getLogger(__name__)
 
@@ -133,6 +143,65 @@ def retrieval_pack_plan(image_mask, caption_mask, chunk, has_task):
     return chunks, bad_chunks, ok_t.count(False)
 
 
+# ------------------------------------------------------------------------------------------ across GPUs
+# the fields of the vector every rank all-gathers before scoring (check_agreement), in order
+AGREEMENT_FIELDS = ("captions", "caption length", "images", "regions", "chunk", "pack", "head", "task", "precision",
+                    "deterministic", "caption ids", "caption masks", "segment ids", "image masks", "image features",
+                    "image spatials", "parameters")
+
+
+def shard_bounds(C, world):
+    """Each rank's contiguous caption block [lo, hi): rank r scores [r·C // W, (r+1)·C // W). Every caption lands in exactly one
+    block, in order, and block sizes differ by at most one; with C < W some blocks are empty."""
+    return [(r * C // world, (r + 1) * C // world) for r in range(world)]
+
+
+def checksum(t):
+    """The int64 sum of t's bytes read as int32 bit patterns (zero-padded to a multiple of 4 bytes). Integer sums are exact, so
+    the value does not depend on summation order or device: equal tensors give equal checksums on every rank."""
+    b = t.detach().contiguous().reshape(-1).view(torch.uint8)
+    if b.numel() % 4 or b.storage_offset() % 4:
+        b = torch.cat((b, b.new_zeros(-b.numel() % 4)))
+    return int(b.view(torch.int32).sum(dtype=torch.int64))
+
+
+def _comm_device(group, device):
+    """Where a collective's tensors live: `device` with NCCL, the host with gloo (or any other backend)."""
+    return torch.device(device) if "nccl" in str(dist.get_backend(group)) else torch.device("cpu")
+
+
+def check_agreement(fields, group, device="cpu"):
+    """All-gathers {AGREEMENT_FIELDS name: int} over `group` (one fixed-length int64 vector per rank) and raises ValueError on
+    every rank, naming each field on which the ranks differ. The vector's length does not depend on the inputs, so this
+    collective is safe to enter with any arguments; the ones whose sizes do depend on them come after it."""
+    mine = torch.tensor([int(fields[n]) for n in AGREEMENT_FIELDS], dtype=torch.int64, device=_comm_device(group, device))
+    world = dist.get_world_size(group)
+    every = torch.empty(world * mine.numel(), dtype=torch.int64, device=mine.device)
+    dist.all_gather_into_tensor(every, mine, group=group)
+    every = every.view(world, -1).cpu()
+    bad = [f"{n} {every[:, i].tolist()}" for i, n in enumerate(AGREEMENT_FIELDS) if bool((every[:, i] != every[0, i]).any())]
+    if bad:
+        raise ValueError(f"retrieval across {world} ranks: every rank must call with the same data, options and weights; "
+                         f"they differ in: {'; '.join(bad)} (per rank)")
+
+
+def gather_rows(block, C, group):
+    """The [C, G] matrix made of every rank's block of rows (shard_bounds(C, W), this rank's is `block`), in caption order, on
+    every rank of `group`. The blocks are padded to ceil(C / W) rows and gathered with one all_gather_into_tensor on block's
+    device."""
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    bounds = shard_bounds(C, world)
+    lo, hi = bounds[rank]
+    if block.shape[0] != hi - lo:
+        raise ValueError(f"rank {rank}: a block of {block.shape[0]} rows; shard_bounds gives it {hi - lo}")
+    per = -(-C // world)
+    padded = block.new_zeros((per, block.shape[1]))
+    padded[:hi - lo] = block
+    every = block.new_empty((world * per, block.shape[1]))
+    dist.all_gather_into_tensor(every, padded, group=group)
+    return torch.cat([every[r * per:r * per + (b - a)] for r, (a, b) in enumerate(bounds)])
+
+
 class RetrievalEvaluator:
     """Scores captions against a fixed image gallery on fast-mode forward-only plans with a precomputed image prefix.
 
@@ -198,10 +267,18 @@ class RetrievalEvaluator:
         plan.load_images(*parts)
         plan.run_image_prefix()
 
-    def score(self, captions, input_mask, segment_ids, task_id=None):
+    def score(self, captions, input_mask, segment_ids, task_id=None, group=None):
         """Device f32 [C, G]: the score of every caption (int64 [C, Nt], with its mask and segment ids) against every image.
         task_id (int or "TASKn") sets the task tokens of a model with config.task_specific_tokens; the pre-training model takes
-        none (TypeError, as its forward has no task_ids parameter)."""
+        none (TypeError, as its forward has no task_ids parameter).
+
+        group: a torch.distributed process group. None, or a group of one rank, scores every caption here and makes no
+        torch.distributed call. With W > 1 ranks, every rank must call with the same arguments (and evaluators built alike): the
+        ranks first compare the shapes, options and checksums of the inputs and the weights (check_agreement, ValueError on
+        every rank if they differ), rank r then scores its caption block shard_bounds(C, W)[r] against the whole gallery, and
+        every rank returns the same gathered [C, G] (gather_rows). A rank with an empty block scores nothing but joins both
+        collectives. Packing is decided per rank on its block, so engine.pack_fallbacks counts what this rank ran: a chunk that
+        falls back is counted once on every rank with captions."""
         model, eng = self.model, self.model.engine
         if self.heads == "pretraining" and task_id is not None:
             raise TypeError("BertForMultiModalPreTraining.forward() takes no task_ids (vilbert.py:1471-1484): score without task_id")
@@ -210,6 +287,32 @@ class RetrievalEvaluator:
         has_task = bool(model.config.task_specific_tokens) and self.heads == "vl"
         if has_task and task_id is None:
             raise ValueError("config.task_specific_tokens is set: task_id is required")
+        world = 1 if group is None else dist.get_world_size(group)
+        if world == 1:
+            return self._score_rows(captions, input_mask, segment_ids, task_id, has_task)
+        C = int(captions.shape[0])
+        check_agreement(self._agreement(captions, input_mask, segment_ids, task_id), group, eng.device)
+        lo, hi = shard_bounds(C, world)[dist.get_rank(group)]
+        if hi > lo:
+            block = self._score_rows(captions[lo:hi], input_mask[lo:hi], segment_ids[lo:hi], task_id, has_task)
+        else:
+            block = torch.empty((0, self.G), dtype=torch.float32, device=eng.device)
+        return gather_rows(block.to(_comm_device(group, eng.device)), C, group).to(eng.device)
+
+    def _agreement(self, captions, input_mask, segment_ids, task_id):
+        """This rank's check_agreement fields for a score() call."""
+        eng = self.model.engine
+        return dict(zip(AGREEMENT_FIELDS, (
+            captions.shape[0], captions.shape[1], self.G, self.Nv, self.chunk,
+            self.pack if self.pack is not None else eng.pack_padding, list(SCORE_HEAD).index(self.heads),
+            -1 if task_id is None else _task_number(task_id), PRECISIONS.index(eng.precision),
+            torch.are_deterministic_algorithms_enabled(),
+            *(checksum(t) for t in (captions, input_mask, segment_ids, self.image_mask, self.features, self.spatials, eng.ps.flat)))))
+
+    def _score_rows(self, captions, input_mask, segment_ids, task_id, has_task):
+        """The scores of these captions against the whole gallery on this device: chunk outer, capacity group middle, caption
+        inner."""
+        model, eng = self.model, self.model.engine
         dev = eng.device
         C, Nt = int(captions.shape[0]), int(captions.shape[1])
         chunks = self._chunks(input_mask, has_task)
@@ -299,16 +402,18 @@ def i2t_metrics(ranks):
     return retrieval_metrics(ranked), int(len(r) - len(ranked))
 
 
-def evaluate_retrieval(model, dataset, task_id=None, chunk=500, k=20, pack=None):
+def evaluate_retrieval(model, dataset, task_id=None, chunk=500, k=20, pack=None, group=None):
     """The loop of eval_retrieval.py:253-358 (and, with the pre-training model and task_id=None, of eval_coco_retrieval.py:336-412):
     (r1, r5, r10, medr, meanr, results), results being each caption's top-k image list (the reference dumps the top 20 into
     *_result.json). The dataset is read through the reference's item protocol (read_retrieval_dataset); metrics are taken over the
     captions evaluated, which with the reference's 5,000 x 1,000 sizes is exactly its number. Puts the model in eval mode, as the
-    reference loop does. pack: score on packed plans (RetrievalEvaluator); None follows model.engine.pack_padding."""
+    reference loop does. pack: score on packed plans (RetrievalEvaluator); None follows model.engine.pack_padding.
+    group: a torch.distributed process group to shard the captions over (RetrievalEvaluator.score); every rank ranks the gathered
+    scores and returns the same result."""
     model.eval()
     feats, spats, imask, caps, masks, segs, targets = read_retrieval_dataset(dataset)
     ev = RetrievalEvaluator(model, feats, spats, imask, chunk=chunk, pack=pack)
-    scores = ev.score(caps, masks, segs, task_id=task_id)
+    scores = ev.score(caps, masks, segs, task_id=task_id, group=group)
     ranks, topk = ev.rank(scores, targets, k=k)
     both = torch.cat((ranks.view(-1, 1), topk), dim=1).cpu()       # the one read-back
     r1, r5, r10, medr, meanr = retrieval_metrics(both[:, 0])
@@ -316,17 +421,18 @@ def evaluate_retrieval(model, dataset, task_id=None, chunk=500, k=20, pack=None)
     return r1, r5, r10, medr, meanr, both[:, 1:1 + min(k, ev.G)].tolist()
 
 
-def evaluate_retrieval_both(model, dataset, task_id=None, chunk=500, k=20, pack=None):
+def evaluate_retrieval_both(model, dataset, task_id=None, chunk=500, k=20, pack=None, group=None):
     """Both retrieval directions from one scoring pass, with the arguments of evaluate_retrieval:
     {"t2i": (r1, r5, r10, medr, meanr, results), "i2t": (r1, r5, r10, medr, meanr, results), "rsum": float,
     "images_without_caption": n}. t2i (caption-to-image, image retrieval) is what evaluate_retrieval returns. i2t (image-to-text,
     text retrieval) ranks each image's best-placed ground-truth caption (rank_captions); its metrics are retrieval_metrics over the
     images with at least one caption (i2t_metrics), and its results are every image's top-k caption list. rsum is the sum of both
-    directions' r1, r5 and r10. Both directions' ranks and top-k lists are read back in one copy."""
+    directions' r1, r5 and r10. Both directions' ranks and top-k lists are read back in one copy. With group=, as for
+    evaluate_retrieval, every rank returns the same dictionary."""
     model.eval()
     feats, spats, imask, caps, masks, segs, targets = read_retrieval_dataset(dataset)
     ev = RetrievalEvaluator(model, feats, spats, imask, chunk=chunk, pack=pack)
-    scores = ev.score(caps, masks, segs, task_id=task_id)
+    scores = ev.score(caps, masks, segs, task_id=task_id, group=group)
     C, G = scores.shape
     ranks_t, topk_t = ev.rank(scores, targets, k=k)
     ranks_i, topk_i = ev.rank_captions(scores, targets, k=k)
