@@ -552,6 +552,18 @@ vb_status vb_radam_step(float* p, float* g, float* m, float* v, void* p16, void*
                         const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step, float grad_scale,
                         int32_t zero_grad, void* stream);
 
+/* vb_adamw_step_capped / vb_radam_step_capped: vb_adamw_step / vb_radam_step on a grid of at most max_ctas CTAs (0: no cap, the
+ * 8 x SMs of the plain calls; < 0 is refused). The same kernels stride over the chunk table, so every element gets bitwise the
+ * update, moments and copies of the plain calls. For a step that runs beside the backward's GEMMs (optim.step_in_backward). */
+vb_status vb_adamw_step_capped(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                               const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
+                               const vb_adamw_group* groups, const int32_t* step, float grad_scale, int32_t zero_grad,
+                               int32_t max_ctas, void* stream);
+vb_status vb_radam_step_capped(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                               const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
+                               const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step,
+                               float grad_scale, int32_t zero_grad, int32_t max_ctas, void* stream);
+
 /* Gradient-norm clipping and non-finite step skipping for the two optimizers above: apex FusedAdam's max_grad_norm (the
  * reference's --fp16 optimizer, train_concap.py:452-457), torch.nn.utils.clip_grad_norm_, and the step skip of
  * torch.amp.GradScaler, decided on the device.

@@ -293,10 +293,12 @@ radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
   }
 }
 
-// Grid of the optimizer kernels: up to 8 CTAs per SM, never more CTAs than chunks.
-static int opt_grid(int n_chunks) {
+// Grid of the optimizer kernels: up to 8 CTAs per SM, at most max_ctas when max_ctas > 0, never more CTAs than chunks. The
+// CTAs stride over the chunk table, so the grid decides only which CTA updates an element, never how.
+static int opt_grid(int n_chunks, int max_ctas = 0) {
   int grid = sm_count() * 8;
   if (grid <= 0) grid = 132 * 8;
+  if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
   return grid > n_chunks ? n_chunks : grid;
 }
 
@@ -310,13 +312,14 @@ static bool opt_buffers_aligned(const void* p, const void* g, const void* m, con
 static vb_status adamw_launch(const char* name, float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b,
                               int32_t p16_fp16, const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
                               int32_t n_chunks, const vb_adamw_group* groups, const int32_t* step, float grad_scale, int32_t zero_grad,
-                              const vb_clip_record* rec, void* stream) {
+                              const vb_clip_record* rec, int32_t max_ctas, void* stream) {
+  if (max_ctas < 0) return set_error(VB_ERR_INVALID, "%s: max_ctas must be >= 0 (0: no cap)", name);
   if (n_chunks <= 0) return VB_OK;
   if (!p || !g || !m || !v || !chunk_start || !chunk_count || !chunk_group || !groups)
     return set_error(VB_ERR_INVALID, "%s: null argument", name);
   if (!opt_buffers_aligned(p, g, m, v, p16, p16_lo, p16_b))
     return set_error(VB_ERR_INVALID, "%s: buffers must be 16-byte aligned (16-bit copies 8-byte)", name);
-  cudaError_t e = launch_pdl(adamw_kernel, dim3(opt_grid(n_chunks)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
+  cudaError_t e = launch_pdl(adamw_kernel, dim3(opt_grid(n_chunks, max_ctas)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
                              static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),
                              reinterpret_cast<const long long*>(chunk_start), chunk_count, chunk_group, (int)n_chunks, groups, step,
                              grad_scale, (int)(zero_grad ? 1 : 0), rec);
@@ -327,8 +330,9 @@ static vb_status adamw_launch(const char* name, float* p, float* g, float* m, fl
 static vb_status radam_launch(const char* name, float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b,
                               int32_t p16_fp16, const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
                               int32_t n_chunks, const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step,
-                              float grad_scale, int32_t zero_grad, const vb_clip_record* rec, void* stream) {
+                              float grad_scale, int32_t zero_grad, const vb_clip_record* rec, int32_t max_ctas, void* stream) {
   if (!step || leader_group < 0) return set_error(VB_ERR_INVALID, "%s: null step counter or negative leader group", name);
+  if (max_ctas < 0) return set_error(VB_ERR_INVALID, "%s: max_ctas must be >= 0 (0: no cap)", name);
   // every argument is checked before the counter moves: a refused call changes nothing
   if (n_chunks > 0) {
     if (!p || !g || !m || !v || !chunk_start || !chunk_count || !chunk_group || !groups)
@@ -341,7 +345,7 @@ static vb_status radam_launch(const char* name, float* p, float* g, float* m, fl
     if (st != VB_OK) return st;
   }
   if (n_chunks <= 0) return VB_OK;
-  cudaError_t e = launch_pdl(radam_kernel, dim3(opt_grid(n_chunks)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
+  cudaError_t e = launch_pdl(radam_kernel, dim3(opt_grid(n_chunks, max_ctas)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
                              static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),
                              reinterpret_cast<const long long*>(chunk_start), chunk_count, chunk_group, (int)n_chunks, groups, (int)leader_group,
                              static_cast<const int*>(step), grad_scale, (int)(zero_grad ? 1 : 0), rec);
@@ -355,7 +359,7 @@ extern "C" vb_status vb_adamw_step(float* p, float* g, float* m, float* v, void*
                                    const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group, int32_t n_chunks,
                                    const vb_adamw_group* groups, const int32_t* step, float grad_scale, int32_t zero_grad, void* stream) {
   return vb::adamw_launch("vb_adamw_step", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group, n_chunks,
-                          groups, step, grad_scale, zero_grad, nullptr, stream);
+                          groups, step, grad_scale, zero_grad, nullptr, 0, stream);
 }
 
 extern "C" vb_status vb_radam_step(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
@@ -363,7 +367,24 @@ extern "C" vb_status vb_radam_step(float* p, float* g, float* m, float* v, void*
                                    const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step, float grad_scale,
                                    int32_t zero_grad, void* stream) {
   return vb::radam_launch("vb_radam_step", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group, n_chunks,
-                          groups, leader_group, step, advance_step, grad_scale, zero_grad, nullptr, stream);
+                          groups, leader_group, step, advance_step, grad_scale, zero_grad, nullptr, 0, stream);
+}
+
+// The same steps on at most max_ctas CTAs, for a step that shares the SMs with the backward's GEMMs (DESIGN.md §4d).
+extern "C" vb_status vb_adamw_step_capped(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                          const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
+                                          int32_t n_chunks, const vb_adamw_group* groups, const int32_t* step, float grad_scale,
+                                          int32_t zero_grad, int32_t max_ctas, void* stream) {
+  return vb::adamw_launch("vb_adamw_step_capped", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group,
+                          n_chunks, groups, step, grad_scale, zero_grad, nullptr, max_ctas, stream);
+}
+
+extern "C" vb_status vb_radam_step_capped(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                          const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
+                                          int32_t n_chunks, const vb_adamw_group* groups, int32_t leader_group, int32_t* step,
+                                          int32_t advance_step, float grad_scale, int32_t zero_grad, int32_t max_ctas, void* stream) {
+  return vb::radam_launch("vb_radam_step_capped", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group,
+                          n_chunks, groups, leader_group, step, advance_step, grad_scale, zero_grad, nullptr, max_ctas, stream);
 }
 
 extern "C" vb_status vb_grad_norm(const float* g, const int64_t* chunk_start, const int32_t* chunk_count, int32_t n_chunks, float grad_scale,
@@ -391,7 +412,7 @@ extern "C" vb_status vb_adamw_step_clipped(float* p, float* g, float* m, float* 
                                            int32_t zero_grad, const vb_clip_record* record, void* stream) {
   if (!record) return vb::set_error(VB_ERR_INVALID, "vb_adamw_step_clipped: null record");
   return vb::adamw_launch("vb_adamw_step_clipped", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group,
-                          n_chunks, groups, step, grad_scale, zero_grad, record, stream);
+                          n_chunks, groups, step, grad_scale, zero_grad, record, 0, stream);
 }
 
 extern "C" vb_status vb_radam_step_clipped(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
@@ -401,5 +422,5 @@ extern "C" vb_status vb_radam_step_clipped(float* p, float* g, float* m, float* 
                                            void* stream) {
   if (!record) return vb::set_error(VB_ERR_INVALID, "vb_radam_step_clipped: null record");
   return vb::radam_launch("vb_radam_step_clipped", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group,
-                          n_chunks, groups, leader_group, step, advance_step, grad_scale, zero_grad, record, stream);
+                          n_chunks, groups, leader_group, step, advance_step, grad_scale, zero_grad, record, 0, stream);
 }

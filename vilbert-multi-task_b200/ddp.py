@@ -84,19 +84,24 @@ class FlatGradAllReducer:
             dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
             t.div_(self.world)
 
+    def comm_stream(self):
+        """The communication stream of the overlapped backward (created on first use)."""
+        if self._comm is None:
+            self._comm = torch.cuda.Stream(device=self.flat.device)
+        return self._comm
+
     def overlapped_backward(self, plan):
         """Runs the backward of `plan` in the pieces of plan.bucket_schedule(self.table) and averages each bucket (allreduce_range,
         asynchronous) on a communication stream as soon as the piece that finishes it has run, so the exchange overlaps the rest of
         the backward. Returns once the current stream waits for every collective: work queued after it (an optimizer step, a
         gradient-norm clip) sees the averaged buffer."""
-        if self._comm is None:
-            self._comm = torch.cuda.Stream(device=self.flat.device)
+        comm = self.comm_stream()
         works = []
 
         def handover(ranges):
             works.extend(self.allreduce_range(lo, hi) for lo, hi in ranges)
-        plan.run_backward_pieces(self.table, handover, self._comm)
-        torch.cuda.current_stream().wait_stream(self._comm)
+        plan.run_backward_pieces(self.table, handover, comm)
+        torch.cuda.current_stream().wait_stream(comm)
         for w in works:
             if w is not None:
                 w.wait()

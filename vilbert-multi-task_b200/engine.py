@@ -970,6 +970,7 @@ class Plan:
         self._scatter_ok = False          # the baseline's row heads may scatter straight into the stream gradient (base_rows)
         self._live_ranges_cache = {}      # (lo, hi) -> live_ranges(lo, hi), for run_step_overlapped
         self._bucket_schedules = {}       # bucket table -> bucket_schedule(table)
+        self._step_schedules = {}         # (bucket table, allreduce) -> step_schedule(table, allreduce)
         self._piece_runs, self._piece_graphs = Counter(), {}     # schedule -> eager runs / its graphs (run_backward_pieces)
         self.n_kernels_fwd = self.n_kernels_bwd = 0
         self.graph_fwd = self.graph_bwd = self.graph_step = None
@@ -3005,6 +3006,49 @@ class Plan:
             c[(lo, hi)] = self.live_ranges(lo, hi)
         return c[(lo, hi)]
 
+    def _bucket_ready(self, key, weights=False):
+        """Per bucket (lo, hi) of `key`: one past the last backward op that passes an address inside the bucket's range of the flat
+        gradient buffer (0 when none does). The launches themselves are read (op_pointers), so side-stream event markers and, in
+        deterministic plans, the ordered sums of split-K and bias gradients are seen where they run. An address stands for the
+        span from it to the end of the outermost range containing it (ranges nest: a fused projection holds its parts): the
+        gradient ranges of grad_touch, which records when a gradient view was taken.
+
+        weights=True: the readiness of a step, which rewrites the weights as well. The addresses inside the fp32 parameters
+        (ps.flat: LayerNorm gammas, the baseline's weight-norm v and g) and inside every 16-bit copy (ps.shadows: the dgrad GEMMs'
+        operands, the tied decoder's word-embedding copy) count too, and any entry or fused projection is such a range."""
+        ps = self.ps
+        spans = sorted(set(self.grad_touch) | ({ps.span(n) for n in list(ps.entries) + list(ps.fused)} if weights else set()))
+        starts = [off for off, _ in spans]
+        outer_end, m = [], 0
+        for off, n in spans:          # the end of the outermost range so far
+            m = max(m, off + n)
+            outer_end.append(m)
+        bufs = [ps.grad] + ([ps.flat] + [t for t in (ps.shadow, ps.shadow_lo, ps.shadows.extra_bw) if t is not None] if weights else [])
+        bases = [(t.data_ptr(), t.data_ptr() + t.element_size() * ps.numel, t.element_size()) for t in bufs]
+        ready = [0] * len(key)
+        for i, (fn, args, _) in enumerate(self.bwd):
+            if fn is None:
+                continue
+            for p in op_pointers(fn, args):
+                for base, end, es in bases:
+                    if base <= p < end:
+                        break
+                else:
+                    continue
+                o = (p - base) // es
+                j = bisect.bisect_right(starts, o) - 1
+                if j < 0 or outer_end[j] <= o:
+                    continue
+                for k, (lo, hi) in enumerate(key):
+                    if lo < outer_end[j] and o < hi:
+                        ready[k] = i + 1
+        return ready
+
+    @staticmethod
+    def _check_buckets(key, what):
+        if any(b[0] >= b[1] for b in key) or any(a[1] > b[0] for a, b in zip(key, key[1:])):
+            raise ValueError(f"{what}: the buckets must be non-empty, disjoint and in ascending order")
+
     def bucket_schedule(self, buckets):
         """The backward of the module surface's overlapped data parallelism (ddp.DistributedDataParallel(delay_allreduce=False)) cut
         into pieces: -> ((op_lo, op_hi, ranges), ...), where `ranges` are the buckets to all-reduce once bwd[op_lo:op_hi] has run.
@@ -3012,12 +3056,10 @@ class Plan:
         `buckets` is the reducer's table, the same on every rank: (lo, hi) ranges of the flat gradient buffer in ascending order.
         They are handed over in descending order, each exactly once, whatever this plan is, so ranks whose plans differ (packed
         capacities, a padded fallback, frozen or deterministic variants) issue the same collectives in the same order; only where
-        the backward pauses for them depends on the plan. A bucket is ready one past the last backward op that passes an address
-        inside a gradient range of grad_touch overlapping it (0 when none does): grad_touch records when a gradient view was
-        taken, which side-stream event markers and, in deterministic plans, the ordered sums of split-K and bias gradients follow,
-        so the launches themselves are read. The op writes from that address to the end of the outermost range containing it.
-        The cut of bucket k is the latest readiness of the buckets at or above it, moved forward to the next position that
-        straddles no side-stream event edge (_straddled). Cached per table: ddp.trainable_ranges changes it with requires_grad."""
+        the backward pauses for them depends on the plan. A bucket is ready once no later backward op writes its gradient
+        (_bucket_ready). The cut of bucket k is the latest readiness of the buckets at or above it, moved forward to the next
+        position that straddles no side-stream event edge (_straddled). Cached per table: ddp.trainable_ranges changes it with
+        requires_grad."""
         key = tuple((int(lo), int(hi)) for lo, hi in buckets)
         sched = self._bucket_schedules.get(key)
         if sched is not None:
@@ -3025,29 +3067,8 @@ class Plan:
         if self.anomaly:
             raise ValueError("bucket_schedule: the NaN checks of an anomaly plan read the gradients after the backward, and their "
                              "report comes before any collective; such plans all-reduce after the backward")
-        if any(b[0] >= b[1] for b in key) or any(a[1] > b[0] for a, b in zip(key, key[1:])):
-            raise ValueError("bucket_schedule: the buckets must be non-empty, disjoint and in ascending order")
-        spans = sorted(self.grad_touch)
-        starts = [off for off, _ in spans]
-        outer_end, m = [], 0
-        for off, n in spans:          # ranges nest (a fused projection holds its parts): the end of the outermost range so far
-            m = max(m, off + n)
-            outer_end.append(m)
-        base, numel = self.ps.grad.data_ptr(), self.ps.numel
-        ready = [0] * len(key)
-        for i, (fn, args, _) in enumerate(self.bwd):
-            if fn is None:
-                continue
-            for p in op_pointers(fn, args):
-                if not base <= p < base + 4 * numel:
-                    continue
-                o = (p - base) // 4
-                j = bisect.bisect_right(starts, o) - 1
-                if j < 0 or outer_end[j] <= o:
-                    continue
-                for k, (lo, hi) in enumerate(key):
-                    if lo < outer_end[j] and o < hi:
-                        ready[k] = i + 1
+        self._check_buckets(key, "bucket_schedule")
+        ready = self._bucket_ready(key)
         straddle = self._straddled()
         pieces, op_lo, cut, pending = [], 0, 0, []
         for k in reversed(range(len(key))):
@@ -3065,46 +3086,102 @@ class Plan:
         sched = self._bucket_schedules[key] = tuple(pieces)
         return sched
 
+    def step_schedule(self, buckets, allreduce):
+        """The backward cut into pieces for an optimizer step that runs while it does (optim step_in_backward):
+        -> ((op_lo, op_hi, ranges, steps), ...), where once bwd[op_lo:op_hi] has run `ranges` are the buckets to all-reduce and
+        `steps` the indexes (into `buckets`, descending) of the buckets whose step may start.
+
+        A bucket may be stepped once no later backward op reads or writes its weights, 16-bit copies or gradient
+        (_bucket_ready(weights=True)), moved forward past side-stream event edges as in bucket_schedule. With `allreduce` (data
+        parallel, delay_allreduce=False) the collectives keep bucket_schedule's pieces, order and cut points exactly, the step of
+        a bucket comes no earlier than its collective's handover, and a step point between two of those cuts is one more join of
+        the streams: nothing here depends on more than the plan and the table, so ranks issue the same collectives. Without it
+        `ranges` are empty. Cached per (table, allreduce)."""
+        key = tuple((int(lo), int(hi)) for lo, hi in buckets)
+        sched = self._step_schedules.get((key, allreduce))
+        if sched is not None:
+            return sched
+        if self.anomaly:
+            raise ValueError("step_schedule: the NaN report of an anomaly plan comes after the backward; its step runs after it")
+        self._check_buckets(key, "step_schedule")
+        straddle = self._straddled()
+        floor, hand, cuts = [0] * len(key), {}, set()
+        if allreduce:
+            index = {b: k for k, b in enumerate(key)}
+            for _, hi, ranges in self.bucket_schedule(key):
+                cuts.add(hi)
+                hand[hi] = ranges
+                for r in ranges:
+                    floor[index[r]] = hi
+        step_at = []
+        for k, r in enumerate(self._bucket_ready(key, weights=True)):
+            c = max(floor[k], r)
+            while straddle[c]:
+                c += 1
+            step_at.append(c)
+        cuts.update(step_at)
+        last = max(cuts, default=0)
+        if any(op[0] is not None for op in self.bwd[last:]):     # kernels that touch no bucket (input gradients): a last piece
+            cuts.add(len(self.bwd))
+        pieces, op_lo = [], 0
+        for c in sorted(cuts):
+            pieces.append((op_lo, c, hand.get(c, ()), tuple(k for k in reversed(range(len(key))) if step_at[k] == c)))
+            op_lo = c
+        sched = self._step_schedules[(key, allreduce)] = tuple(pieces)
+        return sched
+
     def _piece(self, lo, hi):
         """bwd[lo:hi] between two joins of every stream: a piece starts with a fork, so that in a graph capture every side stream it
         uses joins the capture, and ends with a join, so that everything it wrote is done when the main stream's event fires."""
         barrier = [(None, ("all",), 0)]
         return barrier + self.bwd[lo:hi] + barrier
 
-    def run_backward_pieces(self, buckets, handover, comm_stream):
+    def _schedule(self, buckets, step, allreduce):
+        return self.step_schedule(buckets, allreduce) if step is not None else self.bucket_schedule(buckets)
+
+    def run_backward_pieces(self, buckets, handover, comm_stream, step=None, step_stream=None):
         """The backward as the pieces of bucket_schedule(buckets). After each piece that finished buckets, `comm_stream` waits for an
         event recorded on the current stream and handover(ranges) is called under comm_stream with them; it enqueues the
         collectives, which stay outside any graph (DESIGN.md §4c). Pieces run eagerly, or as one CUDA graph each once
-        maybe_capture_pieces captured them. The caller makes the current stream wait for the collectives before reading the buffer."""
+        maybe_capture_pieces captured them. The caller makes the current stream wait for the collectives before reading the buffer.
+
+        With `step`, the pieces of step_schedule(buckets, allreduce=handover is not None): after each piece with step points,
+        `step_stream` waits for the same event and step(bucket indexes) is called under step_stream (after that piece's handover);
+        the caller makes the current stream wait for step_stream too."""
         if not self.holds_forward(self.fwd_id):
             raise L.VBError("shared activation arena: another plan's forward ran between this plan's forward and backward "
                             "(its saved activations are gone); run forward + backward per batch, or disable the arena")
         self.e.grad_clean = False
-        sched = self.bucket_schedule(buckets)
+        sched = self._schedule(buckets, step, handover is not None)
+        sinks = ((handover, comm_stream), (step, step_stream))
         graphs = self._piece_graphs.get(sched)
         main = torch.cuda.current_stream()
-        for i, (lo, hi, ranges) in enumerate(sched):
+        for i, (lo, hi, *items) in enumerate(sched):
             if hi > lo:
                 if graphs is not None:
                     graphs[i].replay()
                 else:
                     self._run(self._piece(lo, hi))
-            if ranges:
-                ev = torch.cuda.Event()
-                ev.record(main)
-                comm_stream.wait_event(ev)
-                with torch.cuda.stream(comm_stream):
-                    handover(ranges)
+            ev = None
+            for (fn, stream), it in zip(sinks, items):
+                if it:
+                    if ev is None:
+                        ev = torch.cuda.Event()
+                        ev.record(main)
+                    stream.wait_event(ev)
+                    with torch.cuda.stream(stream):
+                        fn(it)
         if graphs is None:
             self._piece_runs[sched] += 1
 
-    def maybe_capture_pieces(self, buckets, after=2):
-        """maybe_capture_passes for the pieces of bucket_schedule(buckets): once they have run eagerly `after` times, one CUDA graph
-        per non-empty piece, captured without a warm-up run (it would accumulate into the gradient buffer)."""
-        sched = self.bucket_schedule(buckets)
+    def maybe_capture_pieces(self, buckets, after=2, step=False, allreduce=True):
+        """maybe_capture_passes for the pieces of bucket_schedule(buckets) (with `step`: of step_schedule(buckets, allreduce)): once
+        they have run eagerly `after` times, one CUDA graph per non-empty piece, captured without a warm-up run (it would accumulate
+        into the gradient buffer)."""
+        sched = self._schedule(buckets, True if step else None, allreduce)
         if sched not in self._piece_graphs and self._piece_runs[sched] >= after:
             torch.cuda.synchronize()
-            self._piece_graphs[sched] = [self._record(self._piece(lo, hi)) if hi > lo else None for lo, hi, _ in sched]
+            self._piece_graphs[sched] = [self._record(self._piece(lo, hi)) if hi > lo else None for lo, hi, *_ in sched]
 
     def capture(self, separate=False):
         """Captures the plan into CUDA graphs (one for the whole step, or one per pass)."""

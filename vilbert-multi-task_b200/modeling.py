@@ -9,6 +9,7 @@ import operator
 import os
 import traceback
 import warnings
+import weakref
 
 import torch
 import torch.nn as nn
@@ -104,7 +105,11 @@ class _PlanCall:
     NaN checks (Plan(anomaly=True)) and forward() keeps the Python stack of the call. backward() reads the plan's report right after
     its backward ran; when a gradient held a NaN it warns with that stack and raises RuntimeError naming the first op, as torch
     names the backward node — before the input gradients are copied out and before the all-reduce, so the caller's optimizer step is
-    never reached. The flat gradient buffer keeps what the backward wrote."""
+    never reached. The flat gradient buffer keeps what the backward wrote.
+
+    Inside a fused optimizer's step_in_backward() context (model._step_in_backward), the backward of the model's only pending plan
+    call (model._pending_calls: calls whose forward made outputs that need a gradient and whose backward has not run) runs in the
+    pieces of Plan.step_schedule with the step in it; every other backward runs as above and the context steps after it."""
 
     def __init__(self, model, plan, inputs, targets=None, names=None):
         self.model, self.plan, self.inputs, self.targets, self.names = model, plan, inputs, targets or {}, names
@@ -165,6 +170,8 @@ class _PlanCall:
         plan = self.plan
         red = model._ddp_reducer if model._ddp_sync else None
         overlap = red is not None and model._ddp_overlap and red.world > 1 and not plan.anomaly
+        step = self._step_hook(red, overlap)
+        step_here = step is not None
         now = eng.drop_step_host
         moved = plan.train and now != self.drop_step
         if moved:
@@ -177,7 +184,7 @@ class _PlanCall:
             model._attach_grads()
             if eng.auto_graph:
                 plan.maybe_capture_passes()
-                if overlap:
+                if overlap and not step_here:
                     plan.maybe_capture_pieces(red.table)
             if self.names is not None:
                 for n, g in zip(self.names, grads):
@@ -189,7 +196,9 @@ class _PlanCall:
                         plan.loss_grad[i:i + 1].zero_()
                     else:
                         plan.loss_grad[i:i + 1].copy_(g.detach().reshape(1))
-            if overlap:
+            if step_here:
+                step(plan, red if overlap else None)
+            elif overlap:
                 red.overlapped_backward(plan)
             else:
                 plan.run_backward()
@@ -201,6 +210,19 @@ class _PlanCall:
                 eng.set_dropout_step(now)
         if red is not None and not overlap:     # data parallel: average the flat gradient buffer over the ranks (apex DDP, delay_allreduce=True)
             red.allreduce()
+
+    def _step_hook(self, red, overlap):
+        """The model's step_in_backward hook when this backward runs with the optimizer step in it, else None. It does when the
+        context is active, this call is the model's only pending plan backward, its plan has no anomaly checks and its gradient is
+        not all-reduced after the backward (delay_allreduce=True). The call stops being pending here."""
+        model = self.model
+        pending = model._pending_calls
+        alone = len(pending) == 1 and self in pending
+        pending.discard(self)
+        hook = model._step_in_backward
+        if hook is not None and alone and not self.plan.anomaly and (red is None or overlap):
+            return hook
+        return None
 
     def _raise_on_nan(self, r):
         """torch's anomaly-mode report for the NanRecord `r` (None: nothing to report)."""
@@ -237,6 +259,8 @@ class _PlanFn(torch.autograd.Function):
         dead = [o for o, live in zip(outs, call.differentiable()) if not live]
         if dead:
             ctx.mark_non_differentiable(*dead)
+        if len(dead) < len(outs):
+            call.model._pending_calls.add(call)
         return outs
 
     @staticmethod
@@ -281,6 +305,8 @@ class BertPreTrainedModel(nn.Module):
         self._ddp_set_ranges = None     # data parallel: restricts the reducer to the trainable ranges (ddp.DistributedDataParallel)
         self._ddp_overlap = False       # ... all-reduces the buckets during the backward (delay_allreduce=False)
         self._ddp_sync = True           # False under no_sync()
+        self._step_in_backward = None   # a fused optimizer's step_in_backward(): runs the backward with the step in it
+        self._pending_calls = weakref.WeakSet()   # plan calls whose outputs need a gradient and whose backward has not run
         self.init_weights()
 
     # ---- reference init (vilbert.py:1274-1285): N(0, initializer_range) for Linear/Embedding weights, zero bias, LN 1/0

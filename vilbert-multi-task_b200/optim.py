@@ -18,13 +18,23 @@ of the updated weights and zeroes the gradients, so the training step needs no s
 global L2 norm of the trainable gradients to c as torch.nn.utils.clip_grad_norm_ does, and skips a step whose gradient holds a
 NaN or an inf, both decided on the device: one norm launch over the gradient buffer writes a small record that the optimizer
 launch reads, so nothing is read back to the host.
+
+`with optimizer.step_in_backward(): loss.backward()` runs the same step while the backward runs: each bucket of the flat
+buffers is updated on a side stream as soon as no later backward op touches it (INTEGRATION.md §1k, DESIGN.md §4d).
 """
+import contextlib
 import ctypes as C
 
 import numpy as np
 import torch
 
 from . import _lib as L
+
+# The step in the backward, chosen by measurement on an H100 (DESIGN.md §4d, tools/step_in_backward_probe.py): the number of
+# buckets a single process cuts the trainable ranges into (as ddp.FlatGradAllReducer cuts them), and the CTA cap of each
+# bucket's launch (vb_adamw_step_capped / vb_radam_step_capped; 0: the 8 x SMs grid of step()).
+STEP_BUCKETS = 4
+STEP_MAX_CTAS = 264
 
 _GROUP_DT = np.dtype([("lr", "<f4"), ("beta1", "<f4"), ("beta2", "<f4"), ("eps", "<f4"), ("weight_decay", "<f4"), ("correct_bias", "<i4"),
                       ("one_minus_beta1", "<f4"), ("one_minus_beta2", "<f4")])
@@ -48,6 +58,18 @@ def build_chunks(ranges, chunk=32768):
         for s in range(0, n, chunk):
             st.append(off + s); cn.append(min(chunk, n - s)); gr.append(gi)
     return np.asarray(st, np.int64), np.asarray(cn, np.int32), np.asarray(gr, np.int32)
+
+
+def bucket_chunks(ranges, table, chunk=32768):
+    """ranges: [(flat offset, numel, group index)] of the trainable tensors (as build_chunks takes them); table: disjoint (lo, hi)
+    buckets of the flat buffer in ascending order -> per bucket the chunk table (build_chunks) of the parts of the ranges inside it:
+    chunks are split at bucket edges, which changes nothing per element. Every element of the ranges lies in exactly one bucket's
+    table; one outside every bucket raises ValueError (pure host logic, unit-tested on CPU)."""
+    out = [build_chunks([(max(off, lo), min(off + n, hi) - max(off, lo), gi) for off, n, gi in ranges if off < hi and off + n > lo],
+                        chunk) for lo, hi in table]
+    if sum(int(cn.sum()) for _, cn, _ in out) != sum(n for _, n, _ in ranges):
+        raise ValueError("bucket_chunks: trainable elements lie outside every bucket")
+    return out
 
 
 class _FlatBufferOptimizer(torch.optim.Optimizer):
@@ -80,6 +102,12 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
                                  "without clipping)")
         super().__init__(params, defaults)
         self.engine = engine
+        from .ddp import DistributedDataParallel
+        self._model = model.module if isinstance(model, DistributedDataParallel) else model
+        self._bucket_tables = {}      # (bucket table, trainable key) -> per-bucket launch arguments (_bucket_launches)
+        self._single_tables = {}      # frozen set -> the single-process bucket table
+        self._side = None             # the stream of the step in the backward
+        self._stepped = False         # inside step_in_backward: the step ran in a backward
         self.fused_zero_grad = bool(zero_grad)
         ps = engine.ps
         dev = ps.flat.device
@@ -188,6 +216,155 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
         for fn, args in ops:
             L.call(fn, *args, stream=stream)
 
+    def _trainable_ranges(self):
+        """(flat offset, numel, group index) of the tracked parameters that are trainable now: the chunk table's ranges."""
+        return [(off, n, gi) for (p, off, n, gi), rg in zip(self._tracked, self._trainable_key) if rg]
+
+    # ------------------------------------------------------------------ the step in the backward
+    @contextlib.contextmanager
+    def step_in_backward(self):
+        """`with optimizer.step_in_backward(): loss.backward()` gives the state `loss.backward(); optimizer.step()` gives (weights,
+        moments, 16-bit copies, zeroed gradients, the device step counter, step_count and state[p]["step"]), with the step running
+        while the backward does: each bucket of the flat buffers is updated on a side stream once no later backward op reads or
+        writes its weights, 16-bit copies or gradient (engine Plan.step_schedule), on grid-capped launches of the same kernels. The
+        backward returns after the current stream waited for that stream, so the next forward reads the updated weights. Do not
+        call step() for this iteration; schedulers step as before.
+
+        Entering does what step() does on the host first (the trainable set, the hyper-parameter table), so an lr a scheduler set
+        since the last step applies. Each bucket gets the per-element update step() would give it, so under
+        torch.use_deterministic_algorithms(True) the two paths agree bit for bit.
+
+        Which backward steps: the step runs inside the backward of a plan-backed call of the model when that call is the only
+        pending plan backward of the model, i.e. no other plan-backed forward of the model whose outputs need a gradient is still
+        waiting for its backward (its gradient would not be final when this one's buckets are stepped). Otherwise the step runs
+        after the backward, unoverlapped, with the same result: when the backward reaches more than one plan-backed forward of
+        the model, when it reaches no plan, for a plan with anomaly checks (and not at all when that backward raised: a body that
+        raises steps nothing), and under data parallelism with delay_allreduce=True, where it follows the all-reduce. With
+        delay_allreduce=False a bucket is stepped after its collective.
+
+        Gradient accumulation: the micro-batches before the last use plain loss.backward() (under model.no_sync() with data
+        parallelism); the last one uses this context. Refused with ValueError: max_grad_norm (clipping needs the global norm before
+        any element is updated) and model.no_sync() (a step inside an accumulation micro-batch)."""
+        name = type(self).__name__
+        model = self._model
+        if model is None:
+            raise ValueError(f"{name}.step_in_backward needs the optimizer built with model=")
+        if self.max_grad_norm is not None:
+            raise ValueError(f"{name}.step_in_backward: max_grad_norm clips with the global gradient norm, which is known only after "
+                             "the whole backward; use loss.backward(); optimizer.step()")
+        if not model._ddp_sync:
+            raise ValueError(f"{name}.step_in_backward inside model.no_sync(): an accumulation micro-batch does not step; use plain "
+                             "loss.backward() for it and the context for the last micro-batch")
+        if model._step_in_backward is not None:
+            raise ValueError(f"{name}.step_in_backward: the model is already inside a step_in_backward context")
+        self._refresh()
+        self._upload_groups()
+        self._stepped = False
+        model._step_in_backward = self._backward_with_step
+        raised = True
+        try:
+            yield
+            raised = False
+        finally:
+            model._step_in_backward = None
+            if self._stepped:
+                self._count_step()
+                self._after_step()
+            elif not raised:
+                self.step()
+
+    def _refresh(self):
+        """The host work of step() before its launch that depends on the trainable set."""
+        self._refresh_trainable()
+
+    def _count_step(self):
+        self.step_count += 1
+        for st in self.state.values():
+            st["step"] = self.step_count
+
+    def _single_table(self):
+        """The buckets of a single process: ddp.trainable_ranges cut as ddp.FlatGradAllReducer cuts them (STEP_BUCKETS)."""
+        frozen = self._model._frozen()
+        table = self._single_tables.get(frozen)
+        if table is None:
+            from .ddp import FlatGradAllReducer
+            red = FlatGradAllReducer(self.engine.ps.grad, n_buckets=STEP_BUCKETS)
+            red.set_ranges(self._model._trainable_ranges())
+            table = self._single_tables[frozen] = red.table
+        return table
+
+    def _bucket_launches(self, table):
+        """Per bucket of `table`: (entry point, C arguments of its first launch of a step, C arguments of any later one) over its
+        chunk sub-table (bucket_chunks), which lives on the device with the cache entry."""
+        key = (table, self._trainable_key, self.grad_scale, self.fused_zero_grad, getattr(self, "leader_group", 0), STEP_MAX_CTAS)
+        hit = self._bucket_tables.get(key)
+        if hit is not None:
+            return hit[0]
+        ps, dev = self.engine.ps, self.exp_avg.device
+        subs = bucket_chunks(self._trainable_ranges(), table, self._chunk)
+        st, cn, gr = (torch.from_numpy(np.concatenate([s[i] for s in subs])).to(dev) for i in range(3))
+        out, at = [], 0
+        for s in subs:
+            n = len(s[0])
+            head = (ps.flat, ps.grad, self.exp_avg, self.exp_avg_sq, *ps.shadows.ptrs(), ps.shadows.fp16, st[at:], cn[at:], gr[at:], n,
+                    self._groups_dev)
+            fn = self._capped_fn()
+            out.append((fn, L.launch_args(fn, *self._capped_args(head, True)), L.launch_args(fn, *self._capped_args(head, False))))
+            at += n
+        self._bucket_tables[key] = (out, st, cn, gr)
+        return out
+
+    def _side_stream(self):
+        if self._side is None:
+            self._side = torch.cuda.Stream(device=self.exp_avg.device)
+        return self._side
+
+    def _backward_with_step(self, plan, red):
+        """The backward of `plan` with this step in it (the model's hook while step_in_backward is active): the pieces of
+        plan.step_schedule over the reducer's table (red: a data-parallel reducer all-reducing during the backward) or the
+        single-process table. After each piece the side stream waits for it and, under data parallelism, for the collectives of
+        the buckets it steps; it advances the device step counter once, before the first launch. The current stream waits for
+        the side stream (and the collectives) before this returns."""
+        if self._stepped:
+            raise RuntimeError(f"{type(self).__name__}.step_in_backward: a second backward reached a plan after the step ran; run one "
+                               "backward per context")
+        table = red.table if red is not None else self._single_table()
+        launches = self._bucket_launches(table)
+        side = self._side_stream()
+        if plan.e.auto_graph:
+            plan.maybe_capture_pieces(table, step=True, allreduce=red is not None)
+        works, first = {}, [True]
+
+        def handover(ranges):
+            works.update((r, red.allreduce_range(*r)) for r in ranges)
+
+        def step(ks):
+            if red is not None:          # collectives enqueued on the communication stream itself, then the asynchronous ones
+                side.wait_stream(comm)
+            for k in ks:
+                w = works.get(table[k])
+                if w is not None:
+                    w.wait()
+                self._launch_bucket(launches[k], first[0], side)
+                first[0] = False
+        comm = red.comm_stream() if red is not None else None
+        plan.run_backward_pieces(table, handover if red is not None else None, comm, step, side)
+        if first[0]:          # no bucket: the counter still moves, as in step()
+            with torch.cuda.stream(side):
+                self._step_dev.add_(1)
+        main = torch.cuda.current_stream()
+        if red is not None:
+            main.wait_stream(comm)
+            for w in works.values():
+                if w is not None:
+                    w.wait()
+        main.wait_stream(side)
+        self._stepped = True
+
+    def _launch_bucket(self, launch, first, stream):
+        fn, args_first, args = launch
+        L.check(fn(*(args_first if first else args), stream.cuda_stream), fn.__name__)
+
     def _after_step(self):
         eng = self.engine
         eng.shadow_clean = True
@@ -251,6 +428,18 @@ class FusedAdamW(_FlatBufferOptimizer):
             return [self._op(L.lib().vb_adamw_step, *args)]
         return [self._norm_op(self._step_dev), self._op(L.lib().vb_adamw_step_clipped, *args, self._clip_record)]
 
+    def _capped_fn(self):
+        return L.lib().vb_adamw_step_capped
+
+    def _capped_args(self, head, first):
+        return head + (self._step_dev, C.c_float(self.grad_scale), 1 if self.fused_zero_grad else 0, STEP_MAX_CTAS)
+
+    def _launch_bucket(self, launch, first, stream):
+        if first:            # the counter moves once per step, before the first launch reads it (correct_bias)
+            with torch.cuda.stream(stream):
+                self._step_dev.add_(1)
+        super()._launch_bucket(launch, first, stream)
+
     @torch.no_grad()
     def step(self, closure=None):
         loss = closure() if closure is not None else None
@@ -287,6 +476,18 @@ class FusedRAdam(_FlatBufferOptimizer):
         """The leader is the first param group holding a trainable tensor."""
         trainable = {id(p) for (p, _, _, _), rg in zip(self._tracked, self._trainable_key) if rg}
         self.leader_group = next((gi for gi, g in enumerate(self.param_groups) if any(id(p) in trainable for p in g["params"])), 0)
+
+    def _refresh(self):
+        if self._refresh_trainable():
+            self._set_leader()
+
+    def _capped_fn(self):
+        return L.lib().vb_radam_step_capped
+
+    def _capped_args(self, head, first):
+        """advance_step on the first launch of a step only; the leader-group rule is step()'s."""
+        return head + (self.leader_group, self._step_dev, 1 if first else 0, C.c_float(self.grad_scale), 1 if self.fused_zero_grad else 0,
+                       STEP_MAX_CTAS)
 
     def _args(self, advance_step):
         return self._buffer_args() + (self.leader_group, self._step_dev, advance_step, C.c_float(self.grad_scale),
