@@ -599,6 +599,29 @@ vb_status vb_radam_step_clipped(float* p, float* g, float* m, float* v, void* p1
                                 const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step,
                                 float grad_scale, int32_t zero_grad, const vb_clip_record* record, void* stream);
 
+/* The same steps on one rank's slice of an optimizer state sharded over data-parallel ranks (ZeRO stage 1; optim shard_state=True).
+ * vb_adamw_step_sharded / vb_radam_step_sharded: vb_adamw_step / vb_radam_step with the moments compact: m / v of chunk c start
+ * at element state_start[c] (int64, multiples of 4) of m / v instead of at chunk_start[c]. p, g and the 16-bit copies keep the
+ * flat layout, and every element gets bitwise what the unsharded calls give it (copies written, g zeroed when zero_grad).
+ * record: NULL (no clipping) or a record written by vb_clip_finish, as in the _clipped calls; max_ctas as in the _capped calls.
+ *
+ * vb_grad_norm_partial: *sum = sum of g^2 over the chunk table in float64, in vb_grad_norm's fixed order (partials: double
+ * [n_chunks]). The caller adds the ranks' sums (one all-reduce of one double) and passes the result to
+ * vb_clip_finish: the record of vb_grad_norm from that sum (norm, coef, skip, skipped; *step += 1 unless skip, step may be NULL).
+ * Every rank finishing the same sum writes the same record, so the ranks agree on skip and coefficient. */
+vb_status vb_adamw_step_sharded(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                const int64_t* chunk_start, const int64_t* state_start, const int32_t* chunk_count,
+                                const int32_t* chunk_group, int32_t n_chunks, const vb_adamw_group* groups, const int32_t* step,
+                                float grad_scale, int32_t zero_grad, const vb_clip_record* record, int32_t max_ctas, void* stream);
+vb_status vb_radam_step_sharded(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                const int64_t* chunk_start, const int64_t* state_start, const int32_t* chunk_count,
+                                const int32_t* chunk_group, int32_t n_chunks, const vb_adamw_group* groups, int32_t leader_group,
+                                int32_t* step, int32_t advance_step, float grad_scale, int32_t zero_grad,
+                                const vb_clip_record* record, int32_t max_ctas, void* stream);
+vb_status vb_grad_norm_partial(const float* g, const int64_t* chunk_start, const int32_t* chunk_count, int32_t n_chunks,
+                               double* partials, double* sum, void* stream);
+vb_status vb_clip_finish(const double* sum, float grad_scale, float max_norm, vb_clip_record* record, int32_t* step, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Single-stream baseline (BaseBertForVLTasks, vilbert/basebert.py:893-978).
  *

@@ -110,9 +110,21 @@ grad_sq_partials_kernel(const float* __restrict__ g, const long long* __restrict
   }
 }
 
-// Pass 2 (one CTA): adds the partials in a fixed order and writes the record the clipped optimizer launches read. The clip
-// coefficient is torch.nn.utils.clip_grad_norm_'s fp32 arithmetic, clamp(max_norm * reciprocal(norm + 1e-6), max=1) (torch
-// evaluates `max_norm / tensor` as reciprocal times max_norm), with IEEE rounding whatever the fast-math flags.
+// The record the clipped optimizer launches read, from the float64 sum of squares s (one thread). The clip coefficient is
+// torch.nn.utils.clip_grad_norm_'s fp32 arithmetic, clamp(max_norm * reciprocal(norm + 1e-6), max=1) (torch evaluates
+// `max_norm / tensor` as reciprocal times max_norm), with IEEE rounding whatever the fast-math flags.
+__device__ __forceinline__ void write_clip_record(double s, float grad_scale, float max_norm, vb_clip_record* __restrict__ rec,
+                                                  int* __restrict__ step) {
+  const int skip = isfinite(s) ? 0 : 1;
+  const float norm = (float)(fabs((double)grad_scale) * sqrt(s));
+  rec->norm = norm;
+  rec->coef = skip ? 0.f : fminf(__fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), max_norm), 1.f);
+  rec->skip = skip;
+  rec->skipped += skip;
+  if (step && !skip) *step += 1;
+}
+
+// Pass 2 (one CTA): adds the partials in a fixed order and writes the record.
 __global__ void __launch_bounds__(OPT_THREADS)
 grad_norm_finalize_kernel(const double* __restrict__ partials, int n_chunks, float grad_scale, float max_norm,
                           vb_clip_record* __restrict__ rec, int* __restrict__ step) {
@@ -121,15 +133,25 @@ grad_norm_finalize_kernel(const double* __restrict__ partials, int n_chunks, flo
   double s = 0.0;
   for (int c = threadIdx.x; c < n_chunks; c += OPT_THREADS) s += partials[c];
   s = block_sum_f64(s, red);
-  if (threadIdx.x == 0) {
-    const int skip = isfinite(s) ? 0 : 1;
-    const float norm = (float)(fabs((double)grad_scale) * sqrt(s));
-    rec->norm = norm;
-    rec->coef = skip ? 0.f : fminf(__fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), max_norm), 1.f);
-    rec->skip = skip;
-    rec->skipped += skip;
-    if (step && !skip) *step += 1;
-  }
+  if (threadIdx.x == 0) write_clip_record(s, grad_scale, max_norm, rec, step);
+}
+
+// vb_grad_norm_partial, pass 2 (one CTA): *sum = the partials added in grad_norm_finalize_kernel's fixed order.
+__global__ void __launch_bounds__(OPT_THREADS)
+grad_sq_sum_kernel(const double* __restrict__ partials, int n_chunks, double* __restrict__ sum) {
+  __shared__ double red[OPT_THREADS / 32];
+  pdl_entry();
+  double s = 0.0;
+  for (int c = threadIdx.x; c < n_chunks; c += OPT_THREADS) s += partials[c];
+  s = block_sum_f64(s, red);
+  if (threadIdx.x == 0) *sum = s;
+}
+
+// vb_clip_finish (one thread): the record from a sum of squares reduced over the ranks.
+__global__ void clip_finish_kernel(const double* __restrict__ sum, float grad_scale, float max_norm, vb_clip_record* __restrict__ rec,
+                                   int* __restrict__ step) {
+  pdl_entry();
+  write_clip_record(*sum, grad_scale, max_norm, rec, step);
 }
 
 // What a skipped step still does: zero the gradient over the chunk table (keeps the caller's "gradient is clean" bookkeeping).
@@ -158,10 +180,13 @@ __device__ __forceinline__ bool step_scale(const vb_clip_record* __restrict__ re
 // 1 - b^t in float64 for b = 1 - om, without the cancellation of forming b^t first.
 __device__ __forceinline__ double one_minus_pow(float om, double t) { return -expm1(t * log1p(-(double)om)); }
 
+// COMPACT: the moments of chunk c start at state_start[c] of m / v (a rank's slice of the optimizer state, vb_*_step_sharded)
+// instead of at the weight's flat offset; the per-element arithmetic is the same.
+template <bool COMPACT>
 __global__ void __launch_bounds__(OPT_THREADS)
 adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
              uint16_t* __restrict__ p16, uint16_t* __restrict__ p16_lo, __nv_bfloat16* __restrict__ p16_b, int fp16,
-             const long long* __restrict__ chunk_start,
+             const long long* __restrict__ chunk_start, const long long* __restrict__ state_start,
              const int* __restrict__ chunk_count, const int* __restrict__ chunk_group, int n_chunks,
              const vb_adamw_group* __restrict__ groups, const int* __restrict__ step, float grad_scale, int zero_grad,
              const vb_clip_record* __restrict__ rec) {
@@ -190,10 +215,11 @@ adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
       return pv;
     };
     const int n4 = n >> 2;   // chunk starts are multiples of 4 elements (tensors start on 8-element boundaries)
+    const long long m0 = COMPACT ? state_start[c] : s0;   // the chunk's first moment element
     float4* p4 = reinterpret_cast<float4*>(p + s0);
     float4* g4 = reinterpret_cast<float4*>(g + s0);
-    float4* m4 = reinterpret_cast<float4*>(m + s0);
-    float4* v4 = reinterpret_cast<float4*>(v + s0);
+    float4* m4 = reinterpret_cast<float4*>(m + m0);
+    float4* v4 = reinterpret_cast<float4*>(v + m0);
     for (int i = threadIdx.x; i < n4; i += OPT_THREADS) {
       float4 pv = p4[i], mv = m4[i], vv = v4[i];
       const float4 gv = g4[i];
@@ -204,10 +230,10 @@ adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
       store_copies4(p16, p16_lo, p16_b, fp16, s0, i, pv);
     }
     for (int i = (n4 << 2) + threadIdx.x; i < n; i += OPT_THREADS) {   // ragged tail of a tensor (e.g. a 3129-entry bias)
-      const long long e = s0 + i;
-      float mv = m[e], vv = v[e];
+      const long long e = s0 + i, f = m0 + i;
+      float mv = m[f], vv = v[f];
       const float pv = upd(p[e], g[e], mv, vv);
-      p[e] = pv; m[e] = mv; v[e] = vv;
+      p[e] = pv; m[f] = mv; v[f] = vv;
       if (zero_grad) g[e] = 0.f;
       store_copies1(p16, p16_lo, p16_b, fp16, e, pv);
     }
@@ -224,11 +250,13 @@ adamw_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
 // within a step every tensor uses the values computed from the FIRST tensor's group: the lr, b1 and b2 of the leader group
 // `leader` drive the rectified step of all tensors. Both scalars are computed in float64 like the reference's Python floats:
 // in fp32, 1 - b2^t cancels (at b2 = 0.999 N_sma(6) comes out 6.0005 instead of 5.994). b = 1 - one_minus_beta, not the fp32 b:
-// 2 / (1 - fp32(0.999)) - 1 is N_sma_max = 1999.03 instead of 1999.
+// 2 / (1 - fp32(0.999)) - 1 is N_sma_max = 1999.03 instead of 1999. COMPACT as adamw_kernel.
+template <bool COMPACT>
 __global__ void __launch_bounds__(OPT_THREADS)
 radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
              uint16_t* __restrict__ p16, uint16_t* __restrict__ p16_lo, __nv_bfloat16* __restrict__ p16_b, int fp16,
-             const long long* __restrict__ chunk_start, const int* __restrict__ chunk_count, const int* __restrict__ chunk_group,
+             const long long* __restrict__ chunk_start, const long long* __restrict__ state_start,
+             const int* __restrict__ chunk_count, const int* __restrict__ chunk_group,
              int n_chunks, const vb_adamw_group* __restrict__ groups, int leader, const int* __restrict__ step, float grad_scale,
              int zero_grad, const vb_clip_record* __restrict__ rec) {
   __shared__ float s_step_size;
@@ -269,10 +297,11 @@ radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
       return rect ? pv - step_size * (mv / (sqrtf(vv) + G.eps)) : pv - step_size * mv;
     };
     const int n4 = n >> 2;
+    const long long m0 = COMPACT ? state_start[c] : s0;   // the chunk's first moment element
     float4* p4 = reinterpret_cast<float4*>(p + s0);
     float4* g4 = reinterpret_cast<float4*>(g + s0);
-    float4* m4 = reinterpret_cast<float4*>(m + s0);
-    float4* v4 = reinterpret_cast<float4*>(v + s0);
+    float4* m4 = reinterpret_cast<float4*>(m + m0);
+    float4* v4 = reinterpret_cast<float4*>(v + m0);
     for (int i = threadIdx.x; i < n4; i += OPT_THREADS) {
       float4 pv = p4[i], mv = m4[i], vv = v4[i];
       const float4 gv = g4[i];
@@ -283,10 +312,10 @@ radam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m
       store_copies4(p16, p16_lo, p16_b, fp16, s0, i, pv);
     }
     for (int i = (n4 << 2) + threadIdx.x; i < n; i += OPT_THREADS) {
-      const long long e = s0 + i;
-      float mv = m[e], vv = v[e];
+      const long long e = s0 + i, f = m0 + i;
+      float mv = m[f], vv = v[f];
       const float pv = upd(p[e], g[e], mv, vv);
-      p[e] = pv; m[e] = mv; v[e] = vv;
+      p[e] = pv; m[f] = mv; v[f] = vv;
       if (zero_grad) g[e] = 0.f;
       store_copies1(p16, p16_lo, p16_b, fp16, e, pv);
     }
@@ -312,17 +341,18 @@ static bool opt_buffers_aligned(const void* p, const void* g, const void* m, con
 static vb_status adamw_launch(const char* name, float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b,
                               int32_t p16_fp16, const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
                               int32_t n_chunks, const vb_adamw_group* groups, const int32_t* step, float grad_scale, int32_t zero_grad,
-                              const vb_clip_record* rec, int32_t max_ctas, void* stream) {
+                              const vb_clip_record* rec, int32_t max_ctas, void* stream, const int64_t* state_start = nullptr) {
   if (max_ctas < 0) return set_error(VB_ERR_INVALID, "%s: max_ctas must be >= 0 (0: no cap)", name);
   if (n_chunks <= 0) return VB_OK;
   if (!p || !g || !m || !v || !chunk_start || !chunk_count || !chunk_group || !groups)
     return set_error(VB_ERR_INVALID, "%s: null argument", name);
   if (!opt_buffers_aligned(p, g, m, v, p16, p16_lo, p16_b))
     return set_error(VB_ERR_INVALID, "%s: buffers must be 16-byte aligned (16-bit copies 8-byte)", name);
-  cudaError_t e = launch_pdl(adamw_kernel, dim3(opt_grid(n_chunks, max_ctas)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
+  cudaError_t e = launch_pdl(state_start ? adamw_kernel<true> : adamw_kernel<false>, dim3(opt_grid(n_chunks, max_ctas)), dim3(OPT_THREADS), (size_t)0,
+                             static_cast<cudaStream_t>(stream), p, g, m, v,
                              static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),
-                             reinterpret_cast<const long long*>(chunk_start), chunk_count, chunk_group, (int)n_chunks, groups, step,
-                             grad_scale, (int)(zero_grad ? 1 : 0), rec);
+                             reinterpret_cast<const long long*>(chunk_start), reinterpret_cast<const long long*>(state_start), chunk_count,
+                             chunk_group, (int)n_chunks, groups, step, grad_scale, (int)(zero_grad ? 1 : 0), rec);
   if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "%s: %s", name, cudaGetErrorString(e));
   return VB_OK;
 }
@@ -330,7 +360,8 @@ static vb_status adamw_launch(const char* name, float* p, float* g, float* m, fl
 static vb_status radam_launch(const char* name, float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b,
                               int32_t p16_fp16, const int64_t* chunk_start, const int32_t* chunk_count, const int32_t* chunk_group,
                               int32_t n_chunks, const vb_adamw_group* groups, int32_t leader_group, int32_t* step, int32_t advance_step,
-                              float grad_scale, int32_t zero_grad, const vb_clip_record* rec, int32_t max_ctas, void* stream) {
+                              float grad_scale, int32_t zero_grad, const vb_clip_record* rec, int32_t max_ctas, void* stream,
+                              const int64_t* state_start = nullptr) {
   if (!step || leader_group < 0) return set_error(VB_ERR_INVALID, "%s: null step counter or negative leader group", name);
   if (max_ctas < 0) return set_error(VB_ERR_INVALID, "%s: max_ctas must be >= 0 (0: no cap)", name);
   // every argument is checked before the counter moves: a refused call changes nothing
@@ -345,9 +376,11 @@ static vb_status radam_launch(const char* name, float* p, float* g, float* m, fl
     if (st != VB_OK) return st;
   }
   if (n_chunks <= 0) return VB_OK;
-  cudaError_t e = launch_pdl(radam_kernel, dim3(opt_grid(n_chunks, max_ctas)), dim3(OPT_THREADS), (size_t)0, static_cast<cudaStream_t>(stream), p, g, m, v,
+  cudaError_t e = launch_pdl(state_start ? radam_kernel<true> : radam_kernel<false>, dim3(opt_grid(n_chunks, max_ctas)), dim3(OPT_THREADS), (size_t)0,
+                             static_cast<cudaStream_t>(stream), p, g, m, v,
                              static_cast<uint16_t*>(p16), static_cast<uint16_t*>(p16_lo), static_cast<__nv_bfloat16*>(p16_b), (int)(p16_fp16 ? 1 : 0),
-                             reinterpret_cast<const long long*>(chunk_start), chunk_count, chunk_group, (int)n_chunks, groups, (int)leader_group,
+                             reinterpret_cast<const long long*>(chunk_start), reinterpret_cast<const long long*>(state_start), chunk_count,
+                             chunk_group, (int)n_chunks, groups, (int)leader_group,
                              static_cast<const int*>(step), grad_scale, (int)(zero_grad ? 1 : 0), rec);
   if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "%s: %s", name, cudaGetErrorString(e));
   return VB_OK;
@@ -423,4 +456,55 @@ extern "C" vb_status vb_radam_step_clipped(float* p, float* g, float* m, float* 
   if (!record) return vb::set_error(VB_ERR_INVALID, "vb_radam_step_clipped: null record");
   return vb::radam_launch("vb_radam_step_clipped", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group,
                           n_chunks, groups, leader_group, step, advance_step, grad_scale, zero_grad, record, 0, stream);
+}
+
+// One rank's slice of a sharded optimizer state (optim shard_state=True): the same kernels with the moments of chunk c at
+// state_start[c] of m / v; record may be NULL (no clipping), max_ctas 0 (no cap).
+extern "C" vb_status vb_adamw_step_sharded(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                           const int64_t* chunk_start, const int64_t* state_start, const int32_t* chunk_count,
+                                           const int32_t* chunk_group, int32_t n_chunks, const vb_adamw_group* groups, const int32_t* step,
+                                           float grad_scale, int32_t zero_grad, const vb_clip_record* record, int32_t max_ctas,
+                                           void* stream) {
+  if (n_chunks > 0 && !state_start) return vb::set_error(VB_ERR_INVALID, "vb_adamw_step_sharded: null state_start");
+  return vb::adamw_launch("vb_adamw_step_sharded", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group,
+                          n_chunks, groups, step, grad_scale, zero_grad, record, max_ctas, stream, state_start);
+}
+
+extern "C" vb_status vb_radam_step_sharded(float* p, float* g, float* m, float* v, void* p16, void* p16_lo, void* p16_b, int32_t p16_fp16,
+                                           const int64_t* chunk_start, const int64_t* state_start, const int32_t* chunk_count,
+                                           const int32_t* chunk_group, int32_t n_chunks, const vb_adamw_group* groups, int32_t leader_group,
+                                           int32_t* step, int32_t advance_step, float grad_scale, int32_t zero_grad,
+                                           const vb_clip_record* record, int32_t max_ctas, void* stream) {
+  if (n_chunks > 0 && !state_start) return vb::set_error(VB_ERR_INVALID, "vb_radam_step_sharded: null state_start");
+  return vb::radam_launch("vb_radam_step_sharded", p, g, m, v, p16, p16_lo, p16_b, p16_fp16, chunk_start, chunk_count, chunk_group,
+                          n_chunks, groups, leader_group, step, advance_step, grad_scale, zero_grad, record, max_ctas, stream, state_start);
+}
+
+extern "C" vb_status vb_grad_norm_partial(const float* g, const int64_t* chunk_start, const int32_t* chunk_count, int32_t n_chunks,
+                                          double* partials, double* sum, void* stream) {
+  using namespace vb;
+  if (!sum) return set_error(VB_ERR_INVALID, "vb_grad_norm_partial: null sum");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (n_chunks > 0) {
+    if (!g || !chunk_start || !chunk_count || !partials) return set_error(VB_ERR_INVALID, "vb_grad_norm_partial: null argument");
+    if (reinterpret_cast<uintptr_t>(g) % 16) return set_error(VB_ERR_INVALID, "vb_grad_norm_partial: g must be 16-byte aligned");
+    cudaError_t e = launch_pdl(grad_sq_partials_kernel, dim3(opt_grid(n_chunks)), dim3(OPT_THREADS), (size_t)0, st, g,
+                               reinterpret_cast<const long long*>(chunk_start), chunk_count, (int)n_chunks, partials);
+    if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_grad_norm_partial: %s", cudaGetErrorString(e));
+  }
+  cudaError_t e = launch_pdl(grad_sq_sum_kernel, dim3(1), dim3(OPT_THREADS), (size_t)0, st, (const double*)partials,
+                             (int)(n_chunks > 0 ? n_chunks : 0), sum);
+  if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_grad_norm_partial: %s", cudaGetErrorString(e));
+  return VB_OK;
+}
+
+extern "C" vb_status vb_clip_finish(const double* sum, float grad_scale, float max_norm, vb_clip_record* record, int32_t* step,
+                                    void* stream) {
+  using namespace vb;
+  if (!sum || !record) return set_error(VB_ERR_INVALID, "vb_clip_finish: null sum or record");
+  if (!(max_norm > 0.f)) return set_error(VB_ERR_INVALID, "vb_clip_finish: max_norm must be > 0 (inf: skip without clipping)");
+  cudaError_t e = launch_pdl(clip_finish_kernel, dim3(1), dim3(1), (size_t)0, static_cast<cudaStream_t>(stream), sum, grad_scale,
+                             max_norm, record, static_cast<int*>(step));
+  if (e != cudaSuccess) return set_error(VB_ERR_CUDA, "vb_clip_finish: %s", cudaGetErrorString(e));
+  return VB_OK;
 }

@@ -2827,6 +2827,10 @@ class Plan:
         replayed, e.g. inside the step graph, with the table currently on the device.) With `max_grad_norm` the gradient-norm
         launch precedes it, so every replay clips and skips a non-finite step on the device. A plan with anomaly checks refuses:
         the step would apply a NaN gradient before the host could raise."""
+        if getattr(opt, "shard_state", False):
+            raise ValueError("enable_optimizer: a sharded optimizer (shard_state=True) exchanges gradients and weights with collectives "
+                             "around its launches; a step captured in the plan would need them inside the capture. Use "
+                             "loss.backward(); optimizer.step()")
         if self.anomaly:
             raise ValueError("enable_optimizer: a plan with anomaly checks (torch.autograd.set_detect_anomaly(True)) reports a NaN "
                              "gradient on the host after the backward; a step placed in the plan would apply it first")

@@ -362,6 +362,8 @@ class BertPreTrainedModel(nn.Module):
         the engine accumulates into the flat buffer, dropping the views would only hide the gradients from the optimizer); a
         frozen Parameter's (requires_grad=False) .grad is None."""
         self.engine.zero_grad()
+        if getattr(self._ddp_reducer, "scatter", False):      # a sharded optimizer's reduce-scatter is discarded with the gradient
+            self._ddp_reducer.reset_exchange()
         self._attach_grads(zero_if_detached=False)
 
     @contextlib.contextmanager

@@ -21,6 +21,10 @@ launch reads, so nothing is read back to the host.
 
 `with optimizer.step_in_backward(): loss.backward()` runs the same step while the backward runs: each bucket of the flat
 buffers is updated on a side stream as soon as no later backward op touches it (INTEGRATION.md §1k, DESIGN.md §4d).
+
+`shard_state=True` with model=ddp.DistributedDataParallel(...) shards the moments over the data-parallel ranks (ZeRO stage 1,
+INTEGRATION.md §1a, DESIGN.md §4c): the backward reduce-scatters each gradient bucket instead of all-reducing it, each rank steps
+its own slice against moments it stores for that slice only, and the updated fp32 weights are all-gathered.
 """
 import contextlib
 import ctypes as C
@@ -60,6 +64,40 @@ def build_chunks(ranges, chunk=32768):
     return np.asarray(st, np.int64), np.asarray(cn, np.int32), np.asarray(gr, np.int32)
 
 
+def shard_state_layout(slices, rank):
+    """slices: ddp.shard_slices of a bucket table -> (((lo, hi, state offset) of this rank's slice of every bucket), total): the
+    layout of the rank's compact moment buffers, its slices back to back (pure host logic, unit-tested on CPU)."""
+    out, at = [], 0
+    for sl in slices:
+        lo, hi = sl[rank]
+        out.append((lo, hi, at))
+        at += hi - lo
+    return tuple(out), at
+
+
+def shard_chunks(ranges, layout, chunk=32768):
+    """ranges: [(flat offset, numel, group index)] of the trainable tensors; layout: shard_state_layout -> per slice (start int64[],
+    state start int64[], count int32[], group int32[]): the chunk table (build_chunks) of the parts of the ranges inside the slice,
+    and where each chunk's moments start in the compact buffers (pure host logic, unit-tested on CPU)."""
+    out = []
+    for lo, hi, base in layout:
+        st, cn, gr = build_chunks([(max(off, lo), min(off + n, hi) - max(off, lo), gi) for off, n, gi in ranges
+                                   if off < hi and off + n > lo], chunk)
+        out.append((st, st - lo + base, cn, gr))
+    return out
+
+
+def unshard_state(compacts, layouts, numel):
+    """The flat-layout buffer of `numel` elements assembled from every rank's compact buffer (compacts[r] in layouts[r], as
+    shard_state_layout gives them); elements outside every slice are 0. The host-side statement of what the sharded
+    optimizer's state_dict() gathers on the device."""
+    full = torch.zeros(numel, dtype=compacts[0].dtype)
+    for buf, layout in zip(compacts, layouts):
+        for lo, hi, base in layout:
+            full[lo:hi] = buf[base:base + hi - lo]
+    return full
+
+
 def bucket_chunks(ranges, table, chunk=32768):
     """ranges: [(flat offset, numel, group index)] of the trainable tensors (as build_chunks takes them); table: disjoint (lo, hi)
     buckets of the flat buffer in ascending order -> per bucket the chunk table (build_chunks) of the parts of the ranges inside it:
@@ -72,6 +110,151 @@ def bucket_chunks(ranges, table, chunk=32768):
     return out
 
 
+class _ShardedState:
+    """The moments of a fused optimizer built with shard_state=True, sharded over the ranks of the reducer's group (ZeRO stage 1).
+
+    The reducer's exchange becomes a reduce-scatter (ddp.FlatGradAllReducer.scatter): after the synchronised backward, this
+    rank's slice of every bucket (ddp.shard_slices) holds the averaged gradient. opt.exp_avg / exp_avg_sq hold the moments of
+    those slices back to back (shard_state_layout). A step is one vb_*_step_sharded launch over the slices' chunk tables (which
+    writes the slices' 16-bit copies and zeroes their gradient), the rest of each bucket's gradient zeroed, the fp32 weights
+    all-gathered bucket by bucket, and the 16-bit copies of the gathered parts re-cast. When the bucket table changes (parameters
+    frozen or unfrozen) the moments move to the new slices through one gather of the full moments; the moments of tracked
+    parameters outside the table are kept whole on every rank (`parked`) until they are trainable again."""
+
+    def __init__(self, opt, red):
+        self.opt, self.red = opt, red
+        red.scatter = True
+        self.table = self.key = None
+        self.parked = {}
+        self._launches = {}
+        ps = opt.engine.ps
+        self.norm_sum = torch.zeros(1, dtype=torch.float64, device=ps.flat.device)
+        self._set_layout(None)
+
+    # ------------------------------------------------------------------ layout
+    def sync(self):
+        """Follows the reducer's bucket table and the optimizer's trainable set (collective when the table changed)."""
+        opt = self.opt
+        opt._refresh_trainable()
+        key = (self.red.table, opt._trainable_key)
+        if key == self.key:
+            return
+        if self.red.table != self.table:
+            self._set_layout(self.full_moments())
+        self._build_chunks()
+        self.key = key
+
+    def _set_layout(self, full):
+        """This rank's compact moments under the reducer's current table, taken from the flat-layout pair `full` (None: zeros)."""
+        opt, red, ps = self.opt, self.red, self.opt.engine.ps
+        self.table = red.table
+        self.layout, total = shard_state_layout(red.slices, red.rank)
+        m, v = (torch.zeros(max(total, 4), dtype=torch.float32, device=ps.flat.device) for _ in range(2))
+        if full is not None:
+            for lo, hi, base in self.layout:
+                m[base:base + hi - lo].copy_(full[0][lo:hi])
+                v[base:base + hi - lo].copy_(full[1][lo:hi])
+        self.parked = {}
+        for _, off, n, _ in opt._tracked:
+            if not any(lo < off + n and off < hi for lo, hi in self.table):
+                self.parked[(off, n)] = tuple(f[off:off + n].clone() if full is not None else
+                                              torch.zeros(n, dtype=torch.float32, device=ps.flat.device) for f in (full or (None, None)))
+        opt.exp_avg, opt.exp_avg_sq = m, v
+        self.key = None
+        self._launches.clear()
+
+    def _build_chunks(self):
+        opt, dev = self.opt, self.opt.engine.ps.flat.device
+        self.per_bucket = shard_chunks(opt._trainable_ranges(), self.layout, opt._chunk)
+        cols = [np.concatenate([b[i] for b in self.per_bucket]) if self.per_bucket else np.zeros(0, dt)
+                for i, dt in enumerate((np.int64, np.int64, np.int32, np.int32))]
+        self.start, self.state_start, self.count, self.group = (torch.from_numpy(c).to(dev) for c in cols)
+        self.n_chunks = len(cols[0])
+        self.partials = torch.zeros(max(self.n_chunks, 1), dtype=torch.float64, device=dev)
+        self._launches.clear()
+
+    def full_moments(self):
+        """(exp_avg, exp_avg_sq) in the flat layout on every rank: each rank's slices all-gathered, the parked moments added
+        (collective)."""
+        ps, out = self.opt.engine.ps, []
+        for buf in (self.opt.exp_avg, self.opt.exp_avg_sq):
+            f = torch.zeros_like(ps.flat)
+            for lo, hi, base in self.layout:
+                f[lo:hi].copy_(buf[base:base + hi - lo])
+            for lo, hi in self.table:
+                self.red.all_gather_range(f, lo, hi, async_op=False)
+            out.append(f)
+        for (off, n), (m, v) in self.parked.items():
+            out[0][off:off + n].copy_(m)
+            out[1][off:off + n].copy_(v)
+        return out
+
+    # ------------------------------------------------------------------ stepping
+    def _head(self, start, state_start, count, group, n):
+        ps, opt = self.opt.engine.ps, self.opt
+        return (ps.flat, ps.grad, opt.exp_avg, opt.exp_avg_sq, *ps.shadows.ptrs(), ps.shadows.fp16, start, state_start, count, group, n,
+                opt._groups_dev)
+
+    def step(self, advance):
+        """The sharded step on the current stream: clip record (global norm: one all-reduce of this rank's float64 sum of
+        squares), one launch over this rank's slices, then finish() every bucket. advance: the launch advances the counter (RAdam
+        without max_grad_norm)."""
+        opt, lib, ps = self.opt, L.lib(), self.opt.engine.ps
+        rec = None
+        if opt.max_grad_norm is not None:
+            L.call(lib.vb_grad_norm_partial, ps.grad, self.start, self.count, self.n_chunks, self.partials, self.norm_sum)
+            torch.distributed.all_reduce(self.norm_sum, group=self.red.group)
+            L.call(lib.vb_clip_finish, self.norm_sum, C.c_float(opt.grad_scale), C.c_float(opt.max_grad_norm), opt._clip_record,
+                   opt._step_dev)
+            rec = opt._clip_record
+        fn = opt._sharded_fn()
+        L.call(fn, *opt._sharded_args(self._head(self.start, self.state_start, self.count, self.group, self.n_chunks), advance, rec, 0))
+        if opt.fused_zero_grad:
+            for k in range(len(self.table)):
+                self.zero_others(k)
+        works = [self.gather(k) for k in range(len(self.table))]
+        for k, w in enumerate(works):
+            if w is not None:
+                w.wait()
+            self.recast(k)
+        self.red.reset_exchange()
+
+    def _others(self, k):
+        """The parts of bucket k outside this rank's slice."""
+        (lo, hi), (a, e, _) = self.table[k], self.layout[k]
+        return [(x, y) for x, y in ((lo, a), (e, hi)) if y > x]
+
+    def zero_others(self, k):
+        ps = self.opt.engine.ps
+        for x, y in self._others(k):
+            L.call(L.lib().vb_memset_zero, ps.grad[x:y], (y - x) * 4)
+
+    def gather(self, k):
+        lo, hi = self.table[k]
+        return self.red.all_gather_range(self.opt.engine.ps.flat, lo, hi)
+
+    def recast(self, k):
+        ps = self.opt.engine.ps
+        for x, y in self._others(k):
+            L.call(L.lib().vb_cast_f32_to_bf16, *ps.cast_args(x, y - x))
+
+    def bucket_launches(self):
+        """Per bucket: (entry point, C arguments of its first launch of a step, of any later one), capped as step_in_backward's."""
+        opt = self.opt
+        key = (opt.grad_scale, opt.fused_zero_grad, getattr(opt, "leader_group", 0), STEP_MAX_CTAS)
+        hit = self._launches.get(key)
+        if hit is None:
+            fn, hit, at = opt._sharded_fn(), [], 0
+            for st, _, _, _ in self.per_bucket:
+                n = len(st)
+                head = self._head(self.start[at:], self.state_start[at:], self.count[at:], self.group[at:], n)
+                hit.append((fn, L.launch_args(fn, *opt._sharded_args(head, True, None, STEP_MAX_CTAS)),
+                            L.launch_args(fn, *opt._sharded_args(head, False, None, STEP_MAX_CTAS))))
+                at += n
+            self._launches[key] = hit
+        return hit
+
+
 class _FlatBufferOptimizer(torch.optim.Optimizer):
     """What the fused optimizers share: the parameters must be views of the engine's flat fp32 buffer; the moments are two
     flat buffers of the same layout (per-parameter state entries are views of them); the work list is a chunk table over
@@ -80,10 +263,20 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
 
     Parameters frozen (requires_grad=False) when the optimizer is built stay out of it. One frozen later is skipped from the next
     step() on, as torch skips a parameter whose .grad is None: step() rebuilds the chunk table in place when the trainable set
-    changed. (A step already placed in a plan with Plan.enable_optimizer keeps its chunk count: enable it again after freezing.)"""
+    changed. (A step already placed in a plan with Plan.enable_optimizer keeps its chunk count: enable it again after freezing.)
 
-    def __init__(self, params, defaults, model, engine, zero_grad, chunk, max_grad_norm):
+    shard_state=True (model= a ddp.DistributedDataParallel over more than one rank): the moments are this rank's slices
+    (ddp.shard_slices of the reducer's bucket table) only; see _ShardedState."""
+
+    def __init__(self, params, defaults, model, engine, zero_grad, chunk, max_grad_norm, shard_state=False):
         name = type(self).__name__
+        from .ddp import DistributedDataParallel
+        if shard_state:
+            if not isinstance(model, DistributedDataParallel):
+                raise ValueError(f"{name}(shard_state=True) shards the state over data-parallel ranks: pass "
+                                 "model=vilbert_b200.ddp.DistributedDataParallel(...)")
+            if model.reducer.world < 2:
+                raise ValueError(f"{name}(shard_state=True) needs a data-parallel world of more than one rank")
         if engine is None:
             if model is None:
                 raise ValueError(f"{name} needs model= (a vilbert_b200 model) or engine=")
@@ -102,7 +295,7 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
                                  "without clipping)")
         super().__init__(params, defaults)
         self.engine = engine
-        from .ddp import DistributedDataParallel
+        self.shard_state = bool(shard_state)
         self._model = model.module if isinstance(model, DistributedDataParallel) else model
         self._bucket_tables = {}      # (bucket table, trainable key) -> per-bucket launch arguments (_bucket_launches)
         self._single_tables = {}      # frozen set -> the single-process bucket table
@@ -111,8 +304,8 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
         self.fused_zero_grad = bool(zero_grad)
         ps = engine.ps
         dev = ps.flat.device
-        self.exp_avg = torch.zeros_like(ps.flat)
-        self.exp_avg_sq = torch.zeros_like(ps.flat)
+        self.exp_avg = torch.zeros_like(ps.flat) if not shard_state else None
+        self.exp_avg_sq = torch.zeros_like(ps.flat) if not shard_state else None
         base, numel = ps.flat.data_ptr(), ps.numel
         self._chunk = chunk
         self._tracked = []       # (param, flat offset, numel, group index) of every parameter trainable at construction
@@ -129,8 +322,9 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
                     raise ValueError(f"{name}: every parameter must be a contiguous fp32 view of the engine's flat buffer")
                 ranges.append((off, p.numel(), gi))
                 self._tracked.append((p, off, p.numel(), gi))
-                self.state[p] = dict(step=0, exp_avg=self.exp_avg[off:off + p.numel()].view(p.shape),
-                                     exp_avg_sq=self.exp_avg_sq[off:off + p.numel()].view(p.shape))
+                self.state[p] = dict(step=0) if shard_state else \
+                    dict(step=0, exp_avg=self.exp_avg[off:off + p.numel()].view(p.shape),
+                         exp_avg_sq=self.exp_avg_sq[off:off + p.numel()].view(p.shape))
         st, cn, gr = build_chunks(ranges, chunk)
         self.n_chunks = len(st)
         self._chunk_start = torch.from_numpy(st).to(dev)
@@ -155,6 +349,10 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
             self.grad_norm = self._clip_record.view(torch.float32)[0]
             self.skipped_steps = self._clip_record[3]
         self._upload_groups()
+        self._shard = None
+        if shard_state:
+            self._model._frozen()            # the reducer's table follows the requires_grad flags of now
+            self._shard = _ShardedState(self, model.reducer)
         if dev.type == "cuda":
             engine.refresh_weights()         # frozen tensors (not in any group) keep this copy; updated ones are rewritten every step
             engine.shadow_trusted = True
@@ -276,6 +474,8 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
     def _refresh(self):
         """The host work of step() before its launch that depends on the trainable set."""
         self._refresh_trainable()
+        if self._shard is not None:
+            self._shard.sync()
 
     def _count_step(self):
         self.step_count += 1
@@ -296,6 +496,10 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
     def _bucket_launches(self, table):
         """Per bucket of `table`: (entry point, C arguments of its first launch of a step, C arguments of any later one) over its
         chunk sub-table (bucket_chunks), which lives on the device with the cache entry."""
+        if self._shard is not None:
+            if table != self._shard.table:
+                raise RuntimeError(f"{type(self).__name__}: the sharded state follows another bucket table than the backward's")
+            return self._shard.bucket_launches()
         key = (table, self._trainable_key, self.grad_scale, self.fused_zero_grad, getattr(self, "leader_group", 0), STEP_MAX_CTAS)
         hit = self._bucket_tables.get(key)
         if hit is not None:
@@ -328,12 +532,17 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
         if self._stepped:
             raise RuntimeError(f"{type(self).__name__}.step_in_backward: a second backward reached a plan after the step ran; run one "
                                "backward per context")
+        if self._shard is not None:
+            # the forward inside the context may have frozen parameters (a new bucket table): the moments follow it first, on every
+            # rank at the same point (collective only when the table changed)
+            self._refresh()
         table = red.table if red is not None else self._single_table()
         launches = self._bucket_launches(table)
         side = self._side_stream()
         if plan.e.auto_graph:
             plan.maybe_capture_pieces(table, step=True, allreduce=red is not None)
-        works, first = {}, [True]
+        works, gathers, first = {}, [], [True]
+        shard = self._shard
 
         def handover(ranges):
             works.update((r, red.allreduce_range(*r)) for r in ranges)
@@ -347,6 +556,12 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
                     w.wait()
                 self._launch_bucket(launches[k], first[0], side)
                 first[0] = False
+                if shard is not None:    # sharded: the rest of the bucket's gradient zeroed, its weights gathered after the step
+                    if self.fused_zero_grad:
+                        shard.zero_others(k)
+                    with torch.cuda.stream(comm):
+                        comm.wait_stream(side)
+                        gathers.append(shard.gather(k))
         comm = red.comm_stream() if red is not None else None
         plan.run_backward_pieces(table, handover if red is not None else None, comm, step, side)
         if first[0]:          # no bucket: the counter still moves, as in step()
@@ -355,10 +570,14 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
         main = torch.cuda.current_stream()
         if red is not None:
             main.wait_stream(comm)
-            for w in works.values():
+            for w in list(works.values()) + gathers:
                 if w is not None:
                     w.wait()
         main.wait_stream(side)
+        if shard is not None:
+            for k in range(len(table)):
+                shard.recast(k)
+            red.reset_exchange()
         self._stepped = True
 
     def _launch_bucket(self, launch, first, stream):
@@ -374,9 +593,26 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
     def zero_grad(self, set_to_none=False):
         """The gradients live in the engine's flat buffer and were zeroed by step(); the views stay attached."""
         self.engine.zero_grad()
+        if self._shard is not None:
+            self._shard.red.reset_exchange()
+
+    def _expose(self, full):
+        """Sharded: state[p] as the unsharded optimizer holds it, views of the flat-layout moments `full`."""
+        for p, off, n, _ in self._tracked:
+            self.state[p] = dict(step=self.state[p]["step"], exp_avg=full[0][off:off + n].view(p.shape),
+                                 exp_avg_sq=full[1][off:off + n].view(p.shape))
+
+    def _hide(self):
+        for p, _, _, _ in self._tracked:
+            self.state[p] = dict(step=self.state[p]["step"])
 
     def load_state_dict(self, state_dict):
-        """Copies exp_avg / exp_avg_sq INTO the flat state buffers (the default implementation would replace the views)."""
+        """Copies exp_avg / exp_avg_sq INTO the flat state buffers (the default implementation would replace the views). Sharded: the
+        state dict is the unsharded layout (every parameter's full moments); each rank keeps its slices. Collective."""
+        if self._shard is not None:
+            self._shard.sync()
+            full = self._shard.full_moments()
+            self._expose(full)
         groups = state_dict["param_groups"]
         params = [p for g in self.param_groups for p in g["params"]]
         ids = [i for g in groups for i in g["params"]]
@@ -394,6 +630,10 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
                 if k != "params":
                     g_old[k] = v
         self._upload_groups()
+        if self._shard is not None:
+            self._hide()
+            self._shard._set_layout(full)
+            self._shard.sync()
 
     def state_dict(self):
         """The per-parameter "step" is the device counter's value: replays of a captured step advance it without the host
@@ -401,14 +641,21 @@ class _FlatBufferOptimizer(torch.optim.Optimizer):
         self.step_count = int(self._step_dev.item())
         for st in self.state.values():
             st["step"] = self.step_count
-        return super().state_dict()
+        if self._shard is None:
+            return super().state_dict()
+        self._shard.sync()        # sharded: every rank gathers the full moments (collective)
+        self._expose(self._shard.full_moments())
+        try:
+            return super().state_dict()
+        finally:
+            self._hide()
 
 
 class FusedAdamW(_FlatBufferOptimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0, correct_bias=True, model=None, engine=None,
-                 zero_grad=True, chunk=32768, max_grad_norm=None):
+                 zero_grad=True, chunk=32768, max_grad_norm=None, shard_state=False):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, correct_bias=correct_bias),
-                         model, engine, zero_grad, chunk, max_grad_norm)
+                         model, engine, zero_grad, chunk, max_grad_norm, shard_state)
 
     def _group_row(self, grp):
         return group_row(grp["lr"], grp["betas"], grp["eps"], grp["weight_decay"], grp["correct_bias"])
@@ -431,6 +678,13 @@ class FusedAdamW(_FlatBufferOptimizer):
     def _capped_fn(self):
         return L.lib().vb_adamw_step_capped
 
+    def _sharded_fn(self):
+        return L.lib().vb_adamw_step_sharded
+
+    def _sharded_args(self, head, advance, rec, max_ctas):
+        """The counter is advanced by the caller (step(), _launch_bucket) or by vb_clip_finish, as for the unsharded launch."""
+        return head + (self._step_dev, C.c_float(self.grad_scale), 1 if self.fused_zero_grad else 0, rec, max_ctas)
+
     def _capped_args(self, head, first):
         return head + (self._step_dev, C.c_float(self.grad_scale), 1 if self.fused_zero_grad else 0, STEP_MAX_CTAS)
 
@@ -450,7 +704,10 @@ class FusedAdamW(_FlatBufferOptimizer):
             for st in self.state.values():
                 st["step"] = self.step_count
         self._upload_groups()
-        if self.n_chunks or self.max_grad_norm is not None:
+        if self._shard is not None:
+            self._shard.sync()
+            self._shard.step(False)
+        elif self.n_chunks or self.max_grad_norm is not None:
             self.launch()
         self._after_step()
         return loss
@@ -467,9 +724,9 @@ class FusedRAdam(_FlatBufferOptimizer):
     embeddings' at base_lr, so the vil_* heads' lr of 1e-4 does not reach their RAdam update."""
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, model=None, engine=None, zero_grad=True,
-                 chunk=32768, max_grad_norm=None):
+                 chunk=32768, max_grad_norm=None, shard_state=False):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay), model, engine, zero_grad, chunk,
-                         max_grad_norm)
+                         max_grad_norm, shard_state)
         self._set_leader()
 
     def _set_leader(self):
@@ -480,9 +737,18 @@ class FusedRAdam(_FlatBufferOptimizer):
     def _refresh(self):
         if self._refresh_trainable():
             self._set_leader()
+        if self._shard is not None:
+            self._shard.sync()
 
     def _capped_fn(self):
         return L.lib().vb_radam_step_capped
+
+    def _sharded_fn(self):
+        return L.lib().vb_radam_step_sharded
+
+    def _sharded_args(self, head, advance, rec, max_ctas):
+        return head + (self.leader_group, self._step_dev, 1 if advance else 0, C.c_float(self.grad_scale), 1 if self.fused_zero_grad else 0,
+                       rec, max_ctas)
 
     def _capped_args(self, head, first):
         """advance_step on the first launch of a step only; the leader-group rule is step()'s."""
@@ -519,7 +785,10 @@ class FusedRAdam(_FlatBufferOptimizer):
             for st in self.state.values():
                 st["step"] = self.step_count
         self._upload_groups()
-        if self.n_chunks or self.max_grad_norm is not None:
+        if self._shard is not None:
+            self._shard.sync()
+            self._shard.step(self.max_grad_norm is None)
+        elif self.n_chunks or self.max_grad_norm is not None:
             self.launch(advance_step=True)
         else:
             self._step_dev.add_(1)
