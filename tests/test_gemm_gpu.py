@@ -1,5 +1,6 @@
-"""wgmma GEMM (vb_gemm_bf16) through the C ABI vs torch fp32 matmul of the same bf16 operands.
-Tolerance: 2e-3 of max|ref| (fp32 accumulation-order noise; bf16 output rounding is discounted in the helper)."""
+"""wgmma GEMM (vb_gemm_bf16) through the C ABI. Every case runs through the float64 checker of tests/_gpu_util.py (gemm_case):
+per-element bounds, correctly rounded 16-bit outputs, guard bands, the tile width's kernel asserted, wrong references. The value
+returned and compared with TOL is the largest error past the correctly rounded result, relative to max|ref|."""
 import pytest
 
 from vilbert_b200 import _lib as L

@@ -1,7 +1,7 @@
 """GEMM tile widths and production signatures: the 128- and 256-wide tiles accumulate every output element over k in the same
-order (one m64n256k16 per k step is the two m64n128k16 halves side by side), so their outputs are bitwise identical; every
-GEMM signature of the config-2 training step matches a float64 reference; and the build log shows no GEMM kernel spilling."""
-import ctypes as C
+order (one m64n256k16 per k step is the two m64n128k16 halves side by side), so their outputs are bitwise identical; every GEMM
+form of the bench configs' plans (training steps; config 2's evaluation, capped-backward and deterministic plans) passes the float64
+checker of tests/_gpu_util.py; and the build log shows no GEMM kernel spilling."""
 import os
 import re
 import sys
@@ -13,10 +13,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 from vilbert_b200 import _lib as L  # noqa: E402
+from _gpu_util import GEMM_OUTPUTS, GemmCase, _bits  # noqa: E402
 
 PTXAS_LOG = os.path.join(ROOT, "vilbert-multi-task_b200", "csrc", "vb_gemm.ptxas.log")
-TOL = 2e-3   # tests/test_gemm_gpu.py: max error relative to the largest reference value
-RND16 = {torch.bfloat16: 4e-3, torch.float16: 5e-4}   # output rounding allowance of a 16-bit result
 
 
 def test_gemm_kernels_do_not_spill():
@@ -30,73 +29,35 @@ def test_gemm_kernels_do_not_spill():
     assert "setmaxnreg' ignored" not in text
 
 
-# ------------------------------------------------------------------------------------------ float64 reference
-def _hash32(x):
-    x = x & 0xFFFFFFFF
-    x = x ^ (x >> 16); x = (x * 0x7FEB352D) & 0xFFFFFFFF
-    x = x ^ (x >> 15); x = (x * 0x846CA68B) & 0xFFFFFFFF
-    return x ^ (x >> 16)
+# ------------------------------------------------------------------------------------------ the plans' signatures
+class SigCase(GemmCase):
+    """A signature in gemm_sig_probe's format on guarded device buffers (tests/_gpu_util.GemmCase): the plan's row pitches and
+    base addresses modulo 256, random 16-bit operands (split precision: the low parts of fp32 values), random fp32 bias / residual,
+    bf16 aux; every output filled with a NaN sentinel around and inside its range (atomic outputs and column sums start from
+    random values)."""
 
-
-def _keep_scale(M, N, site, ctr, p):
-    seed = _hash32(torch.tensor(site + ctr * 0x9E3779B9, dtype=torch.int64))
-    idx = (torch.arange(M, device="cuda", dtype=torch.int64)[:, None] * N + torch.arange(N, device="cuda", dtype=torch.int64)[None]) & 0xFFFFFFFF
-    p32 = float(torch.tensor(p, dtype=torch.float32))   # the kernel's threshold and scale come from the float p
-    keep = _hash32(idx ^ seed) >= int(p32 * 4294967296.0)
-    return keep.double() * float(1.0 / (1.0 - torch.tensor(p32, dtype=torch.float32)))
-
-
-def reference(ln):
-    """float64 epilogue value (before the residual), the column sums, the value after the residual and gelu'(pre)."""
-    s, v = ln.s, ln.views
-    M, N, K = s["M"], s["N"], s["K"]
-    op = lambda X, mn, rows: (X[:K, :rows].t() if mn else X[:rows, :K]).double()
-    A = op(v["A"], s["a_mn_major"], M) + (op(v["A_lo"], s["a_mn_major"], M) if "A_lo" in v else 0)
-    B = op(v["B"], s["b_mn_major"], N) + (op(v["B_lo"], s["b_mn_major"], N) if "B_lo" in v else 0)
-    x = s["alpha"] * (A @ B.t())
-    if "bias" in v:
-        x = x + v["bias"][0, :N].double()
-    pre = None
-    if s["act"] == L.VB_ACT_GELU:
-        pre = 0.5 * (1 + torch.erf(x / 2 ** 0.5)) + x * torch.exp(-0.5 * x * x) / (2 * torch.pi) ** 0.5
-        x = x * 0.5 * (1 + torch.erf(x / 2 ** 0.5))
-    elif s["act"] == L.VB_ACT_RELU:
-        x = x.clamp_min(0)
-    elif s["act"] == L.VB_ACT_DGELU:
-        x = x * v["aux"][:M, :N].double()
-    if s["dropout"]:
-        x = x * _keep_scale(M, N, s["dropout"][0], int(ln.ctr.item()), s["dropout"][1])
-    colsum = x.sum(0)
-    y = x + v["residual"][:M, :N].double() if "residual" in v else x
-    return y, colsum, pre
-
-
-def rel(a, ref):
-    return ((a.double() - ref).abs().max() / (ref.abs().max() + 1e-9)).item()
+    def __init__(self, sig, seed=0):
+        from gemm_sig_probe import SCALAR_FIELDS, describe
+        s = describe(sig)
+        ld = {f: s[k] for f, k in (("A", "lda"), ("B", "ldb"), ("residual", "ld_res"), ("aux", "ld_aux"), ("out_f32", "ld_out_f32"),
+                                   ("out_bf16", "ld_out_bf16"), ("out_pre", "ld_out_pre")) if f in s["set"]}
+        st = set(s["set"])
+        super().__init__(s["M"], s["N"], s["K"], outs=[f for f in GEMM_OUTPUTS if f in st], a_mn=bool(s["a_mn_major"]),
+                         b_mn=bool(s["b_mn_major"]), fp16=bool(s["a_fp16"]), out_fp16=bool(s["out_fp16"]), alpha=s["alpha"],
+                         bias="bias" in st, act=s["act"], res="residual" in st, drop=s["dropout"], a_lo="A_lo" in st,
+                         b_lo="B_lo" in st, atomic=s["atomic_out"], split_k=s["split_k"], block_n=s["block_n"],
+                         max_ctas=s["max_ctas"], ld=ld, align=dict(sig[len(SCALAR_FIELDS)]), seed=seed)
+        self.s = s
 
 
 def check_against_reference(ln):
-    s, v = ln.s, ln.views
-    M, N = s["M"], s["N"]
-    y, colsum, pre = reference(ln)
-    errs = {}
-    if "out_f32" in v:
-        out = v["out_f32"]
-        if s["atomic_out"] == L.VB_GEMM_PARTIALS:
-            out = out.view(-1, M, out.shape[1]).sum(0)
-        errs["out_f32"] = rel(out[:M, :N], y)
-    for f in ("out_bf16", "out_b16"):
-        if f in v:
-            hi = v[f][:M, :N].double() + (v["out_lo"][:M, :N].double() if (f == "out_bf16" and "out_lo" in v) else 0)
-            errs[f] = rel(hi, y) - (0 if (f == "out_bf16" and "out_lo" in v) else RND16[v[f].dtype])
-    if "out_pre" in v:
-        errs["out_pre"] = rel(v["out_pre"][:M, :N], pre) - RND16[torch.bfloat16]
-    if "out_colsum" in v:
-        errs["out_colsum"] = rel(v["out_colsum"][0, :N], colsum)
-    assert errs and max(errs.values()) < TOL, (s, errs)
+    """(Re)runs the launch under the profiler (the kernel of the tile width vb_gemm_plan resolves) and holds it to the float64
+    checker of tests/_gpu_util.py: per-element bounds, correctly rounded 16-bit outputs, guard bands, wrong references."""
+    from _gpu_util import gemm_verdict
+    from gemm_sig_probe import short
+    gemm_verdict(ln, short(ln.s), expect=rf"gemm_wgmma_kernel<{ln.bn}, ")
 
 
-# ------------------------------------------------------------------------------------------ the config-2 step's signatures
 def _config2_signatures():
     from gemm_sig_probe import plan_gemm_signatures, short, describe
     return [pytest.param(k, id=short(describe(k)).replace(" ", "_")) for k in plan_gemm_signatures(2)]
@@ -105,11 +66,26 @@ def _config2_signatures():
 @pytest.mark.gpu
 @pytest.mark.parametrize("sig", _config2_signatures())
 def test_config2_signature_against_float64(sig):
-    from gemm_sig_probe import Launch
-    ln = Launch(sig, seed=3)
-    ln(C.c_void_p(torch.cuda.current_stream().cuda_stream))
-    torch.cuda.synchronize()
-    check_against_reference(ln)
+    check_against_reference(SigCase(sig, seed=3))
+
+
+def _other_plan_signatures():
+    """One signature per GEMM form of every bench config's training step, config 2's forward-only evaluation plan, its backward
+    capped at SMs - 16 CTAs and its deterministic step, without the forms of config 2's training step (the test above)."""
+    from gemm_sig_probe import plan_gemm_signatures, plan_signature_union, short, describe
+    seen = set(plan_gemm_signatures(2))
+    out = []
+    for k, src in plan_signature_union().items():
+        if k not in seen:
+            tag = "+".join(f"{c}{kind}" for c, kind in src[:2]) + ("+" if len(src) > 2 else "")
+            out.append(pytest.param(k, id=f"{tag}:{short(describe(k))}".replace(" ", "_")))
+    return out
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("sig", _other_plan_signatures())
+def test_plan_signature_against_float64(sig):
+    check_against_reference(SigCase(sig, seed=3))
 
 
 # ------------------------------------------------------------------------------------------ 128- vs 256-wide tiles
@@ -142,14 +118,14 @@ REORDERED = ("atomic_split_k", "partials")   # float atomics / slice sums: compa
 
 
 def _run(sig, block_n):
-    from gemm_sig_probe import Launch, resolved_tiles, SCALAR_FIELDS
+    from gemm_sig_probe import resolved_tiles, SCALAR_FIELDS
     s = dict(zip(SCALAR_FIELDS, sig[:len(SCALAR_FIELDS)]), block_n=block_n)
     if s["atomic_out"] == L.VB_GEMM_PARTIALS:
         from gemm_sig_probe import describe
         s["split_k"] = resolved_tiles(dict(describe(sig), block_n=block_n))[1]
     sig = tuple(s[f] for f in SCALAR_FIELDS) + sig[len(SCALAR_FIELDS):]
-    ln = Launch(sig, seed=5)
-    ln(C.c_void_p(torch.cuda.current_stream().cuda_stream))
+    ln = SigCase(sig, seed=5)
+    ln.run()
     torch.cuda.synchronize()
     return ln
 
@@ -166,11 +142,9 @@ def test_tile_widths_give_the_same_bits(epi, majors, shape):
         check_against_reference(n128)
         check_against_reference(n256)
         return
-    for f, v in n128.views.items():
-        if f in ("A", "B", "bias", "residual", "aux"):
-            continue
+    for f in n128.outs:
         if f == "out_colsum":   # float atomics across row blocks
-            check_against_reference(n256)
             continue
-        assert torch.equal(v, n256.views[f]), (epi, f)
+        assert torch.equal(_bits(n128.raw[f])[n128.inside[f]], _bits(n256.raw[f])[n256.inside[f]]), (epi, f)
+    check_against_reference(n128)
     check_against_reference(n256)

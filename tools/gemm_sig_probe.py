@@ -55,8 +55,10 @@ def short(s):
             f"{'f16' if s['a_fp16'] else 'bf16'}{'x3' if 'A_lo' in s['set'] else ''} {tag or 'plain'} -> {','.join(o[4:] for o in out)}")
 
 
-def plan_gemm_signatures(config):
-    """{signature: launches per step} of bench.py config `config`'s training step (forward + backward), in first-launch order."""
+def plan_gemm_signatures(config, kind="train", sm_count=132):
+    """{signature: launches per step} of bench.py config `config`'s plans, in first-launch order. kind: "train" (the training step,
+    forward + backward), "eval" (the forward-only evaluation plan), "capped" (the training step with the backward GEMMs capped at
+    sm_count - 16 persistent CTAs, as data-parallel runs leave SMs to NCCL) or "det" (the deterministic training step)."""
     import bench
     from vilbert_b200.config import BertConfig
     from vilbert_b200.engine import Engine, LOSS_HEADS
@@ -65,10 +67,15 @@ def plan_gemm_signatures(config):
     if cf["task_tokens"]:
         cfgj = dict(cfgj, task_specific_tokens=True)
     eng = Engine(BertConfig.from_dict(cfgj), "cpu", heads=cf.get("heads", "vl"), _build_only=True)
+    if kind == "capped":
+        eng.bwd_gemm_max_ctas = sm_count - 16
     sigs = {}
-    for (_name, gb, Nv, Nt, kind) in cf["tasks"]:
+    for (_name, gb, Nv, Nt, loss) in cf["tasks"]:
         B = gb if cf["per_gpu"] else gb // 8
-        plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS[kind], loss=kind, train=True)
+        if kind == "eval":
+            plan = eng.plan(B, Nt, Nv)
+        else:
+            plan = eng.plan(B, Nt, Nv, grad_outputs=LOSS_HEADS[loss], loss=loss, train=True, deterministic=(kind == "det"))
         for fn, args, _sid in plan.prologue + plan.fwd + plan.bwd:
             if fn is None or fn.__name__ != "vb_gemm_bf16":
                 continue
@@ -76,6 +83,29 @@ def plan_gemm_signatures(config):
             k = signature(g)
             sigs[k] = sigs.get(k, 0) + 1
     return sigs
+
+
+def plan_signature_union(kinds=None):
+    """One signature per GEMM form the engine's plans launch: the union over `kinds` ((config, kind) pairs; default: every bench
+    config's training step and config 2's evaluation, capped-backward and deterministic plans) with the row count M left out of
+    the key and base addresses taken modulo 16 (the epilogue's vector-access conditions), each form represented by its launch of
+    the fewest rows. {signature: [(config, kind), ...] it comes from}."""
+    if kinds is None:
+        import bench
+        kinds = [(c, "train") for c in sorted(bench.CONFIGS)] + [(2, "eval"), (2, "capped"), (2, "det")]
+    forms = {}
+    for c, kind in kinds:
+        for k in plan_gemm_signatures(c, kind):
+            s = dict(zip(SCALAR_FIELDS, k[:len(SCALAR_FIELDS)]))
+            s.pop("M")
+            if s["a_mn_major"]:
+                s.pop("lda")      # MN-major A: its pitch is M rounded up
+            key = (tuple(s.items()), tuple((f, o % 16) for f, o in k[len(SCALAR_FIELDS)]), k[-1])
+            rep, src = forms.get(key, (None, []))
+            if rep is None or k[0] < rep[0]:
+                rep = k
+            forms[key] = (rep, src + [(c, kind)] if (c, kind) not in src else src)
+    return {rep: src for rep, src in forms.values()}
 
 
 def resolved_tiles(s):
